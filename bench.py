@@ -65,6 +65,9 @@ def parse_args():
     ap.add_argument("--config", default="headline", choices=sorted(CONFIGS),
                     help="BASELINE.json config: headline (#1, default), quota (#2), fallback (#3), fleet (#4)")
     ap.add_argument("--trace-out", default=None, help="fleet configs: write the recorded admission trace here (JSON)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="headline config: after the timed steps write what the last timed step returned to its callers "
+                         "(generated token ids, serving deployment per request) as DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -73,8 +76,8 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "data sheet (H100 SXM: 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; not reached)"
 
 
 def load_models_module():
@@ -267,7 +270,7 @@ def kernel_table(eng, spec, prompts_np, C, P, M, hbm_peak):
     Runs one short extra burst AFTER the timed region."""
     import ctypes as Ct
     from rr_b200 import _lib
-    NAMES = {1: "gemm/layer (tcgen05)", 3: "decode_attn", 5: "add_rmsnorm", 8: "embed", 9: "argmax", 10: "attn_combine"}
+    NAMES = {1: "gemm/layer (wgmma)", 3: "decode_attn", 5: "add_rmsnorm", 8: "embed", 9: "argmax", 10: "attn_combine"}
     ids = np.ascontiguousarray(prompts_np[:C]).reshape(-1)
     start = np.arange(0, (C + 1) * P, P, dtype=np.int32)
     N = 20000
@@ -303,20 +306,20 @@ def kernel_table(eng, spec, prompts_np, C, P, M, hbm_peak):
         elif kid == 1:
             if gemm_total == L + 1:                            # persistent layer kernels: QKV_0 | layer l (+ QKV_{l+1}) | last (+ lm_head)
                 if n_gemm == 0:
-                    name, nbytes = "decode_layer_tcgen05 [QKV of layer 0]", w_qkv
+                    name, nbytes = "decode_layer_wgmma [QKV of layer 0]", w_qkv
                 elif n_gemm < L:
-                    name, nbytes = "decode_layer_tcgen05 [O + gate/up + down + next QKV]", w_o + w_mlp + w_qkv
+                    name, nbytes = "decode_layer_wgmma [O + gate/up + down + next QKV]", w_o + w_mlp + w_qkv
                 else:
-                    name, nbytes = "decode_layer_tcgen05 [last layer + lm_head]", w_o + w_mlp + w_head
+                    name, nbytes = "decode_layer_wgmma [last layer + lm_head]", w_o + w_mlp + w_head
             elif gemm_total == 3 * L + 1:                       # default path, per layer: QKV GEMM, O GEMM, fused MLP; then lm_head
                 if n_gemm == 3 * L:
-                    name, nbytes = "gemm_bf16_tcgen05<64,1> lm_head", w_head
+                    name, nbytes = "gemm_bf16_wgmma<64,1> lm_head", w_head
                 else:
-                    name, nbytes = [("gemm_bf16_tcgen05<64,1> QKV projection (split-K 3)", w_qkv),
-                                    ("gemm_bf16_tcgen05<64,1> O projection (split-K 4)", w_o),
-                                    ("gemm_mlp_tcgen05<64> gate/up + SiLU + down", w_mlp)][n_gemm % 3]
+                    name, nbytes = [("gemm_bf16_wgmma<64,1> QKV projection (split-K)", w_qkv),
+                                    ("gemm_bf16_wgmma<64,1> O projection (split-K)", w_o),
+                                    ("gemm_mlp_wgmma<64> gate/up + SiLU + down", w_mlp)][n_gemm % 3]
             else:
-                name = "gemm_bf16_tcgen05 (other decode configuration)"
+                name = "gemm_bf16_wgmma (other decode configuration)"
             n_gemm += 1
         r = rows.setdefault(name, {"kernel": name, "launches": 0, "us": 0.0, "bytes": 0})
         r["launches"] += 1; r["us"] += seg_us; r["bytes"] += nbytes
@@ -491,6 +494,7 @@ def main():
 
     ttfts, lat = [], []
     token_sums = []                                                # per step: checksum of every generated token
+    last = {}                                                      # the most recent step's outputs, for --dump-outputs
 
     def one_step(collect: bool):
         """One closed burst through the public path.  Returns nothing; per-request timings collected."""
@@ -505,6 +509,8 @@ def main():
                 if collect:
                     ttfts.append(r._ttft_s); lat.append(r._latency_s)
             token_sums.append(chk)
+            last["tokens"] = np.array([r._token_ids for r in out], dtype=np.float64)
+            last["deployment"] = np.array([r._deployment for r in out], dtype=np.float64)
         else:
             dec = None
             if rank == 0:
@@ -524,6 +530,8 @@ def main():
             token_sums.append(int(ct.item()))
             if collect:
                 ttfts.extend(r.ttft for r in recs); lat.extend(r.latency for r in recs)
+            last[f"request_rank{rank}"] = np.asarray(mine, dtype=np.float64)
+            last[f"tokens_rank{rank}"] = np.array([r.tokens for r in recs], dtype=np.float64).reshape(len(recs), M)
             parallel.gather_done(len(mine), world, rank, device=torch.device("cuda", local))
             if rank == 0:
                 now = router.now_ms()
@@ -549,6 +557,8 @@ def main():
     sync_all()
     wall = time.perf_counter() - t_start
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last)
     st = eng.stats()
     dev_s = (st["prefill_ms_total"] + st["decode_ms_total"]) / 1e3
     # identical prompts every step and deterministic kernels: every step must have generated exactly the same tokens for
@@ -602,7 +612,7 @@ def main():
             "config": {"workload": f"{args.model} shape, seeded random weights, {C} concurrent x {world} GPU(s), "
                                    f"{P}-in/{M}-out greedy, least-busy routing over {world} replica(s)",
                        "global_batch": n_req, "prompt_len": P, "max_new": M, "parallelism": f"replicas x{world} (dp{world})",
-                       "l2": "inputs larger than L2: 15 GB of weights + 4.8 GB of KV are re-read every decode step (L2 = 126 MB)",
+                       "l2": "inputs larger than L2: 15 GB of weights + 4.8 GB of KV are re-read every decode step (L2 = 50 MB)",
                        "timing": "value: CUDA events on each engine stream around every prefill chunk / decode step, max over ranks"},
             "p50_ttft_ms": float(np.percentile(all_ttft, 50) * 1e3), "p99_ttft_ms": float(np.percentile(all_ttft, 99) * 1e3),
             "tokens_per_s": total_completions * M / dev_max,
@@ -615,8 +625,8 @@ def main():
             "gpu_launches": int(sm[5].item() + 2 * K),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
                          "traffic": traffic, "traffic_source": traffic_src,
-                         "kernel": "decode step = 1 CUDA-graph launch (196 kernels, PDL edges); dominant kernels: gemm_mlp_tcgen05<64> / "
-                                   "gemm_bf16_tcgen05<64,1> (weight streams) and decode_attn_mma_kernel<4> (KV stream); see `kernels`",
+                         "kernel": "decode step = 1 CUDA-graph launch (196 kernels, PDL edges); dominant kernels: gemm_mlp_wgmma<64> / "
+                                   "gemm_bf16_wgmma<64,1> (weight streams) and decode_attn_mma_kernel<4> (KV stream); see `kernels`",
                          "bytes_per_launch": bytes_step, "ms_per_launch": dec_ms, "peak_source": peak_src},
             "prefill": {"tflops": pf_tflops, "peak_tflops_sustained": tf_peak, "frac": (pf_tflops / tf_peak) if pf_tflops else None,
                         "ms_per_burst": pf_ms / K, "flops_counted": "executed (last layer's O / MLP and lm_head only on each prompt's last token)",
@@ -649,6 +659,17 @@ def main():
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """Write each array as out_dir/<name>.npy (float64: token ids and deployment indices are exact).  The inputs are
+    seeded, so two builds run with the same arguments can be compared output for output."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > 64 << 20:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the 64 MB bound")
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def router_kernel_timing(router, n_events: int = 2048, reps: int = 5):

@@ -1,4 +1,4 @@
-/* rr_b200.h — public C-ABI of librr_b200.so, the B200-native replacement for the request-router
+/* rr_b200.h — public C-ABI of librr_b200.so, the GPU-native (H100, sm_90a) replacement for the request-router
  * hot path of aws-samples/sample-resilient-llm-inference.
  *
  * The reference has NO native/FFI boundary: its hot path is `litellm.Router` (un-vendored
@@ -177,14 +177,14 @@ enum { RR_OUT_ROWMAJOR_BF16 = 0, RR_OUT_TRANSPOSED_F32 = 1,
        /* fused SiLU(gate)*up epilogues; the weight operand holds gate/up rows interleaved in 64-row blocks
         * [g0..g63, u0..u63, g64..g127, u64..u127, ...] and the output is bf16 act[.., inter]: */
        RR_OUT_TRANSPOSED_SILU = 2,   /* decode: A = interleaved weight [2*inter, K], out[b*ldo + n], splits = 1 */
-       RR_OUT_ROWMAJOR_SILU = 3,     /* prefill: B = interleaved weight, bn = 256, out[a*ldo + n] */
+       RR_OUT_ROWMAJOR_SILU = 3,     /* prefill: B = interleaved weight, bn >= 128, out[a*ldo + n] */
        RR_OUT_ROWMAJOR_ROPE = 4,     /* engine-internal (prefill QKV epilogue with RoPE + KV scatter) */
        RR_OUT_ROWMAJOR_RESID = 5 };  /* out = fp32 residual [rowsA, ldo]: out[a*ldo + b] += acc (bn >= 128) */
 
-/* D[a,b] = sum_k A[a,k] B[b,k] on tcgen05 tensor cores (bf16 in, fp32 accumulate).
+/* D[a,b] = sum_k A[a,k] B[b,k] on wgmma tensor cores (bf16 in, fp32 accumulate).
  * mode RR_OUT_ROWMAJOR_BF16:  out bf16 [rowsA, ldo], out[a*ldo + b]         (splits must be 1)
  * mode RR_OUT_TRANSPOSED_F32: out fp32 [splits, ld_rows, ldo], out[(z*ld_rows + b)*ldo + a]
- * bn = tile width along B rows: 16/32/64/128/256.  splits >= 1. */
+ * bn = tile width along B rows: 16/32/64/128 (256 is accepted and runs 128-wide tiles).  splits >= 1. */
 int rr_gemm_bf16(const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
                  void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream);
 

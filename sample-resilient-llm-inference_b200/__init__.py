@@ -1,4 +1,4 @@
-"""B200-native request router + model replicas (drop-in for the litellm.Router hot path of
+"""GPU-native (H100) request router + model replicas (drop-in for the litellm.Router hot path of
 aws-samples/sample-resilient-llm-inference).  See DESIGN.md.
 
 Importing this package loads librr_b200.so; there is no CPU fallback.

@@ -1,7 +1,7 @@
-"""Build librr_b200.so in-tree with nvcc for sm_100a (no torch extension machinery, no JIT cache).
+"""Build librr_b200.so in-tree with nvcc for sm_90a (Hopper H100; no torch extension machinery, no JIT cache).
 
-Objects go to <repo>/build/, the shared library next to this file so it travels with the gpurun
-snapshot.  Only stale objects are rebuilt (mtime of the .cu and of every header in csrc/ and
+Objects go to <repo>/build/, the shared library next to this file so the package imports from the
+source tree.  Only stale objects are rebuilt (mtime of the .cu and of every header in csrc/ and
 include/).
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ LIB = PKG / "librr_b200.so"
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
@@ -54,7 +54,7 @@ def _compile(src: Path, verbose: bool) -> Path:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every csrc/*.cu for sm_100a and link librr_b200.so. Returns the library path."""
+    """Compile every csrc/*.cu for sm_90a and link librr_b200.so. Returns the library path."""
     OBJ.mkdir(parents=True, exist_ok=True)
     hdr_m = _headers_mtime()
     srcs = _sources()
@@ -70,7 +70,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     need_link = force or bool(stale) or not LIB.exists() or any(
         o.stat().st_mtime > LIB.stat().st_mtime for o in objs)
     if need_link:
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a",
                "-o", str(LIB), *map(str, objs), "-lpthread"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

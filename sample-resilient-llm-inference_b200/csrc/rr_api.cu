@@ -26,7 +26,7 @@ int check_last(void) {
 
 using namespace rr;
 
-RR_API const char* rr_version(void) { return "rr_b200 0.1 (sm_100a)"; }
+RR_API const char* rr_version(void) { return "rr_b200 0.1 (sm_90a)"; }
 
 RR_API const char* rr_strerror(int rc) {
     switch (rc) {

@@ -1,34 +1,21 @@
-// rr_attn_tc.cu — prefill attention (K7) on tcgen05: causal flash attention with both contractions on
-// the 5th-gen tensor cores, S, P and the O accumulator in TMEM, Q / K / V tiles staged by TMA.
+// rr_attn_tc.cu — prefill attention (K7) on Hopper tensor cores: causal flash attention with both contractions on
+// wgmma, Q / K / V tiles staged by TMA, S, P and the O accumulator in registers.
 //
-// Persistent kernel, one CTA per SM, 12 warps = 3 warpgroups (one warp of each per SM sub-partition):
-//   warp 0      TMA producer  : Q tiles (128 rows x 128 dims, two query heads that share a kv head) and a
-//                               3-deep ring of K/V tiles (64 keys x 128 dims each) from the KV cache
-//   warp 1      MMA issuer    : S_h = Q_h K^T   (M128 N64  K16 x 8, K-major smem operands)
-//                               O_h = P_h V     (M128 N128 K16 x 4, P read from TMEM, V MN-major as it
-//                               lies in the cache: keys are rows, the head dim is contiguous)
-//   warps 2-3   idle
-//   warps 4-7   softmax, head 0: thread = one query row (TMEM lane): scale, causal mask, running max,
-//   warps 8-11  softmax, head 1: exp2, row sum, P -> bf16 -> TMEM (tcgen05.st over the S columns it just
-//                               read); at the end of the item reads O from TMEM, normalises, stages the
-//                               rows in smem and stores them row-contiguously.
-// S is double-buffered in TMEM (2 x 64 columns per head) so QK^T of tile j+1 runs under the softmax of
-// tile j; P(j) overwrites the first 32 columns of S(j) (two bf16 per column) and is the A operand of the
-// PV MMA straight from TMEM, so shared memory only carries Q, K and V.  The tensor pipe executes in issue
-// order, which is what protects the S/P columns: S(j+2) is issued after PV(j).  The two heads alternate
-// on the pipe.  TMEM: 2 x (64 + 64 + 128) = 512 columns.
+// Persistent kernel, one CTA per SM, 9 warps:
+//   warps 0-3   consumer warpgroup 0: query rows  0..63 of the item's 128-row tile
+//   warps 4-7   consumer warpgroup 1: query rows 64..127
+//   warp 8      TMA producer: the Q tile (128 rows x 128 dims) and a 4-deep ring of K/V tiles (64 keys x 128 dims
+//               each) from the KV cache
+// Per key tile a consumer warpgroup computes S = Q K^T (m64n64k16 x 8, both operands K-major in shared memory),
+// the causal mask and the online softmax on the S registers, then O += P V (m64n128k16 x 4) with P straight from
+// registers (the accumulator layout of S is the A-fragment layout of the next wgmma) and V as the MN-major B operand
+// exactly as it lies in the cache: 64 dims (128 B) contiguous, 8 keys per 1024 B swizzle atom (SBO), the second
+// 64-dim half one TMA box (8192 B) further (LBO).  A key tile that lies wholly above a warpgroup's rows (the last
+// tile of warpgroup 0) is only waited for and released.
 //
-// O accumulates in TMEM across the key tiles of an item (PV with the accumulate flag).  The exponentials
-// of a row are taken relative to a reference maximum that is only raised when the running maximum has
-// moved by more than 2^8 (warp-uniform vote); raising it rescales the warp's 32 rows of O in TMEM
-// (ld, multiply, st) after the previous PV has completed.  exp2(s - ref) <= 256 keeps P exact to bf16
-// precision and the final O / l is independent of the reference, so the rescale is rare instead of once
-// per tile.
-//
-// Work item = (sequence, head pair, 128-row query tile), heaviest (last) query tiles first, strided
-// over the CTAs.  The two heads of a pair must share their kv head (one K/V ring): even GQA group sizes run pairs;
-// MHA and odd group sizes (Phi-3-mini: 32 heads, 32 kv heads, head_dim 96 zero-padded to 128) run ONE head per item
-// (nh = 1: the second softmax warpgroup and half of the TMEM columns stay idle) on the same tcgen05 / TMA path.
+// Work item = (sequence, query head, 128-row query tile), heaviest (last) query tiles first, strided over the CTAs.
+// Any GQA group size (MHA included): the kv head is head / (n_heads / n_kv_heads).  Head dims below 128 (Phi-3-mini:
+// 96) are zero-padded to 128 in q and the caches; only the true head dim is written.
 //
 // Replaces the remote bedrock:InvokeModel call (reference iam/policy.json:8).
 #include "rr_ptx.cuh"
@@ -39,80 +26,24 @@
 namespace rr {
 namespace {
 
-constexpr int TQ = 128;                 // query rows per head per work item
+constexpr int TQ = 128;                 // query rows per work item
 constexpr int TKV = 64;                 // keys per tile
-constexpr int NH = 2;                   // query heads per CTA
-constexpr int NS = 3;                   // K/V ring depth
-constexpr int TC_THREADS = 128 + 128 * NH;
+constexpr int NS = 4;                   // K/V ring depth
+constexpr int TC_CONSUMERS = 256;       // two warpgroups
+constexpr int TC_THREADS = TC_CONSUMERS + 32;
+constexpr int TC_PRODUCER_WARP = TC_CONSUMERS / 32;
 constexpr uint32_t Q_BYTES = 32768;     // [2 dim halves][128 rows][128 B]
 constexpr uint32_t KV_BYTES = 16384;    // [2 dim halves][64 keys][128 B]
 constexpr uint32_t OFF_Q = 0;
-constexpr uint32_t OFF_KV = OFF_Q + NH * Q_BYTES;
-constexpr uint32_t ST_BYTES = 32768;    // output staging, per head: [128 rows][256 B], 16-byte chunks XOR-swizzled by row
-constexpr uint32_t OFF_ST = OFF_KV + NS * 2 * KV_BYTES;
-constexpr uint32_t OFF_BAR = OFF_ST + NH * ST_BYTES;
+constexpr uint32_t OFF_KV = OFF_Q + Q_BYTES;
+constexpr uint32_t OFF_BAR = OFF_KV + NS * 2 * KV_BYTES;
 constexpr uint32_t TC_SMEM = OFF_BAR + 256 + 1024;   // + barriers + manual 1024 B alignment slack
 
 struct Bars {
     uint64_t q_full, q_empty;
     uint64_t kv_full[NS], kv_empty[NS];
-    uint64_t s_full[NH][2];
-    uint64_t p_full[NH][2];
-    uint64_t o_full[NH][2], o_free[NH];   // o_full alternates by tile parity, see the softmax warps
-    uint32_t tmem;
 };
 static_assert(sizeof(Bars) <= 256, "barrier block");
-
-// Shared-memory matrix descriptors (cute::UMMA::SmemDescriptor), split in 32-bit halves so the issuing
-// thread only carries the low words.  High word (same for every operand here): SBO = 1024 B (8 rows of
-// 128 B) [32,46), version 1 [46,48), SWIZZLE_128B [61,64).  Low word: start address >> 4 [0,14), LBO >> 4
-// [16,30).  K-major operands (Q, K, P): LBO unused (1).  V is the MN-major B operand exactly as it lies
-// in the cache -- 64 dims (128 B) contiguous, 8 keys per 1024 B swizzle atom (SBO), the second 64-dim
-// half one TMA box (8192 B) further (LBO): canonical layout Sw<3,4,3> o ((8,n),(8,k)):((1,LBO),(8,SBO))
-// in 16-byte units.
-constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint32_t desc_lo_kmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint32_t desc_lo_mnmajor(uint32_t smem_addr) { return ((smem_addr & 0x3FFFFu) >> 4) | ((8192u >> 4) << 16); }
-__device__ __forceinline__ void umma_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 da, db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 da, {%1, %5};\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(DESC_HI)
-        : "memory");
-}
-// Same with the A operand in TMEM (lane = row, one 32-bit column = two consecutive bf16 along K).
-__device__ __forceinline__ void umma_ts_lo(uint32_t tmem_d, uint32_t tmem_a, uint32_t b_lo, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        ".reg .b64 db;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "mov.b64 db, {%2, %5};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "r"(tmem_a), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(DESC_HI)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-          "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-          "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-          "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-constexpr uint32_t IDESC_S = umma_idesc_bf16_f32(TQ, TKV);
-constexpr uint32_t IDESC_PV = umma_idesc_bf16_f32(TQ, 128) | (1u << 16);   // b_major = MN
 
 __device__ __forceinline__ float ex2(float x) {
     float y;
@@ -121,26 +52,26 @@ __device__ __forceinline__ float ex2(float x) {
 }
 
 struct Work {
-    int qt, seq, pair, tok0, len, n_kt;
+    int qt, seq, head, tok0, len, n_kt;
 };
-// Work item w -> (query tile, sequence, head pair).  The sequence bounds (and the slot, for the producer)
+// Work item w -> (query tile, sequence, head).  The sequence bounds (and the slot, for the producer)
 // are loaded one item ahead (WorkFetch) so their latency hides under the current item.
 struct WorkFetch {
     int tok0 = 0, tok1 = 0, slot = 0;
 };
-__device__ __forceinline__ void fetch_work(const PrefillAttnArgs& a, int w, int n_work, int n_pairs, bool want_slot, WorkFetch& f) {
+__device__ __forceinline__ void fetch_work(const PrefillAttnArgs& a, int w, int n_work, bool want_slot, WorkFetch& f) {
     if (w >= n_work) return;
-    const int seq = (w % (a.n_seqs * n_pairs)) / n_pairs;
+    const int seq = (w % (a.n_seqs * a.n_heads)) / a.n_heads;
     f.tok0 = __ldg(a.seq_start + seq);
     f.tok1 = __ldg(a.seq_start + seq + 1);
     if (want_slot) f.slot = __ldg(a.seq_slot + seq);
 }
-__device__ __forceinline__ bool decode_work(const PrefillAttnArgs& a, int w, int n_pairs, int max_qt, const WorkFetch& f, Work& k) {
-    const int per_qt = a.n_seqs * n_pairs;
+__device__ __forceinline__ bool decode_work(const PrefillAttnArgs& a, int w, int max_qt, const WorkFetch& f, Work& k) {
+    const int per_qt = a.n_seqs * a.n_heads;
     const int qrev = w / per_qt, rem = w - qrev * per_qt;
     k.qt = max_qt - 1 - qrev;
-    k.seq = rem / n_pairs;
-    k.pair = rem - k.seq * n_pairs;
+    k.seq = rem / a.n_heads;
+    k.head = rem - k.seq * a.n_heads;
     k.tok0 = f.tok0;
     k.len = f.tok1 - f.tok0;
     if (k.qt * TQ >= k.len) return false;
@@ -159,53 +90,37 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 
     griddep_launch();
     const int tr_slot = trace_begin(TR_ATTN_PF);
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == TC_CONSUMERS) {
         tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
-        mbar_init(&bars->q_full, 1); mbar_init(&bars->q_empty, 1);
-        for (int s = 0; s < NS; ++s) { mbar_init(&bars->kv_full[s], 1); mbar_init(&bars->kv_empty[s], 1); }
-        for (int h = 0; h < NH; ++h) {
-            for (int b = 0; b < 2; ++b) {
-                mbar_init(&bars->s_full[h][b], 1);
-                mbar_init(&bars->p_full[h][b], 4);          // one arrival per softmax warp
-            }
-            mbar_init(&bars->o_full[h][0], 1); mbar_init(&bars->o_full[h][1], 1); mbar_init(&bars->o_free[h], 4);
-        }
+        mbar_init(&bars->q_full, 1); mbar_init(&bars->q_empty, TC_CONSUMERS / 32);
+        for (int s = 0; s < NS; ++s) { mbar_init(&bars->kv_full[s], 1); mbar_init(&bars->kv_empty[s], TC_CONSUMERS / 32); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<512>(&bars->tmem);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem = bars->tmem;
 
     const int G = a.n_heads / a.n_kv_heads;
-    const int nh = (G % 2 == 0) ? NH : 1;      // query heads per work item: a pair only when both share one kv head
-    const int n_pairs = a.n_heads / nh;
     const int max_qt = (a.max_len + TQ - 1) / TQ;
-    const int n_work = max_qt * a.n_seqs * n_pairs;
+    const int n_work = max_qt * a.n_seqs * a.n_heads;
 
     griddep_wait();
     trace_dep(tr_slot);
 
-    if (warp == 0) {
+    if (warp == TC_PRODUCER_WARP) {
         // ------------------------------------------------------------------ TMA producer
-        if (elect_one()) {          // elect.sync: lets the compiler keep TMA / MMA operands on the uniform datapath
+        if (elect_one()) {
             uint32_t kv_it = 0, q_it = 0;
             WorkFetch nf;
-            fetch_work(a, blockIdx.x, n_work, n_pairs, true, nf);
+            fetch_work(a, blockIdx.x, n_work, true, nf);
             for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
                 Work k;
                 const WorkFetch f = nf;
-                fetch_work(a, w + gridDim.x, n_work, n_pairs, true, nf);
-                if (!decode_work(a, w, n_pairs, max_qt, f, k)) continue;
-                const int head0 = k.pair * nh, kvh = head0 / G;
-                const int kv_row0 = (f.slot * a.n_kv_heads + kvh) * a.ctx_max;
+                fetch_work(a, w + gridDim.x, n_work, true, nf);
+                if (!decode_work(a, w, max_qt, f, k)) continue;
+                const int kv_row0 = (f.slot * a.n_kv_heads + k.head / G) * a.ctx_max;
                 mbar_wait(&bars->q_empty, (q_it & 1) ^ 1);
-                mbar_arrive_expect_tx(&bars->q_full, nh * Q_BYTES);
-                for (int h = 0; h < nh; ++h)
-                    for (int c = 0; c < 2; ++c)
-                        tma_load_2d(smem + OFF_Q + h * Q_BYTES + c * 16384, &tmQ, &bars->q_full,
-                                    (head0 + h) * 128 + c * 64, k.tok0 + k.qt * TQ);
+                mbar_arrive_expect_tx(&bars->q_full, Q_BYTES);
+                for (int c = 0; c < 2; ++c)
+                    tma_load_2d(smem + OFF_Q + c * 16384, &tmQ, &bars->q_full, k.head * 128 + c * 64, k.tok0 + k.qt * TQ);
                 ++q_it;
                 for (int j = 0; j < k.n_kt; ++j, ++kv_it) {
                     const uint32_t s = kv_it % NS;
@@ -219,195 +134,125 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        if (elect_one()) {
-            uint32_t kv_it = 0, q_it = 0, s_it = 0, item_it = 0;
-            const uint32_t q_u = smem_u32(smem + OFF_Q), kv_u = smem_u32(smem + OFF_KV);
-            // O_h (+)= P_h(t) V(t).  `first`: tile 0 of the item overwrites O, which the softmax warps must
-            // have finished reading for the previous item (o_free).
-            auto pv = [&](uint32_t kvit_t, uint32_t sit_t, bool first) {
-                const uint32_t v_u = kv_u + (kvit_t % NS) * 2 * KV_BYTES + KV_BYTES, b = sit_t & 1;
-                for (int h = 0; h < nh; ++h) {
-                    mbar_wait(&bars->p_full[h][b], (sit_t >> 1) & 1);
-                    if (first) mbar_wait(&bars->o_free[h], (item_it & 1) ^ 1);
-                    tcgen05_fence_after();
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks)        // 16 keys = 8 TMEM columns of P per step
-                        umma_ts_lo(tmem + h * 256 + 128, tmem + h * 256 + b * 64 + ks * 8, desc_lo_mnmajor(v_u) + ks * 128,
-                                   IDESC_PV, (ks > 0 || !first) ? 1u : 0u);
-                    umma_commit(&bars->o_full[h][b]);
-                }
-                umma_commit(&bars->kv_empty[kvit_t % NS]);
-            };
-            WorkFetch nf;
-            fetch_work(a, blockIdx.x, n_work, n_pairs, false, nf);
-            for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
-                Work k;
-                const WorkFetch f = nf;
-                fetch_work(a, w + gridDim.x, n_work, n_pairs, false, nf);
-                if (!decode_work(a, w, n_pairs, max_qt, f, k)) continue;
-                mbar_wait(&bars->q_full, q_it & 1);
-                ++q_it;
-                for (int j = 0; j < k.n_kt; ++j, ++kv_it, ++s_it) {
-                    const uint32_t s = kv_it % NS, b = s_it & 1;
-                    mbar_wait(&bars->kv_full[s], (kv_it / NS) & 1);
-                    tcgen05_fence_after();
-                    const uint32_t k_u = kv_u + s * 2 * KV_BYTES;
-                    for (int h = 0; h < nh; ++h) {
-                        // S(j) lands on the columns of S(j-2) / P(j-2): PV(j-2) was issued before, the pipe runs in order
-#pragma unroll
-                        for (int ks = 0; ks < 8; ++ks)
-                            umma_lo(tmem + h * 256 + b * 64,
-                                    desc_lo_kmajor(q_u + h * Q_BYTES) + (ks >> 2) * 1024 + (ks & 3) * 2,
-                                    desc_lo_kmajor(k_u) + (ks >> 2) * 512 + (ks & 3) * 2, IDESC_S, ks > 0);
-                        umma_commit(&bars->s_full[h][b]);
-                    }
-                    if (j == k.n_kt - 1) umma_commit(&bars->q_empty);
-                    if (j > 0) pv(kv_it - 1, s_it - 1, j == 1);
-                }
-                pv(kv_it - 1, s_it - 1, k.n_kt == 1);
-                ++item_it;
-            }
-        }
-    } else if (warp >= 4 && ((warp - 4) >> 2) < nh) {
-        // ------------------------------------------------------------------ softmax + output
-        const int h = (warp - 4) >> 2, quarter = warp & 3, row = quarter * 32 + lane;
-        const uint32_t t_base = tmem + ((uint32_t)(quarter * 32) << 16) + h * 256;
+    } else {
+        // ------------------------------------------------------------------ consumer warpgroups
+        const int g = warp >> 2, w4 = warp & 3;
+        const int r_in = 64 * g + 16 * w4 + (lane >> 2);            // this thread's rows: r_in and r_in + 8 of the tile
+        const int cq = 2 * (lane & 3);                               // first of its two columns in every group of 8
         const float sc = a.scale * 1.4426950408889634f;
-        uint32_t s_it = 0;                 // global tile counter: S/P buffer, and the o_full phase of that tile's PV
+        const uint32_t q_u = smem_u32(smem + OFF_Q), kv_u = smem_u32(smem + OFF_KV);
+        uint32_t kv_it = 0, q_it = 0;
         WorkFetch nf;
-        fetch_work(a, blockIdx.x, n_work, n_pairs, false, nf);
-        uint8_t* stage = smem + OFF_ST + h * ST_BYTES;          // this head's 128 x 256 B output staging tile
+        fetch_work(a, blockIdx.x, n_work, false, nf);
         for (int w = blockIdx.x; w < n_work; w += gridDim.x) {
             Work k;
             const WorkFetch f = nf;
-            fetch_work(a, w + gridDim.x, n_work, n_pairs, false, nf);
-            if (!decode_work(a, w, n_pairs, max_qt, f, k)) continue;
-            const int head = k.pair * nh + h;
-            const int qi = k.qt * TQ + row;                       // query index inside the sequence
-            const int last_key = qi < k.len ? qi : k.len - 1;     // causal / ragged bound (inclusive)
-            float m_ref = -INFINITY, l = 0.f;                     // reference maximum (log2 domain), row sum
-
-            for (int j = 0; j < k.n_kt; ++j, ++s_it) {
-                const uint32_t b = s_it & 1;
-                mbar_wait(&bars->s_full[h][b], (s_it >> 1) & 1);
-                tcgen05_fence_after();
-                const uint32_t tS = t_base + b * 64;
+            fetch_work(a, w + gridDim.x, n_work, false, nf);
+            if (!decode_work(a, w, max_qt, f, k)) continue;
+            const int q0 = k.qt * TQ + r_in;                         // query indices inside the sequence
+            const int last0 = min(q0, k.len - 1), last1 = min(q0 + 8, k.len - 1);   // causal / ragged bound (inclusive)
+            const int wg_last_row = k.qt * TQ + 64 * g + 63;
+            float o[64];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) o[i] = 0.f;
+            float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running max (log2 domain), partial row sums
+            mbar_wait(&bars->q_full, q_it & 1);
+            ++q_it;
+            for (int j = 0; j < k.n_kt; ++j, ++kv_it) {
+                const uint32_t s = kv_it % NS;
+                mbar_wait(&bars->kv_full[s], (kv_it / NS) & 1);
                 const int key0 = j * TKV;
-                const bool need_mask = (key0 + TKV - 1 > k.qt * TQ) || (key0 + TKV > k.len);
-                const int lim = last_key - key0;                  // keep columns c <= lim
-                uint32_t v0[32], v1[32];                          // the whole S row of this query
-                tmem_ld_32x32b_x32(tS, v0);
-                tmem_ld_32x32b_x32(tS + 32, v1);
-                tmem_ld_wait();
-                if (need_mask) {
+                if (key0 <= wg_last_row) {
+                    const uint32_t k_u = kv_u + s * 2 * KV_BYTES, v_u = k_u + KV_BYTES;
+                    float sa[32];
+                    wgmma_fence_regs(sa);
+                    wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        if (i > lim) v0[i] = 0xff800000u;         // -inf
-                        if (32 + i > lim) v1[i] = 0xff800000u;
+                    for (int ks = 0; ks < 8; ++ks)
+                        wgmma_ss<64>(sa, gmma_desc_sw128(q_u + (ks >> 2) * 16384 + g * 8192) + (ks & 3) * 2,
+                                     gmma_desc_sw128(k_u + (ks >> 2) * 8192) + (ks & 3) * 2, ks > 0 ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(sa);
+                    // ---- causal mask, online softmax (a row lives in the 4 threads of a quad)
+                    const int lim0 = last0 - key0, lim1 = last1 - key0;
+                    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int col = 8 * jj + cq + e;
+                            if (col > lim0) sa[4 * jj + e] = -INFINITY;
+                            if (col > lim1) sa[4 * jj + 2 + e] = -INFINITY;
+                            mx0 = fmaxf(mx0, sa[4 * jj + e]);
+                            mx1 = fmaxf(mx1, sa[4 * jj + 2 + e]);
+                        }
                     }
-                }
-                float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    mx0 = fmaxf(mx0, __uint_as_float(v0[i]));
-                    mx1 = fmaxf(mx1, __uint_as_float(v1[i]));
-                }
-                const float m_new = fmaxf(m_ref, fmaxf(mx0, mx1) * sc);
-                if (j == 0) {
-                    m_ref = m_new;
-                } else if (__any_sync(0xffffffffu, m_new > m_ref + 8.f)) {
-                    // raise the reference: O and l of this warp's rows move to the new scale.  PV(j-1) must be
-                    // complete, and PV(j) cannot start before this warp arrives on p_full(j) below.  o_full is
-                    // not waited on every tile, so it alternates between two barriers: the previous phase of the
-                    // one PV(t) commits to belongs to PV(t-2), which is complete once S(t+1) or later is (in-order
-                    // pipe) -- the parity wait can never be a phase behind.
-                    const float alpha = ex2(m_ref - (m_new == -INFINITY ? 0.f : m_new));
-                    m_ref = m_new;
-                    l *= alpha;
-                    mbar_wait(&bars->o_full[h][(s_it - 1) & 1], ((s_it - 1) >> 1) & 1);
-                    tcgen05_fence_after();
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        uint32_t o[32];
-                        tmem_ld_32x32b_x32(t_base + 128 + c * 32, o);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-                        tmem_st_32x32b_x32(t_base + 128 + c * 32, o);
+                    for (int x = 1; x <= 2; x <<= 1) {
+                        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, x));
+                        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, x));
                     }
-                    tmem_st_wait();
-                }
-                const float ms = m_ref == -INFINITY ? 0.f : m_ref;
-                // ---- P = exp2(S * sc - ref) -> bf16 pairs -> TMEM columns [0, 32) of this S buffer
-                float ps0 = 0.f, ps1 = 0.f;
-                uint32_t pk[32];
+                    const float n0 = fmaxf(m0, mx0 * sc), n1 = fmaxf(m1, mx1 * sc);
+                    const float al0 = ex2(m0 - n0), al1 = ex2(m1 - n1);   // m = -inf on the first tile: 0
+                    m0 = n0; m1 = n1;
+                    l0 *= al0; l1 *= al1;
 #pragma unroll
-                for (int i = 0; i < 16; ++i) {
-                    const float e0 = ex2(fmaf(__uint_as_float(v0[2 * i]), sc, -ms));
-                    const float e1 = ex2(fmaf(__uint_as_float(v0[2 * i + 1]), sc, -ms));
-                    const float e2 = ex2(fmaf(__uint_as_float(v1[2 * i]), sc, -ms));
-                    const float e3 = ex2(fmaf(__uint_as_float(v1[2 * i + 1]), sc, -ms));
-                    ps0 += e0 + e1;
-                    ps1 += e2 + e3;
-                    pk[i] = pack_bf16(e0, e1);
-                    pk[16 + i] = pack_bf16(e2, e3);
+                    for (int jj = 0; jj < 16; ++jj) {
+                        o[4 * jj] *= al0; o[4 * jj + 1] *= al0;
+                        o[4 * jj + 2] *= al1; o[4 * jj + 3] *= al1;
+                    }
+                    uint32_t pa[4][4];                                  // P as the A fragments of the 4 k16 steps
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            const int b = 8 * kk + 4 * h;
+                            const float e0 = ex2(fmaf(sa[b], sc, -n0)), e1 = ex2(fmaf(sa[b + 1], sc, -n0));
+                            const float e2 = ex2(fmaf(sa[b + 2], sc, -n1)), e3 = ex2(fmaf(sa[b + 3], sc, -n1));
+                            l0 += e0 + e1;
+                            l1 += e2 + e3;
+                            pa[kk][2 * h] = pack_bf16(e0, e1);
+                            pa[kk][2 * h + 1] = pack_bf16(e2, e3);
+                        }
+                    }
+                    wgmma_fence_regs(o);
+                    wgmma_fence();
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk)                      // 16 keys = two 8-key swizzle atoms (2048 B) per step
+                        wgmma_rs_n128_tb(o, pa[kk], gmma_desc_sw128(v_u, 8192) + kk * (2048 >> 4), 1u);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_regs(o);
                 }
-                tmem_st_32x32b_x32(tS, pk);
-                l += ps0 + ps1;
-                tmem_st_wait();
-                tcgen05_fence_before();
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&bars->p_full[h][b]);
+                if (lane == 0) mbar_arrive(&bars->kv_empty[s]);
             }
-            // ---- O complete after the last PV (phase s_it - 1): normalise; stage the warp's 32 rows in smem, then
-            //      store them row-contiguously (2 rows of 256 B per warp instruction instead of 32 scattered pieces)
-            mbar_wait(&bars->o_full[h][(s_it - 1) & 1], ((s_it - 1) >> 1) & 1);
-            tcgen05_fence_after();
-            {
-                const float inv = l > 0.f ? 1.f / l : 0.f;
-                uint8_t* srow = stage + row * 256;
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bars->q_empty);                 // Q may be overwritten by the next item
+            // ---- O / l -> bf16, true head dims only
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
-                    uint32_t o[32];
-                    tmem_ld_32x32b_x32(t_base + 128 + c * 32, o);
-                    tmem_ld_wait();
+            for (int x = 1; x <= 2; x <<= 1) {
+                l0 += __shfl_xor_sync(0xffffffffu, l0, x);
+                l1 += __shfl_xor_sync(0xffffffffu, l1, x);
+            }
+            const float inv0 = l0 > 0.f ? 1.f / l0 : 0.f, inv1 = l1 > 0.f ? 1.f / l1 : 0.f;
+            const size_t row_pitch = (size_t)a.n_heads * a.head_dim;
+            __nv_bfloat16* ob = a.out + (size_t)k.tok0 * row_pitch + (size_t)k.head * a.head_dim;
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        uint4 pk;
-                        pk.x = pack_bf16(__uint_as_float(o[u * 8 + 0]) * inv, __uint_as_float(o[u * 8 + 1]) * inv);
-                        pk.y = pack_bf16(__uint_as_float(o[u * 8 + 2]) * inv, __uint_as_float(o[u * 8 + 3]) * inv);
-                        pk.z = pack_bf16(__uint_as_float(o[u * 8 + 4]) * inv, __uint_as_float(o[u * 8 + 5]) * inv);
-                        pk.w = pack_bf16(__uint_as_float(o[u * 8 + 6]) * inv, __uint_as_float(o[u * 8 + 7]) * inv);
-                        *reinterpret_cast<uint4*>(srow + (((c * 4 + u) ^ (row & 7)) << 4)) = pk;
-                    }
+            for (int jj = 0; jj < 16; ++jj) {
+                const int d = 8 * jj + cq;
+                if (d < a.head_dim) {
+                    if (q0 < k.len)
+                        *reinterpret_cast<uint32_t*>(ob + (size_t)q0 * row_pitch + d) = pack_bf16(o[4 * jj] * inv0, o[4 * jj + 1] * inv0);
+                    if (q0 + 8 < k.len)
+                        *reinterpret_cast<uint32_t*>(ob + (size_t)(q0 + 8) * row_pitch + d) =
+                            pack_bf16(o[4 * jj + 2] * inv1, o[4 * jj + 3] * inv1);
                 }
-                tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&bars->o_free[h]);     // O may be overwritten by the next item's first PV
-                const int c = lane & 15;                          // 16-byte chunk = 8 dims
-                const size_t row_pitch = (size_t)a.n_heads * a.head_dim;
-                __nv_bfloat16* obase = a.out + (size_t)k.tok0 * row_pitch + (size_t)head * a.head_dim + c * 8;
-                if (c * 8 < a.head_dim) {                         // dims beyond the true head dim are padding
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        const int rr = quarter * 32 + 2 * i + (lane >> 4);
-                        const int qr = k.qt * TQ + rr;
-                        const uint4 pk = *reinterpret_cast<const uint4*>(stage + rr * 256 + ((c ^ (rr & 7)) << 4));
-                        if (qr < k.len) *reinterpret_cast<uint4*>(obase + (size_t)qr * row_pitch) = pk;
-                    }
-                }
-                __syncwarp();
             }
         }
     }
-    tcgen05_fence_before();
     __syncthreads();
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<512>(tmem);
-    }
     trace_end(tr_slot);
 }
 
@@ -436,16 +281,15 @@ int prefill_attn_make_maps(PrefillAttnArgs* a, long long q_rows, long long kv_ro
 int launch_prefill_attn_tc(const PrefillAttnArgs& a, cudaStream_t st) {
     static std::atomic<uint64_t> attr{0};
     if (ensure_dyn_smem(prefill_attn_tc_kernel, (int)TC_SMEM, attr) != cudaSuccess) return RR_ERR_CUDA;
-    const int nh = ((a.n_heads / a.n_kv_heads) % 2 == 0) ? NH : 1;
-    const int n_work = ((a.max_len + TQ - 1) / TQ) * a.n_seqs * (a.n_heads / nh);
+    const int n_work = ((a.max_len + TQ - 1) / TQ) * a.n_seqs * a.n_heads;
     const int grid = n_work < num_sms() ? n_work : num_sms();
     cudaError_t e = launch_pdl(prefill_attn_tc_kernel, dim3(grid), dim3(TC_THREADS), (size_t)TC_SMEM, st,
                                a.tmQ, a.tmK, a.tmV, a);
     return e == cudaSuccess ? RR_OK : RR_ERR_CUDA;
 }
 
-// The one prefill attention path.  (Round 1 kept an mma.sync kernel for MHA models and as an A/B switch; the tcgen05 kernel
-// now serves every group size, so there is nothing to fall back to: an ineligible call fails.)
+// The one prefill attention path: the wgmma kernel serves every group size, so there is nothing to fall back to: an
+// ineligible call fails.
 int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st) {
     if (a.n_seqs <= 0 || a.max_len <= 0) return RR_OK;
     if (!prefill_attn_tc_eligible(a)) return RR_ERR_ARG;

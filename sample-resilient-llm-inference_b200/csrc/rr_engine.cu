@@ -137,7 +137,7 @@ struct rr_engine {
     int layer_ctr_words = 0;
     float *rowss_a = nullptr, *rowss_b = nullptr;   // [Bm][ceil(hidden / 128)] partial sum(x^2) (deferred RMSNorm)
     bool fuse_silu = false;           // wgu interleaved + one gate/up plane: SiLU*mul lives in the GEMM epilogue
-    bool fuse_mlp = false;            // decode: gate/up and down GEMMs in one persistent launch (gemm_mlp_tcgen05)
+    bool fuse_mlp = false;            // decode: gate/up and down GEMMs in one persistent launch (gemm_mlp_wgmma)
     std::vector<MlpPlan> mlp;         // per layer
     MlpItem* mlp_items = nullptr;     // device copy of the schedule (shared by all layers)
     unsigned* mlp_ready = nullptr;    // [n_slices] dependency counters, reset by the norm kernel before each launch
@@ -195,10 +195,14 @@ static int dalloc(rr_engine* e, T** p, size_t n, bool zero = true) {
     return RR_OK;
 }
 
+// Prefill GEMM tile width: the widest accumulator tile one consumer warpgroup holds in registers (rr_gemm_dev.cuh).
+constexpr int PF_BN = MAX_BN;
+
+// Decode tile width along the batch rows; batches wider than MAX_BN run several B tiles per weight tile.
 static int pick_bn(int rows) {
-    const int opts[5] = {16, 32, 64, 128, 256};
+    const int opts[4] = {16, 32, 64, MAX_BN};
     for (int b : opts) if (rows <= b) return b;
-    return -1;
+    return MAX_BN;
 }
 static int pick_splits(int N, int K) {
     const int tilesA = (N + 127) / 128;
@@ -325,7 +329,7 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
     P.qkv.resize(L); P.o.resize(L); P.gu.resize(L); P.down.resize(L);
     for (int l = 0; l < L; ++l) {
         int rc = gemm_plan_init(&P.qkv[l], e->pxn, T, d.hidden, e->wqkv[l], e->nqkv, d.hidden, d.hidden, e->pqkv,
-                                e->nqkv, 0, 1, e->fuse_rope_pf ? OUT_ROWMAJOR_ROPE : OUT_ROWMAJOR_BF16, 256);
+                                e->nqkv, 0, 1, e->fuse_rope_pf ? OUT_ROWMAJOR_ROPE : OUT_ROWMAJOR_BF16, PF_BN);
         if (rc) return rc;
         if (e->fuse_rope_pf) {
             RopeEpi& r = P.qkv[l].rope;
@@ -335,7 +339,7 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
             r.table = e->rope_table; r.n_heads = d.n_heads; r.n_kv_heads = d.n_kv_heads; r.ctx_max = e->o.ctx_max;
         }
         rc = gemm_plan_init(&P.o[l], e->pattn, T, e->nq, e->wo[l], d.hidden, e->nq, e->nq, e->px, d.hidden, 0, 1,
-                            OUT_ROWMAJOR_RESID, 256);                  // residual add in the epilogue
+                            OUT_ROWMAJOR_RESID, PF_BN);                // residual add in the epilogue
         if (rc) return rc;
         if (e->defer_norm_pf) {
             auto consumer = [&](RopeEpi& r) {
@@ -349,13 +353,13 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
         }
         if (e->fuse_silu)
             rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pact,
-                                d.inter, 0, 1, OUT_ROWMAJOR_SILU, 256);
+                                d.inter, 0, 1, OUT_ROWMAJOR_SILU, PF_BN);
         else
             rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pgu,
-                                2 * d.inter, 0, 1, OUT_ROWMAJOR_BF16, 256);
+                                2 * d.inter, 0, 1, OUT_ROWMAJOR_BF16, PF_BN);
         if (rc) return rc;
         rc = gemm_plan_init(&P.down[l], e->pact, T, d.inter, e->wdown[l], d.hidden, d.inter, d.inter, e->px,
-                            d.hidden, 0, 1, OUT_ROWMAJOR_RESID, 256);
+                            d.hidden, 0, 1, OUT_ROWMAJOR_RESID, PF_BN);
         if (rc) return rc;
         if (e->defer_norm_pf) {
             RopeEpi& c = P.gu[l].rope;
@@ -676,7 +680,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         n_sl = n_sl > 8 ? 8 : (n_sl < 1 ? 1 : n_sl);
         e->mlp_slice_kb = (kb1n + n_sl - 1) / n_sl;
         n_sl = (kb1n + e->mlp_slice_kb - 1) / e->mlp_slice_kb;
-        e->fuse_mlp = e->fuse_silu && opts->reserved[2] == 0 && d.inter % 64 == 0 && kb1n >= 1 && !getenv("RR_NO_MLP_FUSE");
+        e->fuse_mlp = e->fuse_silu && e->Bm <= e->bn_dec && opts->reserved[2] == 0 && d.inter % 64 == 0 && kb1n >= 1 && !getenv("RR_NO_MLP_FUSE");
         e->mlp_slices = e->fuse_mlp ? n_sl : 0;
     }
     TRY(dalloc(e, &e->part_down, (size_t)(e->s_down > e->mlp_slices ? e->s_down : e->mlp_slices) * B * d.hidden));
@@ -748,17 +752,15 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(gemm_plan_init(&e->pl_head_pf, e->lm_head, d.vocab, d.hidden, e->xn_last, B, d.hidden, d.hidden, e->logits,
                        d.vocab, B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
     e->fuse_rope_pf = d.head_dim == 128 && opts->reserved[1] == 0;
-    e->pf_parts = (d.hidden + 255) / 256;
-    // On by default (reserved[3] = 1 or RR_NO_DEFER_NORM=1 restores the two norm kernels per layer).  In-process A/B
-    // (tools/prefill_ab.py): 91.0 -> 85.2 ms per 8192-token chunk once the residual epilogue became line-coalesced;
-    // with the earlier row-per-thread epilogue the same fusion LOST 1.4 % (o-proj +35 %).
+    e->pf_parts = (d.hidden + PF_BN - 1) / PF_BN;
+    // On by default (reserved[3] = 1 or RR_NO_DEFER_NORM=1 restores the two norm kernels per layer; tools/prefill_ab.py
+    // compares the two in one process).
     e->defer_norm_pf = opts->reserved[3] == 0 && !getenv("RR_NO_DEFER_NORM") && d.hidden % 8 == 0 && e->pf_parts <= 64;
     if (e->defer_norm_pf) TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
-    // ---- persistent layer kernel (rr_layer.cu): OFF by default -- reserved[0] = 2 or RR_LAYER_FUSE=1 turns it on.
-    // Measured on B200 (tools/decode_ab.py, same process, alternating): 4.67 ms per decode step against 4.34 ms for the
-    // per-kernel path below.  Under a saturated weight stream every dependent memory round trip costs 2.5 - 4 us (the ring
-    // depth sweep in profiles/r02_layer_kernel_experiment.md), and a dependency counter is 3 - 4 of them (store drain,
-    // release, poll, operand load), while a kernel boundary happens when the memory system has drained.
+    // ---- persistent layer kernel (rr_layer.cu): OFF by default -- reserved[0] = 2 or RR_LAYER_FUSE=1 turns it on
+    // (tools/decode_ab.py compares it with the per-kernel path below in one process).  Under a saturated weight stream every
+    // dependent memory round trip costs microseconds, and a dependency counter is 3 - 4 of them (store drain, release, poll,
+    // operand load), while a kernel boundary happens when the memory system has drained.
     e->use_layer = e->fuse_mlp && (opts->reserved[0] == 2 || getenv("RR_LAYER_FUSE")) && !getenv("RR_NO_LAYER_FUSE");
     if (e->use_layer) {
         const int grid = num_sms();

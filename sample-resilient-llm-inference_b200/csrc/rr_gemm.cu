@@ -1,13 +1,13 @@
 // rr_gemm.cu — the path's one dense contraction (QKV / O / gate-up / down / lm_head projections)
-// on 5th-generation tensor cores: tcgen05.mma (UTCHMMA) with fp32 accumulators in TMEM,
-// operands staged by TMA (UTMALDG) into 128B-swizzled shared memory, persistent
-// warp-specialised CTAs (1 TMA warp, 1 MMA warp, 4 epilogue warps), double-buffered TMEM.
+// on Hopper tensor cores: wgmma (m64nNk16, bf16 in, fp32 accumulators in registers), operands staged by TMA
+// into 128B-swizzled shared memory, persistent warp-specialised CTAs (1 TMA producer warp, 1 consumer
+// warpgroup that issues the wgmma and runs the epilogue from the accumulators staged in shared memory).
 //
 //   D[a, b] = sum_k A[a, k] * B[b, k]          A: [rowsA, K] bf16, B: [rowsB, K] bf16 (both K-major)
 //
 // Two orientations of the same kernel:
 //   * prefill  (OUT_ROWMAJOR_BF16):  A = activations [T, K], B = weight [N, K]  -> C[T, N] bf16
-//   * decode   (OUT_TRANSPOSED_F32): A = weight [N, K] (UMMA M side, streamed once from HBM),
+//   * decode   (OUT_TRANSPOSED_F32): A = weight [N, K] (wgmma M side, streamed once from HBM),
 //                                    B = activations [batch<=BN, K]; fp32 partial planes
 //                                    P[z][b][n] reduced by the consumer kernel (rr_elementwise.cu).
 //     Work split for decode: uniform split-K (splits planes); the wave-quantisation tail of the big gate/up
@@ -27,10 +27,10 @@
 
 namespace rr {
 
-// Epilogue of one work item: TMEM accumulator (this warp's 32 lanes x BN columns at taddr0) -> global memory, in the
-// layout / fusion selected by MODE.  Shared by the 1-CTA kernel, the 2-CTA kernel and (by copy) the chain kernel.
+// Epilogue of one work item: staged accumulator tile (this thread's row, BN columns at arow) -> global memory, in the
+// layout / fusion selected by MODE.  Shared by the GEMM kernel and the fused MLP kernel.
 template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const WorkItem& t, int quarter, int lane,
+__device__ __forceinline__ void epilogue_item(const float* arow, int a_row, const WorkItem& t, int quarter, int lane,
                                               void* __restrict__ out, int rowsA, int rowsB, int ldo, int ld_rows,
                                               const RopeEpi& rope, float* silu_stage) {
     constexpr int CH = (BN >= 32) ? 32 : 16;
@@ -57,8 +57,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
         for (int c = 0; c < BN; c += 32) {
             float* buf = stage + ((c >> 5) & 1) * (32 * 64);
             uint32_t v[32];
-            tmem_ld_32x32b_x32(taddr0 + c, v);
-            tmem_ld_wait();
+            acc_ld32(arow + c, v);
             if (is_up) {
 #pragma unroll
                 for (int j = 0; j < 32; ++j) buf[j * 64 + r64] = __uint_as_float(v[j]);
@@ -75,7 +74,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
             }
         }
     } else if constexpr (MODE == OUT_ROWMAJOR_ROPE) {
-        // 256 columns = two 128-wide heads of the fused qkv projection; thread = token row.
+        // BN / 128 heads of 128 columns of the fused qkv projection; thread = token row.
         const bool row_ok = a_row < rowsA;
         const int slot = row_ok ? rope.slot[a_row] : -1;
         const int pos = row_ok ? rope.pos[a_row] : 0;
@@ -85,7 +84,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
         for (int hb = 0; hb < BN / 128; ++hb) {
             const int H = t.b_tile * (BN / 128) + hb;                  // head index in [q heads | k heads | v heads]
             if (H * 128 >= rowsB) break;
-            const uint32_t tcol = taddr0 + hb * 128;
+            const float* tcol = arow + hb * 128;
             if (H < rope.n_heads + rope.n_kv_heads) {
                 __nv_bfloat16* dst = H < rope.n_heads
                     ? rope.q_out + (size_t)a_row * (rope.n_heads * 128) + H * 128
@@ -93,9 +92,8 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
 #pragma unroll 1
                 for (int c = 0; c < 64; c += 32) {
                     uint32_t lo[32], hi[32];
-                    tmem_ld_32x32b_x32(tcol + c, lo);
-                    tmem_ld_32x32b_x32(tcol + 64 + c, hi);
-                    tmem_ld_wait();
+                    acc_ld32(tcol + c, lo);
+                    acc_ld32(tcol + 64 + c, hi);
                     if (live) {
 #pragma unroll
                         for (int j = 0; j < 32; j += 8) {
@@ -121,8 +119,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
 #pragma unroll 1
                 for (int c = 0; c < 128; c += 32) {
                     uint32_t v[32];
-                    tmem_ld_32x32b_x32(tcol + c, v);
-                    tmem_ld_wait();
+                    acc_ld32(tcol + c, v);
                     if (live) {
 #pragma unroll
                         for (int j = 0; j < 32; j += 8) {
@@ -141,7 +138,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
         float* xres = reinterpret_cast<float*>(out);
         const bool defer = rope.xhat != nullptr;       // also emit bf16(x * gamma) and sum(x^2) of this row over the tile
         if (silu_stage != nullptr) {
-            // Coalesced residual add.  TMEM hands every thread one ROW (32 consecutive columns = one 128-byte line per
+            // Coalesced residual add.  The staged tile hands every thread one ROW (32 consecutive columns = one 128-byte line per
             // chunk), so a direct read-modify-write issues 16-byte pieces of 32 different lines per instruction: 32 LSU
             // wavefronts and half-used sectors.  Each warp instead transposes its 32 x 32 chunk through 4.5 KB of shared
             // memory (row pitch 36 floats: conflict-free both ways) and lets 8 lanes cover one line: 4 full lines per
@@ -155,8 +152,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
 #pragma unroll 1
             for (int c = 0; c < BN; c += 32) {
                 uint32_t v[32];
-                tmem_ld_32x32b_x32(taddr0 + c, v);
-                tmem_ld_wait();
+                acc_ld32(arow + c, v);
                 const int b0 = t.b_tile * BN + c;
                 if (b0 + 32 <= rowsB) {
 #pragma unroll
@@ -233,8 +229,7 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
     #pragma unroll 1
             for (int c = 0; c < BN; c += 32) {
                 uint32_t v[32];
-                tmem_ld_32x32b_x32(taddr0 + c, v);
-                tmem_ld_wait();
+                acc_ld32(arow + c, v);
                 const int b0 = t.b_tile * BN + c;
                 if (a_row < rowsA) {
                     float* dst = xres + (size_t)a_row * ldo + b0;
@@ -278,8 +273,8 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
             if (defer && a_row < rowsA) rope.rowss_out[(size_t)a_row * rope.n_part_out + t.b_tile] = ss;
         }
     } else if constexpr (MODE == OUT_ROWMAJOR_SILU) {
-        // BN == 256 weight rows = [gate 64 | up 64 | gate 64 | up 64]: a token's gate and up values sit in the same
-        // TMEM lane, so silu(g) * u needs no exchange; 128 output columns per tile, ldo = inter.
+        // weight rows interleaved [gate 64 | up 64 | ...] (BN / 128 pairs per tile): a token's gate and up values sit in the same
+        // accumulator row, so silu(g) * u needs no exchange; 128 output columns per tile, ldo = inter.
         __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(out);
         const int n_out = rowsB >> 1;
 #pragma unroll 1
@@ -287,9 +282,8 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
 #pragma unroll 1
             for (int c = 0; c < 64; c += 32) {
                 uint32_t vg[32], vu[32];
-                tmem_ld_32x32b_x32(taddr0 + hb * 128 + c, vg);
-                tmem_ld_32x32b_x32(taddr0 + hb * 128 + 64 + c, vu);
-                tmem_ld_wait();
+                acc_ld32(arow + hb * 128 + c, vg);
+                acc_ld32(arow + hb * 128 + 64 + c, vu);
                 if (rope.n_part > 0) {
 #pragma unroll
                     for (int j = 0; j < 32; ++j) {
@@ -327,14 +321,13 @@ __device__ __forceinline__ void epilogue_item(uint32_t taddr0, int a_row, const 
     for (int c = 0; c < BN; c += CH) {
         uint32_t v[32];
         if constexpr (CH == 32) {
-            tmem_ld_32x32b_x32(taddr0 + c, v);
+            acc_ld32(arow + c, v);
         } else {
             uint32_t v16[16];
-            tmem_ld_32x32b_x16(taddr0 + c, v16);
+            acc_ld16(arow + c, v16);
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] = v16[j];
         }
-        tmem_ld_wait();
         const int b0 = t.b_tile * BN + c;
         if constexpr (MODE == OUT_ROWMAJOR_BF16) {
             if (rope.n_part > 0) {
@@ -383,7 +376,7 @@ __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 4, 128;" ::: 
 
 // planes tile: stage[b][n] fp32, b < BN, n < 128 (n = accumulator row = this thread)  ->  P[z][b][a_tile * 128 + n]
 template <int BN>
-__device__ __forceinline__ void epilogue_planes_tma(uint32_t taddr0, const WorkItem& t, int quarter, int lane, int etid,
+__device__ __forceinline__ void epilogue_planes_tma(const float* arow, const WorkItem& t, int quarter, int lane, int etid,
                                                     const CUtensorMap* tmOut, float* stage) {
     constexpr int CH = (BN >= 32) ? 32 : 16;
     if (etid == 0) bulk_wait_read0();              // the previous item's store has read the staging tile
@@ -393,14 +386,13 @@ __device__ __forceinline__ void epilogue_planes_tma(uint32_t taddr0, const WorkI
     for (int c = 0; c < BN; c += CH) {
         uint32_t v[32];
         if constexpr (CH == 32) {
-            tmem_ld_32x32b_x32(taddr0 + c, v);
+            acc_ld32(arow + c, v);
         } else {
             uint32_t v16[16];
-            tmem_ld_32x32b_x16(taddr0 + c, v16);
+            acc_ld16(arow + c, v16);
 #pragma unroll
             for (int j = 0; j < 16; ++j) v[j] = v16[j];
         }
-        tmem_ld_wait();
 #pragma unroll
         for (int j = 0; j < CH; ++j) col[(c + j) * 128] = __uint_as_float(v[j]);      // lanes = consecutive n: conflict-free
     }
@@ -417,7 +409,7 @@ __device__ __forceinline__ void epilogue_planes_tma(uint32_t taddr0, const WorkI
 // values of columns 0..15 (exch: two [16][64] fp32 halves per chunk, double-buffered), so each thread evaluates 16 SiLUs per
 // chunk instead of the gate threads 32.  act_stage[b][n64] bf16  ->  act[b][a_tile * 64 + n64]
 template <int BN>
-__device__ __forceinline__ void epilogue_silu_tma(uint32_t taddr0, const WorkItem& t, int quarter, int lane, int etid,
+__device__ __forceinline__ void epilogue_silu_tma(const float* arow, const WorkItem& t, int quarter, int lane, int etid,
                                                   const CUtensorMap* tmAct, float* exch, __nv_bfloat16* act_stage) {
     const bool is_up = quarter >= 2;
     const int r64 = (quarter & 1) * 32 + lane;
@@ -427,8 +419,7 @@ __device__ __forceinline__ void epilogue_silu_tma(uint32_t taddr0, const WorkIte
     for (int c = 0; c < BN; c += 32) {
         float* buf = exch + ((c >> 5) & 1) * (32 * 64);     // [0, 16) rows: up values of cols 0..15; [16, 32): gate values of cols 16..31
         uint32_t v[32];
-        tmem_ld_32x32b_x32(taddr0 + c, v);
-        tmem_ld_wait();
+        acc_ld32(arow + c, v);
         if (is_up) {
 #pragma unroll
             for (int j = 0; j < 16; ++j) buf[j * 64 + r64] = __uint_as_float(v[j]);
@@ -462,9 +453,9 @@ __device__ __forceinline__ void epilogue_silu_tma(uint32_t taddr0, const WorkIte
 
 template <int BN, int MODE, int CAP = 8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  void* __restrict__ out, int rowsA, int rowsB, int K, int splits, int ldo,
-                  int ld_rows, const RopeEpi rope, const __grid_constant__ CUtensorMap tmOut, int tma_epi) {
+gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                void* __restrict__ out, int rowsA, int rowsB, int K, int splits, int ldo,
+                int ld_rows, const RopeEpi rope, const __grid_constant__ CUtensorMap tmOut, int tma_epi) {
     using Cfg = GemmCfg<BN, CAP>;
     constexpr int kStages = Cfg::kStages;
 
@@ -474,38 +465,23 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint8_t* smemB = smem + kStages * Cfg::kStageBytesA;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full = empty_bar + kStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+    float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOff);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     griddep_launch();   // PDL: the next kernel may start its prologue now
     const int tr_slot = trace_begin(decode_orient<MODE>() ? TR_GEMM_DEC : TR_GEMM_PF);
 
-    if (warp == 0 && elect_one()) {
+    if (warp == PRODUCER_WARP && elect_one()) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
-    }
-    if (warp == 1) {
-        if (elect_one()) {
-            for (int s = 0; s < kStages; ++s) {
-                mbar_init(&full_bar[s], 1);
-                mbar_init(&empty_bar[s], 1);
-            }
-            for (int s = 0; s < 2; ++s) {
-                mbar_init(&tmem_full[s], 1);
-                mbar_init(&tmem_empty[s], 4);
-            }
-            fence_barrier_init();
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], GEMM_CONSUMERS / 32);   // one arrival per consumer warp
         }
-        __syncwarp();
-        tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
+        fence_barrier_init();
     }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     WorkSched sched;
     sched.init(rowsA, rowsB, K, splits, BN);
@@ -513,7 +489,7 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // detail trace of a plain decode projection: selected by its split-K factor (rr_debug_trace_detail(10 + splits)), CTAs 0 / 37 / 74 / 111
     const int tsm = (decode_orient<MODE>() && rr_trace_detail == 10 + splits && blockIdx.x % 37 == 0) ? 8 + (int)(blockIdx.x / 37) : -1;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             // Streamed-once operand (decode weights) should not displace the KV cache in L2;
@@ -526,8 +502,6 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             bool have = sched.next(t);
             if (tsm >= 0) trace_mark_at(TR_GEMM_MARK + 0, tsm, 0);
             // PDL prefetch of the constant (weight) operand for the first `pre` k-blocks.
-            // (An additional L2 prefetch of the panel behind the ring was measured in round 1: whole panel 5.12 -> 5.37 ms
-            //  per decode step, bounded to 8 / 16 k-blocks no gain / slower; removed.)
             int pre = 0;
             if (have) {
                 pre = min(kStages, t.kb1 - t.kb0);
@@ -574,66 +548,33 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             if (tsm >= 0) trace_mark_at(TR_GEMM_MARK + 2, tsm, 2);
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16_f32(BLOCK_A, BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int it = 0; sched.next(t); ++it) {
-                const int acc = it & 1;
-                const uint32_t acc_phase = (it >> 1) & 1;
-                mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (int kb = t.kb0; kb < t.kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    if (tsm >= 0 && kb == t.kb0) trace_mark_at(TR_GEMM_MARK + 3, tsm, 8 + it);
-                    tcgen05_fence_after();
-                    const uint64_t adesc =
-                        umma_desc_sw128_kmajor(smem_u32(smemA + stage * Cfg::kStageBytesA));
-                    const uint64_t bdesc =
-                        umma_desc_sw128_kmajor(smem_u32(smemB + stage * Cfg::kStageBytesB));
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-                        // advance 16 bf16 = 32 B inside the swizzle row: +2 in 16-byte units
-                        umma_bf16_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc,
-                                     (kb > t.kb0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&empty_bar[stage]);   // smem slot free once these MMAs retire
-                    if (++stage == kStages) {
-                        stage = 0;
-                        phase ^= 1;
-                    }
-                }
-                umma_commit(&tmem_full[acc]);         // accumulator ready for the epilogue
-            }
-        }
     } else {
-        // ===================== epilogue (warps 2..5) =====================
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
+        // ===================== consumer warpgroup: wgmma main loop, then the epilogue (warps 0..3) =====================
+        const int quarter = warp;                     // rows [32 quarter, 32 quarter + 32) of the tile in the epilogue
         const int row_in_tile = quarter * 32 + lane;
-        const int etid = (warp - 2) * 32 + lane;
-        float* epi_stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + 256);
+        const int etid = threadIdx.x;
+        float* epi_stage = reinterpret_cast<float*>(smem + Cfg::kEpiOff);
+        const uint32_t smemA_u = smem_u32(smemA), smemB_u = smem_u32(smemB);
         if (MODE == OUT_TRANSPOSED_F32 && BN <= 64 && tma_epi && etid == 0) tma_prefetch_desc(&tmOut);
         griddep_wait();                               // `out` may still be read by the preceding kernel
+        trace_dep(tr_slot);
+        int stage = 0;
+        uint32_t phase = 0;
         for (int it = 0; sched.next(t); ++it) {
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            mbar_wait(&tmem_full[acc], acc_phase);
+            float acc[2][BN / 2];
+            gmma_mainloop<BN>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages);
             if (tsm >= 0 && etid == 0) trace_mark_at(TR_GEMM_MARK + 4, tsm, 16 + 2 * it);
-            tcgen05_fence_after();
+            acc_bar();                                // the previous item's epilogue is done with the staged tile
+            stage_acc<BN>(acc, acc_tile);
+            acc_bar();
             const int a_row = t.a_tile * BLOCK_A + row_in_tile;
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
+            const float* arow = acc_tile + row_in_tile * Cfg::kAccPitch;
             bool done = false;
             if constexpr (MODE == OUT_TRANSPOSED_F32 && BN <= 64) {
-                if (tma_epi) { epilogue_planes_tma<BN>(taddr0, t, quarter, lane, etid, &tmOut, epi_stage); done = true; }
+                if (tma_epi) { epilogue_planes_tma<BN>(arow, t, quarter, lane, etid, &tmOut, epi_stage); done = true; }
             }
             if (!done)
-                epilogue_item<BN, MODE>(taddr0, a_row, t, quarter, lane, out, rowsA, rowsB, ldo, ld_rows, rope, epi_stage);
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+                epilogue_item<BN, MODE>(arow, a_row, t, quarter, lane, out, rowsA, rowsB, ldo, ld_rows, rope, epi_stage);
             if (tsm >= 0 && etid == 0) trace_mark_at(TR_GEMM_MARK + 5, tsm, 17 + 2 * it);
         }
         if constexpr (MODE == OUT_TRANSPOSED_F32 && BN <= 64) {
@@ -641,19 +582,14 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
     }
 
-    tcgen05_fence_before();
     __syncthreads();
     if (tsm >= 0 && threadIdx.x == 0) trace_mark_at(TR_GEMM_MARK + 6, tsm, 3);
     trace_end(tr_slot);
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
 }
 
 // =================================================================================================
 // Fused decode MLP: act = SiLU(x Wg^T) * (x Wu^T), planes = act Wd^T in ONE persistent launch (decode orientation,
-// weights on the UMMA M side).  Same warp roles, smem ring and TMEM double buffer as gemm_bf16_tcgen05; the pipeline
+// weights on the wgmma M side).  Same warp roles and smem ring as gemm_bf16_wgmma; the pipeline
 // state simply carries from item to item.  Each CTA runs its gate/up tiles from a host-built list, then its down items:
 // drawn from a device counter (a.dyn, default) or from the same list (static schedule, RR_MLP_STATIC).
 // A down item = (128 output features, one K-slice of `slice_kb` k-blocks); k-block kb of the down GEMM is
@@ -661,7 +597,7 @@ gemm_bf16_tcgen05(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // epilogue (TMA store of the act tile, completion wait, fence) bumps ready[slice] and the producer of a down item requests
 // the WEIGHT tiles of its first stages, then acquires ready[slice] == slice length, then requests the activation tiles.
 // No kernel boundary,
-// no wave-quantisation tail of the gate/up grid (224 tiles on 148 SMs): CTAs that own one gate/up tile start on the
+// no wave-quantisation tail of the gate/up grid (224 tiles on 132 SMs): CTAs that own one gate/up tile start on the
 // early slices while the others finish their second tile.
 __device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned* p) {
     unsigned v;
@@ -671,7 +607,7 @@ __device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned* p) {
 
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
+gemm_mlp_wgmma(const __grid_constant__ MlpArgs a) {
     using Cfg = GemmCfg<BN>;
     constexpr int kStages = Cfg::kStages;
 
@@ -681,36 +617,24 @@ gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
     uint8_t* smemB = smem + kStages * Cfg::kStageBytesA;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full = empty_bar + kStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
     volatile int* dyn_q = reinterpret_cast<volatile int*>(smem + kStages * Cfg::kStageBytes + 176);   // [16] dynamic down items of this CTA
-    float* silu_stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + 256);    // exchange; aliased by the planes tile
-    __nv_bfloat16* act_stage = reinterpret_cast<__nv_bfloat16*>(smem + kStages * Cfg::kStageBytes + 256 + Cfg::kSiluStageBytes);
+    float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOff);
+    float* silu_stage = reinterpret_cast<float*>(smem + Cfg::kEpiOff);    // exchange; aliased by the planes tile
+    __nv_bfloat16* act_stage = reinterpret_cast<__nv_bfloat16*>(smem + Cfg::kEpiOff + Cfg::kSiluStageBytes);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     griddep_launch();
     const int tr_slot = trace_begin(TR_GEMM_DEC);
 
-    if (warp == 0 && elect_one()) {
+    if (warp == PRODUCER_WARP && elect_one()) {
         tma_prefetch_desc(&a.tmA0); tma_prefetch_desc(&a.tmB0);
         tma_prefetch_desc(&a.tmA1); tma_prefetch_desc(&a.tmB1);
         if (a.tma_epi) { tma_prefetch_desc(&a.tmAct); tma_prefetch_desc(&a.tmPlanes); }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], GEMM_CONSUMERS / 32); }
+        for (int s = 0; s < 16; ++s) dyn_q[s] = -2;
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        if (elect_one()) {
-            for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-            for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 4); }
-            for (int s = 0; s < 16; ++s) dyn_q[s] = -2;
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     const int4* my = reinterpret_cast<const int4*>(a.items) + (size_t)blockIdx.x * a.max_items;   // constant data
     auto get = [&](int i, WorkItem& t, int& ph) -> bool {
@@ -724,7 +648,7 @@ gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
     // order (z = q / tiles1) from a global counter, so the split follows the real finishing order instead of a host-side time
     // model (the static list schedule left a 10 us tail: CTAs with three down items next to CTAs with one).  The producer thread
     // draws q -- when the last load of the current item is out, so the round trip of the atomic overlaps the drain of the ring and
-    // no CTA sits on an item it cannot start -- and publishes it to the MMA / epilogue warps through dyn_q[] (-2 = not drawn yet,
+    // no CTA sits on an item it cannot start -- and publishes it to the consumer warpgroup through dyn_q[] (-2 = not drawn yet,
     // -1 = no more work).  Which CTA computes an item does not change a single bit of its plane tile.
     auto dyn_decode = [&](int q, WorkItem& t, int& ph) {
         const int z = q / a.tiles1;
@@ -748,7 +672,7 @@ gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
     WorkItem t;
     int ph = 0;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             const uint64_t polA = l2_policy_evict_first(), polB = l2_policy_evict_last();
@@ -815,68 +739,45 @@ gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16_f32(BLOCK_A, BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int nstat = -1;
-            for (int it = 0; next_consumer(it, nstat, t, ph); ++it) {
-                const int acc = it & 1;
-                mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (int kb = t.kb0; kb < t.kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    if (kb == t.kb0) trace_mark_fixed(TR_MLP_MARK + 4 + ph, 64 + it);
-                    tcgen05_fence_after();
-                    const uint64_t adesc = umma_desc_sw128_kmajor(smem_u32(smemA + stage * Cfg::kStageBytesA));
-                    const uint64_t bdesc = umma_desc_sw128_kmajor(smem_u32(smemB + stage * Cfg::kStageBytesB));
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                        umma_bf16_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > t.kb0 || k > 0) ? 1u : 0u);
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tmem_full[acc]);
-            }
-        }
     } else {
-        // ===================== epilogue (warps 2..5) =====================
-        const int quarter = warp & 3;
+        // ===================== consumer warpgroup: wgmma main loop + epilogue (warps 0..3) =====================
+        const int quarter = warp;
         const int row_in_tile = quarter * 32 + lane;
-        const int etid = (warp - 2) * 32 + lane;
+        const int etid = threadIdx.x;
+        const uint32_t smemA_u = smem_u32(smemA), smemB_u = smem_u32(smemB);
+        int stage = 0;
+        uint32_t phase = 0;
         RopeEpi no_rope;
         no_rope.q_out = nullptr; no_rope.k_cache = nullptr; no_rope.v_cache = nullptr; no_rope.slot = nullptr;
         no_rope.pos = nullptr; no_rope.table = nullptr; no_rope.n_heads = 0; no_rope.n_kv_heads = 0; no_rope.ctx_max = 0;
         griddep_wait();
+        trace_dep(tr_slot);
         int nstat = -1;
         for (int it = 0; next_consumer(it, nstat, t, ph); ++it) {
-            const int acc = it & 1;
-            mbar_wait(&tmem_full[acc], (it >> 1) & 1);
+            if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 4 + ph, 64 + it);
+            float acc[2][BN / 2];
+            gmma_mainloop<BN>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages);
             if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 6 + ph, 128 + 4 * it);
-            tcgen05_fence_after();
+            acc_bar();
+            stage_acc<BN>(acc, acc_tile);
+            acc_bar();
             const int a_row = t.a_tile * BLOCK_A + row_in_tile;
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
+            const float* arow = acc_tile + row_in_tile * Cfg::kAccPitch;
             bool tma_done = false;
             if constexpr (BN <= 64) {
                 if (a.tma_epi) {
-                    if (ph == 0) epilogue_silu_tma<BN>(taddr0, t, quarter, lane, etid, &a.tmAct, silu_stage, act_stage);
-                    else epilogue_planes_tma<BN>(taddr0, t, quarter, lane, etid, &a.tmPlanes, silu_stage);
+                    if (ph == 0) epilogue_silu_tma<BN>(arow, t, quarter, lane, etid, &a.tmAct, silu_stage, act_stage);
+                    else epilogue_planes_tma<BN>(arow, t, quarter, lane, etid, &a.tmPlanes, silu_stage);
                     tma_done = true;
                 }
             }
             if (tma_done) {
             } else if (ph == 0)
-                epilogue_item<BN, OUT_TRANSPOSED_SILU>(taddr0, a_row, t, quarter, lane, a.act, 2 * a.inter, a.rows, a.inter, 0,
+                epilogue_item<BN, OUT_TRANSPOSED_SILU>(arow, a_row, t, quarter, lane, a.act, 2 * a.inter, a.rows, a.inter, 0,
                                                        no_rope, silu_stage);
             else
-                epilogue_item<BN, OUT_TRANSPOSED_F32>(taddr0, a_row, t, quarter, lane, a.out1, a.hidden, a.rows, a.hidden,
+                epilogue_item<BN, OUT_TRANSPOSED_F32>(arow, a_row, t, quarter, lane, a.out1, a.hidden, a.rows, a.hidden,
                                                       a.ld_rows, no_rope, nullptr);
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
             if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 10, 128 + 4 * it + 1);      // stores issued
             if (ph == 0) {
                 // publish this tile's 64 act columns: every epilogue thread's stores, then one release-increment
@@ -902,218 +803,9 @@ gemm_mlp_tcgen05(const __grid_constant__ MlpArgs a) {
         }
     }
 
-    if (a.tma_epi && threadIdx.x == 64) bulk_wait_read0();  // epilogue thread 0: the staging tile must outlive the reads of its stores
-    tcgen05_fence_before();
+    if (a.tma_epi && threadIdx.x == 0) bulk_wait_read0();   // epilogue thread 0: the staging tile must outlive the reads of its stores
     __syncthreads();
     trace_end(tr_slot);
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
-}
-
-// =================================================================================================
-// 2-CTA variant for the prefill orientation (tokens on M): a CTA pair (cluster of 2, same TPC) computes a
-// 256 x 256 tile with tcgen05.mma.cta_group::2 (UMMA M = 256).  Each CTA stages its own 128 rows of A and only HALF of
-// the 256 B rows per k-block (the tensor core reads the other half from the peer's shared memory), so the smem fill
-// traffic per FLOP halves and the ring holds 6 stages of 32 KB instead of 4 of 48 KB.  The leader CTA (rank 0) issues
-// the MMAs; both CTAs run a TMA producer (2SM TMA form: transaction bytes land on the leader's full barrier) and 4
-// epilogue warps for their own 128 accumulator rows.  tcgen05.commit multicasts "slot free" / "accumulator ready" to
-// both CTAs; the epilogue warps of both CTAs release the accumulator on the leader's barrier.
-constexpr int K2_BN = 256;
-constexpr int K2_STAGE_A = BLOCK_A * BLOCK_K * 2;          // 16 KB: this CTA's 128 rows of A
-constexpr int K2_STAGE_B = 128 * BLOCK_K * 2;              // 16 KB: this CTA's half of the 256 B rows
-constexpr int K2_STAGE = K2_STAGE_A + K2_STAGE_B;
-constexpr int K2_STAGES = 6;
-constexpr int K2_EPI_STAGE = 4 * 32 * 36 * 4;             // residual epilogue: per-warp 32 x 36 fp32 transpose tiles
-constexpr int K2_SMEM = K2_STAGES * K2_STAGE + 1024 + 256 + K2_EPI_STAGE;
-constexpr int GROUP_PAIRS = 8;
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t addr, uint32_t cta) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(cta));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int32_t c0, int32_t c1,
-                                                uint64_t policy) {
-    // executed by both CTAs; peer bit cleared so the transaction bytes update the leader CTA's barrier
-    const uint32_t mbar = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4}], [%2], %5;"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar), "r"(c0), "r"(c1), "l"(policy)
-        : "memory");
-}
-__device__ __forceinline__ void umma_bf16_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {      // arrives on `bar` in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-                 : "memory");
-}
-
-template <int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_tcgen05_2cta(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                       void* __restrict__ out, int rowsA, int rowsB, int K, int ldo, const RopeEpi rope) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = align_smem_1024(smem_raw);
-    uint8_t* smemA = smem;
-    uint8_t* smemB = smem + K2_STAGES * K2_STAGE_A;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + K2_STAGES * K2_STAGE);
-    uint64_t* empty_bar = full_bar + K2_STAGES;
-    uint64_t* tmem_full = empty_bar + K2_STAGES;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    griddep_launch();
-    const int tr_slot = trace_begin(TR_GEMM_PF);
-
-    if (warp == 0 && elect_one()) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-    }
-    if (warp == 1) {
-        if (elect_one()) {
-            for (int s = 0; s < K2_STAGES; ++s) {
-                mbar_init(&full_bar[s], 1);        // leader's expect_tx arrive; both CTAs' TMA bytes complete on it
-                mbar_init(&empty_bar[s], 1);       // multicast commit
-            }
-            for (int s = 0; s < 2; ++s) {
-                mbar_init(&tmem_full[s], 1);       // multicast commit
-                mbar_init(&tmem_empty[s], 8);      // 4 epilogue warps of each CTA (leader's instance is the one waited on)
-            }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    cluster_sync_all();                            // peer barriers initialised before any remote arrive / multicast
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-
-    const int pairsA = (rowsA + 255) / 256;
-    const int tilesB = (rowsB + K2_BN - 1) / K2_BN;
-    const int kblocks = (K + BLOCK_K - 1) / BLOCK_K;
-    const int n_work = pairsA * tilesB;
-    const int n_clusters = gridDim.x >> 1, cluster_id = blockIdx.x >> 1;
-    auto decode = [&](int w, int& pa, int& tb) {
-        const int per_group = GROUP_PAIRS * tilesB;
-        const int g = w / per_group, r = w - g * per_group;
-        const int a0 = g * GROUP_PAIRS, ga = min(GROUP_PAIRS, pairsA - a0);
-        pa = a0 + r % ga;
-        tb = r / ga;
-    };
-
-    if (warp == 0) {
-        // ===================== TMA producer (both CTAs) =====================
-        if (elect_one()) {
-            const uint64_t polA = l2_policy_evict_last(), polB = l2_policy_evict_last();
-            griddep_wait();
-            trace_dep(tr_slot);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int w = cluster_id; w < n_work; w += n_clusters) {
-                int pa, tb;
-                decode(w, pa, tb);
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    // The peer needs no arrive of its own: its loads for the next phase are only issued after its
-                    // empty barrier fired, i.e. after the leader consumed the previous phase.
-                    if (leader) mbar_arrive_expect_tx(&full_bar[stage], 2 * K2_STAGE);
-                    tma_load_2d_2sm(smemA + stage * K2_STAGE_A, &tmA, &full_bar[stage], kb * BLOCK_K,
-                                    pa * 256 + (int)rank * 128, polA);
-                    tma_load_2d_2sm(smemB + stage * K2_STAGE_B, &tmB, &full_bar[stage], kb * BLOCK_K,
-                                    tb * K2_BN + (int)rank * 128, polB);
-                    if (++stage == K2_STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (leader CTA only) =====================
-        if (leader && elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16_f32(256, K2_BN);
-            int stage = 0, it = 0;
-            uint32_t phase = 0;
-            for (int w = cluster_id; w < n_work; w += n_clusters, ++it) {
-                const int acc = it & 1;
-                mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * K2_BN;
-                for (int kb = 0; kb < kblocks; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tcgen05_fence_after();
-                    const uint64_t adesc = umma_desc_sw128_kmajor(smem_u32(smemA + stage * K2_STAGE_A));
-                    const uint64_t bdesc = umma_desc_sw128_kmajor(smem_u32(smemB + stage * K2_STAGE_B));
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                        umma_bf16_ss_2sm(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-                    umma_commit_2sm(&empty_bar[stage]);
-                    if (++stage == K2_STAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit_2sm(&tmem_full[acc]);
-            }
-        }
-    } else {
-        // ===================== epilogue (both CTAs: own 128 rows x 256 columns) =====================
-        const int quarter = warp & 3;
-        const int row_in_tile = quarter * 32 + lane;
-        const uint32_t empty0_remote = mapa_u32(smem_u32(&tmem_empty[0]), 0);
-        griddep_wait();
-        int it = 0;
-        for (int w = cluster_id; w < n_work; w += n_clusters, ++it) {
-            int pa, tb;
-            decode(w, pa, tb);
-            const int acc = it & 1;
-            mbar_wait(&tmem_full[acc], (it >> 1) & 1);
-            tcgen05_fence_after();
-            WorkItem t;
-            t.a_tile = pa * 2 + (int)rank; t.b_tile = tb; t.z = 0; t.kb0 = 0; t.kb1 = kblocks;
-            const int a_row = t.a_tile * BLOCK_A + row_in_tile;
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * K2_BN;
-            epilogue_item<K2_BN, MODE>(taddr0, a_row, t, quarter, lane, out, rowsA, rowsB, ldo, 0, rope,
-                                       reinterpret_cast<float*>(smem + K2_STAGES * K2_STAGE + 256));
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(empty0_remote + acc * 8);
-        }
-    }
-
-    tcgen05_fence_before();
-    __syncthreads();
-    cluster_sync_all();                            // the peer's tensor core may still read this CTA's shared memory
-    trace_end(tr_slot);
-    if (warp == 1) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
-    }
 }
 
 // ---------------------------------------------------------------- host side
@@ -1191,7 +883,7 @@ int num_sms() {                         // of the current device (one process ma
 template <int BN, int MODE>
 static int launch_one(const GemmPlan& p, cudaStream_t st) {
     constexpr int CAP = 8;
-    auto kern = gemm_bf16_tcgen05<BN, MODE, CAP>;
+    auto kern = gemm_bf16_wgmma<BN, MODE, CAP>;
     static std::atomic<uint64_t> attr_set{0};
     if (ensure_dyn_smem(kern, (int)gemm_smem_bytes<BN, MODE, CAP>(), attr_set) != cudaSuccess) return RR_ERR_CUDA;
     const int tilesA = (p.rowsA + BLOCK_A - 1) / BLOCK_A;
@@ -1203,9 +895,8 @@ static int launch_one(const GemmPlan& p, cudaStream_t st) {
     return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
 }
 
-static bool decode_orient_rt(int mode) { return mode == OUT_TRANSPOSED_F32 || mode == OUT_TRANSPOSED_SILU; }
-
-// splits >= 1: uniform split-K with `splits` planes.
+// splits >= 1: uniform split-K with `splits` planes.  bn = 256 is accepted and runs 128-wide tiles: a consumer warpgroup holds
+// at most 128 x 128 fp32 accumulators in registers.
 int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB,
                    int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn) {
     if (K % 8 != 0 || ldA % 8 != 0 || ldB % 8 != 0) return RR_ERR_ARG;
@@ -1216,8 +907,9 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
     if (mode == OUT_ROWMAJOR_BF16 && (splits != 1 || ldo % 8 != 0)) return RR_ERR_ARG;
     // fused SiLU*mul epilogues: weights row-interleaved in 64-row gate/up blocks, one plane, bf16 act output
     if (mode == OUT_TRANSPOSED_SILU && (splits != 1 || bn < 32 || rowsA % 128 != 0)) return RR_ERR_ARG;
-    if (mode == OUT_ROWMAJOR_SILU && (splits != 1 || bn != 256 || rowsB % 128 != 0 || ldo % 8 != 0)) return RR_ERR_ARG;
-    if (mode == OUT_ROWMAJOR_ROPE && (splits != 1 || bn != 256 || rowsB % 128 != 0)) return RR_ERR_ARG;
+    if (mode == OUT_ROWMAJOR_SILU && (splits != 1 || bn < 128 || rowsB % 128 != 0 || ldo % 8 != 0)) return RR_ERR_ARG;
+    if (mode == OUT_ROWMAJOR_ROPE && (splits != 1 || bn < 128 || rowsB % 128 != 0)) return RR_ERR_ARG;
+    if (bn > MAX_BN) bn = MAX_BN;
     if (mode == OUT_ROWMAJOR_RESID && (splits != 1 || bn < 32 || ldo % 4 != 0)) return RR_ERR_ARG;
     if (mode < 0 || mode > OUT_ROWMAJOR_RESID) return RR_ERR_ARG;
     memset(&p->rope, 0, sizeof(p->rope));
@@ -1225,7 +917,6 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
     p->splits = splits; p->mode = mode; p->bn = bn; p->max_ctas = 0;
     int rc = make_tmap_bf16_2d(&p->tmA, A, rowsA, K, ldA, BLOCK_A);
     if (rc != RR_OK) return rc;
-    // prefill orientation with 256-wide tiles and at least one full 256-row pair: 2-CTA kernel (B box = 128 rows)
     // decode planes through one TMA store per item: needs 16-byte pitches and at most 64 batch columns per tile
     p->tma_epi = 0;
     if (mode == OUT_TRANSPOSED_F32 && bn <= 64 && ldo % 4 == 0 && ((uintptr_t)out & 15) == 0 && !getenv("RR_NO_TMA_EPI")) {
@@ -1233,38 +924,10 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
         if (rc != RR_OK) return rc;
         p->tma_epi = 1;
     }
-    p->two_cta = (bn == 256 && !decode_orient_rt(mode) && rowsA >= 256) ? 1 : 0;
-    if (p->two_cta) {
-        rc = make_tmap_bf16_2d(&p->tmB2, B, rowsB, K, ldB, 128);
-        if (rc != RR_OK) return rc;
-    }
     return make_tmap_bf16_2d(&p->tmB, B, rowsB, K, ldB, bn);
 }
 
-template <int MODE>
-static int launch_2cta(const GemmPlan& p, cudaStream_t st) {
-    auto kern = gemm_bf16_tcgen05_2cta<MODE>;
-    static std::atomic<uint64_t> attr_set{0};
-    if (ensure_dyn_smem(kern, (int)K2_SMEM, attr_set) != cudaSuccess) return RR_ERR_CUDA;
-    const int pairs = (p.rowsA + 255) / 256, tilesB = (p.rowsB + K2_BN - 1) / K2_BN;
-    int clusters = pairs * tilesB;
-    if (clusters > num_sms() / 2) clusters = num_sms() / 2;
-    cudaError_t le = launch_pdl(kern, dim3(2 * clusters), dim3(GEMM_THREADS), (size_t)K2_SMEM, st, p.tmA, p.tmB2, p.out,
-                                p.rowsA, p.rowsB, p.K, p.ldo, p.rope);
-    return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
-}
-
-int g_use_2cta = getenv("RR_NO_2CTA") ? 0 : 1;
-
 int gemm_launch(const GemmPlan& p, cudaStream_t st) {
-    if (p.two_cta && g_use_2cta) {
-        switch (p.mode) {
-            case OUT_ROWMAJOR_BF16: return launch_2cta<OUT_ROWMAJOR_BF16>(p, st);
-            case OUT_ROWMAJOR_SILU: return launch_2cta<OUT_ROWMAJOR_SILU>(p, st);
-            case OUT_ROWMAJOR_ROPE: return launch_2cta<OUT_ROWMAJOR_ROPE>(p, st);
-            case OUT_ROWMAJOR_RESID: return launch_2cta<OUT_ROWMAJOR_RESID>(p, st);
-        }
-    }
 #define RR_CASE(BN_)                                                                                  \
     case BN_:                                                                                         \
         if (p.mode == OUT_ROWMAJOR_BF16) return launch_one<BN_, OUT_ROWMAJOR_BF16>(p, st);             \
@@ -1275,7 +938,7 @@ int gemm_launch(const GemmPlan& p, cudaStream_t st) {
         if constexpr (BN_ >= 128) {                                                                   \
             if (p.mode == OUT_ROWMAJOR_RESID) return launch_one<BN_, OUT_ROWMAJOR_RESID>(p, st);       \
         }                                                                                             \
-        if constexpr (BN_ == 256) {                                                                   \
+        if constexpr (BN_ == 128) {                                                                   \
             if (p.mode == OUT_ROWMAJOR_SILU) return launch_one<BN_, OUT_ROWMAJOR_SILU>(p, st);         \
             if (p.mode == OUT_ROWMAJOR_ROPE) return launch_one<BN_, OUT_ROWMAJOR_ROPE>(p, st);         \
         }                                                                                             \
@@ -1285,7 +948,6 @@ int gemm_launch(const GemmPlan& p, cudaStream_t st) {
         RR_CASE(32)
         RR_CASE(64)
         RR_CASE(128)
-        RR_CASE(256)
     }
 #undef RR_CASE
     return RR_ERR_ARG;
@@ -1347,7 +1009,7 @@ int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hi
                   void* act, void* planes, int ld_rows, int bn, const MlpItem* items_dev, int max_items, int grid,
                   unsigned* ready, int slice_kb, int dynamic) {
     if (!p || !Wgu || !Wd || !xn || !act || !planes || !items_dev || !ready) return RR_ERR_ARG;
-    if (inter % 64 || (2 * inter) % BLOCK_A || hidden % 8 || rows > bn || bn < 32 || slice_kb < 1) return RR_ERR_ARG;
+    if (inter % 64 || (2 * inter) % BLOCK_A || hidden % 8 || rows > bn || bn < 32 || bn > MAX_BN || slice_kb < 1) return RR_ERR_ARG;
     if ((2 * inter) / BLOCK_A > 0xffff || grid < 1 || grid > num_sms()) return RR_ERR_ARG;
     MlpArgs& a = p->args;
     int rc = make_tmap_bf16_2d(&a.tmA0, Wgu, 2 * inter, hidden, hidden, BLOCK_A);
@@ -1373,7 +1035,7 @@ int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hi
 
 template <int BN>
 static int launch_mlp_bn(const MlpPlan& p, cudaStream_t st) {
-    auto kern = gemm_mlp_tcgen05<BN>;
+    auto kern = gemm_mlp_wgmma<BN>;
     static std::atomic<uint64_t> attr_set{0};
     constexpr int smem = GemmCfg<BN>::kSmemBytes + mlp_stage_bytes<BN>();
     static_assert(smem <= 227 * 1024, "fused MLP kernel: shared memory budget");
@@ -1387,7 +1049,6 @@ int mlp_launch(const MlpPlan& p, cudaStream_t st) {
         case 32: return launch_mlp_bn<32>(p, st);
         case 64: return launch_mlp_bn<64>(p, st);
         case 128: return launch_mlp_bn<128>(p, st);
-        case 256: return launch_mlp_bn<256>(p, st);
     }
     return RR_ERR_ARG;
 }

@@ -44,13 +44,15 @@ struct RopeEpi {
     int n_part_out;
 };
 
+// Widest GEMM tile along B rows (and so the largest decode batch): a consumer warpgroup holds 128 x MAX_BN fp32
+// accumulators in registers, 2 x 64 per thread at 128.
+constexpr int MAX_BN = 128;
+
 struct GemmPlan {
     CUtensorMap tmA, tmB;
     void* out;
     int rowsA, rowsB, K, splits, ldo, ld_rows, mode, bn, max_ctas;
     RopeEpi rope;             // OUT_ROWMAJOR_ROPE only
-    CUtensorMap tmB2;         // 2-CTA kernel: B with a 128-row box (each CTA of the pair stages half of the 256 rows)
-    int two_cta;
     CUtensorMap tmOut;        // OUT_TRANSPOSED_F32: planes [splits][rowsB][rowsA] (3-D, box {128, bn, 1}) for the TMA-store epilogue
     int tma_epi;              // 1: the epilogue stages the tile in shared memory and issues ONE TMA store per item
 };
@@ -240,7 +242,7 @@ struct PrefillAttnArgs {
     CUtensorMap tmQ, tmK, tmV;
 };
 int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st);   // RR_ERR_ARG when the maps are missing / shape unsupported
-// tcgen05 kernel (rr_attn_tc.cu): head pairs for even GQA group sizes, one head per item otherwise (MHA).
+// wgmma kernel (rr_attn_tc.cu): one (sequence, head, 128-row query tile) per work item.
 int prefill_attn_make_maps(PrefillAttnArgs* a, long long q_rows, long long kv_rows);
 bool prefill_attn_tc_eligible(const PrefillAttnArgs& a);
 int launch_prefill_attn_tc(const PrefillAttnArgs& a, cudaStream_t st);

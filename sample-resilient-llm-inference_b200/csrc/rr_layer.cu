@@ -5,9 +5,8 @@
 //   phase 2  down projection   act[rows, inter]    x Wd[hidden, inter]    -> x += ... (slice by slice), xhat, sum(x^2)
 //   phase 3  next projection   xhat[rows, hidden]  x W3[rowsA3, hidden]   -> planes * r   (QKV of layer l + 1, or lm_head)
 //
-// Same warp roles, smem ring and TMEM double buffer as gemm_bf16_tcgen05 / gemm_mlp_tcgen05 (rr_gemm.cu): one TMA
-// producer warp, one MMA warp (tcgen05.mma, weights on the UMMA M side, the <= BN batch rows on the N side), four
-// epilogue warps.  The pipeline state carries from item to item and from phase to phase, so the weight stream never
+// Same warp roles and smem ring as gemm_bf16_wgmma / gemm_mlp_wgmma (rr_gemm.cu): one TMA producer warp, one consumer
+// warpgroup (wgmma with the weights on the M side and the <= BN batch rows on the N side, then the epilogue).  The pipeline state carries from item to item and from phase to phase, so the weight stream never
 // drains inside a layer: every CTA walks a host-built list (layer_schedule) and a phase boundary is a dependency
 // counter, not a kernel boundary; the weight tiles of an item's first stages are always requested BEFORE its
 // dependency is awaited.
@@ -21,8 +20,8 @@
 //   * O -> residual: the s_o split-K CTAs of a 128-feature tile (each the FIRST item of its CTA, so all are running)
 //     store their fp32 planes, meet on arr_o[tile], and each reduces rows/s_o of the batch rows: x += sum_z P_z in
 //     fixed order, writes x, xhat, rowss_a[row][tile]; then cnt_o++.  Gate/up items wait for cnt_o == #O items.
-//   * gate/up -> down: per K-slice counters exactly as in gemm_mlp_tcgen05 (ready_gu[slice] == tiles of the slice).
-//   * down -> residual: every (tile, K-slice) item stores its plane and bumps arr_d[tile]; REDUCE items (epilogue warps
+//   * gate/up -> down: per K-slice counters exactly as in gemm_mlp_wgmma (ready_gu[slice] == tiles of the slice).
+//   * down -> residual: every (tile, K-slice) item stores its plane and bumps arr_d[tile]; REDUCE items (consumer warps
 //     only, no MMA; tile x row group, placed after the down items in the lists) wait for arr_d[tile] == #slices and do
 //     the same fixed-order reduction into x, xhat, rowss_b; then cnt_d++.  (A first version added the slices into x in
 //     turn, slice after slice: 8 dependent store->flag->load hops per tile, 63 us per layer instead of 20.)
@@ -63,7 +62,7 @@ constexpr int layer_smem_bytes() { return gemm_smem_bytes<BN, OUT_TRANSPOSED_SIL
 
 template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
+decode_layer_wgmma(const __grid_constant__ LayerArgs a) {
     using Cfg = GemmCfg<BN>;
     constexpr int kStages = Cfg::kStages;
 
@@ -73,10 +72,8 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
     uint8_t* smemB = smem + kStages * Cfg::kStageBytesA;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tmem_full = empty_bar + kStages;
-    uint64_t* tmem_empty = tmem_full + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-    float* silu_stage = reinterpret_cast<float*>(smem + kStages * Cfg::kStageBytes + 256);
+    float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOff);
+    float* silu_stage = reinterpret_cast<float*>(smem + Cfg::kEpiOff);
     // Ring slots actually used (<= kStages).  Bytes in flight beyond bandwidth x latency only queue inside the memory system
     // and delay everything ELSE this SM asks for (dependency counters, reductions, epilogue stores): see DESIGN.md.
     const int depth = a.ring_depth;
@@ -86,25 +83,15 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
     griddep_launch();
     const int tr_slot = trace_begin(TR_GEMM_DEC);
 
-    if (warp == 0 && elect_one()) {
+    if (warp == PRODUCER_WARP && elect_one()) {
         for (int p = 0; p < 4; ++p) {
             tma_prefetch_desc(&a.tmA[p]);
             tma_prefetch_desc(&a.tmB[p]);
         }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], GEMM_CONSUMERS / 32); }
+        fence_barrier_init();
     }
-    if (warp == 1) {
-        if (elect_one()) {
-            for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-            for (int s = 0; s < 2; ++s) { mbar_init(&tmem_full[s], 1); mbar_init(&tmem_empty[s], 4); }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc<Cfg::kTmemCols>(tmem_ptr);
-    }
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     const int4* my = reinterpret_cast<const int4*>(a.items) + (size_t)blockIdx.x * a.max_items;   // constant data
     auto get = [&](int i, WorkItem& t, int& ph) -> bool {
@@ -124,7 +111,7 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
     WorkItem t;
     int ph = 0;
 
-    if (warp == 0) {
+    if (warp == PRODUCER_WARP) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             const uint64_t polA = l2_policy_evict_first(), polB = l2_policy_evict_last();
@@ -132,7 +119,7 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
             uint32_t phase = 0;
             bool first = true, o_seen = false, d_seen = false;
             for (int i = 0; get(i, t, ph); ++i) {
-                if (ph >= PH_RED_D) continue;                  // reduce items: epilogue warps only
+                if (ph >= PH_RED_D) continue;                  // reduce items: consumer warps only
                 const CUtensorMap* tA = &a.tmA[ph];
                 const CUtensorMap* tB = &a.tmB[ph];
                 const int nkb = t.kb1 - t.kb0;
@@ -183,48 +170,20 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
             }
             if (first) { griddep_wait(); trace_dep(tr_slot); }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = umma_idesc_bf16_f32(BLOCK_A, BN);
-            int stage = 0, it = 0;
-            uint32_t phase = 0;
-            for (int i = 0; get(i, t, ph); ++i) {
-                if (ph >= PH_RED_D) continue;
-                const int acc = it & 1;
-                mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);
-                tcgen05_fence_after();
-                const uint32_t tmem_d = tmem_base + acc * BN;
-                for (int kb = t.kb0; kb < t.kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tcgen05_fence_after();
-                    const uint64_t adesc = umma_desc_sw128_kmajor(smem_u32(smemA + stage * Cfg::kStageBytesA));
-                    const uint64_t bdesc = umma_desc_sw128_kmajor(smem_u32(smemB + stage * Cfg::kStageBytesB));
-#pragma unroll
-                    for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-                        umma_bf16_ss(tmem_d, adesc + 2 * k, bdesc + 2 * k, idesc, (kb > t.kb0 || k > 0) ? 1u : 0u);
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == depth) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tmem_full[acc]);
-                ++it;
-            }
-        }
     } else {
-        // ===================== epilogue (warps 2..5) =====================
-        const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-        const int wq = warp - 2;                      // 0..3
+        // ===================== consumer warpgroup: wgmma main loop + epilogue (warps 0..3) =====================
+        const int quarter = warp;                     // rows [32 quarter, 32 quarter + 32) of the tile in the epilogue
+        const int wq = warp;
         const int row_in_tile = quarter * 32 + lane;
-        const int etid = wq * 32 + lane;
+        const int etid = threadIdx.x;
+        const uint32_t smemA_u = smem_u32(smemA), smemB_u = smem_u32(smemB);
+        int stage = 0;
+        uint32_t phase = 0;
         const int rows = a.rows, hidden = a.hidden;
         int rinv_of = -1;                             // which r_b is staged in rinv_s: 1 = after O, 3 = after down
         griddep_wait();                               // outputs may still be read by the preceding kernel
+        trace_dep(tr_slot);
 
-        auto release_tmem = [&](int acc) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        };
         auto publish = [&](unsigned* ctr_add) {
             epi_bar();                                // every epilogue thread's stores
             if (etid == 0) {
@@ -252,13 +211,12 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
             if (etid == 0) trace_mark_cta(38);
         };
         // planes of this item: P[z][b][f] = acc[f][b]
-        auto store_plane = [&](float* planes, int z, uint32_t taddr0, int f) {
+        auto store_plane = [&](float* planes, int z, const float* arow, int f) {
             float* pl = planes + (size_t)z * a.ld_rows * hidden;
 #pragma unroll 1
             for (int c = 0; c < BN; c += 32) {
                 uint32_t v[32];
-                tmem_ld_32x32b_x32(taddr0 + c, v);
-                tmem_ld_wait();
+                acc_ld32(arow + c, v);
                 if (f < hidden) {
 #pragma unroll
                     for (int j = 0; j < 32; ++j)
@@ -327,7 +285,6 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
             }
         };
 
-        int it = 0;                                   // MMA items seen so far (TMEM buffer = it & 1)
         for (int i = 0; get(i, t, ph); ++i) {
             if (ph == PH_RED_D) {
                 // ---------------- reduce item: down planes of a tile complete -> residual rows [q R, (q + 1) R)
@@ -340,18 +297,18 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
                 if (etid == 0) trace_mark_cta(TR_LAYER_PH0 + 3);
                 continue;
             }
-            const int acc = it & 1;
-            mbar_wait(&tmem_full[acc], (it >> 1) & 1);
-            ++it;
-            tcgen05_fence_after();
+            float acc[2][BN / 2];
+            gmma_mainloop<BN>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, depth);
+            acc_bar();                                          // the previous item's epilogue is done with the staged tile
+            stage_acc<BN>(acc, acc_tile);
+            acc_bar();
             if (etid == 0) trace_mark_cta(20 + ph);            // accumulator of an item of phase ph complete
-            const int f = t.a_tile * BLOCK_A + row_in_tile;     // output feature of this thread (TMEM lane)
-            const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN;
+            const int f = t.a_tile * BLOCK_A + row_in_tile;     // output feature of this thread (accumulator row)
+            const float* arow = acc_tile + row_in_tile * Cfg::kAccPitch;
 
             if (ph == 0) {
                 // ---------------- O projection: planes, then the tile's split CTAs reduce the batch rows together
-                store_plane(a.part_o, t.z, taddr0, f);
-                release_tmem(acc);
+                store_plane(a.part_o, t.z, arow, f);
                 epi_bar();
                 if (etid == 0) {
                     trace_mark_cta(30);
@@ -369,15 +326,14 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
             } else if (ph == 1) {
                 // ---------------- gate/up: act[b][n] = silu(g r_b) * (u r_b); weights interleaved in 64-row gate/up blocks
                 if (rinv_of != 1) { stage_rinv(a.rowss_a, cnt_o, a.o_target); rinv_of = 1; }
-                const bool is_up = quarter >= 2;            // TMEM lanes 64..127 of the tile hold the up rows
+                const bool is_up = quarter >= 2;            // accumulator rows 64..127 of the tile hold the up rows
                 const int r64 = (quarter & 1) * 32 + lane;
                 const int n = t.a_tile * 64 + r64;
 #pragma unroll 1
                 for (int c = 0; c < BN; c += 32) {
                     float* buf = silu_stage + ((c >> 5) & 1) * (32 * 64);
                     uint32_t v[32];
-                    tmem_ld_32x32b_x32(taddr0 + c, v);
-                    tmem_ld_wait();
+                    acc_ld32(arow + c, v);
                     if (is_up) {
 #pragma unroll
                         for (int j = 0; j < 32; ++j) buf[j * 64 + r64] = __uint_as_float(v[j]);
@@ -395,12 +351,10 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
                         }
                     }
                 }
-                release_tmem(acc);
                 publish(ready_gu + t.a_tile / a.slice_kb);
             } else if (ph == 2) {
                 // ---------------- down: plane of this K-slice; the tile's reduce items wait for all of them
-                store_plane(a.part_d, t.z, taddr0, f);
-                release_tmem(acc);
+                store_plane(a.part_d, t.z, arow, f);
                 publish(arr_d + t.a_tile);
             } else {
                 // ---------------- next projection (QKV of the next layer / lm_head): planes scaled by r_b
@@ -409,27 +363,20 @@ decode_layer_tcgen05(const __grid_constant__ LayerArgs a) {
 #pragma unroll 1
                 for (int c = 0; c < BN; c += 32) {
                     uint32_t v[32];
-                    tmem_ld_32x32b_x32(taddr0 + c, v);
-                    tmem_ld_wait();
+                    acc_ld32(arow + c, v);
                     if (f < a.rowsA3) {
 #pragma unroll
                         for (int j = 0; j < 32; ++j)
                             if (c + j < rows) pl[(size_t)(c + j) * a.ldo3 + f] = __uint_as_float(v[j]) * rinv_s[c + j];
                     }
                 }
-                release_tmem(acc);
             }
             if (etid == 0) trace_mark_cta(TR_LAYER_PH0 + (ph == 3 ? 4 : ph));      // debug timeline: item finished on this CTA
         }
     }
 
-    tcgen05_fence_before();
     __syncthreads();
     trace_end(tr_slot);
-    if (warp == 1) {
-        tcgen05_fence_after();
-        tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-    }
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
@@ -510,7 +457,7 @@ int layer_counter_words(const LayerShape& s) {
 int layer_plan_init(LayerPlan* p, const LayerShape& s, const LayerBuffers& b, int bn, const MlpItem* items_dev,
                     int max_items, int grid, unsigned* ctr) {
     if (!p || !items_dev || !ctr || !b.x || !b.xhat || !b.rowss_b) return RR_ERR_ARG;
-    if (s.hidden % 64 || b.rows > bn || bn < 32 || grid < 1 || grid > num_sms()) return RR_ERR_ARG;
+    if (s.hidden % 64 || b.rows > bn || bn < 32 || bn > MAX_BN || grid < 1 || grid > num_sms()) return RR_ERR_ARG;
     LayerArgs& a = p->args;
     memset(&a, 0, sizeof(a));
     const int tiles_h = (s.hidden + BLOCK_A - 1) / BLOCK_A;
@@ -560,7 +507,7 @@ int layer_plan_init(LayerPlan* p, const LayerShape& s, const LayerBuffers& b, in
 
 template <int BN>
 static int launch_layer_bn(const LayerPlan& p, cudaStream_t st) {
-    auto kern = decode_layer_tcgen05<BN>;
+    auto kern = decode_layer_wgmma<BN>;
     static std::atomic<uint64_t> attr_set{0};
     if (ensure_dyn_smem(kern, layer_smem_bytes<BN>(), attr_set) != cudaSuccess) return RR_ERR_CUDA;
     LayerArgs args = p.args;
@@ -574,7 +521,6 @@ int layer_launch(const LayerPlan& p, cudaStream_t st) {
         case 32: return launch_layer_bn<32>(p, st);
         case 64: return launch_layer_bn<64>(p, st);
         case 128: return launch_layer_bn<128>(p, st);
-        case 256: return launch_layer_bn<256>(p, st);
     }
     return RR_ERR_ARG;
 }

@@ -57,7 +57,7 @@ def test_tokenizer_counts():
 
 def test_version_and_errors():
     from rr_b200 import _lib
-    assert b"sm_100a" in _lib.lib.rr_version()
+    assert b"sm_90a" in _lib.lib.rr_version()
     assert b"429" in _lib.lib.rr_strerror(1)
 
 

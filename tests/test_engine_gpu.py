@@ -61,7 +61,7 @@ def test_engine_matches_hf_golden_tiny():
 
 def test_engine_matches_hf_mistral_and_phi3_golden():
     """Engine logits against the REAL transformers MistralForCausalLM / Phi3ForCausalLM outputs committed in
-    tests/golden/family_golden.pt (no oracle in between): GQA group size 2 on the tcgen05 attention path, and
+    tests/golden/family_golden.pt (no oracle in between): GQA group size 2 on the wgmma attention path, and
     MHA with head_dim 96 on the mma.sync path with the fused-projection layout HF Phi-3 uses."""
     from test_oracle_llama import family_cases          # tests/ is on sys.path (pytest rootdir/conftest)
     from rr_b200.engine import Engine
@@ -334,7 +334,7 @@ def test_generation_up_to_the_last_kv_slot_and_argument_bounds():
 
 
 def test_long_prompts_match_oracle():
-    """3000- and 1500-token prompts in one prefill chunk (47 / 24 key tiles per query tile in the tcgen05 attention
+    """3000- and 1500-token prompts in one prefill chunk (47 / 24 key tiles per query tile in the wgmma attention
     kernel, deep online-softmax chains), then decode steps at context ~3000 (47 K/V tiles per row in the decode
     attention kernel)."""
     from oracle import llama_ref

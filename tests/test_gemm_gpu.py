@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 GEMM (rr_gemm_bf16) against a torch fp32 reference of the same op.
+"""Parity of the wgmma GEMM (rr_gemm_bf16) against a torch fp32 reference of the same op.
 Tolerance: bf16 inputs are exact in both; fp32 accumulation order differs -> |err| <= 2e-3 * sqrt(K)
 relative to |a||b| scale for fp32 out, plus one bf16 rounding (2^-8 relative) for bf16 out."""
 import ctypes as C
@@ -68,7 +68,7 @@ def test_decode_gemm_tma_store_epilogue_equals_lsu_epilogue_and_clips(rowsA, row
 
 CASES_R = [(128, 256, 64, 256), (512, 6144, 4096, 256), (1000, 520, 256, 128), (2048, 4096, 4096, 256),
            (130, 72, 128, 64), (4096, 28672, 4096, 256),
-           # ragged shapes through the 2-CTA pair kernel (rowsA >= 256, bn 256): partial pair tiles on both axes
+           # ragged shapes with bn 256 (run as 128-wide tiles): partial tiles on both axes
            (1000, 520, 256, 256), (300, 304, 192, 256), (257, 8200, 64, 256), (8192, 1024, 4096, 256)]
 
 

@@ -191,9 +191,9 @@ def test_prefill_attention_causal_ragged(H, KV):
 
 
 def test_prefill_attention_rising_scores_rescale_path():
-    """tcgen05 prefill attention keeps O in TMEM and only raises a row's exponent reference when its running max
-    moved by more than 2^8; random scores never do.  Here every 64-key tile beats the previous one by > 2^8
-    (log2 domain), so every tile after the first takes the rescale path (TMEM ld / multiply / st of O)."""
+    """Online softmax of the prefill attention under rising scores: every 64-key tile beats the previous one by > 2^8
+    (log2 domain), so every tile after the first rescales O and the row sum by a tiny factor; random scores barely
+    exercise that path."""
     lib = L()
     H, KV, ctx_max, slots = 8, 2, 640, 3
     lens = [512, 300, 129]

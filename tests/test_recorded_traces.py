@@ -1,4 +1,4 @@
-"""CPU: admission traces recorded ON THE B200 by `bench.py --config quota|fallback|fleet --trace-out ...` (the events the
+"""CPU: admission traces recorded at full size by `bench.py --config quota|fallback|fleet --trace-out ...` (the events the
 native gateway fed to the K1 router kernel at BASELINE.json's full sizes, with the decisions the kernel returned) replayed
 through the CPU oracle (oracle/router.py): every decision must be bit-exact.  This is the full-size half of the router
 parity statement; the seeded random-trace matrix is tests/test_router_gpu.py.  Fixtures: tests/golden/trace_*.json

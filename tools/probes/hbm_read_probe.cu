@@ -3,7 +3,7 @@
 //   (b) TMA 2-D boxes of 128 rows x 128 B out of a [N, K] bf16 matrix     (what the decode GEMMs request today)
 //   (c) TMA 2-D boxes of the same 16 KB out of a pre-tiled [N*K/64, 64] matrix = one contiguous 16 KB block
 // (b)/(c): one elected thread per CTA keeps DEPTH boxes in flight and recycles a slot as soon as it lands.
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o build/hbm_read_probe tools/probes/hbm_read_probe.cu
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/hbm_read_probe tools/probes/hbm_read_probe.cu
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -210,7 +210,7 @@ int main() {
         const int tiles = (int)(rows / 128) / 4, kblocks = (int)(Kv / 64);
         const double b = (double)tiles * kblocks * 16384;
         CUtensorMap strided = mk(enc, buf, rows, Kv, 1);
-        for (int g : {32, 76, 96, 148}) {
+        for (int g : {32, 66, 96, 132}) {
             float d6 = run_tma<6>(strided, tiles, kblocks, 0, g, 3), d8 = run_tma<8>(strided, tiles, kblocks, 0, g, 3),
                   d10 = run_tma<10>(strided, tiles, kblocks, 0, g, 3), d12 = run_tma<12>(strided, tiles, kblocks, 0, g, 3);
             printf("%3d CTAs: ring 6 %5.1f  ring 8 %5.1f  ring 10 %5.1f  ring 12 %5.1f GB/s per SM\n", g, b / d6 / 1e6 / g, b / d8 / 1e6 / g,

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Evidence run for profiles/ (one B200, under gpurun): ncu launch list of one prefill chunk + two decode steps, ncu --set full
+# Evidence run for profiles/ (one GPU): ncu launch list of one prefill chunk + two decode steps, ncu --set full
 # captures of every kernel of a decode step and of one prefill layer (final code), compute-sanitizer logs.
 # Numbers printed by the profiled programs are NOT bench values.
 set -u

@@ -22,7 +22,7 @@ def demangle(n):
     r = subprocess.run(["c++filt", n], capture_output=True, text=True).stdout.strip()
     r = r.replace("(anonymous namespace)::", "")
     return re.sub(r"\(.*", "", r)[:110]
-print(f"# {os.path.relpath(lib, ROOT)}: {len(hist)} kernels (sm_100a SASS); columns = instruction counts")
+print(f"# {os.path.relpath(lib, ROOT)}: {len(hist)} kernels (sm_90a SASS); columns = instruction counts")
 for k, h in hist.items():
     tot = sum(v for o, v in h.items() if "." not in o)
     keys = [(o, h[o]) for o in KEY if h.get(o)]

@@ -6,7 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from tools.gemm_probe import time_gemm
 for K in (4096, 14336):
-    for n_tiles in (16, 32, 64, 96, 128, 148):
+    for n_tiles in (16, 32, 64, 96, 128, 132):
         N = n_tiles * 128
         nc = max(2, int(300e6 / (N * K * 2)) + 1)
         ms = time_gemm(N, 64, K, 1, 64, 1, iters=20, ncopies=min(nc, 24))

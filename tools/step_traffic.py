@@ -24,7 +24,7 @@ s = m.SPECS["llama-3-8b"]
 alg = s.weight_bytes_per_decode_step + rows * ctx * s.kv_bytes_per_token
 out = {"model": "llama-3-8b", "rows": rows, "prompt_len": prompt_len, "ctx": ctx, "dram_bytes_per_step": int(total),
        "algorithmic_bytes_same_ctx": int(alg),
-       "source": "ncu --set full --clock-control none over one eager decode step of the final code (tools/profile_r02.sh, 1 x B200): sum over "
+       "source": "ncu --set full --clock-control none over one eager decode step of the final code (tools/profile_r02.sh): sum over "
                  "the step's 196 kernels of dram__bytes_read.sum + dram__bytes_write.sum (layer 0's six kernels x 32 + embed, first norm, "
                  "lm_head, argmax); profiles/r02_ncu_full_summary.txt; tools/step_traffic.py.  ncu flushes the caches between kernels, so the "
                  "small consumers (norm planes, logits for argmax) show DRAM reads that are L2 hits inside the real step: an upper bound.",
