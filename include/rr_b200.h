@@ -179,12 +179,13 @@ enum { RR_OUT_ROWMAJOR_BF16 = 0, RR_OUT_TRANSPOSED_F32 = 1,
        RR_OUT_TRANSPOSED_SILU = 2,   /* decode: A = interleaved weight [2*inter, K], out[b*ldo + n], splits = 1 */
        RR_OUT_ROWMAJOR_SILU = 3,     /* prefill: B = interleaved weight, bn >= 128, out[a*ldo + n] */
        RR_OUT_ROWMAJOR_ROPE = 4,     /* engine-internal (prefill QKV epilogue with RoPE + KV scatter) */
-       RR_OUT_ROWMAJOR_RESID = 5 };  /* out = fp32 residual [rowsA, ldo]: out[a*ldo + b] += acc (bn >= 128) */
+       RR_OUT_ROWMAJOR_RESID = 5 };  /* out = fp32 residual [rowsA, ldo]: out[a*ldo + b] += acc (bn >= 32) */
 
 /* D[a,b] = sum_k A[a,k] B[b,k] on wgmma tensor cores (bf16 in, fp32 accumulate).
  * mode RR_OUT_ROWMAJOR_BF16:  out bf16 [rowsA, ldo], out[a*ldo + b]         (splits must be 1)
  * mode RR_OUT_TRANSPOSED_F32: out fp32 [splits, ld_rows, ldo], out[(z*ld_rows + b)*ldo + a]
- * bn = tile width along B rows: 16/32/64/128 (256 is accepted and runs 128-wide tiles).  splits >= 1. */
+ * bn = tile width along B rows of the transposed modes: 16/32/64/128 (256 is accepted and runs 128-wide tiles).  The
+ * row-major modes always run 128 x 256 tiles; their bn is only validated.  splits >= 1. */
 int rr_gemm_bf16(const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
                  void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream);
 

@@ -195,7 +195,8 @@ static int dalloc(rr_engine* e, T** p, size_t n, bool zero = true) {
     return RR_OK;
 }
 
-// Prefill GEMM tile width: the widest accumulator tile one consumer warpgroup holds in registers (rr_gemm_dev.cuh).
+// Column block of the prefill deferred-norm partial sums (pf_parts = hidden / PF_BN): the residual GEMM epilogue writes one
+// sum(x^2) partial per 128 columns, two per 256-wide tile.
 constexpr int PF_BN = MAX_BN;
 
 // Decode tile width along the batch rows; batches wider than MAX_BN run several B tiles per weight tile.

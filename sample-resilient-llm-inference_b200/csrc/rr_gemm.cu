@@ -1,13 +1,15 @@
 // rr_gemm.cu — the path's one dense contraction (QKV / O / gate-up / down / lm_head projections)
 // on Hopper tensor cores: wgmma (m64nNk16, bf16 in, fp32 accumulators in registers), operands staged by TMA
-// into 128B-swizzled shared memory, persistent warp-specialised CTAs (1 TMA producer warp, 1 consumer
-// warpgroup that issues the wgmma and runs the epilogue from the accumulators staged in shared memory).
+// into 128B-swizzled shared memory, persistent warp-specialised CTAs.
 //
 //   D[a, b] = sum_k A[a, k] * B[b, k]          A: [rowsA, K] bf16, B: [rowsB, K] bf16 (both K-major)
 //
-// Two orientations of the same kernel:
-//   * prefill  (OUT_ROWMAJOR_BF16):  A = activations [T, K], B = weight [N, K]  -> C[T, N] bf16
-//   * decode   (OUT_TRANSPOSED_F32): A = weight [N, K] (wgmma M side, streamed once from HBM),
+// Two orientations, two kernels:
+//   * prefill  (OUT_ROWMAJOR_*, gemm_pf_wgmma): A = activations [T, K], B = weight [N, K] -> C[T, N] row-major; 128 x 256
+//     tiles on two consumer warpgroups, epilogues straight from the accumulator registers
+//   * decode   (OUT_TRANSPOSED_*, gemm_bf16_wgmma and the fused MLP kernel): 1 TMA producer warp, 1 consumer warpgroup that
+//     issues the wgmma and runs the epilogue from the accumulators staged in shared memory;
+//                                    A = weight [N, K] (wgmma M side, streamed once from HBM),
 //                                    B = activations [batch<=BN, K]; fp32 partial planes
 //                                    P[z][b][n] reduced by the consumer kernel (rr_elementwise.cu).
 //     Work split for decode: uniform split-K (splits planes); the wave-quantisation tail of the big gate/up
@@ -32,18 +34,8 @@ namespace rr {
 template <int BN, int MODE>
 __device__ __forceinline__ void epilogue_item(const float* arow, int a_row, const WorkItem& t, int quarter, int lane,
                                               void* __restrict__ out, int rowsA, int rowsB, int ldo, int ld_rows,
-                                              const RopeEpi& rope, float* silu_stage) {
+                                              float* silu_stage) {
     constexpr int CH = (BN >= 32) ? 32 : 16;
-    // deferred RMSNorm, consumer side: this thread's row of the A operand was bf16(x * gamma); scale by 1 / rms(x)
-    float rinv = 1.f;
-    if constexpr (MODE == OUT_ROWMAJOR_ROPE || MODE == OUT_ROWMAJOR_SILU || MODE == OUT_ROWMAJOR_BF16) {
-        if (rope.n_part > 0 && a_row < rowsA) {
-            const float* ps = rope.rowss + (size_t)a_row * rope.n_part;
-            float ss = 0.f;
-            for (int j = 0; j < rope.n_part; ++j) ss += ps[j];
-            rinv = rsqrtf(ss * rope.inv_hidden + rope.eps);
-        }
-    }
     if constexpr (MODE == OUT_TRANSPOSED_SILU) {
         // gate/up rows are interleaved in blocks of 64: lanes 0..63 of the tile hold gate rows, lanes 64..127 the
         // matching up rows.  The up warps hand their values over through smem ([col][row] -> conflict-free), the
@@ -73,249 +65,6 @@ __device__ __forceinline__ void epilogue_item(const float* arow, int a_row, cons
                 }
             }
         }
-    } else if constexpr (MODE == OUT_ROWMAJOR_ROPE) {
-        // BN / 128 heads of 128 columns of the fused qkv projection; thread = token row.
-        const bool row_ok = a_row < rowsA;
-        const int slot = row_ok ? rope.slot[a_row] : -1;
-        const int pos = row_ok ? rope.pos[a_row] : 0;
-        const bool live = slot >= 0;
-        const float2* tab = rope.table + (size_t)pos * 64;
-#pragma unroll 1
-        for (int hb = 0; hb < BN / 128; ++hb) {
-            const int H = t.b_tile * (BN / 128) + hb;                  // head index in [q heads | k heads | v heads]
-            if (H * 128 >= rowsB) break;
-            const float* tcol = arow + hb * 128;
-            if (H < rope.n_heads + rope.n_kv_heads) {
-                __nv_bfloat16* dst = H < rope.n_heads
-                    ? rope.q_out + (size_t)a_row * (rope.n_heads * 128) + H * 128
-                    : rope.k_cache + (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads)) * rope.ctx_max + pos) * 128;
-#pragma unroll 1
-                for (int c = 0; c < 64; c += 32) {
-                    uint32_t lo[32], hi[32];
-                    acc_ld32(tcol + c, lo);
-                    acc_ld32(tcol + 64 + c, hi);
-                    if (live) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 8) {
-                            uint4 plo, phi;
-                            uint32_t* wl = reinterpret_cast<uint32_t*>(&plo);
-                            uint32_t* wh = reinterpret_cast<uint32_t*>(&phi);
-#pragma unroll
-                            for (int q = 0; q < 4; ++q) {
-                                const float4 cs = *reinterpret_cast<const float4*>(tab + c + j + 2 * q);   // 2 pairs
-                                const float l0 = __uint_as_float(lo[j + 2 * q]) * rinv, l1 = __uint_as_float(lo[j + 2 * q + 1]) * rinv;
-                                const float h0 = __uint_as_float(hi[j + 2 * q]) * rinv, h1 = __uint_as_float(hi[j + 2 * q + 1]) * rinv;
-                                wl[q] = pack_bf16(l0 * cs.x - h0 * cs.y, l1 * cs.z - h1 * cs.w);
-                                wh[q] = pack_bf16(h0 * cs.x + l0 * cs.y, h1 * cs.z + l1 * cs.w);
-                            }
-                            *reinterpret_cast<uint4*>(dst + c + j) = plo;
-                            *reinterpret_cast<uint4*>(dst + 64 + c + j) = phi;
-                        }
-                    }
-                }
-            } else {
-                __nv_bfloat16* dst = rope.v_cache +
-                    (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads - rope.n_kv_heads)) * rope.ctx_max + pos) * 128;
-#pragma unroll 1
-                for (int c = 0; c < 128; c += 32) {
-                    uint32_t v[32];
-                    acc_ld32(tcol + c, v);
-                    if (live) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 8) {
-                            uint4 pk;
-                            pk.x = pack_bf16(__uint_as_float(v[j + 0]) * rinv, __uint_as_float(v[j + 1]) * rinv);
-                            pk.y = pack_bf16(__uint_as_float(v[j + 2]) * rinv, __uint_as_float(v[j + 3]) * rinv);
-                            pk.z = pack_bf16(__uint_as_float(v[j + 4]) * rinv, __uint_as_float(v[j + 5]) * rinv);
-                            pk.w = pack_bf16(__uint_as_float(v[j + 6]) * rinv, __uint_as_float(v[j + 7]) * rinv);
-                            *reinterpret_cast<uint4*>(dst + c + j) = pk;
-                        }
-                    }
-                }
-            }
-        }
-    } else if constexpr (MODE == OUT_ROWMAJOR_RESID) {
-        float* xres = reinterpret_cast<float*>(out);
-        const bool defer = rope.xhat != nullptr;       // also emit bf16(x * gamma) and sum(x^2) of this row over the tile
-        if (silu_stage != nullptr) {
-            // Coalesced residual add.  The staged tile hands every thread one ROW (32 consecutive columns = one 128-byte line per
-            // chunk), so a direct read-modify-write issues 16-byte pieces of 32 different lines per instruction: 32 LSU
-            // wavefronts and half-used sectors.  Each warp instead transposes its 32 x 32 chunk through 4.5 KB of shared
-            // memory (row pitch 36 floats: conflict-free both ways) and lets 8 lanes cover one line: 4 full lines per
-            // instruction.
-            float* stg = silu_stage + (quarter * 32) * 36;              // this warp's [32][36] tile
-            const int sub_row = lane >> 3, sub_col = (lane & 7) * 4;
-            const int row0 = t.a_tile * BLOCK_A + quarter * 32;         // first of this warp's 32 rows
-            float ssr[8];                                               // deferred norm: sum(x^2) pieces of rows 4i + sub_row
-#pragma unroll
-            for (int i = 0; i < 8; ++i) ssr[i] = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < BN; c += 32) {
-                uint32_t v[32];
-                acc_ld32(arow + c, v);
-                const int b0 = t.b_tile * BN + c;
-                if (b0 + 32 <= rowsB) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4)
-                        *reinterpret_cast<float4*>(stg + lane * 36 + j) =
-                            make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                    __syncwarp();
-                    // all eight loads first: a store between them would fence the later loads (possible aliasing) and
-                    // turn eight independent L2 round trips into a chain
-                    float4 xs[8];
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int r = 4 * i + sub_row;
-                        xs[i] = (row0 + r < rowsA) ? *reinterpret_cast<const float4*>(xres + (size_t)(row0 + r) * ldo + b0 + sub_col)
-                                                   : make_float4(0.f, 0.f, 0.f, 0.f);
-                    }
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const int r = 4 * i + sub_row;
-                        if (row0 + r < rowsA) {
-                            const float4 a4 = *reinterpret_cast<const float4*>(stg + r * 36 + sub_col);
-                            float4 x4 = xs[i];
-                            x4.x += a4.x; x4.y += a4.y; x4.z += a4.z; x4.w += a4.w;
-                            *reinterpret_cast<float4*>(xres + (size_t)(row0 + r) * ldo + b0 + sub_col) = x4;
-                            if (defer) {
-                                const uint2 gw = *reinterpret_cast<const uint2*>(rope.gamma + b0 + sub_col);
-                                ssr[i] += x4.x * x4.x + x4.y * x4.y + x4.z * x4.z + x4.w * x4.w;
-                                uint2 pk;
-                                pk.x = pack_bf16(x4.x * bf16_lo(gw.x), x4.y * bf16_hi(gw.x));
-                                pk.y = pack_bf16(x4.z * bf16_lo(gw.y), x4.w * bf16_hi(gw.y));
-                                *reinterpret_cast<uint2*>(rope.xhat + (size_t)(row0 + r) * ldo + b0 + sub_col) = pk;
-                            }
-                        }
-                    }
-                    __syncwarp();
-                } else {
-                    // ragged last chunk: thread = row, scalar; its sum(x^2) joins the row's lane group through smem
-                    float ss_tail = 0.f;
-                    if (a_row < rowsA) {
-                        float* dst = xres + (size_t)a_row * ldo + b0;
-                        for (int j = 0; j < 32; ++j)
-                            if (b0 + j < rowsB) {
-                                const float xv = dst[j] + __uint_as_float(v[j]);
-                                dst[j] = xv;
-                                if (defer) {
-                                    ss_tail += xv * xv;
-                                    rope.xhat[(size_t)a_row * ldo + b0 + j] = __float2bfloat16(xv * __bfloat162float(rope.gamma[b0 + j]));
-                                }
-                            }
-                    }
-                    if (defer) {
-                        stg[lane * 36] = ss_tail;                     // row `lane` of this warp
-                        __syncwarp();
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            if ((lane & 7) == 0) ssr[i] += stg[(4 * i + sub_row) * 36];
-                        __syncwarp();
-                    }
-                }
-            }
-            if (defer) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    float v2 = ssr[i];
-                    v2 += __shfl_xor_sync(0xffffffffu, v2, 1);
-                    v2 += __shfl_xor_sync(0xffffffffu, v2, 2);
-                    v2 += __shfl_xor_sync(0xffffffffu, v2, 4);
-                    const int r = row0 + 4 * i + sub_row;
-                    if ((lane & 7) == 0 && r < rowsA) rope.rowss_out[(size_t)r * rope.n_part_out + t.b_tile] = v2;
-                }
-            }
-        } else {
-            float ss = 0.f;
-    #pragma unroll 1
-            for (int c = 0; c < BN; c += 32) {
-                uint32_t v[32];
-                acc_ld32(arow + c, v);
-                const int b0 = t.b_tile * BN + c;
-                if (a_row < rowsA) {
-                    float* dst = xres + (size_t)a_row * ldo + b0;
-                    if (b0 + 32 <= rowsB) {
-                        __nv_bfloat16* hdst = defer ? rope.xhat + (size_t)a_row * ldo + b0 : nullptr;
-    #pragma unroll
-                        for (int j = 0; j < 32; j += 8) {
-                            float4 x4 = *reinterpret_cast<const float4*>(dst + j);
-                            float4 y4 = *reinterpret_cast<const float4*>(dst + j + 4);
-                            x4.x += __uint_as_float(v[j + 0]); x4.y += __uint_as_float(v[j + 1]);
-                            x4.z += __uint_as_float(v[j + 2]); x4.w += __uint_as_float(v[j + 3]);
-                            y4.x += __uint_as_float(v[j + 4]); y4.y += __uint_as_float(v[j + 5]);
-                            y4.z += __uint_as_float(v[j + 6]); y4.w += __uint_as_float(v[j + 7]);
-                            *reinterpret_cast<float4*>(dst + j) = x4;
-                            *reinterpret_cast<float4*>(dst + j + 4) = y4;
-                            if (defer) {
-                                const uint4 gw = *reinterpret_cast<const uint4*>(rope.gamma + b0 + j);
-                                ss += x4.x * x4.x + x4.y * x4.y + x4.z * x4.z + x4.w * x4.w
-                                    + y4.x * y4.x + y4.y * y4.y + y4.z * y4.z + y4.w * y4.w;
-                                uint4 pk;
-                                pk.x = pack_bf16(x4.x * bf16_lo(gw.x), x4.y * bf16_hi(gw.x));
-                                pk.y = pack_bf16(x4.z * bf16_lo(gw.y), x4.w * bf16_hi(gw.y));
-                                pk.z = pack_bf16(y4.x * bf16_lo(gw.z), y4.y * bf16_hi(gw.z));
-                                pk.w = pack_bf16(y4.z * bf16_lo(gw.w), y4.w * bf16_hi(gw.w));
-                                *reinterpret_cast<uint4*>(hdst + j) = pk;
-                            }
-                        }
-                    } else {
-                        for (int j = 0; j < 32; ++j)
-                            if (b0 + j < rowsB) {
-                                const float xv = dst[j] + __uint_as_float(v[j]);
-                                dst[j] = xv;
-                                if (defer) {
-                                    ss += xv * xv;
-                                    rope.xhat[(size_t)a_row * ldo + b0 + j] = __float2bfloat16(xv * __bfloat162float(rope.gamma[b0 + j]));
-                                }
-                            }
-                    }
-                }
-            }
-            if (defer && a_row < rowsA) rope.rowss_out[(size_t)a_row * rope.n_part_out + t.b_tile] = ss;
-        }
-    } else if constexpr (MODE == OUT_ROWMAJOR_SILU) {
-        // weight rows interleaved [gate 64 | up 64 | ...] (BN / 128 pairs per tile): a token's gate and up values sit in the same
-        // accumulator row, so silu(g) * u needs no exchange; 128 output columns per tile, ldo = inter.
-        __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(out);
-        const int n_out = rowsB >> 1;
-#pragma unroll 1
-        for (int hb = 0; hb < BN / 128; ++hb) {
-#pragma unroll 1
-            for (int c = 0; c < 64; c += 32) {
-                uint32_t vg[32], vu[32];
-                acc_ld32(arow + hb * 128 + c, vg);
-                acc_ld32(arow + hb * 128 + 64 + c, vu);
-                if (rope.n_part > 0) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        vg[j] = __float_as_uint(__uint_as_float(vg[j]) * rinv);
-                        vu[j] = __float_as_uint(__uint_as_float(vu[j]) * rinv);
-                    }
-                }
-                const int col = t.b_tile * (BN / 2) + hb * 64 + c;
-                if (a_row < rowsA) {
-                    __nv_bfloat16* dst = act + (size_t)a_row * ldo + col;
-                    if (col + 32 <= n_out) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 8) {
-                            uint4 pk;
-                            pk.x = pack_bf16(silu_mul(__uint_as_float(vg[j + 0]), __uint_as_float(vu[j + 0])),
-                                             silu_mul(__uint_as_float(vg[j + 1]), __uint_as_float(vu[j + 1])));
-                            pk.y = pack_bf16(silu_mul(__uint_as_float(vg[j + 2]), __uint_as_float(vu[j + 2])),
-                                             silu_mul(__uint_as_float(vg[j + 3]), __uint_as_float(vu[j + 3])));
-                            pk.z = pack_bf16(silu_mul(__uint_as_float(vg[j + 4]), __uint_as_float(vu[j + 4])),
-                                             silu_mul(__uint_as_float(vg[j + 5]), __uint_as_float(vu[j + 5])));
-                            pk.w = pack_bf16(silu_mul(__uint_as_float(vg[j + 6]), __uint_as_float(vu[j + 6])),
-                                             silu_mul(__uint_as_float(vg[j + 7]), __uint_as_float(vu[j + 7])));
-                            *reinterpret_cast<uint4*>(dst + j) = pk;
-                        }
-                    } else {
-                        for (int j = 0; j < 32; ++j)
-                            if (col + j < n_out)
-                                dst[j] = __float2bfloat16(silu_mul(__uint_as_float(vg[j]), __uint_as_float(vu[j])));
-                    }
-                }
-            }
-        }
     } else {
 #pragma unroll 1
     for (int c = 0; c < BN; c += CH) {
@@ -329,38 +78,13 @@ __device__ __forceinline__ void epilogue_item(const float* arow, int a_row, cons
             for (int j = 0; j < 16; ++j) v[j] = v16[j];
         }
         const int b0 = t.b_tile * BN + c;
-        if constexpr (MODE == OUT_ROWMAJOR_BF16) {
-            if (rope.n_part > 0) {
+        float* dst = reinterpret_cast<float*>(out);
+        if (a_row < rowsA) {
 #pragma unroll
-                for (int j = 0; j < CH; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) * rinv);
-            }
-            if (a_row < rowsA) {
-                __nv_bfloat16* dst =
-                    reinterpret_cast<__nv_bfloat16*>(out) + (size_t)a_row * ldo + b0;
-                if (b0 + CH <= rowsB) {
-#pragma unroll
-                    for (int j = 0; j < CH; j += 8) {
-                        uint4 pk;
-                        pk.x = pack_bf16(__uint_as_float(v[j + 0]), __uint_as_float(v[j + 1]));
-                        pk.y = pack_bf16(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-                        pk.z = pack_bf16(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
-                        pk.w = pack_bf16(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-                        *reinterpret_cast<uint4*>(dst + j) = pk;
-                    }
-                } else {
-                    for (int j = 0; j < CH; ++j)
-                        if (b0 + j < rowsB) dst[j] = __float2bfloat16(__uint_as_float(v[j]));
-                }
-            }
-        } else {
-            float* dst = reinterpret_cast<float*>(out);
-            if (a_row < rowsA) {
-#pragma unroll
-                for (int j = 0; j < CH; ++j) {
-                    const int b = b0 + j;
-                    if (b < rowsB)
-                        dst[((size_t)t.z * ld_rows + b) * ldo + a_row] = __uint_as_float(v[j]);
-                }
+            for (int j = 0; j < CH; ++j) {
+                const int b = b0 + j;
+                if (b < rowsB)
+                    dst[((size_t)t.z * ld_rows + b) * ldo + a_row] = __uint_as_float(v[j]);
             }
         }
     }
@@ -455,7 +179,7 @@ template <int BN, int MODE, int CAP = 8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 void* __restrict__ out, int rowsA, int rowsB, int K, int splits, int ldo,
-                int ld_rows, const RopeEpi rope, const __grid_constant__ CUtensorMap tmOut, int tma_epi) {
+                int ld_rows, const __grid_constant__ CUtensorMap tmOut, int tma_epi) {
     using Cfg = GemmCfg<BN, CAP>;
     constexpr int kStages = Cfg::kStages;
 
@@ -470,7 +194,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     griddep_launch();   // PDL: the next kernel may start its prologue now
-    const int tr_slot = trace_begin(decode_orient<MODE>() ? TR_GEMM_DEC : TR_GEMM_PF);
+    const int tr_slot = trace_begin(TR_GEMM_DEC);
 
     if (warp == PRODUCER_WARP && elect_one()) {
         tma_prefetch_desc(&tmA);
@@ -487,15 +211,14 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     sched.init(rowsA, rowsB, K, splits, BN);
     WorkItem t;
     // detail trace of a plain decode projection: selected by its split-K factor (rr_debug_trace_detail(10 + splits)), CTAs 0 / 37 / 74 / 111
-    const int tsm = (decode_orient<MODE>() && rr_trace_detail == 10 + splits && blockIdx.x % 37 == 0) ? 8 + (int)(blockIdx.x / 37) : -1;
+    const int tsm = (rr_trace_detail == 10 + splits && blockIdx.x % 37 == 0) ? 8 + (int)(blockIdx.x / 37) : -1;
 
     if (warp == PRODUCER_WARP) {
         // ===================== TMA producer =====================
         if (elect_one()) {
             // Streamed-once operand (decode weights) should not displace the KV cache in L2;
             // the small re-read operand is kept.
-            const uint64_t polA = decode_orient<MODE>() ? l2_policy_evict_first()
-                                                               : l2_policy_evict_last();
+            const uint64_t polA = l2_policy_evict_first();
             const uint64_t polB = l2_policy_evict_last();
             int stage = 0;
             uint32_t phase = 0;
@@ -507,26 +230,17 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 pre = min(kStages, t.kb1 - t.kb0);
                 for (int i = 0; i < pre; ++i) {
                     mbar_arrive_expect_tx(&full_bar[i], Cfg::kStageBytes);
-                    if (decode_orient<MODE>())
-                        tma_load_2d_hint(smemA + i * Cfg::kStageBytesA, &tmA, &full_bar[i], (t.kb0 + i) * BLOCK_K,
-                                         t.a_tile * BLOCK_A, polA);
-                    else
-                        tma_load_2d_hint(smemB + i * Cfg::kStageBytesB, &tmB, &full_bar[i], (t.kb0 + i) * BLOCK_K,
-                                         t.b_tile * BN, polB);
+                    tma_load_2d_hint(smemA + i * Cfg::kStageBytesA, &tmA, &full_bar[i], (t.kb0 + i) * BLOCK_K,
+                                     t.a_tile * BLOCK_A, polA);
                 }
             }
             griddep_wait();
             trace_dep(tr_slot);
             if (tsm >= 0) trace_mark_at(TR_GEMM_MARK + 1, tsm, 1);
             if (have) {
-                for (int i = 0; i < pre; ++i) {
-                    if (decode_orient<MODE>())
-                        tma_load_2d_hint(smemB + i * Cfg::kStageBytesB, &tmB, &full_bar[i], (t.kb0 + i) * BLOCK_K,
-                                         t.b_tile * BN, polB);
-                    else
-                        tma_load_2d_hint(smemA + i * Cfg::kStageBytesA, &tmA, &full_bar[i], (t.kb0 + i) * BLOCK_K,
-                                         t.a_tile * BLOCK_A, polA);
-                }
+                for (int i = 0; i < pre; ++i)
+                    tma_load_2d_hint(smemB + i * Cfg::kStageBytesB, &tmB, &full_bar[i], (t.kb0 + i) * BLOCK_K,
+                                     t.b_tile * BN, polB);
                 t.kb0 += pre;                          // already in flight
                 stage = pre % kStages;
                 phase = (pre == kStages) ? 1u : 0u;
@@ -574,7 +288,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 if (tma_epi) { epilogue_planes_tma<BN>(arow, t, quarter, lane, etid, &tmOut, epi_stage); done = true; }
             }
             if (!done)
-                epilogue_item<BN, MODE>(arow, a_row, t, quarter, lane, out, rowsA, rowsB, ldo, ld_rows, rope, epi_stage);
+                epilogue_item<BN, MODE>(arow, a_row, t, quarter, lane, out, rowsA, rowsB, ldo, ld_rows, epi_stage);
             if (tsm >= 0 && etid == 0) trace_mark_at(TR_GEMM_MARK + 5, tsm, 17 + 2 * it);
         }
         if constexpr (MODE == OUT_TRANSPOSED_F32 && BN <= 64) {
@@ -584,6 +298,298 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
     __syncthreads();
     if (tsm >= 0 && threadIdx.x == 0) trace_mark_at(TR_GEMM_MARK + 6, tsm, 3);
+    trace_end(tr_slot);
+}
+
+// =================================================================================================
+// Prefill orientation: A = activations [T, K], B = weight [N, K], row-major outputs (QKV + RoPE, O / down + residual,
+// gate/up + SiLU, plain bf16).  Compute-bound, so the tile is as wide as a warpgroup's registers allow: 128 tokens x 256
+// weight rows, two consumer warpgroups (64 token rows each, m64n256k16: 128 fp32 accumulators per thread), one producer
+// warpgroup of which one thread issues the TMA loads.  setmaxnreg moves the producer's registers to the consumers.  The
+// epilogues run straight from the accumulator fragments: a thread holds rows r and r + 8 at columns 8j + 2(lane % 4) + {0, 1},
+// j < 32, so a quad covers 8 consecutive columns (a full 32-byte sector of fp32), a head's columns d and d + 64 (RoPE) and a
+// block's gate and up columns (SiLU) sit in the same thread.
+struct PfCfg {
+    static constexpr int kTileB = 256;
+    static constexpr int kStages = 4;
+    static constexpr int kStageBytesA = BLOCK_A * BLOCK_K * 2;             // 16 KB
+    static constexpr int kStageBytesB = kTileB * BLOCK_K * 2;              // 32 KB
+    static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
+    static constexpr int kThreads = 384;                                   // warpgroup 0: producer, 1 and 2: consumers
+    static constexpr int kConsumerWarps = 8;
+    static constexpr int kSmemBytes = kStages * kStageBytes + 256 + 1024 /*align slack*/;
+    static constexpr int kProducerRegs = 40, kConsumerRegs = 232;          // 128 x 40 + 256 x 232 <= 64 K registers
+};
+static_assert(2 * PfCfg::kSmemBytes > 227 * 1024 && PfCfg::kSmemBytes <= 227 * 1024, "one prefill GEMM CTA per SM");
+
+// Deferred RMSNorm, consumer side: the operand row was bf16(x * gamma); 1 / rms(x) from its partial sums of squares.
+__device__ __forceinline__ float pf_rinv(const RopeEpi& rope, int row, int rowsA) {
+    if (rope.n_part <= 0 || row >= rowsA) return 1.f;
+    const float* ps = rope.rowss + (size_t)row * rope.n_part;
+    float ss = 0.f;
+    for (int j = 0; j < rope.n_part; ++j) ss += ps[j];
+    return rsqrtf(ss * rope.inv_hidden + rope.eps);
+}
+
+// acc: this thread's fragment of the consumer warpgroup's 64 x 256 block; row0 = its first token row, cb = first column of the tile
+template <int MODE>
+__device__ __forceinline__ void pf_epilogue(const float (&acc)[128], int row0, int b_tile, int quad, void* __restrict__ out,
+                                            int rowsA, int rowsB, int ldo, const RopeEpi& rope) {
+    const int cb = b_tile * PfCfg::kTileB;
+    const int cq = 2 * quad;                                   // column offset of this thread inside each group of 8
+    if constexpr (MODE == OUT_ROWMAJOR_RESID) {
+        float* xres = reinterpret_cast<float*>(out);
+        const bool defer = rope.xhat != nullptr;               // also emit bf16(x * gamma) and sum(x^2) per 128 columns
+        // sum(x^2) of a row over 128 columns, in one fixed order (the deferred norm of the next GEMM depends on its last bit):
+        // columns in groups of 4, g = x0^2 + x1^2 + x2^2 + x3^2; group k of a 32-column chunk accumulated over the 4 chunks
+        // into S_k; then ((S0 + S1) + (S2 + S3)) + ((S4 + S5) + (S6 + S7)).  A group is columns 8j + 4(quad / 2) + [0, 4): the
+        // even lane of a lane pair sums it with its partner's two values, and holds S_k for k = 2 (j % 4) + quad / 2.
+        float ss[2][2][4] = {};                                // [row h][128-column partial][j % 4]
+#pragma unroll
+        for (int c8 = 0; c8 < 32; c8 += 8) {                   // 64 columns at a time: all residual loads before the stores
+            float2 xv[2][8];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int col = cb + 8 * (c8 + j) + cq;
+                    const float* src = xres + (size_t)row * ldo + col;
+                    xv[h][j] = make_float2(0.f, 0.f);
+                    if (row < rowsA) {
+                        if (col + 1 < rowsB) xv[h][j] = *reinterpret_cast<const float2*>(src);
+                        else if (col < rowsB) xv[h][j].x = *src;
+                    }
+                }
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int jj = c8 + j, col = cb + 8 * jj + cq;
+                    const float x0 = xv[h][j].x + acc[4 * jj + 2 * h], x1 = xv[h][j].y + acc[4 * jj + 2 * h + 1];
+                    if (defer) {                               // all lanes: the shuffle needs the whole warp
+                        const float y0 = __shfl_xor_sync(0xffffffffu, x0, 1), y1 = __shfl_xor_sync(0xffffffffu, x1, 1);
+                        ss[h][jj >> 4][jj & 3] += x0 * x0 + x1 * x1 + y0 * y0 + y1 * y1;
+                    }
+                    if (row >= rowsA || col >= rowsB) continue;
+                    float* dst = xres + (size_t)row * ldo + col;
+                    const bool pair = col + 1 < rowsB;
+                    if (pair) *reinterpret_cast<float2*>(dst) = make_float2(x0, x1);
+                    else *dst = x0;
+                    if (defer) {
+                        __nv_bfloat16* hd = rope.xhat + (size_t)row * ldo + col;
+                        if (pair) {
+                            const uint32_t gw = *reinterpret_cast<const uint32_t*>(rope.gamma + col);
+                            *reinterpret_cast<uint32_t*>(hd) = pack_bf16(x0 * bf16_lo(gw), x1 * bf16_hi(gw));
+                        } else {
+                            *hd = __float2bfloat16(x0 * __bfloat162float(rope.gamma[col]));
+                        }
+                    }
+                }
+            }
+        }
+        if (defer) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int p = 0; p < 2; ++p) {
+                    float a[4];                                // lane quad 0: S_2m + S_2m+1 (S_2m+1 from quad 2)
+#pragma unroll
+                    for (int m = 0; m < 4; ++m) a[m] = ss[h][p][m] + __shfl_xor_sync(0xffffffffu, ss[h][p][m], 2);
+                    const float v = (a[0] + a[1]) + (a[2] + a[3]);
+                    const int row = row0 + 8 * h, part = 2 * b_tile + p;
+                    if (quad == 0 && row < rowsA && part * 128 < rowsB) rope.rowss_out[(size_t)row * rope.n_part_out + part] = v;
+                }
+        }
+    } else {
+        const float rinv[2] = {pf_rinv(rope, row0, rowsA), pf_rinv(rope, row0 + 8, rowsA)};
+        if constexpr (MODE == OUT_ROWMAJOR_ROPE) {
+            // two heads of 128 columns of the fused qkv projection: [q heads | k heads | v heads]
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                const int slot = row < rowsA ? rope.slot[row] : -1;
+                if (slot < 0) continue;
+                const int pos = rope.pos[row];
+                const float2* tab = rope.table + (size_t)pos * 64;
+#pragma unroll
+                for (int hb = 0; hb < 2; ++hb) {
+                    const int H = b_tile * 2 + hb;
+                    if (H * 128 >= rowsB) continue;
+                    if (H < rope.n_heads + rope.n_kv_heads) {
+                        __nv_bfloat16* dst = H < rope.n_heads
+                            ? rope.q_out + (size_t)row * (rope.n_heads * 128) + H * 128
+                            : rope.k_cache + (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads)) * rope.ctx_max + pos) * 128;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int d = 8 * j + cq;
+                            const int jl = 16 * hb + j, jh = jl + 8;     // columns d and d + 64 of the head
+                            const float4 cs = *reinterpret_cast<const float4*>(tab + d);   // (cos, sin) of d and d + 1
+                            const float l0 = acc[4 * jl + 2 * h] * rinv[h], l1 = acc[4 * jl + 2 * h + 1] * rinv[h];
+                            const float h0 = acc[4 * jh + 2 * h] * rinv[h], h1 = acc[4 * jh + 2 * h + 1] * rinv[h];
+                            *reinterpret_cast<uint32_t*>(dst + d) = pack_bf16(l0 * cs.x - h0 * cs.y, l1 * cs.z - h1 * cs.w);
+                            *reinterpret_cast<uint32_t*>(dst + 64 + d) = pack_bf16(h0 * cs.x + l0 * cs.y, h1 * cs.z + l1 * cs.w);
+                        }
+                    } else {
+                        __nv_bfloat16* dst = rope.v_cache +
+                            (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads - rope.n_kv_heads)) * rope.ctx_max + pos) * 128;
+#pragma unroll
+                        for (int j = 0; j < 16; ++j) {
+                            const int jj = 16 * hb + j;
+                            *reinterpret_cast<uint32_t*>(dst + 8 * j + cq) =
+                                pack_bf16(acc[4 * jj + 2 * h] * rinv[h], acc[4 * jj + 2 * h + 1] * rinv[h]);
+                        }
+                    }
+                }
+            }
+        } else if constexpr (MODE == OUT_ROWMAJOR_SILU) {
+            // weight rows interleaved [gate 64 | up 64] per 128: 2 x 64 output columns per tile, ldo = inter
+            __nv_bfloat16* act = reinterpret_cast<__nv_bfloat16*>(out);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                if (row >= rowsA) continue;
+#pragma unroll
+                for (int hb = 0; hb < 2; ++hb) {
+                    if (cb + hb * 128 >= rowsB) continue;
+                    __nv_bfloat16* dst = act + (size_t)row * ldo + b_tile * 128 + hb * 64 + cq;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int jg = 16 * hb + j, ju = jg + 8;
+                        const float g0 = acc[4 * jg + 2 * h] * rinv[h], g1 = acc[4 * jg + 2 * h + 1] * rinv[h];
+                        const float u0 = acc[4 * ju + 2 * h] * rinv[h], u1 = acc[4 * ju + 2 * h + 1] * rinv[h];
+                        *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16(silu_mul(g0, u0), silu_mul(g1, u1));
+                    }
+                }
+            }
+        } else {
+            static_assert(MODE == OUT_ROWMAJOR_BF16, "row-major modes");
+            __nv_bfloat16* c = reinterpret_cast<__nv_bfloat16*>(out);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                if (row >= rowsA) continue;
+                __nv_bfloat16* dst = c + (size_t)row * ldo;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const int col = cb + 8 * j + cq;
+                    const float v0 = acc[4 * j + 2 * h] * rinv[h], v1 = acc[4 * j + 2 * h + 1] * rinv[h];
+                    if (col + 1 < rowsB) *reinterpret_cast<uint32_t*>(dst + col) = pack_bf16(v0, v1);
+                    else if (col < rowsB) dst[col] = __float2bfloat16(v0);
+                }
+            }
+        }
+    }
+}
+
+template <int MODE>
+__global__ void __launch_bounds__(PfCfg::kThreads, 1)
+gemm_pf_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* __restrict__ out,
+              int rowsA, int rowsB, int K, int ldo, const RopeEpi rope) {
+    constexpr int kStages = PfCfg::kStages;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = align_smem_1024(smem_raw);
+    uint8_t* smemA = smem;
+    uint8_t* smemB = smem + kStages * PfCfg::kStageBytesA;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * PfCfg::kStageBytes);
+    uint64_t* empty_bar = full_bar + kStages;
+
+    const int wg = threadIdx.x >> 7;
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_GEMM_PF);
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmA);
+        tma_prefetch_desc(&tmB);
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], PfCfg::kConsumerWarps);     // one arrival per consumer warp
+        }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    WorkSched sched;
+    sched.init(rowsA, rowsB, K, 1, PfCfg::kTileB);
+    WorkItem t;
+    if (wg == 0) {
+        // ===================== TMA producer (one thread of warpgroup 0) =====================
+        setmaxnreg_dec<PfCfg::kProducerRegs>();
+        if (threadIdx.x < 32 && elect_one()) {
+            const uint64_t pol = l2_policy_evict_last();     // both operands are re-read by other tiles
+            int stage = 0;
+            uint32_t phase = 0;
+            bool have = sched.next(t);
+            // PDL: the weight stages of the first item go out before the activations are known to exist
+            int pre = 0;
+            if (have) {
+                pre = min(kStages, t.kb1 - t.kb0);
+                for (int i = 0; i < pre; ++i) {
+                    mbar_arrive_expect_tx(&full_bar[i], PfCfg::kStageBytes);
+                    tma_load_2d_hint(smemB + i * PfCfg::kStageBytesB, &tmB, &full_bar[i], (t.kb0 + i) * BLOCK_K,
+                                     t.b_tile * PfCfg::kTileB, pol);
+                }
+            }
+            griddep_wait();
+            trace_dep(tr_slot);
+            if (have) {
+                for (int i = 0; i < pre; ++i)
+                    tma_load_2d_hint(smemA + i * PfCfg::kStageBytesA, &tmA, &full_bar[i], (t.kb0 + i) * BLOCK_K,
+                                     t.a_tile * BLOCK_A, pol);
+                t.kb0 += pre;
+                stage = pre % kStages;
+                phase = (pre == kStages) ? 1u : 0u;
+            }
+            while (have) {
+                for (int kb = t.kb0; kb < t.kb1; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    mbar_arrive_expect_tx(&full_bar[stage], PfCfg::kStageBytes);
+                    tma_load_2d_hint(smemA + stage * PfCfg::kStageBytesA, &tmA, &full_bar[stage], kb * BLOCK_K,
+                                     t.a_tile * BLOCK_A, pol);
+                    tma_load_2d_hint(smemB + stage * PfCfg::kStageBytesB, &tmB, &full_bar[stage], kb * BLOCK_K,
+                                     t.b_tile * PfCfg::kTileB, pol);
+                    if (++stage == kStages) { stage = 0; phase ^= 1; }
+                }
+                have = sched.next(t);
+            }
+        }
+    } else {
+        // ===================== consumer warpgroups: rows [64 (wg - 1), 64 wg) of the tile =====================
+        setmaxnreg_inc<PfCfg::kConsumerRegs>();
+        const int cw = wg - 1;
+        const int wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+        const bool arrive = lane == 0;
+        const uint32_t smemA_u = smem_u32(smemA) + cw * (64 * BLOCK_K * 2), smemB_u = smem_u32(smemB);
+        griddep_wait();                               // `out` may still be read by the preceding kernel
+        int stage = 0;
+        uint32_t phase = 0;
+        while (sched.next(t)) {
+            float acc[128];
+            int prev = -1;
+            wgmma_fence_regs(acc);
+            for (int kb = t.kb0; kb < t.kb1; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint64_t da = gmma_desc_sw128(smemA_u + stage * PfCfg::kStageBytesA);
+                const uint64_t db = gmma_desc_sw128(smemB_u + stage * PfCfg::kStageBytesB);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BLOCK_K / GMMA_K; ++k)
+                    wgmma_ss<256>(acc, da + 2 * k, db + 2 * k, (kb > t.kb0 || k > 0) ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();                      // the group of the previous k-block has retired: release its slot
+                if (prev >= 0 && arrive) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            if (prev >= 0 && arrive) mbar_arrive(&empty_bar[prev]);
+            const int row0 = t.a_tile * BLOCK_A + cw * 64 + wq * 16 + (lane >> 2);
+            pf_epilogue<MODE>(acc, row0, t.b_tile, lane & 3, out, rowsA, rowsB, ldo, rope);
+        }
+    }
+    __syncthreads();
     trace_end(tr_slot);
 }
 
@@ -747,9 +753,6 @@ gemm_mlp_wgmma(const __grid_constant__ MlpArgs a) {
         const uint32_t smemA_u = smem_u32(smemA), smemB_u = smem_u32(smemB);
         int stage = 0;
         uint32_t phase = 0;
-        RopeEpi no_rope;
-        no_rope.q_out = nullptr; no_rope.k_cache = nullptr; no_rope.v_cache = nullptr; no_rope.slot = nullptr;
-        no_rope.pos = nullptr; no_rope.table = nullptr; no_rope.n_heads = 0; no_rope.n_kv_heads = 0; no_rope.ctx_max = 0;
         griddep_wait();
         trace_dep(tr_slot);
         int nstat = -1;
@@ -774,10 +777,10 @@ gemm_mlp_wgmma(const __grid_constant__ MlpArgs a) {
             if (tma_done) {
             } else if (ph == 0)
                 epilogue_item<BN, OUT_TRANSPOSED_SILU>(arow, a_row, t, quarter, lane, a.act, 2 * a.inter, a.rows, a.inter, 0,
-                                                       no_rope, silu_stage);
+                                                       silu_stage);
             else
                 epilogue_item<BN, OUT_TRANSPOSED_F32>(arow, a_row, t, quarter, lane, a.out1, a.hidden, a.rows, a.hidden,
-                                                      a.ld_rows, no_rope, nullptr);
+                                                      a.ld_rows, nullptr);
             if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 10, 128 + 4 * it + 1);      // stores issued
             if (ph == 0) {
                 // publish this tile's 64 act columns: every epilogue thread's stores, then one release-increment
@@ -868,6 +871,10 @@ int make_tmap_act_store(CUtensorMap* map, const void* base, int rows, int n, int
     return r == CUDA_SUCCESS ? RR_OK : RR_ERR_CUDA;
 }
 
+static bool rowmajor(int mode) {
+    return mode == OUT_ROWMAJOR_BF16 || mode == OUT_ROWMAJOR_SILU || mode == OUT_ROWMAJOR_ROPE || mode == OUT_ROWMAJOR_RESID;
+}
+
 static std::atomic<int> g_num_sms[64];
 int num_sms() {                         // of the current device (one process may drive several)
     int dev = 0;
@@ -891,12 +898,27 @@ static int launch_one(const GemmPlan& p, cudaStream_t st) {
     const int n_work = tilesA * tilesB * p.splits;
     const int grid = n_work < num_sms() ? n_work : num_sms();
     cudaError_t le = launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)gemm_smem_bytes<BN, MODE, CAP>(), st, p.tmA, p.tmB,
-                                p.out, p.rowsA, p.rowsB, p.K, p.splits, p.ldo, p.ld_rows, p.rope, p.tmOut, p.tma_epi);
+                                p.out, p.rowsA, p.rowsB, p.K, p.splits, p.ldo, p.ld_rows, p.tmOut, p.tma_epi);
     return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
 }
 
-// splits >= 1: uniform split-K with `splits` planes.  bn = 256 is accepted and runs 128-wide tiles: a consumer warpgroup holds
-// at most 128 x 128 fp32 accumulators in registers.
+template <int MODE>
+static int launch_pf(const GemmPlan& p, cudaStream_t st) {
+    auto kern = gemm_pf_wgmma<MODE>;
+    static std::atomic<uint64_t> attr_set{0};
+    if (ensure_dyn_smem(kern, PfCfg::kSmemBytes, attr_set) != cudaSuccess) return RR_ERR_CUDA;
+    const int tilesA = (p.rowsA + BLOCK_A - 1) / BLOCK_A;
+    const int tilesB = (p.rowsB + PfCfg::kTileB - 1) / PfCfg::kTileB;
+    const int n_work = tilesA * tilesB;
+    const int grid = n_work < num_sms() ? n_work : num_sms();
+    cudaError_t le = launch_pdl(kern, dim3(grid), dim3(PfCfg::kThreads), (size_t)PfCfg::kSmemBytes, st, p.tmA, p.tmB, p.out,
+                                p.rowsA, p.rowsB, p.K, p.ldo, p.rope);
+    return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
+}
+
+// splits >= 1: uniform split-K with `splits` planes.  Decode orientation: bn = 256 is accepted and runs 128-wide tiles (a
+// consumer warpgroup holds at most 128 x 128 fp32 accumulators in registers).  Row-major (prefill) modes always run the
+// 128 x 256 tiles of gemm_pf_wgmma; their bn is only validated.
 int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB,
                    int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn) {
     if (K % 8 != 0 || ldA % 8 != 0 || ldB % 8 != 0) return RR_ERR_ARG;
@@ -924,23 +946,21 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
         if (rc != RR_OK) return rc;
         p->tma_epi = 1;
     }
-    return make_tmap_bf16_2d(&p->tmB, B, rowsB, K, ldB, bn);
+    return make_tmap_bf16_2d(&p->tmB, B, rowsB, K, ldB, rowmajor(mode) ? PfCfg::kTileB : bn);
 }
 
 int gemm_launch(const GemmPlan& p, cudaStream_t st) {
+    switch (p.mode) {
+        case OUT_ROWMAJOR_BF16: return launch_pf<OUT_ROWMAJOR_BF16>(p, st);
+        case OUT_ROWMAJOR_SILU: return launch_pf<OUT_ROWMAJOR_SILU>(p, st);
+        case OUT_ROWMAJOR_ROPE: return launch_pf<OUT_ROWMAJOR_ROPE>(p, st);
+        case OUT_ROWMAJOR_RESID: return launch_pf<OUT_ROWMAJOR_RESID>(p, st);
+    }
 #define RR_CASE(BN_)                                                                                  \
     case BN_:                                                                                         \
-        if (p.mode == OUT_ROWMAJOR_BF16) return launch_one<BN_, OUT_ROWMAJOR_BF16>(p, st);             \
         if (p.mode == OUT_TRANSPOSED_F32) return launch_one<BN_, OUT_TRANSPOSED_F32>(p, st);           \
         if constexpr (BN_ >= 32) {                                                                    \
             if (p.mode == OUT_TRANSPOSED_SILU) return launch_one<BN_, OUT_TRANSPOSED_SILU>(p, st);     \
-        }                                                                                             \
-        if constexpr (BN_ >= 128) {                                                                   \
-            if (p.mode == OUT_ROWMAJOR_RESID) return launch_one<BN_, OUT_ROWMAJOR_RESID>(p, st);       \
-        }                                                                                             \
-        if constexpr (BN_ == 128) {                                                                   \
-            if (p.mode == OUT_ROWMAJOR_SILU) return launch_one<BN_, OUT_ROWMAJOR_SILU>(p, st);         \
-            if (p.mode == OUT_ROWMAJOR_ROPE) return launch_one<BN_, OUT_ROWMAJOR_ROPE>(p, st);         \
         }                                                                                             \
         return RR_ERR_ARG;
     switch (p.bn) {

@@ -2,7 +2,7 @@
 // decode layer kernel (rr_layer.cu): tile configuration, the consumer warpgroup's main loop, the per-CTA work schedule,
 // small helpers.
 //
-// CTA layout of every kernel built on this: warps 0..3 = ONE consumer warpgroup (wgmma issue + epilogue, thread t owns
+// CTA layout of every decode-orientation kernel built on this (the prefill GEMM, gemm_pf_wgmma, has its own): warps 0..3 = ONE consumer warpgroup (wgmma issue + epilogue, thread t owns
 // row t of the 128-row tile in the epilogue), warp 4 = TMA producer.  The tile's accumulators live in the warpgroup's
 // registers (2 x m64nBN: rows 0..63 and 64..127); after the main loop they are staged row-major in shared memory so
 // the epilogues read "row t, 32 consecutive columns" per thread.
@@ -34,7 +34,7 @@ struct GemmCfg {
     static constexpr int kAccPitch = BN + 4;               // fp32 words per staged row: conflict-free 16-byte row reads
     static constexpr int kAccBytes = BLOCK_A * kAccPitch * 4;
     static constexpr int kSiluStageBytes = 2 * 32 * 64 * 4;   // OUT_TRANSPOSED_SILU: up-row exchange, 2 x [32 cols][64 rows] fp32
-    static constexpr int kEpiMax = cmax(cmax(BN <= 64 ? BN * 512 : 0, kSiluStageBytes + (BN <= 64 ? BN * 128 : 0)), 4 * 32 * 36 * 4);
+    static constexpr int kEpiMax = cmax(BN <= 64 ? BN * 512 : 0, kSiluStageBytes + (BN <= 64 ? BN * 128 : 0));
     static constexpr int kStagesRaw = (224 * 1024 - 1024 - 256 - kAccBytes - kEpiMax) / kStageBytes;
     static constexpr int kStages = kStagesRaw > CAP ? CAP : kStagesRaw;
     static constexpr int kAccOff = kStages * kStageBytes + 256;         // staged accumulator tile
@@ -50,14 +50,11 @@ constexpr int mlp_stage_bytes() {
     constexpr int a = planes_stage_bytes<BN>(), b = GemmCfg<BN>::kSiluStageBytes + (BN <= 64 ? BN * 64 * 2 : 0);
     return a > b ? a : b;
 }
-template <int MODE>
-__host__ __device__ constexpr bool decode_orient() { return MODE == OUT_TRANSPOSED_F32 || MODE == OUT_TRANSPOSED_SILU; }
 template <int BN, int MODE, int CAP = 8>
 constexpr int gemm_smem_bytes() {
-    // SILU (decode): up-row exchange; RESID (prefill): per-warp 32 x 36 fp32 transpose tiles (18 KB) -- same slot
+    // SILU: up-row exchange; F32: the planes tile of the TMA-store epilogue
     return GemmCfg<BN, CAP>::kSmemBytes +
-           (MODE == OUT_TRANSPOSED_SILU ? GemmCfg<BN, CAP>::kSiluStageBytes : MODE == OUT_ROWMAJOR_RESID ? 4 * 32 * 36 * 4 :
-            MODE == OUT_TRANSPOSED_F32 ? planes_stage_bytes<BN>() : 0);
+           (MODE == OUT_TRANSPOSED_SILU ? GemmCfg<BN, CAP>::kSiluStageBytes : MODE == OUT_TRANSPOSED_F32 ? planes_stage_bytes<BN>() : 0);
 }
 // ---- consumer warpgroup ------------------------------------------------------------------------------------------------
 // Accumulate the next `nkb` ring slots into acc (acc[0]: tile rows 0..63, acc[1]: rows 64..127).  The first k step
