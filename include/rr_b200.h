@@ -80,7 +80,10 @@ enum {                       /* router_settings.routing_strategy (reference conf
     /* client-side distribution strategies of reference src/demo_account_sharding.py:335-343: */
     RR_STRATEGY_ROUND_ROBIN = 2,  /* req_id % n */
     RR_STRATEGY_SPLIT = 3,        /* first share of the burst to backend 0, next to backend 1, ... (req_id < N / 2) */
-    RR_STRATEGY_RANDOM = 4        /* random.choice, weights ignored */
+    RR_STRATEGY_RANDOM = 4,       /* random.choice, weights ignored */
+    /* litellm's latency-based-routing: random.choice among the eligible deployments whose mean latency per output token
+     * is within (1 + buffer) of the lowest; latency samples arrive on DONE / FAIL events (rr_event.chain_start) */
+    RR_STRATEGY_LATENCY_BASED = 5
 };
 
 /* RR_EV_BURST(target = group, tokens = N) declares the size of the next burst for RR_STRATEGY_SPLIT. */
@@ -101,14 +104,20 @@ typedef struct rr_router_settings {
     int32_t allowed_fails;          /* config.yaml:103 */
     int32_t cooldown_ms;            /* config.yaml:104 (seconds * 1000) */
     int32_t weight_by;              /* 0 = uniform, 1 = weight, 2 = rpm, 3 = tpm (simple-shuffle) */
-    int32_t reserved[3];
+    /* RR_STRATEGY_LATENCY_BASED (router_settings.routing_strategy_args); ignored by the other strategies: */
+    int32_t latency_list_size;      /* max_latency_list_size: samples kept per deployment, 1..32 (0 = 10) */
+    int32_t latency_buffer_ppm;     /* lowest_latency_buffer in millionths, >= 0 (0.5 -> 500000) */
+    int32_t latency_ttl_ms;         /* ttl: a model group's samples are dropped this long after its last write (0 = 1 h) */
 } rr_router_settings;
 
 typedef struct rr_event {
     int32_t type;            /* RR_EV_* */
     int32_t target;          /* ADMIT: group index; DONE/FAIL: deployment index */
     int32_t tokens;          /* ADMIT: prompt tokens; DONE: completion tokens */
-    int32_t chain_start;     /* ADMIT: 0 = try the group itself first, k = start at k-th fallback */
+    int32_t chain_start;     /* ADMIT: 0 = try the group itself first, k = start at k-th fallback;
+                                DONE: measured request latency in microseconds (<= 0: no sample);
+                                FAIL: 1 = the request timed out (penalty sample), 0 = any other failure.
+                                Only RR_STRATEGY_LATENCY_BASED reads it on DONE / FAIL. */
     int64_t now_ms;          /* injectable clock, milliseconds */
 } rr_event;
 
@@ -145,6 +154,11 @@ int rr_router_process(rr_router* r, const rr_event* events, int n_events, rr_dec
 int rr_router_process_device(rr_router* r, const rr_event* d_events, int n_events,
                              rr_decision* d_decisions, void* stream);
 int rr_router_snapshot(rr_router* r, rr_deployment_state* out /* [n_deployments] */);
+/* RR_STRATEGY_LATENCY_BASED state as stored (a TTL expiry is applied at the next write or pick of the group):
+ * per deployment the mean of its latency samples in microseconds per output token (0.0 without samples) and the
+ * sample count.  All zeros for the other strategies. */
+int rr_router_latency_snapshot(rr_router* r, double* mean_out /* [n_deployments] */,
+                               int32_t* n_samples_out /* [n_deployments] */);
 /* Re-seed the MT19937 stream exactly like CPython random.seed(int). */
 int rr_router_seed(rr_router* r, uint64_t seed);
 /* Host-only: the MT19937 state (624 words + index) CPython's random.seed(seed) produces. */

@@ -42,7 +42,8 @@ class DeploymentDesc(C.Structure):
 class RouterSettings(C.Structure):
     _fields_ = [("strategy", C.c_int32), ("enable_pre_call_checks", C.c_int32),
                 ("allowed_fails", C.c_int32), ("cooldown_ms", C.c_int32),
-                ("weight_by", C.c_int32), ("reserved", C.c_int32 * 3)]
+                ("weight_by", C.c_int32), ("latency_list_size", C.c_int32),
+                ("latency_buffer_ppm", C.c_int32), ("latency_ttl_ms", C.c_int32)]
 
 
 class Event(C.Structure):
@@ -131,6 +132,7 @@ PROTOTYPES = {
     "rr_router_process": (C.c_int, [vp, C.POINTER(Event), C.c_int, C.POINTER(Decision)]),
     "rr_router_process_device": (C.c_int, [vp, vp, C.c_int, vp, vp]),
     "rr_router_snapshot": (C.c_int, [vp, C.POINTER(DeploymentState)]),
+    "rr_router_latency_snapshot": (C.c_int, [vp, C.POINTER(C.c_double), c_i32p]),
     "rr_router_seed": (C.c_int, [vp, C.c_uint64]),
     "rr_mt_seed_state": (C.c_int, [C.c_uint64, C.POINTER(C.c_uint32)]),
     "rr_count_tokens": (C.c_int, [C.c_char_p, C.c_size_t, c_i32p]),

@@ -5,7 +5,8 @@ Keeps the keys the reference's config/config.yaml uses (reference config/config.
 `router_settings.{routing_strategy, enable_pre_call_checks, allowed_fails, cooldown_time, fallbacks}`);
 YAML anchors / merge keys (`<<: *aws-defaults`, :40) are resolved by PyYAML.  AWS-only keys
 (`aws_region_name`, `aws_profile_name`, the `aws:` / `cris:` sections) are accepted and ignored.
-Local extension: `litellm_params.gpu: N` pins a deployment to a replica; `litellm_params.model:
+`router_settings.routing_strategy_args` takes litellm's latency-based-routing keys (`lowest_latency_buffer`,
+`max_latency_list_size`, `ttl`).  Local extension: `litellm_params.gpu: N` pins a deployment to a replica; `litellm_params.model:
 b200/<spec>` names an on-box model (models.SPECS) instead of `bedrock/<id>`.
 """
 from __future__ import annotations
@@ -15,7 +16,9 @@ from typing import Any, Dict, List, Optional
 
 import yaml
 
-STRATEGIES = {"simple-shuffle": 0, "least-busy": 1, "round-robin": 2, "split": 3, "random": 4}
+STRATEGIES = {"simple-shuffle": 0, "least-busy": 1, "round-robin": 2, "split": 3, "random": 4,
+              "latency-based-routing": 5}
+_INT32_MAX = 2**31 - 1
 _PROVIDER_PREFIXES = ("bedrock/", "b200/", "openai/", "azure/")
 
 
@@ -55,6 +58,10 @@ class RouterConfig:
     allowed_fails: int = 3
     cooldown_time: float = 5.0
     port: int = 4000
+    # latency-based-routing (router_settings.routing_strategy_args)
+    latency_list_size: int = 10          # max_latency_list_size
+    latency_buffer_ppm: int = 0          # lowest_latency_buffer in millionths
+    latency_ttl_ms: int = 3_600_000      # ttl
 
     @property
     def strategy_id(self) -> int:
@@ -73,6 +80,35 @@ def _int_or(v, default=-1) -> int:
     if isinstance(v, bool) or not isinstance(v, (int, float)) or int(v) != v:
         raise ValueError(f"rpm/tpm/weight must be integers, got {v!r}")
     return int(v)
+
+
+def _number(key: str, v) -> float:
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or v != v or v in (float("inf"), float("-inf")):
+        raise ValueError(f"routing_strategy_args.{key} must be a finite number, got {v!r}")
+    return v
+
+
+def parse_strategy_args(args: Optional[dict]) -> Dict[str, int]:
+    """router_settings.routing_strategy_args of latency-based-routing -> the integer settings the router kernel takes:
+    latency_list_size (max_latency_list_size, 1..32, default 10), latency_buffer_ppm (lowest_latency_buffer >= 0 in
+    millionths, round(v * 1e6), default 0), latency_ttl_ms (ttl seconds > 0, default 3600)."""
+    args = dict(args or {})
+    unknown = sorted(set(args) - {"lowest_latency_buffer", "max_latency_list_size", "ttl"})
+    if unknown:
+        raise ValueError(f"routing_strategy_args: unsupported keys {unknown}; supported: "
+                         "lowest_latency_buffer, max_latency_list_size, ttl")
+    n = args.get("max_latency_list_size", 10)
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= 32:
+        raise ValueError(f"routing_strategy_args.max_latency_list_size must be an integer in 1..32, got {n!r}")
+    buf = _number("lowest_latency_buffer", args.get("lowest_latency_buffer", 0))
+    ppm = round(buf * 1e6)
+    if buf < 0 or ppm > _INT32_MAX:
+        raise ValueError(f"routing_strategy_args.lowest_latency_buffer must be in [0, {_INT32_MAX / 1e6:g}], got {buf!r}")
+    ttl = _number("ttl", args.get("ttl", 3600))
+    ttl_ms = round(ttl * 1000)
+    if ttl_ms < 1 or ttl_ms > _INT32_MAX:
+        raise ValueError(f"routing_strategy_args.ttl must be in (0, {_INT32_MAX // 1000}] seconds, got {ttl!r}")
+    return {"latency_list_size": n, "latency_buffer_ppm": ppm, "latency_ttl_ms": ttl_ms}
 
 
 def build_config(model_list: List[dict], router_settings: Optional[dict] = None, port: int = 4000) -> RouterConfig:
@@ -101,6 +137,10 @@ def build_config(model_list: List[dict], router_settings: Optional[dict] = None,
     strategy = rs.get("routing_strategy", "simple-shuffle")
     if strategy not in STRATEGIES:
         raise ValueError(f"unsupported routing_strategy {strategy!r}; supported: {sorted(STRATEGIES)}")
+    sargs = rs.get("routing_strategy_args")
+    if sargs is not None and not isinstance(sargs, dict):
+        raise ValueError(f"routing_strategy_args must be a mapping, got {sargs!r}")
+    lat = parse_strategy_args(sargs)
     fbs: Dict[int, List[int]] = {}
     for item in rs.get("fallbacks") or []:
         for src, dst in item.items():
@@ -115,7 +155,7 @@ def build_config(model_list: List[dict], router_settings: Optional[dict] = None,
     return RouterConfig(groups=groups, deployments=deps, fallbacks=fbs, routing_strategy=strategy,
                         enable_pre_call_checks=bool(rs.get("enable_pre_call_checks", False)),
                         allowed_fails=int(rs.get("allowed_fails", 3)),
-                        cooldown_time=float(rs.get("cooldown_time", 5.0)), port=port)
+                        cooldown_time=float(rs.get("cooldown_time", 5.0)), port=port, **lat)
 
 
 def load_config(path: str) -> RouterConfig:

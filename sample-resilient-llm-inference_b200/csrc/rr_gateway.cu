@@ -18,6 +18,7 @@
 
 #include <atomic>
 #include <chrono>
+#include <cmath>
 #include <condition_variable>
 #include <deque>
 #include <mutex>
@@ -53,6 +54,7 @@ struct Pending {
     GwReq* req;        // ADMIT
     int target;        // DONE / FAIL: deployment; BURST: group
     int tokens;        // DONE: completion tokens; BURST: burst size
+    int aux = 0;       // rr_event.chain_start of a DONE (latency, us) / FAIL (1 = timeout): latency-based routers only
 };
 
 }  // namespace
@@ -62,6 +64,7 @@ struct rr_gateway {
     std::vector<rr_engine*> engines;        // index = position in the create() arrays
     std::unordered_map<int, int> by_replica;   // replica id -> index into engines
     int n_deps = 0, n_groups = 0;
+    bool latency = false;                   // the router is latency-based: DONE / FAIL events carry samples
     int min_ctx = 0, min_pf = 0, min_vocab = 0;
     rr_gateway_opts opts;
 
@@ -139,11 +142,19 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
             r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
         }
         if (status == RR_OK) {
-            g->pending.push_back(Pending{RR_EV_DONE, nullptr, dep, (int)r->tokens.size()});
+            // latency sample: the engine's submit -> done time of the request, in microseconds
+            int lat_us = 0;
+            if (g->latency && wrc == RR_OK) {
+                const double us = std::round((comp.t_done_s - comp.t_submit_s) * 1e6);
+                lat_us = us < 1.0 ? 1 : (us > 2147483647.0 ? 2147483647 : (int)us);
+            }
+            g->pending.push_back(Pending{RR_EV_DONE, nullptr, dep, (int)r->tokens.size(), lat_us});
             gw_finish(g, r, RR_OK);
         } else if (status == RR_CANCELLED) {
-            // the owner gave up: a client-side timeout counts as a backend failure (cooldown), a disconnect does not
-            g->pending.push_back(Pending{r->cancel_as_failure ? RR_EV_FAIL : RR_EV_DONE, nullptr, dep, n_generated});
+            // the owner gave up: a client-side timeout counts as a backend failure (cooldown), a disconnect does not;
+            // a latency-based router also records the timeout penalty for the deployment
+            g->pending.push_back(Pending{r->cancel_as_failure ? RR_EV_FAIL : RR_EV_DONE, nullptr, dep, n_generated,
+                                         g->latency && r->cancel_as_failure ? 1 : 0});
             gw_finish(g, r, r->cancel_as_failure ? RR_TIMEOUT : RR_CANCELLED);
         } else {
             // backend failure: report it, then walk on down the fallback chain with the same request
@@ -197,7 +208,7 @@ static void gw_dispatch(rr_gateway* g) {
                 // (fields of a queued request are only touched by this thread until the decision is published)
                 e.target = p.req->group; e.tokens = (int32_t)p.req->prompt.size(); e.chain_start = p.req->chain_start;
             } else {
-                e.target = p.target; e.tokens = p.tokens;
+                e.target = p.target; e.tokens = p.tokens; e.chain_start = p.aux;
             }
             ev.push_back(e);
         }
@@ -289,6 +300,7 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
     if (opts) g->opts = *opts;
     memset(&g->st, 0, sizeof(g->st));
     rr::router_shape(router, &g->n_deps, &g->n_groups);
+    g->latency = rr::router_strategy(router) == RR_STRATEGY_LATENCY_BASED;
     g->min_ctx = g->min_pf = g->min_vocab = 0x7fffffff;
     for (int i = 0; i < n_engines; ++i) {
         if (!engines[i]) { delete g; return RR_INVALID_ARGUMENT; }

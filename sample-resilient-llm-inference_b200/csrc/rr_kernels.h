@@ -67,6 +67,7 @@ void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
+int router_strategy(const rr_router* r);
 int make_tmap_bf16_2d(CUtensorMap* map, const void* base, int rows, int K, int ld, int box_rows);
 int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB,
                    int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn);

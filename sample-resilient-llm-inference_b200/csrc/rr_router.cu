@@ -2,8 +2,9 @@
 //
 // Replaces litellm.Router as configured by reference config/config.yaml:35-108 and called from
 // reference src/demo_load_balancing.py:106-110, src/demo_fallback.py:143-147,
-// src/demo_quota_isolation.py:52-56.  Semantics are those of oracle/router.py (serialised-trace:
-// the result of one launch over an ordered event trace equals processing the events one by one).
+// src/demo_quota_isolation.py:52-56.  Semantics are those of oracle/router.py (latency-based routing:
+// oracle/latency_router.py) (serialised-trace: the result of one launch over an ordered event trace equals processing
+// the events one by one).
 //
 // Design: router state (per-deployment window counters, in-flight counts, cooldown deadlines,
 // MT19937 stream, round-robin cursors) is resident in HBM between launches and staged in shared memory for the
@@ -11,7 +12,8 @@
 // other through the RNG stream and the counters, so the trace is consumed by ONE warp in order;
 // the parallelism is across the <=32 candidate deployments of a model group: lane l owns
 // candidate l — eligibility is a ballot, the weighted pick is a rank-ordered scan + ballot
-// bisect, least-busy is a warp min-reduction.  Launches on one router are serialised (rr_router_process_device).
+// bisect, least-busy is a warp min-reduction, latency-based a warp min over per-lane mean latencies + a ballot of the
+// lanes within the buffer + a rank under (mean, lane).  Launches on one router are serialised (rr_router_process_device).
 // The RNG is CPython's: MT19937 with init_by_array seeding, random() = (a>>5, b>>6) 53-bit
 // doubles, _randbelow = getrandbits rejection loop (Lib/random.py:242-250, 454-489).
 // Latency/atomic-bound: not a roofline kernel (SURVEY.md §8d); reported as ns/event.
@@ -54,6 +56,16 @@ struct RouterDev {
     int* burst_size;            // [n_groups] split strategy: size of the declared burst (RR_EV_BURST)
     int* burst_pos;             // [n_groups] split strategy: requests of the burst seen so far
     uint32_t* mt;               // [624] + index at [624]
+    // latency-based strategy only (nullptr otherwise).  The per-deployment sample list is stored in O(1) form: the list
+    // rule freezes its first N-1 entries and only ever replaces the last one, so Python's in-order sum of the list is
+    // exactly  n < N ? lat_head : lat_head + lat_last.
+    int lat_cap;                // N = max_latency_list_size
+    long long lat_ttl_ms;
+    double lat_buf;             // lowest_latency_buffer = ppm / 1e6
+    int* lat_n;                 // [n_deps] samples held, <= N
+    double* lat_head;           // [n_deps] in-order sum (from 0.0) of the first min(n, N-1) samples
+    double* lat_last;           // [n_deps] the N-th sample (valid when n == N)
+    long long* lat_stamp;       // [n_groups] now_ms of the group's last write, -1 = never
 };
 
 // ---------------------------------------------------------------- device MT19937 (one warp)
@@ -140,8 +152,30 @@ template <bool LOCAL> __device__ __forceinline__ int st_add(int* p, int v) {
     return atomicAdd(p, v);
 }
 
-// Walks events[0, n_events) in order (one warp).  `events` / `decisions` may be global or shared memory.
+// Latency-based strategy: one sample for deployment d (one lane).  An expired model group drops every list first; the
+// list rule is litellm's: append while shorter than N, otherwise list[:N-1] + [sample].
 template <bool LOCAL>
+__device__ __forceinline__ void lat_record(const RouterDev& S, int d, double sample, long long now) {
+    const int g = S.dep_group[d];
+    if (now - st_ld<LOCAL>(&S.lat_stamp[g]) > S.lat_ttl_ms) {
+        for (int j = S.group_off[g]; j < S.group_off[g + 1]; ++j) {
+            const int k = S.group_deps[j];
+            st_st<LOCAL>(&S.lat_n[k], 0);
+            st_st<LOCAL>(&S.lat_head[k], 0.0);
+            st_st<LOCAL>(&S.lat_last[k], 0.0);
+        }
+    }
+    const int n = st_ld<LOCAL>(&S.lat_n[d]);
+    if (n < S.lat_cap - 1) st_st<LOCAL>(&S.lat_head[d], __dadd_rn(st_ld<LOCAL>(&S.lat_head[d]), sample));
+    else st_st<LOCAL>(&S.lat_last[d], sample);
+    if (n < S.lat_cap) st_st<LOCAL>(&S.lat_n[d], n + 1);
+    st_st<LOCAL>(&S.lat_stamp[g], now);
+}
+
+// Walks events[0, n_events) in order (one warp).  `events` / `decisions` may be global or shared memory.
+// LAT: the router is latency-based (its state arrays exist); the other strategies run the LAT = false instantiation,
+// which carries none of the latency code.
+template <bool LOCAL, bool LAT>
 __device__ __forceinline__ void run_trace(const RouterDev& S, WarpMT& rng, const rr_event* events, int n_events,
                                           rr_decision* decisions) {
     const int lane = threadIdx.x;
@@ -249,6 +283,42 @@ __device__ __forceinline__ void run_trace(const RouterDev& S, WarpMT& rng, const
                         int idx = n > 0 ? (int)(((long long)i * nh) / n) : 0;
                         if (idx > nh - 1) idx = nh - 1;
                         pick_lane = nth_set_lane(mask, idx);
+                    } else if (LAT) {   // RR_STRATEGY_LATENCY_BASED
+                        // drop an expired group's samples, then mean = total / len per healthy lane (0.0 unmeasured)
+                        const bool expired = now - st_ld<LOCAL>(&S.lat_stamp[grp]) > S.lat_ttl_ms;   // warp-uniform
+                        double mean = 0.0;
+                        if (valid) {
+                            if (expired) {
+                                st_st<LOCAL>(&S.lat_n[d], 0);
+                                st_st<LOCAL>(&S.lat_head[d], 0.0);
+                                st_st<LOCAL>(&S.lat_last[d], 0.0);
+                            } else {
+                                const int n = st_ld<LOCAL>(&S.lat_n[d]);
+                                if (n > 0) {
+                                    const double head = st_ld<LOCAL>(&S.lat_head[d]);
+                                    const double tot = n < S.lat_cap ? head : __dadd_rn(head, st_ld<LOCAL>(&S.lat_last[d]));
+                                    mean = __ddiv_rn(tot, (double)n);
+                                }
+                            }
+                        }
+                        double lowest = healthy ? mean : __longlong_as_double(0x7ff0000000000000ll);   // +inf
+                        for (int o = 16; o > 0; o >>= 1) {
+                            const double other = __shfl_xor_sync(0xffffffffu, lowest, o);
+                            lowest = other < lowest ? other : lowest;
+                        }
+                        // two roundings, as Python computes lowest + (buf * lowest): no FMA
+                        const double threshold = __dadd_rn(lowest, __dmul_rn(S.lat_buf, lowest));
+                        const bool in = healthy && mean <= threshold;
+                        const uint32_t vmask = __ballot_sync(0xffffffffu, in);
+                        // random.choice(sorted(valid, key=mean)): rank of each valid lane under (mean, lane)
+                        const int r = (int)rng.randbelow((uint32_t)__popc(vmask));
+                        int rk = 0;
+                        for (uint32_t m = vmask; m; m &= m - 1) {
+                            const int k = __ffs(m) - 1;
+                            const double mk = __shfl_sync(0xffffffffu, mean, k);
+                            rk += (mk < mean || (mk == mean && k < lane)) ? 1 : 0;
+                        }
+                        pick_lane = __ffs(__ballot_sync(0xffffffffu, in && rk == r)) - 1;
                     } else {   // RR_STRATEGY_RANDOM: uniform, weights ignored
                         uniform = true;
                     }
@@ -304,6 +374,14 @@ __device__ __forceinline__ void run_trace(const RouterDev& S, WarpMT& rng, const
                             cooled = 1;
                         }
                     }
+                    if (LAT) {
+                        // DONE: chain_start = latency in us -> us per output token; FAIL: chain_start 1 = timeout -> 1e9
+                        if (ev.type == RR_EV_DONE && ev.chain_start > 0)
+                            lat_record<LOCAL>(S, d, ev.tokens > 0 ? __ddiv_rn((double)ev.chain_start, (double)ev.tokens)
+                                                                  : (double)ev.chain_start, now);
+                        else if (ev.type == RR_EV_FAIL && ev.chain_start == 1)
+                            lat_record<LOCAL>(S, d, 1e9, now);
+                    }
                 }
                 cooled = __shfl_sync(0xffffffffu, cooled, 0);
                 dec.status = RR_OK;
@@ -321,6 +399,7 @@ __device__ __forceinline__ void run_trace(const RouterDev& S, WarpMT& rng, const
 
 
 // ---- kernel, state in HBM (any topology) ----------------------------------------------------------
+template <bool LAT>
 __global__ void __launch_bounds__(32, 1)
 router_kernel(RouterDev S, const rr_event* __restrict__ events, int n_events,
               rr_decision* __restrict__ decisions) {
@@ -331,7 +410,7 @@ router_kernel(RouterDev S, const rr_event* __restrict__ events, int n_events,
     rng.mt = s_mt;
     rng.mti = (int)S.mt[624];
     __syncwarp();
-    run_trace<false>(S, rng, events, n_events, decisions);
+    run_trace<false, LAT>(S, rng, events, n_events, decisions);
     for (int i = lane; i < 624; i += 32) S.mt[i] = s_mt[i];
     if (lane == 0) S.mt[624] = (uint32_t)rng.mti;
 }
@@ -345,9 +424,10 @@ router_kernel(RouterDev S, const rr_event* __restrict__ events, int n_events,
 constexpr int RT_CHUNK = 128;
 struct RouterSmemLayout {
     uint32_t o_window, o_failw, o_cool, o_total, o_req, o_tok, o_failc, o_infl, o_rpm, o_tpm, o_wt, o_dgrp, o_gdeps,
-        o_goff, o_fboff, o_fbg, o_rr, o_bs, o_bp, o_mt, o_ev, o_dec, total;
+        o_goff, o_fboff, o_fbg, o_rr, o_bs, o_bp, o_mt, o_ev, o_dec, o_lat_n, o_lat_head, o_lat_last, o_lat_stamp, total;
 };
-__host__ __device__ inline RouterSmemLayout router_smem_layout(int n_deps, int n_groups, int n_fb) {
+// `latency`: the latency-based strategy's arrays follow the common ones (zero bytes for every other strategy)
+__host__ __device__ inline RouterSmemLayout router_smem_layout(int n_deps, int n_groups, int n_fb, bool latency) {
     RouterSmemLayout L;
     uint32_t off = 0;
     auto take = [&](uint32_t bytes) { uint32_t o = off; off += (bytes + 15u) & ~15u; return o; };
@@ -359,6 +439,8 @@ __host__ __device__ inline RouterSmemLayout router_smem_layout(int n_deps, int n
     L.o_rr = take(4 * n_groups); L.o_bs = take(4 * n_groups); L.o_bp = take(4 * n_groups);
     L.o_mt = take(4 * 624);
     L.o_ev = take(sizeof(rr_event) * RT_CHUNK); L.o_dec = take(sizeof(rr_decision) * RT_CHUNK);
+    const int ld = latency ? n_deps : 0, lg = latency ? n_groups : 0;
+    L.o_lat_n = take(4 * ld); L.o_lat_head = take(8 * ld); L.o_lat_last = take(8 * ld); L.o_lat_stamp = take(8 * lg);
     L.total = off;
     return L;
 }
@@ -368,11 +450,13 @@ __device__ __forceinline__ void warp_copy(T* dst, const T* src, int n) {
     for (int i = threadIdx.x; i < n; i += 32) dst[i] = src[i];
 }
 
+template <bool LAT>
 __global__ void __launch_bounds__(32, 1)
 router_kernel_smem(RouterDev G, int n_fb, const rr_event* __restrict__ events, int n_events,
                    rr_decision* __restrict__ decisions) {
     extern __shared__ __align__(16) uint8_t rt_smem[];
-    const RouterSmemLayout L = router_smem_layout(G.n_deps, G.n_groups, n_fb);
+    constexpr bool lat = LAT;
+    const RouterSmemLayout L = router_smem_layout(G.n_deps, G.n_groups, n_fb, lat);
     const int lane = threadIdx.x, nd = G.n_deps, ng = G.n_groups;
     RouterDev S = G;                                       // same scalars, pointers redirected into shared memory
     long long* window = (long long*)(rt_smem + L.o_window); long long* failw = (long long*)(rt_smem + L.o_failw);
@@ -400,6 +484,12 @@ router_kernel_smem(RouterDev G, int n_fb, const rr_event* __restrict__ events, i
     S.req_count = req; S.tok_count = tok; S.fail_count = failc; S.inflight = infl;
     S.rpm = rpm; S.tpm = tpm; S.weight = wt; S.dep_group = dgrp; S.group_deps = gdeps; S.group_off = goff;
     S.fb_off = fboff; S.fb_groups = fbg; S.rr_next = rrn; S.burst_size = bs; S.burst_pos = bp;
+    if (lat) {
+        S.lat_n = (int*)(rt_smem + L.o_lat_n); S.lat_head = (double*)(rt_smem + L.o_lat_head);
+        S.lat_last = (double*)(rt_smem + L.o_lat_last); S.lat_stamp = (long long*)(rt_smem + L.o_lat_stamp);
+        warp_copy(S.lat_n, (const int*)G.lat_n, nd); warp_copy(S.lat_head, (const double*)G.lat_head, nd);
+        warp_copy(S.lat_last, (const double*)G.lat_last, nd); warp_copy(S.lat_stamp, (const long long*)G.lat_stamp, ng);
+    }
     WarpMT rng;
     rng.mt = s_mt;
     rng.mti = (int)G.mt[624];
@@ -410,7 +500,7 @@ router_kernel_smem(RouterDev G, int n_fb, const rr_event* __restrict__ events, i
         const int n = min(RT_CHUNK, n_events - base);
         warp_copy((uint32_t*)s_ev, (const uint32_t*)(events + base), n * EW);
         __syncwarp();
-        run_trace<true>(S, rng, s_ev, n, s_dec);
+        run_trace<true, LAT>(S, rng, s_ev, n, s_dec);
         warp_copy((uint32_t*)(decisions + base), (const uint32_t*)s_dec, n * DW);
         __syncwarp();
     }
@@ -421,6 +511,10 @@ router_kernel_smem(RouterDev G, int n_fb, const rr_event* __restrict__ events, i
     warp_copy(G.fail_count, (const int*)failc, nd); warp_copy(G.inflight, (const int*)infl, nd);
     warp_copy(G.rr_next, (const int*)rrn, ng); warp_copy(G.burst_size, (const int*)bs, ng); warp_copy(G.burst_pos, (const int*)bp, ng);
     warp_copy(G.mt, (const uint32_t*)s_mt, 624);
+    if (lat) {
+        warp_copy(G.lat_n, (const int*)S.lat_n, nd); warp_copy(G.lat_head, (const double*)S.lat_head, nd);
+        warp_copy(G.lat_last, (const double*)S.lat_last, nd); warp_copy(G.lat_stamp, (const long long*)S.lat_stamp, ng);
+    }
     if (lane == 0) G.mt[624] = (uint32_t)rng.mti;
 }
 
@@ -499,7 +593,11 @@ RR_API int rr_router_create(const rr_deployment_desc* deps, int n_deps, int n_gr
                             const rr_router_settings* st, uint64_t seed, int device,
                             rr_router** out) {
     if (!deps || !st || !out || n_deps <= 0 || n_groups <= 0 || !fb_offsets) return RR_INVALID_ARGUMENT;
-    if (st->strategy < 0 || st->strategy > RR_STRATEGY_RANDOM) return RR_INVALID_ARGUMENT;
+    if (st->strategy < 0 || st->strategy > RR_STRATEGY_LATENCY_BASED) return RR_INVALID_ARGUMENT;
+    const int lat_cap = st->latency_list_size ? st->latency_list_size : 10;
+    const int lat_ttl = st->latency_ttl_ms ? st->latency_ttl_ms : 3600000;
+    if (lat_cap < 1 || lat_cap > 32 || st->latency_buffer_ppm < 0 || lat_ttl < 0) return RR_INVALID_ARGUMENT;
+    const bool lat = st->strategy == RR_STRATEGY_LATENCY_BASED;
     std::vector<int32_t> goff(n_groups + 1, 0), gdeps(n_deps), dgrp(n_deps), rpm(n_deps), tpm(n_deps), wt(n_deps);
     for (int i = 0; i < n_deps; ++i) {
         if (deps[i].group < 0 || deps[i].group >= n_groups) return RR_INVALID_ARGUMENT;
@@ -540,6 +638,9 @@ RR_API int rr_router_create(const rr_deployment_desc* deps, int n_deps, int n_gr
            o_fboff = take(4 * (n_groups + 1)), o_fbg = take(4 * (n_fb > 0 ? n_fb : 1)),
            o_dgrp = take(4 * n_deps), o_rpm = take(4 * n_deps), o_tpm = take(4 * n_deps),
            o_wt = take(4 * n_deps);
+    const int lat_d = lat ? n_deps : 0, lat_g = lat ? n_groups : 0;   // latency state: latency-based routers only
+    size_t o_lat_n = take(4 * lat_d), o_lat_head = take(8 * lat_d), o_lat_last = take(8 * lat_d),
+           o_lat_stamp = take(8 * lat_g);
     cudaError_t e = cudaMalloc(&r->arena, off);
     if (e != cudaSuccess) { rr::note_cuda_error(e); delete r; return RR_CUDA_ERROR; }
     char* base = (char*)r->arena;
@@ -548,6 +649,8 @@ RR_API int rr_router_create(const rr_deployment_desc* deps, int n_deps, int n_gr
         long long* w = (long long*)(host.data() + o_window);
         long long* fw = (long long*)(host.data() + o_failw);
         for (int i = 0; i < n_deps; ++i) { w[i] = -1; fw[i] = -1; }
+        long long* ls = (long long*)(host.data() + o_lat_stamp);
+        for (int g = 0; g < lat_g; ++g) ls[g] = -1;
         mt_seed_like_cpython(seed, (uint32_t*)(host.data() + o_mt));
         memcpy(host.data() + o_goff, goff.data(), 4 * (n_groups + 1));
         memcpy(host.data() + o_gdeps, gdeps.data(), 4 * n_deps);
@@ -576,6 +679,12 @@ RR_API int rr_router_create(const rr_deployment_desc* deps, int n_deps, int n_gr
     D.cooldown_until = (long long*)(base + o_cool); D.total_admitted = (long long*)(base + o_total);
     D.rr_next = (int*)(base + o_rr); D.mt = (uint32_t*)(base + o_mt);
     D.burst_size = (int*)(base + o_bs); D.burst_pos = (int*)(base + o_bp);
+    D.lat_cap = lat_cap; D.lat_ttl_ms = lat_ttl;
+    D.lat_buf = (double)st->latency_buffer_ppm / 1e6;
+    if (lat) {
+        D.lat_n = (int*)(base + o_lat_n); D.lat_head = (double*)(base + o_lat_head);
+        D.lat_last = (double*)(base + o_lat_last); D.lat_stamp = (long long*)(base + o_lat_stamp);
+    }
 
     e = cudaStreamCreateWithFlags(&r->stream, cudaStreamNonBlocking);
     if (e != cudaSuccess) { rr::note_cuda_error(e); cudaFree(r->arena); delete r; return RR_CUDA_ERROR; }
@@ -584,12 +693,13 @@ RR_API int rr_router_create(const rr_deployment_desc* deps, int n_deps, int n_gr
     r->n_fb = n_fb;
     r->smem_bytes = 0;
     {
-        const RouterSmemLayout L = router_smem_layout(n_deps, n_groups, n_fb);
+        const RouterSmemLayout L = router_smem_layout(n_deps, n_groups, n_fb, lat);
         // The attribute is per function AND per device: raise it once per device to the cap every router may need (a later,
         // smaller router must not lower it under an earlier one); a launch then only states its own size.
-        static std::atomic<uint64_t> attr_set{0};
+        static std::atomic<uint64_t> attr_set{0}, attr_set_lat{0};
         if (L.total <= 200 * 1024 && !getenv("RR_ROUTER_GLOBAL_STATE") &&
-            rr::ensure_dyn_smem(router_kernel_smem, 200 * 1024, attr_set) == cudaSuccess)
+            (lat ? rr::ensure_dyn_smem(router_kernel_smem<true>, 200 * 1024, attr_set_lat)
+                 : rr::ensure_dyn_smem(router_kernel_smem<false>, 200 * 1024, attr_set)) == cudaSuccess)
             r->smem_bytes = (int)L.total;
     }
     int rc = ensure_cap(r, 1024);
@@ -608,6 +718,7 @@ int router_shape(const rr_router* r, int* n_deployments, int* n_groups) {
 int router_dep_replica(const rr_router* r, int deployment) {
     return (r && deployment >= 0 && deployment < r->n_deps) ? r->replica[deployment] : -1;
 }
+int router_strategy(const rr_router* r) { return r ? r->dev.strategy : -1; }
 }  // namespace rr
 
 RR_API void rr_router_destroy(rr_router* r) {
@@ -633,10 +744,15 @@ RR_API int rr_router_process_device(rr_router* r, const rr_event* d_events, int 
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e = cudaStreamWaitEvent(st, r->last, 0);
     if (e != cudaSuccess) { rr::note_cuda_error(e); return RR_CUDA_ERROR; }
-    if (r->smem_bytes > 0)
-        router_kernel_smem<<<1, 32, r->smem_bytes, st>>>(r->dev, r->n_fb, d_events, n_events, d_decisions);
+    const bool lat = r->dev.strategy == RR_STRATEGY_LATENCY_BASED;
+    if (r->smem_bytes > 0 && lat)
+        router_kernel_smem<true><<<1, 32, r->smem_bytes, st>>>(r->dev, r->n_fb, d_events, n_events, d_decisions);
+    else if (r->smem_bytes > 0)
+        router_kernel_smem<false><<<1, 32, r->smem_bytes, st>>>(r->dev, r->n_fb, d_events, n_events, d_decisions);
+    else if (lat)
+        router_kernel<true><<<1, 32, 0, st>>>(r->dev, d_events, n_events, d_decisions);
     else
-        router_kernel<<<1, 32, 0, st>>>(r->dev, d_events, n_events, d_decisions);
+        router_kernel<false><<<1, 32, 0, st>>>(r->dev, d_events, n_events, d_decisions);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaEventRecord(r->last, st);
     if (e != cudaSuccess) { rr::note_cuda_error(e); return RR_CUDA_ERROR; }
@@ -681,6 +797,29 @@ RR_API int rr_router_snapshot(rr_router* r, rr_deployment_state* out) {
         out[i].window = w[i]; out[i].req_count = rq[i]; out[i].tok_count = tk[i];
         out[i].fail_window = fw[i]; out[i].fail_count = fc[i]; out[i].inflight = inf[i];
         out[i].cooldown_until_ms = cu[i]; out[i].total_admitted = tot[i];
+    }
+    return RR_OK;
+}
+
+RR_API int rr_router_latency_snapshot(rr_router* r, double* mean_out, int32_t* n_samples_out) {
+    if (!r || !mean_out || !n_samples_out) return RR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> lk(r->mu);
+    const int n = r->n_deps;
+    if (!r->dev.lat_n) {
+        for (int i = 0; i < n; ++i) { mean_out[i] = 0.0; n_samples_out[i] = 0; }
+        return RR_OK;
+    }
+    CK(cudaSetDevice(r->device));
+    CK(cudaStreamSynchronize(r->stream));
+    std::vector<int> cnt(n);
+    std::vector<double> head(n), last(n);
+    CK(cudaMemcpy(cnt.data(), r->dev.lat_n, 4 * n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(head.data(), r->dev.lat_head, 8 * n, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(last.data(), r->dev.lat_last, 8 * n, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n; ++i) {   // the kernel's mean: total / len, total = head (+ last once the list is full)
+        const double tot = cnt[i] < r->dev.lat_cap ? head[i] : head[i] + last[i];
+        mean_out[i] = cnt[i] > 0 ? tot / (double)cnt[i] : 0.0;
+        n_samples_out[i] = cnt[i];
     }
     return RR_OK;
 }

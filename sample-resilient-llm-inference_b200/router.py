@@ -197,12 +197,13 @@ class Router:
     def __init__(self, model_list: Optional[List[dict]] = None, *, routing_strategy: str = "simple-shuffle",
                  enable_pre_call_checks: bool = False, allowed_fails: Optional[int] = None,
                  cooldown_time: Optional[float] = None, fallbacks: Optional[List[dict]] = None,
+                 routing_strategy_args: Optional[dict] = None,
                  config: Optional[RouterConfig] = None, backends: Optional[Dict[int, Any]] = None,
                  seed: int = 0, device: int = 0, clock: Optional[Callable[[], float]] = None,
                  default_max_tokens: int = 128):
         if config is None:
             rs = {"routing_strategy": routing_strategy, "enable_pre_call_checks": enable_pre_call_checks,
-                  "fallbacks": fallbacks or []}
+                  "fallbacks": fallbacks or [], "routing_strategy_args": routing_strategy_args}
             if allowed_fails is not None:
                 rs["allowed_fails"] = allowed_fails
             if cooldown_time is not None:
@@ -229,7 +230,9 @@ class Router:
             flat += config.fallbacks.get(g, [])
             offs.append(len(flat))
         st = _lib.RouterSettings(config.strategy_id, int(config.enable_pre_call_checks), config.allowed_fails,
-                                 int(round(config.cooldown_time * 1000)), 0)
+                                 int(round(config.cooldown_time * 1000)), 0, config.latency_list_size,
+                                 config.latency_buffer_ppm, config.latency_ttl_ms)
+        self._latency = config.routing_strategy == "latency-based-routing"
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_router_create(arr, len(deps), ng, (C.c_int32 * len(offs))(*offs),
                                              (C.c_int32 * max(1, len(flat)))(*flat), C.byref(st), seed, device,
@@ -435,6 +438,25 @@ class Router:
         _lib.check(_lib.lib.rr_router_snapshot(self._h, s), "rr_router_snapshot")
         return [{k: getattr(x, k) for k, _ in x._fields_} for x in s]
 
+    def latency_snapshot(self) -> List[Tuple[float, int]]:
+        """latency-based-routing: [(mean latency in us per output token, samples held)] per deployment, as stored
+        (a group whose ttl ran out is cleared at its next write or pick).  All (0.0, 0) under the other strategies."""
+        self._quiesce()
+        n = len(self.cfg.deployments)
+        mean, cnt = (C.c_double * n)(), (C.c_int32 * n)()
+        _lib.check(_lib.lib.rr_router_latency_snapshot(self._h, mean, cnt), "rr_router_latency_snapshot")
+        return list(zip(mean, cnt))
+
+    def _done_aux(self, latency_s: float) -> int:
+        """4th field of a DONE event: the request's latency in us (latency-based-routing only; 0 = no sample)."""
+        if not self._latency:
+            return 0
+        return min(max(int(round(latency_s * 1e6)), 1), 2**31 - 1)
+
+    def _fail_aux(self, timed_out: bool) -> int:
+        """4th field of a FAIL event: 1 = the request timed out (latency-based-routing records the penalty)."""
+        return 1 if self._latency and timed_out else 0
+
     # ---- request path ---------------------------------------------------------------------------
     def _backend_for(self, dep_index: int):
         d = self.cfg.deployments[dep_index]
@@ -479,7 +501,7 @@ class Router:
                 self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
                 raise exc if isinstance(exc, APIError) else APIError(f"backend error on deployment {dep}: {exc}")
             if st == 0:
-                self.process([(EV_DONE, dep, len(toks), 0, self.now_ms())])
+                self.process([(EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms())])
                 d = self.cfg.deployments[dep]
                 return ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
@@ -488,7 +510,7 @@ class Router:
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg],
                     _fell_back=pos > 0, _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
             # backend failed / timed out: report, then walk on down the fallback chain
-            self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
+            self.process([(EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms())])
             if st == 6:
                 raise APITimeoutError(f"Request timed out after {timeout}s")
             last_err = APIError(f"backend failure on deployment {dep} ({self.cfg.deployments[dep].model})")
@@ -517,7 +539,7 @@ class Router:
                 raise RateLimitError(f"No deployments available for selected model, passed model={model} (rate limited)")
             if status != 0:
                 raise BadRequestError(f"Invalid model name passed in model={model}")
-            sent, failed, settled = 0, False, False
+            sent, failed, settled, timed_out = 0, False, False, False
             try:
                 backend = self._backend_for(dep)
                 label = self.cfg.deployments[dep].response_model
@@ -528,19 +550,24 @@ class Router:
                         yield label, toks[sent:], False, ttft
                         sent = len(toks)
                     if done:
-                        st, toks, ttft, _lat = backend.wait(h, timeout)
+                        st, toks, ttft, lat = backend.wait(h, timeout)
                         failed = st != 0
+                        timed_out = st == 6
                         break
                     if deadline is not None and time.perf_counter() > deadline:
+                        timed_out = True
                         raise APITimeoutError(f"Request timed out after {timeout}s")
                 if not failed:
-                    self.process([(EV_DONE, dep, sent, 0, self.now_ms())])
+                    self.process([(EV_DONE, dep, sent, self._done_aux(lat), self.now_ms())])
                     settled = True
                     yield label, [], True, ttft
                     return
             finally:
                 if not settled:          # failure, timeout, or the consumer closed the generator: release the slot
-                    self.process([(EV_FAIL if failed or sent == 0 else EV_DONE, dep, sent, 0, self.now_ms())])
+                    if failed or sent == 0:
+                        self.process([(EV_FAIL, dep, sent, self._fail_aux(timed_out), self.now_ms())])
+                    else:
+                        self.process([(EV_DONE, dep, sent, 0, self.now_ms())])
             if sent > 0:
                 raise APIError(f"backend failure on deployment {dep} after {sent} tokens")
             chain_start = pos + 1
@@ -581,7 +608,7 @@ class Router:
             status, dep, sg, pos = dec[i]
             st, toks, ttft, lat = b.wait(hd, timeout)
             if st == 0:
-                post.append((EV_DONE, dep, len(toks), 0, self.now_ms()))
+                post.append((EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms()))
                 d = self.cfg.deployments[dep]
                 out[i] = ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
@@ -590,7 +617,7 @@ class Router:
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
                     _ttft_s=ttft, _latency_s=time.perf_counter() - t0)
             else:
-                post.append((EV_FAIL, dep, 0, 0, self.now_ms()))
+                post.append((EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms()))
                 retry.append((i, pos + 1))
         self.process(post)
         for i, chain_start in retry:          # failed requests walk the fallback chain one by one
@@ -609,7 +636,7 @@ class Router:
             b = self._backend_for(dep)
             st, toks, ttft, lat = b.wait(b.submit(prompt_ids, max_new), timeout)
             if st == 0:
-                self.process([(EV_DONE, dep, len(toks), 0, self.now_ms())])
+                self.process([(EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms())])
                 d = self.cfg.deployments[dep]
                 return ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
@@ -617,7 +644,7 @@ class Router:
                     usage=Usage(len(prompt_ids), len(toks), len(prompt_ids) + len(toks)), created=int(time.time()),
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
                     _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
-            self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
+            self.process([(EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms())])
             chain_start = pos + 1
 
 

@@ -117,6 +117,10 @@ def create_app(router: Router):
     @app.get("/router/state")
     async def state():
         snap = await run_in_threadpool(router.snapshot)
+        if router.cfg.routing_strategy == "latency-based-routing":
+            lat = await run_in_threadpool(router.latency_snapshot)
+            for s, (mean, n) in zip(snap, lat):
+                s.update(latency_us_per_token=mean, latency_samples=n)
         return {"deployments": [dict(model_name=d.model_name, model=d.response_model, gpu=d.gpu, rpm=d.rpm,
                                      tpm=d.tpm, **s) for d, s in zip(router.cfg.deployments, snap)]}
 
