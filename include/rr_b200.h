@@ -223,6 +223,16 @@ int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, v
 int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                        const int32_t* seq_start, const int32_t* seq_slot, int n_seqs, int max_len,
                        int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream);
+/* Fused decode MLP, one launch exactly as the engine runs it for a batch of `rows` (tile width, K slices, grid and
+ * schedule from the engine's rules; env RR_MLP_STATIC / RR_NO_TMA_EPI are read per call):
+ *   act[b, n]       = bf16(SiLU(xn[b] . gate[n]) * (xn[b] . up[n]))                        bf16 [rows, inter]
+ *   planes[z][b][h] = sum over k in slice z of act[b, k] * wdown[h, k]                       fp32 [n_slices][ld_rows][hidden]
+ * Slice z covers the k-blocks (64 act columns each) [z * slice_kb, min((z + 1) * slice_kb, inter / 64)); the sum of the
+ * planes is the down projection.  Plane rows >= rows are not written.  wgu_il = [gate; up] rows interleaved in 64-row
+ * blocks [2*inter, hidden].  Returns RR_INVALID_ARGUMENT before touching the device unless 17 <= rows <= 128,
+ * ld_rows >= rows, hidden and inter are positive multiples of 64, hidden <= 8192 and no pointer is null. */
+int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
+                     void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream);
 
 /* ================================================================================================
  * 4. Engine: one model replica on one GPU (prefill + continuous-batching greedy decode).

@@ -154,6 +154,7 @@ PROTOTYPES = {
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp]),
+    "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_engine_create": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(ModelWeights),
                                    C.POINTER(EngineOpts), C.POINTER(vp)]),
     "rr_engine_destroy": (None, [vp]),

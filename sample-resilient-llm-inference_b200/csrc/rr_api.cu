@@ -220,6 +220,44 @@ RR_API int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_c
     return check_last();
 }
 
+// The fused decode MLP as the engine runs it (rr_engine_create): tile width, K slices, grid and schedule come from the same
+// helpers and environment switches; the schedule and the dependency counters live in stream-ordered scratch memory.
+RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
+                            void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream) {
+    if (!wgu_il || !wdown || !xn || !act || !planes || !n_slices || !slice_kb) return RR_INVALID_ARGUMENT;
+    // the engine fuses the MLP for batches of 17..MAX_BN rows (tile width >= 32, one batch tile)
+    if (rows <= 16 || rows > MAX_BN || ld_rows < rows) return RR_INVALID_ARGUMENT;
+    if (hidden < 64 || hidden % 64 || hidden > 8192 || inter < 64 || inter % 64) return RR_INVALID_ARGUMENT;
+    int skb = 0;
+    const int ns = mlp_slices(inter, &skb);
+    const int grid = num_sms();
+    const int dyn = getenv("RR_MLP_STATIC") ? 0 : 1;
+    std::vector<MlpItem> sched;
+    const int max_items = mlp_schedule(grid, inter, hidden, skb, &sched, dyn);
+    cudaStream_t st = (cudaStream_t)stream;
+    MlpItem* items = nullptr;
+    unsigned* ready = nullptr;
+    cudaError_t e = cudaMallocAsync(&items, sched.size() * sizeof(MlpItem), st);
+    if (e == cudaSuccess) e = cudaMallocAsync(&ready, (size_t)(ns + 1) * sizeof(unsigned), st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(items, sched.data(), sched.size() * sizeof(MlpItem), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ready, 0, (size_t)(ns + 1) * sizeof(unsigned), st);
+    int rc = RR_CUDA_ERROR;
+    if (e == cudaSuccess) {
+        MlpPlan p;
+        rc = mlp_plan_init(&p, wgu_il, wdown, inter, hidden, xn, rows, act, planes, ld_rows, pick_bn(rows), items, max_items,
+                           grid, ready, skb, dyn);
+        if (rc == RR_OK) rc = mlp_launch(p, st);
+    }
+    if (e != cudaSuccess) note_cuda_error(e);
+    else if (rc != RR_OK) note_cuda_error(cudaPeekAtLastError());
+    if (items) cudaFreeAsync(items, st);
+    if (ready) cudaFreeAsync(ready, st);
+    if (rc != RR_OK) return rc;
+    *n_slices = ns;
+    *slice_kb = skb;
+    return check_last();
+}
+
 RR_API int rr_debug_mlp_schedule(int grid, int inter, int hidden, int slice_kb, int32_t* items_out, int capacity,
                                  int* max_items) {
     if (grid < 1 || inter < 64 || inter % 64 || hidden < 8 || slice_kb < 1 || !max_items) return RR_INVALID_ARGUMENT;

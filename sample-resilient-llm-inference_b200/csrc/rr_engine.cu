@@ -199,12 +199,6 @@ static int dalloc(rr_engine* e, T** p, size_t n, bool zero = true) {
 // sum(x^2) partial per 128 columns, two per 256-wide tile.
 constexpr int PF_BN = MAX_BN;
 
-// Decode tile width along the batch rows; batches wider than MAX_BN run several B tiles per weight tile.
-static int pick_bn(int rows) {
-    const int opts[4] = {16, 32, 64, MAX_BN};
-    for (int b : opts) if (rows <= b) return b;
-    return MAX_BN;
-}
 static int pick_splits(int N, int K) {
     const int tilesA = (N + 127) / 128;
     int s = num_sms() / tilesA;
@@ -673,14 +667,10 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->part_qkv, (size_t)e->s_qkv * B * e->nqkv));
     TRY(dalloc(e, &e->part_o, (size_t)e->s_o * B * d.hidden));
     TRY(dalloc(e, &e->part_gu, (size_t)e->s_gu * B * 2 * d.inter));
-    // fused decode MLP: the down GEMM's K range in <= 8 slices (one output plane each); 8 x 28 k-blocks for
-    // Llama-3-8B balances the per-CTA lists to within 5 % (see mlp_schedule)
+    // fused decode MLP: the down GEMM's K range in <= 8 slices, one output plane each (mlp_slices)
     {
         const int kb1n = d.inter / 64;
-        int n_sl = (kb1n + 15) / 16;
-        n_sl = n_sl > 8 ? 8 : (n_sl < 1 ? 1 : n_sl);
-        e->mlp_slice_kb = (kb1n + n_sl - 1) / n_sl;
-        n_sl = (kb1n + e->mlp_slice_kb - 1) / e->mlp_slice_kb;
+        const int n_sl = mlp_slices(d.inter, &e->mlp_slice_kb);
         e->fuse_mlp = e->fuse_silu && e->Bm <= e->bn_dec && opts->reserved[2] == 0 && d.inter % 64 == 0 && kb1n >= 1 && !getenv("RR_NO_MLP_FUSE");
         e->mlp_slices = e->fuse_mlp ? n_sl : 0;
     }

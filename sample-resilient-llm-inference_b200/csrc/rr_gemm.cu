@@ -974,7 +974,22 @@ int gemm_launch(const GemmPlan& p, cudaStream_t st) {
 }
 
 
+int pick_bn(int rows) {
+    const int opts[4] = {16, 32, 64, MAX_BN};
+    for (int b : opts) if (rows <= b) return b;
+    return MAX_BN;
+}
+
 // ---- fused decode MLP: host side ------------------------------------------------------------------
+int mlp_slices(int inter, int* slice_kb) {
+    const int kb1n = inter / BLOCK_K;
+    if (kb1n < 1) { *slice_kb = 0; return 0; }
+    int n_sl = (kb1n + 15) / 16;
+    n_sl = n_sl > 8 ? 8 : n_sl;
+    *slice_kb = (kb1n + n_sl - 1) / n_sl;
+    return (kb1n + *slice_kb - 1) / *slice_kb;
+}
+
 // List schedule on a time line in units of k-blocks (one 16 KB weight tile at a CTA's fair share of the HBM rate, 0.37 us;
 // + a fixed per-item cost for pipeline refill / epilogue).  Gate/up tile t goes to CTA t % grid (wave order: tile t is
 // finished before tile t + grid).  A slice becomes READY kPublish units after its last gate/up tile finished its mainloop --

@@ -100,6 +100,13 @@ struct MlpPlan {
     MlpArgs args;
     int grid, bn, n_slices;
 };
+// Decode tile width along the batch rows: the narrowest of 16 / 32 / 64 / MAX_BN that holds `rows`; wider batches run
+// several MAX_BN tiles per weight tile.
+int pick_bn(int rows);
+// K slices of the fused MLP's down GEMM: its inter / 64 k-blocks in at most 8 slices of about 16 (one output plane each;
+// 8 x 28 k-blocks for Llama-3-8B balances the per-CTA lists to within 5 %, see mlp_schedule).  Sets *slice_kb and
+// returns the number of slices (0 when inter < 64).
+int mlp_slices(int inter, int* slice_kb);
 // Host schedule: `items` gets grid * max_items entries (CTA-major); returns max_items.
 int mlp_schedule(int grid, int inter, int hidden, int slice_kb, std::vector<MlpItem>* items, int dynamic = 0);
 int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hidden, const void* xn, int rows,

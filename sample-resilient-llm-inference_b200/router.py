@@ -282,8 +282,10 @@ class Router:
         return {k: getattr(s, k) for k, _ in s._fields_}
 
     def gateway_trace(self) -> List[Tuple[Tuple[int, int, int, int, int], Tuple[int, int, int, int]]]:
-        """[(event, decision)] recorded by the gateway (record_trace > 0), oldest first: the serialised trace K1 processed."""
+        """[(event, decision)] recorded by the gateway (record_trace > 0), oldest first: the serialised trace K1 processed.
+        Like the snapshots, it waits for the DONE / FAIL reports of finished requests, so it matches the state read after it."""
         gw = self._gateway()
+        self._quiesce()
         n = C.c_int32()
         if gw is None or _lib.lib.rr_gateway_trace(gw, None, None, 0, C.byref(n)) not in (0, 4) or n.value == 0:
             return []

@@ -61,6 +61,15 @@ def test_version_and_errors():
     assert b"429" in _lib.lib.rr_strerror(1)
 
 
+def test_decode_mlp_entry_point_validates_before_touching_the_device():
+    """rr_op_decode_mlp rejects null pointers with RR_INVALID_ARGUMENT before it touches the device (so this passes without
+    one) and leaves its out values alone."""
+    from rr_b200 import _lib
+    ns, skb = C.c_int32(-1), C.c_int32(-1)
+    rc = _lib.lib.rr_op_decode_mlp(None, None, None, 64, 4096, 14336, None, None, 64, C.byref(ns), C.byref(skb), None)
+    assert rc == 4 and (ns.value, skb.value) == (-1, -1)
+
+
 @pytest.mark.parametrize("grid,inter,hidden,slice_kb", [(148, 14336, 4096, 28), (148, 8192, 3072, 16), (132, 2816, 1024, 15),
                                                         (148, 1024, 512, 16), (7, 14336, 4096, 28)])
 def test_fused_mlp_schedule_is_a_partition_and_deadlock_free(grid, inter, hidden, slice_kb):

@@ -30,15 +30,19 @@ def test_embed_and_rmsnorm_splitk_reduce():
     ref = table[ids.long()].float(); ref[5] = 0
     assert torch.equal(x, ref)
 
-    parts = torch.randn(3, rows, hidden, device=DEV, generator=g)
     w = (1 + 0.1 * torch.randn(hidden, device=DEV, generator=g)).bfloat16()
     xn = torch.empty(rows, hidden, device=DEV, dtype=torch.bfloat16)
-    x0 = x.clone()
-    lib.check(lib.lib.rr_op_add_rmsnorm(P(x), P(parts), 0, 3, rows * hidden, hidden, P(w), P(xn), rows, hidden, 1e-5, None))
-    xr = x0 + parts.sum(0)
-    assert torch.allclose(x, xr, atol=1e-5, rtol=1e-5)
-    nr = xr * torch.rsqrt(xr.pow(2).mean(-1, keepdim=True) + 1e-5) * w.float()
-    assert torch.allclose(xn.float(), nr, atol=2e-2, rtol=1e-2)          # one bf16 rounding
+    # fp32 split-K planes summed into the residual; 8 is the fused decode MLP's plane count for Llama-3-8B / Phi-3 and the
+    # most add_rmsnorm_dec_kernel takes
+    for n_splits in (1, 3, 8):
+        parts = torch.randn(n_splits, rows, hidden, device=DEV, generator=g)
+        xs = x.clone()
+        lib.check(lib.lib.rr_op_add_rmsnorm(P(xs), P(parts), 0, n_splits, rows * hidden, hidden, P(w), P(xn), rows, hidden,
+                                            1e-5, None))
+        xr = x + parts.sum(0)
+        assert torch.allclose(xs, xr, atol=1e-5, rtol=1e-5), n_splits
+        nr = xr * torch.rsqrt(xr.pow(2).mean(-1, keepdim=True) + 1e-5) * w.float()
+        assert torch.allclose(xn.float(), nr, atol=2e-2, rtol=1e-2), n_splits      # one bf16 rounding
     # bf16 "part" (prefill orientation) and norm-only (no part)
     pb = torch.randn(rows, hidden, device=DEV, generator=g).bfloat16()
     x1 = xr.clone()
