@@ -233,6 +233,20 @@ int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_cache, 
  * ld_rows >= rows, hidden and inter are positive multiples of 64, hidden <= 8192 and no pointer is null. */
 int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
                      void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream);
+/* Decode attention, one step exactly as the engine runs it: RoPE and the KV append fused in, scale 1 / sqrt(head_dim), the
+ * engine's kv-split rule (returned in *kv_splits) and RoPE table (theta); env RR_ATTN_NO_TRIM is read per call.
+ *   qkv      fp32 split-K planes [n_splits][..][ld], plane z of row b at qkv + z * split_stride + b * ld; columns are the
+ *            q heads, then the k heads, then the v heads, head_dim each (unpadded); q / k / v = the sum of the planes
+ *   k_cache, v_cache  bf16 [n_slots][n_kv_heads][ctx_max][128]; row b (slot[b] >= 0) appends its rotated k and its v at
+ *            position pos[b] of slot[b] (columns [0, head_dim)) and attends over positions 0..pos[b]; rows with
+ *            slot[b] < 0 are skipped
+ *   out      bf16 [rows][n_heads * head_dim]
+ * Returns RR_INVALID_ARGUMENT before touching the device, *kv_splits unchanged, unless no pointer is null, rows >= 1,
+ * n_slots >= 1, n_splits >= 1, n_heads / n_kv_heads is 1, 2, 4 or 8, head_dim is a multiple of 16 in 64..128, ctx_max is
+ * a positive multiple of 64, ld >= (n_heads + 2 * n_kv_heads) * head_dim and ld and split_stride are even. */
+int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache, void* v_cache,
+                          void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads, int n_kv_heads,
+                          int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits, void* stream);
 
 /* ================================================================================================
  * 4. Engine: one model replica on one GPU (prefill + continuous-batching greedy decode).

@@ -155,6 +155,8 @@ PROTOTYPES = {
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
+    "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
+                                        C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp]),
     "rr_engine_create": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(ModelWeights),
                                    C.POINTER(EngineOpts), C.POINTER(vp)]),
     "rr_engine_destroy": (None, [vp]),

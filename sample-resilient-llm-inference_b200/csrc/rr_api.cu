@@ -220,6 +220,48 @@ RR_API int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_c
     return check_last();
 }
 
+// Decode attention as the engine runs it (rr_engine_create): RoPE and the KV append fused in, q / k / v summed from the QKV
+// GEMM's fp32 split-K planes, the engine's scale, kv-split rule and RoPE table; RR_ATTN_NO_TRIM is read per call.  The
+// table and the split-KV workspace live in stream-ordered scratch memory.
+RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                 void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads,
+                                 int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
+                                 void* stream) {
+    if (!qkv || !k_cache || !v_cache || !out || !slot || !pos || !kv_splits) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || n_slots < 1 || n_splits < 1) return RR_INVALID_ARGUMENT;
+    if (n_kv_heads <= 0 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
+    const int G = n_heads / n_kv_heads;
+    if (!(G == 1 || G == 2 || G == 4 || G == 8)) return RR_INVALID_ARGUMENT;
+    if (head_dim < 64 || head_dim > 128 || head_dim % 16 || ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
+    // the kernel reads the planes as float2
+    if (ld < (n_heads + 2 * n_kv_heads) * head_dim || ld % 2 || split_stride % 2) return RR_INVALID_ARGUMENT;
+    DecodeAttnArgs a;
+    a.q = nullptr; a.k_cache = (const __nv_bfloat16*)k_cache; a.v_cache = (const __nv_bfloat16*)v_cache;
+    a.out = (__nv_bfloat16*)out; a.slot = slot; a.pos = pos;
+    a.rows = rows; a.n_heads = n_heads; a.n_kv_heads = n_kv_heads; a.ctx_max = ctx_max;
+    a.scale = 1.0f / sqrtf((float)head_dim);
+    a.kv_splits = pick_kv_splits(rows, n_kv_heads); a.ws = nullptr;
+    a.fuse_rope = 1; a.qkv = mk_part(qkv, 0, n_splits, split_stride, ld); a.head_dim = head_dim;
+    { int rcm = decode_attn_make_maps(&a, n_slots); if (rcm != RR_OK) return rcm; }
+    cudaStream_t st = (cudaStream_t)stream;
+    float2* table = nullptr;
+    float* ws = nullptr;
+    cudaError_t e = cudaMallocAsync(&table, (size_t)ctx_max * 64 * sizeof(float2), st);
+    if (e == cudaSuccess && a.kv_splits > 1) e = cudaMallocAsync(&ws, decode_attn_ws_bytes(rows, n_heads, a.kv_splits), st);
+    if (e == cudaSuccess) {
+        launch_rope_table(table, ctx_max, theta, head_dim, st);
+        a.rope_table = table; a.ws = ws;
+        launch_decode_attn(a, st);
+    } else {
+        note_cuda_error(e);
+    }
+    if (table) cudaFreeAsync(table, st);
+    if (ws) cudaFreeAsync(ws, st);
+    if (e != cudaSuccess) return RR_CUDA_ERROR;
+    *kv_splits = a.kv_splits;
+    return check_last();
+}
+
 // The fused decode MLP as the engine runs it (rr_engine_create): tile width, K slices, grid and schedule come from the same
 // helpers and environment switches; the schedule and the dependency counters live in stream-ordered scratch memory.
 RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,

@@ -415,6 +415,12 @@ __global__ void decode_attn_combine_kernel(const float* __restrict__ ws, __nv_bf
     *reinterpret_cast<uint32_t*>(out + (size_t)row * n_heads * head_dim + head * head_dim + dp * 2) = pack_bf16(o0 * inv, o1 * inv);
 }
 
+int pick_kv_splits(int rows, int n_kv_heads) {
+    int ks = 1;
+    while (rows * n_kv_heads * ks < 2 * num_sms() && ks < 8) ks *= 2;
+    return ks;
+}
+
 size_t decode_attn_ws_bytes(int rows, int n_heads, int kv_splits) {
     return kv_splits > 1 ? (size_t)rows * n_heads * kv_splits * (HD + 2) * sizeof(float) : 0;
 }

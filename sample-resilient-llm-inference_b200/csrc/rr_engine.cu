@@ -683,9 +683,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->kcache, e->kv_layer_stride * L));
     TRY(dalloc(e, &e->vcache, e->kv_layer_stride * L));
     {   // split-KV only when the grid would not fill the GPU
-        int ctas = B * d.n_kv_heads;
-        int ks = 1;
-        while (ctas * ks < 2 * num_sms() && ks < 8) ks *= 2;
+        const int ks = pick_kv_splits(B, d.n_kv_heads);
         e->kv_splits = ks;
         e->attn_ws = nullptr;
         if (ks > 1) TRY(dalloc(e, &e->attn_ws, decode_attn_ws_bytes(B, d.n_heads, ks) / sizeof(float)));

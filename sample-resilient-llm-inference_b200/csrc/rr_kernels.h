@@ -107,6 +107,9 @@ int pick_bn(int rows);
 // 8 x 28 k-blocks for Llama-3-8B balances the per-CTA lists to within 5 %, see mlp_schedule).  Sets *slice_kb and
 // returns the number of slices (0 when inter < 64).
 int mlp_slices(int inter, int* slice_kb);
+// KV splits of decode attention (rr_attn_decode.cu): one CTA per (row, kv head) as long as that grid fills the GPU twice;
+// otherwise each row's KV range is split over 2, 4 or 8 CTAs, merged by decode_attn_combine_kernel.
+int pick_kv_splits(int rows, int n_kv_heads);
 // Host schedule: `items` gets grid * max_items entries (CTA-major); returns max_items.
 int mlp_schedule(int grid, int inter, int hidden, int slice_kb, std::vector<MlpItem>* items, int dynamic = 0);
 int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hidden, const void* xn, int rows,

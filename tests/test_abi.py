@@ -70,6 +70,16 @@ def test_decode_mlp_entry_point_validates_before_touching_the_device():
     assert rc == 4 and (ns.value, skb.value) == (-1, -1)
 
 
+def test_decode_attn_entry_point_validates_before_touching_the_device():
+    """rr_op_decode_attn_qkv rejects null pointers with RR_INVALID_ARGUMENT before it touches the device (so this passes
+    without one) and leaves *kv_splits alone."""
+    from rr_b200 import _lib
+    ks = C.c_int32(-1)
+    rc = _lib.lib.rr_op_decode_attn_qkv(None, 3, 64 * 6144, 6144, None, None, None, None, None, 64, 32, 8, 128, 4096, 64,
+                                        5e5, C.byref(ks), None)
+    assert rc == 4 and ks.value == -1
+
+
 @pytest.mark.parametrize("grid,inter,hidden,slice_kb", [(148, 14336, 4096, 28), (148, 8192, 3072, 16), (132, 2816, 1024, 15),
                                                         (148, 1024, 512, 16), (7, 14336, 4096, 28)])
 def test_fused_mlp_schedule_is_a_partition_and_deadlock_free(grid, inter, hidden, slice_kb):
