@@ -216,6 +216,16 @@ int rr_op_rope_kv(const void* qkv, int is_bf16, int n_splits, long long split_st
                   float theta, void* stream);
 int rr_op_argmax(const float* logits, int ld, int rows, int vocab, int32_t* out_tok,
                  float* out_val, const int32_t* row_active, int32_t* pos_inc, void* stream);
+/* Log-probabilities of the best tokens of fp32 logits rows (row r at logits + r * ld), as the engine computes them for
+ * `top_logprobs`: a row with top_n[r] >= 0 gets k = min(max(1, top_n[r]), max_top) entries, the k largest logits ordered by
+ * value descending then token id ascending (entry 0 is rr_op_argmax's token), lp_out[r][j] = x - logsumexp(row) in fp32
+ * and id_out[r][j] = the token id.
+ * lp_out fp32 / id_out int32 [rows][max_top]; row r gets k = min(max(1, top_n[r]), max_top) entries, the rest of its
+ * row and every row with top_n[r] < 0 untouched.  RR_INVALID_ARGUMENT before touching the device unless no pointer is
+ * null, 1 <= rows <= 65535, 1 <= vocab <= ld, vocab <= 524288, ld % 4 == 0 and 1 <= max_top <= 20.  Deterministic: every
+ * reduction runs in a fixed order. */
+int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top,
+                   float* lp_out, int32_t* id_out, void* stream);
 int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                       const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                       int n_kv_heads, int ctx_max /* % 64 == 0 */, int n_slots, float scale,
@@ -330,6 +340,20 @@ int rr_engine_cancel(rr_engine* e, uint64_t ticket);
  * copies the tokens generated so far.  Does not consume the request — finish with rr_engine_wait. */
 int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
                    int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s);
+/* Per-token log-probabilities (OpenAI `logprobs` / `top_logprobs`).  top_logprobs = -1: off (rr_engine_submit);
+ * 0..20: for every generated token the engine records K = max(1, top_logprobs) (logprob, token id) pairs, the K most
+ * likely tokens of that step ordered by logprob descending then id ascending (pair 0 is the greedy token), computed on
+ * the GPU from the same fp32 logits the greedy pick reads (rr_op_logprobs).  Tokens are the same as without logprobs.
+ * RR_INVALID_ARGUMENT for top_logprobs outside -1..20 (or >= 0 with a vocabulary that is not a multiple of 4).
+ * wait / peek behave like rr_engine_wait / rr_engine_peek and also fill lp_out / id_out [max_tokens_out][K] (either may be
+ * NULL; nothing is written for a request submitted with top_logprobs = -1). */
+int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                              int top_logprobs, uint64_t* ticket);
+int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                            int max_tokens_out, float* lp_out, int32_t* id_out);
+int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                            int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
+                            float* lp_out, int32_t* id_out);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -405,6 +429,16 @@ int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway
 /* Streaming: returns once more than `have` tokens exist, the request is finished, or timeout_s elapsed. */
 int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
                     int32_t* n_generated, int32_t* done, rr_gateway_result* out);
+/* The same with per-token log-probabilities (rr_engine_submit_logprobs): top_logprobs -1..20 travels with the request,
+ * a fallback re-admission included; wait / peek also fill lp_out / id_out [max_tokens_out][max(1, top_logprobs)].  The
+ * admission trace is the same as rr_gateway_submit's. */
+int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                               int top_logprobs, uint64_t* ticket);
+int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                             int max_tokens_out, float* lp_out, int32_t* id_out);
+int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                             int max_tokens_out, int32_t* n_generated, int32_t* done, rr_gateway_result* out,
+                             float* lp_out, int32_t* id_out);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

@@ -195,7 +195,23 @@ RR_API int rr_op_argmax(const float* logits, int ld, int rows, int vocab, int32_
     return check_last();
 }
 
-RR_API int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
+// Log-softmax + top-k as the engine runs it after the argmax; the chunk workspace is stream-ordered scratch memory.
+RR_API int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top,
+                          float* lp_out, int32_t* id_out, void* stream) {
+    if (!logits || !top_n || !lp_out || !id_out) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > 65535 || vocab < 1 || vocab > ld || ld % 4 || max_top < 1 || max_top > LP_MAX_TOP)
+        return RR_INVALID_ARGUMENT;
+    if (vocab > LP_MAX_CHUNKS * LP_CHUNK) return RR_INVALID_ARGUMENT;
+    cudaStream_t st = (cudaStream_t)stream;
+    void* ws = nullptr;
+    cudaError_t e = cudaMallocAsync(&ws, logprobs_ws_bytes(rows, vocab), st);
+    if (e != cudaSuccess) { note_cuda_error(e); return RR_CUDA_ERROR; }
+    launch_logprobs(logits, ld, rows, vocab, top_n, max_top, ws, lp_out, id_out, st);
+    cudaFreeAsync(ws, st);
+    return check_last();
+}
+
+RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_cache, void* out,
                              const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                              int n_kv_heads, int ctx_max, int n_slots, float scale, int kv_splits, void* stream) {
     if (!q || !k_cache || !v_cache || !out || !slot || !pos || n_slots < 1) return RR_INVALID_ARGUMENT;

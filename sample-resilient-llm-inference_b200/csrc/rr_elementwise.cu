@@ -448,6 +448,166 @@ void launch_argmax(PartIn logits, int rows, int vocab, int32_t* out_tok, float* 
     launch_pdl(argmax_kernel, dim3(rows), dim3(1024), 0, st, logits, vocab, out_tok, out_val, row_active, pos_inc);
 }
 
+// ---- log-softmax + top-k (logprobs) ---------------------------------------------------------------
+// One CTA per LP_CHUNK columns of a row (so 64 rows x 128 k vocabulary is 1024 CTAs, not 64 on 132 SMs): it reads its chunk
+// from HBM once into shared memory and writes the chunk's max m_c, s_c = sum exp(x - m_c) and its k best (value, id) in the
+// argmax order (value descending, id ascending).  k rounds over shared memory each pick the best element strictly after the
+// previous pick in that order, so equal values need no special case.  The merge CTA of the row combines the chunks in chunk
+// order: m = max m_c, s = sum s_c exp(m_c - m), lse = m + log s, and ranks the chunks' candidates.  Every sum runs in a
+// fixed order, so two calls give the same bits.
+constexpr int LP_THREADS = 256;
+struct LpPart {
+    float m, s;
+    float v[LP_MAX_TOP];
+    int32_t id[LP_MAX_TOP];   // -1: the chunk has fewer than k columns
+};
+
+__device__ __forceinline__ bool lp_before(float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); }
+
+__device__ __forceinline__ float block_max(float v, float* red) {
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+    if (lane == 0) red[warp] = v;
+    __syncthreads();
+    float t = (lane < nw) ? red[lane] : -INFINITY;
+    for (int o = 16; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(0xffffffffu, t, o));
+    __syncthreads();
+    return t;
+}
+
+// best (value, id) of the block in the argmax order; every thread gets it
+__device__ __forceinline__ void block_best(float& v, int& i, float* s_v, int* s_i) {
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+        if (lp_before(ov, oi, v, i)) { v = ov; i = oi; }
+    }
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+    if (lane == 0) { s_v[warp] = v; s_i[warp] = i; }
+    __syncthreads();
+    v = lane < nw ? s_v[lane] : -INFINITY;
+    i = lane < nw ? s_i[lane] : 0x7fffffff;
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+        if (lp_before(ov, oi, v, i)) { v = ov; i = oi; }
+    }
+    __syncthreads();
+}
+
+__global__ void __launch_bounds__(LP_THREADS)
+logprobs_chunk_kernel(const float* __restrict__ logits, int ld, int vocab, const int32_t* __restrict__ top_n, int max_top,
+                      LpPart* __restrict__ ws) {
+    __shared__ __align__(16) float s_x[LP_CHUNK];
+    __shared__ float s_rv[32];
+    __shared__ int s_ri[32];
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_LOGPROBS);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.y, c = blockIdx.x;
+    const int tn = top_n[row];
+    if (tn < 0) return;
+    const int k = min(max(1, tn), max_top);
+    const int c0 = c * LP_CHUNK;
+    const int n = min(LP_CHUNK, vocab - c0);
+    const float* x = logits + (size_t)row * ld + c0;          // 16-byte aligned: ld % 4 == 0, c0 % 4 == 0
+    float mx = -INFINITY;
+    const int n4 = n & ~3;
+#pragma unroll 8
+    for (int j = threadIdx.x * 4; j < n4; j += LP_THREADS * 4) {
+        const float4 v = __ldcs(reinterpret_cast<const float4*>(x + j));
+        *reinterpret_cast<float4*>(s_x + j) = v;
+        mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+    }
+    for (int j = n4 + threadIdx.x; j < n; j += LP_THREADS) {     // scalar tail (vocab % 4 != 0)
+        const float v = x[j];
+        s_x[j] = v;
+        mx = fmaxf(mx, v);
+    }
+    __syncthreads();
+    const float m = block_max(mx, s_rv);
+    float s = 0.f;
+    for (int j = threadIdx.x; j < n; j += LP_THREADS) s += expf(s_x[j] - m);
+    s = block_sum(s, s_rv);
+    LpPart* out = ws + (size_t)row * gridDim.x + c;
+    if (threadIdx.x == 0) { out->m = m; out->s = s; }
+    float pv = INFINITY;                                          // previous pick; (+inf, -1) precedes every element
+    int pi = -1;
+    for (int r = 0; r < k; ++r) {
+        float bv = -INFINITY;
+        int bi = 0x7fffffff;
+        for (int j = threadIdx.x; j < n; j += LP_THREADS) {
+            const float v = s_x[j];
+            const int id = c0 + j;
+            if (lp_before(pv, pi, v, id) && lp_before(v, id, bv, bi)) { bv = v; bi = id; }
+        }
+        block_best(bv, bi, s_rv, s_ri);
+        if (threadIdx.x == 0) { out->v[r] = bv; out->id[r] = bi == 0x7fffffff ? -1 : bi; }
+        pv = bv; pi = bi;
+    }
+    trace_end(tr_slot);
+}
+
+__global__ void __launch_bounds__(LP_THREADS)
+logprobs_merge_kernel(const int32_t* __restrict__ top_n, int max_top, int n_chunks, const LpPart* __restrict__ ws,
+                      float* __restrict__ lp_out, int32_t* __restrict__ id_out) {
+    __shared__ float s_v[LP_MAX_CHUNKS * LP_MAX_TOP];
+    __shared__ int s_i[LP_MAX_CHUNKS * LP_MAX_TOP];
+    __shared__ float s_lse;
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_LOGPROBS);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.x;
+    const int tn = top_n[row];
+    if (tn < 0) return;
+    const int k = min(max(1, tn), max_top);
+    const LpPart* p = ws + (size_t)row * n_chunks;
+    const int nk = n_chunks * k;
+    for (int t = threadIdx.x; t < nk; t += blockDim.x) {
+        const int c = t / k, j = t - c * k;
+        s_v[t] = p[c].v[j];
+        s_i[t] = p[c].id[j];
+    }
+    if (threadIdx.x == 0) {
+        float m = -INFINITY;
+        for (int c = 0; c < n_chunks; ++c) m = fmaxf(m, p[c].m);
+        float s = 0.f;
+        for (int c = 0; c < n_chunks; ++c) s += p[c].s * expf(p[c].m - m);
+        s_lse = m + logf(s);
+    }
+    __syncthreads();
+    const float lse = s_lse;
+    // the global k best are among the chunks' k best; a candidate's rank is the number of candidates before it
+    for (int t = threadIdx.x; t < nk; t += blockDim.x) {
+        const int id = s_i[t];
+        if (id < 0) continue;
+        const float v = s_v[t];
+        int rank = 0;
+        for (int u = 0; u < nk; ++u) rank += (s_i[u] >= 0 && lp_before(s_v[u], s_i[u], v, id)) ? 1 : 0;
+        if (rank < k) {
+            lp_out[(size_t)row * max_top + rank] = v - lse;
+            id_out[(size_t)row * max_top + rank] = id;
+        }
+    }
+    trace_end(tr_slot);
+}
+
+size_t logprobs_ws_bytes(int rows, int vocab) {
+    return (size_t)rows * ((vocab + LP_CHUNK - 1) / LP_CHUNK) * sizeof(LpPart);
+}
+
+void launch_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top, void* ws,
+                     float* lp_out, int32_t* id_out, cudaStream_t st) {
+    if (rows <= 0) return;
+    const int nc = (vocab + LP_CHUNK - 1) / LP_CHUNK;
+    launch_pdl(logprobs_chunk_kernel, dim3(nc, rows), dim3(LP_THREADS), 0, st, logits, ld, vocab, top_n, max_top,
+               (LpPart*)ws);
+    launch_pdl(logprobs_merge_kernel, dim3(rows), dim3(LP_THREADS), 0, st, top_n, max_top, nc, (const LpPart*)ws, lp_out,
+               id_out);
+}
+
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }
 
 }  // namespace rr

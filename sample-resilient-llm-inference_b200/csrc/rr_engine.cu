@@ -86,6 +86,9 @@ struct Request {
     uint64_t tag = 0;          // opaque caller value handed to the done hook (the gateway's request id)
     bool cancel = false;       // rr_engine_cancel: the worker drops the row at the next step
     bool detached = false;     // nobody will call rr_engine_wait: the worker frees the request when it finishes
+    int top_lp = -1;           // rr_engine_submit_logprobs: -1 off, else max(1, top_lp) (logprob, id) pairs per token
+    std::vector<float> lp;     // [out.size()][max(1, top_lp)]
+    std::vector<int32_t> lp_id;
 };
 
 }  // namespace rr
@@ -144,6 +147,12 @@ struct rr_engine {
     int mlp_slices = 0, mlp_slice_kb = 0;
     cudaGraphExec_t graph = nullptr;
     bool warmed = false;
+    // logprobs: a second graph (the step + launch_logprobs on `logits`), replayed only on steps with a logprobs row
+    cudaGraphExec_t graph_lp = nullptr;
+    int32_t *d_topn = nullptr, *d_topn_pf = nullptr;   // per decode row / per prefill sequence: top_lp, -1 = off
+    void* lp_ws = nullptr;
+    float* d_lp = nullptr;                             // [Bm][LP_MAX_TOP]
+    int32_t* d_lp_id = nullptr;
 
     // prefill working set
     int Tmax;
@@ -158,6 +167,9 @@ struct rr_engine {
     size_t h_stage_ints;
     int32_t* h_tok;       // [Bm] tokens read back each step
     float* h_logits = nullptr;
+    float* h_lp = nullptr;        // [Bm][LP_MAX_TOP] logprobs read back on steps that computed them
+    int32_t* h_lp_id = nullptr;
+    int32_t* h_topn = nullptr;    // [Bm] staging of d_topn / d_topn_pf
 
     // serving state
     std::mutex mu;                       // queues + request table
@@ -168,13 +180,15 @@ struct rr_engine {
     std::vector<Request*> row_req;       // [Bm]
     std::vector<int32_t> h_slot_mirror;  // host mirror of d_slot
     bool slots_dirty = false;
+    std::vector<int32_t> h_topn_mirror;  // host mirror of d_topn (uploaded before a step that replays graph_lp)
+    bool topn_dirty = false;
     std::thread worker;
     std::atomic<bool> stop{false};
     uint64_t next_ticket = 1;
     std::chrono::steady_clock::time_point t0;
 
     rr_engine_stats st;                  // written under gpu_mu (launch / timing counters) or mu (queued, active_rows)
-    uint64_t step_launches = 0;
+    uint64_t step_launches = 0, step_launches_lp = 0;
     // completion hook (the native gateway, rr_gateway.cu): called on the worker / submitting thread, outside `mu`
     rr::EngineDoneHook hook = nullptr;
     void* hook_ctx = nullptr;
@@ -230,7 +244,12 @@ static PartIn part_bf16(const __nv_bfloat16* p, int ld) {
 static PartIn part_none() { PartIn r; r.ptr = nullptr; r.is_bf16 = 0; r.n_splits = 1; r.split_stride = 0; r.ld = 0; return r; }
 
 // ---------------------------------------------------------------- decode step (enqueue only)
-static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch) {
+static void enqueue_logprobs(rr_engine* e, const int32_t* top_n, int rows, cudaStream_t s) {
+    launch_logprobs(e->logits, e->d.vocab, rows, e->d.vocab, top_n, LP_MAX_TOP, e->lp_ws, e->d_lp, e->d_lp_id, s);
+}
+
+// logprobs: launch_logprobs after the argmax for the rows with d_topn[row] >= 0 (the logits are left as they were)
+static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, bool logprobs = false) {
     const rr_model_desc& d = e->d;
     const int B = e->Bm, L = d.n_layers;
     uint64_t nl = 0;
@@ -246,6 +265,7 @@ static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch)
             if (layer_launch(e->layer[1 + l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         }
         launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
+        if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s); nl += LP_LAUNCHES; }
         if (n_launch) *n_launch = nl;
         cudaError_t err = cudaGetLastError();
         if (err != cudaSuccess) { rr::note_cuda_error(err); return RR_CUDA_ERROR; }
@@ -279,38 +299,53 @@ static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch)
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
     launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
+    if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s); nl += LP_LAUNCHES; }
     if (n_launch) *n_launch = nl;
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) { rr::note_cuda_error(err); return RR_CUDA_ERROR; }
     return RR_OK;
 }
 
-static int run_decode_step(rr_engine* e) {
+static int capture_decode_step(rr_engine* e, bool logprobs, cudaGraphExec_t* out, uint64_t* n_launch) {
+    cudaStream_t s = e->stream;
+    cudaGraph_t g = nullptr;
+    CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    int rc = enqueue_decode_step(e, s, n_launch, logprobs);
+    cudaError_t ce = cudaStreamEndCapture(s, &g);
+    if (rc != RR_OK || ce != cudaSuccess) { rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
+    CK(cudaGraphInstantiate(out, g, 0));
+    cudaGraphDestroy(g);
+    return RR_OK;
+}
+
+// logprobs: also run launch_logprobs for the rows with d_topn >= 0 (graph_lp, captured on first use); a step without
+// logprobs rows replays the plain graph.
+static int run_decode_step(rr_engine* e, bool logprobs = false) {
     cudaStream_t s = e->stream;
     if (!e->warmed || !e->o.use_cuda_graph) {
         uint64_t nl = 0;
-        int rc = enqueue_decode_step(e, s, &nl);
+        int rc = enqueue_decode_step(e, s, &nl, logprobs);
         if (rc != RR_OK) return rc;
-        e->step_launches = nl;
+        (logprobs ? e->step_launches_lp : e->step_launches) = nl;
+        e->st.kernel_launches += nl;
         // NOTE: the warm-up step is a real step (it advances positions); graph capture follows.
         if (!e->warmed) {
             e->warmed = true;
             if (e->o.use_cuda_graph) {
                 CK(cudaStreamSynchronize(s));
                 // capture for subsequent steps
-                cudaGraph_t g = nullptr;
-                CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-                rc = enqueue_decode_step(e, s, nullptr);
-                cudaError_t ce = cudaStreamEndCapture(s, &g);
-                if (rc != RR_OK || ce != cudaSuccess) { rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
-                CK(cudaGraphInstantiate(&e->graph, g, 0));
-                cudaGraphDestroy(g);
+                rc = capture_decode_step(e, false, &e->graph, &e->step_launches);
+                if (rc != RR_OK) return rc;
             }
         }
-    } else {
-        CK(cudaGraphLaunch(e->graph, s));
+        return RR_OK;
     }
-    e->st.kernel_launches += e->step_launches;
+    if (logprobs && !e->graph_lp) {
+        const int rc = capture_decode_step(e, true, &e->graph_lp, &e->step_launches_lp);
+        if (rc != RR_OK) return rc;
+    }
+    CK(cudaGraphLaunch(logprobs ? e->graph_lp : e->graph, s));
+    e->st.kernel_launches += logprobs ? e->step_launches_lp : e->step_launches;
     return RR_OK;
 }
 
@@ -370,9 +405,10 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 }
 
 // ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
-// activates the rows. Caller holds gpu_mu.
+// activates the rows. Caller holds gpu_mu.  topn_host[n_seqs] (optional): sequences with topn_host[i] >= 0 also get their
+// first token's logprobs in e->h_lp / e->h_lp_id row i.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
-                       int n_seqs, int32_t* first_tok_host, float* logits_host) {
+                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
@@ -462,6 +498,18 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
     launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
                (const int32_t*)e->p_first, (const int32_t*)p_ss, n_seqs, e->d_tok, e->d_pos, e->d_slot); ++nl;
+    bool lp = false;
+    for (int i = 0; topn_host && i < n_seqs; ++i) lp = lp || topn_host[i] >= 0;
+    if (lp) {
+        memcpy(e->h_topn, topn_host, sizeof(int32_t) * n_seqs);
+        CK(cudaMemcpyAsync(e->d_topn_pf, e->h_topn, sizeof(int32_t) * n_seqs, cudaMemcpyHostToDevice, s));
+        e->st.h2d_bytes += sizeof(int32_t) * n_seqs;
+        enqueue_logprobs(e, e->d_topn_pf, n_seqs, s); nl += LP_LAUNCHES;
+        const size_t n = (size_t)n_seqs * LP_MAX_TOP;
+        CK(cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
+    }
     CK(cudaMemcpyAsync(e->h_tok, e->p_first, sizeof(int32_t) * n_seqs, cudaMemcpyDeviceToHost, s));
     e->st.d2h_bytes += sizeof(int32_t) * n_seqs;
     if (logits_host) {
@@ -485,6 +533,21 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
 // ---------------------------------------------------------------- worker (continuous batching)
 struct DoneNote { uint64_t tag, ticket; int status, n_gen; };
 
+// Caller holds e->mu.  Appends row `row` of h_lp / h_lp_id to the request's pairs.
+static void record_logprobs(rr_engine* e, Request* r, int row) {
+    const int k = r->top_lp > 1 ? r->top_lp : 1;
+    const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
+    const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
+    r->lp.insert(r->lp.end(), v, v + k);
+    r->lp_id.insert(r->lp_id.end(), id, id + k);
+}
+
+// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirror of d_topn in step.
+static void set_row_topn(rr_engine* e, int b, const Request* r) {
+    const int t = r ? r->top_lp : -1;
+    if (e->h_topn_mirror[b] != t) { e->h_topn_mirror[b] = t; e->topn_dirty = true; }
+}
+
 // Caller holds e->mu.  Returns the hook call to make once the lock is released (tag == 0 and no hook: nothing).
 static void finish_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes = nullptr) {
     r->status = status;
@@ -503,24 +566,27 @@ static void run_hooks(rr_engine* e, std::vector<DoneNote>& notes) {
 
 static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
-    std::vector<int32_t> ids, seq_start, slots;
+    std::vector<int32_t> ids, seq_start, slots, topn;
     std::vector<Request*> chunk;
     std::vector<DoneNote> notes;
     while (!e->stop.load()) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
-        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear();
+        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); topn.clear();
         int active = 0;
+        bool lp_step = false;
         {
             std::unique_lock<std::mutex> lk(e->mu);
             for (int b = 0; b < e->Bm; ++b) {
                 Request* r = e->row_req[b];
                 if (r && r->cancel) {                      // rr_engine_cancel: free the row, keep what was generated
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
+                    set_row_topn(e, b, nullptr);
                     finish_request(e, r, RR_CANCELLED, &notes);
                     continue;
                 }
                 active += r != nullptr;
+                lp_step = lp_step || (r && r->top_lp >= 0);
             }
             if (e->waiting.empty() && active == 0) {
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
@@ -537,6 +603,7 @@ static void worker_main(rr_engine* e) {
                 r->slot = b;
                 chunk.push_back(r);
                 slots.push_back(b);
+                topn.push_back(r->top_lp);
                 ids.insert(ids.end(), r->prompt.begin(), r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
@@ -547,7 +614,8 @@ static void worker_main(rr_engine* e) {
         std::lock_guard<std::mutex> gl(e->gpu_mu);
         std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
         if (!chunk.empty()) {
-            int rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr);
+            int rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
+                                 topn.data());
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
@@ -560,11 +628,14 @@ static void worker_main(rr_engine* e) {
                 }
                 r->t_first = t;
                 r->out.push_back(e->h_tok[i]);
+                if (r->top_lp >= 0) record_logprobs(e, r, (int)i);
                 e->st.generated_tokens += 1;
                 if ((int)r->out.size() >= r->max_new) {
                     e->row_req[r->slot] = nullptr;
                     e->h_slot_mirror[r->slot] = -1; e->slots_dirty = true;
                     finish_request(e, r, RR_OK, &notes);
+                } else {
+                    set_row_topn(e, r->slot, r);
                 }
             }
             e->cv_done.notify_all();
@@ -579,10 +650,22 @@ static void worker_main(rr_engine* e) {
             e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
             e->slots_dirty = false;
         }
+        if (lp_step && e->topn_dirty) {           // (the mirror is only touched by this thread)
+            memcpy(e->h_topn, e->h_topn_mirror.data(), sizeof(int32_t) * e->Bm);
+            e->topn_dirty = false;
+            cudaMemcpyAsync(e->d_topn, e->h_topn, sizeof(int32_t) * e->Bm, cudaMemcpyHostToDevice, s);
+            e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
+        }
         cudaEventRecord(e->ev0, s);
-        int rc = run_decode_step(e);
+        int rc = run_decode_step(e, lp_step);
         cudaEventRecord(e->ev1, s);
         cudaMemcpyAsync(e->h_tok, e->d_tok, sizeof(int32_t) * e->Bm, cudaMemcpyDeviceToHost, s);
+        if (lp_step) {
+            const size_t n = (size_t)e->Bm * LP_MAX_TOP;
+            cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s);
+            cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s);
+            e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
+        }
         cudaError_t se = cudaStreamSynchronize(s);
         e->st.d2h_bytes += sizeof(int32_t) * e->Bm;
         if (se != cudaSuccess) { rr::note_cuda_error(se); rc = RR_CUDA_ERROR; }
@@ -597,13 +680,16 @@ static void worker_main(rr_engine* e) {
                 if (!r) continue;
                 if (rc != RR_OK) {
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
+                    set_row_topn(e, b, nullptr);
                     finish_request(e, r, RR_INTERNAL, &notes);
                     continue;
                 }
                 r->out.push_back(e->h_tok[b]);
+                if (r->top_lp >= 0) record_logprobs(e, r, b);
                 e->st.generated_tokens += 1;
                 if ((int)r->out.size() >= r->max_new) {
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
+                    set_row_topn(e, b, nullptr);
                     finish_request(e, r, RR_OK, &notes);
                 }
             }
@@ -702,6 +788,13 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->h_stage_ints = (size_t)3 * T + 3 * B + 8;
     TRYC(cudaMallocHost(&e->h_stage, e->h_stage_ints * sizeof(int32_t)));
     TRYC(cudaMallocHost(&e->h_tok, sizeof(int32_t) * (B > 16 ? B : 16)));
+    TRY(dalloc(e, &e->d_topn, B)); TRY(dalloc(e, &e->d_topn_pf, B));
+    TRYC(cudaMemset(e->d_topn, 0xff, sizeof(int32_t) * B));
+    TRY(dalloc(e, (char**)&e->lp_ws, logprobs_ws_bytes(B, d.vocab), false));
+    TRY(dalloc(e, &e->d_lp, (size_t)B * LP_MAX_TOP)); TRY(dalloc(e, &e->d_lp_id, (size_t)B * LP_MAX_TOP));
+    TRYC(cudaMallocHost(&e->h_lp, sizeof(float) * B * LP_MAX_TOP));
+    TRYC(cudaMallocHost(&e->h_lp_id, sizeof(int32_t) * B * LP_MAX_TOP));
+    TRYC(cudaMallocHost(&e->h_topn, sizeof(int32_t) * B));
 
     e->pl_qkv.resize(L); e->pl_o.resize(L); e->pl_gu.resize(L); e->pl_down.resize(L);
     e->attn_args.resize(L);
@@ -826,6 +919,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRYC(cudaDeviceSynchronize());
     e->row_req.assign(B, nullptr);
     e->h_slot_mirror.assign(B, -1);
+    e->h_topn_mirror.assign(B, -1);
     e->worker = std::thread(worker_main, e);
     *out = e;
     return RR_OK;
@@ -841,9 +935,13 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     cudaSetDevice(e->o.device);
     if (e->stream) cudaStreamSynchronize(e->stream);
     if (e->graph) cudaGraphExecDestroy(e->graph);
+    if (e->graph_lp) cudaGraphExecDestroy(e->graph_lp);
     for (void* p : e->allocs) cudaFree(p);
     if (e->h_stage) cudaFreeHost(e->h_stage);
     if (e->h_tok) cudaFreeHost(e->h_tok);
+    if (e->h_lp) cudaFreeHost(e->h_lp);
+    if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
+    if (e->h_topn) cudaFreeHost(e->h_topn);
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) cudaStreamDestroy(e->stream);
@@ -908,8 +1006,10 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
 
 namespace rr {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket) {
+                         uint64_t* ticket, int top_logprobs) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
+    if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
+    if (top_logprobs >= 0 && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK)) return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
         if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
@@ -919,6 +1019,11 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     r->max_new = max_new_tokens;
     r->out.reserve(max_new_tokens);
     r->tag = tag;
+    r->top_lp = top_logprobs;
+    if (top_logprobs >= 0) {
+        const size_t k = top_logprobs > 1 ? top_logprobs : 1;
+        r->lp.reserve(k * max_new_tokens); r->lp_id.reserve(k * max_new_tokens);
+    }
     std::vector<DoneNote> notes;
     {
         std::lock_guard<std::mutex> lk(e->mu);
@@ -956,6 +1061,20 @@ RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_promp
     return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket);
 }
 
+RR_API int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                     int top_logprobs, uint64_t* ticket) {
+    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs);
+}
+
+// Caller holds e->mu.  The first min(n, max_tokens_out) tokens' pairs of a logprobs request into [max_tokens_out][K].
+static void copy_logprobs(const Request* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    const int t = n < max_tokens_out ? n : max_tokens_out;
+    if (r->top_lp < 0 || t <= 0) return;
+    const size_t m = (size_t)t * (r->top_lp > 1 ? r->top_lp : 1);
+    if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
+    if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
+}
+
 // Abandon a request (client gone / timed out): a queued request is dropped, a running one gives up its decode row at the
 // next step; a finished one is just freed.  The ticket is consumed: do not wait on it afterwards.
 RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
@@ -986,8 +1105,9 @@ RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
 
 // Streaming support: block until the request has more than `have` tokens (or is done / the wait times out), then
 // copy the tokens generated so far.  Does not consume the request; finish with rr_engine_wait.
-RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                          int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s) {
+RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                                   int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
+                                   float* lp_out, int32_t* id_out) {
     if (!e || !n_generated || !done) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1014,11 +1134,18 @@ RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeou
         const int m = n < max_tokens_out ? n : max_tokens_out;
         memcpy(tokens_out, r->out.data(), sizeof(int32_t) * m);
     }
+    copy_logprobs(r, n, max_tokens_out, lp_out, id_out);
     return RR_OK;
 }
 
-RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                          int max_tokens_out) {
+RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                          int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s) {
+    return rr_engine_peek_logprobs(e, ticket, have, timeout_s, tokens_out, max_tokens_out, n_generated, done,
+                                   t_first_token_s, nullptr, nullptr);
+}
+
+RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
+                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
     if (!e || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1044,10 +1171,16 @@ RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_co
         const int n = (int)r->out.size() < max_tokens_out ? (int)r->out.size() : max_tokens_out;
         memcpy(tokens_out, r->out.data(), sizeof(int32_t) * n);
     }
+    copy_logprobs(r, (int)r->out.size(), max_tokens_out, lp_out, id_out);
     const int status = r->status;
     e->table.erase(ticket);
     delete r;
     return status == RR_OK ? RR_OK : status;
+}
+
+RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                          int max_tokens_out) {
+    return rr_engine_wait_logprobs(e, ticket, timeout_s, out, tokens_out, max_tokens_out, nullptr, nullptr);
 }
 
 RR_API int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start, int n_requests,

@@ -45,6 +45,9 @@ struct GwReq {
     rr_engine* eng = nullptr;
     uint64_t eng_ticket = 0;
     std::vector<int32_t> tokens;
+    int top_lp = -1;                  // rr_gateway_submit_logprobs: handed to every engine the request is admitted to
+    std::vector<float> lp;            // [tokens.size()][max(1, top_lp)]
+    std::vector<int32_t> lp_id;
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
 };
@@ -115,7 +118,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     if (tag == 0) return;                                    // not submitted through this gateway
     GwReq* r = nullptr;
     rr_engine* eng = nullptr;
-    int max_new = 0;
+    int max_new = 0, top_lp = -1;
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -123,13 +126,19 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         r = it->second;
         eng = r->eng;
         max_new = r->max_new;
+        top_lp = r->top_lp;
     }
-    // consume the engine's record (tokens + timestamps); a cancelled request has none left
+    // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
     memset(&comp, 0, sizeof(comp));
     std::vector<int32_t> toks((size_t)(max_new > 0 ? max_new : 1));
+    const size_t k = top_lp > 1 ? (size_t)top_lp : 1;
+    std::vector<float> lps(top_lp >= 0 ? toks.size() * k : 0);
+    std::vector<int32_t> lp_ids(lps.size());
     int wrc = RR_INVALID_ARGUMENT;
-    if (eng && status != RR_CANCELLED) wrc = rr_engine_wait(eng, eng_ticket, 0.001, &comp, toks.data(), max_new);
+    if (eng && status != RR_CANCELLED)
+        wrc = rr_engine_wait_logprobs(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, top_lp >= 0 ? lps.data() : nullptr,
+                                      top_lp >= 0 ? lp_ids.data() : nullptr);
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -139,6 +148,10 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
             const int n = comp.n_generated < max_new ? comp.n_generated : max_new;
             r->tokens.assign(toks.begin(), toks.begin() + (n > 0 ? n : 0));
+            if (top_lp >= 0) {
+                r->lp.assign(lps.begin(), lps.begin() + r->tokens.size() * k);
+                r->lp_id.assign(lp_ids.begin(), lp_ids.begin() + r->tokens.size() * k);
+            }
             r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
         }
         if (status == RR_OK) {
@@ -166,6 +179,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
                 r->state = Q_ADMIT;
                 r->eng = nullptr;
                 r->tokens.clear();
+                r->lp.clear(); r->lp_id.clear();
                 g->st.failed_over++;
                 g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
             }
@@ -260,7 +274,8 @@ static void gw_dispatch(rr_gateway* g) {
             }
             uint64_t tk = 0;
             int src = RR_INTERNAL;
-            if (!cancelled && eng) src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk);
+            if (!cancelled && eng) src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk,
+                                                           r->top_lp);
             bool cancel_now = false;
             std::unique_lock<std::mutex> lk(g->mu);
             if (src == RR_OK) {
@@ -351,9 +366,10 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
     return RR_OK;
 }
 
-RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
-                                   int max_new_tokens, int declare_burst, uint64_t* tickets) {
+static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
+                     int max_new_tokens, int declare_burst, int top_logprobs, uint64_t* tickets) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
+    if (top_logprobs < -1 || top_logprobs > rr::LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n; ++i) {
         const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens);
         if (rc != RR_OK) return rc;
@@ -362,7 +378,7 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
     for (int i = 0; i < n; ++i) {
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
-        r->group = group; r->max_new = max_new_tokens;
+        r->group = group; r->max_new = max_new_tokens; r->top_lp = top_logprobs;
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -384,10 +400,30 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
     return RR_OK;
 }
 
+RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
+                                   int max_new_tokens, int declare_burst, uint64_t* tickets) {
+    return gw_submit(g, group, prompt_ids, prompt_start, n, max_new_tokens, declare_burst, -1, tickets);
+}
+
 RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                              uint64_t* ticket) {
     const int32_t start[2] = {0, n_prompt};
-    return rr_gateway_submit_batch(g, group, prompt_ids, start, 1, max_new_tokens, 0, ticket);
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, -1, ticket);
+}
+
+RR_API int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                      int top_logprobs, uint64_t* ticket) {
+    const int32_t start[2] = {0, n_prompt};
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket);
+}
+
+// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][max(1, top_lp)].
+static void gw_copy_logprobs(const GwReq* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    const int t = n < max_tokens_out ? n : max_tokens_out;
+    if (r->top_lp < 0 || t <= 0) return;
+    const size_t m = (size_t)t * (r->top_lp > 1 ? r->top_lp : 1);
+    if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
+    if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
 }
 
 static void gw_fill(const GwReq* r, rr_gateway_result* out) {
@@ -398,8 +434,8 @@ static void gw_fill(const GwReq* r, rr_gateway_result* out) {
     out->t_submit_s = r->t_submit; out->t_admit_s = r->t_admit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
 }
 
-RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                           int max_tokens_out) {
+RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
+                                    int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
     if (!g || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(g->mu);
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
@@ -424,14 +460,21 @@ RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_
         const int n = (int)r->tokens.size() < max_tokens_out ? (int)r->tokens.size() : max_tokens_out;
         if (n > 0) memcpy(tokens_out, r->tokens.data(), sizeof(int32_t) * (size_t)n);
     }
+    gw_copy_logprobs(r, (int)r->tokens.size(), max_tokens_out, lp_out, id_out);
     const int status = r->status;
     g->table.erase(ticket);
     delete r;
     return status;
 }
 
-RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
-                           int32_t* n_generated, int32_t* done, rr_gateway_result* out) {
+RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                           int max_tokens_out) {
+    return rr_gateway_wait_logprobs(g, ticket, timeout_s, out, tokens_out, max_tokens_out, nullptr, nullptr);
+}
+
+RR_API int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                                    int max_tokens_out, int32_t* n_generated, int32_t* done, rr_gateway_result* out,
+                                    float* lp_out, int32_t* id_out) {
     if (!g || !n_generated || !done) return RR_INVALID_ARGUMENT;
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
     for (;;) {
@@ -448,6 +491,7 @@ RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double time
                     const int n = (int)r->tokens.size();
                     *n_generated = n; *done = 1;
                     if (tokens_out && n > 0) memcpy(tokens_out, r->tokens.data(), sizeof(int32_t) * (size_t)(n < max_tokens_out ? n : max_tokens_out));
+                    gw_copy_logprobs(r, n, max_tokens_out, lp_out, id_out);
                     return RR_OK;
                 }
                 if (r->state == RUNNING) { eng = r->eng; tk = r->eng_ticket; break; }
@@ -456,13 +500,20 @@ RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double time
         }
         const double left = std::chrono::duration<double>(deadline - std::chrono::steady_clock::now()).count();
         int32_t n = 0, d = 0;
-        const int rc = rr_engine_peek(eng, tk, have, left > 0.001 ? left : 0.001, tokens_out, max_tokens_out, &n, &d, nullptr);
+        const int rc = rr_engine_peek_logprobs(eng, tk, have, left > 0.001 ? left : 0.001, tokens_out, max_tokens_out, &n, &d,
+                                               nullptr, lp_out, id_out);
         if (rc == RR_OK && !d) { *n_generated = n; *done = 0; return RR_OK; }
         // finished (the hook is consuming / has consumed the engine's record) or failed over: look at our own record again
         if (std::chrono::steady_clock::now() >= deadline) { *n_generated = rc == RR_OK ? n : 0; *done = 0; return RR_OK; }
         std::unique_lock<std::mutex> lk(g->mu);
         g->cv_done.wait_for(lk, std::chrono::milliseconds(1));
     }
+}
+
+RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
+                           int32_t* n_generated, int32_t* done, rr_gateway_result* out) {
+    return rr_gateway_peek_logprobs(g, ticket, have, timeout_s, tokens_out, max_tokens_out, n_generated, done, out, nullptr,
+                                    nullptr);
 }
 
 RR_API int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure) {

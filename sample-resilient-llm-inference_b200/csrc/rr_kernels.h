@@ -62,7 +62,7 @@ int num_sms();
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)
 typedef void (*EngineDoneHook)(void* ctx, uint64_t tag, uint64_t ticket, int status, int n_generated);
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket);
+                         uint64_t* ticket, int top_logprobs = -1);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
@@ -211,6 +211,17 @@ void launch_rope_table(float2* table, int ctx_max, float theta, int head_dim, cu
 // advance != 0: pos[row]++ (decode bookkeeping folded into the same launch).
 void launch_argmax(PartIn logits, int rows, int vocab, int32_t* out_tok, float* out_val,
                    const int32_t* row_active, int32_t* pos_inc, cudaStream_t st);
+// log-softmax + top-k over fp32 logits [rows][ld] (ld % 4 == 0, vocab <= ld): rows with top_n[r] >= 0 get
+// k = min(max(1, top_n[r]), max_top) entries lp_out[r][j] = x - logsumexp(x), id_out[r][j], ordered by (value desc, id asc);
+// other rows and entries j >= k are not written.  Two launches: LP_CHUNK-column chunks of every row in parallel, then one
+// merge CTA per row.  ws = logprobs_ws_bytes(rows, vocab) of scratch, no initialisation needed.
+constexpr int LP_MAX_TOP = 20;        // OpenAI's limit for top_logprobs
+constexpr int LP_CHUNK = 8192;        // columns per chunk CTA (staged in 32 KB of shared memory)
+constexpr int LP_MAX_CHUNKS = 64;     // vocab <= 64 * 8192 = 524288
+constexpr int LP_LAUNCHES = 2;
+size_t logprobs_ws_bytes(int rows, int vocab);
+void launch_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top, void* ws,
+                     float* lp_out, int32_t* id_out, cudaStream_t st);
 
 // ---- attention (rr_attn_decode.cu, rr_attn_tc.cu) ---------------------------------------------------
 struct DecodeAttnArgs {

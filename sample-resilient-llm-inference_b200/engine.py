@@ -8,13 +8,14 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import _lib
 from .models import ModelSpec, Weights, make_weights
+from .router import logprob_pairs
 
 
 @dataclass
@@ -26,6 +27,8 @@ class CompletionRecord:
     t_submit: float
     t_first_token: float
     t_done: float
+    # submit(top_logprobs=k): per generated token the max(1, k) most likely (token id, logprob) pairs, best first
+    logprobs: Optional[List[List[Tuple[int, float]]]] = None
 
     @property
     def ttft(self) -> float:
@@ -90,6 +93,7 @@ class Engine:
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
                                (C.c_int32 * 4)(2 if fuse_layer else 1, 0, 0 if fuse_mlp else 1, 0 if defer_norm else 1))
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
+        self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -133,29 +137,52 @@ class Engine:
         return nxt, logits
 
     # ---- serving interface ----------------------------------------------------------------------
-    def submit(self, prompt_ids: Sequence[int], max_new_tokens: int) -> int:
+    def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None) -> int:
+        """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
+        (the generated tokens do not change)."""
         ids = _i32(prompt_ids)
         t = C.c_uint64()
-        _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(t)),
-                   "rr_engine_submit")
+        if top_logprobs is None:
+            _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(t)),
+                       "rr_engine_submit")
+            return t.value
+        _lib.check(_lib.lib.rr_engine_submit_logprobs(self._h, _p(ids), len(ids), max_new_tokens, int(top_logprobs),
+                                                      C.byref(t)), "rr_engine_submit_logprobs")
+        self._lp_k[t.value] = max(1, int(top_logprobs))
         return t.value
+
+    def _lp_bufs(self, ticket: int, max_tokens: int):
+        k = self._lp_k.get(ticket)
+        if k is None:
+            return None, None, None, None
+        lp, ids = np.zeros((max_tokens, k), dtype=np.float32), np.zeros((max_tokens, k), dtype=np.int32)
+        return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), _p(ids)
 
     def wait(self, ticket: int, timeout: float = 0.0, max_tokens: int = 4096) -> CompletionRecord:
         c = _lib.Completion()
         buf = np.zeros(max_tokens, dtype=np.int32)
-        rc = _lib.lib.rr_engine_wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens)
+        lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens)
+        rc = _lib.lib.rr_engine_wait_logprobs(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
+        if rc != 6:
+            self._lp_k.pop(ticket, None)
         if rc not in (0, 6, 7):
             _lib.check(rc, "rr_engine_wait")
+        n = min(c.n_generated, max_tokens)
         return CompletionRecord(ticket, rc, c.n_prompt, buf[:c.n_generated].tolist(), c.t_submit_s,
-                                c.t_first_token_s, c.t_done_s)
+                                c.t_first_token_s, c.t_done_s, logprob_pairs(lp, ids, 0, n) if lp is not None else None)
 
     def peek(self, ticket: int, have: int, timeout: float = 0.05, max_tokens: int = 4096):
-        """Streaming: wait until more than `have` tokens exist (or done / timeout). -> (tokens so far, done, ttft_s)."""
+        """Streaming: wait until more than `have` tokens exist (or done / timeout). -> (tokens so far, done, ttft_s), and
+        for a request submitted with top_logprobs a fourth element: the per-token pairs so far (see CompletionRecord)."""
         buf = np.zeros(max_tokens, dtype=np.int32)
         n, done, ttft = C.c_int32(), C.c_int32(), C.c_double()
-        _lib.check(_lib.lib.rr_engine_peek(self._h, ticket, have, float(timeout), _p(buf), max_tokens, C.byref(n),
-                                           C.byref(done), C.byref(ttft)), "rr_engine_peek")
-        return buf[: n.value].tolist(), bool(done.value), ttft.value
+        lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens)
+        _lib.check(_lib.lib.rr_engine_peek_logprobs(self._h, ticket, have, float(timeout), _p(buf), max_tokens, C.byref(n),
+                                                    C.byref(done), C.byref(ttft), lp_p, ids_p), "rr_engine_peek")
+        if lp is None:
+            return buf[: n.value].tolist(), bool(done.value), ttft.value
+        m = min(n.value, max_tokens)
+        return buf[: n.value].tolist(), bool(done.value), ttft.value, logprob_pairs(lp, ids, 0, m)
 
     def run_batch(self, prompt_ids: np.ndarray, prompt_start: np.ndarray, max_new_tokens: int):
         """Closed burst: submit every prompt, wait for all.  `prompt_ids` is a host buffer; the

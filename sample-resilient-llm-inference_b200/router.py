@@ -68,6 +68,7 @@ class Choice:
     index: int
     message: Message
     finish_reason: str = "length"
+    logprobs: Optional[dict] = None      # OpenAI ChoiceLogprobs {"content": [...], "refusal": None}; only when requested
 
 
 @dataclass
@@ -95,8 +96,9 @@ class ModelResponse:
 
     def model_dump(self) -> dict:
         return {"id": self.id, "object": self.object, "created": self.created, "model": self.model,
-                "choices": [{"index": c.index, "finish_reason": c.finish_reason,
-                             "message": {"role": c.message.role, "content": c.message.content}}
+                "choices": [dict({"index": c.index, "finish_reason": c.finish_reason,
+                                  "message": {"role": c.message.role, "content": c.message.content}},
+                                 **({} if c.logprobs is None else {"logprobs": c.logprobs}))
                             for c in self.choices],
                 "usage": {"prompt_tokens": self.usage.prompt_tokens,
                           "completion_tokens": self.usage.completion_tokens,
@@ -141,6 +143,46 @@ def tokenize_host(text: str, vocab: int) -> np.ndarray:
 
 def detokenize(ids: Sequence[int]) -> str:
     return bytes(((int(t) - 3) % 256) for t in ids if int(t) >= 3).decode("utf-8", errors="replace")
+
+
+MAX_TOP_LOGPROBS = 20        # OpenAI's limit
+
+
+def check_logprobs(logprobs: Any, top_logprobs: Any) -> Optional[int]:
+    """OpenAI's rules for the `logprobs` / `top_logprobs` request fields -> None (off) or the number of alternatives per
+    token, 0..20.  Raises BadRequestError (HTTP 400) for anything else."""
+    if logprobs is not None and not isinstance(logprobs, bool):
+        raise BadRequestError("`logprobs` must be a boolean")
+    if top_logprobs is not None:
+        if not logprobs:
+            raise BadRequestError("`top_logprobs` requires `logprobs` to be true")
+        if isinstance(top_logprobs, bool) or not isinstance(top_logprobs, int) or not 0 <= top_logprobs <= MAX_TOP_LOGPROBS:
+            raise BadRequestError(f"`top_logprobs` must be an integer from 0 to {MAX_TOP_LOGPROBS}")
+    if not logprobs:
+        return None
+    return 0 if top_logprobs is None else top_logprobs
+
+
+def _token_entry(tok: int, logprob: float) -> dict:
+    """One token of the byte tokenizer in OpenAI's logprob shape (`token` is detokenize([tok]), `bytes` its byte)."""
+    return {"token": detokenize([tok]), "logprob": logprob, "bytes": [(tok - 3) % 256] if tok >= 3 else []}
+
+
+def logprobs_content(tokens: Sequence[int], pairs: Sequence[Sequence[Tuple[int, float]]], top: int) -> List[dict]:
+    """`choices[0].logprobs.content` for the generated tokens: pairs[i] = the engine's (id, logprob) list of token i, best
+    first; `top` alternatives each."""
+    out = []
+    for tok, p in zip(tokens, pairs):
+        lp = next((v for i, v in p if i == tok), p[0][1])
+        e = _token_entry(int(tok), lp)
+        e["top_logprobs"] = [_token_entry(i, v) for i, v in p[:top]]
+        out.append(e)
+    return out
+
+
+def logprob_pairs(lp: np.ndarray, ids: np.ndarray, a: int, b: int) -> List[List[Tuple[int, float]]]:
+    """Rows a..b of the library's [tokens][K] logprob / id buffers -> per token [(token id, logprob)], best first."""
+    return [[(int(i), float(v)) for i, v in zip(ids[t], lp[t])] for t in range(a, b)]
 
 
 def messages_to_text(messages: Sequence[dict]) -> str:
@@ -294,12 +336,12 @@ class Router:
         return [((e.type, e.target, e.tokens, e.chain_start, e.now_ms), (d.status, d.deployment, d.served_group, d.chain_pos))
                 for e, d in zip(ev[: n.value], dec[: n.value])]
 
-    def _gw_response(self, res, toks, n_prompt, t_start, detok=True) -> ModelResponse:
+    def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None) -> ModelResponse:
         d = self.cfg.deployments[res.deployment]
         toks = [int(t) for t in toks[: res.n_generated]]
         return ModelResponse(
             id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-            choices=[Choice(0, Message("assistant", detokenize(toks) if detok else ""))],
+            choices=[Choice(0, Message("assistant", detokenize(toks) if detok else ""), logprobs=logprobs)],
             usage=Usage(n_prompt, len(toks), n_prompt + len(toks)), created=int(time.time()),
             _token_ids=toks, _deployment=res.deployment, _model_group=self.cfg.groups[res.served_group],
             _fell_back=res.chain_pos > 0, _ttft_s=res.t_first_token_s - res.t_submit_s,
@@ -320,55 +362,82 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None) -> int:
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new, C.byref(t))
+        if top is None:
+            rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new, C.byref(t))
+        else:
+            rc = _lib.lib.rr_gateway_submit_logprobs(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                                     top, C.byref(t))
         if rc != 0:
             raise self._gw_error(rc, model)
         return t.value
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout):
+    @staticmethod
+    def _lp_bufs(top: Optional[int], max_new: int):
+        if top is None:
+            return None, None, None, None
+        lp = np.zeros((max_new, max(1, top)), dtype=np.float32)
+        ids = np.zeros((max_new, max(1, top)), dtype=np.int32)
+        return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
+
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top)
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
-        rc = _lib.lib.rr_gateway_wait(gw, ticket, float(timeout or 0.0), C.byref(res),
-                                      toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new)
+        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new)
+        rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, float(timeout or 0.0), C.byref(res),
+                                               toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
         if rc == 6:                      # client-side timeout: give the row back, count a failure against the deployment
             _lib.lib.rr_gateway_cancel(gw, ticket, 1)
             raise self._gw_error(6, model, res, timeout)
         if rc != 0:
             raise self._gw_error(rc, model, res, timeout)
-        return self._gw_response(res, toks, len(prompt_ids), t_start)
+        content = None
+        if top is not None:
+            n = min(res.n_generated, max_new)
+            content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), top), "refusal": None}
+        return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
 
-    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout):
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model)
+    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None):
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top)
         deadline = None if not timeout else time.perf_counter() + timeout
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
+        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new)
         n, done = C.c_int32(), C.c_int32()
         sent, finished = 0, False
+
+        def item(label, a, b, ttft):
+            """(label, tokens a..b, done=False, ttft) + with logprobs: the OpenAI content entries of those tokens."""
+            new = [int(t) for t in toks[a: b]]
+            if top is None:
+                return label, new, False, ttft
+            return label, new, False, ttft, logprobs_content(new, logprob_pairs(lp, ids, a, b), top)
         try:
             while True:
-                _lib.check(_lib.lib.rr_gateway_peek(gw, ticket, sent, 0.05, toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
-                                                    C.byref(n), C.byref(done), C.byref(res)), "rr_gateway_peek")
+                _lib.check(_lib.lib.rr_gateway_peek_logprobs(gw, ticket, sent, 0.05, toks.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                             max_new, C.byref(n), C.byref(done), C.byref(res), lp_p, ids_p),
+                           "rr_gateway_peek")
                 if done.value:
-                    rc = _lib.lib.rr_gateway_wait(gw, ticket, 1.0, C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new)
+                    rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, 1.0, C.byref(res),
+                                                           toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
                     finished = True
                     if rc != 0:
                         raise self._gw_error(rc, model, res, timeout)
                     label = self.cfg.deployments[res.deployment].response_model
                     ttft = res.t_first_token_s - res.t_submit_s
                     if res.n_generated > sent:
-                        yield label, [int(t) for t in toks[sent: res.n_generated]], False, ttft
-                    yield label, [], True, ttft
+                        yield item(label, sent, res.n_generated, ttft)
+                    yield (label, [], True, ttft) if top is None else (label, [], True, ttft, [])
                     return
                 if n.value > sent and res.deployment >= 0:
                     label = self.cfg.deployments[res.deployment].response_model
-                    yield label, [int(t) for t in toks[sent: n.value]], False, 0.0
+                    yield item(label, sent, n.value, 0.0)
                     sent = n.value
                 if deadline is not None and time.perf_counter() > deadline:
                     _lib.lib.rr_gateway_cancel(gw, ticket, 1)
@@ -471,9 +540,19 @@ class Router:
         """Token ids must be valid on every replica a request may fall back to: the smallest vocabulary attached."""
         return min((b.vocab for b in self.backends.values()), default=128256)
 
+    def _logprobs_top(self, logprobs, top_logprobs) -> Optional[int]:
+        """Validated logprobs setting (None = off); only engine replicas have logits to serve it."""
+        top = check_logprobs(logprobs, top_logprobs)
+        if top is not None and self._gateway() is None:
+            raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
+        return top
+
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
-                   **_ignored) -> ModelResponse:
+                   logprobs: bool = False, top_logprobs: Optional[int] = None, **_ignored) -> ModelResponse:
+        """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
+        (0..20) most likely alternatives, as the OpenAI API returns them."""
+        top = self._logprobs_top(logprobs, top_logprobs)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -483,7 +562,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout)
+            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top)
         # ---- host loop (StubBackend): same admission events, one K1 launch per event
         t_start = time.perf_counter()
         chain_start = 0
@@ -519,10 +598,13 @@ class Router:
             chain_start = pos + 1
 
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
-                          max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None):
+                          max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
+                          logprobs: bool = False, top_logprobs: Optional[int] = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
-        (model_label, new_token_ids, done, ttft_s) as tokens arrive.  A backend failure before the first token walks the
+        (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
+        `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
         fallback chain; rate limiting raises RateLimitError before anything is yielded."""
+        top = self._logprobs_top(logprobs, top_logprobs)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -531,7 +613,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout)
+            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top)
             return
         deadline = None if not timeout else time.perf_counter() + timeout
         chain_start = 0

@@ -16,7 +16,7 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend)
+                     StubBackend, check_logprobs)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -38,14 +38,15 @@ def create_app(router: Router):
         import anyio.to_thread
         anyio.to_thread.current_default_thread_limiter().total_tokens = 2048
 
-    async def stream_completion(model, messages, body):
-        """Server-sent events in the OpenAI chunk format; the first chunk leaves when the first token exists (TTFT)."""
+    async def stream_completion(model, messages, body, lp_kw):
+        """Server-sent events in the OpenAI chunk format; the first chunk leaves when the first token exists (TTFT).
+        With logprobs, every chunk carries `logprobs.content` for the tokens of its delta (the closing chunk null)."""
         import json as _json
         import uuid
         from fastapi.responses import StreamingResponse
         from .router import detokenize
         gen = router.completion_stream(model=model, messages=messages, timeout=body.get("timeout"),
-                                       max_tokens=body.get("max_tokens"))
+                                       max_tokens=body.get("max_tokens"), **lp_kw)
         try:
             first = await run_in_threadpool(next, gen)            # admission errors surface before the 200
         except RateLimitError as e:
@@ -56,19 +57,21 @@ def create_app(router: Router):
             return JSONResponse(_error_body(e, "api_error"), e.status_code)
         cid = "chatcmpl-" + uuid.uuid4().hex[:24]
 
-        def chunk(label, toks, done):
+        def chunk(item):
+            label, toks, done = item[:3]
             delta = {} if done else {"role": "assistant", "content": detokenize(toks)}
+            choice = {"index": 0, "delta": delta, "finish_reason": "length" if done else None}
+            if lp_kw:
+                choice["logprobs"] = None if done else {"content": item[4], "refusal": None}
             return "data: " + _json.dumps({"id": cid, "object": "chat.completion.chunk", "created": int(time.time()),
-                                           "model": label, "choices": [{"index": 0, "delta": delta,
-                                                                        "finish_reason": "length" if done else None}]}) + "\n\n"
+                                           "model": label, "choices": [choice]}) + "\n\n"
 
         def events():
             try:
-                label, toks, done, _ = first
-                yield chunk(label, toks, done)
-                if not done:
-                    for label, toks, done, _ in gen:
-                        yield chunk(label, toks, done)
+                yield chunk(first)
+                if not first[2]:
+                    for item in gen:
+                        yield chunk(item)
                 yield "data: [DONE]\n\n"
             finally:
                 gen.close()        # client gone before the last chunk: the router cancels the request and frees its decode row
@@ -84,11 +87,18 @@ def create_app(router: Router):
         if not isinstance(model, str) or not isinstance(messages, list):
             return JSONResponse(_error_body(BadRequestError("`model` and `messages` are required"),
                                             "invalid_request_error"), 400)
+        try:
+            # passed on only when asked for: a request without them reaches the router exactly as before
+            lp_kw = {}
+            if check_logprobs(body.get("logprobs"), body.get("top_logprobs")) is not None:
+                lp_kw = {"logprobs": True, "top_logprobs": body.get("top_logprobs")}
+        except BadRequestError as e:
+            return JSONResponse(_error_body(e, "invalid_request_error"), 400)
         if body.get("stream"):
-            return await stream_completion(model, messages, body)
+            return await stream_completion(model, messages, body, lp_kw)
         try:
             resp = await run_in_threadpool(router.completion, model=model, messages=messages,
-                                           timeout=body.get("timeout"), max_tokens=body.get("max_tokens"))
+                                           timeout=body.get("timeout"), max_tokens=body.get("max_tokens"), **lp_kw)
             return JSONResponse(resp.model_dump())
         except RateLimitError as e:
             return JSONResponse(_error_body(e, "rate_limit_error"), 429, headers={"retry-after": "1"})
