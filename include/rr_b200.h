@@ -233,6 +233,24 @@ int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, v
 int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                        const int32_t* seq_start, const int32_t* seq_slot, int n_seqs, int max_len,
                        int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream);
+/* Prefill attention over a cached prompt prefix, as the engine runs it with prefix caching on (rr_engine_opts.prefix_cache):
+ * sequence i's seq_start[i + 1] - seq_start[i] query rows sit at positions seq_pos0[i] .. seq_pos0[i] + len - 1 of slot
+ * seq_slot[i] and attend to positions 0 .. own position of that slot's cache (positions < seq_pos0[i] hold the prefix).
+ * max_len = the longest len.  Caches [n_slots][n_kv_heads][ctx_max][128], q / out [T][n_heads * 128] bf16.  Row r of a
+ * sequence equals, bit for bit, row seq_pos0[i] + r of rr_op_prefill_attn over the whole sequence.  Returns
+ * RR_INVALID_ARGUMENT before touching the device for a null pointer, n_seqs or max_len below 1, a group size that does not
+ * divide, or ctx_max not a positive multiple of 64; and after reading the index arrays back, for a negative pos0, a
+ * sequence longer than max_len or pos0 + len > ctx_max. */
+int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out,
+                              const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                              int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream);
+/* KV prefix copy, one launch for a list of n_copies (src[i], dst[i], n_tok[i]) (host arrays): positions [0, n_tok[i]) of
+ * slot src[i] are copied to slot dst[i] in K and V, for every layer and kv head.  Caches [n_layers][n_slots][n_kv_heads]
+ * [ctx_max][128] bf16 (device).  No other byte changes.  Returns RR_INVALID_ARGUMENT before touching the device for a null
+ * pointer, n_copies outside 1..256, a slot outside [0, n_slots), n_tok outside 1..ctx_max, a destination listed twice, or a
+ * destination that is also a source in the same call. */
+int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                         const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies, void* stream);
 /* Fused decode MLP, one launch exactly as the engine runs it for a batch of `rows` (tile width, K slices, grid and
  * schedule from the engine's rules; env RR_MLP_STATIC / RR_NO_TMA_EPI are read per call):
  *   act[b, n]       = bf16(SiLU(xn[b] . gate[n]) * (xn[b] . up[n]))                        bf16 [rows, inter]
@@ -299,13 +317,17 @@ typedef struct rr_engine_opts {
     float fail_prob;              /* fault injection: P(request fails) (BASELINE config #4) */
     int32_t reserved[4];          /* A/B switches: [0] = 2 persistent decode layer kernel (rr_layer.cu; off by default, measured slower); [1] = 1 no RoPE fusion in the prefill
                                      QKV epilogue; [2] = 1 no fused decode MLP kernel; [3] = 1 prefill RMSNorm as separate kernels instead of deferred into the GEMM epilogues */
+    int32_t prefix_cache;         /* 1: prompt prefix caching.  A slot keeps the prompt KV its last prefill wrote; a new prompt
+                                     sharing >= 64 leading tokens with one is prefilled from there on (the prefix is copied
+                                     when that slot is busy).  Tokens and logits are bit-identical to a cold prefill.  Off
+                                     by default: a resident prefix is a timing side channel between the engine's users. */
 } rr_engine_opts;
 
 int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w,
                      const rr_engine_opts* opts, rr_engine** out);
 void rr_engine_destroy(rr_engine* e);
 
-/* Low-level synchronous steps (parity tests).  Host buffers.
+/* Low-level synchronous steps (parity tests).  Host buffers.  Both forget every retained prompt prefix (prefix_cache).
  * prefill: n_seqs prompts concatenated in `ids`; seq_start[n_seqs+1]; slots[n_seqs] = KV slots.
  *          Writes first generated token per prompt to first_tok[n_seqs].
  *          If logits_out != NULL: fp32 [n_seqs, vocab] last-position logits. */
@@ -324,7 +346,7 @@ typedef struct rr_completion {
     int32_t status;               /* RR_OK / RR_BACKEND_FAILED / RR_TIMEOUT */
     int32_t n_prompt;
     int32_t n_generated;
-    int32_t reserved;
+    int32_t n_cached;             /* prompt tokens whose KV came from the prefix cache (prefix_cache; 0 otherwise) */
     double t_submit_s, t_first_token_s, t_done_s;   /* engine monotonic clock */
 } rr_completion;
 
@@ -367,6 +389,8 @@ typedef struct rr_engine_stats {
     double decode_ms_total, prefill_ms_total;   /* CUDA-event time on the engine stream */
     int32_t active_rows, queued;
     uint64_t h2d_bytes, d2h_bytes;
+    /* prefix_cache: requests that hit, prompt tokens they did not prefill, tokens copied between slots */
+    uint64_t prefix_hits, prefix_cached_tokens, kv_copy_tokens;
 } rr_engine_stats;
 int rr_engine_get_stats(rr_engine* e, rr_engine_stats* out);
 int rr_engine_reset_stats(rr_engine* e);
@@ -398,6 +422,8 @@ typedef struct rr_gateway_result {
     int32_t n_prompt, n_generated;
     int32_t attempts;          /* admissions this request went through (1 + backends that failed under it) */
     double t_submit_s, t_admit_s, t_first_token_s, t_done_s;   /* gateway monotonic clock, seconds */
+    int32_t n_cached;          /* rr_completion.n_cached of the engine that served the request */
+    int32_t reserved;
 } rr_gateway_result;
 
 typedef struct rr_gateway_stats {

@@ -78,12 +78,13 @@ class ModelWeights(C.Structure):
 class EngineOpts(C.Structure):
     _fields_ = [("device", C.c_int32), ("max_batch", C.c_int32), ("ctx_max", C.c_int32),
                 ("max_prefill_tokens", C.c_int32), ("use_cuda_graph", C.c_int32),
-                ("fail_seed", C.c_int32), ("fail_prob", C.c_float), ("reserved", C.c_int32 * 4)]
+                ("fail_seed", C.c_int32), ("fail_prob", C.c_float), ("reserved", C.c_int32 * 4),
+                ("prefix_cache", C.c_int32)]
 
 
 class Completion(C.Structure):
     _fields_ = [("ticket", C.c_uint64), ("status", C.c_int32), ("n_prompt", C.c_int32),
-                ("n_generated", C.c_int32), ("reserved", C.c_int32),
+                ("n_generated", C.c_int32), ("n_cached", C.c_int32),
                 ("t_submit_s", C.c_double), ("t_first_token_s", C.c_double),
                 ("t_done_s", C.c_double)]
 
@@ -93,7 +94,8 @@ class EngineStats(C.Structure):
                 ("prefill_chunks", C.c_uint64), ("prefill_tokens", C.c_uint64),
                 ("generated_tokens", C.c_uint64), ("decode_ms_total", C.c_double),
                 ("prefill_ms_total", C.c_double), ("active_rows", C.c_int32),
-                ("queued", C.c_int32), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64)]
+                ("queued", C.c_int32), ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64),
+                ("prefix_hits", C.c_uint64), ("prefix_cached_tokens", C.c_uint64), ("kv_copy_tokens", C.c_uint64)]
 
 
 class GatewayOpts(C.Structure):
@@ -105,7 +107,8 @@ class GatewayResult(C.Structure):
     _fields_ = [("ticket", C.c_uint64), ("status", C.c_int32), ("deployment", C.c_int32), ("served_group", C.c_int32),
                 ("chain_pos", C.c_int32), ("replica", C.c_int32), ("n_prompt", C.c_int32), ("n_generated", C.c_int32),
                 ("attempts", C.c_int32), ("t_submit_s", C.c_double), ("t_admit_s", C.c_double),
-                ("t_first_token_s", C.c_double), ("t_done_s", C.c_double)]
+                ("t_first_token_s", C.c_double), ("t_done_s", C.c_double), ("n_cached", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 class GatewayStats(C.Structure):
@@ -155,6 +158,9 @@ PROTOTYPES = {
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp]),
+    "rr_op_prefill_attn_cached": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                            C.c_int, C.c_float, vp]),
+    "rr_op_kv_copy_prefix": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp]),

@@ -6,8 +6,9 @@ Keeps the keys the reference's config/config.yaml uses (reference config/config.
 YAML anchors / merge keys (`<<: *aws-defaults`, :40) are resolved by PyYAML.  AWS-only keys
 (`aws_region_name`, `aws_profile_name`, the `aws:` / `cris:` sections) are accepted and ignored.
 `router_settings.routing_strategy_args` takes litellm's latency-based-routing keys (`lowest_latency_buffer`,
-`max_latency_list_size`, `ttl`).  Local extension: `litellm_params.gpu: N` pins a deployment to a replica; `litellm_params.model:
-b200/<spec>` names an on-box model (models.SPECS) instead of `bedrock/<id>`.
+`max_latency_list_size`, `ttl`).  Local extensions: `litellm_params.gpu: N` pins a deployment to a replica; `litellm_params.model:
+b200/<spec>` names an on-box model (models.SPECS) instead of `bedrock/<id>`; `litellm_params.prefix_cache: true` turns on
+prompt prefix caching in the replica (deployments on one GPU share its engine, so they must agree).
 """
 from __future__ import annotations
 
@@ -41,6 +42,7 @@ class DeploymentCfg:
     tpm: int = -1
     weight: int = -1           # simple-shuffle weight (litellm_params.weight / rpm / tpm), -1 = unset
     gpu: int = 0
+    prefix_cache: bool = False  # litellm_params.prefix_cache: the replica reuses cached prompt prefixes
     params: Dict[str, Any] = field(default_factory=dict)
 
     @property
@@ -125,8 +127,16 @@ def build_config(model_list: List[dict], router_settings: Optional[dict] = None,
         # limits: top level of the entry (reference config.yaml:41-42) or inside litellm_params
         rpm = _int_or(entry.get("rpm", lp.get("rpm")))
         tpm = _int_or(entry.get("tpm", lp.get("tpm")))
+        pc = lp.get("prefix_cache", False)
+        if not isinstance(pc, bool):
+            raise ValueError(f"model_list[{i}].litellm_params.prefix_cache must be true or false, got {pc!r}")
         deps.append(DeploymentCfg(index=i, model_name=name, model=lp["model"], group=groups.index(name),
-                                  rpm=rpm, tpm=tpm, gpu=int(lp.get("gpu", 0)), params=lp))
+                                  rpm=rpm, tpm=tpm, gpu=int(lp.get("gpu", 0)), prefix_cache=pc, params=lp))
+    for d in deps:                       # one engine per GPU: its deployments share the setting
+        first = next(x for x in deps if x.gpu == d.gpu)
+        if d.prefix_cache != first.prefix_cache:
+            raise ValueError(f"model_list[{first.index}] and model_list[{d.index}] share gpu {d.gpu} but disagree on "
+                             "litellm_params.prefix_cache")
     # simple-shuffle weights: the first of weight / rpm / tpm present in the litellm_params of the
     # group's first deployment decides the key for the whole group (oracle/router.py header).
     for g in range(len(groups)):

@@ -369,3 +369,53 @@ RR_API int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_
     if (rcl != RR_OK) return rcl;
     return check_last();
 }
+
+// Prefill attention with a cached prefix per sequence (seq_pos0): the engine's launch.  Like rr_op_prefill_attn, the TMA
+// maps need the extents of q and of the caches, read back from the caller's index arrays; the positions are checked
+// against ctx_max on the way.
+RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                     const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                                     int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream) {
+    if (!q || !k_cache || !v_cache || !out || !seq_start || !seq_slot || !seq_pos0) return RR_INVALID_ARGUMENT;
+    if (n_seqs < 1 || max_len < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
+    if (ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<int32_t> h(3 * (size_t)n_seqs + 1);         // seq_start[n + 1] | seq_slot[n] | seq_pos0[n]
+    cudaError_t e = cudaMemcpyAsync(h.data(), seq_start, sizeof(int32_t) * (n_seqs + 1), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h[n_seqs + 1], seq_slot, sizeof(int32_t) * n_seqs, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&h[2 * n_seqs + 1], seq_pos0, sizeof(int32_t) * n_seqs, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { note_cuda_error(e); return RR_CUDA_ERROR; }
+    int max_slot = 0;
+    for (int i = 0; i < n_seqs; ++i) {
+        const int len = h[i + 1] - h[i], slot = h[n_seqs + 1 + i], p0 = h[2 * n_seqs + 1 + i];
+        if (len < 0 || len > max_len || slot < 0 || p0 < 0 || p0 + len > ctx_max) return RR_INVALID_ARGUMENT;
+        max_slot = slot > max_slot ? slot : max_slot;
+    }
+    PrefillAttnArgs a;
+    a.q = (const __nv_bfloat16*)q; a.k_cache = (const __nv_bfloat16*)k_cache;
+    a.v_cache = (const __nv_bfloat16*)v_cache; a.out = (__nv_bfloat16*)out; a.seq_start = seq_start;
+    a.seq_slot = seq_slot; a.seq_pos0 = seq_pos0; a.n_seqs = n_seqs; a.max_len = max_len; a.n_heads = n_heads;
+    a.n_kv_heads = n_kv_heads; a.ctx_max = ctx_max; a.scale = scale; a.head_dim = 128;
+    (void)prefill_attn_make_maps(&a, h[n_seqs], (long long)(max_slot + 1) * n_kv_heads * ctx_max);
+    const int rcl = launch_prefill_attn(a, st);
+    if (rcl != RR_OK) return rcl;
+    return check_last();
+}
+
+// Prefix copy between KV slots as the engine runs it at the start of a prefill chunk.  The lists are host arrays, checked
+// before the device is touched.
+RR_API int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                                const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies, void* stream) {
+    if (!k_cache || !v_cache || !src || !dst || !n_tok) return RR_INVALID_ARGUMENT;
+    if (n_layers < 1 || n_slots < 1 || n_kv_heads < 1 || ctx_max < 1 || n_copies < 1 || n_copies > KV_COPY_MAX)
+        return RR_INVALID_ARGUMENT;
+    KvCopyList c;
+    c.count = n_copies;
+    for (int i = 0; i < n_copies; ++i) { c.src[i] = src[i]; c.dst[i] = dst[i]; c.n[i] = n_tok[i]; }
+    if (kv_copy_check(c, n_slots, ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
+    if (launch_kv_copy((__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, n_layers, n_slots, n_kv_heads, ctx_max, c,
+                       (cudaStream_t)stream) != RR_OK)
+        note_cuda_error(cudaPeekAtLastError());
+    return check_last();
+}

@@ -14,6 +14,11 @@
 // tile of warpgroup 0) is only waited for and released.
 //
 // Work item = (sequence, query head, 128-row query tile), heaviest (last) query tiles first, strided over the CTAs.
+// Prefix caching: a sequence's `len` query rows may sit at positions pos0 .. pos0 + len - 1 of its slot (seq_pos0; the
+// prefix 0 .. pos0 - 1 is already in the cache).  They attend to positions 0 .. own position; the key tiles, the causal
+// mask and the skip test use absolute positions, Q stays at the sequence's rows of q.  A query row visits key tiles
+// 0, 1, ... in order whatever its tile, and a fully masked tile leaves m, l and O bit-unchanged (alpha = 1, P = 0 against
+// finite V), so a row's output does not depend on pos0: it is the row of a cold run over the whole sequence, bit for bit.
 // Any GQA group size (MHA included): the kv head is head / (n_heads / n_kv_heads).  Head dims below 128 (Phi-3-mini:
 // 96) are zero-padded to 128 in q and the caches; only the true head dim is written.
 //
@@ -52,18 +57,19 @@ __device__ __forceinline__ float ex2(float x) {
 }
 
 struct Work {
-    int qt, seq, head, tok0, len, n_kt;
+    int qt, seq, head, tok0, len, pos0, n_kt;
 };
-// Work item w -> (query tile, sequence, head).  The sequence bounds (and the slot, for the producer)
+// Work item w -> (query tile, sequence, head).  The sequence bounds, its first position (and the slot, for the producer)
 // are loaded one item ahead (WorkFetch) so their latency hides under the current item.
 struct WorkFetch {
-    int tok0 = 0, tok1 = 0, slot = 0;
+    int tok0 = 0, tok1 = 0, pos0 = 0, slot = 0;
 };
 __device__ __forceinline__ void fetch_work(const PrefillAttnArgs& a, int w, int n_work, bool want_slot, WorkFetch& f) {
     if (w >= n_work) return;
     const int seq = (w % (a.n_seqs * a.n_heads)) / a.n_heads;
     f.tok0 = __ldg(a.seq_start + seq);
     f.tok1 = __ldg(a.seq_start + seq + 1);
+    f.pos0 = a.seq_pos0 ? __ldg(a.seq_pos0 + seq) : 0;
     if (want_slot) f.slot = __ldg(a.seq_slot + seq);
 }
 __device__ __forceinline__ bool decode_work(const PrefillAttnArgs& a, int w, int max_qt, const WorkFetch& f, Work& k) {
@@ -74,9 +80,11 @@ __device__ __forceinline__ bool decode_work(const PrefillAttnArgs& a, int w, int
     k.head = rem - k.seq * a.n_heads;
     k.tok0 = f.tok0;
     k.len = f.tok1 - f.tok0;
+    k.pos0 = f.pos0;
     if (k.qt * TQ >= k.len) return false;
-    const int causal = 2 * k.qt + 2, avail = (k.len + TKV - 1) / TKV;
-    k.n_kt = causal < avail ? causal : avail;
+    // key tiles up to the tile's last query position (absolute: the cached prefix comes first)
+    const int rows = (k.qt + 1) * TQ < k.len ? (k.qt + 1) * TQ : k.len;
+    k.n_kt = (k.pos0 + rows + TKV - 1) / TKV;
     return true;
 }
 
@@ -150,8 +158,9 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             fetch_work(a, w + gridDim.x, n_work, false, nf);
             if (!decode_work(a, w, max_qt, f, k)) continue;
             const int q0 = k.qt * TQ + r_in;                         // query indices inside the sequence
-            const int last0 = min(q0, k.len - 1), last1 = min(q0 + 8, k.len - 1);   // causal / ragged bound (inclusive)
-            const int wg_last_row = k.qt * TQ + 64 * g + 63;
+            // causal / ragged bound (inclusive) and the warpgroup's last row, as absolute positions of the slot
+            const int last0 = k.pos0 + min(q0, k.len - 1), last1 = k.pos0 + min(q0 + 8, k.len - 1);
+            const int wg_last_row = k.pos0 + k.qt * TQ + 64 * g + 63;
             float o[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) o[i] = 0.f;

@@ -255,6 +255,21 @@ void launch_add_rmsnorm(float* x, PartIn part, const __nv_bfloat16* w, __nv_bflo
                    rowss_out, n_part_out);
 }
 
+// Prefill chunks: the kernel, and so the order of the sum of squares, depends on the hidden size only, never on the row
+// count, so a token's bits do not depend on how many tokens share its chunk (a prefix-cache hit must reproduce a cold
+// prefill exactly).  These are the kernels chunks of more than 256 rows always ran.
+void launch_add_rmsnorm_pf(float* x, const __nv_bfloat16* w, __nv_bfloat16* xn, int rows, int hidden, float eps,
+                           cudaStream_t st, float* rowss_out, int n_part_out) {
+    if (rows <= 0 || hidden > 8192) return;
+    PartIn none; none.ptr = nullptr; none.is_bf16 = 0; none.n_splits = 1; none.split_stride = 0; none.ld = 0;
+    if (hidden <= 4096)
+        launch_pdl(add_rmsnorm_kernel<256, 4>, dim3(rows), dim3(256), 0, st, x, none, w, xn, hidden, eps, (unsigned*)nullptr, 0,
+                   rowss_out, n_part_out);
+    else
+        launch_pdl(add_rmsnorm_kernel<256, 8>, dim3(rows), dim3(256), 0, st, x, none, w, xn, hidden, eps, (unsigned*)nullptr, 0,
+                   rowss_out, n_part_out);
+}
+
 // ---- SiLU(gate) * up -----------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 silu_mul_kernel(PartIn gu, __nv_bfloat16* __restrict__ act, int inter) {

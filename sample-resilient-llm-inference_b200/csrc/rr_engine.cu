@@ -60,17 +60,18 @@ __global__ void gather_last_kernel(const __nv_bfloat16* __restrict__ attn, const
     for (int c = threadIdx.x; c < hidden / 4; c += blockDim.x) xo[c] = xs[c];
 }
 
-// After a prefill chunk: row/slot s becomes an active decode row fed with its first token.
+// After a prefill chunk: row/slot s becomes an active decode row fed with its first token, at the position after the
+// prompt's last (a cached prefix included).
 __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const int32_t* __restrict__ first_tok,
-                                     const int32_t* __restrict__ seq_start, int n, int32_t* __restrict__ d_tok,
-                                     int32_t* __restrict__ d_pos, int32_t* __restrict__ d_slot) {
+                                     const int32_t* __restrict__ tok_pos, const int32_t* __restrict__ last, int n,
+                                     int32_t* __restrict__ d_tok, int32_t* __restrict__ d_pos, int32_t* __restrict__ d_slot) {
     griddep_launch();
     griddep_wait();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const int s = seq_slot[i];
     d_tok[s] = first_tok[i];
-    d_pos[s] = seq_start[i + 1] - seq_start[i];
+    d_pos[s] = tok_pos[last[i]] + 1;
     d_slot[s] = s;
 }
 
@@ -89,7 +90,12 @@ struct Request {
     int top_lp = -1;           // rr_engine_submit_logprobs: -1 off, else max(1, top_lp) (logprob, id) pairs per token
     std::vector<float> lp;     // [out.size()][max(1, top_lp)]
     std::vector<int32_t> lp_id;
+    int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
 };
+
+// Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
+// prefixes (a BOS and a role tag) stay misses.
+constexpr int PREFIX_MIN = 64;
 
 }  // namespace rr
 
@@ -182,6 +188,12 @@ struct rr_engine {
     bool slots_dirty = false;
     std::vector<int32_t> h_topn_mirror;  // host mirror of d_topn (uploaded before a step that replays graph_lp)
     bool topn_dirty = false;
+    // prefix caching (o.prefix_cache), under mu: retained[b] = the prompt tokens whose KV the last successful prefill into
+    // slot b wrote (computed or copied; never a position decode wrote, since decode rounds differently), kept after the
+    // request ends; retained_used[b] = LRU stamp.  index_epoch counts the low-level calls that cleared every list.
+    std::vector<std::vector<int32_t>> retained;
+    std::vector<uint64_t> retained_used;
+    uint64_t lru_clock = 0, index_epoch = 0;
     std::thread worker;
     std::atomic<bool> stop{false};
     uint64_t next_ticket = 1;
@@ -407,32 +419,41 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 // ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
 // activates the rows. Caller holds gpu_mu.  topn_host[n_seqs] (optional): sequences with topn_host[i] >= 0 also get their
 // first token's logprobs in e->h_lp / e->h_lp_id row i.
+// Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
+// position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
-                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr) {
+                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr,
+                       const int32_t* pos0 = nullptr, const KvCopyList* copies = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
     cudaStream_t s = e->stream;
-    // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n]
+    // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n] (| pos0[n])
     int32_t* h = e->h_stage;
     int32_t *h_ids = h, *h_pos = h + T, *h_slt = h + 2 * T, *h_ss = h + 3 * T, *h_sl = h_ss + n_seqs + 1,
-            *h_last = h_sl + n_seqs;
+            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs;
     int max_len = 0;
     memcpy(h_ids, ids, sizeof(int32_t) * T);
     for (int i = 0; i < n_seqs; ++i) {
-        const int a = seq_start[i], b = seq_start[i + 1];
-        if (b <= a || b - a + 1 > e->o.ctx_max || slots[i] < 0 || slots[i] >= e->Bm) return RR_INVALID_ARGUMENT;
-        for (int t = a; t < b; ++t) { h_pos[t] = t - a; h_slt[t] = slots[i]; }
+        const int a = seq_start[i], b = seq_start[i + 1], p0 = pos0 ? pos0[i] : 0;
+        if (b <= a || p0 < 0 || p0 + b - a + 1 > e->o.ctx_max || slots[i] < 0 || slots[i] >= e->Bm) return RR_INVALID_ARGUMENT;
+        for (int t = a; t < b; ++t) { h_pos[t] = p0 + t - a; h_slt[t] = slots[i]; }
         h_ss[i] = a; h_sl[i] = slots[i]; h_last[i] = b - 1;
+        if (pos0) h_p0[i] = p0;
         if (b - a > max_len) max_len = b - a;
     }
     h_ss[n_seqs] = T;
-    const size_t n_ints = (size_t)3 * T + 3 * n_seqs + 1;
+    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1;
+    uint64_t copy_tokens = 0;
+    if (copies && copies->count > 0) {
+        if (kv_copy_check(*copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
+        for (int i = 0; i < copies->count; ++i) copy_tokens += copies->n[i];
+    }
     CK(cudaEventRecord(e->ev0, s));
     CK(cudaMemcpyAsync(e->p_ids, h, n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     e->st.h2d_bytes += n_ints * sizeof(int32_t);
     int32_t *p_ids = e->p_ids, *p_pos = p_ids + T, *p_slt = p_ids + 2 * T, *p_ss = p_ids + 3 * T,
-            *p_sl = p_ss + n_seqs + 1, *p_last = p_sl + n_seqs;
+            *p_sl = p_ss + n_seqs + 1, *p_last = p_sl + n_seqs, *p_p0 = p_last + n_seqs;
 
     // One set of plans (4 L TMA descriptors) built for Tmax rows; the live row count is a launch argument: TMA reads of
     // rows >= T stay inside the Tmax-row buffers and every store is guarded by rowsA.
@@ -441,12 +462,17 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     if (rc != RR_OK) return rc;
     auto launch_rows = [&](const GemmPlan& pl) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s); };
     uint64_t nl = 0;
+    if (copy_tokens) {      // cached prefixes of busy slots into this chunk's slots, before any layer reads them
+        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, e->Bm, d.n_kv_heads, e->o.ctx_max, *copies, s) != RR_OK)
+            return RR_CUDA_ERROR;
+        ++nl;
+    }
     launch_embed(p_ids, (const __nv_bfloat16*)e->embed, e->px, T, d.hidden, nullptr, s); ++nl;
     if (e->defer_norm_pf)       // layer 0's operand in the deferred form: bf16(x * gamma), sum(x^2) in partial 0
-        launch_add_rmsnorm(e->px, part_none(), (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s,
-                           nullptr, 0, e->p_rowss, e->pf_parts);
+        launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s, e->p_rowss,
+                              e->pf_parts);
     else
-        launch_add_rmsnorm(e->px, part_none(), (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s);
+        launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s);
     ++nl;
     for (int l = 0; l < d.n_layers; ++l) {
         __nv_bfloat16* kc = e->kcache + (size_t)l * e->kv_layer_stride;
@@ -463,7 +489,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer TMA maps made at create
         pa.q = e->pq; pa.k_cache = kc; pa.v_cache = vc; pa.out = e->pattn; pa.seq_start = p_ss; pa.seq_slot = p_sl;
-        pa.n_seqs = n_seqs; pa.max_len = max_len; pa.n_heads = d.n_heads; pa.n_kv_heads = d.n_kv_heads;
+        pa.seq_pos0 = pos0 ? p_p0 : nullptr; pa.n_seqs = n_seqs; pa.max_len = max_len; pa.n_heads = d.n_heads; pa.n_kv_heads = d.n_kv_heads;
         pa.ctx_max = e->o.ctx_max; pa.scale = 1.0f / sqrtf((float)d.head_dim); pa.head_dim = d.head_dim;
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (l + 1 == d.n_layers) {
@@ -483,21 +509,20 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         }
         if (launch_rows(P->o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->defer_norm_pf) {
-            launch_add_rmsnorm(e->px, part_none(), (const __nv_bfloat16*)e->norm_mlp[l], e->pxn, T,
-                               d.hidden, d.rms_eps, s); ++nl;
+            launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_mlp[l], e->pxn, T, d.hidden, d.rms_eps, s); ++nl;
         }
         if (launch_rows(P->gu[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->fuse_silu) { launch_silu_mul(part_bf16(e->pgu, 2 * d.inter), e->pact, T, d.inter, s); ++nl; }
         if (launch_rows(P->down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->defer_norm_pf) {
-            launch_add_rmsnorm(e->px, part_none(), (const __nv_bfloat16*)e->norm_attn[l + 1], e->pxn, T, d.hidden,
-                               d.rms_eps, s); ++nl;
+            launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[l + 1], e->pxn, T, d.hidden, d.rms_eps, s); ++nl;
         }
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
     launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
-               (const int32_t*)e->p_first, (const int32_t*)p_ss, n_seqs, e->d_tok, e->d_pos, e->d_slot); ++nl;
+               (const int32_t*)e->p_first, (const int32_t*)p_pos, (const int32_t*)p_last, n_seqs, e->d_tok, e->d_pos,
+               e->d_slot); ++nl;
     bool lp = false;
     for (int i = 0; topn_host && i < n_seqs; ++i) lp = lp || topn_host[i] >= 0;
     if (lp) {
@@ -522,6 +547,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     e->st.prefill_ms_total += ms;
     e->st.prefill_chunks += 1;
     e->st.prefill_tokens += T;
+    e->st.kv_copy_tokens += copy_tokens;
     e->st.kernel_launches += nl;
     for (int i = 0; i < n_seqs; ++i) {
         if (first_tok_host) first_tok_host[i] = e->h_tok[i];
@@ -564,17 +590,62 @@ static void run_hooks(rr_engine* e, std::vector<DoneNote>& notes) {
     notes.clear();
 }
 
+// Caller holds e->mu.  Prefix caching: the slot a prompt p is admitted into and how many of its tokens are cached there.
+// m_b = the longest common prefix of retained[b] and p, capped at |p| - 1 (the last prompt token is always prefilled: its
+// logits give the first token); a hit needs m_b >= PREFIX_MIN.  The best m wins, then a free slot, then the lower index.
+// A hit on a free slot takes that slot as it is; a hit on a busy slot (*src = it) copies m tokens into the slot a miss
+// takes: the lowest free slot with nothing retained, else the free slot whose prefix was used least recently.  Slots taken
+// in the current chunk have nothing retained, so requests of one chunk never share.  false: no free slot.
+static bool pick_slot_cached(const rr_engine* e, const std::vector<int32_t>& p, int* slot, int* m, int* src) {
+    const int cap = (int)p.size() - 1;
+    int best = -1, best_m = 0;
+    bool best_free = false;
+    for (int b = 0; b < e->Bm; ++b) {
+        const std::vector<int32_t>& R = e->retained[b];
+        const int lim = (int)R.size() < cap ? (int)R.size() : cap;
+        int k = 0;
+        while (k < lim && R[k] == p[k]) ++k;
+        if (k < PREFIX_MIN) continue;
+        const bool fr = e->row_req[b] == nullptr;
+        if (k > best_m || (k == best_m && fr && !best_free)) { best = b; best_m = k; best_free = fr; }
+    }
+    *m = best >= 0 ? best_m : 0;
+    *src = -1;
+    if (best >= 0 && best_free) { *slot = best; return true; }
+    int fresh = -1;
+    for (int b = 0; b < e->Bm; ++b) {
+        if (e->row_req[b]) continue;
+        if (e->retained[b].empty()) { fresh = b; break; }
+        if (fresh < 0 || e->retained_used[b] < e->retained_used[fresh]) fresh = b;
+    }
+    if (fresh < 0) return false;
+    *slot = fresh;
+    *src = best;
+    return true;
+}
+
+// Caller holds gpu_mu.  A low-level call writes slots behind the index's back: forget every retained prefix.
+static void forget_prefixes(rr_engine* e) {
+    if (!e->o.prefix_cache) return;
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (auto& R : e->retained) R.clear();
+    ++e->index_epoch;
+}
+
 static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
-    std::vector<int32_t> ids, seq_start, slots, topn;
+    std::vector<int32_t> ids, seq_start, slots, topn, pos0;
     std::vector<Request*> chunk;
     std::vector<DoneNote> notes;
+    KvCopyList* copies = new KvCopyList();
     while (!e->stop.load()) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
-        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); topn.clear();
+        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); topn.clear(); pos0.clear();
+        copies->count = 0;
         int active = 0;
         bool lp_step = false;
+        uint64_t epoch = 0;
         {
             std::unique_lock<std::mutex> lk(e->mu);
             for (int b = 0; b < e->Bm; ++b) {
@@ -593,18 +664,34 @@ static void worker_main(rr_engine* e) {
                 continue;
             }
             int b = 0;
+            epoch = e->index_epoch;
             while (!e->waiting.empty()) {
                 Request* r = e->waiting.front();
-                if ((int)ids.size() + (int)r->prompt.size() > e->Tmax) break;
-                while (b < e->Bm && e->row_req[b] != nullptr) ++b;
-                if (b >= e->Bm) break;
+                int m = 0, src = -1;
+                if (e->o.prefix_cache) {
+                    if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
+                } else {
+                    while (b < e->Bm && e->row_req[b] != nullptr) ++b;
+                    if (b >= e->Bm) break;
+                }
+                if ((int)ids.size() + (int)r->prompt.size() - m > e->Tmax) break;   // a chunk holds Tmax uncached tokens
                 e->waiting.pop_front();
                 e->row_req[b] = r;
                 r->slot = b;
+                r->n_cached = m;
+                if (e->o.prefix_cache) {
+                    if (m > 0) e->retained_used[src >= 0 ? src : b] = ++e->lru_clock;
+                    if (src >= 0) {
+                        const int c = copies->count++;
+                        copies->src[c] = src; copies->dst[c] = b; copies->n[c] = m;
+                    }
+                    e->retained[b].clear();                // rewritten by this chunk; set again once its prefill succeeds
+                    pos0.push_back(m);
+                }
                 chunk.push_back(r);
                 slots.push_back(b);
                 topn.push_back(r->top_lp);
-                ids.insert(ids.end(), r->prompt.begin(), r->prompt.end());
+                ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
             }
@@ -613,9 +700,23 @@ static void worker_main(rr_engine* e) {
         }
         std::lock_guard<std::mutex> gl(e->gpu_mu);
         std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
+        if (!chunk.empty() && e->o.prefix_cache) {
+            // a low-level call took the GPU between admission and here and cleared the index: its matches may be stale,
+            // so the chunk goes back to the head of the queue and is admitted again
+            std::lock_guard<std::mutex> lk(e->mu);
+            if (e->index_epoch != epoch) {
+                for (size_t i = chunk.size(); i-- > 0;) {
+                    Request* r = chunk[i];
+                    e->row_req[r->slot] = nullptr;
+                    r->slot = -1; r->n_cached = 0;
+                    e->waiting.push_front(r);
+                }
+                continue;
+            }
+        }
         if (!chunk.empty()) {
             int rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 topn.data());
+                                 topn.data(), e->o.prefix_cache ? pos0.data() : nullptr, copies);
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
@@ -625,6 +726,11 @@ static void worker_main(rr_engine* e) {
                     e->h_slot_mirror[r->slot] = -1; e->slots_dirty = true;
                     finish_request(e, r, RR_INTERNAL, &notes);
                     continue;
+                }
+                if (e->o.prefix_cache) {
+                    e->retained[r->slot] = r->prompt;
+                    e->retained_used[r->slot] = ++e->lru_clock;
+                    if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
                 r->t_first = t;
                 r->out.push_back(e->h_tok[i]);
@@ -697,6 +803,7 @@ static void worker_main(rr_engine* e) {
         e->cv_done.notify_all();
     }
     run_hooks(e, notes);
+    delete copies;
 }
 
 // ---------------------------------------------------------------- C-ABI
@@ -775,7 +882,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         if (ks > 1) TRY(dalloc(e, &e->attn_ws, decode_attn_ws_bytes(B, d.n_heads, ks) / sizeof(float)));
     }
     const int T = e->Tmax;
-    TRY(dalloc(e, &e->p_ids, (size_t)3 * T + 3 * B + 8));
+    TRY(dalloc(e, &e->p_ids, (size_t)3 * T + 4 * B + 8));
     TRY(dalloc(e, &e->p_first, B));
     TRY(dalloc(e, &e->px, (size_t)T * d.hidden, false));
     TRY(dalloc(e, &e->pxn, (size_t)T * d.hidden, false));
@@ -785,7 +892,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->po, (size_t)T * d.hidden, false));
     TRY(dalloc(e, &e->pgu, (size_t)T * 2 * d.inter, false));
     TRY(dalloc(e, &e->pact, (size_t)T * d.inter, false));
-    e->h_stage_ints = (size_t)3 * T + 3 * B + 8;
+    e->h_stage_ints = (size_t)3 * T + 4 * B + 8;
     TRYC(cudaMallocHost(&e->h_stage, e->h_stage_ints * sizeof(int32_t)));
     TRYC(cudaMallocHost(&e->h_tok, sizeof(int32_t) * (B > 16 ? B : 16)));
     TRY(dalloc(e, &e->d_topn, B)); TRY(dalloc(e, &e->d_topn_pf, B));
@@ -920,6 +1027,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->row_req.assign(B, nullptr);
     e->h_slot_mirror.assign(B, -1);
     e->h_topn_mirror.assign(B, -1);
+    if (e->o.prefix_cache) { e->retained.assign(B, {}); e->retained_used.assign(B, 0); }
     e->worker = std::thread(worker_main, e);
     *out = e;
     return RR_OK;
@@ -954,6 +1062,7 @@ RR_API int rr_engine_prefill(rr_engine* e, const int32_t* ids, const int32_t* se
     if (!e || !ids || !seq_start || !slots || n_seqs < 1) return RR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> gl(e->gpu_mu);
     std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
+    forget_prefixes(e);
     CK(cudaSetDevice(e->o.device));
     return run_prefill(e, ids, seq_start, slots, n_seqs, first_tok, logits_out);
 }
@@ -963,6 +1072,7 @@ RR_API int rr_engine_decode_step(rr_engine* e, const int32_t* slots, const int32
     if (!e || !slots || !tok || !pos || n < 1 || n > e->Bm || !next_tok) return RR_INVALID_ARGUMENT;
     std::lock_guard<std::mutex> gl(e->gpu_mu);
     std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
+    forget_prefixes(e);
     CK(cudaSetDevice(e->o.device));
     const int B = e->Bm;
     int32_t* h = e->h_stage;                 // tok[B] | pos[B] | slot[B]
@@ -1165,7 +1275,7 @@ RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout
         }
     }
     out->ticket = ticket; out->status = r->status; out->n_prompt = (int)r->prompt.size();
-    out->n_generated = (int)r->out.size(); out->reserved = 0;
+    out->n_generated = (int)r->out.size(); out->n_cached = r->n_cached;
     out->t_submit_s = r->t_submit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
     if (tokens_out) {
         const int n = (int)r->out.size() < max_tokens_out ? (int)r->out.size() : max_tokens_out;

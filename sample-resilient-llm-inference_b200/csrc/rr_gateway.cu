@@ -48,6 +48,7 @@ struct GwReq {
     int top_lp = -1;                  // rr_gateway_submit_logprobs: handed to every engine the request is admitted to
     std::vector<float> lp;            // [tokens.size()][max(1, top_lp)]
     std::vector<int32_t> lp_id;
+    int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
 };
@@ -153,6 +154,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
                 r->lp_id.assign(lp_ids.begin(), lp_ids.begin() + r->tokens.size() * k);
             }
             r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
+            r->n_cached = comp.n_cached;
         }
         if (status == RR_OK) {
             // latency sample: the engine's submit -> done time of the request, in microseconds
@@ -180,6 +182,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
                 r->eng = nullptr;
                 r->tokens.clear();
                 r->lp.clear(); r->lp_id.clear();
+                r->n_cached = 0;
                 g->st.failed_over++;
                 g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
             }
@@ -432,6 +435,7 @@ static void gw_fill(const GwReq* r, rr_gateway_result* out) {
     out->replica = r->replica; out->n_prompt = (int32_t)r->prompt.size(); out->n_generated = (int32_t)r->tokens.size();
     out->attempts = r->attempts;
     out->t_submit_s = r->t_submit; out->t_admit_s = r->t_admit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
+    out->n_cached = r->n_cached; out->reserved = 0;
 }
 
 RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,

@@ -190,6 +190,10 @@ void launch_embed(const int32_t* ids, const __nv_bfloat16* table, float* x, int 
 void launch_add_rmsnorm(float* x, PartIn part, const __nv_bfloat16* w, __nv_bfloat16* xn, int rows,
                         int hidden, float eps, cudaStream_t st, unsigned* zero = nullptr, int zero_n = 0,
                         float* rowss_out = nullptr, int n_part_out = 0);
+// The same in place over the rows of a prefill chunk (no partials), with a kernel chosen by the hidden size only: the row
+// count never changes a row's bits.
+void launch_add_rmsnorm_pf(float* x, const __nv_bfloat16* w, __nv_bfloat16* xn, int rows, int hidden, float eps,
+                           cudaStream_t st, float* rowss_out = nullptr, int n_part_out = 0);
 // act[row, j] = silu(gate[row, j]) * up[row, j]; gate = cols [0, inter), up = cols [inter, 2*inter)
 void launch_silu_mul(PartIn gu, __nv_bfloat16* act, int rows, int inter, cudaStream_t st);
 // qkv (partials) -> RoPE(q), RoPE(k); q -> q_out [rows, n_heads*128] bf16; k, v -> KV cache.
@@ -257,7 +261,8 @@ struct PrefillAttnArgs {
     __nv_bfloat16* out;       // [T, n_heads*128]
     const int32_t* seq_start; // [n_seqs+1] token offsets into T
     const int32_t* seq_slot;  // [n_seqs]
-    int n_seqs, max_len, n_heads, n_kv_heads, ctx_max;
+    const int32_t* seq_pos0 = nullptr;   // [n_seqs] position of each sequence's first query row (cached prefix); null: all 0
+    int n_seqs, max_len, n_heads, n_kv_heads, ctx_max;   // max_len: longest sequence (suffix) in rows
     float scale;
     int head_dim;             // true head dim: `out` head stride; q / caches padded to 128
     int has_maps = 0;         // tmQ/tmK/tmV valid (prefill_attn_make_maps): required
@@ -268,5 +273,18 @@ int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st);   // RR_ERR_
 int prefill_attn_make_maps(PrefillAttnArgs* a, long long q_rows, long long kv_rows);
 bool prefill_attn_tc_eligible(const PrefillAttnArgs& a);
 int launch_prefill_attn_tc(const PrefillAttnArgs& a, cudaStream_t st);
+
+// ---- prompt prefix caching (rr_kv_copy.cu): positions [0, n[i]) of slot src[i] -> slot dst[i], every layer and kv head,
+// K and V, one launch for the whole list (passed by value as a kernel parameter).
+constexpr int KV_COPY_MAX = 256;      // = the largest max_batch
+struct KvCopyList {
+    int32_t src[KV_COPY_MAX], dst[KV_COPY_MAX], n[KV_COPY_MAX];
+    int count;
+};
+// RR_ERR_ARG unless 1 <= count <= KV_COPY_MAX, every slot is in [0, n_slots), every n in [1, ctx_max], no destination
+// repeats and no destination is also a source.
+int kv_copy_check(const KvCopyList& c, int n_slots, int ctx_max);
+int launch_kv_copy(__nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                   const KvCopyList& c, cudaStream_t st);
 
 }  // namespace rr

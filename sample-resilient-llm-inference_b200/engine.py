@@ -29,6 +29,8 @@ class CompletionRecord:
     t_done: float
     # submit(top_logprobs=k): per generated token the max(1, k) most likely (token id, logprob) pairs, best first
     logprobs: Optional[List[List[Tuple[int, float]]]] = None
+    # prompt tokens whose KV came from the prefix cache (Engine(prefix_cache=True)); 0 otherwise
+    n_cached: int = 0
 
     @property
     def ttft(self) -> float:
@@ -51,7 +53,10 @@ class Engine:
     def __init__(self, weights: Weights, device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
                  max_prefill_tokens: int = 8192, use_cuda_graph: bool = True,
                  fail_prob: float = 0.0, fail_seed: int = 0, fuse_silu: bool = True, fuse_layer: bool = False,
-                 fuse_mlp: bool = True, defer_norm: bool = True):
+                 fuse_mlp: bool = True, defer_norm: bool = True, prefix_cache: bool = False):
+        """prefix_cache=True: a KV slot keeps the prompt its last prefill wrote, and a prompt that shares at least 64
+        leading tokens with one is prefilled from there on (tokens and logits bit-identical to a cold prefill).  Off by
+        default: a resident prefix is a timing side channel between the engine's users."""
         if not torch.cuda.is_available():
             raise RuntimeError("rr_b200.Engine needs a CUDA device (no CPU fallback)")
         self.spec: ModelSpec = weights.spec
@@ -59,6 +64,7 @@ class Engine:
         self.device = device
         self.max_batch = max_batch
         self.ctx_max = ctx_max
+        self.prefix_cache = bool(prefix_cache)
         s = self.spec
         desc = _lib.ModelDesc(s.vocab, s.hidden, s.inter, s.n_layers, s.n_heads, s.n_kv_heads,
                               s.head_dim, s.rope_theta, s.rms_eps)
@@ -91,7 +97,8 @@ class Engine:
                                weights.final_norm.data_ptr(), *self._arrs, 1 if self.fuse_silu else 0, 0)
         opts = _lib.EngineOpts(device, max_batch, ctx_max, max_prefill_tokens,
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
-                               (C.c_int32 * 4)(2 if fuse_layer else 1, 0, 0 if fuse_mlp else 1, 0 if defer_norm else 1))
+                               (C.c_int32 * 4)(2 if fuse_layer else 1, 0, 0 if fuse_mlp else 1, 0 if defer_norm else 1),
+                               1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
         self._h = C.c_void_p()
@@ -169,7 +176,8 @@ class Engine:
             _lib.check(rc, "rr_engine_wait")
         n = min(c.n_generated, max_tokens)
         return CompletionRecord(ticket, rc, c.n_prompt, buf[:c.n_generated].tolist(), c.t_submit_s,
-                                c.t_first_token_s, c.t_done_s, logprob_pairs(lp, ids, 0, n) if lp is not None else None)
+                                c.t_first_token_s, c.t_done_s, logprob_pairs(lp, ids, 0, n) if lp is not None else None,
+                                c.n_cached)
 
     def peek(self, ticket: int, have: int, timeout: float = 0.05, max_tokens: int = 4096):
         """Streaming: wait until more than `have` tokens exist (or done / timeout). -> (tokens so far, done, ttft_s), and
@@ -195,7 +203,8 @@ class Engine:
         if rc not in (0, 7):
             _lib.check(rc, "rr_engine_run_batch")
         recs = [CompletionRecord(c.ticket, c.status, c.n_prompt, toks[i, :c.n_generated].tolist(),
-                                 c.t_submit_s, c.t_first_token_s, c.t_done_s) for i, c in enumerate(comps)]
+                                 c.t_submit_s, c.t_first_token_s, c.t_done_s, n_cached=c.n_cached)
+                for i, c in enumerate(comps)]
         return recs, toks
 
     def now(self) -> float:

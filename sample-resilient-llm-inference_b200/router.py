@@ -76,6 +76,8 @@ class Usage:
     prompt_tokens: int
     completion_tokens: int
     total_tokens: int
+    # {"cached_tokens": n}: responses of deployments with litellm_params.prefix_cache only (OpenAI's usage shape)
+    prompt_tokens_details: Optional[dict] = None
 
 
 @dataclass
@@ -100,9 +102,11 @@ class ModelResponse:
                                   "message": {"role": c.message.role, "content": c.message.content}},
                                  **({} if c.logprobs is None else {"logprobs": c.logprobs}))
                             for c in self.choices],
-                "usage": {"prompt_tokens": self.usage.prompt_tokens,
-                          "completion_tokens": self.usage.completion_tokens,
-                          "total_tokens": self.usage.total_tokens}}
+                "usage": dict({"prompt_tokens": self.usage.prompt_tokens,
+                               "completion_tokens": self.usage.completion_tokens,
+                               "total_tokens": self.usage.total_tokens},
+                              **({} if self.usage.prompt_tokens_details is None
+                                 else {"prompt_tokens_details": self.usage.prompt_tokens_details}))}
 
 
 # ---------------------------------------------------------------- tokenizer (byte level, CUDA kernel K2 in the library)
@@ -222,6 +226,7 @@ class EngineBackend:
     def __init__(self, engine):
         self.engine = engine
         self.vocab = engine.spec.vocab
+        self.prefix_cache = bool(getattr(engine, "prefix_cache", False))
 
     def peek(self, handle, have, timeout=0.05):
         return self.engine.peek(handle, have, timeout=timeout)
@@ -230,8 +235,9 @@ class EngineBackend:
         return self.engine.submit(prompt_ids, max_new)
 
     def wait(self, handle, timeout):
+        """-> (status, tokens, ttft, latency, prompt tokens served from the prefix cache)"""
         rec = self.engine.wait(handle, timeout=timeout or 0.0)
-        return rec.status, rec.tokens, rec.ttft, rec.latency
+        return rec.status, rec.tokens, rec.ttft, rec.latency, rec.n_cached
 
 
 # ---------------------------------------------------------------- the router
@@ -336,13 +342,18 @@ class Router:
         return [((e.type, e.target, e.tokens, e.chain_start, e.now_ms), (d.status, d.deployment, d.served_group, d.chain_pos))
                 for e, d in zip(ev[: n.value], dec[: n.value])]
 
+    def _usage(self, dep: int, n_prompt: int, n_gen: int, n_cached: int = 0) -> Usage:
+        """prompt_tokens counts the whole prompt, cached or not (as litellm does; so does the tpm debit)."""
+        details = {"cached_tokens": int(n_cached)} if self.cfg.deployments[dep].prefix_cache else None
+        return Usage(n_prompt, n_gen, n_prompt + n_gen, details)
+
     def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None) -> ModelResponse:
         d = self.cfg.deployments[res.deployment]
         toks = [int(t) for t in toks[: res.n_generated]]
         return ModelResponse(
             id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
             choices=[Choice(0, Message("assistant", detokenize(toks) if detok else ""), logprobs=logprobs)],
-            usage=Usage(n_prompt, len(toks), n_prompt + len(toks)), created=int(time.time()),
+            usage=self._usage(res.deployment, n_prompt, len(toks), res.n_cached), created=int(time.time()),
             _token_ids=toks, _deployment=res.deployment, _model_group=self.cfg.groups[res.served_group],
             _fell_back=res.chain_pos > 0, _ttft_s=res.t_first_token_s - res.t_submit_s,
             _latency_s=time.perf_counter() - t_start)
@@ -577,7 +588,7 @@ class Router:
             remaining = None if timeout is None else max(0.001, timeout - (time.perf_counter() - t_start))
             try:
                 backend = self._backend_for(dep)
-                st, toks, ttft, lat = backend.wait(backend.submit(prompt_ids, max_new), remaining)
+                st, toks, ttft, lat, *cached = backend.wait(backend.submit(prompt_ids, max_new), remaining)
             except Exception as exc:     # the request was admitted: never leave its in-flight slot behind
                 self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
                 raise exc if isinstance(exc, APIError) else APIError(f"backend error on deployment {dep}: {exc}")
@@ -587,7 +598,7 @@ class Router:
                 return ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
                     choices=[Choice(0, Message("assistant", detokenize(toks)))],
-                    usage=Usage(n_prompt, len(toks), n_prompt + len(toks)), created=int(time.time()),
+                    usage=self._usage(dep, n_prompt, len(toks), cached[0] if cached else 0), created=int(time.time()),
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg],
                     _fell_back=pos > 0, _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
             # backend failed / timed out: report, then walk on down the fallback chain
@@ -634,7 +645,7 @@ class Router:
                         yield label, toks[sent:], False, ttft
                         sent = len(toks)
                     if done:
-                        st, toks, ttft, lat = backend.wait(h, timeout)
+                        st, toks, ttft, lat, *_ = backend.wait(h, timeout)
                         failed = st != 0
                         timed_out = st == 6
                         break
@@ -690,14 +701,15 @@ class Router:
                 continue
             b, hd = h
             status, dep, sg, pos = dec[i]
-            st, toks, ttft, lat = b.wait(hd, timeout)
+            st, toks, ttft, lat, *cached = b.wait(hd, timeout)
             if st == 0:
                 post.append((EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms()))
                 d = self.cfg.deployments[dep]
                 out[i] = ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
                     choices=[Choice(0, Message("assistant", ""))],
-                    usage=Usage(len(prompts[i]), len(toks), len(prompts[i]) + len(toks)), created=int(time.time()),
+                    usage=self._usage(dep, len(prompts[i]), len(toks), cached[0] if cached else 0),
+                    created=int(time.time()),
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
                     _ttft_s=ttft, _latency_s=time.perf_counter() - t0)
             else:
@@ -718,14 +730,15 @@ class Router:
             if status != 0:
                 raise APIError(f"backend failure and no fallback available for model={model}")
             b = self._backend_for(dep)
-            st, toks, ttft, lat = b.wait(b.submit(prompt_ids, max_new), timeout)
+            st, toks, ttft, lat, *cached = b.wait(b.submit(prompt_ids, max_new), timeout)
             if st == 0:
                 self.process([(EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms())])
                 d = self.cfg.deployments[dep]
                 return ModelResponse(
                     id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
                     choices=[Choice(0, Message("assistant", detokenize(toks)))],
-                    usage=Usage(len(prompt_ids), len(toks), len(prompt_ids) + len(toks)), created=int(time.time()),
+                    usage=self._usage(dep, len(prompt_ids), len(toks), cached[0] if cached else 0),
+                    created=int(time.time()),
                     _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
                     _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
             self.process([(EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms())])

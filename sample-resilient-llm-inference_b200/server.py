@@ -150,7 +150,7 @@ def build_backends(cfg: RouterConfig, stub: bool, spec_override: Optional[str] =
         from .engine import Engine
         spec = resolve_spec(spec_override or d.model)
         backends[d.gpu] = EngineBackend(Engine.synthetic(spec, seed=0, device=d.gpu, max_batch=max_batch,
-                                                         ctx_max=ctx_max))
+                                                         ctx_max=ctx_max, prefix_cache=d.prefix_cache))
     return backends
 
 
