@@ -51,7 +51,8 @@ int rr_set_pdl(int enabled);
  * (4 x uint64 each) to `out`. */
 int rr_debug_trace_start(int max_entries);
 int rr_debug_trace_stop(unsigned long long* out, int max_entries, int* n);
-/* on != 0: sample CTAs of the persistent decode layer kernel also record one mark per finished work item (kernel id 12 + phase). */
+/* on != 0: sample CTAs of the fused decode MLP kernel, of decode attention and of one plain decode projection also record
+ * per-phase marks (kernel ids 50 +, 80 +, 100 +) into fixed slots at the end of the buffer. */
 int rr_debug_trace_detail(int on);
 /* Host-side work schedule of the fused decode MLP kernel (gate/up + down GEMMs in one launch, DESIGN.md section 3), for
  * inspection and tests; no device is touched.  items_out receives grid * (*max_items) entries of 4 x int32
@@ -59,12 +60,6 @@ int rr_debug_trace_detail(int on);
  * returns RR_INVALID_ARGUMENT when `capacity` (in entries) is too small (*max_items is still set). */
 int rr_debug_mlp_schedule(int grid, int inter, int hidden, int slice_kb, int32_t* items_out, int capacity,
                           int* max_items);
-
-/* Host-side work schedule of the persistent decode layer kernel (O -> gate/up -> down -> next projection in one launch,
- * DESIGN.md section 3): same entry format with phase 0 = O (slice = split-K plane), 1 = gate/up, 2 = down (slice = K-slice),
- * 3 = next projection (QKV of the next layer / lm_head; slice = split-K plane).  has_main = 0: phase 3 only. */
-int rr_debug_layer_schedule(int grid, int hidden, int inter, int nq, int rows_a3, int s_o, int s3, int slice_kb,
-                            int has_main, int32_t* items_out, int capacity, int* max_items);
 
 /* ================================================================================================
  * 1. Router: admission + rpm/tpm bucket debit + backend pick + cooldown + fallback chain (K1).
@@ -315,8 +310,7 @@ typedef struct rr_engine_opts {
     int32_t use_cuda_graph;       /* capture the decode step */
     int32_t fail_seed;            /* fault injection: seed of the Bernoulli failure mask */
     float fail_prob;              /* fault injection: P(request fails) (BASELINE config #4) */
-    int32_t reserved[4];          /* A/B switches: [0] = 2 persistent decode layer kernel (rr_layer.cu; off by default, measured slower); [1] = 1 no RoPE fusion in the prefill
-                                     QKV epilogue; [2] = 1 no fused decode MLP kernel; [3] = 1 prefill RMSNorm as separate kernels instead of deferred into the GEMM epilogues */
+    int32_t reserved[4];          /* ignored (pass zeros); keeps prefix_cache at offset 44 */
     int32_t prefix_cache;         /* 1: prompt prefix caching.  A slot keeps the prompt KV its last prefill wrote; a new prompt
                                      sharing >= 64 leading tokens with one is prefilled from there on (the prefix is copied
                                      when that slot is busy).  Tokens and logits are bit-identical to a cold prefill.  Off

@@ -7,7 +7,6 @@
 //
 // Replaces (together with rr_gemm.cu / rr_attn_tc.cu / rr_attn_decode.cu) the remote bedrock:InvokeModel call
 // (reference iam/policy.json:8; src/demo_cris.py:233-238).
-#include <stdlib.h>
 #include "rr_ptx.cuh"
 #include "rr_launch.cuh"
 #include "rr_kernels.h"
@@ -97,7 +96,6 @@ add_rmsnorm_kernel(float* __restrict__ x, PartIn part, const __nv_bfloat16* __re
     griddep_wait();
     trace_dep(tr_slot);
     // optional: reset the dependency counters of the fused MLP kernel that follows (its previous user has completed)
-    // (grid-stride: the layer-kernel path resets every counter of the step here)
     for (int i = blockIdx.x * THREADS + threadIdx.x; i < zero_n; i += gridDim.x * THREADS) zero[i] = 0u;
     float4 v[MAXV];
     float ss = 0.f;
@@ -164,8 +162,7 @@ __device__ __forceinline__ void pin4(float4& v) { asm volatile("" : "+f"(v.x), "
 template <int MAXV>
 __global__ void __maxnreg__(88)
 add_rmsnorm_dec_kernel(float* __restrict__ x, PartIn part, const __nv_bfloat16* __restrict__ w,
-                       __nv_bfloat16* __restrict__ xn, int hidden, float eps, unsigned* __restrict__ zero, int zero_n,
-                       float* __restrict__ rowss_out, int n_part_out) {
+                       __nv_bfloat16* __restrict__ xn, int hidden, float eps, unsigned* __restrict__ zero, int zero_n) {
     constexpr int THREADS = 512, NP = 8;
     __shared__ float red[32];
     __shared__ float one_s;
@@ -220,9 +217,7 @@ add_rmsnorm_dec_kernel(float* __restrict__ x, PartIn part, const __nv_bfloat16* 
         }
     }
     ss = block_sum(ss, red);
-    if (rowss_out != nullptr && (int)threadIdx.x < n_part_out)
-        rowss_out[(size_t)row * n_part_out + threadIdx.x] = threadIdx.x == 0 ? ss : 0.f;
-    const float inv = rowss_out != nullptr ? 1.f : rsqrtf(ss / (float)hidden + eps);
+    const float inv = rsqrtf(ss / (float)hidden + eps);
     __nv_bfloat16* out = xn + (size_t)row * hidden;
 #pragma unroll
     for (int i = 0; i < MAXV; ++i) {
@@ -238,21 +233,19 @@ add_rmsnorm_dec_kernel(float* __restrict__ x, PartIn part, const __nv_bfloat16* 
 }
 
 void launch_add_rmsnorm(float* x, PartIn part, const __nv_bfloat16* w, __nv_bfloat16* xn, int rows,
-                        int hidden, float eps, cudaStream_t st, unsigned* zero, int zero_n, float* rowss_out, int n_part_out) {
+                        int hidden, float eps, cudaStream_t st, unsigned* zero, int zero_n) {
     if (rows <= 0 || hidden > 8192) return;
-    const bool no_dec = getenv("RR_NO_DEC_NORM") != nullptr;     // A/B switch (tools/decode_ab.py); launches are graph-captured
-    if (rows <= 256 && hidden <= 4096 && !no_dec && (part.ptr == nullptr || (!part.is_bf16 && part.n_splits <= 8)))
-        launch_pdl(add_rmsnorm_dec_kernel<2>, dim3(rows), dim3(512), 0, st, x, part, w, xn, hidden, eps, zero, zero_n,
-                   rowss_out, n_part_out);
+    if (rows <= 256 && hidden <= 4096 && (part.ptr == nullptr || (!part.is_bf16 && part.n_splits <= 8)))
+        launch_pdl(add_rmsnorm_dec_kernel<2>, dim3(rows), dim3(512), 0, st, x, part, w, xn, hidden, eps, zero, zero_n);
     else if (rows <= 256)
         launch_pdl(add_rmsnorm_kernel<1024, 2>, dim3(rows), dim3(1024), 0, st, x, part, w, xn, hidden, eps, zero, zero_n,
-                   rowss_out, n_part_out);
+                   (float*)nullptr, 0);
     else if (hidden <= 4096)      // fewer registers -> more rows in flight per SM (HBM-bound at thousands of rows)
         launch_pdl(add_rmsnorm_kernel<256, 4>, dim3(rows), dim3(256), 0, st, x, part, w, xn, hidden, eps, zero, zero_n,
-                   rowss_out, n_part_out);
+                   (float*)nullptr, 0);
     else
         launch_pdl(add_rmsnorm_kernel<256, 8>, dim3(rows), dim3(256), 0, st, x, part, w, xn, hidden, eps, zero, zero_n,
-                   rowss_out, n_part_out);
+                   (float*)nullptr, 0);
 }
 
 // Prefill chunks: the kernel, and so the order of the sum of squares, depends on the hidden size only, never on the row
@@ -282,7 +275,7 @@ silu_mul_kernel(PartIn gu, __nv_bfloat16* __restrict__ act, int inter) {
     if (c >= inter) return;
     const float4 g = part_load4(gu, row, c);
     const float4 u = part_load4(gu, row, inter + c);
-    auto f = [](float a, float b) { return __fdividef(a, 1.f + __expf(-a)) * b; };   // same formula as silu_mul (rr_gemm_dev.cuh)
+    auto f = [](float a, float b) { return __fdividef(a, 1.f + __expf(-a)) * b; };   // same formula as silu_mul (rr_gemm.cu)
     uint2 o;
     o.x = pack_bf16(f(g.x, u.x), f(g.y, u.y));
     o.y = pack_bf16(f(g.z, u.z), f(g.w, u.w));

@@ -135,16 +135,10 @@ struct rr_engine {
     GemmPlan pl_head, pl_head_pf;
     int s_qkv, s_o, s_gu, s_down;
     bool fuse_rope_pf = false;        // prefill: RoPE + KV append live in the QKV GEMM epilogue (head_dim 128)
-    bool defer_norm_pf = false;       // prefill: no norm kernels -- RESID epilogues emit bf16(x * gamma) + sum(x^2), the next
-                                      // GEMM's epilogue applies 1 / rms (RopeEpi)
+    // prefill defers RMSNorm: no norm kernels inside the layers -- RESID epilogues emit bf16(x * gamma) + sum(x^2), the next
+    // GEMM's epilogue applies 1 / rms (RopeEpi)
     float* p_rowss = nullptr;         // [Tmax][pf_parts]
     int pf_parts = 0;
-    bool use_layer = false;           // decode: one persistent dataflow launch per layer between attention kernels (rr_layer.cu)
-    std::vector<LayerPlan> layer;     // [0] = QKV projection of layer 0 only; [1 + l] = layer l (phase 3 = QKV of l + 1 / lm_head)
-    MlpItem* layer_items = nullptr;   // device copies of the three schedules (first | mid | last)
-    unsigned* layer_ctr = nullptr;    // [(L + 1) * layer_ctr_words] dependency counters, zeroed by the first kernel of every step
-    int layer_ctr_words = 0;
-    float *rowss_a = nullptr, *rowss_b = nullptr;   // [Bm][ceil(hidden / 128)] partial sum(x^2) (deferred RMSNorm)
     bool fuse_silu = false;           // wgu interleaved + one gate/up plane: SiLU*mul lives in the GEMM epilogue
     bool fuse_mlp = false;            // decode: gate/up and down GEMMs in one persistent launch (gemm_mlp_wgmma)
     std::vector<MlpPlan> mlp;         // per layer
@@ -235,11 +229,10 @@ static int pick_splits(int N, int K) {
     return s;
 }
 
-// One engine at a time per device.  The fused MLP kernel and the layer kernel (rr_layer.cu) are persistent grids whose
-// CTAs spin on work of sibling CTAs; two such grids interleaved on one GPU (two engines, two streams) could each hold
-// SMs the other's not-yet-resident CTAs need.  Every path below synchronises its stream before it releases this lock, so
-// engines that share a device alternate at prefill-chunk / decode-step granularity.  (The gateway creates one engine per
-// GPU, so this lock is uncontended there.)
+// One engine at a time per device.  The fused MLP kernel is a persistent grid whose CTAs spin on work of sibling CTAs;
+// two such grids interleaved on one GPU (two engines, two streams) could each hold SMs the other's not-yet-resident CTAs
+// need.  Every path below synchronises its stream before it releases this lock, so engines that share a device alternate
+// at prefill-chunk / decode-step granularity.  (The gateway creates one engine per GPU, so this lock is uncontended there.)
 static std::mutex& device_mutex(int dev) {
     static std::mutex mu[64];
     return mu[dev & 63];
@@ -265,24 +258,6 @@ static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch,
     const rr_model_desc& d = e->d;
     const int B = e->Bm, L = d.n_layers;
     uint64_t nl = 0;
-    if (e->use_layer) {
-        // 3 + 2 L + 1 launches: embed, norm (deferred form: xn = bf16(x * gamma), sum(x^2); also zeroes every dependency
-        // counter of the step), QKV_0, then per layer attention + one persistent layer kernel (phase 3 of the last = lm_head)
-        launch_embed(e->d_tok, (const __nv_bfloat16*)e->embed, e->x, B, d.hidden, e->d_slot, s); ++nl;
-        launch_add_rmsnorm(e->x, part_none(), (const __nv_bfloat16*)e->norm_attn[0], e->xn, B, d.hidden, d.rms_eps, s,
-                           e->layer_ctr, (L + 1) * e->layer_ctr_words, e->rowss_b, (d.hidden + 127) / 128); ++nl;
-        if (layer_launch(e->layer[0], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        for (int l = 0; l < L; ++l) {
-            launch_decode_attn(e->attn_args[l], s); nl += e->kv_splits > 1 ? 2 : 1;
-            if (layer_launch(e->layer[1 + l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        }
-        launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
-        if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s); nl += LP_LAUNCHES; }
-        if (n_launch) *n_launch = nl;
-        cudaError_t err = cudaGetLastError();
-        if (err != cudaSuccess) { rr::note_cuda_error(err); return RR_CUDA_ERROR; }
-        return RR_OK;
-    }
     launch_embed(e->d_tok, (const __nv_bfloat16*)e->embed, e->x, B, d.hidden, e->d_slot, s); ++nl;
     launch_add_rmsnorm(e->x, part_none(), (const __nv_bfloat16*)e->norm_attn[0], e->xn, B, d.hidden, d.rms_eps, s); ++nl;
     for (int l = 0; l < L; ++l) {
@@ -383,16 +358,11 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
         rc = gemm_plan_init(&P.o[l], e->pattn, T, e->nq, e->wo[l], d.hidden, e->nq, e->nq, e->px, d.hidden, 0, 1,
                             OUT_ROWMAJOR_RESID, PF_BN);                // residual add in the epilogue
         if (rc) return rc;
-        if (e->defer_norm_pf) {
-            auto consumer = [&](RopeEpi& r) {
-                r.rowss = e->p_rowss; r.n_part = e->pf_parts; r.inv_hidden = 1.0f / (float)d.hidden; r.eps = d.rms_eps;
-            };
-            auto producer = [&](RopeEpi& r, const void* gamma) {
-                r.gamma = (const __nv_bfloat16*)gamma; r.xhat = e->pxn; r.rowss_out = e->p_rowss; r.n_part_out = e->pf_parts;
-            };
-            consumer(P.qkv[l].rope);
-            producer(P.o[l].rope, e->norm_mlp[l]);
-        }
+        // deferred RMSNorm: the residual GEMMs (O, down) produce the next operand and its sum(x^2); QKV and gate/up apply 1 / rms
+        RopeEpi& cq = P.qkv[l].rope;
+        cq.rowss = e->p_rowss; cq.n_part = e->pf_parts; cq.inv_hidden = 1.0f / (float)d.hidden; cq.eps = d.rms_eps;
+        RopeEpi& po = P.o[l].rope;
+        po.gamma = (const __nv_bfloat16*)e->norm_mlp[l]; po.xhat = e->pxn; po.rowss_out = e->p_rowss; po.n_part_out = e->pf_parts;
         if (e->fuse_silu)
             rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pact,
                                 d.inter, 0, 1, OUT_ROWMAJOR_SILU, PF_BN);
@@ -403,13 +373,11 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
         rc = gemm_plan_init(&P.down[l], e->pact, T, d.inter, e->wdown[l], d.hidden, d.inter, d.inter, e->px,
                             d.hidden, 0, 1, OUT_ROWMAJOR_RESID, PF_BN);
         if (rc) return rc;
-        if (e->defer_norm_pf) {
-            RopeEpi& c = P.gu[l].rope;
-            c.rowss = e->p_rowss; c.n_part = e->pf_parts; c.inv_hidden = 1.0f / (float)d.hidden; c.eps = d.rms_eps;
-            RopeEpi& r = P.down[l].rope;
-            r.gamma = (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm);
-            r.xhat = e->pxn; r.rowss_out = e->p_rowss; r.n_part_out = e->pf_parts;
-        }
+        RopeEpi& cg = P.gu[l].rope;
+        cg.rowss = e->p_rowss; cg.n_part = e->pf_parts; cg.inv_hidden = 1.0f / (float)d.hidden; cg.eps = d.rms_eps;
+        RopeEpi& pd = P.down[l].rope;
+        pd.gamma = (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm);
+        pd.xhat = e->pxn; pd.rowss_out = e->p_rowss; pd.n_part_out = e->pf_parts;
     }
     auto ins = e->pf_plans.emplace(T, std::move(P));
     *out = &ins.first->second;
@@ -468,12 +436,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ++nl;
     }
     launch_embed(p_ids, (const __nv_bfloat16*)e->embed, e->px, T, d.hidden, nullptr, s); ++nl;
-    if (e->defer_norm_pf)       // layer 0's operand in the deferred form: bf16(x * gamma), sum(x^2) in partial 0
-        launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s, e->p_rowss,
-                              e->pf_parts);
-    else
-        launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s);
-    ++nl;
+    // layer 0's operand in the deferred form: bf16(x * gamma), sum(x^2) in partial 0
+    launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[0], e->pxn, T, d.hidden, d.rms_eps, s, e->p_rowss,
+                          e->pf_parts); ++nl;
     for (int l = 0; l < d.n_layers; ++l) {
         __nv_bfloat16* kc = e->kcache + (size_t)l * e->kv_layer_stride;
         __nv_bfloat16* vc = e->vcache + (size_t)l * e->kv_layer_stride;
@@ -508,15 +473,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
             break;
         }
         if (launch_rows(P->o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (!e->defer_norm_pf) {
-            launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_mlp[l], e->pxn, T, d.hidden, d.rms_eps, s); ++nl;
-        }
         if (launch_rows(P->gu[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->fuse_silu) { launch_silu_mul(part_bf16(e->pgu, 2 * d.inter), e->pact, T, d.inter, s); ++nl; }
         if (launch_rows(P->down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (!e->defer_norm_pf) {
-            launch_add_rmsnorm_pf(e->px, (const __nv_bfloat16*)e->norm_attn[l + 1], e->pxn, T, d.hidden, d.rms_eps, s); ++nl;
-        }
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
@@ -862,9 +821,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->part_gu, (size_t)e->s_gu * B * 2 * d.inter));
     // fused decode MLP: the down GEMM's K range in <= 8 slices, one output plane each (mlp_slices)
     {
-        const int kb1n = d.inter / 64;
         const int n_sl = mlp_slices(d.inter, &e->mlp_slice_kb);
-        e->fuse_mlp = e->fuse_silu && e->Bm <= e->bn_dec && opts->reserved[2] == 0 && d.inter % 64 == 0 && kb1n >= 1 && !getenv("RR_NO_MLP_FUSE");
+        e->fuse_mlp = e->fuse_silu && e->Bm <= e->bn_dec && n_sl > 0;
         e->mlp_slices = e->fuse_mlp ? n_sl : 0;
     }
     TRY(dalloc(e, &e->part_down, (size_t)(e->s_down > e->mlp_slices ? e->s_down : e->mlp_slices) * B * d.hidden));
@@ -940,75 +898,11 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
                        B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
     TRY(gemm_plan_init(&e->pl_head_pf, e->lm_head, d.vocab, d.hidden, e->xn_last, B, d.hidden, d.hidden, e->logits,
                        d.vocab, B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
-    e->fuse_rope_pf = d.head_dim == 128 && opts->reserved[1] == 0;
+    e->fuse_rope_pf = d.head_dim == 128;
+    // deferred prefill RMSNorm: hidden % 64 == 0 and hidden <= 8192 (checked above) give the 16-byte rows and the <= 64 partial
+    // sums per row that the residual epilogue writes
     e->pf_parts = (d.hidden + PF_BN - 1) / PF_BN;
-    // On by default (reserved[3] = 1 or RR_NO_DEFER_NORM=1 restores the two norm kernels per layer; tools/prefill_ab.py
-    // compares the two in one process).
-    e->defer_norm_pf = opts->reserved[3] == 0 && !getenv("RR_NO_DEFER_NORM") && d.hidden % 8 == 0 && e->pf_parts <= 64;
-    if (e->defer_norm_pf) TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
-    // ---- persistent layer kernel (rr_layer.cu): OFF by default -- reserved[0] = 2 or RR_LAYER_FUSE=1 turns it on
-    // (tools/decode_ab.py compares it with the per-kernel path below in one process).  Under a saturated weight stream every
-    // dependent memory round trip costs microseconds, and a dependency counter is 3 - 4 of them (store drain, release, poll,
-    // operand load), while a kernel boundary happens when the memory system has drained.
-    e->use_layer = e->fuse_mlp && (opts->reserved[0] == 2 || getenv("RR_LAYER_FUSE")) && !getenv("RR_NO_LAYER_FUSE");
-    if (e->use_layer) {
-        const int grid = num_sms();
-        const int tiles_h = (d.hidden + 127) / 128, kb_o = (e->nq + 63) / 64;
-        int s_o = grid / tiles_h;                         // one O item per CTA (their epilogues wait for each other)
-        if (s_o > 8) s_o = 8;
-        while (s_o > 1 && kb_o / s_o < 4) --s_o;
-        if (s_o > e->s_o) s_o = e->s_o > 0 ? e->s_o : 1;  // part_o holds e->s_o planes
-        if (s_o < 1 || tiles_h * s_o > grid) e->use_layer = false;
-        if (e->use_layer) {
-            LayerShape sh[3];
-            for (int k = 0; k < 3; ++k) {
-                sh[k].hidden = d.hidden; sh[k].inter = d.inter; sh[k].nq = e->nq; sh[k].s_o = s_o;
-                sh[k].slice_kb = e->mlp_slice_kb; sh[k].has_main = k > 0;
-                sh[k].rowsA3 = k < 2 ? e->nqkv : d.vocab; sh[k].s3 = k < 2 ? e->s_qkv : 1;
-            }
-            std::vector<MlpItem> sched[3];
-            int mx[3];
-            size_t total = 0;
-            for (int k = 0; k < 3; ++k) {
-                mx[k] = layer_schedule(grid, sh[k], &sched[k]);
-                if (mx[k] < 0) { e->use_layer = false; break; }
-                total += sched[k].size();
-            }
-            if (e->use_layer) {
-                TRY(dalloc(e, &e->layer_items, total));
-                size_t off[3], o = 0;
-                for (int k = 0; k < 3; ++k) {
-                    off[k] = o;
-                    TRYC(cudaMemcpy(e->layer_items + o, sched[k].data(), sched[k].size() * sizeof(MlpItem), cudaMemcpyHostToDevice));
-                    o += sched[k].size();
-                }
-                e->layer_ctr_words = (layer_counter_words(sh[1]) + 31) & ~31;
-                TRY(dalloc(e, &e->layer_ctr, (size_t)(L + 1) * e->layer_ctr_words));
-                TRY(dalloc(e, &e->rowss_a, (size_t)B * tiles_h));
-                TRY(dalloc(e, &e->rowss_b, (size_t)B * tiles_h));
-                e->layer.resize(L + 1);
-                for (int i = 0; i <= L; ++i) {
-                    const int l = i - 1;                  // -1: the QKV projection of layer 0 alone
-                    const int k = i == 0 ? 0 : (l + 1 < L ? 1 : 2);
-                    LayerBuffers bf;
-                    memset(&bf, 0, sizeof(bf));
-                    bf.x = e->x; bf.xhat = e->xn; bf.rowss_a = e->rowss_a; bf.rowss_b = e->rowss_b; bf.rows = B; bf.ld_rows = B;
-                    bf.eps = d.rms_eps;
-                    bf.l2_ahead = getenv("RR_LAYER_L2_AHEAD") ? atoi(getenv("RR_LAYER_L2_AHEAD")) : 0;
-                    bf.ring_depth = getenv("RR_LAYER_RING_DEPTH") ? atoi(getenv("RR_LAYER_RING_DEPTH")) : 0;
-                    if (l >= 0) {
-                        bf.wo = e->wo[l]; bf.wgu = e->wgu[l]; bf.wdown = e->wdown[l]; bf.attn_out = e->attn_out; bf.act = e->act;
-                        bf.part_o = e->part_o; bf.part_d = e->part_down; bf.gamma_a = (const __nv_bfloat16*)e->norm_mlp[l];
-                        bf.gamma_b = (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm);
-                    }
-                    if (k < 2) { bf.w3 = e->wqkv[l + 1]; bf.out3 = e->part_qkv; bf.ldo3 = e->nqkv; }
-                    else { bf.w3 = e->lm_head; bf.out3 = e->logits; bf.ldo3 = d.vocab; }
-                    TRY(layer_plan_init(&e->layer[i], sh[k], bf, e->bn_dec, e->layer_items + off[k], mx[k], grid,
-                                        e->layer_ctr + (size_t)i * e->layer_ctr_words));
-                }
-            }
-        }
-    }
+    TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
     if (e->fuse_mlp) {
         std::vector<MlpItem> sched;
         const int grid = num_sms();

@@ -52,8 +52,7 @@ def _p(a: np.ndarray):
 class Engine:
     def __init__(self, weights: Weights, device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
                  max_prefill_tokens: int = 8192, use_cuda_graph: bool = True,
-                 fail_prob: float = 0.0, fail_seed: int = 0, fuse_silu: bool = True, fuse_layer: bool = False,
-                 fuse_mlp: bool = True, defer_norm: bool = True, prefix_cache: bool = False):
+                 fail_prob: float = 0.0, fail_seed: int = 0, prefix_cache: bool = False):
         """prefix_cache=True: a KV slot keeps the prompt its last prefill wrote, and a prompt that shares at least 64
         leading tokens with one is prefilled from there on (tokens and logits bit-identical to a cold prefill).  Off by
         default: a resident prefix is a timing side channel between the engine's users."""
@@ -81,9 +80,9 @@ class Engine:
         gu_splits = max(1, min(8, n_sm // tiles))                 # mirrors pick_splits() in csrc/rr_engine.cu
         while gu_splits > 1 and kb // gu_splits < 8:
             gu_splits -= 1
-        self.fuse_silu = bool(fuse_silu and s.inter % 64 == 0 and gu_splits == 1 and max_batch > 16)
+        interleave = s.inter % 64 == 0 and gu_splits == 1 and max_batch > 16
         wgu = weights.wgu
-        if self.fuse_silu:
+        if interleave:
             self._wgu_il = []
             for t in weights.wgu:
                 g, u = t[: s.inter].view(-1, 64, s.hidden), t[s.inter:].view(-1, 64, s.hidden)
@@ -94,10 +93,10 @@ class Engine:
         for t in weights.tensors():
             assert t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()
         mw = _lib.ModelWeights(weights.embed.data_ptr(), weights.lm_head.data_ptr(),
-                               weights.final_norm.data_ptr(), *self._arrs, 1 if self.fuse_silu else 0, 0)
+                               weights.final_norm.data_ptr(), *self._arrs, 1 if interleave else 0, 0)
         opts = _lib.EngineOpts(device, max_batch, ctx_max, max_prefill_tokens,
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
-                               (C.c_int32 * 4)(2 if fuse_layer else 1, 0, 0 if fuse_mlp else 1, 0 if defer_norm else 1),
+                               (C.c_int32 * 4)(),
                                1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs

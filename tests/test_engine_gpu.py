@@ -119,49 +119,6 @@ def test_engine_matches_oracle(spec_name, max_batch):
         eng.close()
 
 
-@pytest.mark.parametrize("spec_name,max_batch", [("small", 64), ("llama-3-8b-2l", 64), ("phi-3-mini-2l", 64), ("small", 128),
-                                                 ("small96", 32)])
-def test_persistent_layer_kernel_option_matches_oracle(spec_name, max_batch):
-    """fuse_layer=True: the decode layer as one persistent dataflow launch (csrc/rr_layer.cu: O -> gate/up -> down ->
-    next QKV / lm_head, deferred RMSNorm, dependency counters).  Off by default (measured slower than the per-kernel path,
-    profiles/r02_layer_kernel_experiment.md) but kept correct: same tolerance as every other engine test, serving loop
-    under the CUDA graph equal to the stepwise path."""
-    from oracle import llama_ref
-    from rr_b200.models import SPECS, make_weights
-    from rr_b200.engine import Engine
-    spec = SPECS[spec_name]
-    w = make_weights(spec, seed=3, sigma=0.03 if spec.hidden < 2048 else 0.02, device="cuda", norm_jitter=0.1)
-    eng = Engine(w, max_batch=max_batch, ctx_max=640, max_prefill_tokens=2048, use_cuda_graph=True, fuse_layer=True)
-    try:
-        g = torch.Generator().manual_seed(5)
-        lens = [3, 64, 129, 300, 512]
-        prompts = [torch.randint(0, spec.vocab, (n,), generator=g).tolist() for n in lens]
-        slots = [max_batch - 1, 0, 5, 2, 3]
-        first, _ = eng.prefill(prompts, slots)
-        toks = [list(p) for p in prompts]
-        cur = [int(t) for t in first]
-        for j in range(3):
-            pos = [len(t) for t in toks]
-            for t, c in zip(toks, cur):
-                t.append(c)
-            nxt, lg = eng.decode_step(slots, cur, pos, want_logits=True)
-            for i in range(len(lens)):
-                _cmp(lg[i], llama_ref.forward_logits(w, toks[i])[-1], f"layer-kernel decode {spec_name} step {j} seq {i}")
-            cur = [int(t) for t in nxt]
-        # serving loop (CUDA graph replays of the layer kernels) == stepwise, and deterministic
-        recs = [eng.wait(eng.submit(p, 6), timeout=120) for p in prompts[:3]]
-        recs2 = [eng.wait(eng.submit(p, 6), timeout=120) for p in prompts[:3]]
-        assert [r.tokens for r in recs] == [r.tokens for r in recs2]
-        f1, _ = eng.prefill([prompts[1]], [2])
-        out, pos = [int(f1[0])], lens[1]
-        while len(out) < 6:
-            nx, _ = eng.decode_step([2], [out[-1]], [pos])
-            out.append(int(nx[0])); pos += 1
-        assert out == recs[1].tokens
-    finally:
-        eng.close()
-
-
 def test_serving_loop_equals_stepwise_and_is_deterministic():
     """submit/wait (continuous batching, CUDA graph) must produce exactly the tokens of the
     synchronous prefill + decode_step path (same kernels, same order of arithmetic)."""
@@ -251,28 +208,6 @@ def test_run_batch_and_fault_injection():
         assert len(ok1) > 0
     finally:
         eng.close()
-
-
-def test_separate_norm_kernels_prefill_option_matches_oracle():
-    """The default prefill defers RMSNorm into the GEMM epilogues (residual epilogues emit bf16(x * gamma) and sum(x^2),
-    the next GEMM's epilogue applies 1 / rms; RopeEpi in csrc/rr_kernels.h) -- every other test here runs that path.
-    This one covers the fallback with two norm kernels per layer (defer_norm=False).  Same tolerance."""
-    from oracle import llama_ref
-    from rr_b200.models import SPECS, make_weights
-    from rr_b200.engine import Engine
-    for name in ("small", "small96"):                     # fused-RoPE epilogue / bf16 epilogue + rope kernel
-        spec = SPECS[name]
-        w = make_weights(spec, seed=3, sigma=0.03, device="cuda", norm_jitter=0.1)
-        eng = Engine(w, max_batch=16, ctx_max=640, max_prefill_tokens=2048, use_cuda_graph=False, defer_norm=False)
-        try:
-            g = torch.Generator().manual_seed(5)
-            lens = [3, 64, 129, 300, 512]
-            prompts = [torch.randint(0, spec.vocab, (n,), generator=g).tolist() for n in lens]
-            first, logits = eng.prefill(prompts, [15, 0, 5, 2, 3], want_logits=True)
-            for i, p in enumerate(prompts):
-                _cmp(logits[i], llama_ref.forward_logits(w, p)[-1], f"separate-norm prefill {name} len={lens[i]}")
-        finally:
-            eng.close()
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs in one process")

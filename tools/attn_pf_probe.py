@@ -1,6 +1,6 @@
 """Standalone prefill-attention probe: correctness vs an fp32 torch reference and CUDA-event timing at the
-bench chunk shape (16 prompts x 512 tokens, 32 query heads, 8 kv heads).  RR_NO_ATTN_TC=1 selects the
-mma.sync kernel, default the tcgen05 kernel."""
+bench chunk shape (16 prompts x 512 tokens, 32 query heads, 8 kv heads) and a ragged batch, on the wgmma kernel
+(prefill_attn_tc_kernel)."""
 import math, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

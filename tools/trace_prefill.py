@@ -21,10 +21,8 @@ _lib.check(_lib.lib.rr_debug_trace_stop(buf, N, C.byref(n)))
 a = np.frombuffer(buf, dtype=np.uint64)[: 4 * n.value].reshape(-1, 4).astype(np.int64)
 a = a[np.argsort(a[:, 1])]
 print(f"{n.value} kernels; chunk span {(a[-1, 3] - a[0, 1]) / 1e6:.2f} ms")
-# per layer (after embed, norm0): qkv, rope, attn, o, norm, gu(+silu), down, norm
-DEFER = not os.environ.get("RR_NO_DEFER_NORM")      # deferred RMSNorm (default): no norm kernels inside the layers
-names = (["gemm_qkv(+rope,*rinv)", "attn", "gemm_o(+resid,xhat)", "gemm_gate_up(+silu,*rinv)", "gemm_down(+resid,xhat)"] if DEFER else
-         ["gemm_qkv(+rope)", "attn", "gemm_o", "norm_mlp", "gemm_gate_up(+silu)", "gemm_down", "norm_next"])
+# per layer (after embed, norm0): deferred RMSNorm, so no norm kernels inside the layers
+names = ["gemm_qkv(+rope,*rinv)", "attn", "gemm_o(+resid,xhat)", "gemm_gate_up(+silu,*rinv)", "gemm_down(+resid,xhat)"]
 PER = len(names)
 agg = {}
 for i in range(len(a) - 1):

@@ -22,16 +22,14 @@ _lib.check(_lib.lib.rr_debug_trace_stop(buf, N, C.byref(n)))
 a = np.frombuffer(buf, dtype=np.uint64)[: 4 * n.value].reshape(-1, 4).astype(np.int64)
 a = a[np.argsort(a[:, 1])]
 L = spec.n_layers
-FUSED_MLP = not os.environ.get("RR_NO_MLP_FUSE")                # gate/up + down in one launch (gemm_mlp_tcgen05)
-PER = 6 if FUSED_MLP else 7                                     # qkv, attn(+rope), o, norm, [gate_up(+silu), down | mlp], norm
+layer_names = ["gemm_qkv", "attn(+rope)", "gemm_o", "norm_mlp", "mlp(gate_up+down)", "norm_next"]   # 64 rows: fused MLP
+PER = len(layer_names)
 n_step = 2 + PER * L + 2
 dec = a[-n_step:]                                               # last decode step
 t0 = dec[0, 1]
 print(f"{n.value} kernels traced; last decode step ({n_step} launches): {(dec[-1, 3] - t0) / 1e3:.1f} us first start -> last end")
 # critical-path segment of kernel k = (dependency of kernel k+1 resolved) - (dependency of kernel k resolved):
 # griddepcontrol.wait returns when the WHOLE preceding grid has completed and flushed.
-layer_names = (["gemm_qkv", "attn(+rope)", "gemm_o", "norm_mlp", "mlp(gate_up+down)", "norm_next"] if FUSED_MLP else
-               ["gemm_qkv", "attn(+rope)", "gemm_o", "norm_mlp", "gemm_gate_up(+silu)", "gemm_down", "norm_next"])
 agg = {}
 for i in range(len(dec) - 1):
     kid, s_, d, e = dec[i]
