@@ -270,6 +270,44 @@ int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int 
 int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache, void* v_cache,
                           void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads, int n_kv_heads,
                           int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits, void* stream);
+/* Prefill, deferred RMSNorm.  The engine does not normalise the operands of a prefill chunk's projections: the operand row
+ * is xhat = bf16(x * gamma) and comes with n_part = ceil(hidden / 128) partial sums of squares rowss[row][p]; the consuming
+ * GEMM scales its fp32 accumulators by rsqrt(sum_p rowss[row][p] / hidden + eps) before its epilogue.  The entry points
+ * below run the prefill kernels exactly as the engine does (plans made for plan_rows rows and launched for the first T,
+ * deferred-norm fields filled by the engine's helpers).  Each returns RR_INVALID_ARGUMENT before touching the device, with
+ * its out-parameters unchanged, for the arguments listed.
+ *
+ * Layer 0's norm of a prefill chunk: xn[r] = bf16(x[r] * w) (not normalised), rowss_out[r][0] = sum(x[r]^2) in fp32,
+ * rowss_out[r][1 .. n_part_out) = 0, for rows r < rows; x is not written.  Rejects a null pointer, rows < 1, hidden not a
+ * multiple of 64 in 64..8192, and n_part_out != ceil(hidden / 128). */
+int rr_op_add_rmsnorm_pf(float* x, const void* w, void* xn, int rows, int hidden, float eps, float* rowss_out,
+                         int n_part_out, void* stream);
+/* The QKV projection of a prefill chunk with RoPE and the KV append (theta: the engine's RoPE table):
+ *   xhat     bf16 [plan_rows][hidden], rowss fp32 [plan_rows][ceil(hidden / 128)]; rows >= T are not read into any output
+ *   wqkv     bf16 [(n_heads + 2 n_kv_heads) head_dim][hidden]: q heads, then k heads, then v heads
+ *   q_out    bf16 [T][n_heads * 128]: rotated q, columns [0, head_dim) of each head
+ *   k_cache, v_cache  bf16 [..][n_kv_heads][ctx_max][128]: token t writes its rotated k and its v to columns [0, head_dim)
+ *            of position pos[t] of slot slot[t] (slot[t] >= 0)
+ * *fused = 1 when the GEMM epilogue did RoPE and the append (head_dim 128), 0 when rope_kv_kernel did them from a bf16 qkv
+ * matrix.  Rejects a null pointer, T outside 1..plan_rows, hidden not a multiple of 64 in 64..8192, n_heads / n_kv_heads
+ * not 1, 2, 4 or 8, head_dim not a multiple of 16 in 64..128, and ctx_max not a positive multiple of 64. */
+int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                      int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
+                      const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
+                      void* stream);
+/* The O, gate/up and down projections of a prefill chunk: rr_gemm_bf16's row-major modes on A [plan_rows][K] (pitch ldA),
+ * launched for rows < T.
+ *   mode RR_OUT_ROWMAJOR_BF16 / RR_OUT_ROWMAJOR_SILU with n_part > 0: deferred-norm consumer (rowss [plan_rows][n_part],
+ *        n_part = ceil(hidden / 128)); n_part = 0: A is used as it is
+ *   mode RR_OUT_ROWMAJOR_RESID: out is the fp32 residual [..][ldo], out[t][n] += acc.  With xhat: deferred-norm producer,
+ *        xhat[t][n] = bf16(out[t][n] * gamma[n]) (pitch ldo) and rowss_out[t][p] = sum of out[t][n]^2 over n in
+ *        [128 p, 128 p + 128), n_part_out = ceil(rowsW / 128)
+ * Rejects a null A, W or out, T outside 1..plan_rows, rowsW < 1, another mode, a consumer with a null rowss, mode RESID or
+ * the wrong n_part, a producer outside mode RESID, with a null gamma or rowss_out, or the wrong n_part_out, and whatever
+ * rr_gemm_bf16 rejects. */
+int rr_op_prefill_gemm(const void* A, int plan_rows, int T, int ldA, const void* W, int rowsW, int K, void* out, int ldo,
+                       int mode, const float* rowss, int n_part, int hidden, float eps, const void* gamma, void* xhat,
+                       float* rowss_out, int n_part_out, void* stream);
 
 /* ================================================================================================
  * 4. Engine: one model replica on one GPU (prefill + continuous-batching greedy decode).

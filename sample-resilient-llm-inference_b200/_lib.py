@@ -163,6 +163,11 @@ PROTOTYPES = {
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp]),
+    "rr_op_add_rmsnorm_pf": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp]),
+    "rr_op_prefill_qkv": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                    C.c_float, vp, vp, vp, vp, vp, c_i32p, vp]),
+    "rr_op_prefill_gemm": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp,
+                                     C.c_int, C.c_int, C.c_float, vp, vp, vp, C.c_int, vp]),
     "rr_engine_create": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(ModelWeights),
                                    C.POINTER(EngineOpts), C.POINTER(vp)]),
     "rr_engine_destroy": (None, [vp]),

@@ -276,6 +276,97 @@ RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split
     return check_last();
 }
 
+// Layer 0's RMSNorm of a prefill chunk in the deferred form, the only form run_prefill launches.
+RR_API int rr_op_add_rmsnorm_pf(float* x, const void* w, void* xn, int rows, int hidden, float eps, float* rowss_out,
+                                int n_part_out, void* stream) {
+    if (!x || !w || !xn || !rowss_out) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || hidden < 64 || hidden % 64 || hidden > 8192 || n_part_out != pf_norm_parts(hidden)) return RR_INVALID_ARGUMENT;
+    launch_add_rmsnorm_pf(x, (const __nv_bfloat16*)w, (__nv_bfloat16*)xn, rows, hidden, eps, (cudaStream_t)stream, rowss_out,
+                          n_part_out);
+    return check_last();
+}
+
+// The prefill QKV projection as run_prefill runs it: the plan is made for plan_rows rows and launched for T, the deferred
+// norm scale comes from rowss, and RoPE + KV append run in the epilogue (head_dim 128) or in rope_kv_kernel from a bf16
+// qkv matrix.  The RoPE table and that matrix live in stream-ordered scratch memory.
+RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                             int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
+                             const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
+                             void* stream) {
+    if (!xhat || !rowss || !wqkv || !slot || !pos || !q_out || !k_cache || !v_cache || !fused) return RR_INVALID_ARGUMENT;
+    if (T < 1 || T > plan_rows || hidden < 64 || hidden % 64 || hidden > 8192) return RR_INVALID_ARGUMENT;
+    if (n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
+    const int G = n_heads / n_kv_heads;
+    if (!(G == 1 || G == 2 || G == 4 || G == 8)) return RR_INVALID_ARGUMENT;
+    if (head_dim < 64 || head_dim > 128 || head_dim % 16 || ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
+    const int nqkv = (n_heads + 2 * n_kv_heads) * head_dim;
+    const bool fuse = pf_rope_fused(head_dim);
+    GemmPlan p;
+    int rc = gemm_plan_init(&p, xhat, plan_rows, hidden, wqkv, nqkv, hidden, hidden, nullptr, nqkv, 0, 1,
+                            fuse ? OUT_ROWMAJOR_ROPE : OUT_ROWMAJOR_BF16, MAX_BN);
+    if (rc != RR_OK) return rc;
+    pf_norm_consumer(&p.rope, rowss, hidden, eps);
+    p.rowsA = T;
+    cudaStream_t st = (cudaStream_t)stream;
+    float2* table = nullptr;
+    __nv_bfloat16* qkv = nullptr;
+    cudaError_t e = cudaMallocAsync(&table, (size_t)ctx_max * 64 * sizeof(float2), st);
+    if (e == cudaSuccess && !fuse) e = cudaMallocAsync(&qkv, (size_t)plan_rows * nqkv * sizeof(__nv_bfloat16), st);
+    rc = RR_CUDA_ERROR;
+    if (e == cudaSuccess) {
+        launch_rope_table(table, ctx_max, theta, head_dim, st);
+        if (fuse) {
+            RopeEpi& r = p.rope;
+            r.q_out = (__nv_bfloat16*)q_out; r.k_cache = (__nv_bfloat16*)k_cache; r.v_cache = (__nv_bfloat16*)v_cache;
+            r.slot = slot; r.pos = pos; r.table = table; r.n_heads = n_heads; r.n_kv_heads = n_kv_heads; r.ctx_max = ctx_max;
+        } else {
+            p.out = qkv;
+        }
+        rc = gemm_launch(p, st);
+        if (rc == RR_OK && !fuse) {
+            RopeArgs ra;
+            ra.qkv = mk_part(qkv, 1, 1, 0, nqkv);
+            ra.q_out = (__nv_bfloat16*)q_out; ra.k_cache = (__nv_bfloat16*)k_cache; ra.v_cache = (__nv_bfloat16*)v_cache;
+            ra.slot = slot; ra.pos = pos; ra.rows = T; ra.n_heads = n_heads; ra.n_kv_heads = n_kv_heads; ra.ctx_max = ctx_max;
+            ra.theta = theta; ra.table = table; ra.head_dim = head_dim;
+            launch_rope_kv(ra, st);
+        }
+        if (rc != RR_OK) note_cuda_error(cudaPeekAtLastError());
+    } else {
+        note_cuda_error(e);
+    }
+    if (table) cudaFreeAsync(table, st);
+    if (qkv) cudaFreeAsync(qkv, st);
+    if (rc != RR_OK) return rc;
+    *fused = fuse ? 1 : 0;
+    return check_last();
+}
+
+// The O, gate/up and down projections of a prefill chunk as run_prefill runs them: planned for plan_rows rows, launched
+// for T, with the deferred-norm fields of the epilogue filled by the engine's helpers.
+RR_API int rr_op_prefill_gemm(const void* A, int plan_rows, int T, int ldA, const void* W, int rowsW, int K, void* out,
+                              int ldo, int mode, const float* rowss, int n_part, int hidden, float eps, const void* gamma,
+                              void* xhat, float* rowss_out, int n_part_out, void* stream) {
+    if (!A || !W || !out) return RR_INVALID_ARGUMENT;
+    if (T < 1 || T > plan_rows || rowsW < 1) return RR_INVALID_ARGUMENT;
+    if (mode != OUT_ROWMAJOR_BF16 && mode != OUT_ROWMAJOR_SILU && mode != OUT_ROWMAJOR_RESID) return RR_INVALID_ARGUMENT;
+    if (n_part < 0 || (n_part > 0 && (!rowss || mode == OUT_ROWMAJOR_RESID || hidden < 1 || n_part != pf_norm_parts(hidden))))
+        return RR_INVALID_ARGUMENT;
+    if (xhat && (mode != OUT_ROWMAJOR_RESID || !gamma || !rowss_out || n_part_out != pf_norm_parts(rowsW)))
+        return RR_INVALID_ARGUMENT;
+    GemmPlan p;
+    const int rc = gemm_plan_init(&p, A, plan_rows, ldA, W, rowsW, K, K, out, ldo, 0, 1, mode, MAX_BN);
+    if (rc != RR_OK) return rc;
+    if (n_part > 0) pf_norm_consumer(&p.rope, rowss, hidden, eps);
+    if (xhat) pf_norm_producer(&p.rope, (const __nv_bfloat16*)gamma, (__nv_bfloat16*)xhat, rowss_out, rowsW);
+    p.rowsA = T;
+    if (gemm_launch(p, (cudaStream_t)stream) != RR_OK) {
+        note_cuda_error(cudaPeekAtLastError());
+        return RR_CUDA_ERROR;
+    }
+    return check_last();
+}
+
 // The fused decode MLP as the engine runs it (rr_engine_create): tile width, K slices, grid and schedule come from the same
 // helpers and environment switches; the schedule and the dependency counters live in stream-ordered scratch memory.
 RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,

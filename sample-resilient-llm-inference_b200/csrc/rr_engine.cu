@@ -215,8 +215,7 @@ static int dalloc(rr_engine* e, T** p, size_t n, bool zero = true) {
     return RR_OK;
 }
 
-// Column block of the prefill deferred-norm partial sums (pf_parts = hidden / PF_BN): the residual GEMM epilogue writes one
-// sum(x^2) partial per 128 columns, two per 256-wide tile.
+// Tile width argument of the prefill plans (row-major modes only validate it; their tiles are 128 x 256).
 constexpr int PF_BN = MAX_BN;
 
 static int pick_splits(int N, int K) {
@@ -359,10 +358,8 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
                             OUT_ROWMAJOR_RESID, PF_BN);                // residual add in the epilogue
         if (rc) return rc;
         // deferred RMSNorm: the residual GEMMs (O, down) produce the next operand and its sum(x^2); QKV and gate/up apply 1 / rms
-        RopeEpi& cq = P.qkv[l].rope;
-        cq.rowss = e->p_rowss; cq.n_part = e->pf_parts; cq.inv_hidden = 1.0f / (float)d.hidden; cq.eps = d.rms_eps;
-        RopeEpi& po = P.o[l].rope;
-        po.gamma = (const __nv_bfloat16*)e->norm_mlp[l]; po.xhat = e->pxn; po.rowss_out = e->p_rowss; po.n_part_out = e->pf_parts;
+        pf_norm_consumer(&P.qkv[l].rope, e->p_rowss, d.hidden, d.rms_eps);
+        pf_norm_producer(&P.o[l].rope, (const __nv_bfloat16*)e->norm_mlp[l], e->pxn, e->p_rowss, d.hidden);
         if (e->fuse_silu)
             rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pact,
                                 d.inter, 0, 1, OUT_ROWMAJOR_SILU, PF_BN);
@@ -373,11 +370,9 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
         rc = gemm_plan_init(&P.down[l], e->pact, T, d.inter, e->wdown[l], d.hidden, d.inter, d.inter, e->px,
                             d.hidden, 0, 1, OUT_ROWMAJOR_RESID, PF_BN);
         if (rc) return rc;
-        RopeEpi& cg = P.gu[l].rope;
-        cg.rowss = e->p_rowss; cg.n_part = e->pf_parts; cg.inv_hidden = 1.0f / (float)d.hidden; cg.eps = d.rms_eps;
-        RopeEpi& pd = P.down[l].rope;
-        pd.gamma = (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm);
-        pd.xhat = e->pxn; pd.rowss_out = e->p_rowss; pd.n_part_out = e->pf_parts;
+        pf_norm_consumer(&P.gu[l].rope, e->p_rowss, d.hidden, d.rms_eps);
+        pf_norm_producer(&P.down[l].rope, (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm), e->pxn,
+                         e->p_rowss, d.hidden);
     }
     auto ins = e->pf_plans.emplace(T, std::move(P));
     *out = &ins.first->second;
@@ -898,10 +893,10 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
                        B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
     TRY(gemm_plan_init(&e->pl_head_pf, e->lm_head, d.vocab, d.hidden, e->xn_last, B, d.hidden, d.hidden, e->logits,
                        d.vocab, B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
-    e->fuse_rope_pf = d.head_dim == 128;
+    e->fuse_rope_pf = pf_rope_fused(d.head_dim);
     // deferred prefill RMSNorm: hidden % 64 == 0 and hidden <= 8192 (checked above) give the 16-byte rows and the <= 64 partial
     // sums per row that the residual epilogue writes
-    e->pf_parts = (d.hidden + PF_BN - 1) / PF_BN;
+    e->pf_parts = pf_norm_parts(d.hidden);
     TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
     if (e->fuse_mlp) {
         std::vector<MlpItem> sched;

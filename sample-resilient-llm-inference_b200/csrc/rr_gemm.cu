@@ -479,6 +479,7 @@ struct PfCfg {
     static constexpr int kProducerRegs = 40, kConsumerRegs = 232;          // 128 x 40 + 256 x 232 <= 64 K registers
 };
 static_assert(2 * PfCfg::kSmemBytes > 227 * 1024 && PfCfg::kSmemBytes <= 227 * 1024, "one prefill GEMM CTA per SM");
+static_assert(2 * PF_NORM_COLS == PfCfg::kTileB, "the residual epilogue writes two sum(x^2) partials per tile");
 
 // Deferred RMSNorm, consumer side: the operand row was bf16(x * gamma); 1 / rms(x) from its partial sums of squares.
 __device__ __forceinline__ float pf_rinv(const RopeEpi& rope, int row, int rowsA) {

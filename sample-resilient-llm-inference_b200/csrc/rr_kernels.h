@@ -57,6 +57,22 @@ struct GemmPlan {
     int tma_epi;              // 1: the epilogue stages the tile in shared memory and issues ONE TMA store per item
 };
 
+// ---- prefill decisions shared by the engine (get_pf_plans, run_prefill) and the kernel-level entry points (rr_api.cu)
+// RoPE and the KV append run in the QKV GEMM's epilogue (OUT_ROWMAJOR_ROPE) only at head_dim 128, where a head is half of a
+// 256-wide tile; other head dims take OUT_ROWMAJOR_BF16 into a qkv matrix, then rope_kv_kernel.
+inline bool pf_rope_fused(int head_dim) { return head_dim == 128; }
+// Deferred RMSNorm: the OUT_ROWMAJOR_RESID epilogue writes one partial sum(x^2) per 128 columns of the residual.
+constexpr int PF_NORM_COLS = 128;
+inline int pf_norm_parts(int hidden) { return (hidden + PF_NORM_COLS - 1) / PF_NORM_COLS; }
+// Consumer side (QKV, gate/up): scale the accumulators of row r by rsqrt(sum(rowss[r][0..n_part)) / hidden + eps).
+inline void pf_norm_consumer(RopeEpi* r, const float* rowss, int hidden, float eps) {
+    r->rowss = rowss; r->n_part = pf_norm_parts(hidden); r->inv_hidden = 1.0f / (float)hidden; r->eps = eps;
+}
+// Producer side (O, down): also write xhat = bf16(x * gamma) and rowss_out[r][0..pf_norm_parts(hidden)).
+inline void pf_norm_producer(RopeEpi* r, const __nv_bfloat16* gamma, __nv_bfloat16* xhat, float* rowss_out, int hidden) {
+    r->gamma = gamma; r->xhat = xhat; r->rowss_out = rowss_out; r->n_part_out = pf_norm_parts(hidden);
+}
+
 int num_sms();
 
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)

@@ -80,7 +80,35 @@ def test_decode_attn_entry_point_validates_before_touching_the_device():
     assert rc == 4 and ks.value == -1
 
 
-@pytest.mark.parametrize("grid,inter,hidden,slice_kb", [(148, 14336, 4096, 28), (148, 8192, 3072, 16), (132, 2816, 1024, 15),
+def test_prefill_norm_entry_point_validates_before_touching_the_device():
+    """rr_op_add_rmsnorm_pf rejects null pointers with RR_INVALID_ARGUMENT before it touches the device."""
+    from rr_b200 import _lib
+    assert _lib.lib.rr_op_add_rmsnorm_pf(None, None, None, 64, 4096, 1e-5, None, 32, None) == 4
+
+
+def test_prefill_qkv_entry_point_validates_before_touching_the_device():
+    """rr_op_prefill_qkv rejects null pointers with RR_INVALID_ARGUMENT before it touches the device and leaves *fused
+    alone."""
+    from rr_b200 import _lib
+    fused = C.c_int32(-1)
+    rc = _lib.lib.rr_op_prefill_qkv(None, None, 128, 64, 4096, None, 32, 8, 128, 4096, 5e5, 1e-5, None, None, None, None,
+                                    None, C.byref(fused), None)
+    assert rc == 4 and fused.value == -1
+
+
+def test_prefill_gemm_entry_point_validates_before_touching_the_device():
+    """rr_op_prefill_gemm rejects null pointers with RR_INVALID_ARGUMENT before it touches the device, for the consumer
+    (gate/up) and the producer (down) forms."""
+    from rr_b200 import _lib
+    rc = _lib.lib.rr_op_prefill_gemm(None, 128, 64, 4096, None, 28672, 4096, None, 14336, 3, None, 32, 4096, 1e-5, None,
+                                     None, None, 0, None)
+    assert rc == 4
+    rc = _lib.lib.rr_op_prefill_gemm(None, 128, 64, 14336, None, 4096, 14336, None, 4096, 5, None, 0, 0, 0.0, None, None,
+                                     None, 32, None)
+    assert rc == 4
+
+
+@pytest.mark.parametrize("grid,inter,hidden,slice_kb",[(148, 14336, 4096, 28), (148, 8192, 3072, 16), (132, 2816, 1024, 15),
                                                         (148, 1024, 512, 16), (7, 14336, 4096, 28)])
 def test_fused_mlp_schedule_is_a_partition_and_deadlock_free(grid, inter, hidden, slice_kb):
     """Host logic of the fused decode MLP kernel (csrc/rr_gemm.cu, mlp_schedule): every gate/up tile and every
