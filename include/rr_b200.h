@@ -221,6 +221,18 @@ int rr_op_argmax(const float* logits, int ld, int rows, int vocab, int32_t* out_
  * reduction runs in a fixed order. */
 int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top,
                    float* lp_out, int32_t* id_out, void* stream);
+/* Seeded temperature / top-p draw from fp32 logits rows x (row r at logits + r * ld), as the engine samples a token.  All
+ * per-row arrays are device memory [rows].  A row with temperature[r] = T > 0 gets out_tok[r] =
+ *   argmax over {i : x_i >= tau} of x_i / T + G_i, ties to the lowest id, where
+ *   tau = the largest logit value such that {j : x_j >= tau} holds at least top_p[r] of the mass of softmax(x / T)
+ *         (top_p >= 1: every token; tokens tied at tau are all inside),
+ *   G_i = -log(-log u_i), u_i = (2 (r_i >> 9) + 1) / 2^24, r_i = word 0 of Philox4x32-10 with key seed[r] (low word first)
+ *         and counter (i, position[r], 0, 0).
+ * Rows with temperature[r] <= 0 are not touched.  The draw is a pure function of (row, T, top_p, seed, position).
+ * RR_INVALID_ARGUMENT before touching the device unless no pointer is null, 1 <= rows <= 65535, 1 <= vocab <= ld,
+ * vocab <= 524288 and ld % 4 == 0.  Deterministic: every sum is exact (fixed point) or runs in a fixed order. */
+int rr_op_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
+                 const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* stream);
 int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                       const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                       int n_kv_heads, int ctx_max /* % 64 == 0 */, int n_slots, float scale,
@@ -408,6 +420,16 @@ int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_
 int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
                             int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
                             float* lp_out, int32_t* id_out);
+/* Seeded sampling (OpenAI `temperature` / `top_p` / `seed`): every token of the request is drawn by rr_op_sample with
+ * these parameters at its own position (n_prompt for the first generated token, n_prompt + j for the j-th after it), so
+ * the tokens depend only on the prompt, the weights and (temperature, top_p, seed): not on the batch, the slot, the prefix
+ * cache or the replica.  temperature = 0 is greedy, exactly as rr_engine_submit_logprobs.  top_logprobs as in
+ * rr_engine_submit_logprobs; for a request with temperature > 0 and top_logprobs >= 0 the pair buffers of
+ * rr_engine_wait_logprobs / rr_engine_peek_logprobs are [max_tokens_out][max(1, top_logprobs) + 1], the last column
+ * being (the generated token's logprob, its id).  RR_INVALID_ARGUMENT unless 0 <= temperature <= 2 and
+ * 0 <= top_p <= 1. */
+int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int top_logprobs,
+                             float temperature, float top_p, uint64_t seed, uint64_t* ticket);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -497,6 +519,12 @@ int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, r
 int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
                              int max_tokens_out, int32_t* n_generated, int32_t* done, rr_gateway_result* out,
                              float* lp_out, int32_t* id_out);
+/* Seeded sampling (rr_engine_submit_sampled): the parameters travel with the request, a fallback re-admission included,
+ * so a re-admitted request draws the same tokens on a replica with the same weights.  Results through
+ * rr_gateway_wait_logprobs / rr_gateway_peek_logprobs, pair buffers as rr_engine_submit_sampled describes.  The admission
+ * trace is the same as rr_gateway_submit's. */
+int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                              int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

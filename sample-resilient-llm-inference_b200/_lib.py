@@ -153,6 +153,7 @@ PROTOTYPES = {
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, vp]),
     "rr_op_argmax": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]),
     "rr_op_logprobs": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp]),
+    "rr_op_sample": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "rr_op_decode_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -183,6 +184,8 @@ PROTOTYPES = {
                                           c_i32p]),
     "rr_engine_peek_logprobs": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
                                           C.POINTER(C.c_double), c_f32p, c_i32p]),
+    "rr_engine_submit_sampled": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
+                                           C.POINTER(C.c_uint64)]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
                                       C.POINTER(Completion), c_i32p]),
     "rr_engine_now": (C.c_double, [vp]),
@@ -202,6 +205,8 @@ PROTOTYPES = {
                                            c_i32p]),
     "rr_gateway_peek_logprobs": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
                                            C.POINTER(GatewayResult), c_f32p, c_i32p]),
+    "rr_gateway_submit_sampled": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                            C.c_uint64, C.POINTER(C.c_uint64)]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),
     "rr_gateway_quiesce": (C.c_int, [vp, C.c_double]),
     "rr_gateway_get_stats": (C.c_int, [vp, C.POINTER(GatewayStats)]),

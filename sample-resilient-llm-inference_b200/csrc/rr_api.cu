@@ -209,6 +209,21 @@ RR_API int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, cons
     return check_last();
 }
 
+// Seeded temperature / top-p draw as the engine runs it after the argmax; the workspace is stream-ordered scratch memory.
+RR_API int rr_op_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
+                        const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* stream) {
+    if (!logits || !temperature || !top_p || !seed || !position || !out_tok) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > 65535 || vocab < 1 || vocab > ld || ld % 4 || vocab > LP_MAX_CHUNKS * LP_CHUNK)
+        return RR_INVALID_ARGUMENT;
+    cudaStream_t st = (cudaStream_t)stream;
+    void* ws = nullptr;
+    cudaError_t e = cudaMallocAsync(&ws, sample_ws_bytes(rows, vocab), st);
+    if (e != cudaSuccess) { note_cuda_error(e); return RR_CUDA_ERROR; }
+    launch_sample(logits, ld, rows, vocab, temperature, top_p, seed, position, out_tok, ws, st);
+    cudaFreeAsync(ws, st);
+    return check_last();
+}
+
 RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_cache, void* out,
                              const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                              int n_kv_heads, int ctx_max, int n_slots, float scale, int kv_splits, void* stream) {

@@ -559,7 +559,8 @@ logprobs_chunk_kernel(const float* __restrict__ logits, int ld, int vocab, const
 
 __global__ void __launch_bounds__(LP_THREADS)
 logprobs_merge_kernel(const int32_t* __restrict__ top_n, int max_top, int n_chunks, const LpPart* __restrict__ ws,
-                      float* __restrict__ lp_out, int32_t* __restrict__ id_out) {
+                      float* __restrict__ lp_out, int32_t* __restrict__ id_out, const float* __restrict__ logits, int ld,
+                      const int32_t* __restrict__ tok, float* __restrict__ tok_lp) {
     __shared__ float s_v[LP_MAX_CHUNKS * LP_MAX_TOP];
     __shared__ int s_i[LP_MAX_CHUNKS * LP_MAX_TOP];
     __shared__ float s_lse;
@@ -584,6 +585,8 @@ logprobs_merge_kernel(const int32_t* __restrict__ top_n, int max_top, int n_chun
         float s = 0.f;
         for (int c = 0; c < n_chunks; ++c) s += p[c].s * expf(p[c].m - m);
         s_lse = m + logf(s);
+        // a sampled token may lie outside the top k: its own pair, from the same value and lse as the ranked entries
+        if (tok) tok_lp[row] = logits[(size_t)row * ld + tok[row]] - s_lse;
     }
     __syncthreads();
     const float lse = s_lse;
@@ -607,13 +610,247 @@ size_t logprobs_ws_bytes(int rows, int vocab) {
 }
 
 void launch_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top, void* ws,
-                     float* lp_out, int32_t* id_out, cudaStream_t st) {
+                     float* lp_out, int32_t* id_out, cudaStream_t st, const int32_t* tok, float* tok_lp) {
     if (rows <= 0) return;
     const int nc = (vocab + LP_CHUNK - 1) / LP_CHUNK;
     launch_pdl(logprobs_chunk_kernel, dim3(nc, rows), dim3(LP_THREADS), 0, st, logits, ld, vocab, top_n, max_top,
                (LpPart*)ws);
     launch_pdl(logprobs_merge_kernel, dim3(rows), dim3(LP_THREADS), 0, st, top_n, max_top, nc, (const LpPart*)ws, lp_out,
-               id_out);
+               id_out, logits, ld, tok, tok_lp);
+}
+
+// ---- seeded temperature / top-p sampling ------------------------------------------------------------
+// Contract (include/rr_b200.h, rr_op_sample): for a row with T > 0, tau = the largest logit value whose set {x >= tau}
+// holds at least top_p of the mass of softmax(x / T); the token is argmax over {x >= tau} of x / T + G_i (lowest id on
+// ties), G_i = -log(-log u_i), u_i from Philox4x32-10 with key = seed and counter = (i, position, 0, 0).
+//
+// Three launches.  (1) One CTA per row finds tau by a mass-weighted radix select on the order-preserving key of x: the row
+// max m, then one pass per key digit (11, 11, 10 bits) building the histogram of w = exp((x - m) / T) over the keys that
+// share the digits found so far; the crossing bin's digit is appended.  Weights are summed as 2^-40 fixed-point integers,
+// so the shared-memory atomics are order-independent and the result is bit-reproducible; an element lighter than 2^-40 of
+// the row max counts as 0.  top_p >= 1 skips the search (tau = -inf).  (2) One CTA per LP_CHUNK columns draws the chunk's
+// Gumbel-max candidate over {x >= tau}.  (3) One warp per row merges the chunks' candidates in the argmax order, which is
+// a total order, so the result does not depend on the merge order either.
+constexpr int SP_THREADS = 1024;
+constexpr int SP_BINS = 2048;
+struct SpPart { float v; int32_t id; };
+
+__device__ __forceinline__ uint32_t sample_key(float x) {
+    uint32_t b = __float_as_uint(x);
+    if (b == 0x80000000u) b = 0;                             // -0 and +0 are one value
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float sample_key_value(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// First 32-bit word of Philox4x32-10 (Salmon et al., SC'11) for counter (c0, c1, 0, 0) and the 64-bit key `seed`.
+__device__ __forceinline__ uint32_t philox_first(uint32_t c0, uint32_t c1, uint64_t seed) {
+    uint32_t c2 = 0, c3 = 0, k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    return c0;
+}
+
+// u = (2 (r >> 9) + 1) / 2^24: 2^23 odd multiples of 2^-24, exact in fp32 and strictly inside (0, 1)
+__device__ __forceinline__ float sample_gumbel(uint32_t r) {
+    const float u = (float)(((r >> 9) << 1) | 1u) * 5.9604644775390625e-8f;
+    return -logf(-logf(u));
+}
+
+// f(v) for every value of a row, each thread in increasing column order; U 16-byte loads in flight per thread (the row is
+// read once per pass, and a single load per iteration would leave each pass latency-bound)
+template <class F>
+__device__ __forceinline__ void sample_row_pass(const float* __restrict__ x, int vocab, F&& f) {
+    constexpr int U = 4;
+    const int v4 = vocab & ~3, stride = SP_THREADS * 4;
+    for (int c0 = threadIdx.x * 4; c0 < v4; c0 += stride * U) {
+        float4 v[U];
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+            const int c = c0 + k * stride;
+            v[k] = c < v4 ? *reinterpret_cast<const float4*>(x + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+#pragma unroll
+        for (int k = 0; k < U; ++k) {
+            if (c0 + k * stride >= v4) break;
+            f(v[k].x); f(v[k].y); f(v[k].z); f(v[k].w);
+        }
+    }
+    for (int j = v4 + threadIdx.x; j < vocab; j += SP_THREADS) f(x[j]);
+}
+
+__device__ __forceinline__ unsigned long long sample_weight(float x, float m, float T) {
+    return (unsigned long long)(expf((x - m) / T) * 1099511627776.0f);   // 2^40
+}
+
+__global__ void __launch_bounds__(SP_THREADS)
+sample_threshold_kernel(const float* __restrict__ logits, int ld, int vocab, const float* __restrict__ temperature,
+                        const float* __restrict__ top_p, float* __restrict__ tau_out) {
+    __shared__ unsigned long long s_h[SP_BINS];
+    __shared__ unsigned long long s_scan[32];
+    __shared__ float s_red[32];
+    __shared__ unsigned long long s_need, s_above;
+    __shared__ uint32_t s_prefix;
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_SAMPLE);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.x, tid = threadIdx.x;
+    const float T = temperature[row], p = top_p[row];
+    if (!(T > 0.f)) return;
+    if (p >= 1.f) {
+        if (tid == 0) tau_out[row] = -INFINITY;
+        return;
+    }
+    const float* x = logits + (size_t)row * ld;
+    float mx = -INFINITY;
+    sample_row_pass(x, vocab, [&](float v) { mx = fmaxf(mx, v); });
+    const float m = block_max(mx, s_red);
+    if (tid == 0) { s_prefix = 0; s_above = 0; }
+    const int lane = tid & 31, warp = tid >> 5;
+    for (int d = 0; d < 3; ++d) {
+        const int shift = d == 0 ? 21 : (d == 1 ? 10 : 0);
+        const int nbins = d == 2 ? 1024 : 2048;
+        for (int b = tid; b < SP_BINS; b += SP_THREADS) s_h[b] = 0;
+        __syncthreads();
+        const uint32_t prefix = s_prefix;
+        const int hi = shift + (d == 2 ? 10 : 11);          // key bits [hi, 32) are already fixed
+        // consecutive elements of a thread often share a bin (a flat row sits in a few top-digit bins): add runs, not elements
+        int run_bin = -1;
+        unsigned long long run = 0;
+        sample_row_pass(x, vocab, [&](float v) {
+            const uint32_t k = sample_key(v);
+            if (d > 0 && (k >> hi) != (prefix >> hi)) return;
+            const int b = (int)((k >> shift) & (uint32_t)(nbins - 1));
+            if (b != run_bin) {
+                if (run) atomicAdd(&s_h[run_bin], run);
+                run_bin = b; run = 0;
+            }
+            run += sample_weight(v, m, T);
+        });
+        if (run) atomicAdd(&s_h[run_bin], run);
+        __syncthreads();
+        // bins in descending key order: thread t holds bins nbins-1-2t and nbins-2-2t; inclusive scan over threads
+        const int b0 = nbins - 1 - 2 * tid, b1 = b0 - 1;
+        const unsigned long long h0 = b0 >= 0 ? s_h[b0] : 0, h1 = b1 >= 0 ? s_h[b1] : 0;
+        unsigned long long a = h0 + h1, incl = a;
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long t = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += t;
+        }
+        if (lane == 31) s_scan[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            unsigned long long w = s_scan[lane];
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned long long t = __shfl_up_sync(0xffffffffu, w, o);
+                if (lane >= o) w += t;
+            }
+            s_scan[lane] = w;                                  // inclusive over warps
+        }
+        __syncthreads();
+        incl += warp > 0 ? s_scan[warp - 1] : 0ull;
+        if (d == 0 && tid == SP_THREADS - 1) {               // total mass Z: need = max(1, ceil(top_p Z))
+            const double need = ceil((double)p * (double)incl);
+            s_need = need < 1.0 ? 1ull : (unsigned long long)need;
+        }
+        __syncthreads();
+        const unsigned long long need = s_need, above = s_above;
+        const unsigned long long e0 = above + incl - a;        // mass of every key above bin b0
+        // every thread has read s_above before the crossing thread overwrites it: a late reader of the new value would
+        // shift its e0 and could find a second crossing
+        __syncthreads();
+        // the crossing bin is the first, in descending order, whose cumulative mass reaches `need`; exactly one thread has
+        // it, because the mass above this prefix is < need and the mass up to the end of it is >= need
+        if (e0 < need && e0 + a >= need) {
+            const bool first = e0 + h0 >= need;
+            s_prefix = prefix | ((uint32_t)(first ? b0 : b1) << shift);
+            s_above = first ? e0 : e0 + h0;
+        }
+        __syncthreads();
+    }
+    if (tid == 0) tau_out[row] = sample_key_value(s_prefix);
+    trace_end(tr_slot);
+}
+
+__global__ void __launch_bounds__(LP_THREADS)
+sample_chunk_kernel(const float* __restrict__ logits, int ld, int vocab, const float* __restrict__ temperature,
+                    const uint64_t* __restrict__ seed, const int32_t* __restrict__ position, const float* __restrict__ tau,
+                    SpPart* __restrict__ ws) {
+    __shared__ float s_v[32];
+    __shared__ int s_i[32];
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_SAMPLE);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.y, c = blockIdx.x;
+    const float T = temperature[row];
+    if (!(T > 0.f)) return;
+    const float t = tau[row];
+    const uint64_t key = seed[row];
+    const uint32_t pos = (uint32_t)position[row];
+    const int c0 = c * LP_CHUNK;
+    const int n = min(LP_CHUNK, vocab - c0);
+    const float* x = logits + (size_t)row * ld + c0;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int j = threadIdx.x; j < n; j += LP_THREADS) {
+        const float v = x[j];
+        if (!(v >= t)) continue;
+        const int id = c0 + j;
+        const float s = v / T + sample_gumbel(philox_first((uint32_t)id, pos, key));
+        if (lp_before(s, id, bv, bi)) { bv = s; bi = id; }
+    }
+    block_best(bv, bi, s_v, s_i);
+    if (threadIdx.x == 0) ws[(size_t)row * gridDim.x + c] = SpPart{bv, bi};
+    trace_end(tr_slot);
+}
+
+__global__ void __launch_bounds__(32)
+sample_merge_kernel(const float* __restrict__ temperature, int n_chunks, const SpPart* __restrict__ ws,
+                    int32_t* __restrict__ out_tok) {
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_SAMPLE);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.x;
+    if (!(temperature[row] > 0.f)) return;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int c = threadIdx.x; c < n_chunks; c += 32) {
+        const SpPart q = ws[(size_t)row * n_chunks + c];
+        if (lp_before(q.v, q.id, bv, bi)) { bv = q.v; bi = q.id; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (lp_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+    }
+    if (threadIdx.x == 0) out_tok[row] = bi;
+    trace_end(tr_slot);
+}
+
+size_t sample_ws_bytes(int rows, int vocab) {
+    const size_t tau = ((size_t)rows * sizeof(float) + 15) & ~(size_t)15;
+    return tau + (size_t)rows * ((vocab + LP_CHUNK - 1) / LP_CHUNK) * sizeof(SpPart);
+}
+
+void launch_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
+                   const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* ws, cudaStream_t st) {
+    if (rows <= 0) return;
+    const int nc = (vocab + LP_CHUNK - 1) / LP_CHUNK;
+    float* tau = (float*)ws;
+    SpPart* part = (SpPart*)((char*)ws + (((size_t)rows * sizeof(float) + 15) & ~(size_t)15));
+    launch_pdl(sample_threshold_kernel, dim3(rows), dim3(SP_THREADS), 0, st, logits, ld, vocab, temperature, top_p, tau);
+    launch_pdl(sample_chunk_kernel, dim3(nc, rows), dim3(LP_THREADS), 0, st, logits, ld, vocab, temperature, seed, position,
+               (const float*)tau, part);
+    launch_pdl(sample_merge_kernel, dim3(rows), dim3(32), 0, st, temperature, nc, (const SpPart*)part, out_tok);
 }
 
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }

@@ -91,11 +91,19 @@ struct Request {
     std::vector<float> lp;     // [out.size()][max(1, top_lp)]
     std::vector<int32_t> lp_id;
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
+    float temp = 0.f, top_p = 1.f;   // rr_engine_submit_sampled: temp > 0 draws every token with rr_op_sample
+    uint64_t seed = 0;
+    bool sampled() const { return temp > 0.f; }
+    // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
+    int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
 };
 
 // Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
 // prefixes (a BOS and a role tag) stay misses.
 constexpr int PREFIX_MIN = 64;
+
+// Sampling parameter blocks, per row at stride n: seed (8 bytes) | temperature | top_p, and in prefill also | position.
+constexpr int SAMP_BYTES = 16, SAMP_PF_BYTES = 20;
 
 }  // namespace rr
 
@@ -145,14 +153,19 @@ struct rr_engine {
     MlpItem* mlp_items = nullptr;     // device copy of the schedule (shared by all layers)
     unsigned* mlp_ready = nullptr;    // [n_slices] dependency counters, reset by the norm kernel before each launch
     int mlp_slices = 0, mlp_slice_kb = 0;
-    cudaGraphExec_t graph = nullptr;
+    // decode step graphs by step_mode(): [0] plain, [1] + launch_logprobs, [2] + launch_sample, [3] both.  [0] is captured
+    // after the warm-up step, the others on first use: a step without logprobs or sampled rows replays the plain graph.
+    cudaGraphExec_t graph[4] = {nullptr, nullptr, nullptr, nullptr};
     bool warmed = false;
-    // logprobs: a second graph (the step + launch_logprobs on `logits`), replayed only on steps with a logprobs row
-    cudaGraphExec_t graph_lp = nullptr;
     int32_t *d_topn = nullptr, *d_topn_pf = nullptr;   // per decode row / per prefill sequence: top_lp, -1 = off
     void* lp_ws = nullptr;
     float* d_lp = nullptr;                             // [Bm][LP_MAX_TOP]
     int32_t* d_lp_id = nullptr;
+    // sampling: per decode row seed[Bm] | temperature[Bm] | top_p[Bm] (temperature 0 = greedy row); the prefill block holds
+    // the same per sequence plus position[n], packed at stride n_seqs
+    char *d_samp = nullptr, *d_samp_pf = nullptr;
+    void* sample_ws = nullptr;
+    float* d_tok_lp = nullptr;                         // [Bm] the sampled token's logprob (sampled logprobs rows)
 
     // prefill working set
     int Tmax;
@@ -170,6 +183,8 @@ struct rr_engine {
     float* h_lp = nullptr;        // [Bm][LP_MAX_TOP] logprobs read back on steps that computed them
     int32_t* h_lp_id = nullptr;
     int32_t* h_topn = nullptr;    // [Bm] staging of d_topn / d_topn_pf
+    char* h_samp = nullptr;       // [Bm * SAMP_PF_BYTES] staging of d_samp / d_samp_pf
+    float* h_tok_lp = nullptr;    // [Bm]
 
     // serving state
     std::mutex mu;                       // queues + request table
@@ -180,8 +195,11 @@ struct rr_engine {
     std::vector<Request*> row_req;       // [Bm]
     std::vector<int32_t> h_slot_mirror;  // host mirror of d_slot
     bool slots_dirty = false;
-    std::vector<int32_t> h_topn_mirror;  // host mirror of d_topn (uploaded before a step that replays graph_lp)
+    std::vector<int32_t> h_topn_mirror;  // host mirror of d_topn (uploaded before a step that computes logprobs)
     bool topn_dirty = false;
+    std::vector<uint64_t> h_seed_mirror; // host mirrors of d_samp (uploaded before a step that samples)
+    std::vector<float> h_temp_mirror, h_topp_mirror;
+    bool samp_dirty = false;
     // prefix caching (o.prefix_cache), under mu: retained[b] = the prompt tokens whose KV the last successful prefill into
     // slot b wrote (computed or copied; never a position decode wrote, since decode rounds differently), kept after the
     // request ends; retained_used[b] = LRU stamp.  index_epoch counts the low-level calls that cleared every list.
@@ -194,7 +212,7 @@ struct rr_engine {
     std::chrono::steady_clock::time_point t0;
 
     rr_engine_stats st;                  // written under gpu_mu (launch / timing counters) or mu (queued, active_rows)
-    uint64_t step_launches = 0, step_launches_lp = 0;
+    uint64_t step_launches[4] = {0, 0, 0, 0};   // launches of one decode step, by step_mode()
     // completion hook (the native gateway, rr_gateway.cu): called on the worker / submitting thread, outside `mu`
     rr::EngineDoneHook hook = nullptr;
     void* hook_ctx = nullptr;
@@ -248,12 +266,26 @@ static PartIn part_bf16(const __nv_bfloat16* p, int ld) {
 static PartIn part_none() { PartIn r; r.ptr = nullptr; r.is_bf16 = 0; r.n_splits = 1; r.split_stride = 0; r.ld = 0; return r; }
 
 // ---------------------------------------------------------------- decode step (enqueue only)
-static void enqueue_logprobs(rr_engine* e, const int32_t* top_n, int rows, cudaStream_t s) {
-    launch_logprobs(e->logits, e->d.vocab, rows, e->d.vocab, top_n, LP_MAX_TOP, e->lp_ws, e->d_lp, e->d_lp_id, s);
+// tok (sampled rows): also the logprob of the row's final token into d_tok_lp
+static void enqueue_logprobs(rr_engine* e, const int32_t* top_n, int rows, cudaStream_t s, const int32_t* tok = nullptr) {
+    launch_logprobs(e->logits, e->d.vocab, rows, e->d.vocab, top_n, LP_MAX_TOP, e->lp_ws, e->d_lp, e->d_lp_id, s, tok,
+                    tok ? e->d_tok_lp : nullptr);
 }
 
+// The sampler over `rows` rows of `logits` with a parameter block at stride n (seed | temperature | top_p).
+static void enqueue_sample(rr_engine* e, const char* samp, int n, int rows, const int32_t* position, int32_t* tok,
+                           cudaStream_t s) {
+    launch_sample(e->logits, e->d.vocab, rows, e->d.vocab, (const float*)(samp + (size_t)8 * n),
+                  (const float*)(samp + (size_t)12 * n), (const uint64_t*)samp, position, tok, e->sample_ws, s);
+}
+
+static int step_mode(bool logprobs, bool sample) { return (logprobs ? 1 : 0) | (sample ? 2 : 0); }
+
 // logprobs: launch_logprobs after the argmax for the rows with d_topn[row] >= 0 (the logits are left as they were)
-static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, bool logprobs = false) {
+// sample: rows with temperature > 0 replace the argmax token by rr_op_sample's draw at position d_pos (argmax advanced it
+// to the generated token's position), before logprobs, which then also gives the drawn token's own logprob
+static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, bool logprobs = false,
+                               bool sample = false) {
     const rr_model_desc& d = e->d;
     const int B = e->Bm, L = d.n_layers;
     uint64_t nl = 0;
@@ -285,18 +317,19 @@ static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch,
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
     launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
-    if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s); nl += LP_LAUNCHES; }
+    if (sample) { enqueue_sample(e, e->d_samp, B, B, e->d_pos, e->d_tok, s); nl += SAMPLE_LAUNCHES; }
+    if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s, sample ? e->d_tok : nullptr); nl += LP_LAUNCHES; }
     if (n_launch) *n_launch = nl;
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) { rr::note_cuda_error(err); return RR_CUDA_ERROR; }
     return RR_OK;
 }
 
-static int capture_decode_step(rr_engine* e, bool logprobs, cudaGraphExec_t* out, uint64_t* n_launch) {
+static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uint64_t* n_launch) {
     cudaStream_t s = e->stream;
     cudaGraph_t g = nullptr;
     CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_decode_step(e, s, n_launch, logprobs);
+    int rc = enqueue_decode_step(e, s, n_launch, mode & 1, mode & 2);
     cudaError_t ce = cudaStreamEndCapture(s, &g);
     if (rc != RR_OK || ce != cudaSuccess) { rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
     CK(cudaGraphInstantiate(out, g, 0));
@@ -304,15 +337,16 @@ static int capture_decode_step(rr_engine* e, bool logprobs, cudaGraphExec_t* out
     return RR_OK;
 }
 
-// logprobs: also run launch_logprobs for the rows with d_topn >= 0 (graph_lp, captured on first use); a step without
-// logprobs rows replays the plain graph.
-static int run_decode_step(rr_engine* e, bool logprobs = false) {
+// logprobs: also run launch_logprobs for the rows with d_topn >= 0; sample: also draw the rows with temperature > 0.  Each
+// combination has its own graph, captured on first use; a step without logprobs or sampled rows replays the plain graph.
+static int run_decode_step(rr_engine* e, bool logprobs = false, bool sample = false) {
     cudaStream_t s = e->stream;
+    const int mode = step_mode(logprobs, sample);
     if (!e->warmed || !e->o.use_cuda_graph) {
         uint64_t nl = 0;
-        int rc = enqueue_decode_step(e, s, &nl, logprobs);
+        int rc = enqueue_decode_step(e, s, &nl, logprobs, sample);
         if (rc != RR_OK) return rc;
-        (logprobs ? e->step_launches_lp : e->step_launches) = nl;
+        e->step_launches[mode] = nl;
         e->st.kernel_launches += nl;
         // NOTE: the warm-up step is a real step (it advances positions); graph capture follows.
         if (!e->warmed) {
@@ -320,18 +354,18 @@ static int run_decode_step(rr_engine* e, bool logprobs = false) {
             if (e->o.use_cuda_graph) {
                 CK(cudaStreamSynchronize(s));
                 // capture for subsequent steps
-                rc = capture_decode_step(e, false, &e->graph, &e->step_launches);
+                rc = capture_decode_step(e, 0, &e->graph[0], &e->step_launches[0]);
                 if (rc != RR_OK) return rc;
             }
         }
         return RR_OK;
     }
-    if (logprobs && !e->graph_lp) {
-        const int rc = capture_decode_step(e, true, &e->graph_lp, &e->step_launches_lp);
+    if (!e->graph[mode]) {
+        const int rc = capture_decode_step(e, mode, &e->graph[mode], &e->step_launches[mode]);
         if (rc != RR_OK) return rc;
     }
-    CK(cudaGraphLaunch(logprobs ? e->graph_lp : e->graph, s));
-    e->st.kernel_launches += logprobs ? e->step_launches_lp : e->step_launches;
+    CK(cudaGraphLaunch(e->graph[mode], s));
+    e->st.kernel_launches += e->step_launches[mode];
     return RR_OK;
 }
 
@@ -384,9 +418,13 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 // first token's logprobs in e->h_lp / e->h_lp_id row i.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
+// Sampling: temp_host / topp_host / seed_host[n_seqs] (optional): sequences with temp_host[i] > 0 draw their first token
+// with rr_op_sample at position pos0[i] + their length (the prompt length); with logprobs its own logprob lands in h_tok_lp.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr,
-                       const int32_t* pos0 = nullptr, const KvCopyList* copies = nullptr) {
+                       const int32_t* pos0 = nullptr, const KvCopyList* copies = nullptr,
+                       const float* temp_host = nullptr, const float* topp_host = nullptr,
+                       const uint64_t* seed_host = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
@@ -474,6 +512,22 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
+    bool samp = false;
+    for (int i = 0; temp_host && i < n_seqs; ++i) samp = samp || temp_host[i] > 0.f;
+    if (samp) {
+        char* h = e->h_samp;
+        const size_t n = (size_t)n_seqs;
+        for (int i = 0; i < n_seqs; ++i) {
+            ((uint64_t*)h)[i] = seed_host[i];
+            ((float*)(h + 8 * n))[i] = temp_host[i];
+            ((float*)(h + 12 * n))[i] = topp_host[i];
+            ((int32_t*)(h + 16 * n))[i] = (pos0 ? pos0[i] : 0) + seq_start[i + 1] - seq_start[i];
+        }
+        CK(cudaMemcpyAsync(e->d_samp_pf, h, SAMP_PF_BYTES * n, cudaMemcpyHostToDevice, s));
+        e->st.h2d_bytes += SAMP_PF_BYTES * n;
+        enqueue_sample(e, e->d_samp_pf, n_seqs, n_seqs, (const int32_t*)(e->d_samp_pf + 16 * n), e->p_first, s);
+        nl += SAMPLE_LAUNCHES;
+    }
     launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
                (const int32_t*)e->p_first, (const int32_t*)p_pos, (const int32_t*)p_last, n_seqs, e->d_tok, e->d_pos,
                e->d_slot); ++nl;
@@ -483,11 +537,15 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         memcpy(e->h_topn, topn_host, sizeof(int32_t) * n_seqs);
         CK(cudaMemcpyAsync(e->d_topn_pf, e->h_topn, sizeof(int32_t) * n_seqs, cudaMemcpyHostToDevice, s));
         e->st.h2d_bytes += sizeof(int32_t) * n_seqs;
-        enqueue_logprobs(e, e->d_topn_pf, n_seqs, s); nl += LP_LAUNCHES;
+        enqueue_logprobs(e, e->d_topn_pf, n_seqs, s, samp ? e->p_first : nullptr); nl += LP_LAUNCHES;
         const size_t n = (size_t)n_seqs * LP_MAX_TOP;
         CK(cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
         e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
+        if (samp) {
+            CK(cudaMemcpyAsync(e->h_tok_lp, e->d_tok_lp, sizeof(float) * n_seqs, cudaMemcpyDeviceToHost, s));
+            e->st.d2h_bytes += sizeof(float) * n_seqs;
+        }
     }
     CK(cudaMemcpyAsync(e->h_tok, e->p_first, sizeof(int32_t) * n_seqs, cudaMemcpyDeviceToHost, s));
     e->st.d2h_bytes += sizeof(int32_t) * n_seqs;
@@ -513,19 +571,27 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
 // ---------------------------------------------------------------- worker (continuous batching)
 struct DoneNote { uint64_t tag, ticket; int status, n_gen; };
 
-// Caller holds e->mu.  Appends row `row` of h_lp / h_lp_id to the request's pairs.
+// Caller holds e->mu.  Appends row `row` of h_lp / h_lp_id to the request's pairs, and for a sampled request the pair of
+// the token it just generated (h_tok_lp).
 static void record_logprobs(rr_engine* e, Request* r, int row) {
     const int k = r->top_lp > 1 ? r->top_lp : 1;
     const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
     const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
     r->lp.insert(r->lp.end(), v, v + k);
     r->lp_id.insert(r->lp_id.end(), id, id + k);
+    if (r->sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
 }
 
-// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirror of d_topn in step.
+// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirrors of d_topn and d_samp in step.
 static void set_row_topn(rr_engine* e, int b, const Request* r) {
     const int t = r ? r->top_lp : -1;
     if (e->h_topn_mirror[b] != t) { e->h_topn_mirror[b] = t; e->topn_dirty = true; }
+    const float temp = r ? r->temp : 0.f, top_p = r ? r->top_p : 1.f;
+    const uint64_t seed = r ? r->seed : 0;
+    if (e->h_temp_mirror[b] != temp || e->h_topp_mirror[b] != top_p || e->h_seed_mirror[b] != seed) {
+        e->h_temp_mirror[b] = temp; e->h_topp_mirror[b] = top_p; e->h_seed_mirror[b] = seed;
+        e->samp_dirty = true;
+    }
 }
 
 // Caller holds e->mu.  Returns the hook call to make once the lock is released (tag == 0 and no hook: nothing).
@@ -589,6 +655,8 @@ static void forget_prefixes(rr_engine* e) {
 static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
     std::vector<int32_t> ids, seq_start, slots, topn, pos0;
+    std::vector<float> temps, topps;
+    std::vector<uint64_t> seeds;
     std::vector<Request*> chunk;
     std::vector<DoneNote> notes;
     KvCopyList* copies = new KvCopyList();
@@ -596,9 +664,10 @@ static void worker_main(rr_engine* e) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
         chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); topn.clear(); pos0.clear();
+        temps.clear(); topps.clear(); seeds.clear();
         copies->count = 0;
         int active = 0;
-        bool lp_step = false;
+        bool lp_step = false, samp_step = false;
         uint64_t epoch = 0;
         {
             std::unique_lock<std::mutex> lk(e->mu);
@@ -612,6 +681,7 @@ static void worker_main(rr_engine* e) {
                 }
                 active += r != nullptr;
                 lp_step = lp_step || (r && r->top_lp >= 0);
+                samp_step = samp_step || (r && r->sampled());
             }
             if (e->waiting.empty() && active == 0) {
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
@@ -645,6 +715,7 @@ static void worker_main(rr_engine* e) {
                 chunk.push_back(r);
                 slots.push_back(b);
                 topn.push_back(r->top_lp);
+                temps.push_back(r->temp); topps.push_back(r->top_p); seeds.push_back(r->seed);
                 ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
@@ -670,7 +741,8 @@ static void worker_main(rr_engine* e) {
         }
         if (!chunk.empty()) {
             int rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 topn.data(), e->o.prefix_cache ? pos0.data() : nullptr, copies);
+                                 topn.data(), e->o.prefix_cache ? pos0.data() : nullptr, copies, temps.data(), topps.data(),
+                                 seeds.data());
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
@@ -716,8 +788,17 @@ static void worker_main(rr_engine* e) {
             cudaMemcpyAsync(e->d_topn, e->h_topn, sizeof(int32_t) * e->Bm, cudaMemcpyHostToDevice, s);
             e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
         }
+        if (samp_step && e->samp_dirty) {
+            const size_t B = (size_t)e->Bm;
+            memcpy(e->h_samp, e->h_seed_mirror.data(), sizeof(uint64_t) * B);
+            memcpy(e->h_samp + 8 * B, e->h_temp_mirror.data(), sizeof(float) * B);
+            memcpy(e->h_samp + 12 * B, e->h_topp_mirror.data(), sizeof(float) * B);
+            e->samp_dirty = false;
+            cudaMemcpyAsync(e->d_samp, e->h_samp, SAMP_BYTES * B, cudaMemcpyHostToDevice, s);
+            e->st.h2d_bytes += SAMP_BYTES * B;
+        }
         cudaEventRecord(e->ev0, s);
-        int rc = run_decode_step(e, lp_step);
+        int rc = run_decode_step(e, lp_step, samp_step);
         cudaEventRecord(e->ev1, s);
         cudaMemcpyAsync(e->h_tok, e->d_tok, sizeof(int32_t) * e->Bm, cudaMemcpyDeviceToHost, s);
         if (lp_step) {
@@ -725,6 +806,10 @@ static void worker_main(rr_engine* e) {
             cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s);
             cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s);
             e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
+            if (samp_step) {
+                cudaMemcpyAsync(e->h_tok_lp, e->d_tok_lp, sizeof(float) * e->Bm, cudaMemcpyDeviceToHost, s);
+                e->st.d2h_bytes += sizeof(float) * e->Bm;
+            }
         }
         cudaError_t se = cudaStreamSynchronize(s);
         e->st.d2h_bytes += sizeof(int32_t) * e->Bm;
@@ -855,6 +940,12 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRYC(cudaMallocHost(&e->h_lp, sizeof(float) * B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_lp_id, sizeof(int32_t) * B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_topn, sizeof(int32_t) * B));
+    TRY(dalloc(e, &e->d_samp, (size_t)SAMP_BYTES * B));           // zero: every row greedy
+    TRY(dalloc(e, &e->d_samp_pf, (size_t)SAMP_PF_BYTES * B));
+    TRY(dalloc(e, (char**)&e->sample_ws, sample_ws_bytes(B, d.vocab), false));
+    TRY(dalloc(e, &e->d_tok_lp, B));
+    TRYC(cudaMallocHost(&e->h_samp, (size_t)SAMP_PF_BYTES * B));
+    TRYC(cudaMallocHost(&e->h_tok_lp, sizeof(float) * B));
 
     e->pl_qkv.resize(L); e->pl_o.resize(L); e->pl_gu.resize(L); e->pl_down.resize(L);
     e->attn_args.resize(L);
@@ -916,6 +1007,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->row_req.assign(B, nullptr);
     e->h_slot_mirror.assign(B, -1);
     e->h_topn_mirror.assign(B, -1);
+    e->h_seed_mirror.assign(B, 0); e->h_temp_mirror.assign(B, 0.f); e->h_topp_mirror.assign(B, 1.f);
+    e->samp_dirty = true;
     if (e->o.prefix_cache) { e->retained.assign(B, {}); e->retained_used.assign(B, 0); }
     e->worker = std::thread(worker_main, e);
     *out = e;
@@ -931,14 +1024,16 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->worker.joinable()) e->worker.join();
     cudaSetDevice(e->o.device);
     if (e->stream) cudaStreamSynchronize(e->stream);
-    if (e->graph) cudaGraphExecDestroy(e->graph);
-    if (e->graph_lp) cudaGraphExecDestroy(e->graph_lp);
+    for (cudaGraphExec_t g : e->graph)
+        if (g) cudaGraphExecDestroy(g);
     for (void* p : e->allocs) cudaFree(p);
     if (e->h_stage) cudaFreeHost(e->h_stage);
     if (e->h_tok) cudaFreeHost(e->h_tok);
     if (e->h_lp) cudaFreeHost(e->h_lp);
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
     if (e->h_topn) cudaFreeHost(e->h_topn);
+    if (e->h_samp) cudaFreeHost(e->h_samp);
+    if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) cudaStreamDestroy(e->stream);
@@ -1005,10 +1100,12 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
 
 namespace rr {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, int top_logprobs) {
+                         uint64_t* ticket, int top_logprobs, float temperature, float top_p, uint64_t seed) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
     if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
-    if (top_logprobs >= 0 && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK)) return RR_INVALID_ARGUMENT;
+    if (!sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
+    if ((top_logprobs >= 0 || temperature > 0.f) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
+        return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
         if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
@@ -1019,8 +1116,9 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     r->out.reserve(max_new_tokens);
     r->tag = tag;
     r->top_lp = top_logprobs;
+    if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
     if (top_logprobs >= 0) {
-        const size_t k = top_logprobs > 1 ? top_logprobs : 1;
+        const size_t k = r->lp_width();
         r->lp.reserve(k * max_new_tokens); r->lp_id.reserve(k * max_new_tokens);
     }
     std::vector<DoneNote> notes;
@@ -1065,11 +1163,17 @@ RR_API int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, in
     return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs);
 }
 
+RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                    int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
+    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs, temperature, top_p,
+                                    seed);
+}
+
 // Caller holds e->mu.  The first min(n, max_tokens_out) tokens' pairs of a logprobs request into [max_tokens_out][K].
 static void copy_logprobs(const Request* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
     if (r->top_lp < 0 || t <= 0) return;
-    const size_t m = (size_t)t * (r->top_lp > 1 ? r->top_lp : 1);
+    const size_t m = (size_t)t * r->lp_width();
     if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
     if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
 }

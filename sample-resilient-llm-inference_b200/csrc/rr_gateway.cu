@@ -48,6 +48,8 @@ struct GwReq {
     int top_lp = -1;                  // rr_gateway_submit_logprobs: handed to every engine the request is admitted to
     std::vector<float> lp;            // [tokens.size()][max(1, top_lp)]
     std::vector<int32_t> lp_id;
+    float temp = 0.f, top_p = 1.f;    // rr_gateway_submit_sampled: handed to every engine the request is admitted to
+    uint64_t seed = 0;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
@@ -60,6 +62,9 @@ struct Pending {
     int tokens;        // DONE: completion tokens; BURST: burst size
     int aux = 0;       // rr_event.chain_start of a DONE (latency, us) / FAIL (1 = timeout): latency-based routers only
 };
+
+// pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair (rr_engine_submit_sampled)
+static size_t gw_lp_width(const GwReq* r) { return (size_t)(r->top_lp > 1 ? r->top_lp : 1) + (r->temp > 0.f ? 1 : 0); }
 
 }  // namespace
 
@@ -120,6 +125,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     GwReq* r = nullptr;
     rr_engine* eng = nullptr;
     int max_new = 0, top_lp = -1;
+    size_t k = 1;
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -128,12 +134,12 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         eng = r->eng;
         max_new = r->max_new;
         top_lp = r->top_lp;
+        k = gw_lp_width(r);
     }
     // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
     memset(&comp, 0, sizeof(comp));
     std::vector<int32_t> toks((size_t)(max_new > 0 ? max_new : 1));
-    const size_t k = top_lp > 1 ? (size_t)top_lp : 1;
     std::vector<float> lps(top_lp >= 0 ? toks.size() * k : 0);
     std::vector<int32_t> lp_ids(lps.size());
     int wrc = RR_INVALID_ARGUMENT;
@@ -278,7 +284,7 @@ static void gw_dispatch(rr_gateway* g) {
             uint64_t tk = 0;
             int src = RR_INTERNAL;
             if (!cancelled && eng) src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk,
-                                                           r->top_lp);
+                                                           r->top_lp, r->temp, r->top_p, r->seed);
             bool cancel_now = false;
             std::unique_lock<std::mutex> lk(g->mu);
             if (src == RR_OK) {
@@ -370,9 +376,11 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
 }
 
 static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
-                     int max_new_tokens, int declare_burst, int top_logprobs, uint64_t* tickets) {
+                     int max_new_tokens, int declare_burst, int top_logprobs, uint64_t* tickets, float temperature = 0.f,
+                     float top_p = 1.f, uint64_t seed = 0) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
     if (top_logprobs < -1 || top_logprobs > rr::LP_MAX_TOP) return RR_INVALID_ARGUMENT;
+    if (!rr::sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n; ++i) {
         const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens);
         if (rc != RR_OK) return rc;
@@ -382,6 +390,7 @@ static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const 
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
         r->group = group; r->max_new = max_new_tokens; r->top_lp = top_logprobs;
+        if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -420,11 +429,17 @@ RR_API int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* p
     return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket);
 }
 
-// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][max(1, top_lp)].
+RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                     int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
+    const int32_t start[2] = {0, n_prompt};
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket, temperature, top_p, seed);
+}
+
+// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][gw_lp_width(r)].
 static void gw_copy_logprobs(const GwReq* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
     if (r->top_lp < 0 || t <= 0) return;
-    const size_t m = (size_t)t * (r->top_lp > 1 ? r->top_lp : 1);
+    const size_t m = (size_t)t * gw_lp_width(r);
     if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
     if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
 }

@@ -78,7 +78,12 @@ int num_sms();
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)
 typedef void (*EngineDoneHook)(void* ctx, uint64_t tag, uint64_t ticket, int status, int n_generated);
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, int top_logprobs = -1);
+                         uint64_t* ticket, int top_logprobs = -1, float temperature = 0.f, float top_p = 1.f,
+                         uint64_t seed = 0);
+// OpenAI's ranges for a sampled request (rr_engine_submit_sampled): 0 <= temperature <= 2, 0 <= top_p <= 1 (NaN fails).
+inline bool sample_params_ok(float temperature, float top_p) {
+    return temperature >= 0.f && temperature <= 2.f && top_p >= 0.f && top_p <= 1.f;
+}
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
@@ -186,8 +191,16 @@ constexpr int LP_CHUNK = 8192;        // columns per chunk CTA (staged in 32 KB 
 constexpr int LP_MAX_CHUNKS = 64;     // vocab <= 64 * 8192 = 524288
 constexpr int LP_LAUNCHES = 2;
 size_t logprobs_ws_bytes(int rows, int vocab);
+// tok (optional): also tok_lp[r] = x[tok[r]] - logsumexp(x) for those rows (a sampled token's own logprob).
 void launch_logprobs(const float* logits, int ld, int rows, int vocab, const int32_t* top_n, int max_top, void* ws,
-                     float* lp_out, int32_t* id_out, cudaStream_t st);
+                     float* lp_out, int32_t* id_out, cudaStream_t st, const int32_t* tok = nullptr,
+                     float* tok_lp = nullptr);
+// Seeded temperature / top-p draw (rr_op_sample) over fp32 logits [rows][ld], same shape limits as launch_logprobs: rows
+// with temperature[r] > 0 get out_tok[r], the others are not touched.  ws = sample_ws_bytes(rows, vocab) of scratch.
+constexpr int SAMPLE_LAUNCHES = 3;
+size_t sample_ws_bytes(int rows, int vocab);
+void launch_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
+                   const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* ws, cudaStream_t st);
 
 // ---- attention (rr_attn_decode.cu, rr_attn_tc.cu) ---------------------------------------------------
 struct DecodeAttnArgs {

@@ -7,6 +7,7 @@ computation happens in the CUDA library.  Replaces one `bedrock/...` deployment 
 from __future__ import annotations
 
 import ctypes as C
+import secrets
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -27,7 +28,8 @@ class CompletionRecord:
     t_submit: float
     t_first_token: float
     t_done: float
-    # submit(top_logprobs=k): per generated token the max(1, k) most likely (token id, logprob) pairs, best first
+    # submit(top_logprobs=k): per generated token the max(1, k) most likely (token id, logprob) pairs, best first; with
+    # temperature > 0 followed by the generated token's own pair
     logprobs: Optional[List[List[Tuple[int, float]]]] = None
     # prompt tokens whose KV came from the prefix cache (Engine(prefix_cache=True)); 0 otherwise
     n_cached: int = 0
@@ -143,11 +145,23 @@ class Engine:
         return nxt, logits
 
     # ---- serving interface ----------------------------------------------------------------------
-    def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None) -> int:
+    def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
+               temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
-        (the generated tokens do not change)."""
+        (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
+        nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
+        rr_engine_submit_sampled; None or 0 is greedy."""
         ids = _i32(prompt_ids)
         t = C.c_uint64()
+        if temperature:
+            seed = secrets.randbits(64) if seed is None else int(seed) % 2**64
+            k = -1 if top_logprobs is None else int(top_logprobs)
+            _lib.check(_lib.lib.rr_engine_submit_sampled(self._h, _p(ids), len(ids), max_new_tokens, k, float(temperature),
+                                                         1.0 if top_p is None else float(top_p), seed, C.byref(t)),
+                       "rr_engine_submit_sampled")
+            if k >= 0:
+                self._lp_k[t.value] = max(1, k) + 1
+            return t.value
         if top_logprobs is None:
             _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(t)),
                        "rr_engine_submit")

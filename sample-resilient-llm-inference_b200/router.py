@@ -15,6 +15,8 @@ Python/CPU implementation of the routing logic on this path.
 from __future__ import annotations
 
 import ctypes as C
+import math
+import secrets
 import threading
 import time
 import uuid
@@ -167,6 +169,30 @@ def check_logprobs(logprobs: Any, top_logprobs: Any) -> Optional[int]:
     return 0 if top_logprobs is None else top_logprobs
 
 
+MAX_TEMPERATURE = 2.0        # OpenAI's range for `temperature`
+
+
+def _is_number(v: Any) -> bool:
+    return isinstance(v, (int, float)) and not isinstance(v, bool) and math.isfinite(v)
+
+
+def check_sampling(temperature: Any = None, top_p: Any = None, seed: Any = None) -> Optional[Tuple[float, float, Optional[int]]]:
+    """OpenAI's rules for the `temperature` / `top_p` / `seed` request fields -> None (greedy: temperature absent or 0)
+    or (temperature, top_p, seed modulo 2^64 or None).  Raises BadRequestError (HTTP 400) for anything else.
+
+    Unlike OpenAI, whose default temperature is 1, an absent temperature means greedy decoding here, so that requests
+    without these fields generate exactly what they did before sampling existed."""
+    if temperature is not None and (not _is_number(temperature) or not 0 <= temperature <= MAX_TEMPERATURE):
+        raise BadRequestError(f"`temperature` must be a number from 0 to {MAX_TEMPERATURE:g}")
+    if top_p is not None and (not _is_number(top_p) or not 0 <= top_p <= 1):
+        raise BadRequestError("`top_p` must be a number from 0 to 1")
+    if seed is not None and (isinstance(seed, bool) or not isinstance(seed, int) or not -2**63 <= seed < 2**64):
+        raise BadRequestError("`seed` must be an integer from -2^63 to 2^64 - 1")
+    if temperature is None or temperature == 0:
+        return None
+    return float(temperature), 1.0 if top_p is None else float(top_p), None if seed is None else seed % 2**64
+
+
 def _token_entry(tok: int, logprob: float) -> dict:
     """One token of the byte tokenizer in OpenAI's logprob shape (`token` is detokenize([tok]), `bytes` its byte)."""
     return {"token": detokenize([tok]), "logprob": logprob, "bytes": [(tok - 3) % 256] if tok >= 3 else []}
@@ -174,7 +200,7 @@ def _token_entry(tok: int, logprob: float) -> dict:
 
 def logprobs_content(tokens: Sequence[int], pairs: Sequence[Sequence[Tuple[int, float]]], top: int) -> List[dict]:
     """`choices[0].logprobs.content` for the generated tokens: pairs[i] = the engine's (id, logprob) list of token i, best
-    first; `top` alternatives each."""
+    first (a sampled request adds the token's own pair after them); `top` alternatives each."""
     out = []
     for tok, p in zip(tokens, pairs):
         lp = next((v for i, v in p if i == tok), p[0][1])
@@ -373,12 +399,15 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None, samp=None) -> int:
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        if top is None:
+        if samp is not None:
+            rc = _lib.lib.rr_gateway_submit_sampled(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                                    -1 if top is None else top, samp[0], samp[1], samp[2], C.byref(t))
+        elif top is None:
             rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new, C.byref(t))
         else:
             rc = _lib.lib.rr_gateway_submit_logprobs(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
@@ -388,19 +417,21 @@ class Router:
         return t.value
 
     @staticmethod
-    def _lp_bufs(top: Optional[int], max_new: int):
+    def _lp_bufs(top: Optional[int], max_new: int, sampled: bool = False):
+        """[max_new][max(1, top)] pair buffers; a sampled request has one more column, the generated token's own pair."""
         if top is None:
             return None, None, None, None
-        lp = np.zeros((max_new, max(1, top)), dtype=np.float32)
-        ids = np.zeros((max_new, max(1, top)), dtype=np.int32)
+        w = max(1, top) + (1 if sampled else 0)
+        lp = np.zeros((max_new, w), dtype=np.float32)
+        ids = np.zeros((max_new, w), dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None):
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp)
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new)
+        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new, samp is not None)
         rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, float(timeout or 0.0), C.byref(res),
                                                toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
         if rc == 6:                      # client-side timeout: give the row back, count a failure against the deployment
@@ -414,12 +445,12 @@ class Router:
             content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), top), "refusal": None}
         return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
 
-    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None):
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top)
+    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None):
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp)
         deadline = None if not timeout else time.perf_counter() + timeout
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new)
+        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new, samp is not None)
         n, done = C.c_int32(), C.c_int32()
         sent, finished = 0, False
 
@@ -558,12 +589,25 @@ class Router:
             raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
         return top
 
+    @staticmethod
+    def _sampling(temperature, top_p, seed):
+        """Validated sampling setting (None = greedy); a request without a seed gets one here, once, so that a fallback
+        re-admission draws the same tokens."""
+        samp = check_sampling(temperature, top_p, seed)
+        if samp is not None and samp[2] is None:
+            samp = (samp[0], samp[1], secrets.randbits(64))
+        return samp
+
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
-                   logprobs: bool = False, top_logprobs: Optional[int] = None, **_ignored) -> ModelResponse:
+                   logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
+                   top_p: Optional[float] = None, seed: Optional[int] = None, **_ignored) -> ModelResponse:
         """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
-        (0..20) most likely alternatives, as the OpenAI API returns them."""
+        (0..20) most likely alternatives, as the OpenAI API returns them.  temperature > 0: every token is drawn from
+        the top_p nucleus of softmax(logits / temperature) with the request's seed (rr_op_sample); absent or 0 is
+        greedy.  Stub backends validate these and keep their fixed reply."""
         top = self._logprobs_top(logprobs, top_logprobs)
+        samp = self._sampling(temperature, top_p, seed)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -573,7 +617,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top)
+            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp)
         # ---- host loop (StubBackend): same admission events, one K1 launch per event
         t_start = time.perf_counter()
         chain_start = 0
@@ -610,12 +654,14 @@ class Router:
 
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                           max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
-                          logprobs: bool = False, top_logprobs: Optional[int] = None):
+                          logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
+                          top_p: Optional[float] = None, seed: Optional[int] = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
         (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
-        fallback chain; rate limiting raises RateLimitError before anything is yielded."""
+        fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling as in completion()."""
         top = self._logprobs_top(logprobs, top_logprobs)
+        samp = self._sampling(temperature, top_p, seed)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -624,7 +670,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top)
+            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp)
             return
         deadline = None if not timeout else time.perf_counter() + timeout
         chain_start = 0

@@ -16,7 +16,7 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend, check_logprobs)
+                     StubBackend, check_logprobs, check_sampling)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -38,7 +38,7 @@ def create_app(router: Router):
         import anyio.to_thread
         anyio.to_thread.current_default_thread_limiter().total_tokens = 2048
 
-    async def stream_completion(model, messages, body, lp_kw):
+    async def stream_completion(model, messages, body, lp_kw, samp_kw):
         """Server-sent events in the OpenAI chunk format; the first chunk leaves when the first token exists (TTFT).
         With logprobs, every chunk carries `logprobs.content` for the tokens of its delta (the closing chunk null)."""
         import json as _json
@@ -46,7 +46,7 @@ def create_app(router: Router):
         from fastapi.responses import StreamingResponse
         from .router import detokenize
         gen = router.completion_stream(model=model, messages=messages, timeout=body.get("timeout"),
-                                       max_tokens=body.get("max_tokens"), **lp_kw)
+                                       max_tokens=body.get("max_tokens"), **lp_kw, **samp_kw)
         try:
             first = await run_in_threadpool(next, gen)            # admission errors surface before the 200
         except RateLimitError as e:
@@ -92,13 +92,16 @@ def create_app(router: Router):
             lp_kw = {}
             if check_logprobs(body.get("logprobs"), body.get("top_logprobs")) is not None:
                 lp_kw = {"logprobs": True, "top_logprobs": body.get("top_logprobs")}
+            samp_kw = {k: body[k] for k in ("temperature", "top_p", "seed") if body.get(k) is not None}
+            check_sampling(**samp_kw)
         except BadRequestError as e:
             return JSONResponse(_error_body(e, "invalid_request_error"), 400)
         if body.get("stream"):
-            return await stream_completion(model, messages, body, lp_kw)
+            return await stream_completion(model, messages, body, lp_kw, samp_kw)
         try:
             resp = await run_in_threadpool(router.completion, model=model, messages=messages,
-                                           timeout=body.get("timeout"), max_tokens=body.get("max_tokens"), **lp_kw)
+                                           timeout=body.get("timeout"), max_tokens=body.get("max_tokens"), **lp_kw,
+                                           **samp_kw)
             return JSONResponse(resp.model_dump())
         except RateLimitError as e:
             return JSONResponse(_error_body(e, "rate_limit_error"), 429, headers={"retry-after": "1"})
