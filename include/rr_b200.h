@@ -233,6 +233,20 @@ int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, const int32
  * vocab <= 524288 and ld % 4 == 0.  Deterministic: every sum is exact (fixed point) or runs in a fixed order. */
 int rr_op_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
                  const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* stream);
+/* Frequency / presence penalties and logit bias, in place over fp32 logits rows x (row r at logits + r * ld), as the
+ * engine applies them before the argmax, the sampler and logprobs.  All per-row arrays are device memory.  With c_j the
+ * number of times token j occurs in row r's history (hist + r * hist_ld, hist_len[r] tokens: the tokens generated so far)
+ * and b_j the bias of token j (the n_bias[r] entries of bias_ids / bias_vals + r * bias_ld; ids unique), every processed
+ * logit becomes
+ *   x'_j = (x_j + b_j) - (c_j * frequency_penalty[r] + [c_j > 0] * presence_penalty[r]),
+ * each operation one fp32 round-to-nearest op without FMA contraction.  A token without a bias entry skips the addition, one
+ * with c_j = 0 the subtraction; a row with both penalties 0 and no bias entries is not touched.  Deterministic: the counts
+ * are integer atomics and exactly one thread writes each logit.  History ids outside [0, vocab) are ignored; hist_len[r] is
+ * clamped to [0, hist_ld] and n_bias[r] to [0, bias_ld].  RR_INVALID_ARGUMENT before touching the device unless no pointer
+ * is null, 1 <= rows <= 65535, 1 <= vocab <= ld, vocab <= 524288, ld % 4 == 0, hist_ld >= 0 and 0 <= bias_ld <= 300. */
+int rr_op_logit_penalties(float* logits, int ld, int rows, int vocab, const int32_t* hist, int hist_ld,
+                          const int32_t* hist_len, const float* frequency_penalty, const float* presence_penalty,
+                          const int32_t* bias_ids, const float* bias_vals, int bias_ld, const int32_t* n_bias, void* stream);
 int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                       const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                       int n_kv_heads, int ctx_max /* % 64 == 0 */, int n_slots, float scale,
@@ -430,6 +444,17 @@ int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double time
  * 0 <= top_p <= 1. */
 int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int top_logprobs,
                              float temperature, float top_p, uint64_t seed, uint64_t* ticket);
+/* Penalties and logit bias (OpenAI `frequency_penalty` / `presence_penalty` / `logit_bias`) on top of
+ * rr_engine_submit_sampled: before every token of the request is picked (argmax, or the draw with temperature > 0), its
+ * logits go through rr_op_logit_penalties with the tokens the request generated so far as the history (prompt tokens do
+ * not count, so the first token gets the bias only).  Logprobs describe the processed logits.  Tokens depend only on the
+ * prompt, the weights and the parameters.  Penalties 0 and n_bias = 0 behave exactly as rr_engine_submit_sampled.
+ * RR_INVALID_ARGUMENT unless rr_engine_submit_sampled's ranges hold, -2 <= penalties <= 2, 0 <= n_bias <= 300, the
+ * bias ids are unique and in [0, vocab) and -100 <= bias values <= 100. */
+int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int top_logprobs,
+                               float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                               float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
+                               uint64_t* ticket);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -525,6 +550,13 @@ int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double ti
  * trace is the same as rr_gateway_submit's. */
 int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                               int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket);
+/* Penalties and logit bias (rr_engine_submit_processed): stored with the request and handed to every engine it is admitted
+ * to, a fallback re-admission included.  Bias ids must lie in [0, the smallest vocabulary of the gateway's engines).  The
+ * admission trace is the same as rr_gateway_submit's. */
+int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                                float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
+                                uint64_t* ticket);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

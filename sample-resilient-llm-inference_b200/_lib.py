@@ -154,6 +154,7 @@ PROTOTYPES = {
     "rr_op_argmax": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]),
     "rr_op_logprobs": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp]),
     "rr_op_sample": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
+    "rr_op_logit_penalties": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, vp]),
     "rr_op_decode_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -186,6 +187,8 @@ PROTOTYPES = {
                                           C.POINTER(C.c_double), c_f32p, c_i32p]),
     "rr_engine_submit_sampled": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
                                            C.POINTER(C.c_uint64)]),
+    "rr_engine_submit_processed": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
+                                             C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.POINTER(C.c_uint64)]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
                                       C.POINTER(Completion), c_i32p]),
     "rr_engine_now": (C.c_double, [vp]),
@@ -207,6 +210,9 @@ PROTOTYPES = {
                                            C.POINTER(GatewayResult), c_f32p, c_i32p]),
     "rr_gateway_submit_sampled": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
                                             C.c_uint64, C.POINTER(C.c_uint64)]),
+    "rr_gateway_submit_processed": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                              C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
+                                              C.POINTER(C.c_uint64)]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),
     "rr_gateway_quiesce": (C.c_int, [vp, C.c_double]),
     "rr_gateway_get_stats": (C.c_int, [vp, C.POINTER(GatewayStats)]),

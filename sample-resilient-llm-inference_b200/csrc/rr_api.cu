@@ -224,6 +224,34 @@ RR_API int rr_op_sample(const float* logits, int ld, int rows, int vocab, const 
     return check_last();
 }
 
+// Penalties and logit bias in place, as the engine applies them before the argmax.  hist_len and n_bias are device data:
+// the kernel clamps them to [0, hist_ld] and [0, bias_ld] and skips ids outside [0, vocab).  The count workspace is
+// stream-ordered scratch memory, zeroed here; the kernel leaves it zero.
+RR_API int rr_op_logit_penalties(float* logits, int ld, int rows, int vocab, const int32_t* hist, int hist_ld,
+                                 const int32_t* hist_len, const float* frequency_penalty, const float* presence_penalty,
+                                 const int32_t* bias_ids, const float* bias_vals, int bias_ld, const int32_t* n_bias,
+                                 void* stream) {
+    if (!logits || !hist || !hist_len || !frequency_penalty || !presence_penalty || !bias_ids || !bias_vals || !n_bias)
+        return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > 65535 || vocab < 1 || vocab > ld || ld % 4 || vocab > LP_MAX_CHUNKS * LP_CHUNK)
+        return RR_INVALID_ARGUMENT;
+    if (hist_ld < 0 || bias_ld < 0 || bias_ld > PEN_MAX_BIAS) return RR_INVALID_ARGUMENT;
+    cudaStream_t st = (cudaStream_t)stream;
+    void* ws = nullptr;
+    const size_t ws_bytes = sizeof(int32_t) * (size_t)rows * vocab;
+    cudaError_t e = cudaMallocAsync(&ws, ws_bytes, st);
+    if (e != cudaSuccess) { note_cuda_error(e); return RR_CUDA_ERROR; }
+    e = cudaMemsetAsync(ws, 0, ws_bytes, st);
+    if (e != cudaSuccess) { cudaFreeAsync(ws, st); note_cuda_error(e); return RR_CUDA_ERROR; }
+    PenaltyArgs a;
+    a.freq = frequency_penalty; a.pres = presence_penalty; a.bias_ids = bias_ids; a.n_bias = n_bias; a.bias_vals = bias_vals;
+    a.bias_ld = bias_ld; a.hist = const_cast<int32_t*>(hist); a.hist_ld = hist_ld; a.hist_len = hist_len;
+    a.app_tok = nullptr; a.app_pos = nullptr; a.gen0 = nullptr;
+    launch_logit_penalties(logits, ld, rows, vocab, a, (int32_t*)ws, st);
+    cudaFreeAsync(ws, st);
+    return check_last();
+}
+
 RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_cache, void* out,
                              const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                              int n_kv_heads, int ctx_max, int n_slots, float scale, int kv_splits, void* stream) {

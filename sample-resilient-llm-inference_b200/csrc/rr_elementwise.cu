@@ -853,6 +853,69 @@ void launch_sample(const float* logits, int ld, int rows, int vocab, const float
     launch_pdl(sample_merge_kernel, dim3(rows), dim3(32), 0, st, temperature, nc, (const SpPart*)part, out_tok);
 }
 
+// ---- frequency / presence penalties and logit bias (rr_op_logit_penalties) ------------------------------------------
+// One CTA per row, three phases separated by barriers: (1) x_j += b_j over the row's bias entries (unique ids: no two
+// threads write one logit); (2) cnt[t] += 1 for every history token t, integer atomics into the row's [vocab] slice of the
+// workspace; (3) per history entry old = atomicExch(&cnt[t], 0): the one thread that sees old > 0 applies the penalty with
+// c = old.  Whichever thread wins computes the same value, and the exchange leaves the workspace zeroed for the next call.
+// Work per row is O(history + bias entries); nothing is sized by shared memory, so the history has no cap.
+constexpr int PEN_THREADS = 256;
+
+__global__ void __launch_bounds__(PEN_THREADS)
+logit_penalties_kernel(float* __restrict__ logits, int ld, int vocab, PenaltyArgs a, int32_t* __restrict__ cnt_ws) {
+    griddep_launch();
+    const int tr_slot = trace_begin(TR_PENALTY);
+    griddep_wait();
+    trace_dep(tr_slot);
+    const int row = blockIdx.x, tid = threadIdx.x;
+    const float af = a.freq[row], ap = a.pres[row];
+    const int nb = min(max(a.n_bias[row], 0), a.bias_ld);
+    const bool pen = af != 0.f || ap != 0.f;
+    if (!pen && nb == 0) return;
+    float* x = logits + (size_t)row * ld;
+    int32_t* h = a.hist ? a.hist + (size_t)row * a.hist_ld : nullptr;
+    int len = 0;
+    if (h && a.app_tok) {
+        // the engine's decode step: the row's input token (its last generated token, at position app_pos) joins the
+        // history at index app_pos - gen0 before the logits are processed
+        const int i = a.app_pos[row] - a.gen0[row];
+        if (i >= 0 && i < a.hist_ld) {
+            if (tid == 0) h[i] = a.app_tok[row];
+            len = i + 1;
+        }
+        __syncthreads();
+    } else if (h && a.hist_len) {
+        len = min(max(a.hist_len[row], 0), a.hist_ld);
+    }
+    const int32_t* bid = a.bias_ids + (size_t)row * a.bias_ld;
+    const float* bv = a.bias_vals + (size_t)row * a.bias_ld;
+    for (int k = tid; k < nb; k += PEN_THREADS) {
+        const int j = bid[k];
+        if (j >= 0 && j < vocab) x[j] = __fadd_rn(x[j], bv[k]);
+    }
+    if (!pen || len == 0) { trace_end(tr_slot); return; }
+    int32_t* cnt = cnt_ws + (size_t)row * vocab;
+    __syncthreads();
+    for (int k = tid; k < len; k += PEN_THREADS) {
+        const int t = h[k];
+        if (t >= 0 && t < vocab) atomicAdd(&cnt[t], 1);
+    }
+    __syncthreads();
+    for (int k = tid; k < len; k += PEN_THREADS) {
+        const int t = h[k];
+        if (t < 0 || t >= vocab) continue;
+        const int c = atomicExch(&cnt[t], 0);
+        if (c > 0) x[t] = __fsub_rn(x[t], __fadd_rn(__fmul_rn((float)c, af), ap));
+    }
+    trace_end(tr_slot);
+}
+
+void launch_logit_penalties(float* logits, int ld, int rows, int vocab, const PenaltyArgs& a, int32_t* cnt_ws,
+                            cudaStream_t st) {
+    if (rows <= 0) return;
+    launch_pdl(logit_penalties_kernel, dim3(rows), dim3(PEN_THREADS), 0, st, logits, ld, vocab, a, cnt_ws);
+}
+
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }
 
 }  // namespace rr

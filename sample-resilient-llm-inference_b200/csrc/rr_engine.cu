@@ -15,6 +15,7 @@
 #include "rr_kernels.h"
 #include "rr_launch.cuh"
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -96,6 +97,12 @@ struct Request {
     bool sampled() const { return temp > 0.f; }
     // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
     int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
+    // rr_engine_submit_processed: frequency / presence penalties over the generated tokens and a logit bias, applied to
+    // the logits before the token is picked (rr_op_logit_penalties)
+    float fpen = 0.f, ppen = 0.f;
+    std::vector<int32_t> bias_id;
+    std::vector<float> bias_val;
+    bool processed() const { return fpen != 0.f || ppen != 0.f || !bias_id.empty(); }
 };
 
 // Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
@@ -104,6 +111,43 @@ constexpr int PREFIX_MIN = 64;
 
 // Sampling parameter blocks, per row at stride n: seed (8 bytes) | temperature | top_p, and in prefill also | position.
 constexpr int SAMP_BYTES = 16, SAMP_PF_BYTES = 20;
+
+// Penalty parameter blocks, per row at stride n: frequency_penalty | presence_penalty | gen0 (the position of the first
+// generated token) | n_bias, then bias ids [n][bias_ld] and values [n][bias_ld].  Decode rows use bias_ld = PEN_MAX_BIAS
+// (fixed: the graphs hold it); a prefill chunk uses the largest bias count among its sequences.
+static size_t pen_bytes(int n, int bias_ld) { return (size_t)n * (16 + 8 * (size_t)bias_ld); }
+static PenaltyArgs pen_args(const char* blk, int n, int bias_ld) {
+    PenaltyArgs a;
+    a.freq = (const float*)blk; a.pres = (const float*)(blk + 4 * (size_t)n);
+    a.gen0 = (const int32_t*)(blk + 8 * (size_t)n); a.n_bias = (const int32_t*)(blk + 12 * (size_t)n);
+    a.bias_ids = (const int32_t*)(blk + 16 * (size_t)n);
+    a.bias_vals = (const float*)(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld);
+    a.bias_ld = bias_ld;
+    a.hist = nullptr; a.hist_ld = 0; a.hist_len = nullptr; a.app_tok = nullptr; a.app_pos = nullptr;
+    return a;
+}
+// Writes row i of a block at stride n (r == nullptr: an unprocessed row, all zero).
+static void pen_fill_row(char* blk, int n, int bias_ld, int i, const Request* r, float freq, float pres, int gen0) {
+    const int nb = r ? (int)r->bias_id.size() : 0;
+    ((float*)blk)[i] = freq; ((float*)(blk + 4 * (size_t)n))[i] = pres;
+    ((int32_t*)(blk + 8 * (size_t)n))[i] = gen0; ((int32_t*)(blk + 12 * (size_t)n))[i] = nb;
+    if (nb) {
+        memcpy(blk + 16 * (size_t)n + 4 * ((size_t)i * bias_ld), r->bias_id.data(), 4 * (size_t)nb);
+        memcpy(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld + 4 * ((size_t)i * bias_ld), r->bias_val.data(), 4 * (size_t)nb);
+    }
+}
+
+bool penalty_params_ok(float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                       const float* bias_vals, int vocab) {
+    if (!(frequency_penalty >= -2.f && frequency_penalty <= 2.f && presence_penalty >= -2.f && presence_penalty <= 2.f))
+        return false;
+    if (n_bias < 0 || n_bias > PEN_MAX_BIAS || (n_bias > 0 && (!bias_ids || !bias_vals))) return false;
+    std::vector<int32_t> ids(bias_ids, bias_ids + n_bias);
+    for (int i = 0; i < n_bias; ++i)
+        if (ids[i] < 0 || ids[i] >= vocab || !(bias_vals[i] >= -100.f && bias_vals[i] <= 100.f)) return false;
+    std::sort(ids.begin(), ids.end());
+    return std::adjacent_find(ids.begin(), ids.end()) == ids.end();
+}
 
 }  // namespace rr
 
@@ -153,9 +197,10 @@ struct rr_engine {
     MlpItem* mlp_items = nullptr;     // device copy of the schedule (shared by all layers)
     unsigned* mlp_ready = nullptr;    // [n_slices] dependency counters, reset by the norm kernel before each launch
     int mlp_slices = 0, mlp_slice_kb = 0;
-    // decode step graphs by step_mode(): [0] plain, [1] + launch_logprobs, [2] + launch_sample, [3] both.  [0] is captured
-    // after the warm-up step, the others on first use: a step without logprobs or sampled rows replays the plain graph.
-    cudaGraphExec_t graph[4] = {nullptr, nullptr, nullptr, nullptr};
+    // decode step graphs by step_mode(): bit 0 + launch_logprobs, bit 1 + launch_sample, bit 2 + launch_logit_penalties.
+    // [0] (plain) is captured after the warm-up step, the others on first use: a step without logprobs, sampled or
+    // processed rows replays the plain graph.
+    cudaGraphExec_t graph[8] = {};
     bool warmed = false;
     int32_t *d_topn = nullptr, *d_topn_pf = nullptr;   // per decode row / per prefill sequence: top_lp, -1 = off
     void* lp_ws = nullptr;
@@ -166,6 +211,12 @@ struct rr_engine {
     char *d_samp = nullptr, *d_samp_pf = nullptr;
     void* sample_ws = nullptr;
     float* d_tok_lp = nullptr;                         // [Bm] the sampled token's logprob (sampled logprobs rows)
+    // penalties / logit bias, allocated on the first processed request (ensure_pen_buffers): the decode rows' parameter
+    // block (pen_args layout, stride Bm) and its pinned host mirror, the prefill chunk's block and its staging, the
+    // generated-token history [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
+    char *d_pen = nullptr, *d_pen_pf = nullptr, *h_pen = nullptr, *h_pen_pf = nullptr;
+    int32_t *d_hist = nullptr, *pen_ws = nullptr;
+    bool pen_dirty = false;
 
     // prefill working set
     int Tmax;
@@ -212,7 +263,7 @@ struct rr_engine {
     std::chrono::steady_clock::time_point t0;
 
     rr_engine_stats st;                  // written under gpu_mu (launch / timing counters) or mu (queued, active_rows)
-    uint64_t step_launches[4] = {0, 0, 0, 0};   // launches of one decode step, by step_mode()
+    uint64_t step_launches[8] = {};              // launches of one decode step, by step_mode()
     // completion hook (the native gateway, rr_gateway.cu): called on the worker / submitting thread, outside `mu`
     rr::EngineDoneHook hook = nullptr;
     void* hook_ctx = nullptr;
@@ -279,13 +330,43 @@ static void enqueue_sample(rr_engine* e, const char* samp, int n, int rows, cons
                   (const float*)(samp + (size_t)12 * n), (const uint64_t*)samp, position, tok, e->sample_ws, s);
 }
 
-static int step_mode(bool logprobs, bool sample) { return (logprobs ? 1 : 0) | (sample ? 2 : 0); }
+static int step_mode(bool logprobs, bool sample, bool pen) {
+    return (logprobs ? 1 : 0) | (sample ? 2 : 0) | (pen ? 4 : 0);
+}
+
+// Caller holds gpu_mu.  The penalty buffers, allocated on the first processed request, so an engine that never sees one
+// keeps its footprint.
+static int ensure_pen_buffers(rr_engine* e) {
+    if (e->d_pen) return RR_OK;
+    const int B = e->Bm;
+    const size_t blk = pen_bytes(B, PEN_MAX_BIAS);
+    char *dp = nullptr, *dpf = nullptr;
+    int32_t *hist = nullptr, *ws = nullptr;
+    int rc = dalloc(e, &dp, blk);
+    if (rc == RR_OK) rc = dalloc(e, &dpf, blk, false);
+    if (rc == RR_OK) rc = dalloc(e, &hist, (size_t)B * e->o.ctx_max, false);
+    if (rc == RR_OK) rc = dalloc(e, &ws, (size_t)B * e->d.vocab, false);
+    if (rc != RR_OK) return rc;
+    CK(cudaMemsetAsync(dp, 0, blk, e->stream));
+    CK(cudaMemsetAsync(ws, 0, sizeof(int32_t) * B * (size_t)e->d.vocab, e->stream));
+    char *hp = nullptr, *hpf = nullptr;
+    CK(cudaMallocHost(&hp, blk));
+    cudaError_t ce = cudaMallocHost(&hpf, blk);
+    if (ce != cudaSuccess) { cudaFreeHost(hp); rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
+    memset(hp, 0, blk);
+    CK(cudaStreamSynchronize(e->stream));
+    e->d_pen_pf = dpf; e->d_hist = hist; e->pen_ws = ws; e->h_pen = hp; e->h_pen_pf = hpf;
+    e->d_pen = dp;
+    return RR_OK;
+}
 
 // logprobs: launch_logprobs after the argmax for the rows with d_topn[row] >= 0 (the logits are left as they were)
 // sample: rows with temperature > 0 replace the argmax token by rr_op_sample's draw at position d_pos (argmax advanced it
 // to the generated token's position), before logprobs, which then also gives the drawn token's own logprob
+// pen: before the argmax, processed rows append their input token (the last generated one, at position d_pos) to the
+// history and get their penalties and logit bias applied to the logits, which argmax, sampler and logprobs then read
 static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, bool logprobs = false,
-                               bool sample = false) {
+                               bool sample = false, bool pen = false) {
     const rr_model_desc& d = e->d;
     const int B = e->Bm, L = d.n_layers;
     uint64_t nl = 0;
@@ -316,6 +397,11 @@ static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch,
                            d.hidden, d.rms_eps, s); ++nl;
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
+    if (pen) {
+        PenaltyArgs a = pen_args(e->d_pen, B, PEN_MAX_BIAS);
+        a.hist = e->d_hist; a.hist_ld = e->o.ctx_max; a.app_tok = e->d_tok; a.app_pos = e->d_pos;
+        launch_logit_penalties(e->logits, d.vocab, B, d.vocab, a, e->pen_ws, s); ++nl;
+    }
     launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
     if (sample) { enqueue_sample(e, e->d_samp, B, B, e->d_pos, e->d_tok, s); nl += SAMPLE_LAUNCHES; }
     if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s, sample ? e->d_tok : nullptr); nl += LP_LAUNCHES; }
@@ -329,7 +415,7 @@ static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uin
     cudaStream_t s = e->stream;
     cudaGraph_t g = nullptr;
     CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_decode_step(e, s, n_launch, mode & 1, mode & 2);
+    int rc = enqueue_decode_step(e, s, n_launch, mode & 1, mode & 2, mode & 4);
     cudaError_t ce = cudaStreamEndCapture(s, &g);
     if (rc != RR_OK || ce != cudaSuccess) { rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
     CK(cudaGraphInstantiate(out, g, 0));
@@ -337,14 +423,15 @@ static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uin
     return RR_OK;
 }
 
-// logprobs: also run launch_logprobs for the rows with d_topn >= 0; sample: also draw the rows with temperature > 0.  Each
-// combination has its own graph, captured on first use; a step without logprobs or sampled rows replays the plain graph.
-static int run_decode_step(rr_engine* e, bool logprobs = false, bool sample = false) {
+// logprobs: also run launch_logprobs for the rows with d_topn >= 0; sample: also draw the rows with temperature > 0; pen:
+// also process the logits of the rows with penalties or a logit bias.  Each combination has its own graph, captured on
+// first use; a step without logprobs, sampled or processed rows replays the plain graph.
+static int run_decode_step(rr_engine* e, bool logprobs = false, bool sample = false, bool pen = false) {
     cudaStream_t s = e->stream;
-    const int mode = step_mode(logprobs, sample);
+    const int mode = step_mode(logprobs, sample, pen);
     if (!e->warmed || !e->o.use_cuda_graph) {
         uint64_t nl = 0;
-        int rc = enqueue_decode_step(e, s, &nl, logprobs, sample);
+        int rc = enqueue_decode_step(e, s, &nl, logprobs, sample, pen);
         if (rc != RR_OK) return rc;
         e->step_launches[mode] = nl;
         e->st.kernel_launches += nl;
@@ -420,11 +507,13 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
 // Sampling: temp_host / topp_host / seed_host[n_seqs] (optional): sequences with temp_host[i] > 0 draw their first token
 // with rr_op_sample at position pos0[i] + their length (the prompt length); with logprobs its own logprob lands in h_tok_lp.
+// Logit bias: reqs[n_seqs] (optional): the logits of sequences whose request has a logit bias get it before the argmax and
+// the sampler (penalties count generated tokens only, so the first token has none); needs ensure_pen_buffers.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr,
                        const int32_t* pos0 = nullptr, const KvCopyList* copies = nullptr,
                        const float* temp_host = nullptr, const float* topp_host = nullptr,
-                       const uint64_t* seed_host = nullptr) {
+                       const uint64_t* seed_host = nullptr, Request* const* reqs = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
@@ -511,6 +600,18 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (launch_rows(P->down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
+    int max_bias = 0;
+    for (int i = 0; reqs && i < n_seqs; ++i)
+        if ((int)reqs[i]->bias_id.size() > max_bias) max_bias = (int)reqs[i]->bias_id.size();
+    if (max_bias > 0) {
+        if (!e->d_pen) return RR_INTERNAL;
+        for (int i = 0; i < n_seqs; ++i) pen_fill_row(e->h_pen_pf, n_seqs, max_bias, i, reqs[i], 0.f, 0.f, 0);
+        const size_t nb = pen_bytes(n_seqs, max_bias);
+        CK(cudaMemcpyAsync(e->d_pen_pf, e->h_pen_pf, nb, cudaMemcpyHostToDevice, s));
+        e->st.h2d_bytes += nb;
+        launch_logit_penalties(e->logits, d.vocab, n_seqs, d.vocab, pen_args(e->d_pen_pf, n_seqs, max_bias), e->pen_ws, s);
+        ++nl;
+    }
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
     bool samp = false;
     for (int i = 0; temp_host && i < n_seqs; ++i) samp = samp || temp_host[i] > 0.f;
@@ -582,7 +683,8 @@ static void record_logprobs(rr_engine* e, Request* r, int row) {
     if (r->sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
 }
 
-// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirrors of d_topn and d_samp in step.
+// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirrors of d_topn, d_samp and d_pen
+// in step.
 static void set_row_topn(rr_engine* e, int b, const Request* r) {
     const int t = r ? r->top_lp : -1;
     if (e->h_topn_mirror[b] != t) { e->h_topn_mirror[b] = t; e->topn_dirty = true; }
@@ -591,6 +693,18 @@ static void set_row_topn(rr_engine* e, int b, const Request* r) {
     if (e->h_temp_mirror[b] != temp || e->h_topp_mirror[b] != top_p || e->h_seed_mirror[b] != seed) {
         e->h_temp_mirror[b] = temp; e->h_topp_mirror[b] = top_p; e->h_seed_mirror[b] = seed;
         e->samp_dirty = true;
+    }
+    // h_pen is the host mirror of d_pen (absent until the first processed request; every row is unprocessed until then)
+    if (!e->h_pen) return;
+    const int B = e->Bm;
+    const bool was = ((const float*)e->h_pen)[b] != 0.f || ((const float*)(e->h_pen + 4 * (size_t)B))[b] != 0.f ||
+                     ((const int32_t*)(e->h_pen + 12 * (size_t)B))[b] != 0;
+    if (r && r->processed()) {
+        pen_fill_row(e->h_pen, B, PEN_MAX_BIAS, b, r, r->fpen, r->ppen, (int)r->prompt.size());
+        e->pen_dirty = true;
+    } else if (was) {
+        pen_fill_row(e->h_pen, B, PEN_MAX_BIAS, b, nullptr, 0.f, 0.f, 0);
+        e->pen_dirty = true;
     }
 }
 
@@ -667,7 +781,7 @@ static void worker_main(rr_engine* e) {
         temps.clear(); topps.clear(); seeds.clear();
         copies->count = 0;
         int active = 0;
-        bool lp_step = false, samp_step = false;
+        bool lp_step = false, samp_step = false, pen_step = false, pen_chunk = false;
         uint64_t epoch = 0;
         {
             std::unique_lock<std::mutex> lk(e->mu);
@@ -682,6 +796,7 @@ static void worker_main(rr_engine* e) {
                 active += r != nullptr;
                 lp_step = lp_step || (r && r->top_lp >= 0);
                 samp_step = samp_step || (r && r->sampled());
+                pen_step = pen_step || (r && r->processed());
             }
             if (e->waiting.empty() && active == 0) {
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
@@ -716,6 +831,7 @@ static void worker_main(rr_engine* e) {
                 slots.push_back(b);
                 topn.push_back(r->top_lp);
                 temps.push_back(r->temp); topps.push_back(r->top_p); seeds.push_back(r->seed);
+                pen_chunk = pen_chunk || r->processed();
                 ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
@@ -740,9 +856,11 @@ static void worker_main(rr_engine* e) {
             }
         }
         if (!chunk.empty()) {
-            int rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
+            int rc = pen_chunk ? ensure_pen_buffers(e) : RR_OK;
+            if (rc == RR_OK)
+                rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
                                  topn.data(), e->o.prefix_cache ? pos0.data() : nullptr, copies, temps.data(), topps.data(),
-                                 seeds.data());
+                                 seeds.data(), chunk.data());
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
@@ -797,8 +915,14 @@ static void worker_main(rr_engine* e) {
             cudaMemcpyAsync(e->d_samp, e->h_samp, SAMP_BYTES * B, cudaMemcpyHostToDevice, s);
             e->st.h2d_bytes += SAMP_BYTES * B;
         }
+        if (pen_step && e->pen_dirty) {
+            const size_t nb = pen_bytes(e->Bm, PEN_MAX_BIAS);
+            e->pen_dirty = false;
+            cudaMemcpyAsync(e->d_pen, e->h_pen, nb, cudaMemcpyHostToDevice, s);
+            e->st.h2d_bytes += nb;
+        }
         cudaEventRecord(e->ev0, s);
-        int rc = run_decode_step(e, lp_step, samp_step);
+        int rc = run_decode_step(e, lp_step, samp_step, pen_step);
         cudaEventRecord(e->ev1, s);
         cudaMemcpyAsync(e->h_tok, e->d_tok, sizeof(int32_t) * e->Bm, cudaMemcpyDeviceToHost, s);
         if (lp_step) {
@@ -1034,6 +1158,8 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_topn) cudaFreeHost(e->h_topn);
     if (e->h_samp) cudaFreeHost(e->h_samp);
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
+    if (e->h_pen) cudaFreeHost(e->h_pen);
+    if (e->h_pen_pf) cudaFreeHost(e->h_pen_pf);
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) cudaStreamDestroy(e->stream);
@@ -1100,10 +1226,13 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
 
 namespace rr {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, int top_logprobs, float temperature, float top_p, uint64_t seed) {
+                         uint64_t* ticket, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                         const PenaltyParams* pen) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
     if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     if (!sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
+    if (pen && !penalty_params_ok(pen->freq, pen->pres, pen->n_bias, pen->ids, pen->vals, e->d.vocab))
+        return RR_INVALID_ARGUMENT;
     if ((top_logprobs >= 0 || temperature > 0.f) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
@@ -1117,6 +1246,10 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     r->tag = tag;
     r->top_lp = top_logprobs;
     if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
+    if (pen) {
+        r->fpen = pen->freq; r->ppen = pen->pres;
+        r->bias_id.assign(pen->ids, pen->ids + pen->n_bias); r->bias_val.assign(pen->vals, pen->vals + pen->n_bias);
+    }
     if (top_logprobs >= 0) {
         const size_t k = r->lp_width();
         r->lp.reserve(k * max_new_tokens); r->lp_id.reserve(k * max_new_tokens);
@@ -1167,6 +1300,16 @@ RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int
                                     int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
     return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs, temperature, top_p,
                                     seed);
+}
+
+RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                      int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                      float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                      const float* bias_vals, uint64_t* ticket) {
+    rr::PenaltyParams pen;
+    pen.freq = frequency_penalty; pen.pres = presence_penalty; pen.n_bias = n_bias; pen.ids = bias_ids; pen.vals = bias_vals;
+    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs, temperature, top_p,
+                                    seed, &pen);
 }
 
 // Caller holds e->mu.  The first min(n, max_tokens_out) tokens' pairs of a logprobs request into [max_tokens_out][K].

@@ -50,6 +50,10 @@ struct GwReq {
     std::vector<int32_t> lp_id;
     float temp = 0.f, top_p = 1.f;    // rr_gateway_submit_sampled: handed to every engine the request is admitted to
     uint64_t seed = 0;
+    float fpen = 0.f, ppen = 0.f;     // rr_gateway_submit_processed: handed to every engine the request is admitted to
+    std::vector<int32_t> bias_id;
+    std::vector<float> bias_val;
+    bool processed = false;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
@@ -283,8 +287,14 @@ static void gw_dispatch(rr_gateway* g) {
             }
             uint64_t tk = 0;
             int src = RR_INTERNAL;
+            rr::PenaltyParams pen;
+            if (r->processed) {
+                pen.freq = r->fpen; pen.pres = r->ppen; pen.n_bias = (int)r->bias_id.size();
+                pen.ids = r->bias_id.data(); pen.vals = r->bias_val.data();
+            }
             if (!cancelled && eng) src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk,
-                                                           r->top_lp, r->temp, r->top_p, r->seed);
+                                                           r->top_lp, r->temp, r->top_p, r->seed,
+                                                           r->processed ? &pen : nullptr);
             bool cancel_now = false;
             std::unique_lock<std::mutex> lk(g->mu);
             if (src == RR_OK) {
@@ -377,7 +387,7 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
 
 static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
                      int max_new_tokens, int declare_burst, int top_logprobs, uint64_t* tickets, float temperature = 0.f,
-                     float top_p = 1.f, uint64_t seed = 0) {
+                     float top_p = 1.f, uint64_t seed = 0, const rr::PenaltyParams* pen = nullptr) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
     if (top_logprobs < -1 || top_logprobs > rr::LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     if (!rr::sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
@@ -385,12 +395,20 @@ static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const 
         const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens);
         if (rc != RR_OK) return rc;
     }
+    // bias ids against the smallest vocabulary, as prompt ids: a fallback to any engine accepts them
+    if (pen && !rr::penalty_params_ok(pen->freq, pen->pres, pen->n_bias, pen->ids, pen->vals, g->min_vocab))
+        return RR_INVALID_ARGUMENT;
+    const bool processed = pen && (pen->freq != 0.f || pen->pres != 0.f || pen->n_bias > 0);
     std::vector<GwReq*> reqs((size_t)n);
     for (int i = 0; i < n; ++i) {
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
         r->group = group; r->max_new = max_new_tokens; r->top_lp = top_logprobs;
         if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
+        if (processed) {
+            r->processed = true; r->fpen = pen->freq; r->ppen = pen->pres;
+            r->bias_id.assign(pen->ids, pen->ids + pen->n_bias); r->bias_val.assign(pen->vals, pen->vals + pen->n_bias);
+        }
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -433,6 +451,16 @@ RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* pr
                                      int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
     const int32_t start[2] = {0, n_prompt};
     return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket, temperature, top_p, seed);
+}
+
+RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
+                                       int max_new_tokens, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                       float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                       const float* bias_vals, uint64_t* ticket) {
+    const int32_t start[2] = {0, n_prompt};
+    rr::PenaltyParams pen;
+    pen.freq = frequency_penalty; pen.pres = presence_penalty; pen.n_bias = n_bias; pen.ids = bias_ids; pen.vals = bias_vals;
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket, temperature, top_p, seed, &pen);
 }
 
 // caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][gw_lp_width(r)].

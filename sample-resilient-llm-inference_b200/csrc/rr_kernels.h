@@ -77,13 +77,24 @@ int num_sms();
 
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)
 typedef void (*EngineDoneHook)(void* ctx, uint64_t tag, uint64_t ticket, int status, int n_generated);
+// Penalties and logit bias of a request (rr_engine_submit_processed); host arrays of n_bias entries.
+struct PenaltyParams {
+    float freq = 0.f, pres = 0.f;
+    int n_bias = 0;
+    const int32_t* ids = nullptr;
+    const float* vals = nullptr;
+};
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, int top_logprobs = -1, float temperature = 0.f, float top_p = 1.f,
-                         uint64_t seed = 0);
+                         uint64_t seed = 0, const PenaltyParams* pen = nullptr);
 // OpenAI's ranges for a sampled request (rr_engine_submit_sampled): 0 <= temperature <= 2, 0 <= top_p <= 1 (NaN fails).
 inline bool sample_params_ok(float temperature, float top_p) {
     return temperature >= 0.f && temperature <= 2.f && top_p >= 0.f && top_p <= 1.f;
 }
+// OpenAI's ranges for a processed request (rr_engine_submit_processed): -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS,
+// bias ids unique and in [0, vocab), -100 <= bias values <= 100 (NaN fails).
+bool penalty_params_ok(float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                       const float* bias_vals, int vocab);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
@@ -201,6 +212,24 @@ constexpr int SAMPLE_LAUNCHES = 3;
 size_t sample_ws_bytes(int rows, int vocab);
 void launch_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
                    const uint64_t* seed, const int32_t* position, int32_t* out_tok, void* ws, cudaStream_t st);
+// Frequency / presence penalties and logit bias (rr_op_logit_penalties), in place over fp32 logits [rows][ld], one launch.
+// Per row r: freq[r], pres[r], n_bias[r] entries of bias_ids / bias_vals (row stride bias_ld, ids unique).  History: row r's
+// generated tokens at hist + r * hist_ld, hist_len[r] of them; or, in the engine's decode step (app_tok set), the kernel
+// first stores app_tok[r] at index app_pos[r] - gen0[r] and takes that index + 1 as the length.  A row with both penalties
+// 0 and no bias entries is not touched.  cnt_ws: [rows][vocab] int32, all zero on entry and left all zero.
+constexpr int PEN_MAX_BIAS = 300;
+struct PenaltyArgs {
+    const float *freq, *pres;
+    const int32_t *bias_ids, *n_bias;
+    const float* bias_vals;
+    int bias_ld;
+    int32_t* hist;                   // nullptr: no history (prefill: c = 0 for every token)
+    int hist_ld;
+    const int32_t* hist_len;
+    const int32_t *app_tok, *app_pos, *gen0;
+};
+void launch_logit_penalties(float* logits, int ld, int rows, int vocab, const PenaltyArgs& a, int32_t* cnt_ws,
+                            cudaStream_t st);
 
 // ---- attention (rr_attn_decode.cu, rr_attn_tc.cu) ---------------------------------------------------
 struct DecodeAttnArgs {

@@ -24,7 +24,7 @@ static inline void rr_trace_set_local(unsigned long long* p) { cudaMemcpyToSymbo
 static inline void rr_trace_set_detail_local(int on) { cudaMemcpyToSymbol(rr_trace_detail, &on, sizeof(on)); }
 enum TraceId { TR_GEMM_DEC = 1, TR_GEMM_PF = 2, TR_ATTN_DEC = 3, TR_ATTN_PF = 4, TR_NORM = 5, TR_ROPE = 6,
                TR_SILU = 7, TR_EMBED = 8, TR_ARGMAX = 9, TR_COMBINE = 10, TR_MISC = 11, TR_LOGPROBS = 20,
-               TR_SAMPLE = 21, TR_MLP_MARK = 50, TR_ATTN_MARK = 80, TR_GEMM_MARK = 100 };  // *_MARK + k: detail mark k (tools/trace_*.py)
+               TR_SAMPLE = 21, TR_PENALTY = 22, TR_MLP_MARK = 50, TR_ATTN_MARK = 80, TR_GEMM_MARK = 100 };  // *_MARK + k: detail mark k (tools/trace_*.py)
 __device__ __forceinline__ unsigned long long rr_gtimer() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

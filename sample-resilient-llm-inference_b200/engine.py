@@ -146,13 +146,30 @@ class Engine:
 
     # ---- serving interface ----------------------------------------------------------------------
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
-               temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None) -> int:
+               temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None,
+               frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
+               logit_bias: Optional[Dict[int, float]] = None) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
-        rr_engine_submit_sampled; None or 0 is greedy."""
+        rr_engine_submit_sampled; None or 0 is greedy.  frequency_penalty / presence_penalty in [-2, 2] and logit_bias
+        {token id: bias in [-100, 100]} (at most 300 entries): applied to the logits before every token is picked, the
+        penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing."""
         ids = _i32(prompt_ids)
         t = C.c_uint64()
+        if frequency_penalty or presence_penalty or logit_bias:
+            seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temperature else 0
+            k = -1 if top_logprobs is None else int(top_logprobs)
+            b_ids = _i32(list((logit_bias or {}).keys()))
+            b_vals = np.ascontiguousarray(np.asarray(list((logit_bias or {}).values()), dtype=np.float32))
+            _lib.check(_lib.lib.rr_engine_submit_processed(
+                self._h, _p(ids), len(ids), max_new_tokens, k, float(temperature or 0.0),
+                1.0 if top_p is None else float(top_p), seed, float(frequency_penalty or 0.0),
+                float(presence_penalty or 0.0), len(b_ids), _p(b_ids),
+                b_vals.ctypes.data_as(C.POINTER(C.c_float)), C.byref(t)), "rr_engine_submit_processed")
+            if k >= 0:
+                self._lp_k[t.value] = max(1, k) + (1 if temperature else 0)
+            return t.value
         if temperature:
             seed = secrets.randbits(64) if seed is None else int(seed) % 2**64
             k = -1 if top_logprobs is None else int(top_logprobs)

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import re
 import secrets
 import threading
 import time
@@ -191,6 +192,47 @@ def check_sampling(temperature: Any = None, top_p: Any = None, seed: Any = None)
     if temperature is None or temperature == 0:
         return None
     return float(temperature), 1.0 if top_p is None else float(top_p), None if seed is None else seed % 2**64
+
+
+MAX_PENALTY = 2.0            # OpenAI's range for `frequency_penalty` / `presence_penalty`: [-2, 2]
+MAX_LOGIT_BIAS = 100.0       # OpenAI's range for a `logit_bias` value: [-100, 100]
+MAX_LOGIT_BIAS_ENTRIES = 300  # this project's cap on the `logit_bias` map (PEN_MAX_BIAS of the engine)
+
+
+def check_penalties(frequency_penalty: Any = None, presence_penalty: Any = None, logit_bias: Any = None,
+                    vocab: Optional[int] = None) -> Optional[Tuple[float, float, List[int], List[float]]]:
+    """OpenAI's rules for the `frequency_penalty` / `presence_penalty` / `logit_bias` request fields -> None (nothing to
+    apply: both penalties absent or 0 and no bias entries) or (frequency_penalty, presence_penalty, bias ids, bias values).
+    `logit_bias` maps token ids, as decimal strings of integers, to numbers; ids must be distinct and, with `vocab`, below
+    it.  Raises BadRequestError (HTTP 400) for anything else."""
+    for name, v in (("frequency_penalty", frequency_penalty), ("presence_penalty", presence_penalty)):
+        if v is not None and (not _is_number(v) or not -MAX_PENALTY <= v <= MAX_PENALTY):
+            raise BadRequestError(f"`{name}` must be a number from {-MAX_PENALTY:g} to {MAX_PENALTY:g}")
+    ids: List[int] = []
+    vals: List[float] = []
+    if logit_bias is not None:
+        if not isinstance(logit_bias, dict):
+            raise BadRequestError("`logit_bias` must be an object mapping token ids to numbers")
+        if len(logit_bias) > MAX_LOGIT_BIAS_ENTRIES:
+            raise BadRequestError(f"`logit_bias` may hold at most {MAX_LOGIT_BIAS_ENTRIES} entries")
+        for k, v in logit_bias.items():
+            if isinstance(k, bool) or not (isinstance(k, int) or (isinstance(k, str) and re.fullmatch(r"[+-]?[0-9]+", k))):
+                raise BadRequestError(f"`logit_bias` key {k!r} is not an integer token id")
+            t = int(k)
+            if t < 0 or (vocab is not None and t >= vocab):
+                raise BadRequestError(f"`logit_bias` token id {t} is out of range"
+                                      + ("" if vocab is None else f" [0, {vocab})"))
+            if not _is_number(v) or not -MAX_LOGIT_BIAS <= v <= MAX_LOGIT_BIAS:
+                raise BadRequestError(f"`logit_bias` values must be numbers from {-MAX_LOGIT_BIAS:g} to {MAX_LOGIT_BIAS:g}")
+            ids.append(t)
+            vals.append(float(v))
+        if len(set(ids)) != len(ids):
+            raise BadRequestError("`logit_bias` names the same token id twice")
+    fp = 0.0 if frequency_penalty is None else float(frequency_penalty)
+    pp = 0.0 if presence_penalty is None else float(presence_penalty)
+    if fp == 0 and pp == 0 and not ids:
+        return None
+    return fp, pp, ids, vals
 
 
 def _token_entry(tok: int, logprob: float) -> dict:
@@ -399,12 +441,21 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None, samp=None) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None, samp=None,
+                   pen=None) -> int:
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        if samp is not None:
+        if pen is not None:
+            b_ids = np.ascontiguousarray(np.asarray(pen[2], dtype=np.int32))
+            b_vals = np.ascontiguousarray(np.asarray(pen[3], dtype=np.float32))
+            temp, top_p, seed = samp if samp is not None else (0.0, 1.0, 0)
+            rc = _lib.lib.rr_gateway_submit_processed(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                                      -1 if top is None else top, temp, top_p, seed, pen[0], pen[1],
+                                                      len(b_ids), b_ids.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                      b_vals.ctypes.data_as(C.POINTER(C.c_float)), C.byref(t))
+        elif samp is not None:
             rc = _lib.lib.rr_gateway_submit_sampled(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
                                                     -1 if top is None else top, samp[0], samp[1], samp[2], C.byref(t))
         elif top is None:
@@ -426,9 +477,9 @@ class Router:
         ids = np.zeros((max_new, w), dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None):
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None, pen=None):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp, pen)
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new, samp is not None)
@@ -445,8 +496,8 @@ class Router:
             content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), top), "refusal": None}
         return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
 
-    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None):
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp)
+    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None, pen=None):
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp, pen)
         deadline = None if not timeout else time.perf_counter() + timeout
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
@@ -598,16 +649,26 @@ class Router:
             samp = (samp[0], samp[1], secrets.randbits(64))
         return samp
 
+    def _penalties(self, frequency_penalty, presence_penalty, logit_bias):
+        """Validated penalties and logit bias (None = nothing to apply); bias ids must be valid on every replica the
+        request may fall back to."""
+        return check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab())
+
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
                    logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
-                   top_p: Optional[float] = None, seed: Optional[int] = None, **_ignored) -> ModelResponse:
+                   top_p: Optional[float] = None, seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
+                   presence_penalty: Optional[float] = None, logit_bias: Optional[Dict[str, float]] = None,
+                   **_ignored) -> ModelResponse:
         """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
         (0..20) most likely alternatives, as the OpenAI API returns them.  temperature > 0: every token is drawn from
         the top_p nucleus of softmax(logits / temperature) with the request's seed (rr_op_sample); absent or 0 is
-        greedy.  Stub backends validate these and keep their fixed reply."""
+        greedy.  frequency_penalty / presence_penalty / logit_bias: applied to the logits before every token is picked
+        (rr_op_logit_penalties; the penalties count the tokens generated so far).  Stub backends validate these and keep
+        their fixed reply."""
         top = self._logprobs_top(logprobs, top_logprobs)
         samp = self._sampling(temperature, top_p, seed)
+        pen = self._penalties(frequency_penalty, presence_penalty, logit_bias)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -617,7 +678,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp)
+            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp, pen)
         # ---- host loop (StubBackend): same admission events, one K1 launch per event
         t_start = time.perf_counter()
         chain_start = 0
@@ -655,13 +716,17 @@ class Router:
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                           max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
                           logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
-                          top_p: Optional[float] = None, seed: Optional[int] = None):
+                          top_p: Optional[float] = None, seed: Optional[int] = None,
+                          frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
+                          logit_bias: Optional[Dict[str, float]] = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
         (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
-        fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling as in completion()."""
+        fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties and logit
+        bias as in completion()."""
         top = self._logprobs_top(logprobs, top_logprobs)
         samp = self._sampling(temperature, top_p, seed)
+        pen = self._penalties(frequency_penalty, presence_penalty, logit_bias)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -670,7 +735,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp)
+            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp, pen)
             return
         deadline = None if not timeout else time.perf_counter() + timeout
         chain_start = 0
