@@ -88,21 +88,10 @@ struct Request {
     uint64_t tag = 0;          // opaque caller value handed to the done hook (the gateway's request id)
     bool cancel = false;       // rr_engine_cancel: the worker drops the row at the next step
     bool detached = false;     // nobody will call rr_engine_wait: the worker frees the request when it finishes
-    int top_lp = -1;           // rr_engine_submit_logprobs: -1 off, else max(1, top_lp) (logprob, id) pairs per token
-    std::vector<float> lp;     // [out.size()][max(1, top_lp)]
+    GenParams gen;
+    std::vector<float> lp;     // [out.size()][gen.lp_width()]
     std::vector<int32_t> lp_id;
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
-    float temp = 0.f, top_p = 1.f;   // rr_engine_submit_sampled: temp > 0 draws every token with rr_op_sample
-    uint64_t seed = 0;
-    bool sampled() const { return temp > 0.f; }
-    // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
-    int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
-    // rr_engine_submit_processed: frequency / presence penalties over the generated tokens and a logit bias, applied to
-    // the logits before the token is picked (rr_op_logit_penalties)
-    float fpen = 0.f, ppen = 0.f;
-    std::vector<int32_t> bias_id;
-    std::vector<float> bias_val;
-    bool processed() const { return fpen != 0.f || ppen != 0.f || !bias_id.empty(); }
 };
 
 // Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
@@ -126,27 +115,38 @@ static PenaltyArgs pen_args(const char* blk, int n, int bias_ld) {
     a.hist = nullptr; a.hist_ld = 0; a.hist_len = nullptr; a.app_tok = nullptr; a.app_pos = nullptr;
     return a;
 }
-// Writes row i of a block at stride n (r == nullptr: an unprocessed row, all zero).
-static void pen_fill_row(char* blk, int n, int bias_ld, int i, const Request* r, float freq, float pres, int gen0) {
-    const int nb = r ? (int)r->bias_id.size() : 0;
+// Writes row i of a block at stride n: p's bias, the given penalties and gen0.
+static void pen_fill_row(char* blk, int n, int bias_ld, int i, const GenParams& p, float freq, float pres, int gen0) {
+    const int nb = (int)p.bias_id.size();
     ((float*)blk)[i] = freq; ((float*)(blk + 4 * (size_t)n))[i] = pres;
     ((int32_t*)(blk + 8 * (size_t)n))[i] = gen0; ((int32_t*)(blk + 12 * (size_t)n))[i] = nb;
     if (nb) {
-        memcpy(blk + 16 * (size_t)n + 4 * ((size_t)i * bias_ld), r->bias_id.data(), 4 * (size_t)nb);
-        memcpy(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld + 4 * ((size_t)i * bias_ld), r->bias_val.data(), 4 * (size_t)nb);
+        memcpy(blk + 16 * (size_t)n + 4 * ((size_t)i * bias_ld), p.bias_id.data(), 4 * (size_t)nb);
+        memcpy(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld + 4 * ((size_t)i * bias_ld), p.bias_val.data(), 4 * (size_t)nb);
     }
 }
 
-bool penalty_params_ok(float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                       const float* bias_vals, int vocab) {
+int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_, uint64_t seed_, float frequency_penalty,
+                   float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals) {
+    if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
+    if (!(temperature >= 0.f && temperature <= 2.f && top_p_ >= 0.f && top_p_ <= 1.f)) return RR_INVALID_ARGUMENT;
     if (!(frequency_penalty >= -2.f && frequency_penalty <= 2.f && presence_penalty >= -2.f && presence_penalty <= 2.f))
-        return false;
-    if (n_bias < 0 || n_bias > PEN_MAX_BIAS || (n_bias > 0 && (!bias_ids || !bias_vals))) return false;
-    std::vector<int32_t> ids(bias_ids, bias_ids + n_bias);
+        return RR_INVALID_ARGUMENT;
+    if (n_bias < 0 || n_bias > PEN_MAX_BIAS || (n_bias > 0 && (!bias_ids || !bias_vals))) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_bias; ++i)
-        if (ids[i] < 0 || ids[i] >= vocab || !(bias_vals[i] >= -100.f && bias_vals[i] <= 100.f)) return false;
+        if (bias_ids[i] < 0 || bias_ids[i] >= vocab || !(bias_vals[i] >= -100.f && bias_vals[i] <= 100.f))
+            return RR_INVALID_ARGUMENT;
+    std::vector<int32_t> ids(bias_ids, bias_ids + n_bias);
     std::sort(ids.begin(), ids.end());
-    return std::adjacent_find(ids.begin(), ids.end()) == ids.end();
+    if (std::adjacent_find(ids.begin(), ids.end()) != ids.end()) return RR_INVALID_ARGUMENT;
+    *this = GenParams();
+    top_lp = top_logprobs;
+    if (temperature > 0.f) { temp = temperature; top_p = top_p_; seed = seed_; }
+    if (frequency_penalty != 0.f || presence_penalty != 0.f || n_bias > 0) {
+        fpen = frequency_penalty; ppen = presence_penalty;
+        bias_id.assign(bias_ids, bias_ids + n_bias); bias_val.assign(bias_vals, bias_vals + n_bias);
+    }
+    return RR_OK;
 }
 
 }  // namespace rr
@@ -202,6 +202,9 @@ struct rr_engine {
     // processed rows replays the plain graph.
     cudaGraphExec_t graph[8] = {};
     bool warmed = false;
+    // Per-row parameter blocks of the decode rows (d_topn, d_samp, d_pen), each with a pinned host mirror (h_topn, h_samp,
+    // h_pen) that set_row_params keeps in step with row_req, and a dirty flag; upload_row_params copies a dirty block before
+    // a step that reads it.  A prefill chunk packs its sequences' parameters into its own blocks (*_pf) and staging.
     int32_t *d_topn = nullptr, *d_topn_pf = nullptr;   // per decode row / per prefill sequence: top_lp, -1 = off
     void* lp_ws = nullptr;
     float* d_lp = nullptr;                             // [Bm][LP_MAX_TOP]
@@ -211,12 +214,12 @@ struct rr_engine {
     char *d_samp = nullptr, *d_samp_pf = nullptr;
     void* sample_ws = nullptr;
     float* d_tok_lp = nullptr;                         // [Bm] the sampled token's logprob (sampled logprobs rows)
-    // penalties / logit bias, allocated on the first processed request (ensure_pen_buffers): the decode rows' parameter
-    // block (pen_args layout, stride Bm) and its pinned host mirror, the prefill chunk's block and its staging, the
-    // generated-token history [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
+    // penalties / logit bias, allocated on the first processed request (ensure_pen_buffers): the decode rows' block
+    // (pen_args layout, stride Bm) and its mirror, the prefill chunk's block and its staging, the generated-token history
+    // [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
     char *d_pen = nullptr, *d_pen_pf = nullptr, *h_pen = nullptr, *h_pen_pf = nullptr;
     int32_t *d_hist = nullptr, *pen_ws = nullptr;
-    bool pen_dirty = false;
+    bool topn_dirty = false, samp_dirty = false, pen_dirty = false;
 
     // prefill working set
     int Tmax;
@@ -233,8 +236,8 @@ struct rr_engine {
     float* h_logits = nullptr;
     float* h_lp = nullptr;        // [Bm][LP_MAX_TOP] logprobs read back on steps that computed them
     int32_t* h_lp_id = nullptr;
-    int32_t* h_topn = nullptr;    // [Bm] staging of d_topn / d_topn_pf
-    char* h_samp = nullptr;       // [Bm * SAMP_PF_BYTES] staging of d_samp / d_samp_pf
+    int32_t *h_topn = nullptr, *h_topn_pf = nullptr;   // [Bm] mirror of d_topn / staging of d_topn_pf
+    char *h_samp = nullptr, *h_samp_pf = nullptr;      // [Bm * SAMP_BYTES] mirror of d_samp / [Bm * SAMP_PF_BYTES] staging
     float* h_tok_lp = nullptr;    // [Bm]
 
     // serving state
@@ -246,11 +249,6 @@ struct rr_engine {
     std::vector<Request*> row_req;       // [Bm]
     std::vector<int32_t> h_slot_mirror;  // host mirror of d_slot
     bool slots_dirty = false;
-    std::vector<int32_t> h_topn_mirror;  // host mirror of d_topn (uploaded before a step that computes logprobs)
-    bool topn_dirty = false;
-    std::vector<uint64_t> h_seed_mirror; // host mirrors of d_samp (uploaded before a step that samples)
-    std::vector<float> h_temp_mirror, h_topp_mirror;
-    bool samp_dirty = false;
     // prefix caching (o.prefix_cache), under mu: retained[b] = the prompt tokens whose KV the last successful prefill into
     // slot b wrote (computed or copied; never a position decode wrote, since decode rounds differently), kept after the
     // request ends; retained_used[b] = LRU stamp.  index_epoch counts the low-level calls that cleared every list.
@@ -501,19 +499,16 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 }
 
 // ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
-// activates the rows. Caller holds gpu_mu.  topn_host[n_seqs] (optional): sequences with topn_host[i] >= 0 also get their
-// first token's logprobs in e->h_lp / e->h_lp_id row i.
+// activates the rows. Caller holds gpu_mu.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
-// Sampling: temp_host / topp_host / seed_host[n_seqs] (optional): sequences with temp_host[i] > 0 draw their first token
-// with rr_op_sample at position pos0[i] + their length (the prompt length); with logprobs its own logprob lands in h_tok_lp.
-// Logit bias: reqs[n_seqs] (optional): the logits of sequences whose request has a logit bias get it before the argmax and
-// the sampler (penalties count generated tokens only, so the first token has none); needs ensure_pen_buffers.
+// gen[n_seqs] (optional): each sequence's request parameters.  A logit bias is added to the logits before the argmax and
+// the sampler (penalties count generated tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled
+// sequence draws its first token with rr_op_sample at position pos0[i] + its length (the prompt length).  A logprobs
+// sequence also gets its first token's logprobs in e->h_lp / e->h_lp_id row i, and if sampled its own logprob in h_tok_lp.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
-                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* topn_host = nullptr,
-                       const int32_t* pos0 = nullptr, const KvCopyList* copies = nullptr,
-                       const float* temp_host = nullptr, const float* topp_host = nullptr,
-                       const uint64_t* seed_host = nullptr, Request* const* reqs = nullptr) {
+                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
+                       const KvCopyList* copies = nullptr, const GenParams* const* gen = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
@@ -601,11 +596,15 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
     int max_bias = 0;
-    for (int i = 0; reqs && i < n_seqs; ++i)
-        if ((int)reqs[i]->bias_id.size() > max_bias) max_bias = (int)reqs[i]->bias_id.size();
+    bool samp = false, lp = false;
+    for (int i = 0; gen && i < n_seqs; ++i) {
+        if ((int)gen[i]->bias_id.size() > max_bias) max_bias = (int)gen[i]->bias_id.size();
+        samp = samp || gen[i]->sampled();
+        lp = lp || gen[i]->logprobs();
+    }
     if (max_bias > 0) {
         if (!e->d_pen) return RR_INTERNAL;
-        for (int i = 0; i < n_seqs; ++i) pen_fill_row(e->h_pen_pf, n_seqs, max_bias, i, reqs[i], 0.f, 0.f, 0);
+        for (int i = 0; i < n_seqs; ++i) pen_fill_row(e->h_pen_pf, n_seqs, max_bias, i, *gen[i], 0.f, 0.f, 0);
         const size_t nb = pen_bytes(n_seqs, max_bias);
         CK(cudaMemcpyAsync(e->d_pen_pf, e->h_pen_pf, nb, cudaMemcpyHostToDevice, s));
         e->st.h2d_bytes += nb;
@@ -613,15 +612,13 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ++nl;
     }
     launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
-    bool samp = false;
-    for (int i = 0; temp_host && i < n_seqs; ++i) samp = samp || temp_host[i] > 0.f;
     if (samp) {
-        char* h = e->h_samp;
+        char* h = e->h_samp_pf;
         const size_t n = (size_t)n_seqs;
         for (int i = 0; i < n_seqs; ++i) {
-            ((uint64_t*)h)[i] = seed_host[i];
-            ((float*)(h + 8 * n))[i] = temp_host[i];
-            ((float*)(h + 12 * n))[i] = topp_host[i];
+            ((uint64_t*)h)[i] = gen[i]->seed;
+            ((float*)(h + 8 * n))[i] = gen[i]->temp;
+            ((float*)(h + 12 * n))[i] = gen[i]->top_p;
             ((int32_t*)(h + 16 * n))[i] = (pos0 ? pos0[i] : 0) + seq_start[i + 1] - seq_start[i];
         }
         CK(cudaMemcpyAsync(e->d_samp_pf, h, SAMP_PF_BYTES * n, cudaMemcpyHostToDevice, s));
@@ -632,11 +629,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
                (const int32_t*)e->p_first, (const int32_t*)p_pos, (const int32_t*)p_last, n_seqs, e->d_tok, e->d_pos,
                e->d_slot); ++nl;
-    bool lp = false;
-    for (int i = 0; topn_host && i < n_seqs; ++i) lp = lp || topn_host[i] >= 0;
     if (lp) {
-        memcpy(e->h_topn, topn_host, sizeof(int32_t) * n_seqs);
-        CK(cudaMemcpyAsync(e->d_topn_pf, e->h_topn, sizeof(int32_t) * n_seqs, cudaMemcpyHostToDevice, s));
+        for (int i = 0; i < n_seqs; ++i) e->h_topn_pf[i] = gen[i]->top_lp;
+        CK(cudaMemcpyAsync(e->d_topn_pf, e->h_topn_pf, sizeof(int32_t) * n_seqs, cudaMemcpyHostToDevice, s));
         e->st.h2d_bytes += sizeof(int32_t) * n_seqs;
         enqueue_logprobs(e, e->d_topn_pf, n_seqs, s, samp ? e->p_first : nullptr); nl += LP_LAUNCHES;
         const size_t n = (size_t)n_seqs * LP_MAX_TOP;
@@ -675,36 +670,47 @@ struct DoneNote { uint64_t tag, ticket; int status, n_gen; };
 // Caller holds e->mu.  Appends row `row` of h_lp / h_lp_id to the request's pairs, and for a sampled request the pair of
 // the token it just generated (h_tok_lp).
 static void record_logprobs(rr_engine* e, Request* r, int row) {
-    const int k = r->top_lp > 1 ? r->top_lp : 1;
+    const int k = r->gen.top_lp > 1 ? r->gen.top_lp : 1;
     const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
     const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
     r->lp.insert(r->lp.end(), v, v + k);
     r->lp_id.insert(r->lp_id.end(), id, id + k);
-    if (r->sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
+    if (r->gen.sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
 }
 
-// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): keep the host mirrors of d_topn, d_samp and d_pen
-// in step.
-static void set_row_topn(rr_engine* e, int b, const Request* r) {
-    const int t = r ? r->top_lp : -1;
-    if (e->h_topn_mirror[b] != t) { e->h_topn_mirror[b] = t; e->topn_dirty = true; }
-    const float temp = r ? r->temp : 0.f, top_p = r ? r->top_p : 1.f;
-    const uint64_t seed = r ? r->seed : 0;
-    if (e->h_temp_mirror[b] != temp || e->h_topp_mirror[b] != top_p || e->h_seed_mirror[b] != seed) {
-        e->h_temp_mirror[b] = temp; e->h_topp_mirror[b] = top_p; e->h_seed_mirror[b] = seed;
-        e->samp_dirty = true;
+// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): write row b of each parameter block's mirror from
+// r's parameters or the defaults.  A block is marked dirty only when the row uses it before or after: the other rows of a
+// mirror hold the defaults, as a request that does not use the block does (GenParams::set), so they never need a copy.
+static void set_row_params(rr_engine* e, int b, const Request* r) {
+    static const GenParams plain;
+    const GenParams& p = r ? r->gen : plain;
+    const size_t B = (size_t)e->Bm;
+    if (e->h_topn[b] >= 0 || p.logprobs()) e->topn_dirty = true;
+    e->h_topn[b] = p.top_lp;
+    float* temp = (float*)(e->h_samp + 8 * B);
+    if (temp[b] > 0.f || p.sampled()) e->samp_dirty = true;
+    ((uint64_t*)e->h_samp)[b] = p.seed; temp[b] = p.temp; ((float*)(e->h_samp + 12 * B))[b] = p.top_p;
+    if (!e->h_pen) return;     // allocated with d_pen on the first processed request: every row is unprocessed until then
+    const bool was = ((const float*)e->h_pen)[b] != 0.f || ((const float*)(e->h_pen + 4 * B))[b] != 0.f ||
+                     ((const int32_t*)(e->h_pen + 12 * B))[b] != 0;
+    if (was || p.processed()) {
+        pen_fill_row(e->h_pen, (int)B, PEN_MAX_BIAS, b, p, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
+        e->pen_dirty = true;
     }
-    // h_pen is the host mirror of d_pen (absent until the first processed request; every row is unprocessed until then)
-    if (!e->h_pen) return;
-    const int B = e->Bm;
-    const bool was = ((const float*)e->h_pen)[b] != 0.f || ((const float*)(e->h_pen + 4 * (size_t)B))[b] != 0.f ||
-                     ((const int32_t*)(e->h_pen + 12 * (size_t)B))[b] != 0;
-    if (r && r->processed()) {
-        pen_fill_row(e->h_pen, B, PEN_MAX_BIAS, b, r, r->fpen, r->ppen, (int)r->prompt.size());
-        e->pen_dirty = true;
-    } else if (was) {
-        pen_fill_row(e->h_pen, B, PEN_MAX_BIAS, b, nullptr, 0.f, 0.f, 0);
-        e->pen_dirty = true;
+}
+
+// Before a decode step: copy each parameter block the step reads (step_mode bits) whose mirror changed.
+static void upload_row_params(rr_engine* e, int mode) {
+    const size_t B = (size_t)e->Bm;
+    struct { bool* dirty; void* d; const void* h; size_t bytes; } blk[3] = {
+        {&e->topn_dirty, e->d_topn, e->h_topn, sizeof(int32_t) * B},
+        {&e->samp_dirty, e->d_samp, e->h_samp, SAMP_BYTES * B},
+        {&e->pen_dirty, e->d_pen, e->h_pen, pen_bytes(e->Bm, PEN_MAX_BIAS)}};
+    for (int i = 0; i < 3; ++i) {
+        if (!(mode >> i & 1) || !*blk[i].dirty) continue;
+        *blk[i].dirty = false;
+        cudaMemcpyAsync(blk[i].d, blk[i].h, blk[i].bytes, cudaMemcpyHostToDevice, e->stream);
+        e->st.h2d_bytes += blk[i].bytes;
     }
 }
 
@@ -768,17 +774,15 @@ static void forget_prefixes(rr_engine* e) {
 
 static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
-    std::vector<int32_t> ids, seq_start, slots, topn, pos0;
-    std::vector<float> temps, topps;
-    std::vector<uint64_t> seeds;
+    std::vector<int32_t> ids, seq_start, slots, pos0;
     std::vector<Request*> chunk;
+    std::vector<const GenParams*> gen;
     std::vector<DoneNote> notes;
     KvCopyList* copies = new KvCopyList();
     while (!e->stop.load()) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
-        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); topn.clear(); pos0.clear();
-        temps.clear(); topps.clear(); seeds.clear();
+        chunk.clear(); gen.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
         copies->count = 0;
         int active = 0;
         bool lp_step = false, samp_step = false, pen_step = false, pen_chunk = false;
@@ -789,14 +793,14 @@ static void worker_main(rr_engine* e) {
                 Request* r = e->row_req[b];
                 if (r && r->cancel) {                      // rr_engine_cancel: free the row, keep what was generated
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_topn(e, b, nullptr);
+                    set_row_params(e, b, nullptr);
                     finish_request(e, r, RR_CANCELLED, &notes);
                     continue;
                 }
                 active += r != nullptr;
-                lp_step = lp_step || (r && r->top_lp >= 0);
-                samp_step = samp_step || (r && r->sampled());
-                pen_step = pen_step || (r && r->processed());
+                lp_step = lp_step || (r && r->gen.logprobs());
+                samp_step = samp_step || (r && r->gen.sampled());
+                pen_step = pen_step || (r && r->gen.processed());
             }
             if (e->waiting.empty() && active == 0) {
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
@@ -828,10 +832,9 @@ static void worker_main(rr_engine* e) {
                     pos0.push_back(m);
                 }
                 chunk.push_back(r);
+                gen.push_back(&r->gen);
                 slots.push_back(b);
-                topn.push_back(r->top_lp);
-                temps.push_back(r->temp); topps.push_back(r->top_p); seeds.push_back(r->seed);
-                pen_chunk = pen_chunk || r->processed();
+                pen_chunk = pen_chunk || r->gen.processed();
                 ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
@@ -859,8 +862,7 @@ static void worker_main(rr_engine* e) {
             int rc = pen_chunk ? ensure_pen_buffers(e) : RR_OK;
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 topn.data(), e->o.prefix_cache ? pos0.data() : nullptr, copies, temps.data(), topps.data(),
-                                 seeds.data(), chunk.data());
+                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, gen.data());
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
@@ -878,14 +880,14 @@ static void worker_main(rr_engine* e) {
                 }
                 r->t_first = t;
                 r->out.push_back(e->h_tok[i]);
-                if (r->top_lp >= 0) record_logprobs(e, r, (int)i);
+                if (r->gen.logprobs()) record_logprobs(e, r, (int)i);
                 e->st.generated_tokens += 1;
                 if ((int)r->out.size() >= r->max_new) {
                     e->row_req[r->slot] = nullptr;
                     e->h_slot_mirror[r->slot] = -1; e->slots_dirty = true;
                     finish_request(e, r, RR_OK, &notes);
                 } else {
-                    set_row_topn(e, r->slot, r);
+                    set_row_params(e, r->slot, r);
                 }
             }
             e->cv_done.notify_all();
@@ -900,27 +902,7 @@ static void worker_main(rr_engine* e) {
             e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
             e->slots_dirty = false;
         }
-        if (lp_step && e->topn_dirty) {           // (the mirror is only touched by this thread)
-            memcpy(e->h_topn, e->h_topn_mirror.data(), sizeof(int32_t) * e->Bm);
-            e->topn_dirty = false;
-            cudaMemcpyAsync(e->d_topn, e->h_topn, sizeof(int32_t) * e->Bm, cudaMemcpyHostToDevice, s);
-            e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
-        }
-        if (samp_step && e->samp_dirty) {
-            const size_t B = (size_t)e->Bm;
-            memcpy(e->h_samp, e->h_seed_mirror.data(), sizeof(uint64_t) * B);
-            memcpy(e->h_samp + 8 * B, e->h_temp_mirror.data(), sizeof(float) * B);
-            memcpy(e->h_samp + 12 * B, e->h_topp_mirror.data(), sizeof(float) * B);
-            e->samp_dirty = false;
-            cudaMemcpyAsync(e->d_samp, e->h_samp, SAMP_BYTES * B, cudaMemcpyHostToDevice, s);
-            e->st.h2d_bytes += SAMP_BYTES * B;
-        }
-        if (pen_step && e->pen_dirty) {
-            const size_t nb = pen_bytes(e->Bm, PEN_MAX_BIAS);
-            e->pen_dirty = false;
-            cudaMemcpyAsync(e->d_pen, e->h_pen, nb, cudaMemcpyHostToDevice, s);
-            e->st.h2d_bytes += nb;
-        }
+        upload_row_params(e, step_mode(lp_step, samp_step, pen_step));
         cudaEventRecord(e->ev0, s);
         int rc = run_decode_step(e, lp_step, samp_step, pen_step);
         cudaEventRecord(e->ev1, s);
@@ -949,16 +931,16 @@ static void worker_main(rr_engine* e) {
                 if (!r) continue;
                 if (rc != RR_OK) {
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_topn(e, b, nullptr);
+                    set_row_params(e, b, nullptr);
                     finish_request(e, r, RR_INTERNAL, &notes);
                     continue;
                 }
                 r->out.push_back(e->h_tok[b]);
-                if (r->top_lp >= 0) record_logprobs(e, r, b);
+                if (r->gen.logprobs()) record_logprobs(e, r, b);
                 e->st.generated_tokens += 1;
                 if ((int)r->out.size() >= r->max_new) {
                     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_topn(e, b, nullptr);
+                    set_row_params(e, b, nullptr);
                     finish_request(e, r, RR_OK, &notes);
                 }
             }
@@ -1063,12 +1045,14 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->d_lp, (size_t)B * LP_MAX_TOP)); TRY(dalloc(e, &e->d_lp_id, (size_t)B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_lp, sizeof(float) * B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_lp_id, sizeof(int32_t) * B * LP_MAX_TOP));
-    TRYC(cudaMallocHost(&e->h_topn, sizeof(int32_t) * B));
+    TRYC(cudaMallocHost(&e->h_topn, sizeof(int32_t) * B)); TRYC(cudaMallocHost(&e->h_topn_pf, sizeof(int32_t) * B));
+    memset(e->h_topn, 0xff, sizeof(int32_t) * B);                 // the mirrors start as their device blocks
     TRY(dalloc(e, &e->d_samp, (size_t)SAMP_BYTES * B));           // zero: every row greedy
     TRY(dalloc(e, &e->d_samp_pf, (size_t)SAMP_PF_BYTES * B));
     TRY(dalloc(e, (char**)&e->sample_ws, sample_ws_bytes(B, d.vocab), false));
     TRY(dalloc(e, &e->d_tok_lp, B));
-    TRYC(cudaMallocHost(&e->h_samp, (size_t)SAMP_PF_BYTES * B));
+    TRYC(cudaMallocHost(&e->h_samp, (size_t)SAMP_BYTES * B)); TRYC(cudaMallocHost(&e->h_samp_pf, (size_t)SAMP_PF_BYTES * B));
+    memset(e->h_samp, 0, (size_t)SAMP_BYTES * B);
     TRYC(cudaMallocHost(&e->h_tok_lp, sizeof(float) * B));
 
     e->pl_qkv.resize(L); e->pl_o.resize(L); e->pl_gu.resize(L); e->pl_down.resize(L);
@@ -1130,9 +1114,6 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRYC(cudaDeviceSynchronize());
     e->row_req.assign(B, nullptr);
     e->h_slot_mirror.assign(B, -1);
-    e->h_topn_mirror.assign(B, -1);
-    e->h_seed_mirror.assign(B, 0); e->h_temp_mirror.assign(B, 0.f); e->h_topp_mirror.assign(B, 1.f);
-    e->samp_dirty = true;
     if (e->o.prefix_cache) { e->retained.assign(B, {}); e->retained_used.assign(B, 0); }
     e->worker = std::thread(worker_main, e);
     *out = e;
@@ -1156,7 +1137,9 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_lp) cudaFreeHost(e->h_lp);
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
     if (e->h_topn) cudaFreeHost(e->h_topn);
+    if (e->h_topn_pf) cudaFreeHost(e->h_topn_pf);
     if (e->h_samp) cudaFreeHost(e->h_samp);
+    if (e->h_samp_pf) cudaFreeHost(e->h_samp_pf);
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
     if (e->h_pen) cudaFreeHost(e->h_pen);
     if (e->h_pen_pf) cudaFreeHost(e->h_pen_pf);
@@ -1226,14 +1209,10 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
 
 namespace rr {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                         const PenaltyParams* pen) {
+                         uint64_t* ticket, const GenParams& p) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
-    if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
-    if (!sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
-    if (pen && !penalty_params_ok(pen->freq, pen->pres, pen->n_bias, pen->ids, pen->vals, e->d.vocab))
-        return RR_INVALID_ARGUMENT;
-    if ((top_logprobs >= 0 || temperature > 0.f) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
+    // the vocabularies the logprobs / sampling kernels handle
+    if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
@@ -1244,14 +1223,9 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     r->max_new = max_new_tokens;
     r->out.reserve(max_new_tokens);
     r->tag = tag;
-    r->top_lp = top_logprobs;
-    if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
-    if (pen) {
-        r->fpen = pen->freq; r->ppen = pen->pres;
-        r->bias_id.assign(pen->ids, pen->ids + pen->n_bias); r->bias_val.assign(pen->vals, pen->vals + pen->n_bias);
-    }
-    if (top_logprobs >= 0) {
-        const size_t k = r->lp_width();
+    r->gen = p;
+    if (p.logprobs()) {
+        const size_t k = p.lp_width();
         r->lp.reserve(k * max_new_tokens); r->lp_id.reserve(k * max_new_tokens);
     }
     std::vector<DoneNote> notes;
@@ -1286,37 +1260,40 @@ int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab
 }
 }  // namespace rr
 
-RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                            uint64_t* ticket) {
-    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket);
-}
-
-RR_API int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                     int top_logprobs, uint64_t* ticket) {
-    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs);
-}
-
-RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                    int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
-    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs, temperature, top_p,
-                                    seed);
-}
-
 RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                                       int top_logprobs, float temperature, float top_p, uint64_t seed,
                                       float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
                                       const float* bias_vals, uint64_t* ticket) {
-    rr::PenaltyParams pen;
-    pen.freq = frequency_penalty; pen.pres = presence_penalty; pen.n_bias = n_bias; pen.ids = bias_ids; pen.vals = bias_vals;
-    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, top_logprobs, temperature, top_p,
-                                    seed, &pen);
+    if (!e) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals);
+    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p);
+}
+
+RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                            uint64_t* ticket) {
+    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, -1, 0.f, 1.f, 0, 0.f, 0.f, 0, nullptr,
+                                      nullptr, ticket);
+}
+
+RR_API int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                     int top_logprobs, uint64_t* ticket) {
+    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, top_logprobs, 0.f, 1.f, 0, 0.f, 0.f, 0,
+                                      nullptr, nullptr, ticket);
+}
+
+RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                    int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
+    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, top_logprobs, temperature, top_p, seed, 0.f,
+                                      0.f, 0, nullptr, nullptr, ticket);
 }
 
 // Caller holds e->mu.  The first min(n, max_tokens_out) tokens' pairs of a logprobs request into [max_tokens_out][K].
 static void copy_logprobs(const Request* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (r->top_lp < 0 || t <= 0) return;
-    const size_t m = (size_t)t * r->lp_width();
+    if (!r->gen.logprobs() || t <= 0) return;
+    const size_t m = (size_t)t * r->gen.lp_width();
     if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
     if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
 }

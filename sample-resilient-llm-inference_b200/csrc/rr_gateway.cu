@@ -45,15 +45,9 @@ struct GwReq {
     rr_engine* eng = nullptr;
     uint64_t eng_ticket = 0;
     std::vector<int32_t> tokens;
-    int top_lp = -1;                  // rr_gateway_submit_logprobs: handed to every engine the request is admitted to
-    std::vector<float> lp;            // [tokens.size()][max(1, top_lp)]
+    rr::GenParams gen;                // handed to every engine the request is admitted to
+    std::vector<float> lp;            // [tokens.size()][gen.lp_width()]
     std::vector<int32_t> lp_id;
-    float temp = 0.f, top_p = 1.f;    // rr_gateway_submit_sampled: handed to every engine the request is admitted to
-    uint64_t seed = 0;
-    float fpen = 0.f, ppen = 0.f;     // rr_gateway_submit_processed: handed to every engine the request is admitted to
-    std::vector<int32_t> bias_id;
-    std::vector<float> bias_val;
-    bool processed = false;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
@@ -66,9 +60,6 @@ struct Pending {
     int tokens;        // DONE: completion tokens; BURST: burst size
     int aux = 0;       // rr_event.chain_start of a DONE (latency, us) / FAIL (1 = timeout): latency-based routers only
 };
-
-// pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair (rr_engine_submit_sampled)
-static size_t gw_lp_width(const GwReq* r) { return (size_t)(r->top_lp > 1 ? r->top_lp : 1) + (r->temp > 0.f ? 1 : 0); }
 
 }  // namespace
 
@@ -128,7 +119,8 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     if (tag == 0) return;                                    // not submitted through this gateway
     GwReq* r = nullptr;
     rr_engine* eng = nullptr;
-    int max_new = 0, top_lp = -1;
+    int max_new = 0;
+    bool logprobs = false;
     size_t k = 1;
     {
         std::lock_guard<std::mutex> lk(g->mu);
@@ -137,19 +129,19 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         r = it->second;
         eng = r->eng;
         max_new = r->max_new;
-        top_lp = r->top_lp;
-        k = gw_lp_width(r);
+        logprobs = r->gen.logprobs();
+        k = (size_t)r->gen.lp_width();
     }
     // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
     memset(&comp, 0, sizeof(comp));
     std::vector<int32_t> toks((size_t)(max_new > 0 ? max_new : 1));
-    std::vector<float> lps(top_lp >= 0 ? toks.size() * k : 0);
+    std::vector<float> lps(logprobs ? toks.size() * k : 0);
     std::vector<int32_t> lp_ids(lps.size());
     int wrc = RR_INVALID_ARGUMENT;
     if (eng && status != RR_CANCELLED)
-        wrc = rr_engine_wait_logprobs(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, top_lp >= 0 ? lps.data() : nullptr,
-                                      top_lp >= 0 ? lp_ids.data() : nullptr);
+        wrc = rr_engine_wait_logprobs(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
+                                      logprobs ? lp_ids.data() : nullptr);
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -159,7 +151,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
             const int n = comp.n_generated < max_new ? comp.n_generated : max_new;
             r->tokens.assign(toks.begin(), toks.begin() + (n > 0 ? n : 0));
-            if (top_lp >= 0) {
+            if (logprobs) {
                 r->lp.assign(lps.begin(), lps.begin() + r->tokens.size() * k);
                 r->lp_id.assign(lp_ids.begin(), lp_ids.begin() + r->tokens.size() * k);
             }
@@ -287,14 +279,8 @@ static void gw_dispatch(rr_gateway* g) {
             }
             uint64_t tk = 0;
             int src = RR_INTERNAL;
-            rr::PenaltyParams pen;
-            if (r->processed) {
-                pen.freq = r->fpen; pen.pres = r->ppen; pen.n_bias = (int)r->bias_id.size();
-                pen.ids = r->bias_id.data(); pen.vals = r->bias_val.data();
-            }
-            if (!cancelled && eng) src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk,
-                                                           r->top_lp, r->temp, r->top_p, r->seed,
-                                                           r->processed ? &pen : nullptr);
+            if (!cancelled && eng)
+                src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk, r->gen);
             bool cancel_now = false;
             std::unique_lock<std::mutex> lk(g->mu);
             if (src == RR_OK) {
@@ -385,30 +371,19 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
     return RR_OK;
 }
 
+// p is checked (GenParams::set) against the smallest vocabulary, as prompt ids are: any engine of a fallback accepts it.
 static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
-                     int max_new_tokens, int declare_burst, int top_logprobs, uint64_t* tickets, float temperature = 0.f,
-                     float top_p = 1.f, uint64_t seed = 0, const rr::PenaltyParams* pen = nullptr) {
+                     int max_new_tokens, int declare_burst, const rr::GenParams& p, uint64_t* tickets) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
-    if (top_logprobs < -1 || top_logprobs > rr::LP_MAX_TOP) return RR_INVALID_ARGUMENT;
-    if (!rr::sample_params_ok(temperature, top_p)) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n; ++i) {
         const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens);
         if (rc != RR_OK) return rc;
     }
-    // bias ids against the smallest vocabulary, as prompt ids: a fallback to any engine accepts them
-    if (pen && !rr::penalty_params_ok(pen->freq, pen->pres, pen->n_bias, pen->ids, pen->vals, g->min_vocab))
-        return RR_INVALID_ARGUMENT;
-    const bool processed = pen && (pen->freq != 0.f || pen->pres != 0.f || pen->n_bias > 0);
     std::vector<GwReq*> reqs((size_t)n);
     for (int i = 0; i < n; ++i) {
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
-        r->group = group; r->max_new = max_new_tokens; r->top_lp = top_logprobs;
-        if (temperature > 0.f) { r->temp = temperature; r->top_p = top_p; r->seed = seed; }
-        if (processed) {
-            r->processed = true; r->fpen = pen->freq; r->ppen = pen->pres;
-            r->bias_id.assign(pen->ids, pen->ids + pen->n_bias); r->bias_val.assign(pen->vals, pen->vals + pen->n_bias);
-        }
+        r->group = group; r->max_new = max_new_tokens; r->gen = p;
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -432,42 +407,46 @@ static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const 
 
 RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
                                    int max_new_tokens, int declare_burst, uint64_t* tickets) {
-    return gw_submit(g, group, prompt_ids, prompt_start, n, max_new_tokens, declare_burst, -1, tickets);
+    return gw_submit(g, group, prompt_ids, prompt_start, n, max_new_tokens, declare_burst, rr::GenParams(), tickets);
 }
 
-RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                             uint64_t* ticket) {
-    const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, -1, ticket);
-}
-
-RR_API int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                      int top_logprobs, uint64_t* ticket) {
-    const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket);
-}
-
-RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                     int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
-    const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket, temperature, top_p, seed);
-}
-
+// The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
+// gets RR_INVALID_ARGUMENT.
 RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
                                        int max_new_tokens, int top_logprobs, float temperature, float top_p, uint64_t seed,
                                        float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
                                        const float* bias_vals, uint64_t* ticket) {
+    if (!g) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals);
     const int32_t start[2] = {0, n_prompt};
-    rr::PenaltyParams pen;
-    pen.freq = frequency_penalty; pen.pres = presence_penalty; pen.n_bias = n_bias; pen.ids = bias_ids; pen.vals = bias_vals;
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, top_logprobs, ticket, temperature, top_p, seed, &pen);
+    return rc != RR_OK ? rc : gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, ticket);
 }
 
-// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][gw_lp_width(r)].
+RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                             uint64_t* ticket) {
+    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, -1, 0.f, 1.f, 0, 0.f, 0.f, 0, nullptr,
+                                       nullptr, ticket);
+}
+
+RR_API int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                      int top_logprobs, uint64_t* ticket) {
+    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, top_logprobs, 0.f, 1.f, 0, 0.f, 0.f, 0,
+                                       nullptr, nullptr, ticket);
+}
+
+RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                     int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
+    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, top_logprobs, temperature, top_p, seed,
+                                       0.f, 0.f, 0, nullptr, nullptr, ticket);
+}
+
+// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][r->gen.lp_width()].
 static void gw_copy_logprobs(const GwReq* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (r->top_lp < 0 || t <= 0) return;
-    const size_t m = (size_t)t * gw_lp_width(r);
+    if (!r->gen.logprobs() || t <= 0) return;
+    const size_t m = (size_t)t * r->gen.lp_width();
     if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
     if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
 }

@@ -77,24 +77,29 @@ int num_sms();
 
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)
 typedef void (*EngineDoneHook)(void* ctx, uint64_t tag, uint64_t ticket, int status, int n_generated);
-// Penalties and logit bias of a request (rr_engine_submit_processed); host arrays of n_bias entries.
-struct PenaltyParams {
-    float freq = 0.f, pres = 0.f;
-    int n_bias = 0;
-    const int32_t* ids = nullptr;
-    const float* vals = nullptr;
+// What a request asks the decoder to do (the parameters of rr_engine_submit_processed / rr_gateway_submit_processed;
+// the defaults are a plain greedy request).  The gateway hands it unchanged to every engine the request is admitted to.
+struct GenParams {
+    int top_lp = -1;                  // -1: no logprobs, else max(1, top_lp) (logprob, id) pairs per token
+    float temp = 0.f, top_p = 1.f;    // temp > 0 draws every token with rr_op_sample
+    uint64_t seed = 0;
+    float fpen = 0.f, ppen = 0.f;     // frequency / presence penalties over the generated tokens, and a logit bias, applied
+    std::vector<int32_t> bias_id;     // to the logits before the token is picked (rr_op_logit_penalties)
+    std::vector<float> bias_val;
+    bool logprobs() const { return top_lp >= 0; }
+    bool sampled() const { return temp > 0.f; }
+    bool processed() const { return fpen != 0.f || ppen != 0.f || !bias_id.empty(); }
+    // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
+    int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
+    // The raw C arguments, checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and OpenAI's ranges
+    // 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null arrays when
+    // n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails.  A greedy request keeps the
+    // default top_p and seed, an unprocessed one the default penalties.  RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
+    int set(int vocab, int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals);
 };
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, int top_logprobs = -1, float temperature = 0.f, float top_p = 1.f,
-                         uint64_t seed = 0, const PenaltyParams* pen = nullptr);
-// OpenAI's ranges for a sampled request (rr_engine_submit_sampled): 0 <= temperature <= 2, 0 <= top_p <= 1 (NaN fails).
-inline bool sample_params_ok(float temperature, float top_p) {
-    return temperature >= 0.f && temperature <= 2.f && top_p >= 0.f && top_p <= 1.f;
-}
-// OpenAI's ranges for a processed request (rr_engine_submit_processed): -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS,
-// bias ids unique and in [0, vocab), -100 <= bias values <= 100 (NaN fails).
-bool penalty_params_ok(float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                       const float* bias_vals, int vocab);
+                         uint64_t* ticket, const GenParams& p);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);

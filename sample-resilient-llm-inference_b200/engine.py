@@ -7,7 +7,6 @@ computation happens in the CUDA library.  Replaces one `bedrock/...` deployment 
 from __future__ import annotations
 
 import ctypes as C
-import secrets
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -16,7 +15,7 @@ import torch
 
 from . import _lib
 from .models import ModelSpec, Weights, make_weights
-from .router import logprob_pairs
+from .router import gen_args, logprob_pairs
 
 
 @dataclass
@@ -156,36 +155,14 @@ class Engine:
         {token id: bias in [-100, 100]} (at most 300 entries): applied to the logits before every token is picked, the
         penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing."""
         ids = _i32(prompt_ids)
+        bias = logit_bias or {}
+        gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
+                       list(bias.values()))
         t = C.c_uint64()
-        if frequency_penalty or presence_penalty or logit_bias:
-            seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temperature else 0
-            k = -1 if top_logprobs is None else int(top_logprobs)
-            b_ids = _i32(list((logit_bias or {}).keys()))
-            b_vals = np.ascontiguousarray(np.asarray(list((logit_bias or {}).values()), dtype=np.float32))
-            _lib.check(_lib.lib.rr_engine_submit_processed(
-                self._h, _p(ids), len(ids), max_new_tokens, k, float(temperature or 0.0),
-                1.0 if top_p is None else float(top_p), seed, float(frequency_penalty or 0.0),
-                float(presence_penalty or 0.0), len(b_ids), _p(b_ids),
-                b_vals.ctypes.data_as(C.POINTER(C.c_float)), C.byref(t)), "rr_engine_submit_processed")
-            if k >= 0:
-                self._lp_k[t.value] = max(1, k) + (1 if temperature else 0)
-            return t.value
-        if temperature:
-            seed = secrets.randbits(64) if seed is None else int(seed) % 2**64
-            k = -1 if top_logprobs is None else int(top_logprobs)
-            _lib.check(_lib.lib.rr_engine_submit_sampled(self._h, _p(ids), len(ids), max_new_tokens, k, float(temperature),
-                                                         1.0 if top_p is None else float(top_p), seed, C.byref(t)),
-                       "rr_engine_submit_sampled")
-            if k >= 0:
-                self._lp_k[t.value] = max(1, k) + 1
-            return t.value
-        if top_logprobs is None:
-            _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(t)),
-                       "rr_engine_submit")
-            return t.value
-        _lib.check(_lib.lib.rr_engine_submit_logprobs(self._h, _p(ids), len(ids), max_new_tokens, int(top_logprobs),
-                                                      C.byref(t)), "rr_engine_submit_logprobs")
-        self._lp_k[t.value] = max(1, int(top_logprobs))
+        _lib.check(_lib.lib.rr_engine_submit_processed(self._h, _p(ids), len(ids), max_new_tokens, *gen.tail, C.byref(t)),
+                   "rr_engine_submit_processed")
+        if gen.width:
+            self._lp_k[t.value] = gen.width
         return t.value
 
     def _lp_bufs(self, ticket: int, max_tokens: int):

@@ -22,7 +22,7 @@ import threading
 import time
 import uuid
 from dataclasses import dataclass, field
-from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
+from typing import Any, Callable, Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -235,6 +235,33 @@ def check_penalties(frequency_penalty: Any = None, presence_penalty: Any = None,
     return fp, pp, ids, vals
 
 
+class GenArgs(NamedTuple):
+    """A request's generation parameters in the form the native submit calls take them (gen_args)."""
+    top: Optional[int]     # top_logprobs; None: no logprobs
+    tail: tuple            # rr_engine_submit_processed / rr_gateway_submit_processed: top_logprobs .. bias_vals
+    width: int             # (logprob, id) pairs per generated token; 0 without logprobs
+
+
+def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
+             seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
+             presence_penalty: Optional[float] = None, bias_ids: Sequence[int] = (),
+             bias_vals: Sequence[float] = ()) -> GenArgs:
+    """None and absent fields take the defaults of a plain greedy request.  A sampled request (temperature > 0) without
+    a seed gets a random one here, once, so that a fallback re-admission draws the same tokens; the seed is taken modulo
+    2^64.  Without bias entries the bias arrays are null pointers.  Ranges are checked by the native call (check_* raise
+    HTTP 400 first on the router's path)."""
+    k = -1 if top_logprobs is None else int(top_logprobs)
+    temp = float(temperature or 0.0)
+    seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temp else 0
+    b_ids = b_vals = None
+    if len(bias_ids):
+        b_ids = np.ascontiguousarray(np.asarray(bias_ids, dtype=np.int32)).ctypes.data_as(C.POINTER(C.c_int32))
+        b_vals = np.ascontiguousarray(np.asarray(bias_vals, dtype=np.float32)).ctypes.data_as(C.POINTER(C.c_float))
+    tail = (k, temp, 1.0 if top_p is None else float(top_p), seed, float(frequency_penalty or 0.0),
+            float(presence_penalty or 0.0), len(bias_ids), b_ids, b_vals)
+    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0)
+
+
 def _token_entry(tok: int, logprob: float) -> dict:
     """One token of the byte tokenizer in OpenAI's logprob shape (`token` is detokenize([tok]), `bytes` its byte)."""
     return {"token": detokenize([tok]), "logprob": logprob, "bytes": [(tok - 3) % 256] if tok >= 3 else []}
@@ -441,48 +468,32 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, top: Optional[int] = None, samp=None,
-                   pen=None) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs) -> int:
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        if pen is not None:
-            b_ids = np.ascontiguousarray(np.asarray(pen[2], dtype=np.int32))
-            b_vals = np.ascontiguousarray(np.asarray(pen[3], dtype=np.float32))
-            temp, top_p, seed = samp if samp is not None else (0.0, 1.0, 0)
-            rc = _lib.lib.rr_gateway_submit_processed(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
-                                                      -1 if top is None else top, temp, top_p, seed, pen[0], pen[1],
-                                                      len(b_ids), b_ids.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                      b_vals.ctypes.data_as(C.POINTER(C.c_float)), C.byref(t))
-        elif samp is not None:
-            rc = _lib.lib.rr_gateway_submit_sampled(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
-                                                    -1 if top is None else top, samp[0], samp[1], samp[2], C.byref(t))
-        elif top is None:
-            rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new, C.byref(t))
-        else:
-            rc = _lib.lib.rr_gateway_submit_logprobs(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
-                                                     top, C.byref(t))
+        rc = _lib.lib.rr_gateway_submit_processed(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                                  *gen.tail, C.byref(t))
         if rc != 0:
             raise self._gw_error(rc, model)
         return t.value
 
     @staticmethod
-    def _lp_bufs(top: Optional[int], max_new: int, sampled: bool = False):
-        """[max_new][max(1, top)] pair buffers; a sampled request has one more column, the generated token's own pair."""
-        if top is None:
+    def _lp_bufs(gen: GenArgs, max_new: int):
+        """[max_new][gen.width] pair buffers of a logprobs request."""
+        if gen.top is None:
             return None, None, None, None
-        w = max(1, top) + (1 if sampled else 0)
-        lp = np.zeros((max_new, w), dtype=np.float32)
-        ids = np.zeros((max_new, w), dtype=np.int32)
+        lp = np.zeros((max_new, gen.width), dtype=np.float32)
+        ids = np.zeros((max_new, gen.width), dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None, pen=None):
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp, pen)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new, samp is not None)
+        lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new)
         rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, float(timeout or 0.0), C.byref(res),
                                                toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
         if rc == 6:                      # client-side timeout: give the row back, count a failure against the deployment
@@ -491,17 +502,19 @@ class Router:
         if rc != 0:
             raise self._gw_error(rc, model, res, timeout)
         content = None
-        if top is not None:
+        if gen.top is not None:
             n = min(res.n_generated, max_new)
-            content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), top), "refusal": None}
+            content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), gen.top),
+                       "refusal": None}
         return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
 
-    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, top=None, samp=None, pen=None):
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, top, samp, pen)
+    def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
+        top = gen.top
         deadline = None if not timeout else time.perf_counter() + timeout
         res = _lib.GatewayResult()
         toks = np.zeros(max_new, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(top, max_new, samp is not None)
+        lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new)
         n, done = C.c_int32(), C.c_int32()
         sent, finished = 0, False
 
@@ -633,26 +646,16 @@ class Router:
         """Token ids must be valid on every replica a request may fall back to: the smallest vocabulary attached."""
         return min((b.vocab for b in self.backends.values()), default=128256)
 
-    def _logprobs_top(self, logprobs, top_logprobs) -> Optional[int]:
-        """Validated logprobs setting (None = off); only engine replicas have logits to serve it."""
+    def _params(self, logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
+                logit_bias) -> GenArgs:
+        """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs; bias ids
+        must be valid on every replica the request may fall back to."""
         top = check_logprobs(logprobs, top_logprobs)
         if top is not None and self._gateway() is None:
             raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
-        return top
-
-    @staticmethod
-    def _sampling(temperature, top_p, seed):
-        """Validated sampling setting (None = greedy); a request without a seed gets one here, once, so that a fallback
-        re-admission draws the same tokens."""
-        samp = check_sampling(temperature, top_p, seed)
-        if samp is not None and samp[2] is None:
-            samp = (samp[0], samp[1], secrets.randbits(64))
-        return samp
-
-    def _penalties(self, frequency_penalty, presence_penalty, logit_bias):
-        """Validated penalties and logit bias (None = nothing to apply); bias ids must be valid on every replica the
-        request may fall back to."""
-        return check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab())
+        samp = check_sampling(temperature, top_p, seed) or (None, None, None)
+        pen = check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab()) or (None, None, (), ())
+        return gen_args(top, *samp, *pen)
 
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
@@ -666,9 +669,8 @@ class Router:
         greedy.  frequency_penalty / presence_penalty / logit_bias: applied to the logits before every token is picked
         (rr_op_logit_penalties; the penalties count the tokens generated so far).  Stub backends validate these and keep
         their fixed reply."""
-        top = self._logprobs_top(logprobs, top_logprobs)
-        samp = self._sampling(temperature, top_p, seed)
-        pen = self._penalties(frequency_penalty, presence_penalty, logit_bias)
+        gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
+                           logit_bias)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -678,7 +680,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp, pen)
+            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, gen)
         # ---- host loop (StubBackend): same admission events, one K1 launch per event
         t_start = time.perf_counter()
         chain_start = 0
@@ -724,9 +726,8 @@ class Router:
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
         fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties and logit
         bias as in completion()."""
-        top = self._logprobs_top(logprobs, top_logprobs)
-        samp = self._sampling(temperature, top_p, seed)
-        pen = self._penalties(frequency_penalty, presence_penalty, logit_bias)
+        gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
+                           logit_bias)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -735,7 +736,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         gw = self._gateway()
         if gw is not None:
-            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, top, samp, pen)
+            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, gen)
             return
         deadline = None if not timeout else time.perf_counter() + timeout
         chain_start = 0

@@ -302,7 +302,7 @@ def test_launches_and_copies_of_plain_logprobs_and_sampled_runs():
     w = make_weights(spec, seed=3, sigma=0.05, device="cuda")
     B, N = 16, 40
     eng = Engine(w, max_batch=B, ctx_max=1024, max_prefill_tokens=512, use_cuda_graph=True)
-    keys = ("kernel_launches", "decode_steps", "prefill_chunks", "d2h_bytes")
+    keys = ("kernel_launches", "decode_steps", "prefill_chunks", "d2h_bytes", "h2d_bytes")
     prompt = list(range(5, 40))
     try:
         def run(**kw):
@@ -316,19 +316,21 @@ def test_launches_and_copies_of_plain_logprobs_and_sampled_runs():
         eng.wait(eng.submit(prompt, 1))
         F = eng.stats()["kernel_launches"]                             # one prefill chunk
         P = (s1["kernel_launches"] - F) // (N - 1)
+        H = s1["h2d_bytes"]
         assert s1 == {"kernel_launches": F + (N - 1) * P, "decode_steps": N - 1, "prefill_chunks": 1,
-                      "d2h_bytes": 4 + (N - 1) * 4 * B}
+                      "d2h_bytes": 4 + (N - 1) * 4 * B, "h2d_bytes": H}
         samp = dict(temperature=1.0, top_p=0.9, seed=1)
         run(**samp); run(top_logprobs=2, **samp); run(top_logprobs=2)   # capture every graph
         _, s = run(**samp)
         assert s == {"kernel_launches": F + 3 + (N - 1) * (P + 3), "decode_steps": N - 1, "prefill_chunks": 1,
-                     "d2h_bytes": 4 + (N - 1) * 4 * B}
+                     "d2h_bytes": 4 + (N - 1) * 4 * B, "h2d_bytes": H + 16 * B + 20}
         _, s = run(top_logprobs=2)
         assert s == {"kernel_launches": F + 2 + (N - 1) * (P + 2), "decode_steps": N - 1, "prefill_chunks": 1,
-                     "d2h_bytes": 4 + 20 * 8 + (N - 1) * (4 * B + 20 * 8 * B)}
+                     "d2h_bytes": 4 + 20 * 8 + (N - 1) * (4 * B + 20 * 8 * B), "h2d_bytes": H + 4 * B + 4}
         _, s = run(top_logprobs=2, **samp)
         assert s == {"kernel_launches": F + 5 + (N - 1) * (P + 5), "decode_steps": N - 1, "prefill_chunks": 1,
-                     "d2h_bytes": 4 + 20 * 8 + 4 + (N - 1) * (4 * B + 20 * 8 * B + 4 * B)}
+                     "d2h_bytes": 4 + 20 * 8 + 4 + (N - 1) * (4 * B + 20 * 8 * B + 4 * B),
+                     "h2d_bytes": H + 16 * B + 20 + 4 * B + 4}
         _, s = run()
         assert s == s1                                                  # plain again: today's totals
     finally:
