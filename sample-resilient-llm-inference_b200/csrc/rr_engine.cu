@@ -9,7 +9,7 @@
 // Layout in HBM (one replica): bf16 weights (caller-owned), KV cache
 // [layer][slot][kv_head][ctx_max][128] bf16 for K and for V, a decode working set of max_batch
 // rows (row b == KV slot b) and a prefill working set of max_prefill_tokens rows.
-// The decode step is a fixed sequence of 9 launches per layer + 4, captured once in a CUDA graph
+// The decode step is a fixed sequence of 6 launches per layer + 4, captured once in a CUDA graph
 // and replayed; per-row metadata (token, position, active flag) lives on the device so replays
 // need no parameter changes.
 #include "rr_kernels.h"
@@ -20,7 +20,6 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
-#include <map>
 #include <mutex>
 #include <new>
 #include <string.h>
@@ -32,16 +31,6 @@
 
 namespace rr {
 void note_cuda_error(cudaError_t e);
-
-__global__ void gather_rows_kernel(const __nv_bfloat16* __restrict__ src, const int32_t* __restrict__ idx,
-                                   __nv_bfloat16* __restrict__ dst, int hidden) {
-    griddep_launch();
-    griddep_wait();
-    const int r = blockIdx.x;
-    const uint4* s = reinterpret_cast<const uint4*>(src + (size_t)idx[r] * hidden);
-    uint4* d = reinterpret_cast<uint4*>(dst + (size_t)r * hidden);
-    for (int c = threadIdx.x; c < hidden / 8; c += blockDim.x) d[c] = s[c];
-}
 
 // Last layer of a prefill chunk: only the last token of every prompt still matters after attention.  Gather those
 // rows (attention output bf16, residual fp32) into the decode working set; the rest of the layer and lm_head then run
@@ -98,33 +87,68 @@ struct Request {
 // prefixes (a BOS and a role tag) stay misses.
 constexpr int PREFIX_MIN = 64;
 
-// Sampling parameter blocks, per row at stride n: seed (8 bytes) | temperature | top_p, and in prefill also | position.
-constexpr int SAMP_BYTES = 16, SAMP_PF_BYTES = 20;
+// The per-row parameter blocks of n rows, one per step_mode bit, each a structure of arrays at stride n:
+//   0 top_n  top_lp i32[n] (-1: no logprobs)
+//   1 samp   seed u64[n] | temperature f32[n] (0: greedy) | top_p f32[n], with a position column also | position i32[n]
+//   2 pen    frequency_penalty f32[n] | presence_penalty f32[n] | gen0 i32[n] (the position of the first generated token)
+//            | n_bias i32[n] | bias ids i32[n][bias_ld] | bias values f32[n][bias_ld]
+// The decode rows use n = Bm and bias_ld = PEN_MAX_BIAS (fixed: the graphs hold it).  A prefill chunk uses n = n_seqs, the
+// largest bias count among its sequences and a position column, in buffers sized for Bm rows and PEN_MAX_BIAS.
+struct ParamBlocks {
+    char* blk[3] = {};            // pen stays null until the first processed request (ensure_pen_buffers)
+    int n = 0, bias_ld = 0;
+    bool has_pos = false;
 
-// Penalty parameter blocks, per row at stride n: frequency_penalty | presence_penalty | gen0 (the position of the first
-// generated token) | n_bias, then bias ids [n][bias_ld] and values [n][bias_ld].  Decode rows use bias_ld = PEN_MAX_BIAS
-// (fixed: the graphs hold it); a prefill chunk uses the largest bias count among its sequences.
-static size_t pen_bytes(int n, int bias_ld) { return (size_t)n * (16 + 8 * (size_t)bias_ld); }
-static PenaltyArgs pen_args(const char* blk, int n, int bias_ld) {
-    PenaltyArgs a;
-    a.freq = (const float*)blk; a.pres = (const float*)(blk + 4 * (size_t)n);
-    a.gen0 = (const int32_t*)(blk + 8 * (size_t)n); a.n_bias = (const int32_t*)(blk + 12 * (size_t)n);
-    a.bias_ids = (const int32_t*)(blk + 16 * (size_t)n);
-    a.bias_vals = (const float*)(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld);
-    a.bias_ld = bias_ld;
-    a.hist = nullptr; a.hist_ld = 0; a.hist_len = nullptr; a.app_tok = nullptr; a.app_pos = nullptr;
-    return a;
-}
-// Writes row i of a block at stride n: p's bias, the given penalties and gen0.
-static void pen_fill_row(char* blk, int n, int bias_ld, int i, const GenParams& p, float freq, float pres, int gen0) {
-    const int nb = (int)p.bias_id.size();
-    ((float*)blk)[i] = freq; ((float*)(blk + 4 * (size_t)n))[i] = pres;
-    ((int32_t*)(blk + 8 * (size_t)n))[i] = gen0; ((int32_t*)(blk + 12 * (size_t)n))[i] = nb;
-    if (nb) {
-        memcpy(blk + 16 * (size_t)n + 4 * ((size_t)i * bias_ld), p.bias_id.data(), 4 * (size_t)nb);
-        memcpy(blk + 16 * (size_t)n + 4 * (size_t)n * bias_ld + 4 * ((size_t)i * bias_ld), p.bias_val.data(), 4 * (size_t)nb);
+    ParamBlocks at(int rows, int ld) const { ParamBlocks p = *this; p.n = rows; p.bias_ld = ld; return p; }
+    size_t bytes(int i) const { return (size_t)n * (i == 0 ? 4 : i == 1 ? (has_pos ? 20 : 16) : 16 + 8 * (size_t)bias_ld); }
+    int32_t* top_n() const { return (int32_t*)blk[0]; }
+    uint64_t* seed() const { return (uint64_t*)blk[1]; }
+    float* temp() const { return (float*)(blk[1] + 8 * (size_t)n); }
+    float* top_p() const { return (float*)(blk[1] + 12 * (size_t)n); }
+    int32_t* pos() const { return (int32_t*)(blk[1] + 16 * (size_t)n); }
+    float* freq() const { return (float*)blk[2]; }
+    float* pres() const { return (float*)(blk[2] + 4 * (size_t)n); }
+    int32_t* gen0() const { return (int32_t*)(blk[2] + 8 * (size_t)n); }
+    int32_t* n_bias() const { return (int32_t*)(blk[2] + 12 * (size_t)n); }
+    int32_t* bias_ids() const { return (int32_t*)(blk[2] + 16 * (size_t)n); }
+    float* bias_vals() const { return (float*)(bias_ids() + (size_t)n * bias_ld); }
+
+    PenaltyArgs pen_args() const {
+        PenaltyArgs a;
+        a.freq = freq(); a.pres = pres(); a.gen0 = gen0(); a.n_bias = n_bias();
+        a.bias_ids = bias_ids(); a.bias_vals = bias_vals(); a.bias_ld = bias_ld;
+        a.hist = nullptr; a.hist_ld = 0; a.hist_len = nullptr; a.app_tok = nullptr; a.app_pos = nullptr;
+        return a;
     }
-}
+    // The step_mode bits of the blocks whose row i differs from the defaults.
+    int row_mode(int i) const {
+        return (top_n()[i] >= 0 ? 1 : 0) | (temp()[i] > 0.f ? 2 : 0) |
+               (blk[2] && (freq()[i] != 0.f || pres()[i] != 0.f || n_bias()[i] != 0) ? 4 : 0);
+    }
+    // Row i from p: drawn at `position` (with a position column), p's bias, and penalties f / pr from position g0 on.
+    void put_row(int i, const GenParams& p, int position, float f, float pr, int g0) const {
+        top_n()[i] = p.top_lp;
+        seed()[i] = p.seed; temp()[i] = p.temp; top_p()[i] = p.top_p;
+        if (has_pos) pos()[i] = position;
+        if (!blk[2]) return;
+        const int nb = (int)p.bias_id.size();
+        freq()[i] = f; pres()[i] = pr; gen0()[i] = g0; n_bias()[i] = nb;
+        if (nb) {
+            memcpy(bias_ids() + (size_t)i * bias_ld, p.bias_id.data(), 4 * (size_t)nb);
+            memcpy(bias_vals() + (size_t)i * bias_ld, p.bias_val.data(), 4 * (size_t)nb);
+        }
+    }
+    // Copies the blocks whose bit is in `mask` from these (pinned) blocks to d, of the same n and bias_ld.
+    cudaError_t upload(const ParamBlocks& d, int mask, cudaStream_t s, uint64_t* h2d_bytes) const {
+        for (int i = 0; i < 3; ++i) {
+            if (!(mask >> i & 1)) continue;
+            const cudaError_t err = cudaMemcpyAsync(d.blk[i], blk[i], bytes(i), cudaMemcpyHostToDevice, s);
+            if (err != cudaSuccess) return err;
+            *h2d_bytes += bytes(i);
+        }
+        return cudaSuccess;
+    }
+};
 
 int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_, uint64_t seed_, float frequency_penalty,
                    float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals) {
@@ -184,7 +208,7 @@ struct rr_engine {
     std::vector<GemmPlan> pl_qkv, pl_o, pl_gu, pl_down;
     std::vector<DecodeAttnArgs> attn_args;   // per layer (TMA maps of that layer's K / V cache)
     std::vector<PrefillAttnArgs> pf_attn;    // per layer (TMA maps of q and of that layer's K / V cache)
-    GemmPlan pl_head, pl_head_pf;
+    GemmPlan pl_head;
     int s_qkv, s_o, s_gu, s_down;
     bool fuse_rope_pf = false;        // prefill: RoPE + KV append live in the QKV GEMM epilogue (head_dim 128)
     // prefill defers RMSNorm: no norm kernels inside the layers -- RESID epilogues emit bf16(x * gamma) + sum(x^2), the next
@@ -202,42 +226,34 @@ struct rr_engine {
     // processed rows replays the plain graph.
     cudaGraphExec_t graph[8] = {};
     bool warmed = false;
-    // Per-row parameter blocks of the decode rows (d_topn, d_samp, d_pen), each with a pinned host mirror (h_topn, h_samp,
-    // h_pen) that set_row_params keeps in step with row_req, and a dirty flag; upload_row_params copies a dirty block before
-    // a step that reads it.  A prefill chunk packs its sequences' parameters into its own blocks (*_pf) and staging.
-    int32_t *d_topn = nullptr, *d_topn_pf = nullptr;   // per decode row / per prefill sequence: top_lp, -1 = off
+    // The decode rows' parameter blocks (d_rows) and their pinned host mirror (h_rows), which set_row_params keeps in step
+    // with row_req, marking the blocks it changes in rows_dirty (step_mode bits); upload_row_params copies a dirty block
+    // before a step that reads it.  A prefill chunk packs its sequences' parameters into staging (h_pf) and blocks of its
+    // own (d_pf).
+    ParamBlocks d_rows, h_rows, d_pf, h_pf;
+    int rows_dirty = 0;
     void* lp_ws = nullptr;
     float* d_lp = nullptr;                             // [Bm][LP_MAX_TOP]
     int32_t* d_lp_id = nullptr;
-    // sampling: per decode row seed[Bm] | temperature[Bm] | top_p[Bm] (temperature 0 = greedy row); the prefill block holds
-    // the same per sequence plus position[n], packed at stride n_seqs
-    char *d_samp = nullptr, *d_samp_pf = nullptr;
     void* sample_ws = nullptr;
     float* d_tok_lp = nullptr;                         // [Bm] the sampled token's logprob (sampled logprobs rows)
-    // penalties / logit bias, allocated on the first processed request (ensure_pen_buffers): the decode rows' block
-    // (pen_args layout, stride Bm) and its mirror, the prefill chunk's block and its staging, the generated-token history
-    // [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
-    char *d_pen = nullptr, *d_pen_pf = nullptr, *h_pen = nullptr, *h_pen_pf = nullptr;
+    // penalties, allocated with the pen blocks on the first processed request (ensure_pen_buffers): the generated-token
+    // history [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
     int32_t *d_hist = nullptr, *pen_ws = nullptr;
-    bool topn_dirty = false, samp_dirty = false, pen_dirty = false;
 
     // prefill working set
     int Tmax;
     int32_t *p_ids, *p_pos, *p_slot, *p_seq_start, *p_seq_slot, *p_last, *p_first;
     float* px;
-    __nv_bfloat16 *pxn, *pqkv, *pq, *pattn, *po, *pgu, *pact, *xn_last;
-    struct PfPlans { std::vector<GemmPlan> qkv, o, gu, down; };
-    std::map<int, PfPlans> pf_plans;
+    __nv_bfloat16 *pxn, *pqkv, *pq, *pattn, *pgu, *pact;
+    // prefill GEMM plans (4 L TMA descriptors), built at create for Tmax rows
+    struct PfPlans { std::vector<GemmPlan> qkv, o, gu, down; } pf;
 
     // pinned staging
     int32_t* h_stage;     // ids | pos | slot | seq_start | seq_slot | last   (prefill) / rows meta (decode)
-    size_t h_stage_ints;
     int32_t* h_tok;       // [Bm] tokens read back each step
-    float* h_logits = nullptr;
     float* h_lp = nullptr;        // [Bm][LP_MAX_TOP] logprobs read back on steps that computed them
     int32_t* h_lp_id = nullptr;
-    int32_t *h_topn = nullptr, *h_topn_pf = nullptr;   // [Bm] mirror of d_topn / staging of d_topn_pf
-    char *h_samp = nullptr, *h_samp_pf = nullptr;      // [Bm * SAMP_BYTES] mirror of d_samp / [Bm * SAMP_PF_BYTES] staging
     float* h_tok_lp = nullptr;    // [Bm]
 
     // serving state
@@ -315,29 +331,18 @@ static PartIn part_bf16(const __nv_bfloat16* p, int ld) {
 static PartIn part_none() { PartIn r; r.ptr = nullptr; r.is_bf16 = 0; r.n_splits = 1; r.split_stride = 0; r.ld = 0; return r; }
 
 // ---------------------------------------------------------------- decode step (enqueue only)
-// tok (sampled rows): also the logprob of the row's final token into d_tok_lp
-static void enqueue_logprobs(rr_engine* e, const int32_t* top_n, int rows, cudaStream_t s, const int32_t* tok = nullptr) {
-    launch_logprobs(e->logits, e->d.vocab, rows, e->d.vocab, top_n, LP_MAX_TOP, e->lp_ws, e->d_lp, e->d_lp_id, s, tok,
-                    tok ? e->d_tok_lp : nullptr);
-}
-
-// The sampler over `rows` rows of `logits` with a parameter block at stride n (seed | temperature | top_p).
-static void enqueue_sample(rr_engine* e, const char* samp, int n, int rows, const int32_t* position, int32_t* tok,
-                           cudaStream_t s) {
-    launch_sample(e->logits, e->d.vocab, rows, e->d.vocab, (const float*)(samp + (size_t)8 * n),
-                  (const float*)(samp + (size_t)12 * n), (const uint64_t*)samp, position, tok, e->sample_ws, s);
-}
-
-static int step_mode(bool logprobs, bool sample, bool pen) {
-    return (logprobs ? 1 : 0) | (sample ? 2 : 0) | (pen ? 4 : 0);
+// The step_mode bits a request needs: 1 logprobs, 2 sampling, 4 penalties / logit bias.  Over a step's rows or a chunk's
+// sequences they pick the parameter blocks to upload, the kernels of the logits tail and the decode graph.
+static int step_mode(const GenParams& p) {
+    return (p.logprobs() ? 1 : 0) | (p.sampled() ? 2 : 0) | (p.processed() ? 4 : 0);
 }
 
 // Caller holds gpu_mu.  The penalty buffers, allocated on the first processed request, so an engine that never sees one
 // keeps its footprint.
 static int ensure_pen_buffers(rr_engine* e) {
-    if (e->d_pen) return RR_OK;
+    if (e->d_rows.blk[2]) return RR_OK;
     const int B = e->Bm;
-    const size_t blk = pen_bytes(B, PEN_MAX_BIAS);
+    const size_t blk = e->d_rows.bytes(2);            // also the prefill blocks' size: Bm rows of PEN_MAX_BIAS
     char *dp = nullptr, *dpf = nullptr;
     int32_t *hist = nullptr, *ws = nullptr;
     int rc = dalloc(e, &dp, blk);
@@ -353,56 +358,100 @@ static int ensure_pen_buffers(rr_engine* e) {
     if (ce != cudaSuccess) { cudaFreeHost(hp); rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
     memset(hp, 0, blk);
     CK(cudaStreamSynchronize(e->stream));
-    e->d_pen_pf = dpf; e->d_hist = hist; e->pen_ws = ws; e->h_pen = hp; e->h_pen_pf = hpf;
-    e->d_pen = dp;
+    e->d_pf.blk[2] = dpf; e->d_hist = hist; e->pen_ws = ws; e->h_rows.blk[2] = hp; e->h_pf.blk[2] = hpf;
+    e->d_rows.blk[2] = dp;
     return RR_OK;
 }
 
-// logprobs: launch_logprobs after the argmax for the rows with d_topn[row] >= 0 (the logits are left as they were)
-// sample: rows with temperature > 0 replace the argmax token by rr_op_sample's draw at position d_pos (argmax advanced it
-// to the generated token's position), before logprobs, which then also gives the drawn token's own logprob
-// pen: before the argmax, processed rows append their input token (the last generated one, at position d_pos) to the
-// history and get their penalties and logit bias applied to the logits, which argmax, sampler and logprobs then read
-static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, bool logprobs = false,
-                               bool sample = false, bool pen = false) {
+// The rest of layer l after attention on `rows` rows of the decode working set, with the unfused kernels: O GEMM,
+// add_rmsnorm, gate/up GEMM (SiLU), down GEMM, add_rmsnorm with the next layer's (or the final) norm weight.
+static int enqueue_o_mlp(rr_engine* e, int l, int rows, cudaStream_t s, uint64_t* nl) {
+    const rr_model_desc& d = e->d;
+    const int B = e->Bm;
+    const void* nw = (l + 1 < d.n_layers) ? e->norm_attn[l + 1] : e->final_norm;
+    if (gemm_launch(e->pl_o[l], s) != RR_OK) return RR_CUDA_ERROR; ++*nl;
+    launch_add_rmsnorm(e->x, part_f32(e->part_o, e->s_o, B, d.hidden), (const __nv_bfloat16*)e->norm_mlp[l], e->xn, rows,
+                       d.hidden, d.rms_eps, s); ++*nl;
+    if (gemm_launch(e->pl_gu[l], s) != RR_OK) return RR_CUDA_ERROR; ++*nl;
+    if (!e->fuse_silu) { launch_silu_mul(part_f32(e->part_gu, e->s_gu, B, 2 * d.inter), e->act, rows, d.inter, s); ++*nl; }
+    if (gemm_launch(e->pl_down[l], s) != RR_OK) return RR_CUDA_ERROR; ++*nl;
+    launch_add_rmsnorm(e->x, part_f32(e->part_down, e->s_down, B, d.hidden), (const __nv_bfloat16*)nw, e->xn, rows,
+                       d.hidden, d.rms_eps, s); ++*nl;
+    return RR_OK;
+}
+
+// The logits tail over `rows` rows of e->logits (lm_head's output), reading the parameter blocks p; returns its launches.
+//   mode & 4: penalties and logit bias, applied to the logits that everything after reads.  With hist (decode) each row
+//             first appends its input token tok[r] (the last generated one, at `position`) to its history.
+//   argmax into tok; decode passes row_active (d_slot) and pos_inc (d_pos, advanced to the generated token's position).
+//   mode & 2: rows with temperature > 0 replace the argmax token by rr_op_sample's draw at `position`.
+//   mode & 1: logprobs of the rows with top_n >= 0 (the logits are left as they were), with mode & 2 also the logprob of
+//             the token in tok into d_tok_lp.
+static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int mode, int32_t* tok,
+                             const int32_t* row_active, int32_t* pos_inc, const int32_t* position, int32_t* hist,
+                             cudaStream_t s) {
+    const int V = e->d.vocab;
+    uint64_t nl = 0;
+    if (mode & 4) {
+        PenaltyArgs a = p.pen_args();
+        if (hist) { a.hist = hist; a.hist_ld = e->o.ctx_max; a.app_tok = tok; a.app_pos = position; }
+        launch_logit_penalties(e->logits, V, rows, V, a, e->pen_ws, s); ++nl;
+    }
+    launch_argmax(part_f32(e->logits, 1, e->Bm, V), rows, V, tok, nullptr, row_active, pos_inc, s); ++nl;
+    if (mode & 2) {
+        launch_sample(e->logits, V, rows, V, p.temp(), p.top_p(), p.seed(), position, tok, e->sample_ws, s);
+        nl += SAMPLE_LAUNCHES;
+    }
+    if (mode & 1) {
+        launch_logprobs(e->logits, V, rows, V, p.top_n(), LP_MAX_TOP, e->lp_ws, e->d_lp, e->d_lp_id, s,
+                        mode & 2 ? tok : nullptr, mode & 2 ? e->d_tok_lp : nullptr);
+        nl += LP_LAUNCHES;
+    }
+    return nl;
+}
+
+// Reads a tail's results for `rows` rows back to the host: the tokens (h_tok), with mode & 1 the [rows][LP_MAX_TOP]
+// logprobs and ids (h_lp, h_lp_id), and with mode & 3 == 3 the drawn tokens' logprobs (h_tok_lp).
+static int enqueue_readback(rr_engine* e, const int32_t* tok, int rows, int mode, cudaStream_t s) {
+    CK(cudaMemcpyAsync(e->h_tok, tok, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
+    e->st.d2h_bytes += sizeof(int32_t) * rows;
+    if (!(mode & 1)) return RR_OK;
+    const size_t n = (size_t)rows * LP_MAX_TOP;
+    CK(cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+    e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
+    if (mode & 2) {
+        CK(cudaMemcpyAsync(e->h_tok_lp, e->d_tok_lp, sizeof(float) * rows, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += sizeof(float) * rows;
+    }
+    return RR_OK;
+}
+
+// The decode step over all Bm rows; mode (step_mode bits) selects the kernels of the logits tail.
+static int enqueue_decode_step(rr_engine* e, cudaStream_t s, uint64_t* n_launch, int mode = 0) {
     const rr_model_desc& d = e->d;
     const int B = e->Bm, L = d.n_layers;
     uint64_t nl = 0;
     launch_embed(e->d_tok, (const __nv_bfloat16*)e->embed, e->x, B, d.hidden, e->d_slot, s); ++nl;
     launch_add_rmsnorm(e->x, part_none(), (const __nv_bfloat16*)e->norm_attn[0], e->xn, B, d.hidden, d.rms_eps, s); ++nl;
     for (int l = 0; l < L; ++l) {
-        __nv_bfloat16* kc = e->kcache + (size_t)l * e->kv_layer_stride;
-        __nv_bfloat16* vc = e->vcache + (size_t)l * e->kv_layer_stride;
         if (gemm_launch(e->pl_qkv[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         // RoPE + KV append are fused into the attention kernel (reads the QKV split-K planes directly)
         launch_decode_attn(e->attn_args[l], s); nl += e->kv_splits > 1 ? 2 : 1;
-        if (gemm_launch(e->pl_o[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        const void* nw = (l + 1 < L) ? e->norm_attn[l + 1] : e->final_norm;
-        if (e->fuse_mlp) {
-            launch_add_rmsnorm(e->x, part_f32(e->part_o, e->s_o, B, d.hidden), (const __nv_bfloat16*)e->norm_mlp[l],
-                               e->xn, B, d.hidden, d.rms_eps, s, e->mlp_ready, e->mlp_slices + 1); ++nl;
-            if (mlp_launch(e->mlp[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-            launch_add_rmsnorm(e->x, part_f32(e->part_down, e->mlp_slices, B, d.hidden), (const __nv_bfloat16*)nw, e->xn, B,
-                               d.hidden, d.rms_eps, s); ++nl;
+        if (!e->fuse_mlp) {
+            if (enqueue_o_mlp(e, l, B, s, &nl) != RR_OK) return RR_CUDA_ERROR;
             continue;
         }
+        const void* nw = (l + 1 < L) ? e->norm_attn[l + 1] : e->final_norm;
+        if (gemm_launch(e->pl_o[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         launch_add_rmsnorm(e->x, part_f32(e->part_o, e->s_o, B, d.hidden), (const __nv_bfloat16*)e->norm_mlp[l],
-                           e->xn, B, d.hidden, d.rms_eps, s); ++nl;
-        if (gemm_launch(e->pl_gu[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (!e->fuse_silu) { launch_silu_mul(part_f32(e->part_gu, e->s_gu, B, 2 * d.inter), e->act, B, d.inter, s); ++nl; }
-        if (gemm_launch(e->pl_down[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        launch_add_rmsnorm(e->x, part_f32(e->part_down, e->s_down, B, d.hidden), (const __nv_bfloat16*)nw, e->xn, B,
+                           e->xn, B, d.hidden, d.rms_eps, s, e->mlp_ready, e->mlp_slices + 1); ++nl;
+        if (mlp_launch(e->mlp[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        launch_add_rmsnorm(e->x, part_f32(e->part_down, e->mlp_slices, B, d.hidden), (const __nv_bfloat16*)nw, e->xn, B,
                            d.hidden, d.rms_eps, s); ++nl;
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-    if (pen) {
-        PenaltyArgs a = pen_args(e->d_pen, B, PEN_MAX_BIAS);
-        a.hist = e->d_hist; a.hist_ld = e->o.ctx_max; a.app_tok = e->d_tok; a.app_pos = e->d_pos;
-        launch_logit_penalties(e->logits, d.vocab, B, d.vocab, a, e->pen_ws, s); ++nl;
-    }
-    launch_argmax(part_f32(e->logits, 1, B, d.vocab), B, d.vocab, e->d_tok, nullptr, e->d_slot, e->d_pos, s); ++nl;
-    if (sample) { enqueue_sample(e, e->d_samp, B, B, e->d_pos, e->d_tok, s); nl += SAMPLE_LAUNCHES; }
-    if (logprobs) { enqueue_logprobs(e, e->d_topn, B, s, sample ? e->d_tok : nullptr); nl += LP_LAUNCHES; }
+    nl += enqueue_tail(e, e->d_rows, B, mode, e->d_tok, e->d_slot, e->d_pos, e->d_pos, e->d_hist, s);
     if (n_launch) *n_launch = nl;
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) { rr::note_cuda_error(err); return RR_CUDA_ERROR; }
@@ -413,7 +462,7 @@ static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uin
     cudaStream_t s = e->stream;
     cudaGraph_t g = nullptr;
     CK(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_decode_step(e, s, n_launch, mode & 1, mode & 2, mode & 4);
+    int rc = enqueue_decode_step(e, s, n_launch, mode);
     cudaError_t ce = cudaStreamEndCapture(s, &g);
     if (rc != RR_OK || ce != cudaSuccess) { rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
     CK(cudaGraphInstantiate(out, g, 0));
@@ -421,15 +470,13 @@ static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uin
     return RR_OK;
 }
 
-// logprobs: also run launch_logprobs for the rows with d_topn >= 0; sample: also draw the rows with temperature > 0; pen:
-// also process the logits of the rows with penalties or a logit bias.  Each combination has its own graph, captured on
-// first use; a step without logprobs, sampled or processed rows replays the plain graph.
-static int run_decode_step(rr_engine* e, bool logprobs = false, bool sample = false, bool pen = false) {
+// mode: the step_mode bits of the active rows (enqueue_tail).  Each combination has its own graph, captured on first use;
+// a step without logprobs, sampled or processed rows replays the plain graph.
+static int run_decode_step(rr_engine* e, int mode) {
     cudaStream_t s = e->stream;
-    const int mode = step_mode(logprobs, sample, pen);
     if (!e->warmed || !e->o.use_cuda_graph) {
         uint64_t nl = 0;
-        int rc = enqueue_decode_step(e, s, &nl, logprobs, sample, pen);
+        int rc = enqueue_decode_step(e, s, &nl, mode);
         if (rc != RR_OK) return rc;
         e->step_launches[mode] = nl;
         e->st.kernel_launches += nl;
@@ -455,12 +502,12 @@ static int run_decode_step(rr_engine* e, bool logprobs = false, bool sample = fa
 }
 
 // ---------------------------------------------------------------- prefill chunk
-static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
-    auto it = e->pf_plans.find(T);
-    if (it != e->pf_plans.end()) { *out = &it->second; return RR_OK; }
+// One set of plans (4 L TMA descriptors) built for Tmax rows; the live row count is a launch argument: TMA reads of
+// rows >= T stay inside the Tmax-row buffers and every store is guarded by rowsA.
+static int init_pf_plans(rr_engine* e) {
     const rr_model_desc& d = e->d;
-    rr_engine::PfPlans P;
-    const int L = d.n_layers;
+    rr_engine::PfPlans& P = e->pf;
+    const int L = d.n_layers, T = e->Tmax;
     P.qkv.resize(L); P.o.resize(L); P.gu.resize(L); P.down.resize(L);
     for (int l = 0; l < L; ++l) {
         int rc = gemm_plan_init(&P.qkv[l], e->pxn, T, d.hidden, e->wqkv[l], e->nqkv, d.hidden, d.hidden, e->pqkv,
@@ -493,8 +540,6 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
         pf_norm_producer(&P.down[l].rope, (const __nv_bfloat16*)(l + 1 < L ? e->norm_attn[l + 1] : e->final_norm), e->pxn,
                          e->p_rowss, d.hidden);
     }
-    auto ins = e->pf_plans.emplace(T, std::move(P));
-    *out = &ins.first->second;
     return RR_OK;
 }
 
@@ -502,13 +547,14 @@ static int get_pf_plans(rr_engine* e, int T, rr_engine::PfPlans** out) {
 // activates the rows. Caller holds gpu_mu.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
-// gen[n_seqs] (optional): each sequence's request parameters.  A logit bias is added to the logits before the argmax and
-// the sampler (penalties count generated tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled
-// sequence draws its first token with rr_op_sample at position pos0[i] + its length (the prompt length).  A logprobs
-// sequence also gets its first token's logprobs in e->h_lp / e->h_lp_id row i, and if sampled its own logprob in h_tok_lp.
+// gen[n_seqs] (with mode): each sequence's request parameters, and mode = the step_mode bits over them, for the logits
+// tail on the chunk's rows.  Only a logit bias applies (penalties count generated tokens only, so the first token has
+// none; needs ensure_pen_buffers).  A sampled sequence draws its first token at position pos0[i] + its length (the prompt
+// length).  A logprobs sequence also gets its first token's logprobs in e->h_lp / e->h_lp_id row i, and if sampled its
+// own logprob in h_tok_lp.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
-                       const KvCopyList* copies = nullptr, const GenParams* const* gen = nullptr) {
+                       const KvCopyList* copies = nullptr, const GenParams* const* gen = nullptr, int mode = 0) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
@@ -534,17 +580,22 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (kv_copy_check(*copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
         for (int i = 0; i < copies->count; ++i) copy_tokens += copies->n[i];
     }
+    // the chunk's parameter blocks, at the stride of its sequences and of its largest bias count
+    int max_bias = 0;
+    for (int i = 0; (mode & 4) && i < n_seqs; ++i) max_bias = std::max(max_bias, (int)gen[i]->bias_id.size());
+    if (max_bias == 0) mode &= ~4;
+    else if (!e->d_pf.blk[2]) return RR_INTERNAL;
+    const ParamBlocks hp = e->h_pf.at(n_seqs, max_bias), dp = e->d_pf.at(n_seqs, max_bias);
+    for (int i = 0; mode && i < n_seqs; ++i)
+        hp.put_row(i, *gen[i], (pos0 ? pos0[i] : 0) + seq_start[i + 1] - seq_start[i], 0.f, 0.f, 0);
     CK(cudaEventRecord(e->ev0, s));
     CK(cudaMemcpyAsync(e->p_ids, h, n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     e->st.h2d_bytes += n_ints * sizeof(int32_t);
+    CK(hp.upload(dp, mode, s, &e->st.h2d_bytes));
     int32_t *p_ids = e->p_ids, *p_pos = p_ids + T, *p_slt = p_ids + 2 * T, *p_ss = p_ids + 3 * T,
             *p_sl = p_ss + n_seqs + 1, *p_last = p_sl + n_seqs, *p_p0 = p_last + n_seqs;
 
-    // One set of plans (4 L TMA descriptors) built for Tmax rows; the live row count is a launch argument: TMA reads of
-    // rows >= T stay inside the Tmax-row buffers and every store is guarded by rowsA.
-    rr_engine::PfPlans* P = nullptr;
-    int rc = get_pf_plans(e, e->Tmax, &P);
-    if (rc != RR_OK) return rc;
+    rr_engine::PfPlans& P = e->pf;
     auto launch_rows = [&](const GemmPlan& pl) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s); };
     uint64_t nl = 0;
     if (copy_tokens) {      // cached prefixes of busy slots into this chunk's slots, before any layer reads them
@@ -560,9 +611,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         __nv_bfloat16* kc = e->kcache + (size_t)l * e->kv_layer_stride;
         __nv_bfloat16* vc = e->vcache + (size_t)l * e->kv_layer_stride;
         if (e->fuse_rope_pf) {
-            P->qkv[l].rope.slot = p_slt; P->qkv[l].rope.pos = p_pos;
+            P.qkv[l].rope.slot = p_slt; P.qkv[l].rope.pos = p_pos;
         }
-        if (launch_rows(P->qkv[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        if (launch_rows(P.qkv[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         RopeArgs ra;
         ra.qkv = part_bf16(e->pqkv, e->nqkv);
         ra.q_out = e->pq; ra.k_cache = kc; ra.v_cache = vc; ra.slot = p_slt; ra.pos = p_pos; ra.rows = T;
@@ -575,76 +626,25 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         pa.ctx_max = e->o.ctx_max; pa.scale = 1.0f / sqrtf((float)d.head_dim); pa.head_dim = d.head_dim;
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (l + 1 == d.n_layers) {
-            // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers)
-            const int B = e->Bm;
+            // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers).  The
+            // unfused kernels even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
             launch_pdl(gather_last_kernel, dim3(n_seqs), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
                        (const int32_t*)p_last, e->attn_out, e->x, e->nq, d.hidden); ++nl;
-            if (gemm_launch(e->pl_o[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-            launch_add_rmsnorm(e->x, part_f32(e->part_o, e->s_o, B, d.hidden), (const __nv_bfloat16*)e->norm_mlp[l], e->xn,
-                               n_seqs, d.hidden, d.rms_eps, s); ++nl;
-            if (gemm_launch(e->pl_gu[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-            if (!e->fuse_silu) { launch_silu_mul(part_f32(e->part_gu, e->s_gu, B, 2 * d.inter), e->act, n_seqs, d.inter, s); ++nl; }
-            if (gemm_launch(e->pl_down[l], s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-            launch_add_rmsnorm(e->x, part_f32(e->part_down, e->s_down, B, d.hidden), (const __nv_bfloat16*)e->final_norm, e->xn,
-                               n_seqs, d.hidden, d.rms_eps, s); ++nl;
+            if (enqueue_o_mlp(e, l, n_seqs, s, &nl) != RR_OK) return RR_CUDA_ERROR;
             break;
         }
-        if (launch_rows(P->o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (launch_rows(P->gu[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        if (launch_rows(P.o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        if (launch_rows(P.gu[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->fuse_silu) { launch_silu_mul(part_bf16(e->pgu, 2 * d.inter), e->pact, T, d.inter, s); ++nl; }
-        if (launch_rows(P->down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        if (launch_rows(P.down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
-    int max_bias = 0;
-    bool samp = false, lp = false;
-    for (int i = 0; gen && i < n_seqs; ++i) {
-        if ((int)gen[i]->bias_id.size() > max_bias) max_bias = (int)gen[i]->bias_id.size();
-        samp = samp || gen[i]->sampled();
-        lp = lp || gen[i]->logprobs();
-    }
-    if (max_bias > 0) {
-        if (!e->d_pen) return RR_INTERNAL;
-        for (int i = 0; i < n_seqs; ++i) pen_fill_row(e->h_pen_pf, n_seqs, max_bias, i, *gen[i], 0.f, 0.f, 0);
-        const size_t nb = pen_bytes(n_seqs, max_bias);
-        CK(cudaMemcpyAsync(e->d_pen_pf, e->h_pen_pf, nb, cudaMemcpyHostToDevice, s));
-        e->st.h2d_bytes += nb;
-        launch_logit_penalties(e->logits, d.vocab, n_seqs, d.vocab, pen_args(e->d_pen_pf, n_seqs, max_bias), e->pen_ws, s);
-        ++nl;
-    }
-    launch_argmax(part_f32(e->logits, 1, e->Bm, d.vocab), n_seqs, d.vocab, e->p_first, nullptr, nullptr, nullptr, s); ++nl;
-    if (samp) {
-        char* h = e->h_samp_pf;
-        const size_t n = (size_t)n_seqs;
-        for (int i = 0; i < n_seqs; ++i) {
-            ((uint64_t*)h)[i] = gen[i]->seed;
-            ((float*)(h + 8 * n))[i] = gen[i]->temp;
-            ((float*)(h + 12 * n))[i] = gen[i]->top_p;
-            ((int32_t*)(h + 16 * n))[i] = (pos0 ? pos0[i] : 0) + seq_start[i + 1] - seq_start[i];
-        }
-        CK(cudaMemcpyAsync(e->d_samp_pf, h, SAMP_PF_BYTES * n, cudaMemcpyHostToDevice, s));
-        e->st.h2d_bytes += SAMP_PF_BYTES * n;
-        enqueue_sample(e, e->d_samp_pf, n_seqs, n_seqs, (const int32_t*)(e->d_samp_pf + 16 * n), e->p_first, s);
-        nl += SAMPLE_LAUNCHES;
-    }
+    nl += enqueue_tail(e, dp, n_seqs, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s);
     launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
                (const int32_t*)e->p_first, (const int32_t*)p_pos, (const int32_t*)p_last, n_seqs, e->d_tok, e->d_pos,
                e->d_slot); ++nl;
-    if (lp) {
-        for (int i = 0; i < n_seqs; ++i) e->h_topn_pf[i] = gen[i]->top_lp;
-        CK(cudaMemcpyAsync(e->d_topn_pf, e->h_topn_pf, sizeof(int32_t) * n_seqs, cudaMemcpyHostToDevice, s));
-        e->st.h2d_bytes += sizeof(int32_t) * n_seqs;
-        enqueue_logprobs(e, e->d_topn_pf, n_seqs, s, samp ? e->p_first : nullptr); nl += LP_LAUNCHES;
-        const size_t n = (size_t)n_seqs * LP_MAX_TOP;
-        CK(cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
-        e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
-        if (samp) {
-            CK(cudaMemcpyAsync(e->h_tok_lp, e->d_tok_lp, sizeof(float) * n_seqs, cudaMemcpyDeviceToHost, s));
-            e->st.d2h_bytes += sizeof(float) * n_seqs;
-        }
-    }
-    CK(cudaMemcpyAsync(e->h_tok, e->p_first, sizeof(int32_t) * n_seqs, cudaMemcpyDeviceToHost, s));
-    e->st.d2h_bytes += sizeof(int32_t) * n_seqs;
+    const int rc = enqueue_readback(e, e->p_first, n_seqs, mode, s);
+    if (rc != RR_OK) return rc;
     if (logits_host) {
         CK(cudaMemcpyAsync(logits_host, e->logits, sizeof(float) * (size_t)n_seqs * d.vocab, cudaMemcpyDeviceToHost, s));
     }
@@ -667,51 +667,21 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
 // ---------------------------------------------------------------- worker (continuous batching)
 struct DoneNote { uint64_t tag, ticket; int status, n_gen; };
 
-// Caller holds e->mu.  Appends row `row` of h_lp / h_lp_id to the request's pairs, and for a sampled request the pair of
-// the token it just generated (h_tok_lp).
-static void record_logprobs(rr_engine* e, Request* r, int row) {
-    const int k = r->gen.top_lp > 1 ? r->gen.top_lp : 1;
-    const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
-    const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
-    r->lp.insert(r->lp.end(), v, v + k);
-    r->lp_id.insert(r->lp_id.end(), id, id + k);
-    if (r->gen.sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
-}
-
-// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): write row b of each parameter block's mirror from
-// r's parameters or the defaults.  A block is marked dirty only when the row uses it before or after: the other rows of a
-// mirror hold the defaults, as a request that does not use the block does (GenParams::set), so they never need a copy.
+// Caller holds e->mu.  Decode row b is taken (r) or freed (nullptr): write row b of the mirror from r's parameters or the
+// defaults.  A block is marked dirty only when the row uses it before or after: the other rows of a mirror hold the
+// defaults, as a request that does not use the block does (GenParams::set), so they never need a copy.  A freed row's
+// mirror row holds the defaults, so freeing a row that never held parameters changes nothing.
 static void set_row_params(rr_engine* e, int b, const Request* r) {
     static const GenParams plain;
     const GenParams& p = r ? r->gen : plain;
-    const size_t B = (size_t)e->Bm;
-    if (e->h_topn[b] >= 0 || p.logprobs()) e->topn_dirty = true;
-    e->h_topn[b] = p.top_lp;
-    float* temp = (float*)(e->h_samp + 8 * B);
-    if (temp[b] > 0.f || p.sampled()) e->samp_dirty = true;
-    ((uint64_t*)e->h_samp)[b] = p.seed; temp[b] = p.temp; ((float*)(e->h_samp + 12 * B))[b] = p.top_p;
-    if (!e->h_pen) return;     // allocated with d_pen on the first processed request: every row is unprocessed until then
-    const bool was = ((const float*)e->h_pen)[b] != 0.f || ((const float*)(e->h_pen + 4 * B))[b] != 0.f ||
-                     ((const int32_t*)(e->h_pen + 12 * B))[b] != 0;
-    if (was || p.processed()) {
-        pen_fill_row(e->h_pen, (int)B, PEN_MAX_BIAS, b, p, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
-        e->pen_dirty = true;
-    }
+    e->rows_dirty |= e->h_rows.row_mode(b) | step_mode(p);
+    e->h_rows.put_row(b, p, 0, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
 }
 
 // Before a decode step: copy each parameter block the step reads (step_mode bits) whose mirror changed.
 static void upload_row_params(rr_engine* e, int mode) {
-    const size_t B = (size_t)e->Bm;
-    struct { bool* dirty; void* d; const void* h; size_t bytes; } blk[3] = {
-        {&e->topn_dirty, e->d_topn, e->h_topn, sizeof(int32_t) * B},
-        {&e->samp_dirty, e->d_samp, e->h_samp, SAMP_BYTES * B},
-        {&e->pen_dirty, e->d_pen, e->h_pen, pen_bytes(e->Bm, PEN_MAX_BIAS)}};
-    for (int i = 0; i < 3; ++i) {
-        if (!(mode >> i & 1) || !*blk[i].dirty) continue;
-        *blk[i].dirty = false;
-        cudaMemcpyAsync(blk[i].d, blk[i].h, blk[i].bytes, cudaMemcpyHostToDevice, e->stream);
-        e->st.h2d_bytes += blk[i].bytes;
-    }
+    e->h_rows.upload(e->d_rows, mode & e->rows_dirty, e->stream, &e->st.h2d_bytes);
+    e->rows_dirty &= ~mode;
 }
 
 // Caller holds e->mu.  Returns the hook call to make once the lock is released (tag == 0 and no hook: nothing).
@@ -728,6 +698,31 @@ static void finish_request(rr_engine* e, Request* r, int status, std::vector<Don
 static void run_hooks(rr_engine* e, std::vector<DoneNote>& notes) {
     for (const DoneNote& n : notes) e->hook(e->hook_ctx, n.tag, n.ticket, n.status, n.n_gen);
     notes.clear();
+}
+
+// Caller holds e->mu.  Frees decode row b (inactive from the next step, parameters back to the defaults) and finishes its
+// request with `status`.
+static void release_row(rr_engine* e, int b, int status, std::vector<DoneNote>* notes) {
+    Request* r = e->row_req[b];
+    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
+    set_row_params(e, b, nullptr);
+    finish_request(e, r, status, notes);
+}
+
+// Caller holds e->mu.  Appends the token read back for row `row` to r, with its pairs (h_lp / h_lp_id row `row`, and for
+// a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  True once r has max_new tokens.
+static bool take_token(rr_engine* e, Request* r, int row) {
+    r->out.push_back(e->h_tok[row]);
+    if (r->gen.logprobs()) {
+        const int k = r->gen.top_lp > 1 ? r->gen.top_lp : 1;
+        const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
+        const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
+        r->lp.insert(r->lp.end(), v, v + k);
+        r->lp_id.insert(r->lp_id.end(), id, id + k);
+        if (r->gen.sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
+    }
+    e->st.generated_tokens += 1;
+    return (int)r->out.size() >= r->max_new;
 }
 
 // Caller holds e->mu.  Prefix caching: the slot a prompt p is admitted into and how many of its tokens are cached there.
@@ -785,22 +780,19 @@ static void worker_main(rr_engine* e) {
         chunk.clear(); gen.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
         copies->count = 0;
         int active = 0;
-        bool lp_step = false, samp_step = false, pen_step = false, pen_chunk = false;
+        int step = 0, chunk_mode = 0;                      // step_mode bits of the active rows / of the chunk's requests
         uint64_t epoch = 0;
         {
             std::unique_lock<std::mutex> lk(e->mu);
             for (int b = 0; b < e->Bm; ++b) {
                 Request* r = e->row_req[b];
-                if (r && r->cancel) {                      // rr_engine_cancel: free the row, keep what was generated
-                    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_params(e, b, nullptr);
-                    finish_request(e, r, RR_CANCELLED, &notes);
+                if (!r) continue;
+                if (r->cancel) {                           // rr_engine_cancel: free the row, keep what was generated
+                    release_row(e, b, RR_CANCELLED, &notes);
                     continue;
                 }
-                active += r != nullptr;
-                lp_step = lp_step || (r && r->gen.logprobs());
-                samp_step = samp_step || (r && r->gen.sampled());
-                pen_step = pen_step || (r && r->gen.processed());
+                ++active;
+                step |= step_mode(r->gen);
             }
             if (e->waiting.empty() && active == 0) {
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
@@ -834,7 +826,7 @@ static void worker_main(rr_engine* e) {
                 chunk.push_back(r);
                 gen.push_back(&r->gen);
                 slots.push_back(b);
-                pen_chunk = pen_chunk || r->gen.processed();
+                chunk_mode |= step_mode(r->gen);
                 ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
                 ++active;
@@ -859,18 +851,16 @@ static void worker_main(rr_engine* e) {
             }
         }
         if (!chunk.empty()) {
-            int rc = pen_chunk ? ensure_pen_buffers(e) : RR_OK;
+            int rc = (chunk_mode & 4) ? ensure_pen_buffers(e) : RR_OK;
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, gen.data());
+                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, gen.data(), chunk_mode);
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0; i < chunk.size(); ++i) {
                 Request* r = chunk[i];
                 if (rc != RR_OK) {
-                    e->row_req[r->slot] = nullptr;
-                    e->h_slot_mirror[r->slot] = -1; e->slots_dirty = true;
-                    finish_request(e, r, RR_INTERNAL, &notes);
+                    release_row(e, r->slot, RR_INTERNAL, &notes);
                     continue;
                 }
                 if (e->o.prefix_cache) {
@@ -879,16 +869,8 @@ static void worker_main(rr_engine* e) {
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
                 r->t_first = t;
-                r->out.push_back(e->h_tok[i]);
-                if (r->gen.logprobs()) record_logprobs(e, r, (int)i);
-                e->st.generated_tokens += 1;
-                if ((int)r->out.size() >= r->max_new) {
-                    e->row_req[r->slot] = nullptr;
-                    e->h_slot_mirror[r->slot] = -1; e->slots_dirty = true;
-                    finish_request(e, r, RR_OK, &notes);
-                } else {
-                    set_row_params(e, r->slot, r);
-                }
+                if (take_token(e, r, (int)i)) release_row(e, r->slot, RR_OK, &notes);
+                else set_row_params(e, r->slot, r);
             }
             e->cv_done.notify_all();
             continue;   // look for more waiting prompts before decoding
@@ -902,23 +884,13 @@ static void worker_main(rr_engine* e) {
             e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
             e->slots_dirty = false;
         }
-        upload_row_params(e, step_mode(lp_step, samp_step, pen_step));
+        upload_row_params(e, step);
         cudaEventRecord(e->ev0, s);
-        int rc = run_decode_step(e, lp_step, samp_step, pen_step);
+        int rc = run_decode_step(e, step);
         cudaEventRecord(e->ev1, s);
-        cudaMemcpyAsync(e->h_tok, e->d_tok, sizeof(int32_t) * e->Bm, cudaMemcpyDeviceToHost, s);
-        if (lp_step) {
-            const size_t n = (size_t)e->Bm * LP_MAX_TOP;
-            cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s);
-            cudaMemcpyAsync(e->h_lp_id, e->d_lp_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s);
-            e->st.d2h_bytes += (sizeof(float) + sizeof(int32_t)) * n;
-            if (samp_step) {
-                cudaMemcpyAsync(e->h_tok_lp, e->d_tok_lp, sizeof(float) * e->Bm, cudaMemcpyDeviceToHost, s);
-                e->st.d2h_bytes += sizeof(float) * e->Bm;
-            }
-        }
+        const int rb = enqueue_readback(e, e->d_tok, e->Bm, step, s);     // outside ev0 .. ev1: decode_ms_total excludes it
+        if (rc == RR_OK) rc = rb;
         cudaError_t se = cudaStreamSynchronize(s);
-        e->st.d2h_bytes += sizeof(int32_t) * e->Bm;
         if (se != cudaSuccess) { rr::note_cuda_error(se); rc = RR_CUDA_ERROR; }
         float ms = 0;
         cudaEventElapsedTime(&ms, e->ev0, e->ev1);
@@ -929,20 +901,8 @@ static void worker_main(rr_engine* e) {
             for (int b = 0; b < e->Bm; ++b) {
                 Request* r = e->row_req[b];
                 if (!r) continue;
-                if (rc != RR_OK) {
-                    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_params(e, b, nullptr);
-                    finish_request(e, r, RR_INTERNAL, &notes);
-                    continue;
-                }
-                r->out.push_back(e->h_tok[b]);
-                if (r->gen.logprobs()) record_logprobs(e, r, b);
-                e->st.generated_tokens += 1;
-                if ((int)r->out.size() >= r->max_new) {
-                    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-                    set_row_params(e, b, nullptr);
-                    finish_request(e, r, RR_OK, &notes);
-                }
+                if (rc != RR_OK) release_row(e, b, RR_INTERNAL, &notes);
+                else if (take_token(e, r, b)) release_row(e, b, RR_OK, &notes);
             }
         }
         e->cv_done.notify_all();
@@ -1013,7 +973,6 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     }
     TRY(dalloc(e, &e->part_down, (size_t)(e->s_down > e->mlp_slices ? e->s_down : e->mlp_slices) * B * d.hidden));
     TRY(dalloc(e, &e->logits, (size_t)B * d.vocab));
-    TRY(dalloc(e, &e->xn_last, (size_t)B * d.hidden));
     TRY(dalloc(e, &e->rope_table, (size_t)opts->ctx_max * 64));
     launch_rope_table(e->rope_table, opts->ctx_max, d.rope_theta, d.head_dim, e->stream);
     e->kv_layer_stride = (size_t)B * d.n_kv_heads * opts->ctx_max * 128;
@@ -1033,27 +992,28 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->pqkv, (size_t)T * e->nqkv, false));
     TRY(dalloc(e, &e->pq, (size_t)T * d.n_heads * 128));                 // zeroed: columns beyond head_dim stay 0
     TRY(dalloc(e, &e->pattn, (size_t)T * e->nq, false));
-    TRY(dalloc(e, &e->po, (size_t)T * d.hidden, false));
     TRY(dalloc(e, &e->pgu, (size_t)T * 2 * d.inter, false));
     TRY(dalloc(e, &e->pact, (size_t)T * d.inter, false));
-    e->h_stage_ints = (size_t)3 * T + 4 * B + 8;
-    TRYC(cudaMallocHost(&e->h_stage, e->h_stage_ints * sizeof(int32_t)));
+    TRYC(cudaMallocHost(&e->h_stage, ((size_t)3 * T + 4 * B + 8) * sizeof(int32_t)));
     TRYC(cudaMallocHost(&e->h_tok, sizeof(int32_t) * (B > 16 ? B : 16)));
-    TRY(dalloc(e, &e->d_topn, B)); TRY(dalloc(e, &e->d_topn_pf, B));
-    TRYC(cudaMemset(e->d_topn, 0xff, sizeof(int32_t) * B));
     TRY(dalloc(e, (char**)&e->lp_ws, logprobs_ws_bytes(B, d.vocab), false));
     TRY(dalloc(e, &e->d_lp, (size_t)B * LP_MAX_TOP)); TRY(dalloc(e, &e->d_lp_id, (size_t)B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_lp, sizeof(float) * B * LP_MAX_TOP));
     TRYC(cudaMallocHost(&e->h_lp_id, sizeof(int32_t) * B * LP_MAX_TOP));
-    TRYC(cudaMallocHost(&e->h_topn, sizeof(int32_t) * B)); TRYC(cudaMallocHost(&e->h_topn_pf, sizeof(int32_t) * B));
-    memset(e->h_topn, 0xff, sizeof(int32_t) * B);                 // the mirrors start as their device blocks
-    TRY(dalloc(e, &e->d_samp, (size_t)SAMP_BYTES * B));           // zero: every row greedy
-    TRY(dalloc(e, &e->d_samp_pf, (size_t)SAMP_PF_BYTES * B));
     TRY(dalloc(e, (char**)&e->sample_ws, sample_ws_bytes(B, d.vocab), false));
     TRY(dalloc(e, &e->d_tok_lp, B));
-    TRYC(cudaMallocHost(&e->h_samp, (size_t)SAMP_BYTES * B)); TRYC(cudaMallocHost(&e->h_samp_pf, (size_t)SAMP_PF_BYTES * B));
-    memset(e->h_samp, 0, (size_t)SAMP_BYTES * B);
     TRYC(cudaMallocHost(&e->h_tok_lp, sizeof(float) * B));
+    // top_n and samp blocks (pen: ensure_pen_buffers), all zero but the decode rows' top_n and its mirror, which start at -1:
+    // every row plain (no logprobs, greedy), as the mirror is
+    e->d_rows.n = B; e->d_rows.bias_ld = PEN_MAX_BIAS;
+    e->d_pf = e->d_rows; e->d_pf.has_pos = true;
+    e->h_rows = e->d_rows; e->h_pf = e->d_pf;
+    for (ParamBlocks* p : {&e->d_rows, &e->d_pf})
+        for (int i = 0; i < 2; ++i) TRY(dalloc(e, &p->blk[i], p->bytes(i)));
+    for (ParamBlocks* p : {&e->h_rows, &e->h_pf})
+        for (int i = 0; i < 2; ++i) { TRYC(cudaMallocHost(&p->blk[i], p->bytes(i))); memset(p->blk[i], 0, p->bytes(i)); }
+    TRYC(cudaMemset(e->d_rows.top_n(), 0xff, e->d_rows.bytes(0)));
+    memset(e->h_rows.top_n(), 0xff, e->h_rows.bytes(0));
 
     e->pl_qkv.resize(L); e->pl_o.resize(L); e->pl_gu.resize(L); e->pl_down.resize(L);
     e->attn_args.resize(L);
@@ -1090,13 +1050,12 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     }
     TRY(gemm_plan_init(&e->pl_head, e->lm_head, d.vocab, d.hidden, e->xn, B, d.hidden, d.hidden, e->logits, d.vocab,
                        B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
-    TRY(gemm_plan_init(&e->pl_head_pf, e->lm_head, d.vocab, d.hidden, e->xn_last, B, d.hidden, d.hidden, e->logits,
-                       d.vocab, B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
     e->fuse_rope_pf = pf_rope_fused(d.head_dim);
     // deferred prefill RMSNorm: hidden % 64 == 0 and hidden <= 8192 (checked above) give the 16-byte rows and the <= 64 partial
     // sums per row that the residual epilogue writes
     e->pf_parts = pf_norm_parts(d.hidden);
     TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
+    TRY(init_pf_plans(e));
     if (e->fuse_mlp) {
         std::vector<MlpItem> sched;
         const int grid = num_sms();
@@ -1136,13 +1095,10 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_tok) cudaFreeHost(e->h_tok);
     if (e->h_lp) cudaFreeHost(e->h_lp);
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
-    if (e->h_topn) cudaFreeHost(e->h_topn);
-    if (e->h_topn_pf) cudaFreeHost(e->h_topn_pf);
-    if (e->h_samp) cudaFreeHost(e->h_samp);
-    if (e->h_samp_pf) cudaFreeHost(e->h_samp_pf);
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
-    if (e->h_pen) cudaFreeHost(e->h_pen);
-    if (e->h_pen_pf) cudaFreeHost(e->h_pen_pf);
+    for (const ParamBlocks* p : {&e->h_rows, &e->h_pf})
+        for (char* b : p->blk)
+            if (b) cudaFreeHost(b);
     if (e->ev0) cudaEventDestroy(e->ev0);
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->stream) cudaStreamDestroy(e->stream);

@@ -57,7 +57,7 @@ struct GemmPlan {
     int tma_epi;              // 1: the epilogue stages the tile in shared memory and issues ONE TMA store per item
 };
 
-// ---- prefill decisions shared by the engine (get_pf_plans, run_prefill) and the kernel-level entry points (rr_api.cu)
+// ---- prefill decisions shared by the engine (init_pf_plans, run_prefill) and the kernel-level entry points (rr_api.cu)
 // RoPE and the KV append run in the QKV GEMM's epilogue (OUT_ROWMAJOR_ROPE) only at head_dim 128, where a head is half of a
 // 256-wide tile; other head dims take OUT_ROWMAJOR_BF16 into a qkv matrix, then rope_kv_kernel.
 inline bool pf_rope_fused(int head_dim) { return head_dim == 128; }
