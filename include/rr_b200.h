@@ -482,7 +482,8 @@ int rr_engine_reset_stats(rr_engine* e);
  *    rr_gateway_submit is thread-safe and non-blocking: the request enters an admission queue; a dispatcher
  *    thread coalesces everything pending (ADMIT / DONE / FAIL / fallback re-ADMIT) into ONE ordered trace per
  *    K1 launch (rr_router_process) and hands admitted prompts straight to the engine of the picked
- *    deployment.  A backend failure walks the fallback chain inside the library. */
+ *    deployment, or serves them itself on a mock replica (rr_stub_desc).  A backend failure walks the fallback chain
+ *    inside the library. */
 
 typedef struct rr_gateway rr_gateway;
 
@@ -514,10 +515,21 @@ typedef struct rr_gateway_stats {
     double admit_wait_s;       /* sum over admissions of (decision time - submit time) */
 } rr_gateway_stats;
 
-/* engines[i] serves the deployments whose rr_deployment_desc.replica == replica_ids[i].  The router and the engines
- * must outlive the gateway; the engines' completion hooks are taken by the gateway until it is destroyed. */
+/* A mock-completion replica, served by the gateway itself in place of an engine.  The n-th request handed to it (n from 1,
+ * per replica and gateway) fails without tokens when fail_every > 0 and n % fail_every == 0; any other completes with
+ * min(max_new_tokens, reply_tokens) tokens 3 + (i % 200).  Generation parameters are ignored. */
+typedef struct rr_stub_desc {
+    int32_t reply_tokens, fail_every, vocab, reserved;
+} rr_stub_desc;
+
+/* engines[i] serves the deployments whose rr_deployment_desc.replica == replica_ids[i]; engines[i] == NULL makes that
+ * replica a mock one described by stubs[i] (stubs is read only there and may be NULL when no engine is NULL).
+ * RR_INVALID_ARGUMENT, with nothing created, for a NULL engine without a descriptor, reply_tokens < 0, fail_every < 0 or
+ * vocab < 1.  A mock replica's vocab counts toward the smallest vocabulary; it sets no context or prefill limit.  A
+ * gateway with a mock replica refuses logprobs (top_logprobs >= 0) at submit with RR_INVALID_ARGUMENT.  The router and
+ * the engines must outlive the gateway; the engines' completion hooks are taken by the gateway until it is destroyed. */
 int rr_gateway_create(rr_router* router, rr_engine* const* engines, const int32_t* replica_ids, int n_engines,
-                      const rr_gateway_opts* opts, rr_gateway** out);
+                      const rr_stub_desc* stubs, const rr_gateway_opts* opts, rr_gateway** out);
 void rr_gateway_destroy(rr_gateway* g);
 int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
 /* group = index of the model group (model_name) the client asked for.  Returns RR_NO_GROUP / RR_INVALID_ARGUMENT

@@ -103,6 +103,10 @@ class GatewayOpts(C.Structure):
                 ("reserved", C.c_int32 * 5)]
 
 
+class StubDesc(C.Structure):
+    _fields_ = [("reply_tokens", C.c_int32), ("fail_every", C.c_int32), ("vocab", C.c_int32), ("reserved", C.c_int32)]
+
+
 class GatewayResult(C.Structure):
     _fields_ = [("ticket", C.c_uint64), ("status", C.c_int32), ("deployment", C.c_int32), ("served_group", C.c_int32),
                 ("chain_pos", C.c_int32), ("replica", C.c_int32), ("n_prompt", C.c_int32), ("n_generated", C.c_int32),
@@ -195,7 +199,8 @@ PROTOTYPES = {
     "rr_engine_get_stats": (C.c_int, [vp, C.POINTER(EngineStats)]),
     "rr_engine_reset_stats": (C.c_int, [vp]),
     "rr_engine_cancel": (C.c_int, [vp, C.c_uint64]),
-    "rr_gateway_create": (C.c_int, [vp, C.POINTER(vp), c_i32p, C.c_int, C.POINTER(GatewayOpts), C.POINTER(vp)]),
+    "rr_gateway_create": (C.c_int, [vp, C.POINTER(vp), c_i32p, C.c_int, C.POINTER(StubDesc), C.POINTER(GatewayOpts),
+                                    C.POINTER(vp)]),
     "rr_gateway_destroy": (None, [vp]),
     "rr_gateway_set_now": (C.c_int, [vp, C.c_int64]),
     "rr_gateway_submit": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),

@@ -11,6 +11,8 @@
 // through a hook.  Concurrent admissions are therefore COALESCED: under a burst of N callers the path costs
 // ~N / batch launches instead of 2 N, and the serialised-trace semantics of K1 are unchanged (the trace is the
 // arrival order at the queue; it can be recorded and replayed through the oracle, tests/test_gateway_gpu.py).
+// A mock replica (rr_stub_desc) is served by the dispatcher itself at hand-off and settles through the same code as
+// the hook (gw_settle), so failure, fallback and cancellation are one path for both kinds of replica.
 //
 // Replaces: litellm.Router's async request handling behind the proxy (reference pyproject.toml:8,
 // config/config.yaml:100-108) for the call shape of reference src/demo_fallback.py:143-147.
@@ -49,7 +51,7 @@ struct GwReq {
     std::vector<float> lp;            // [tokens.size()][gen.lp_width()]
     std::vector<int32_t> lp_id;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
-    double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;
+    double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;   // t_eng_submit: hand-off to the replica
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
 };
 
@@ -65,7 +67,10 @@ struct Pending {
 
 struct rr_gateway {
     rr_router* router = nullptr;
-    std::vector<rr_engine*> engines;        // index = position in the create() arrays
+    std::vector<rr_engine*> engines;        // index = position in the create() arrays; nullptr: a mock replica
+    std::vector<rr_stub_desc> stubs;        // same index: the mock replicas' descriptors
+    std::vector<uint64_t> stub_handed;      // same index: requests handed to each mock replica so far
+    bool has_stub = false;
     std::unordered_map<int, int> by_replica;   // replica id -> index into engines
     int n_deps = 0, n_groups = 0;
     bool latency = false;                   // the router is latency-based: DONE / FAIL events carry samples
@@ -113,6 +118,57 @@ static void gw_finish(rr_gateway* g, GwReq* r, int status) {
     }
 }
 
+// caller holds g->mu.  Request r ended on the replica it was handed to with `status` (n_generated tokens by then).  When
+// the replica's record of it was read (wrc RR_OK / RR_BACKEND_FAILED: comp, toks, and with logprobs lps / lp_ids), the
+// result is stored.  Then DONE (with the latency sample) / FAIL / the cancel report is posted and the request finishes,
+// or after a backend failure goes back into the queue one step further down its fallback chain.
+static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int wrc, const rr_completion& comp,
+                      const int32_t* toks, const float* lps, const int32_t* lp_ids) {
+    const int dep = r->deployment;
+    if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
+        const int n = comp.n_generated < r->max_new ? comp.n_generated : r->max_new;
+        r->tokens.assign(toks, toks + (n > 0 ? n : 0));
+        if (r->gen.logprobs()) {
+            const size_t m = r->tokens.size() * (size_t)r->gen.lp_width();
+            r->lp.assign(lps, lps + m);
+            r->lp_id.assign(lp_ids, lp_ids + m);
+        }
+        r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
+        r->n_cached = comp.n_cached;
+    }
+    if (status == RR_OK) {
+        // latency sample: the replica's submit -> done time of the request, in microseconds
+        int lat_us = 0;
+        if (g->latency && wrc == RR_OK) {
+            const double us = std::round((comp.t_done_s - comp.t_submit_s) * 1e6);
+            lat_us = us < 1.0 ? 1 : (us > 2147483647.0 ? 2147483647 : (int)us);
+        }
+        g->pending.push_back(Pending{RR_EV_DONE, nullptr, dep, (int)r->tokens.size(), lat_us});
+        gw_finish(g, r, RR_OK);
+    } else if (status == RR_CANCELLED) {
+        // the owner gave up: a client-side timeout counts as a backend failure (cooldown), a disconnect does not;
+        // a latency-based router also records the timeout penalty for the deployment
+        g->pending.push_back(Pending{r->cancel_as_failure ? RR_EV_FAIL : RR_EV_DONE, nullptr, dep, n_generated,
+                                     g->latency && r->cancel_as_failure ? 1 : 0});
+        gw_finish(g, r, r->cancel_as_failure ? RR_TIMEOUT : RR_CANCELLED);
+    } else {
+        // backend failure: report it, then walk on down the fallback chain with the same request
+        g->pending.push_back(Pending{RR_EV_FAIL, nullptr, dep, 0});
+        if (r->cancelled) {
+            gw_finish(g, r, r->cancel_as_failure ? RR_TIMEOUT : RR_CANCELLED);
+        } else {
+            r->chain_start = r->chain_pos + 1;
+            r->state = Q_ADMIT;
+            r->eng = nullptr;
+            r->tokens.clear();
+            r->lp.clear(); r->lp_id.clear();
+            r->n_cached = 0;
+            g->st.failed_over++;
+            g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
+        }
+    }
+}
+
 // Engine worker thread (or the submitting thread for an injected failure): a request of ours finished on `eng`.
 static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status, int n_generated) {
     rr_gateway* g = (rr_gateway*)ctx;
@@ -146,52 +202,27 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
         if (it == g->table.end()) return;
-        r = it->second;
-        const int dep = r->deployment;
-        if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
-            const int n = comp.n_generated < max_new ? comp.n_generated : max_new;
-            r->tokens.assign(toks.begin(), toks.begin() + (n > 0 ? n : 0));
-            if (logprobs) {
-                r->lp.assign(lps.begin(), lps.begin() + r->tokens.size() * k);
-                r->lp_id.assign(lp_ids.begin(), lp_ids.begin() + r->tokens.size() * k);
-            }
-            r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
-            r->n_cached = comp.n_cached;
-        }
-        if (status == RR_OK) {
-            // latency sample: the engine's submit -> done time of the request, in microseconds
-            int lat_us = 0;
-            if (g->latency && wrc == RR_OK) {
-                const double us = std::round((comp.t_done_s - comp.t_submit_s) * 1e6);
-                lat_us = us < 1.0 ? 1 : (us > 2147483647.0 ? 2147483647 : (int)us);
-            }
-            g->pending.push_back(Pending{RR_EV_DONE, nullptr, dep, (int)r->tokens.size(), lat_us});
-            gw_finish(g, r, RR_OK);
-        } else if (status == RR_CANCELLED) {
-            // the owner gave up: a client-side timeout counts as a backend failure (cooldown), a disconnect does not;
-            // a latency-based router also records the timeout penalty for the deployment
-            g->pending.push_back(Pending{r->cancel_as_failure ? RR_EV_FAIL : RR_EV_DONE, nullptr, dep, n_generated,
-                                         g->latency && r->cancel_as_failure ? 1 : 0});
-            gw_finish(g, r, r->cancel_as_failure ? RR_TIMEOUT : RR_CANCELLED);
-        } else {
-            // backend failure: report it, then walk on down the fallback chain with the same request
-            g->pending.push_back(Pending{RR_EV_FAIL, nullptr, dep, 0});
-            if (r->cancelled) {
-                gw_finish(g, r, r->cancel_as_failure ? RR_TIMEOUT : RR_CANCELLED);
-            } else {
-                r->chain_start = r->chain_pos + 1;
-                r->state = Q_ADMIT;
-                r->eng = nullptr;
-                r->tokens.clear();
-                r->lp.clear(); r->lp_id.clear();
-                r->n_cached = 0;
-                g->st.failed_over++;
-                g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
-            }
-        }
+        gw_settle(g, it->second, status, n_generated, wrc, comp, toks.data(), lps.data(), lp_ids.data());
     }
     g->cv_work.notify_one();
     g->cv_done.notify_all();
+}
+
+// Dispatcher thread, caller holds g->mu: mock replica `rep` serves request r (handed to it at r->t_eng_submit) at once.
+// Its latency sample is the gateway's hand-off -> settle time.
+static void gw_serve_stub(rr_gateway* g, GwReq* r, int rep) {
+    const rr_stub_desc& s = g->stubs[(size_t)rep];
+    const uint64_t n = ++g->stub_handed[(size_t)rep];
+    const bool failed = s.fail_every > 0 && n % (uint64_t)s.fail_every == 0;
+    rr_completion comp;
+    memset(&comp, 0, sizeof(comp));
+    comp.n_generated = failed ? 0 : (r->max_new < s.reply_tokens ? r->max_new : s.reply_tokens);
+    std::vector<int32_t> toks((size_t)comp.n_generated);
+    for (int i = 0; i < comp.n_generated; ++i) toks[(size_t)i] = 3 + (i % 200);
+    comp.t_submit_s = r->t_eng_submit;
+    comp.t_first_token_s = comp.t_done_s = gw_now_s(g);
+    const int status = failed ? RR_BACKEND_FAILED : RR_OK;
+    gw_settle(g, r, status, comp.n_generated, status, comp, toks.data(), nullptr, nullptr);
 }
 
 static void gw_dispatch(rr_gateway* g) {
@@ -269,13 +300,15 @@ static void gw_dispatch(rr_gateway* g) {
         }
         for (GwReq* r : to_submit) {
             auto it = g->by_replica.find(r->replica);
-            rr_engine* eng = it == g->by_replica.end() ? nullptr : g->engines[it->second];
+            const int rep = it == g->by_replica.end() ? -1 : it->second;
+            rr_engine* eng = rep < 0 ? nullptr : g->engines[rep];
             const uint64_t id = r->id;           // `r` may be finished and freed by the done hook once it is submitted
             bool cancelled;
             {
                 std::lock_guard<std::mutex> lk(g->mu);
                 cancelled = r->cancelled;
                 if (!cancelled) { r->eng = eng; r->eng_ticket = 0; r->t_eng_submit = gw_now_s(g); }
+                if (!cancelled && rep >= 0 && !eng) { gw_serve_stub(g, r, rep); continue; }
             }
             uint64_t tk = 0;
             int src = RR_INTERNAL;
@@ -311,7 +344,7 @@ static void gw_dispatch(rr_gateway* g) {
 
 // ---------------------------------------------------------------------------------------------------- C-ABI
 RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const int32_t* replica_ids, int n_engines,
-                             const rr_gateway_opts* opts, rr_gateway** out) {
+                             const rr_stub_desc* stubs, const rr_gateway_opts* opts, rr_gateway** out) {
     if (!router || !engines || !replica_ids || n_engines < 1 || !out) return RR_INVALID_ARGUMENT;
     rr_gateway* g = new (std::nothrow) rr_gateway();
     if (!g) return RR_INTERNAL;
@@ -322,12 +355,23 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
     rr::router_shape(router, &g->n_deps, &g->n_groups);
     g->latency = rr::router_strategy(router) == RR_STRATEGY_LATENCY_BASED;
     g->min_ctx = g->min_pf = g->min_vocab = 0x7fffffff;
+    g->stubs.assign((size_t)n_engines, rr_stub_desc{0, 0, 0, 0});
+    g->stub_handed.assign((size_t)n_engines, 0);
     for (int i = 0; i < n_engines; ++i) {
-        if (!engines[i]) { delete g; return RR_INVALID_ARGUMENT; }
         g->engines.push_back(engines[i]);
         g->by_replica[replica_ids[i]] = i;
-        int c = 0, p = 0, v = 0;
-        rr::engine_limits(engines[i], &c, &p, &v);
+        int c = 0x7fffffff, p = 0x7fffffff, v = 0;
+        if (engines[i]) {
+            rr::engine_limits(engines[i], &c, &p, &v);
+        } else {
+            if (!stubs || stubs[i].reply_tokens < 0 || stubs[i].fail_every < 0 || stubs[i].vocab < 1) {
+                delete g;
+                return RR_INVALID_ARGUMENT;
+            }
+            g->stubs[(size_t)i] = stubs[i];
+            g->has_stub = true;
+            v = stubs[i].vocab;
+        }
         if (c < g->min_ctx) g->min_ctx = c;
         if (p < g->min_pf) g->min_pf = p;
         if (v < g->min_vocab) g->min_vocab = v;
@@ -337,7 +381,8 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
         g->tr_dec.resize((size_t)g->opts.record_trace);
     }
     g->t0 = std::chrono::steady_clock::now();
-    for (rr_engine* e : g->engines) rr::engine_set_done_hook(e, gw_on_done, g);
+    for (rr_engine* e : g->engines)
+        if (e) rr::engine_set_done_hook(e, gw_on_done, g);
     g->dispatcher = std::thread(gw_dispatch, g);
     *out = g;
     return RR_OK;
@@ -351,7 +396,8 @@ RR_API void rr_gateway_destroy(rr_gateway* g) {
     }
     g->cv_work.notify_all();
     if (g->dispatcher.joinable()) g->dispatcher.join();
-    for (rr_engine* e : g->engines) rr::engine_set_done_hook(e, nullptr, nullptr);
+    for (rr_engine* e : g->engines)
+        if (e) rr::engine_set_done_hook(e, nullptr, nullptr);
     for (auto& kv : g->table) delete kv.second;
     delete g;
 }
@@ -420,8 +466,10 @@ RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* 
     rr::GenParams p;
     const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
                          bias_ids, bias_vals);
+    if (rc != RR_OK) return rc;
+    if (p.logprobs() && g->has_stub) return RR_INVALID_ARGUMENT;     // a mock replica has no logits to fill the pairs from
     const int32_t start[2] = {0, n_prompt};
-    return rc != RR_OK ? rc : gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, ticket);
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, ticket);
 }
 
 RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,

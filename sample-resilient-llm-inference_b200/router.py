@@ -8,9 +8,11 @@ the demos make (reference src/demo_load_balancing.py:106-110, src/demo_fallback.
 src/demo_quota_isolation.py:52-56), the result exposes `.model` the way they read it (:116), and a
 rate-limited request raises `RateLimitError` (HTTP 429; src/demo_quota_isolation.py:80).
 
-All routing state and decisions live in the CUDA library (K1, rr_router.cu): this file builds event
-records, calls `rr_router_process`, and moves token ids to and from the per-GPU engines.  There is no
-Python/CPU implementation of the routing logic on this path.
+All routing state and decisions live in the CUDA library (K1, rr_router.cu), and the whole request lifecycle in its
+native gateway (rr_gateway.cu): admission, hand-off to the per-GPU engines or to mock replicas, DONE / FAIL reports and
+the fallback walk.  This file validates requests, submits them to the gateway and shapes its results as OpenAI
+responses.  There is no Python/CPU implementation of the routing logic or the request lifecycle on this path
+(`Router.process` hands event records to K1 directly, for benchmarks and parity tests).
 """
 from __future__ import annotations
 
@@ -28,8 +30,6 @@ import numpy as np
 
 from . import _lib
 from .config import RouterConfig, build_config, load_config
-
-EV_ADMIT, EV_DONE, EV_FAIL, EV_BURST = 0, 1, 2, 3
 
 
 # ---------------------------------------------------------------- errors (OpenAI-SDK names)
@@ -289,50 +289,21 @@ def messages_to_text(messages: Sequence[dict]) -> str:
 
 
 # ---------------------------------------------------------------- backends
+@dataclass
 class StubBackend:
-    """Mock-completion backend (BASELINE.json configs[0]: plumbing only): a fixed reply of
-    `reply_tokens` token ids, optional seeded failures."""
-
-    def __init__(self, vocab: int = 128256, reply_tokens: int = 8, fail_every: int = 0):
-        self.vocab = vocab
-        self.reply = reply_tokens
-        self.fail_every = fail_every
-        self._n = 0
-        self._lock = threading.Lock()
-
-    def submit(self, prompt_ids, max_new):
-        with self._lock:
-            self._n += 1
-            failed = self.fail_every > 0 and self._n % self.fail_every == 0
-        t = time.perf_counter()
-        return (failed, min(max_new, self.reply), t)
-
-    def wait(self, handle, timeout):
-        failed, n, t = handle
-        now = time.perf_counter()
-        return (7 if failed else 0), ([] if failed else [3 + (i % 200) for i in range(n)]), now - t, now - t
-
-    def peek(self, handle, have, timeout=0.05):
-        failed, n, t = handle
-        return ([] if failed else [3 + (i % 200) for i in range(n)]), True, time.perf_counter() - t
+    """Mock-completion replica (BASELINE.json configs[0]: plumbing only), served inside the gateway (rr_stub_desc): a
+    fixed reply of `reply_tokens` token ids; with fail_every = n, every n-th request handed to it fails."""
+    vocab: int = 128256
+    reply_tokens: int = 8
+    fail_every: int = 0
 
 
 class EngineBackend:
+    """A model replica: the gateway hands its admitted requests to `engine`."""
+
     def __init__(self, engine):
         self.engine = engine
         self.vocab = engine.spec.vocab
-        self.prefix_cache = bool(getattr(engine, "prefix_cache", False))
-
-    def peek(self, handle, have, timeout=0.05):
-        return self.engine.peek(handle, have, timeout=timeout)
-
-    def submit(self, prompt_ids, max_new):
-        return self.engine.submit(prompt_ids, max_new)
-
-    def wait(self, handle, timeout):
-        """-> (status, tokens, ttft, latency, prompt tokens served from the prefix cache)"""
-        rec = self.engine.wait(handle, timeout=timeout or 0.0)
-        return rec.status, rec.tokens, rec.ttft, rec.latency, rec.n_cached
 
 
 # ---------------------------------------------------------------- the router
@@ -375,7 +346,6 @@ class Router:
         st = _lib.RouterSettings(config.strategy_id, int(config.enable_pre_call_checks), config.allowed_fails,
                                  int(round(config.cooldown_time * 1000)), 0, config.latency_list_size,
                                  config.latency_buffer_ppm, config.latency_ttl_ms)
-        self._latency = config.routing_strategy == "latency-based-routing"
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_router_create(arr, len(deps), ng, (C.c_int32 * len(offs))(*offs),
                                              (C.c_int32 * max(1, len(flat)))(*flat), C.byref(st), seed, device,
@@ -395,11 +365,11 @@ class Router:
 
     # ---- native per-request path (rr_gateway.cu) ------------------------------------------------------
     def _gateway(self):
-        """rr_gateway over this router and its engines, or None when a backend is not a native engine (StubBackend:
-        BASELINE config #1, plumbing only -- the host loop below serves those)."""
-        if not self.backends or not all(isinstance(b, EngineBackend) for b in self.backends.values()):
-            return None
-        sig = tuple(sorted((k, id(b.engine)) for k, b in self.backends.items()))
+        """rr_gateway over this router and its replicas (the engine of an EngineBackend; a StubBackend is a mock replica
+        the gateway serves itself), built on first use and again when the backends change."""
+        if not self.backends:
+            raise ServiceUnavailableError("no backend attached to this router")
+        sig = tuple(sorted((k, id(b.engine if isinstance(b, EngineBackend) else b)) for k, b in self.backends.items()))
         with self._gw_lock:
             if self._gw is not None and self._gw_sig == sig:
                 return self._gw
@@ -407,21 +377,25 @@ class Router:
                 _lib.lib.rr_gateway_destroy(self._gw)
                 self._gw = None
             keys = sorted(self.backends)
-            engs = (C.c_void_p * len(keys))(*[self.backends[k].engine._h for k in keys])
+            engs = (C.c_void_p * len(keys))()                # NULL: a mock replica, described in stubs
+            stubs = (_lib.StubDesc * len(keys))()
+            for i, k in enumerate(keys):
+                b = self.backends[k]
+                if isinstance(b, StubBackend):
+                    stubs[i] = _lib.StubDesc(b.reply_tokens, b.fail_every, b.vocab, 0)
+                else:
+                    engs[i] = b.engine._h
             reps = (C.c_int32 * len(keys))(*keys)
             opts = _lib.GatewayOpts(1 if self._custom_clock else 0, int(self.record_trace), 0)
             h = C.c_void_p()
-            _lib.check(_lib.lib.rr_gateway_create(self._h, engs, reps, len(keys), C.byref(opts), C.byref(h)),
+            _lib.check(_lib.lib.rr_gateway_create(self._h, engs, reps, len(keys), stubs, C.byref(opts), C.byref(h)),
                        "rr_gateway_create")
             self._gw, self._gw_sig = h, sig
             return h
 
     def gateway_stats(self) -> dict:
-        gw = self._gateway()
-        if gw is None:
-            return {}
         s = _lib.GatewayStats()
-        _lib.check(_lib.lib.rr_gateway_get_stats(gw, C.byref(s)), "rr_gateway_get_stats")
+        _lib.check(_lib.lib.rr_gateway_get_stats(self._gateway(), C.byref(s)), "rr_gateway_get_stats")
         return {k: getattr(s, k) for k, _ in s._fields_}
 
     def gateway_trace(self) -> List[Tuple[Tuple[int, int, int, int, int], Tuple[int, int, int, int]]]:
@@ -430,7 +404,7 @@ class Router:
         gw = self._gateway()
         self._quiesce()
         n = C.c_int32()
-        if gw is None or _lib.lib.rr_gateway_trace(gw, None, None, 0, C.byref(n)) not in (0, 4) or n.value == 0:
+        if _lib.lib.rr_gateway_trace(gw, None, None, 0, C.byref(n)) not in (0, 4) or n.value == 0:
             return []
         ev, dec = (_lib.Event * n.value)(), (_lib.Decision * n.value)()
         _lib.check(_lib.lib.rr_gateway_trace(gw, ev, dec, n.value, C.byref(n)), "rr_gateway_trace")
@@ -624,24 +598,7 @@ class Router:
         _lib.check(_lib.lib.rr_router_latency_snapshot(self._h, mean, cnt), "rr_router_latency_snapshot")
         return list(zip(mean, cnt))
 
-    def _done_aux(self, latency_s: float) -> int:
-        """4th field of a DONE event: the request's latency in us (latency-based-routing only; 0 = no sample)."""
-        if not self._latency:
-            return 0
-        return min(max(int(round(latency_s * 1e6)), 1), 2**31 - 1)
-
-    def _fail_aux(self, timed_out: bool) -> int:
-        """4th field of a FAIL event: 1 = the request timed out (latency-based-routing records the penalty)."""
-        return 1 if self._latency and timed_out else 0
-
     # ---- request path ---------------------------------------------------------------------------
-    def _backend_for(self, dep_index: int):
-        d = self.cfg.deployments[dep_index]
-        b = self.backends.get(d.gpu)
-        if b is None:
-            raise ServiceUnavailableError(f"no backend attached for replica {d.gpu} ({d.model})")
-        return b
-
     def _vocab(self) -> int:
         """Token ids must be valid on every replica a request may fall back to: the smallest vocabulary attached."""
         return min((b.vocab for b in self.backends.values()), default=128256)
@@ -651,7 +608,7 @@ class Router:
         """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs; bias ids
         must be valid on every replica the request may fall back to."""
         top = check_logprobs(logprobs, top_logprobs)
-        if top is not None and self._gateway() is None:
+        if top is not None and any(isinstance(b, StubBackend) for b in self.backends.values()):
             raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
         samp = check_sampling(temperature, top_p, seed) or (None, None, None)
         pen = check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab()) or (None, None, (), ())
@@ -676,44 +633,8 @@ class Router:
             raise BadRequestError(f"Invalid model name passed in model={model}")
         if prompt_ids is None:
             prompt_ids = tokenize(messages_to_text(messages or []), self._vocab())
-        n_prompt = len(prompt_ids)
         max_new = max_tokens or self.default_max_tokens
-        gw = self._gateway()
-        if gw is not None:
-            return self._completion_gw(gw, model, g, prompt_ids, max_new, timeout, gen)
-        # ---- host loop (StubBackend): same admission events, one K1 launch per event
-        t_start = time.perf_counter()
-        chain_start = 0
-        last_err: Optional[APIError] = None
-        while True:
-            (status, dep, sg, pos), = self.process([(EV_ADMIT, g, n_prompt, chain_start, self.now_ms())])
-            if status == 1:
-                raise last_err or RateLimitError(
-                    f"No deployments available for selected model, passed model={model} (rate limited)")
-            if status != 0:
-                raise BadRequestError(f"Invalid model name passed in model={model}")
-            remaining = None if timeout is None else max(0.001, timeout - (time.perf_counter() - t_start))
-            try:
-                backend = self._backend_for(dep)
-                st, toks, ttft, lat, *cached = backend.wait(backend.submit(prompt_ids, max_new), remaining)
-            except Exception as exc:     # the request was admitted: never leave its in-flight slot behind
-                self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
-                raise exc if isinstance(exc, APIError) else APIError(f"backend error on deployment {dep}: {exc}")
-            if st == 0:
-                self.process([(EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms())])
-                d = self.cfg.deployments[dep]
-                return ModelResponse(
-                    id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-                    choices=[Choice(0, Message("assistant", detokenize(toks)))],
-                    usage=self._usage(dep, n_prompt, len(toks), cached[0] if cached else 0), created=int(time.time()),
-                    _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg],
-                    _fell_back=pos > 0, _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
-            # backend failed / timed out: report, then walk on down the fallback chain
-            self.process([(EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms())])
-            if st == 6:
-                raise APITimeoutError(f"Request timed out after {timeout}s")
-            last_err = APIError(f"backend failure on deployment {dep} ({self.cfg.deployments[dep].model})")
-            chain_start = pos + 1
+        return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen)
 
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                           max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
@@ -734,50 +655,7 @@ class Router:
         if prompt_ids is None:
             prompt_ids = tokenize(messages_to_text(messages or []), self._vocab())
         max_new = max_tokens or self.default_max_tokens
-        gw = self._gateway()
-        if gw is not None:
-            yield from self._stream_gw(gw, model, g, prompt_ids, max_new, timeout, gen)
-            return
-        deadline = None if not timeout else time.perf_counter() + timeout
-        chain_start = 0
-        while True:
-            (status, dep, sg, pos), = self.process([(EV_ADMIT, g, len(prompt_ids), chain_start, self.now_ms())])
-            if status == 1:
-                raise RateLimitError(f"No deployments available for selected model, passed model={model} (rate limited)")
-            if status != 0:
-                raise BadRequestError(f"Invalid model name passed in model={model}")
-            sent, failed, settled, timed_out = 0, False, False, False
-            try:
-                backend = self._backend_for(dep)
-                label = self.cfg.deployments[dep].response_model
-                h = backend.submit(prompt_ids, max_new)
-                while True:
-                    toks, done, ttft = backend.peek(h, sent)
-                    if len(toks) > sent:
-                        yield label, toks[sent:], False, ttft
-                        sent = len(toks)
-                    if done:
-                        st, toks, ttft, lat, *_ = backend.wait(h, timeout)
-                        failed = st != 0
-                        timed_out = st == 6
-                        break
-                    if deadline is not None and time.perf_counter() > deadline:
-                        timed_out = True
-                        raise APITimeoutError(f"Request timed out after {timeout}s")
-                if not failed:
-                    self.process([(EV_DONE, dep, sent, self._done_aux(lat), self.now_ms())])
-                    settled = True
-                    yield label, [], True, ttft
-                    return
-            finally:
-                if not settled:          # failure, timeout, or the consumer closed the generator: release the slot
-                    if failed or sent == 0:
-                        self.process([(EV_FAIL, dep, sent, self._fail_aux(timed_out), self.now_ms())])
-                    else:
-                        self.process([(EV_DONE, dep, sent, 0, self.now_ms())])
-            if sent > 0:
-                raise APIError(f"backend failure on deployment {dep} after {sent} tokens")
-            chain_start = pos + 1
+        yield from self._stream_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen)
 
     def completion_batch(self, model: str, prompts: Sequence[Sequence[int]], max_tokens: int,
                          timeout: Optional[float] = None) -> List[Any]:
@@ -787,74 +665,7 @@ class Router:
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
-        gw = self._gateway()
-        if gw is not None:
-            return self._batch_gw(gw, model, g, prompts, max_tokens, timeout)
-        now = self.now_ms()
-        head = [(EV_BURST, g, len(prompts), 0, now)] if self.cfg.routing_strategy == "split" else []
-        dec = self.process(head + [(EV_ADMIT, g, len(p), 0, now) for p in prompts])[len(head):]
-        t0 = time.perf_counter()
-        handles: List[Any] = [None] * len(prompts)
-        out: List[Any] = [None] * len(prompts)
-        for i, (status, dep, sg, pos) in enumerate(dec):
-            if status != 0:
-                out[i] = RateLimitError(f"No deployments available for model={model} (rate limited)")
-                continue
-            try:
-                b = self._backend_for(dep)
-                handles[i] = (b, b.submit(prompts[i], max_tokens))
-            except Exception as exc:     # admitted but never started: release the slot, keep serving the others
-                self.process([(EV_FAIL, dep, 0, 0, self.now_ms())])
-                out[i] = exc if isinstance(exc, APIError) else APIError(f"backend error on deployment {dep}: {exc}")
-        post = []
-        retry = []
-        for i, h in enumerate(handles):
-            if h is None:
-                continue
-            b, hd = h
-            status, dep, sg, pos = dec[i]
-            st, toks, ttft, lat, *cached = b.wait(hd, timeout)
-            if st == 0:
-                post.append((EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms()))
-                d = self.cfg.deployments[dep]
-                out[i] = ModelResponse(
-                    id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-                    choices=[Choice(0, Message("assistant", ""))],
-                    usage=self._usage(dep, len(prompts[i]), len(toks), cached[0] if cached else 0),
-                    created=int(time.time()),
-                    _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
-                    _ttft_s=ttft, _latency_s=time.perf_counter() - t0)
-            else:
-                post.append((EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms()))
-                retry.append((i, pos + 1))
-        self.process(post)
-        for i, chain_start in retry:          # failed requests walk the fallback chain one by one
-            try:
-                out[i] = self._retry_from(model, g, prompts[i], max_tokens, chain_start, timeout)
-            except APIError as e:
-                out[i] = e
-        return out
-
-    def _retry_from(self, model, g, prompt_ids, max_new, chain_start, timeout):
-        t_start = time.perf_counter()
-        while True:
-            (status, dep, sg, pos), = self.process([(EV_ADMIT, g, len(prompt_ids), chain_start, self.now_ms())])
-            if status != 0:
-                raise APIError(f"backend failure and no fallback available for model={model}")
-            b = self._backend_for(dep)
-            st, toks, ttft, lat, *cached = b.wait(b.submit(prompt_ids, max_new), timeout)
-            if st == 0:
-                self.process([(EV_DONE, dep, len(toks), self._done_aux(lat), self.now_ms())])
-                d = self.cfg.deployments[dep]
-                return ModelResponse(
-                    id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-                    choices=[Choice(0, Message("assistant", detokenize(toks)))],
-                    usage=self._usage(dep, len(prompt_ids), len(toks), cached[0] if cached else 0),
-                    created=int(time.time()),
-                    _token_ids=list(toks), _deployment=dep, _model_group=self.cfg.groups[sg], _fell_back=pos > 0,
-                    _ttft_s=ttft, _latency_s=time.perf_counter() - t_start)
-            self.process([(EV_FAIL, dep, 0, self._fail_aux(st == 6), self.now_ms())])
-            chain_start = pos + 1
+        return self._batch_gw(self._gateway(), model, g, prompts, max_tokens, timeout)
 
 
 # ---------------------------------------------------------------- OpenAI-SDK-shaped facade

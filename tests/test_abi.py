@@ -33,6 +33,7 @@ def test_struct_sizes_match_header():
     assert C.sizeof(_lib.DeploymentDesc) == 24 and C.sizeof(_lib.RouterSettings) == 32
     assert C.sizeof(_lib.DeploymentState) == 48
     assert C.sizeof(_lib.ModelDesc) == 36 and C.sizeof(_lib.Completion) == 48
+    assert C.sizeof(_lib.StubDesc) == 16
 
 
 def test_mt19937_seeding_matches_cpython():

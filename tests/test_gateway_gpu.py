@@ -86,15 +86,15 @@ def test_concurrent_callers_are_coalesced_and_decisions_replay_bit_exact():
     r.close(); eng.close()
 
 
-def test_backend_failures_walk_the_chain_inside_the_library():
-    """BASELINE config #4 shape: primary replica with a seeded 50 % failure mask, fallback replica healthy."""
-    from rr_b200 import EngineBackend, Router
-    bad, good = _tiny_engine(fail_prob=0.5, fail_seed=42), _tiny_engine()
+def _failures_walk_the_chain(bad, good):
+    """BASELINE config #4 shape: primary replica `bad` fails about half its requests, fallback replica `good` is healthy.
+    Checks the fallback walk inside the library and returns how many requests fell back."""
+    from rr_b200 import APIError, RateLimitError, Router
     ml = [{"model_name": "primary", "litellm_params": {"model": "b200/tiny", "gpu": 0}},
           {"model_name": "backup", "litellm_params": {"model": "b200/tiny-backup", "gpu": 1}}]
     now = [7000.0]
     r = Router(model_list=ml, routing_strategy="simple-shuffle", fallbacks=[{"primary": ["backup"]}], allowed_fails=1000,
-               cooldown_time=15, backends={0: EngineBackend(bad), 1: EngineBackend(good)}, seed=0, clock=lambda: now[0])
+               cooldown_time=15, backends={0: bad, 1: good}, seed=0, clock=lambda: now[0])
     r.record_trace = 4096
     outs = r.completion_batch("primary", [list(range(3, 20))] * 40, 3)
     assert all(not isinstance(o, Exception) for o in outs)
@@ -109,13 +109,53 @@ def test_backend_failures_walk_the_chain_inside_the_library():
     assert _replay(r, trace) == 40 + n_fb                          # every re-admission is an ADMIT with chain_start = 1
     assert sum(1 for e, _ in trace if e[0] == 0 and e[3] == 1) == n_fb
     # no fallback left: the error is a backend failure (500), not a 429
-    from rr_b200 import APIError, RateLimitError
-    r2 = Router(model_list=ml[:1], backends={0: EngineBackend(bad)}, seed=0, clock=lambda: now[0], allowed_fails=1000)
+    r2 = Router(model_list=ml[:1], backends={0: bad}, seed=0, clock=lambda: now[0], allowed_fails=1000)
     res = r2.completion_batch("primary", [list(range(3, 20))] * 20, 2)
     errs = [o for o in res if isinstance(o, Exception)]
     assert errs and all(isinstance(e, APIError) and not isinstance(e, RateLimitError) and e.status_code == 500 for e in errs)
     assert sum(s["inflight"] for s in r2.snapshot()) == 0
-    r2.close(); r.close(); bad.close(); good.close()
+    r2.close(); r.close()
+    return n_fb
+
+
+def test_backend_failures_walk_the_chain_inside_the_library():
+    """Engine replicas: the primary has a seeded 50 % failure mask."""
+    from rr_b200 import EngineBackend
+    bad, good = _tiny_engine(fail_prob=0.5, fail_seed=42), _tiny_engine()
+    try:
+        _failures_walk_the_chain(EngineBackend(bad), EngineBackend(good))
+    finally:
+        bad.close(); good.close()
+
+
+def test_mock_replica_failures_walk_the_chain_inside_the_library():
+    """Mock replicas take the same native path: the primary fails every second request handed to it, exactly."""
+    from rr_b200 import StubBackend
+    assert _failures_walk_the_chain(StubBackend(fail_every=2), StubBackend()) == 20
+
+
+def test_mock_replica_descriptors_are_checked_and_logprobs_refused():
+    """rr_gateway_create refuses a NULL engine without a valid rr_stub_desc and creates nothing; a gateway with a mock
+    replica refuses logprobs at submit (no logits to fill the pairs from) and serves its fixed reply."""
+    import ctypes as C
+    from rr_b200 import Router, StubBackend, _lib
+    ml = [{"model_name": "chat", "litellm_params": {"model": "b200/tiny", "gpu": 0}}]
+    r = Router(model_list=ml, backends={0: StubBackend()}, seed=0)
+    try:
+        engs, reps, gw = (C.c_void_p * 1)(), (C.c_int32 * 1)(0), C.c_void_p()
+        assert _lib.lib.rr_gateway_create(r._h, engs, reps, 1, None, None, C.byref(gw)) == 4
+        for bad in ((-1, 0, 100, 0), (8, -1, 100, 0), (8, 0, 0, 0)):
+            stubs = (_lib.StubDesc * 1)(_lib.StubDesc(*bad))
+            assert _lib.lib.rr_gateway_create(r._h, engs, reps, 1, stubs, None, C.byref(gw)) == 4
+        assert not gw.value
+        ids, t = (C.c_int32 * 3)(5, 6, 7), C.c_uint64()
+        assert _lib.lib.rr_gateway_submit_logprobs(r._gateway(), 0, ids, 3, 4, 0, C.byref(t)) == 4
+        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 3, 4, C.byref(t)) == 0
+        res, toks = _lib.GatewayResult(), (C.c_int32 * 4)()
+        assert _lib.lib.rr_gateway_wait(r._gateway(), t.value, 30.0, C.byref(res), toks, 4) == 0
+        assert list(toks) == [3, 4, 5, 6] and res.n_generated == 4 and res.deployment == 0
+    finally:
+        r.close()
 
 
 def test_bad_requests_are_rejected_before_any_debit_and_timeouts_release_the_row():

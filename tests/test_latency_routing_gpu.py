@@ -1,6 +1,6 @@
 """GPU: latency-based-routing in the admission kernel K1 (csrc/rr_router.cu) against the oracle (oracle/latency_router.py), bit for
 bit, in both state variants; the other strategies unchanged by the latency fields; the native gateway feeding measured
-engine latencies and timeout penalties into K1; the host loop feeding StubBackend latencies."""
+engine latencies and timeout penalties into K1, and the hand-off -> settle latencies of its mock replicas."""
 import ctypes as C
 import random
 import time
@@ -226,18 +226,19 @@ def test_gateway_routes_to_the_faster_replica_and_avoids_a_timed_out_one(capsys)
         slow.close()
 
 
-# ---------------------------------------------------------------- host loop (StubBackend)
-def test_host_loop_posts_stub_latencies():
-    from rr_b200 import Router, StubBackend
+# ---------------------------------------------------------------- native gateway, mock replicas (StubBackend)
+def test_stub_replicas_post_latencies():
+    from rr_b200 import APIError, Router, StubBackend
     ml = [{"model_name": "chat", "litellm_params": {"model": "b200/tiny@a", "gpu": 0}},
           {"model_name": "chat", "litellm_params": {"model": "b200/tiny@b", "gpu": 1}},
           {"model_name": "spill", "litellm_params": {"model": "b200/tiny@c", "gpu": 2}}]
     r = Router(model_list=ml, routing_strategy="latency-based-routing", fallbacks=[{"chat": ["spill"]}],
                allowed_fails=1000, routing_strategy_args={"lowest_latency_buffer": 10, "max_latency_list_size": 32},
                backends={0: StubBackend(), 1: StubBackend(), 2: StubBackend(fail_every=2)}, seed=1)
-    events = []
-    real = r.process
-    r.process = lambda ev: (events.extend(ev), real(ev))[1]
+    r.record_trace = 4096
+
+    def events():
+        return [e for e, _ in r.gateway_trace()]
     try:
         for _ in range(5):
             r.completion(model="chat", prompt_ids=[5, 6, 7], max_tokens=4)
@@ -248,14 +249,19 @@ def test_host_loop_posts_stub_latencies():
         lat = r.latency_snapshot()
         assert lat[0][1] + lat[1][1] == 12 and lat[2] == (0.0, 0)
         assert all(m > 0.0 for m, n in lat[:2] if n)
-        dones = [e for e in events if e[0] == O.EV_DONE]
+        dones = [e for e in events() if e[0] == O.EV_DONE]
         assert len(dones) == 12 and all(e[3] >= 1 for e in dones)
         # a backend failure is not a timeout: FAIL without the flag, no sample
         r.completion(model="spill", prompt_ids=[5], max_tokens=2)
-        with pytest.raises(Exception):
+        n_before = len(events())
+        with pytest.raises(APIError):
             r.completion(model="spill", prompt_ids=[5], max_tokens=2)
-        fails = [e for e in events if e[0] == O.EV_FAIL]
+        fails = [e for e in events() if e[0] == O.EV_FAIL]
         assert len(fails) == 1 and fails[0][3] == 0
         assert r.latency_snapshot()[2][1] == 1
+        # the failing request: ADMIT, FAIL, re-ADMIT one step down the chain, rejected (no fallback for `spill`)
+        spill = r.gateway_trace()[n_before:]
+        assert [(e[0], e[3]) for e, _ in spill] == [(O.EV_ADMIT, 0), (O.EV_FAIL, 0), (O.EV_ADMIT, 1)]
+        assert spill[0][1][0] == 0 and spill[2][1][0] != 0
     finally:
         r.close()

@@ -90,12 +90,13 @@ def test_backend_failure_walks_fallback_chain_and_cools_down():
     r = Router(config=cfg, backends={0: bad, 1: good}, seed=0, clock=lambda: now[0])
     outs = [r.completion(model="claude-sonnet-fallback-demo", messages=[{"role": "user", "content": "x"}]) for _ in range(5)]
     assert all(o._fell_back and "claude-3-5-sonnet" in o.model for o in outs)
-    assert bad._n == 3                                  # 4th and 5th request never reached the cooling primary
     snap = r.snapshot()
+    # every admission of the primary is one hand-off to the failing replica
+    assert snap[0]["total_admitted"] == 3               # 4th and 5th request never reached the cooling primary
     assert snap[0]["fail_count"] == 3 and snap[0]["cooldown_until_ms"] == int(now[0] * 1000) + 15000
     now[0] += 61.0                                    # past the cooldown AND into a fresh rpm window
     r.completion(model="claude-sonnet-fallback-demo", messages=[{"role": "user", "content": "x"}])
-    assert bad._n == 4                                  # cooldown over: the primary is tried again
+    assert r.snapshot()[0]["total_admitted"] == 4       # cooldown over: the primary is tried again
     r.close()
 
 

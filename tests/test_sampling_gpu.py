@@ -354,6 +354,8 @@ def test_stub_router_validates_and_keeps_its_fixed_reply():
             r.completion("g", messages=msgs, temperature=3.0)
         with pytest.raises(BadRequestError):
             next(r.completion_stream("g", messages=msgs, top_p=2))
+        with pytest.raises(BadRequestError):                  # a mock replica has no logits to serve logprobs from
+            r.completion("g", messages=msgs, logprobs=True)
     finally:
         r.close()
 
