@@ -455,6 +455,26 @@ int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_pr
                                float temperature, float top_p, uint64_t seed, float frequency_penalty,
                                float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
                                uint64_t* ticket);
+/* Several choices per request (OpenAI `n`): rr_engine_submit_processed with n_choices (1..max_batch) completions of the same
+ * prompt.  The prompt is prefilled once; its KV is then copied into n_choices - 1 further KV slots, and every choice decodes
+ * in a row of its own.  Choice i is exactly what rr_engine_submit_processed gives with seed (seed + i) mod 2^64 and the same
+ * other parameters (greedy: every choice is the greedy completion); penalties count the choice's own tokens.  The choices
+ * run in lockstep: they are admitted together (a request waits at the head of the queue until n_choices rows are free;
+ * nothing overtakes it), get one token each per step and end together, so rr_completion.n_generated counts the tokens of
+ * each choice.  Cancellation, an injected failure or an internal error ends every choice.  n_choices = 1 is
+ * rr_engine_submit_processed.  RR_INVALID_ARGUMENT, before anything is queued, for n_choices outside 1..max_batch and
+ * whatever rr_engine_submit_processed rejects.
+ * wait_choices: rr_engine_wait_logprobs for any n_choices, with tokens_out [n_choices][max_tokens_out] and lp_out / id_out
+ * [n_choices][max_tokens_out][K] (K as rr_engine_submit_sampled describes).  rr_engine_wait / _wait_logprobs / _peek /
+ * _peek_logprobs return RR_INVALID_ARGUMENT for a request of n_choices > 1 (it stays in flight).
+ * Stats: prefill_tokens counts the prompt once, kv_copy_tokens grows by (n_choices - 1) x the prompt length,
+ * generated_tokens counts every choice's tokens. */
+int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
+                             int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                             float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
+                             uint64_t* ticket);
+int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                           int max_tokens_out, float* lp_out, int32_t* id_out);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -569,6 +589,19 @@ int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_
                                 int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
                                 float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
                                 uint64_t* ticket);
+/* Several choices per request (rr_engine_submit_choices): n_choices is stored with the request and travels with it, a
+ * fallback re-admission included (all choices restart there).  The request is one ADMIT event (the prompt's tokens) and
+ * one DONE event carrying the tokens of all choices.  RR_INVALID_ARGUMENT before anything is debited for n_choices below 1
+ * or above the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices copies
+ * of its reply).  wait_choices: rr_gateway_wait_logprobs for any n_choices, with tokens_out [n_choices][max_tokens_out]
+ * and lp_out / id_out [n_choices][max_tokens_out][K]; rr_gateway_result.n_generated counts the tokens of each choice.
+ * rr_gateway_wait / _wait_logprobs / _peek / _peek_logprobs return RR_INVALID_ARGUMENT for a request of n_choices > 1. */
+int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                              int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                              float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                              const float* bias_vals, uint64_t* ticket);
+int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                            int max_tokens_out, float* lp_out, int32_t* id_out);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

@@ -193,6 +193,11 @@ PROTOTYPES = {
                                            C.POINTER(C.c_uint64)]),
     "rr_engine_submit_processed": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
                                              C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.POINTER(C.c_uint64)]),
+    "rr_engine_submit_choices": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                           C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
+                                           C.POINTER(C.c_uint64)]),
+    "rr_engine_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p,
+                                         c_i32p]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
                                       C.POINTER(Completion), c_i32p]),
     "rr_engine_now": (C.c_double, [vp]),
@@ -218,6 +223,11 @@ PROTOTYPES = {
     "rr_gateway_submit_processed": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
                                               C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
                                               C.POINTER(C.c_uint64)]),
+    "rr_gateway_submit_choices": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                            C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
+                                            C.POINTER(C.c_uint64)]),
+    "rr_gateway_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
+                                          c_i32p]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),
     "rr_gateway_quiesce": (C.c_int, [vp, C.c_double]),
     "rr_gateway_get_stats": (C.c_int, [vp, C.POINTER(GatewayStats)]),

@@ -65,22 +65,28 @@ __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const
     d_slot[s] = s;
 }
 
+// One request of n_choices choices.  Choice c decodes in row rows[c] (== its KV slot); the prompt is prefilled once, into
+// rows[0], and its KV copied to the other rows.  All choices run in lockstep: admitted in one chunk, one token each per
+// step, released together.
 struct Request {
     uint64_t ticket;
     std::vector<int32_t> prompt;
     int max_new;
-    std::vector<int32_t> out;
+    int n_choices = 1;
+    std::vector<std::vector<int32_t>> out;     // [n_choices][tokens generated so far]
     int status = RR_OK;
     bool done = false;
     double t_submit = 0, t_first = 0, t_done = 0;
-    int slot = -1;
+    std::vector<int> rows;     // [n_choices] while admitted, else empty
     uint64_t tag = 0;          // opaque caller value handed to the done hook (the gateway's request id)
-    bool cancel = false;       // rr_engine_cancel: the worker drops the row at the next step
+    bool cancel = false;       // rr_engine_cancel: the worker drops the rows at the next step
     bool detached = false;     // nobody will call rr_engine_wait: the worker frees the request when it finishes
     GenParams gen;
-    std::vector<float> lp;     // [out.size()][gen.lp_width()]
-    std::vector<int32_t> lp_id;
+    std::vector<std::vector<float>> lp;        // [n_choices][out[c].size()][gen.lp_width()]
+    std::vector<std::vector<int32_t>> lp_id;
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
+
+    int n_generated() const { return (int)out[0].size(); }      // tokens per choice
 };
 
 // Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
@@ -125,10 +131,11 @@ struct ParamBlocks {
         return (top_n()[i] >= 0 ? 1 : 0) | (temp()[i] > 0.f ? 2 : 0) |
                (blk[2] && (freq()[i] != 0.f || pres()[i] != 0.f || n_bias()[i] != 0) ? 4 : 0);
     }
-    // Row i from p: drawn at `position` (with a position column), p's bias, and penalties f / pr from position g0 on.
-    void put_row(int i, const GenParams& p, int position, float f, float pr, int g0) const {
+    // Row i from p for its choice `choice`: drawn at `position` (with a position column) with seed p.seed + choice, p's
+    // bias, and penalties f / pr from position g0 on.
+    void put_row(int i, const GenParams& p, int choice, int position, float f, float pr, int g0) const {
         top_n()[i] = p.top_lp;
-        seed()[i] = p.seed; temp()[i] = p.temp; top_p()[i] = p.top_p;
+        seed()[i] = p.sampled() ? p.seed + (uint64_t)choice : p.seed; temp()[i] = p.temp; top_p()[i] = p.top_p;
         if (has_pos) pos()[i] = position;
         if (!blk[2]) return;
         const int nb = (int)p.bias_id.size();
@@ -263,6 +270,7 @@ struct rr_engine {
     std::deque<Request*> waiting;
     std::unordered_map<uint64_t, Request*> table;
     std::vector<Request*> row_req;       // [Bm]
+    std::vector<int> row_choice;         // [Bm] the choice of row_req[b] that row b decodes
     std::vector<int32_t> h_slot_mirror;  // host mirror of d_slot
     bool slots_dirty = false;
     // prefix caching (o.prefix_cache), under mu: retained[b] = the prompt tokens whose KV the last successful prefill into
@@ -543,26 +551,41 @@ static int init_pf_plans(rr_engine* e) {
     return RR_OK;
 }
 
+// The tail rows of a prefill chunk: the rows the trimmed last layer, lm_head and the logits tail run on, one per choice of
+// each request.  Row j reads the last token of sequence seq[j], decodes in slot[j] and is choice choice[j] of the request
+// whose parameters are gen[j]; mode = the step_mode bits over gen.  Rows of the same sequence in other slots than the
+// sequence's get its prompt KV copied there.  Without a tail, row i is sequence i in slots[i], plain greedy.
+struct PrefillTail {
+    int n = 0;
+    const int32_t *seq = nullptr, *slot = nullptr, *choice = nullptr;
+    const GenParams* const* gen = nullptr;
+    int mode = 0;
+};
+
 // ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
 // activates the rows. Caller holds gpu_mu.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
-// gen[n_seqs] (with mode): each sequence's request parameters, and mode = the step_mode bits over them, for the logits
-// tail on the chunk's rows.  Only a logit bias applies (penalties count generated tokens only, so the first token has
-// none; needs ensure_pen_buffers).  A sampled sequence draws its first token at position pos0[i] + its length (the prompt
-// length).  A logprobs sequence also gets its first token's logprobs in e->h_lp / e->h_lp_id row i, and if sampled its
-// own logprob in h_tok_lp.
+// tail (optional): the tail rows and their request parameters.  Only a logit bias applies (penalties count generated
+// tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position
+// pos0 + the sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's
+// logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
+// slots, one launch after the last layer copies positions [0, prompt length) of its slot to each of them.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
-                       const KvCopyList* copies = nullptr, const GenParams* const* gen = nullptr, int mode = 0) {
+                       const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
-    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm) return RR_INVALID_ARGUMENT;
+    const int nt = tail ? tail->n : n_seqs;
+    const bool fan = nt != n_seqs;                     // some sequence has more than one tail row
+    int mode = tail ? tail->mode : 0;
+    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < n_seqs || nt > e->Bm) return RR_INVALID_ARGUMENT;
     cudaStream_t s = e->stream;
     // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n] (| pos0[n])
+    //                 (| tail_slot[nt] | tail_last[nt] with fan-out)
     int32_t* h = e->h_stage;
     int32_t *h_ids = h, *h_pos = h + T, *h_slt = h + 2 * T, *h_ss = h + 3 * T, *h_sl = h_ss + n_seqs + 1,
-            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs;
+            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs, *h_tsl = h_p0 + (pos0 ? n_seqs : 0), *h_tlast = h_tsl + nt;
     int max_len = 0;
     memcpy(h_ids, ids, sizeof(int32_t) * T);
     for (int i = 0; i < n_seqs; ++i) {
@@ -574,31 +597,53 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (b - a > max_len) max_len = b - a;
     }
     h_ss[n_seqs] = T;
-    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1;
+    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1 + (fan ? 2 * nt : 0);
     uint64_t copy_tokens = 0;
     if (copies && copies->count > 0) {
         if (kv_copy_check(*copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
         for (int i = 0; i < copies->count; ++i) copy_tokens += copies->n[i];
     }
-    // the chunk's parameter blocks, at the stride of its sequences and of its largest bias count
+    KvCopyList fan_copies;                             // the fan-out: source slot -> the slot of each further tail row
+    fan_copies.count = 0;
+    for (int j = 0; tail && j < nt; ++j) {
+        const int q = tail->seq[j], sl = tail->slot[j];
+        if (q < 0 || q >= n_seqs || sl < 0 || sl >= e->Bm) return RR_INVALID_ARGUMENT;
+        if (!fan) {
+            if (q != j || sl != slots[j]) return RR_INVALID_ARGUMENT;
+            continue;
+        }
+        h_tsl[j] = sl; h_tlast[j] = h_last[q];
+        if (sl == slots[q]) continue;
+        const int c = fan_copies.count++;              // < nt <= Bm <= KV_COPY_MAX
+        fan_copies.src[c] = slots[q]; fan_copies.dst[c] = sl;
+        fan_copies.n[c] = (pos0 ? pos0[q] : 0) + seq_start[q + 1] - seq_start[q];
+        copy_tokens += fan_copies.n[c];
+    }
+    if (fan_copies.count && kv_copy_check(fan_copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
+    // the chunk's parameter blocks, at the stride of its tail rows and of its largest bias count
     int max_bias = 0;
-    for (int i = 0; (mode & 4) && i < n_seqs; ++i) max_bias = std::max(max_bias, (int)gen[i]->bias_id.size());
+    for (int j = 0; (mode & 4) && j < nt; ++j) max_bias = std::max(max_bias, (int)tail->gen[j]->bias_id.size());
     if (max_bias == 0) mode &= ~4;
     else if (!e->d_pf.blk[2]) return RR_INTERNAL;
-    const ParamBlocks hp = e->h_pf.at(n_seqs, max_bias), dp = e->d_pf.at(n_seqs, max_bias);
-    for (int i = 0; mode && i < n_seqs; ++i)
-        hp.put_row(i, *gen[i], (pos0 ? pos0[i] : 0) + seq_start[i + 1] - seq_start[i], 0.f, 0.f, 0);
+    const ParamBlocks hp = e->h_pf.at(nt, max_bias), dp = e->d_pf.at(nt, max_bias);
+    for (int j = 0; mode && j < nt; ++j) {
+        const int q = tail->seq[j];
+        hp.put_row(j, *tail->gen[j], tail->choice[j], (pos0 ? pos0[q] : 0) + seq_start[q + 1] - seq_start[q], 0.f, 0.f,
+                   0);
+    }
     CK(cudaEventRecord(e->ev0, s));
     CK(cudaMemcpyAsync(e->p_ids, h, n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     e->st.h2d_bytes += n_ints * sizeof(int32_t);
     CK(hp.upload(dp, mode, s, &e->st.h2d_bytes));
     int32_t *p_ids = e->p_ids, *p_pos = p_ids + T, *p_slt = p_ids + 2 * T, *p_ss = p_ids + 3 * T,
             *p_sl = p_ss + n_seqs + 1, *p_last = p_sl + n_seqs, *p_p0 = p_last + n_seqs;
+    const int32_t* p_tsl = fan ? p_ids + (h_tsl - h) : p_sl;       // the tail rows' slots and last-token indices
+    const int32_t* p_tlast = fan ? p_ids + (h_tlast - h) : p_last;
 
     rr_engine::PfPlans& P = e->pf;
     auto launch_rows = [&](const GemmPlan& pl) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s); };
     uint64_t nl = 0;
-    if (copy_tokens) {      // cached prefixes of busy slots into this chunk's slots, before any layer reads them
+    if (copies && copies->count > 0) {   // cached prefixes of busy slots into this chunk's slots, before any layer reads them
         if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, e->Bm, d.n_kv_heads, e->o.ctx_max, *copies, s) != RR_OK)
             return RR_CUDA_ERROR;
         ++nl;
@@ -628,9 +673,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (l + 1 == d.n_layers) {
             // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers).  The
             // unfused kernels even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
-            launch_pdl(gather_last_kernel, dim3(n_seqs), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
-                       (const int32_t*)p_last, e->attn_out, e->x, e->nq, d.hidden); ++nl;
-            if (enqueue_o_mlp(e, l, n_seqs, s, &nl) != RR_OK) return RR_CUDA_ERROR;
+            launch_pdl(gather_last_kernel, dim3(nt), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
+                       p_tlast, e->attn_out, e->x, e->nq, d.hidden); ++nl;
+            if (enqueue_o_mlp(e, l, nt, s, &nl) != RR_OK) return RR_CUDA_ERROR;
             break;
         }
         if (launch_rows(P.o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
@@ -638,12 +683,16 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (!e->fuse_silu) { launch_silu_mul(part_bf16(e->pgu, 2 * d.inter), e->pact, T, d.inter, s); ++nl; }
         if (launch_rows(P.down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
     }
-    if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..n_seqs-1)
-    nl += enqueue_tail(e, dp, n_seqs, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s);
-    launch_pdl(activate_rows_kernel, dim3((n_seqs + 127) / 128), dim3(128), 0, s, (const int32_t*)p_sl,
-               (const int32_t*)e->p_first, (const int32_t*)p_pos, (const int32_t*)p_last, n_seqs, e->d_tok, e->d_pos,
-               e->d_slot); ++nl;
-    const int rc = enqueue_readback(e, e->p_first, n_seqs, mode, s);
+    if (fan_copies.count) {     // every layer's KV of the prompts is written: fan it out before any decode step reads it
+        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, e->Bm, d.n_kv_heads, e->o.ctx_max, fan_copies, s) != RR_OK)
+            return RR_CUDA_ERROR;
+        ++nl;
+    }
+    if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..nt-1)
+    nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s);
+    launch_pdl(activate_rows_kernel, dim3((nt + 127) / 128), dim3(128), 0, s, p_tsl, (const int32_t*)e->p_first,
+               (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
+    const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
     if (rc != RR_OK) return rc;
     if (logits_host) {
         CK(cudaMemcpyAsync(logits_host, e->logits, sizeof(float) * (size_t)n_seqs * d.vocab, cudaMemcpyDeviceToHost, s));
@@ -657,9 +706,10 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     e->st.prefill_tokens += T;
     e->st.kv_copy_tokens += copy_tokens;
     e->st.kernel_launches += nl;
-    for (int i = 0; i < n_seqs; ++i) {
-        if (first_tok_host) first_tok_host[i] = e->h_tok[i];
-        e->h_slot_mirror[slots[i]] = slots[i];
+    for (int j = 0; j < nt; ++j) {
+        if (first_tok_host) first_tok_host[j] = e->h_tok[j];
+        const int sl = fan ? h_tsl[j] : slots[j];
+        e->h_slot_mirror[sl] = sl;
     }
     return RR_OK;
 }
@@ -671,11 +721,11 @@ struct DoneNote { uint64_t tag, ticket; int status, n_gen; };
 // defaults.  A block is marked dirty only when the row uses it before or after: the other rows of a mirror hold the
 // defaults, as a request that does not use the block does (GenParams::set), so they never need a copy.  A freed row's
 // mirror row holds the defaults, so freeing a row that never held parameters changes nothing.
-static void set_row_params(rr_engine* e, int b, const Request* r) {
+static void set_row_params(rr_engine* e, int b, const Request* r, int choice = 0) {
     static const GenParams plain;
     const GenParams& p = r ? r->gen : plain;
     e->rows_dirty |= e->h_rows.row_mode(b) | step_mode(p);
-    e->h_rows.put_row(b, p, 0, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
+    e->h_rows.put_row(b, p, choice, 0, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
 }
 
 // Before a decode step: copy each parameter block the step reads (step_mode bits) whose mirror changed.
@@ -689,7 +739,7 @@ static void finish_request(rr_engine* e, Request* r, int status, std::vector<Don
     r->status = status;
     r->t_done = now_s(e);
     r->done = true;
-    if (notes && e->hook) notes->push_back(DoneNote{r->tag, r->ticket, status, (int)r->out.size()});
+    if (notes && e->hook) notes->push_back(DoneNote{r->tag, r->ticket, status, r->n_generated() * r->n_choices});
     if (r->detached) {                   // cancelled by its owner: nobody waits for it
         e->table.erase(r->ticket);
         delete r;
@@ -700,29 +750,35 @@ static void run_hooks(rr_engine* e, std::vector<DoneNote>& notes) {
     notes.clear();
 }
 
-// Caller holds e->mu.  Frees decode row b (inactive from the next step, parameters back to the defaults) and finishes its
-// request with `status`.
-static void release_row(rr_engine* e, int b, int status, std::vector<DoneNote>* notes) {
-    Request* r = e->row_req[b];
-    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1; e->slots_dirty = true;
-    set_row_params(e, b, nullptr);
+// Caller holds e->mu.  Frees every decode row of r (inactive from the next step, parameters back to the defaults) and
+// finishes r with `status`.
+static void release_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes) {
+    for (int b : r->rows) {
+        e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1;
+        set_row_params(e, b, nullptr);
+    }
+    e->slots_dirty = true;
+    r->rows.clear();
     finish_request(e, r, status, notes);
 }
 
-// Caller holds e->mu.  Appends the token read back for row `row` to r, with its pairs (h_lp / h_lp_id row `row`, and for
-// a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  True once r has max_new tokens.
-static bool take_token(rr_engine* e, Request* r, int row) {
-    r->out.push_back(e->h_tok[row]);
+// Caller holds e->mu.  Appends the token read back for row `row` to choice c of r, with its pairs (h_lp / h_lp_id row
+// `row`, and for a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  True once every
+// choice of r has max_new tokens: the choices run in lockstep, so that is the step's last row of r.
+static bool take_token(rr_engine* e, Request* r, int c, int row) {
+    r->out[c].push_back(e->h_tok[row]);
     if (r->gen.logprobs()) {
         const int k = r->gen.top_lp > 1 ? r->gen.top_lp : 1;
         const float* v = e->h_lp + (size_t)row * LP_MAX_TOP;
         const int32_t* id = e->h_lp_id + (size_t)row * LP_MAX_TOP;
-        r->lp.insert(r->lp.end(), v, v + k);
-        r->lp_id.insert(r->lp_id.end(), id, id + k);
-        if (r->gen.sampled()) { r->lp.push_back(e->h_tok_lp[row]); r->lp_id.push_back(r->out.back()); }
+        r->lp[c].insert(r->lp[c].end(), v, v + k);
+        r->lp_id[c].insert(r->lp_id[c].end(), id, id + k);
+        if (r->gen.sampled()) { r->lp[c].push_back(e->h_tok_lp[row]); r->lp_id[c].push_back(r->out[c].back()); }
     }
     e->st.generated_tokens += 1;
-    return (int)r->out.size() >= r->max_new;
+    for (const std::vector<int32_t>& o : r->out)
+        if ((int)o.size() < r->max_new) return false;
+    return true;
 }
 
 // Caller holds e->mu.  Prefix caching: the slot a prompt p is admitted into and how many of its tokens are cached there.
@@ -731,6 +787,16 @@ static bool take_token(rr_engine* e, Request* r, int row) {
 // A hit on a free slot takes that slot as it is; a hit on a busy slot (*src = it) copies m tokens into the slot a miss
 // takes: the lowest free slot with nothing retained, else the free slot whose prefix was used least recently.  Slots taken
 // in the current chunk have nothing retained, so requests of one chunk never share.  false: no free slot.
+// pick_slot_miss: the slot a miss takes (-1: none free); the further choices of a request take their slots by it.
+static int pick_slot_miss(const rr_engine* e) {
+    int fresh = -1;
+    for (int b = 0; b < e->Bm; ++b) {
+        if (e->row_req[b]) continue;
+        if (e->retained[b].empty()) return b;
+        if (fresh < 0 || e->retained_used[b] < e->retained_used[fresh]) fresh = b;
+    }
+    return fresh;
+}
 static bool pick_slot_cached(const rr_engine* e, const std::vector<int32_t>& p, int* slot, int* m, int* src) {
     const int cap = (int)p.size() - 1;
     int best = -1, best_m = 0;
@@ -747,12 +813,7 @@ static bool pick_slot_cached(const rr_engine* e, const std::vector<int32_t>& p, 
     *m = best >= 0 ? best_m : 0;
     *src = -1;
     if (best >= 0 && best_free) { *slot = best; return true; }
-    int fresh = -1;
-    for (int b = 0; b < e->Bm; ++b) {
-        if (e->row_req[b]) continue;
-        if (e->retained[b].empty()) { fresh = b; break; }
-        if (fresh < 0 || e->retained_used[b] < e->retained_used[fresh]) fresh = b;
-    }
+    const int fresh = pick_slot_miss(e);
     if (fresh < 0) return false;
     *slot = fresh;
     *src = best;
@@ -771,13 +832,15 @@ static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
     std::vector<int32_t> ids, seq_start, slots, pos0;
     std::vector<Request*> chunk;
-    std::vector<const GenParams*> gen;
     std::vector<DoneNote> notes;
     KvCopyList* copies = new KvCopyList();
+    std::vector<int32_t> tail_seq, tail_slot, tail_choice;      // the chunk's tail rows (PrefillTail), one per choice
+    std::vector<const GenParams*> tail_gen;
     while (!e->stop.load()) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
-        chunk.clear(); gen.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
+        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
+        tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear();
         copies->count = 0;
         int active = 0;
         int step = 0, chunk_mode = 0;                      // step_mode bits of the active rows / of the chunk's requests
@@ -787,14 +850,16 @@ static void worker_main(rr_engine* e) {
             for (int b = 0; b < e->Bm; ++b) {
                 Request* r = e->row_req[b];
                 if (!r) continue;
-                if (r->cancel) {                           // rr_engine_cancel: free the row, keep what was generated
-                    release_row(e, b, RR_CANCELLED, &notes);
+                if (r->cancel) {                           // rr_engine_cancel: free the rows, keep what was generated
+                    release_request(e, r, RR_CANCELLED, &notes);
                     continue;
                 }
                 ++active;
                 step |= step_mode(r->gen);
             }
             if (e->waiting.empty() && active == 0) {
+                if (!notes.empty()) continue;              // report the requests a cancel just ended before idling
+                e->st.queued = 0; e->st.active_rows = 0;   // idle: every row is free and every done hook has run
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
                 continue;
             }
@@ -802,6 +867,7 @@ static void worker_main(rr_engine* e) {
             epoch = e->index_epoch;
             while (!e->waiting.empty()) {
                 Request* r = e->waiting.front();
+                if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all in this chunk
                 int m = 0, src = -1;
                 if (e->o.prefix_cache) {
                     if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
@@ -811,8 +877,6 @@ static void worker_main(rr_engine* e) {
                 }
                 if ((int)ids.size() + (int)r->prompt.size() - m > e->Tmax) break;   // a chunk holds Tmax uncached tokens
                 e->waiting.pop_front();
-                e->row_req[b] = r;
-                r->slot = b;
                 r->n_cached = m;
                 if (e->o.prefix_cache) {
                     if (m > 0) e->retained_used[src >= 0 ? src : b] = ++e->lru_clock;
@@ -820,16 +884,26 @@ static void worker_main(rr_engine* e) {
                         const int c = copies->count++;
                         copies->src[c] = src; copies->dst[c] = b; copies->n[c] = m;
                     }
-                    e->retained[b].clear();                // rewritten by this chunk; set again once its prefill succeeds
                     pos0.push_back(m);
                 }
+                for (int c = 0; c < r->n_choices; ++c) {   // choice 0 in the prompt's slot, the others in free ones
+                    if (c > 0) {
+                        if (e->o.prefix_cache) b = pick_slot_miss(e);
+                        else while (e->row_req[b] != nullptr) ++b;
+                    }
+                    e->row_req[b] = r;
+                    e->row_choice[b] = c;
+                    r->rows.push_back(b);
+                    if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this chunk; set again once it succeeds
+                    tail_seq.push_back((int)chunk.size()); tail_slot.push_back(b); tail_choice.push_back(c);
+                    tail_gen.push_back(&r->gen);
+                }
                 chunk.push_back(r);
-                gen.push_back(&r->gen);
-                slots.push_back(b);
+                slots.push_back(r->rows[0]);
                 chunk_mode |= step_mode(r->gen);
                 ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
                 seq_start.push_back((int)ids.size());
-                ++active;
+                active += r->n_choices;
             }
             e->st.queued = (int)e->waiting.size();
             e->st.active_rows = active;
@@ -843,34 +917,41 @@ static void worker_main(rr_engine* e) {
             if (e->index_epoch != epoch) {
                 for (size_t i = chunk.size(); i-- > 0;) {
                     Request* r = chunk[i];
-                    e->row_req[r->slot] = nullptr;
-                    r->slot = -1; r->n_cached = 0;
+                    for (int b : r->rows) e->row_req[b] = nullptr;
+                    r->rows.clear(); r->n_cached = 0;
                     e->waiting.push_front(r);
                 }
                 continue;
             }
         }
         if (!chunk.empty()) {
+            PrefillTail tail;
+            tail.n = (int)tail_seq.size(); tail.seq = tail_seq.data(); tail.slot = tail_slot.data();
+            tail.choice = tail_choice.data(); tail.gen = tail_gen.data(); tail.mode = chunk_mode;
             int rc = (chunk_mode & 4) ? ensure_pen_buffers(e) : RR_OK;
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, gen.data(), chunk_mode);
+                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, &tail);
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
-            for (size_t i = 0; i < chunk.size(); ++i) {
-                Request* r = chunk[i];
+            int j = 0;                                     // the request's first tail row
+            for (Request* r : chunk) {
+                const int row0 = j;
+                j += r->n_choices;
                 if (rc != RR_OK) {
-                    release_row(e, r->slot, RR_INTERNAL, &notes);
+                    release_request(e, r, RR_INTERNAL, &notes);
                     continue;
                 }
-                if (e->o.prefix_cache) {
-                    e->retained[r->slot] = r->prompt;
-                    e->retained_used[r->slot] = ++e->lru_clock;
+                if (e->o.prefix_cache) {                   // every choice's slot holds the prompt's prefill-written KV
+                    for (int b : r->rows) { e->retained[b] = r->prompt; e->retained_used[b] = ++e->lru_clock; }
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
                 r->t_first = t;
-                if (take_token(e, r, (int)i)) release_row(e, r->slot, RR_OK, &notes);
-                else set_row_params(e, r->slot, r);
+                bool done = false;
+                for (int c = 0; c < r->n_choices; ++c) done = take_token(e, r, c, row0 + c);
+                if (done) release_request(e, r, RR_OK, &notes);
+                else
+                    for (int c = 0; c < r->n_choices; ++c) set_row_params(e, r->rows[c], r, c);
             }
             e->cv_done.notify_all();
             continue;   // look for more waiting prompts before decoding
@@ -898,11 +979,11 @@ static void worker_main(rr_engine* e) {
         e->st.decode_steps += 1;
         {
             std::lock_guard<std::mutex> lk(e->mu);
-            for (int b = 0; b < e->Bm; ++b) {
+            for (int b = 0; b < e->Bm; ++b) {              // a released request's later rows are already free
                 Request* r = e->row_req[b];
                 if (!r) continue;
-                if (rc != RR_OK) release_row(e, b, RR_INTERNAL, &notes);
-                else if (take_token(e, r, b)) release_row(e, b, RR_OK, &notes);
+                if (rc != RR_OK) release_request(e, r, RR_INTERNAL, &notes);
+                else if (take_token(e, r, e->row_choice[b], b)) release_request(e, r, RR_OK, &notes);
             }
         }
         e->cv_done.notify_all();
@@ -985,7 +1066,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         if (ks > 1) TRY(dalloc(e, &e->attn_ws, decode_attn_ws_bytes(B, d.n_heads, ks) / sizeof(float)));
     }
     const int T = e->Tmax;
-    TRY(dalloc(e, &e->p_ids, (size_t)3 * T + 4 * B + 8));
+    TRY(dalloc(e, &e->p_ids, (size_t)3 * T + 6 * B + 8));
     TRY(dalloc(e, &e->p_first, B));
     TRY(dalloc(e, &e->px, (size_t)T * d.hidden, false));
     TRY(dalloc(e, &e->pxn, (size_t)T * d.hidden, false));
@@ -994,7 +1075,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->pattn, (size_t)T * e->nq, false));
     TRY(dalloc(e, &e->pgu, (size_t)T * 2 * d.inter, false));
     TRY(dalloc(e, &e->pact, (size_t)T * d.inter, false));
-    TRYC(cudaMallocHost(&e->h_stage, ((size_t)3 * T + 4 * B + 8) * sizeof(int32_t)));
+    TRYC(cudaMallocHost(&e->h_stage, ((size_t)3 * T + 6 * B + 8) * sizeof(int32_t)));
     TRYC(cudaMallocHost(&e->h_tok, sizeof(int32_t) * (B > 16 ? B : 16)));
     TRY(dalloc(e, (char**)&e->lp_ws, logprobs_ws_bytes(B, d.vocab), false));
     TRY(dalloc(e, &e->d_lp, (size_t)B * LP_MAX_TOP)); TRY(dalloc(e, &e->d_lp_id, (size_t)B * LP_MAX_TOP));
@@ -1072,6 +1153,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     }
     TRYC(cudaDeviceSynchronize());
     e->row_req.assign(B, nullptr);
+    e->row_choice.assign(B, 0);
     e->h_slot_mirror.assign(B, -1);
     if (e->o.prefix_cache) { e->retained.assign(B, {}); e->retained_used.assign(B, 0); }
     e->worker = std::thread(worker_main, e);
@@ -1165,8 +1247,9 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
 
 namespace rr {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, const GenParams& p) {
+                         uint64_t* ticket, const GenParams& p, int n_choices) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
+    if (n_choices < 1 || n_choices > e->Bm) return RR_INVALID_ARGUMENT;      // the choices decode side by side
     // the vocabularies the logprobs / sampling kernels handle
     if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
@@ -1177,13 +1260,18 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     if (!r) return RR_INTERNAL;
     r->prompt.assign(prompt_ids, prompt_ids + n_prompt);
     r->max_new = max_new_tokens;
-    r->out.reserve(max_new_tokens);
+    r->n_choices = n_choices;
+    r->out.resize(n_choices);
+    r->lp.resize(n_choices); r->lp_id.resize(n_choices);
+    for (int c = 0; c < n_choices; ++c) {
+        r->out[c].reserve(max_new_tokens);
+        if (p.logprobs()) {
+            const size_t k = p.lp_width();
+            r->lp[c].reserve(k * max_new_tokens); r->lp_id[c].reserve(k * max_new_tokens);
+        }
+    }
     r->tag = tag;
     r->gen = p;
-    if (p.logprobs()) {
-        const size_t k = p.lp_width();
-        r->lp.reserve(k * max_new_tokens); r->lp_id.reserve(k * max_new_tokens);
-    }
     std::vector<DoneNote> notes;
     {
         std::lock_guard<std::mutex> lk(e->mu);
@@ -1207,8 +1295,9 @@ void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx) {
     std::lock_guard<std::mutex> lk(e->mu);
     e->hook = fn; e->hook_ctx = ctx;
 }
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab) {
+int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch) {
     if (!e) return RR_INVALID_ARGUMENT;
+    if (max_batch) *max_batch = e->Bm;
     if (ctx_max) *ctx_max = e->o.ctx_max;
     if (max_prefill) *max_prefill = e->Tmax;
     if (vocab) *vocab = e->d.vocab;
@@ -1216,15 +1305,23 @@ int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab
 }
 }  // namespace rr
 
-RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                      int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                      float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                      const float* bias_vals, uint64_t* ticket) {
+RR_API int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                    int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                    float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                    const float* bias_vals, uint64_t* ticket) {
     if (!e) return RR_INVALID_ARGUMENT;
     rr::GenParams p;
     const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
                          bias_ids, bias_vals);
-    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p);
+    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
+}
+
+RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                      int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                      float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                      const float* bias_vals, uint64_t* ticket) {
+    return rr_engine_submit_choices(e, prompt_ids, n_prompt, max_new_tokens, 1, top_logprobs, temperature, top_p, seed,
+                                    frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, ticket);
 }
 
 RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
@@ -1245,16 +1342,23 @@ RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int
                                       0.f, 0, nullptr, nullptr, ticket);
 }
 
-// Caller holds e->mu.  The first min(n, max_tokens_out) tokens' pairs of a logprobs request into [max_tokens_out][K].
-static void copy_logprobs(const Request* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
+// Caller holds e->mu.  The first min(n, max_tokens_out) tokens of each choice of r into tokens_out [n_choices]
+// [max_tokens_out], and of a logprobs request their pairs into lp_out / id_out [n_choices][max_tokens_out][K] (any may
+// be null).
+static void copy_choices(const Request* r, int n, int max_tokens_out, int32_t* tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (!r->gen.logprobs() || t <= 0) return;
-    const size_t m = (size_t)t * r->gen.lp_width();
-    if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
-    if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
+    if (t <= 0) return;
+    const size_t k = (size_t)r->gen.lp_width();
+    for (int c = 0; c < r->n_choices; ++c) {
+        const size_t o = (size_t)c * max_tokens_out;
+        if (tokens_out) memcpy(tokens_out + o, r->out[c].data(), sizeof(int32_t) * t);
+        if (!r->gen.logprobs()) continue;
+        if (lp_out) memcpy(lp_out + o * k, r->lp[c].data(), sizeof(float) * t * k);
+        if (id_out) memcpy(id_out + o * k, r->lp_id[c].data(), sizeof(int32_t) * t * k);
+    }
 }
 
-// Abandon a request (client gone / timed out): a queued request is dropped, a running one gives up its decode row at the
+// Abandon a request (client gone / timed out): a queued request is dropped, a running one gives up its decode rows at the
 // next step; a finished one is just freed.  The ticket is consumed: do not wait on it afterwards.
 RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
     if (!e) return RR_INVALID_ARGUMENT;
@@ -1273,7 +1377,7 @@ RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
             for (auto q = e->waiting.begin(); q != e->waiting.end(); ++q)
                 if (*q == r) { e->waiting.erase(q); queued = true; break; }
             if (queued) finish_request(e, r, RR_CANCELLED, &notes);      // frees it (detached)
-            else r->cancel = true;                                       // active row: the worker drops it
+            else r->cancel = true;                                       // active rows: the worker drops them
         }
     }
     e->cv_work.notify_one();
@@ -1283,7 +1387,8 @@ RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
 }
 
 // Streaming support: block until the request has more than `have` tokens (or is done / the wait times out), then
-// copy the tokens generated so far.  Does not consume the request; finish with rr_engine_wait.
+// copy the tokens generated so far.  Does not consume the request; finish with rr_engine_wait.  A request of several
+// choices gets RR_INVALID_ARGUMENT.
 RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
                                    int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
                                    float* lp_out, int32_t* id_out) {
@@ -1297,7 +1402,8 @@ RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, doub
         auto it = e->table.find(ticket);
         if (it == e->table.end()) return RR_INVALID_ARGUMENT;
         r = it->second;
-        if (r->done || (int)r->out.size() > have) break;
+        if (r->n_choices > 1) return RR_INVALID_ARGUMENT;
+        if (r->done || r->n_generated() > have) break;
         if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
             it = e->table.find(ticket);
             if (it == e->table.end()) return RR_INVALID_ARGUMENT;
@@ -1305,15 +1411,11 @@ RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, doub
             break;
         }
     }
-    const int n = (int)r->out.size();
+    const int n = r->n_generated();
     *n_generated = n;
     *done = r->done ? 1 : 0;
     if (t_first_token_s) *t_first_token_s = r->t_first - r->t_submit;
-    if (tokens_out) {
-        const int m = n < max_tokens_out ? n : max_tokens_out;
-        memcpy(tokens_out, r->out.data(), sizeof(int32_t) * m);
-    }
-    copy_logprobs(r, n, max_tokens_out, lp_out, id_out);
+    copy_choices(r, n, max_tokens_out, tokens_out, lp_out, id_out);
     return RR_OK;
 }
 
@@ -1323,8 +1425,10 @@ RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeou
                                    t_first_token_s, nullptr, nullptr);
 }
 
-RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
-                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+// rr_engine_wait_choices, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
+// choices, which stays in flight.
+static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                       int max_tokens_out, float* lp_out, int32_t* id_out, bool choices) {
     if (!e || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1334,6 +1438,7 @@ RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout
         auto it = e->table.find(ticket);
         if (it == e->table.end()) return RR_INVALID_ARGUMENT;      // unknown, already consumed, or cancelled
         r = it->second;
+        if (!choices && r->n_choices > 1) return RR_INVALID_ARGUMENT;
         if (r->done) break;
         if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
             it = e->table.find(ticket);
@@ -1344,17 +1449,23 @@ RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout
         }
     }
     out->ticket = ticket; out->status = r->status; out->n_prompt = (int)r->prompt.size();
-    out->n_generated = (int)r->out.size(); out->n_cached = r->n_cached;
+    out->n_generated = r->n_generated(); out->n_cached = r->n_cached;
     out->t_submit_s = r->t_submit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
-    if (tokens_out) {
-        const int n = (int)r->out.size() < max_tokens_out ? (int)r->out.size() : max_tokens_out;
-        memcpy(tokens_out, r->out.data(), sizeof(int32_t) * n);
-    }
-    copy_logprobs(r, (int)r->out.size(), max_tokens_out, lp_out, id_out);
+    copy_choices(r, r->n_generated(), max_tokens_out, tokens_out, lp_out, id_out);
     const int status = r->status;
     e->table.erase(ticket);
     delete r;
     return status == RR_OK ? RR_OK : status;
+}
+
+RR_API int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
+                                  int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true);
+}
+
+RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
+                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, false);
 }
 
 RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,

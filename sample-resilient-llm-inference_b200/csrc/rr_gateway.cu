@@ -39,6 +39,7 @@ enum ReqState { Q_ADMIT = 0, RUNNING = 1, FINISHED = 2 };
 struct GwReq {
     uint64_t id = 0;
     int group = 0, max_new = 0;
+    int n_choices = 1;                // handed with gen to every engine the request is admitted to
     std::vector<int32_t> prompt;
     int chain_start = 0, attempts = 0;
     ReqState state = Q_ADMIT;
@@ -46,13 +47,15 @@ struct GwReq {
     int deployment = -1, served_group = -1, chain_pos = 0, replica = -1;
     rr_engine* eng = nullptr;
     uint64_t eng_ticket = 0;
-    std::vector<int32_t> tokens;
+    std::vector<int32_t> tokens;      // [n_choices][n_gen()]
     rr::GenParams gen;                // handed to every engine the request is admitted to
-    std::vector<float> lp;            // [tokens.size()][gen.lp_width()]
+    std::vector<float> lp;            // [n_choices][n_gen()][gen.lp_width()]
     std::vector<int32_t> lp_id;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;   // t_eng_submit: hand-off to the replica
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
+
+    int n_gen() const { return (int)tokens.size() / n_choices; }      // tokens per choice
 };
 
 struct Pending {
@@ -74,7 +77,7 @@ struct rr_gateway {
     std::unordered_map<int, int> by_replica;   // replica id -> index into engines
     int n_deps = 0, n_groups = 0;
     bool latency = false;                   // the router is latency-based: DONE / FAIL events carry samples
-    int min_ctx = 0, min_pf = 0, min_vocab = 0;
+    int min_ctx = 0, min_pf = 0, min_vocab = 0, min_rows = 0;     // min_rows: decode rows, the limit of n_choices
     rr_gateway_opts opts;
 
     std::mutex mu;
@@ -118,20 +121,25 @@ static void gw_finish(rr_gateway* g, GwReq* r, int status) {
     }
 }
 
-// caller holds g->mu.  Request r ended on the replica it was handed to with `status` (n_generated tokens by then).  When
-// the replica's record of it was read (wrc RR_OK / RR_BACKEND_FAILED: comp, toks, and with logprobs lps / lp_ids), the
-// result is stored.  Then DONE (with the latency sample) / FAIL / the cancel report is posted and the request finishes,
+// caller holds g->mu.  Request r ended on the replica it was handed to with `status` (n_generated tokens by then, over all
+// choices).  When the replica's record of it was read (wrc RR_OK / RR_BACKEND_FAILED: comp, toks [n_choices][max_new],
+// and with logprobs lps / lp_ids [n_choices][max_new][K]), the result is stored.  Then DONE (with the latency sample) / FAIL / the cancel report is posted and the request finishes,
 // or after a backend failure goes back into the queue one step further down its fallback chain.
 static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int wrc, const rr_completion& comp,
                       const int32_t* toks, const float* lps, const int32_t* lp_ids) {
     const int dep = r->deployment;
     if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
-        const int n = comp.n_generated < r->max_new ? comp.n_generated : r->max_new;
-        r->tokens.assign(toks, toks + (n > 0 ? n : 0));
-        if (r->gen.logprobs()) {
-            const size_t m = r->tokens.size() * (size_t)r->gen.lp_width();
-            r->lp.assign(lps, lps + m);
-            r->lp_id.assign(lp_ids, lp_ids + m);
+        int n = comp.n_generated < r->max_new ? comp.n_generated : r->max_new;
+        n = n > 0 ? n : 0;
+        const size_t k = (size_t)r->gen.lp_width();
+        r->tokens.clear(); r->lp.clear(); r->lp_id.clear();
+        for (int c = 0; c < r->n_choices; ++c) {
+            const size_t o = (size_t)c * r->max_new;
+            r->tokens.insert(r->tokens.end(), toks + o, toks + o + n);
+            if (r->gen.logprobs()) {
+                r->lp.insert(r->lp.end(), lps + o * k, lps + (o + n) * k);
+                r->lp_id.insert(r->lp_id.end(), lp_ids + o * k, lp_ids + (o + n) * k);
+            }
         }
         r->t_first = r->t_eng_submit + (comp.t_first_token_s - comp.t_submit_s);
         r->n_cached = comp.n_cached;
@@ -177,7 +185,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     rr_engine* eng = nullptr;
     int max_new = 0;
     bool logprobs = false;
-    size_t k = 1;
+    size_t k = 1, n_ch = 1;
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -187,17 +195,18 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         max_new = r->max_new;
         logprobs = r->gen.logprobs();
         k = (size_t)r->gen.lp_width();
+        n_ch = (size_t)r->n_choices;
     }
     // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
     memset(&comp, 0, sizeof(comp));
-    std::vector<int32_t> toks((size_t)(max_new > 0 ? max_new : 1));
+    std::vector<int32_t> toks(n_ch * (size_t)(max_new > 0 ? max_new : 1));
     std::vector<float> lps(logprobs ? toks.size() * k : 0);
     std::vector<int32_t> lp_ids(lps.size());
     int wrc = RR_INVALID_ARGUMENT;
     if (eng && status != RR_CANCELLED)
-        wrc = rr_engine_wait_logprobs(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
-                                      logprobs ? lp_ids.data() : nullptr);
+        wrc = rr_engine_wait_choices(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
+                                     logprobs ? lp_ids.data() : nullptr);
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -208,8 +217,8 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     g->cv_done.notify_all();
 }
 
-// Dispatcher thread, caller holds g->mu: mock replica `rep` serves request r (handed to it at r->t_eng_submit) at once.
-// Its latency sample is the gateway's hand-off -> settle time.
+// Dispatcher thread, caller holds g->mu: mock replica `rep` serves request r (handed to it at r->t_eng_submit) at once,
+// with the same reply for every choice.  Its latency sample is the gateway's hand-off -> settle time.
 static void gw_serve_stub(rr_gateway* g, GwReq* r, int rep) {
     const rr_stub_desc& s = g->stubs[(size_t)rep];
     const uint64_t n = ++g->stub_handed[(size_t)rep];
@@ -217,12 +226,13 @@ static void gw_serve_stub(rr_gateway* g, GwReq* r, int rep) {
     rr_completion comp;
     memset(&comp, 0, sizeof(comp));
     comp.n_generated = failed ? 0 : (r->max_new < s.reply_tokens ? r->max_new : s.reply_tokens);
-    std::vector<int32_t> toks((size_t)comp.n_generated);
-    for (int i = 0; i < comp.n_generated; ++i) toks[(size_t)i] = 3 + (i % 200);
+    std::vector<int32_t> toks((size_t)r->n_choices * r->max_new);
+    for (int c = 0; c < r->n_choices; ++c)
+        for (int i = 0; i < comp.n_generated; ++i) toks[(size_t)c * r->max_new + i] = 3 + (i % 200);
     comp.t_submit_s = r->t_eng_submit;
     comp.t_first_token_s = comp.t_done_s = gw_now_s(g);
     const int status = failed ? RR_BACKEND_FAILED : RR_OK;
-    gw_settle(g, r, status, comp.n_generated, status, comp, toks.data(), nullptr, nullptr);
+    gw_settle(g, r, status, comp.n_generated * r->n_choices, status, comp, toks.data(), nullptr, nullptr);
 }
 
 static void gw_dispatch(rr_gateway* g) {
@@ -313,7 +323,8 @@ static void gw_dispatch(rr_gateway* g) {
             uint64_t tk = 0;
             int src = RR_INTERNAL;
             if (!cancelled && eng)
-                src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk, r->gen);
+                src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk, r->gen,
+                                               r->n_choices);
             bool cancel_now = false;
             std::unique_lock<std::mutex> lk(g->mu);
             if (src == RR_OK) {
@@ -354,15 +365,15 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
     memset(&g->st, 0, sizeof(g->st));
     rr::router_shape(router, &g->n_deps, &g->n_groups);
     g->latency = rr::router_strategy(router) == RR_STRATEGY_LATENCY_BASED;
-    g->min_ctx = g->min_pf = g->min_vocab = 0x7fffffff;
+    g->min_ctx = g->min_pf = g->min_vocab = g->min_rows = 0x7fffffff;
     g->stubs.assign((size_t)n_engines, rr_stub_desc{0, 0, 0, 0});
     g->stub_handed.assign((size_t)n_engines, 0);
     for (int i = 0; i < n_engines; ++i) {
         g->engines.push_back(engines[i]);
         g->by_replica[replica_ids[i]] = i;
-        int c = 0x7fffffff, p = 0x7fffffff, v = 0;
+        int c = 0x7fffffff, p = 0x7fffffff, v = 0, rows = 0x7fffffff;
         if (engines[i]) {
-            rr::engine_limits(engines[i], &c, &p, &v);
+            rr::engine_limits(engines[i], &c, &p, &v, &rows);
         } else {
             if (!stubs || stubs[i].reply_tokens < 0 || stubs[i].fail_every < 0 || stubs[i].vocab < 1) {
                 delete g;
@@ -375,6 +386,7 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
         if (c < g->min_ctx) g->min_ctx = c;
         if (p < g->min_pf) g->min_pf = p;
         if (v < g->min_vocab) g->min_vocab = v;
+        if (rows < g->min_rows) g->min_rows = rows;
     }
     if (g->opts.record_trace > 0) {
         g->tr_ev.resize((size_t)g->opts.record_trace);
@@ -408,9 +420,10 @@ RR_API int rr_gateway_set_now(rr_gateway* g, int64_t now_ms) {
     return RR_OK;
 }
 
-static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, int max_new) {
+static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, int max_new, int n_choices) {
     if (group < 0 || group >= g->n_groups) return RR_NO_GROUP;
     if (!ids || n_prompt < 1 || max_new < 1) return RR_INVALID_ARGUMENT;
+    if (n_choices < 1 || n_choices > g->min_rows) return RR_INVALID_ARGUMENT;     // every choice takes a decode row
     if (n_prompt + max_new > g->min_ctx || n_prompt > g->min_pf) return RR_INVALID_ARGUMENT;   // -> HTTP 400, before any debit
     for (int i = 0; i < n_prompt; ++i)
         if (ids[i] < 0 || ids[i] >= g->min_vocab) return RR_INVALID_ARGUMENT;
@@ -419,17 +432,18 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
 
 // p is checked (GenParams::set) against the smallest vocabulary, as prompt ids are: any engine of a fallback accepts it.
 static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
-                     int max_new_tokens, int declare_burst, const rr::GenParams& p, uint64_t* tickets) {
+                     int max_new_tokens, int declare_burst, const rr::GenParams& p, int n_choices, uint64_t* tickets) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n; ++i) {
-        const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens);
+        const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens,
+                                n_choices);
         if (rc != RR_OK) return rc;
     }
     std::vector<GwReq*> reqs((size_t)n);
     for (int i = 0; i < n; ++i) {
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
-        r->group = group; r->max_new = max_new_tokens; r->gen = p;
+        r->group = group; r->max_new = max_new_tokens; r->gen = p; r->n_choices = n_choices;
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -453,15 +467,15 @@ static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const 
 
 RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
                                    int max_new_tokens, int declare_burst, uint64_t* tickets) {
-    return gw_submit(g, group, prompt_ids, prompt_start, n, max_new_tokens, declare_burst, rr::GenParams(), tickets);
+    return gw_submit(g, group, prompt_ids, prompt_start, n, max_new_tokens, declare_burst, rr::GenParams(), 1, tickets);
 }
 
 // The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
 // gets RR_INVALID_ARGUMENT.
-RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
-                                       int max_new_tokens, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                       float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                       const float* bias_vals, uint64_t* ticket) {
+RR_API int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                     int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                     float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                     const float* bias_vals, uint64_t* ticket) {
     if (!g) return RR_INVALID_ARGUMENT;
     rr::GenParams p;
     const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
@@ -469,7 +483,15 @@ RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* 
     if (rc != RR_OK) return rc;
     if (p.logprobs() && g->has_stub) return RR_INVALID_ARGUMENT;     // a mock replica has no logits to fill the pairs from
     const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, ticket);
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
+}
+
+RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
+                                       int max_new_tokens, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                       float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                       const float* bias_vals, uint64_t* ticket) {
+    return rr_gateway_submit_choices(g, group, prompt_ids, n_prompt, max_new_tokens, 1, top_logprobs, temperature, top_p,
+                                     seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, ticket);
 }
 
 RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
@@ -490,26 +512,35 @@ RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* pr
                                        0.f, 0.f, 0, nullptr, nullptr, ticket);
 }
 
-// caller holds g->mu.  The pairs of the first min(n, max_tokens_out) tokens into [max_tokens_out][r->gen.lp_width()].
-static void gw_copy_logprobs(const GwReq* r, int n, int max_tokens_out, float* lp_out, int32_t* id_out) {
+// caller holds g->mu.  The first min(n, max_tokens_out) tokens of each choice into tokens_out [n_choices][max_tokens_out],
+// and of a logprobs request their pairs into lp_out / id_out [n_choices][max_tokens_out][r->gen.lp_width()] (any may be
+// null).
+static void gw_copy_choices(const GwReq* r, int n, int max_tokens_out, int32_t* tokens_out, float* lp_out, int32_t* id_out) {
     const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (!r->gen.logprobs() || t <= 0) return;
-    const size_t m = (size_t)t * r->gen.lp_width();
-    if (lp_out) memcpy(lp_out, r->lp.data(), sizeof(float) * m);
-    if (id_out) memcpy(id_out, r->lp_id.data(), sizeof(int32_t) * m);
+    if (t <= 0) return;
+    const size_t k = (size_t)r->gen.lp_width(), have = (size_t)r->n_gen();
+    for (int c = 0; c < r->n_choices; ++c) {
+        const size_t o = (size_t)c * max_tokens_out, src = (size_t)c * have;
+        if (tokens_out) memcpy(tokens_out + o, r->tokens.data() + src, sizeof(int32_t) * (size_t)t);
+        if (!r->gen.logprobs()) continue;
+        if (lp_out) memcpy(lp_out + o * k, r->lp.data() + src * k, sizeof(float) * t * k);
+        if (id_out) memcpy(id_out + o * k, r->lp_id.data() + src * k, sizeof(int32_t) * t * k);
+    }
 }
 
 static void gw_fill(const GwReq* r, rr_gateway_result* out) {
     out->ticket = r->id; out->status = r->state == FINISHED ? r->status : -1;
     out->deployment = r->deployment; out->served_group = r->served_group; out->chain_pos = r->chain_pos;
-    out->replica = r->replica; out->n_prompt = (int32_t)r->prompt.size(); out->n_generated = (int32_t)r->tokens.size();
+    out->replica = r->replica; out->n_prompt = (int32_t)r->prompt.size(); out->n_generated = (int32_t)r->n_gen();
     out->attempts = r->attempts;
     out->t_submit_s = r->t_submit; out->t_admit_s = r->t_admit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
     out->n_cached = r->n_cached; out->reserved = 0;
 }
 
-RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
-                                    int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+// rr_gateway_wait_choices, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
+// choices, which stays in flight.
+static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                   int max_tokens_out, float* lp_out, int32_t* id_out, bool choices) {
     if (!g || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(g->mu);
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
@@ -518,6 +549,7 @@ RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeo
         auto it = g->table.find(ticket);
         if (it == g->table.end()) return RR_INVALID_ARGUMENT;
         r = it->second;
+        if (!choices && r->n_choices > 1) return RR_INVALID_ARGUMENT;
         if (r->state == FINISHED) break;
         if (g->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
             it = g->table.find(ticket);
@@ -530,15 +562,21 @@ RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeo
         }
     }
     gw_fill(r, out);
-    if (tokens_out) {
-        const int n = (int)r->tokens.size() < max_tokens_out ? (int)r->tokens.size() : max_tokens_out;
-        if (n > 0) memcpy(tokens_out, r->tokens.data(), sizeof(int32_t) * (size_t)n);
-    }
-    gw_copy_logprobs(r, (int)r->tokens.size(), max_tokens_out, lp_out, id_out);
+    gw_copy_choices(r, r->n_gen(), max_tokens_out, tokens_out, lp_out, id_out);
     const int status = r->status;
     g->table.erase(ticket);
     delete r;
     return status;
+}
+
+RR_API int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
+                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true);
+}
+
+RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
+                                    int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
+    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, false);
 }
 
 RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
@@ -560,12 +598,12 @@ RR_API int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, do
                 auto it = g->table.find(ticket);
                 if (it == g->table.end()) return RR_INVALID_ARGUMENT;
                 GwReq* r = it->second;
+                if (r->n_choices > 1) return RR_INVALID_ARGUMENT;
                 if (out) gw_fill(r, out);
                 if (r->state == FINISHED) {
-                    const int n = (int)r->tokens.size();
+                    const int n = r->n_gen();
                     *n_generated = n; *done = 1;
-                    if (tokens_out && n > 0) memcpy(tokens_out, r->tokens.data(), sizeof(int32_t) * (size_t)(n < max_tokens_out ? n : max_tokens_out));
-                    gw_copy_logprobs(r, n, max_tokens_out, lp_out, id_out);
+                    gw_copy_choices(r, n, max_tokens_out, tokens_out, lp_out, id_out);
                     return RR_OK;
                 }
                 if (r->state == RUNNING) { eng = r->eng; tk = r->eng_ticket; break; }

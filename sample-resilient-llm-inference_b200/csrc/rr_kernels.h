@@ -98,10 +98,11 @@ struct GenParams {
     int set(int vocab, int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
             float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals);
 };
+// n_choices (1..max_batch): choices of the request (rr_engine_submit_choices); the done hook's n_generated is their total.
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
-                         uint64_t* ticket, const GenParams& p);
+                         uint64_t* ticket, const GenParams& p, int n_choices);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab);
+int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
 int router_strategy(const rr_router* r);

@@ -7,7 +7,7 @@ computation happens in the CUDA library.  Replaces one `bedrock/...` deployment 
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -32,6 +32,9 @@ class CompletionRecord:
     logprobs: Optional[List[List[Tuple[int, float]]]] = None
     # prompt tokens whose KV came from the prefix cache (Engine(prefix_cache=True)); 0 otherwise
     n_cached: int = 0
+    # submit(n=k): every choice's tokens and, with top_logprobs, pairs ([k][tokens]); tokens / logprobs are choice 0's
+    choices: List[List[int]] = field(default_factory=list)
+    choice_logprobs: Optional[List[List[List[Tuple[int, float]]]]] = None
 
     @property
     def ttft(self) -> float:
@@ -64,6 +67,7 @@ class Engine:
         self.device = device
         self.max_batch = max_batch
         self.ctx_max = ctx_max
+        self.max_prefill_tokens = max_prefill_tokens
         self.prefix_cache = bool(prefix_cache)
         s = self.spec
         desc = _lib.ModelDesc(s.vocab, s.hidden, s.inter, s.n_layers, s.n_heads, s.n_kv_heads,
@@ -101,6 +105,7 @@ class Engine:
                                1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
+        self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -147,44 +152,55 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
                temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None,
                frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-               logit_bias: Optional[Dict[int, float]] = None) -> int:
+               logit_bias: Optional[Dict[int, float]] = None, n: int = 1) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
         rr_engine_submit_sampled; None or 0 is greedy.  frequency_penalty / presence_penalty in [-2, 2] and logit_bias
         {token id: bias in [-100, 100]} (at most 300 entries): applied to the logits before every token is picked, the
-        penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing."""
+        penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing.
+        n in 1..max_batch: n choices of the prompt, prefilled once (rr_engine_submit_choices); choice i is drawn with
+        seed + i.  wait() returns them all; peek() is for n = 1 only."""
         ids = _i32(prompt_ids)
         bias = logit_bias or {}
         gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
                        list(bias.values()))
         t = C.c_uint64()
-        _lib.check(_lib.lib.rr_engine_submit_processed(self._h, _p(ids), len(ids), max_new_tokens, *gen.tail, C.byref(t)),
-                   "rr_engine_submit_processed")
+        if n == 1:
+            _lib.check(_lib.lib.rr_engine_submit_processed(self._h, _p(ids), len(ids), max_new_tokens, *gen.tail,
+                                                           C.byref(t)), "rr_engine_submit_processed")
+        else:
+            _lib.check(_lib.lib.rr_engine_submit_choices(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail,
+                                                         C.byref(t)), "rr_engine_submit_choices")
+            self._n[t.value] = n
         if gen.width:
             self._lp_k[t.value] = gen.width
         return t.value
 
-    def _lp_bufs(self, ticket: int, max_tokens: int):
+    def _lp_bufs(self, ticket: int, max_tokens: int, n: int = 1):
         k = self._lp_k.get(ticket)
         if k is None:
             return None, None, None, None
-        lp, ids = np.zeros((max_tokens, k), dtype=np.float32), np.zeros((max_tokens, k), dtype=np.int32)
+        lp, ids = np.zeros((n, max_tokens, k), dtype=np.float32), np.zeros((n, max_tokens, k), dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), _p(ids)
 
     def wait(self, ticket: int, timeout: float = 0.0, max_tokens: int = 4096) -> CompletionRecord:
         c = _lib.Completion()
-        buf = np.zeros(max_tokens, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens)
-        rc = _lib.lib.rr_engine_wait_logprobs(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
+        nc = self._n.get(ticket, 1)
+        buf = np.zeros((nc, max_tokens), dtype=np.int32)
+        lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens, nc)
+        wait = _lib.lib.rr_engine_wait_choices if nc > 1 else _lib.lib.rr_engine_wait_logprobs
+        rc = wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
         if rc != 6:
             self._lp_k.pop(ticket, None)
+            self._n.pop(ticket, None)
         if rc not in (0, 6, 7):
             _lib.check(rc, "rr_engine_wait")
         n = min(c.n_generated, max_tokens)
-        return CompletionRecord(ticket, rc, c.n_prompt, buf[:c.n_generated].tolist(), c.t_submit_s,
-                                c.t_first_token_s, c.t_done_s, logprob_pairs(lp, ids, 0, n) if lp is not None else None,
-                                c.n_cached)
+        toks = [row[:n].tolist() for row in buf]
+        pairs = [logprob_pairs(a, b, 0, n) for a, b in zip(lp, ids)] if lp is not None else None
+        return CompletionRecord(ticket, rc, c.n_prompt, toks[0], c.t_submit_s, c.t_first_token_s, c.t_done_s,
+                                pairs[0] if pairs else None, c.n_cached, toks, pairs)
 
     def peek(self, ticket: int, have: int, timeout: float = 0.05, max_tokens: int = 4096):
         """Streaming: wait until more than `have` tokens exist (or done / timeout). -> (tokens so far, done, ttft_s), and
@@ -192,6 +208,7 @@ class Engine:
         buf = np.zeros(max_tokens, dtype=np.int32)
         n, done, ttft = C.c_int32(), C.c_int32(), C.c_double()
         lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens)
+        lp, ids = (None, None) if lp is None else (lp[0], ids[0])
         _lib.check(_lib.lib.rr_engine_peek_logprobs(self._h, ticket, have, float(timeout), _p(buf), max_tokens, C.byref(n),
                                                     C.byref(done), C.byref(ttft), lp_p, ids_p), "rr_engine_peek")
         if lp is None:

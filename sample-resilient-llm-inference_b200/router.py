@@ -98,6 +98,7 @@ class ModelResponse:
     _fell_back: bool = False
     _ttft_s: float = 0.0
     _latency_s: float = 0.0
+    _choice_token_ids: List[List[int]] = field(default_factory=list)     # every choice's tokens, choices[i] <-> [i]
 
     def model_dump(self) -> dict:
         return {"id": self.id, "object": self.object, "created": self.created, "model": self.model,
@@ -233,6 +234,19 @@ def check_penalties(frequency_penalty: Any = None, presence_penalty: Any = None,
     if fp == 0 and pp == 0 and not ids:
         return None
     return fp, pp, ids, vals
+
+
+MAX_N = 128                  # OpenAI's range for `n`: 1..128
+
+
+def check_n(n: Any) -> int:
+    """OpenAI's rule for the `n` request field (the number of choices) -> 1 when absent, else the integer in 1..128.
+    Raises BadRequestError (HTTP 400) for anything else, bools and floats included."""
+    if n is None:
+        return 1
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= MAX_N:
+        raise BadRequestError(f"`n` must be an integer from 1 to {MAX_N}")
+    return n
 
 
 class GenArgs(NamedTuple):
@@ -417,15 +431,39 @@ class Router:
         return Usage(n_prompt, n_gen, n_prompt + n_gen, details)
 
     def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None) -> ModelResponse:
+        """toks [n choices][max_new] (or one row), logprobs: one `logprobs` object per choice (or None)."""
         d = self.cfg.deployments[res.deployment]
-        toks = [int(t) for t in toks[: res.n_generated]]
+        rows = [[int(t) for t in row[: res.n_generated]] for row in np.atleast_2d(toks)]
+        lps = logprobs if isinstance(logprobs, list) else [logprobs] * len(rows)
         return ModelResponse(
             id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-            choices=[Choice(0, Message("assistant", detokenize(toks) if detok else ""), logprobs=logprobs)],
-            usage=self._usage(res.deployment, n_prompt, len(toks), res.n_cached), created=int(time.time()),
-            _token_ids=toks, _deployment=res.deployment, _model_group=self.cfg.groups[res.served_group],
+            choices=[Choice(i, Message("assistant", detokenize(t) if detok else ""), logprobs=lp)
+                     for i, (t, lp) in enumerate(zip(rows, lps))],
+            usage=self._usage(res.deployment, n_prompt, sum(len(t) for t in rows), res.n_cached), created=int(time.time()),
+            _token_ids=rows[0], _deployment=res.deployment, _model_group=self.cfg.groups[res.served_group],
             _fell_back=res.chain_pos > 0, _ttft_s=res.t_first_token_s - res.t_submit_s,
-            _latency_s=time.perf_counter() - t_start)
+            _latency_s=time.perf_counter() - t_start, _choice_token_ids=rows)
+
+    def _limits(self) -> Tuple[int, int, int]:
+        """(context window, prefill chunk, decode rows) of the smallest engine replica attached; a mock replica sets none."""
+        engs = [b.engine for b in self.backends.values() if isinstance(b, EngineBackend)]
+        big = 2**31 - 1
+        return (min((e.ctx_max for e in engs), default=big), min((e.max_prefill_tokens for e in engs), default=big),
+                min((e.max_batch for e in engs), default=big))
+
+    def _invalid(self, n_prompt: int = 0, max_new: int = 0, n: int = 1) -> BadRequestError:
+        """The HTTP 400 of a request the gateway refused with RR_INVALID_ARGUMENT, naming the limit it broke."""
+        ctx, pf, rows = self._limits()
+        if n > rows:
+            return BadRequestError(f"`n` = {n} exceeds the {rows} decode rows of the smallest replica")
+        if n_prompt + max_new > ctx:
+            return BadRequestError(f"prompt ({n_prompt} tokens) + max_tokens ({max_new}) exceed the context window "
+                                   f"({ctx} tokens) of the deployment")
+        if n_prompt > pf:
+            return BadRequestError(f"the prompt ({n_prompt} tokens) exceeds the prefill chunk ({pf} tokens) of the "
+                                   "deployment")
+        return BadRequestError("a token id is outside the vocabulary of the deployment, or a generation parameter is out "
+                               "of range")
 
     def _gw_error(self, status: int, model: str, res=None, timeout=None) -> APIError:
         if status == 1:
@@ -433,8 +471,7 @@ class Router:
         if status == 2:
             return BadRequestError(f"Invalid model name passed in model={model}")
         if status == 4:
-            return BadRequestError("prompt + max_tokens exceed the context window of the deployment, or a token id is "
-                                   "outside its vocabulary")
+            return self._invalid() if res is None else self._invalid(res.n_prompt, 0)
         if status == 6:
             return APITimeoutError(f"Request timed out after {timeout}s")
         if status == 7:
@@ -442,44 +479,54 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs, n: int = 1) -> int:
+        """n > 1: rr_gateway_submit_choices; a request of one choice takes rr_gateway_submit_processed, as before."""
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        rc = _lib.lib.rr_gateway_submit_processed(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
-                                                  *gen.tail, C.byref(t))
+        p = ids.ctypes.data_as(C.POINTER(C.c_int32))
+        if n > 1:
+            rc = _lib.lib.rr_gateway_submit_choices(gw, g, p, len(ids), max_new, n, *gen.tail, C.byref(t))
+        else:
+            rc = _lib.lib.rr_gateway_submit_processed(gw, g, p, len(ids), max_new, *gen.tail, C.byref(t))
+        if rc == 4:
+            raise self._invalid(len(ids), max_new, n)
         if rc != 0:
             raise self._gw_error(rc, model)
         return t.value
 
     @staticmethod
-    def _lp_bufs(gen: GenArgs, max_new: int):
-        """[max_new][gen.width] pair buffers of a logprobs request."""
+    def _lp_bufs(gen: GenArgs, max_new: int, n: int = 1):
+        """[max_new][gen.width] pair buffers of a logprobs request ([n][max_new][gen.width] for n choices)."""
         if gen.top is None:
             return None, None, None, None
-        lp = np.zeros((max_new, gen.width), dtype=np.float32)
-        ids = np.zeros((max_new, gen.width), dtype=np.int32)
+        shape = (max_new, gen.width) if n == 1 else (n, max_new, gen.width)
+        lp = np.zeros(shape, dtype=np.float32)
+        ids = np.zeros(shape, dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs, n: int = 1):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen, n)
         res = _lib.GatewayResult()
-        toks = np.zeros(max_new, dtype=np.int32)
-        lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new)
-        rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, float(timeout or 0.0), C.byref(res),
-                                               toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
-        if rc == 6:                      # client-side timeout: give the row back, count a failure against the deployment
+        toks = np.zeros(max_new if n == 1 else (n, max_new), dtype=np.int32)
+        lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new, n)
+        wait = _lib.lib.rr_gateway_wait_choices if n > 1 else _lib.lib.rr_gateway_wait_logprobs
+        rc = wait(gw, ticket, float(timeout or 0.0), C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
+                  lp_p, ids_p)
+        if rc == 6:                      # client-side timeout: give the rows back, count a failure against the deployment
             _lib.lib.rr_gateway_cancel(gw, ticket, 1)
             raise self._gw_error(6, model, res, timeout)
         if rc != 0:
             raise self._gw_error(rc, model, res, timeout)
         content = None
         if gen.top is not None:
-            n = min(res.n_generated, max_new)
-            content = {"content": logprobs_content(toks[:n].tolist(), logprob_pairs(lp, ids, 0, n), gen.top),
-                       "refusal": None}
+            k = min(res.n_generated, max_new)
+            content = [{"content": logprobs_content(t[:k].tolist(), logprob_pairs(a, b, 0, k), gen.top), "refusal": None}
+                       for t, a, b in zip(np.atleast_2d(toks), lp.reshape(-1, max_new, gen.width),
+                                          ids.reshape(-1, max_new, gen.width))]
+            content = content[0] if n == 1 else content
         return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
 
     def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
@@ -539,6 +586,8 @@ class Router:
         rc = _lib.lib.rr_gateway_submit_batch(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)),
                                               start.ctypes.data_as(C.POINTER(C.c_int32)), n, max_new,
                                               1 if self.cfg.routing_strategy == "split" else 0, tk)
+        if rc == 4:
+            raise self._invalid(max(len(p) for p in prompts), max_new)
         if rc != 0:
             raise self._gw_error(rc, model)
         out: List[Any] = [None] * n
@@ -619,13 +668,18 @@ class Router:
                    logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                    top_p: Optional[float] = None, seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
                    presence_penalty: Optional[float] = None, logit_bias: Optional[Dict[str, float]] = None,
-                   **_ignored) -> ModelResponse:
+                   n: Optional[int] = None, **_ignored) -> ModelResponse:
         """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
         (0..20) most likely alternatives, as the OpenAI API returns them.  temperature > 0: every token is drawn from
         the top_p nucleus of softmax(logits / temperature) with the request's seed (rr_op_sample); absent or 0 is
         greedy.  frequency_penalty / presence_penalty / logit_bias: applied to the logits before every token is picked
         (rr_op_logit_penalties; the penalties count the tokens generated so far).  Stub backends validate these and keep
-        their fixed reply."""
+        their fixed reply.
+        n (1..128, at most the decode rows of the smallest engine replica): n choices of the same prompt, prefilled once
+        (rr_gateway_submit_choices).  Choice i of a sampled request is drawn with seed + i (mod 2^64), so it equals the
+        n=1 response with that seed; greedy choices are all the greedy response.  usage.completion_tokens sums the
+        choices and `_choice_token_ids` holds each choice's tokens (`_token_ids`: choice 0's)."""
+        n = check_n(n)
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
                            logit_bias)
         g = self.cfg.group_index(model)
@@ -634,19 +688,23 @@ class Router:
         if prompt_ids is None:
             prompt_ids = tokenize(messages_to_text(messages or []), self._vocab())
         max_new = max_tokens or self.default_max_tokens
-        return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen)
+        if n > self._limits()[2]:
+            raise self._invalid(n=n)
+        return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen, n)
 
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                           max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
                           logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                           top_p: Optional[float] = None, seed: Optional[int] = None,
                           frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-                          logit_bias: Optional[Dict[str, float]] = None):
+                          logit_bias: Optional[Dict[str, float]] = None, n: Optional[int] = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
         (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
         fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties and logit
-        bias as in completion()."""
+        bias as in completion().  n > 1 is not streamed: BadRequestError."""
+        if check_n(n) > 1:
+            raise BadRequestError("streaming is not available with `n` > 1: send the request without `stream`")
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
                            logit_bias)
         g = self.cfg.group_index(model)

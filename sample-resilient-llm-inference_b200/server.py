@@ -16,7 +16,7 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend, check_logprobs, check_penalties, check_sampling)
+                     StubBackend, check_logprobs, check_n, check_penalties, check_sampling)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -97,6 +97,10 @@ def create_app(router: Router):
             samp_kw.update({k: body[k] for k in ("frequency_penalty", "presence_penalty", "logit_bias")
                             if body.get(k) is not None})
             check_penalties(**{k: v for k, v in samp_kw.items() if k not in ("temperature", "top_p", "seed")})
+            if "n" in body:
+                samp_kw["n"] = body["n"]
+                if check_n(body["n"]) > 1 and body.get("stream"):
+                    raise BadRequestError("streaming is not available with `n` > 1: send the request without `stream`")
         except BadRequestError as e:
             return JSONResponse(_error_body(e, "invalid_request_error"), 400)
         if body.get("stream"):
