@@ -247,6 +247,23 @@ int rr_op_sample(const float* logits, int ld, int rows, int vocab, const float* 
 int rr_op_logit_penalties(float* logits, int ld, int rows, int vocab, const int32_t* hist, int hist_ld,
                           const int32_t* hist_len, const float* frequency_penalty, const float* presence_penalty,
                           const int32_t* bias_ids, const float* bias_vals, int bias_ld, const int32_t* n_bias, void* stream);
+/* Stop sequences, as the engine matches them after a token is picked.  All arrays are device memory.  Row r has n_stop[r]
+ * (0..4) sequences, sequence s the stop_len[r * 4 + s] (1..64) bytes at stop_bytes + (r * 4 + s) * 64 (stop_bytes 4-byte
+ * aligned).  The reply text of a row is its history tokens mapped like the byte tokenizer maps them back: a token t >= 3 is
+ * the byte (t - 3) % 256, a token < 3 is no text.  For every row with n_stop[r] > 0 and (row_active NULL or
+ * row_active[r] >= 0) the kernel stores tok[r] at hist[r * hist_ld + i], i = position[r] - gen0[r], and over the text of
+ * hist[r][0 .. i] writes
+ *   cut_out[r]  = -1, or when tok[r] has a byte and the text ends in a sequence: the index in the history of the first
+ *                 token of the longest such sequence, which is the number of tokens that come before the match;
+ *   hold_out[r] = 0 on a hit, else the number of newest tokens from the first token of the longest suffix of the text that
+ *                 is a proper prefix of a sequence (0 when there is none): what a streaming reader must not be shown yet.
+ * Other rows are not touched; i outside [0, hist_ld) gives (-1, 0) and no store.  No other history cell is written.  Work
+ * per row is O(64 x 4) plus the length of any run of byteless tokens; integer only, so two calls agree bit for bit.
+ * RR_INVALID_ARGUMENT before touching the device for a null pointer other than row_active, rows outside 1..65535,
+ * hist_ld < 1 or a misaligned stop_bytes. */
+int rr_op_stop_match(int32_t* hist, int hist_ld, const int32_t* tok, const int32_t* position, const int32_t* row_active,
+                     const int32_t* n_stop, const int32_t* gen0, const uint8_t* stop_len, const uint8_t* stop_bytes,
+                     int32_t* cut_out, int32_t* hold_out, int rows, void* stream);
 int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                       const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                       int n_kv_heads, int ctx_max /* % 64 == 0 */, int n_slots, float scale,
@@ -460,8 +477,8 @@ int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_pr
  * in a row of its own.  Choice i is exactly what rr_engine_submit_processed gives with seed (seed + i) mod 2^64 and the same
  * other parameters (greedy: every choice is the greedy completion); penalties count the choice's own tokens.  The choices
  * run in lockstep: they are admitted together (a request waits at the head of the queue until n_choices rows are free;
- * nothing overtakes it), get one token each per step and end together, so rr_completion.n_generated counts the tokens of
- * each choice.  Cancellation, an injected failure or an internal error ends every choice.  n_choices = 1 is
+ * nothing overtakes it), get one token each per step and, without stop sequences (rr_engine_submit_stop), end together,
+ * so rr_completion.n_generated counts the tokens of each choice.  Cancellation, an injected failure or an internal error ends every choice.  n_choices = 1 is
  * rr_engine_submit_processed.  RR_INVALID_ARGUMENT, before anything is queued, for n_choices outside 1..max_batch and
  * whatever rr_engine_submit_processed rejects.
  * wait_choices: rr_engine_wait_logprobs for any n_choices, with tokens_out [n_choices][max_tokens_out] and lp_out / id_out
@@ -475,6 +492,30 @@ int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prom
                              uint64_t* ticket);
 int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
                            int max_tokens_out, float* lp_out, int32_t* id_out);
+/* Stop sequences (OpenAI `stop`): rr_engine_submit_choices with n_stop (0..4) sequences of 1..64 bytes each, sequence i =
+ * stop_bytes[stop_off[i] .. stop_off[i + 1]).  They are matched on the reply text (a generated token t >= 3 is the byte
+ * (t - 3) % 256, a token < 3 is no text) by rr_op_stop_match after every generated token, the first included.  A choice
+ * whose text comes to end in a sequence finishes with reason 1 (stop): it returns the tokens before the first token of the
+ * match (of the longest sequence when several end there), its logprob pairs likewise, and its decode row is free from the
+ * next step on, while the request's other choices go on.  A choice that reaches max_new_tokens finishes with reason 0
+ * (length).  The request is done when every choice has finished.  Stop sequences change no logit and no draw: the tokens
+ * returned are a prefix of those of the same request without them.  n_stop = 0 is rr_engine_submit_choices.
+ * RR_INVALID_ARGUMENT, before anything is queued, for n_stop outside 0..4, a length outside 1..64, null arrays with
+ * n_stop > 0, and whatever rr_engine_submit_choices rejects.
+ * wait_stop: rr_engine_wait_choices, and n_tokens_out[c] = the tokens choice c returned, finish_out[c] = its reason (either
+ * may be NULL).  Row c of tokens_out / lp_out / id_out holds min(n_tokens_out[c], max_tokens_out) entries.
+ * rr_completion.n_generated is the longest choice's count; the other wait calls report the same.  While a request runs,
+ * rr_engine_peek[_logprobs] shows a token only once no stop sequence can take it back (hold_out of rr_op_stop_match), so
+ * n_generated there never shrinks; a request that ends by length releases the held tokens with its last ones.  After a
+ * cancel, an injected failure or an internal error the tokens shown so far are what is kept.
+ * Stats: generated_tokens counts every token produced, the cut ones included. */
+int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
+                          int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                          float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
+                          const uint8_t* stop_bytes, const int32_t* stop_off, uint64_t* ticket);
+int rr_engine_wait_stop(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                        int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out /* [n_choices] */,
+                        int32_t* finish_out /* [n_choices] */);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -523,7 +564,7 @@ typedef struct rr_gateway_result {
     int32_t attempts;          /* admissions this request went through (1 + backends that failed under it) */
     double t_submit_s, t_admit_s, t_first_token_s, t_done_s;   /* gateway monotonic clock, seconds */
     int32_t n_cached;          /* rr_completion.n_cached of the engine that served the request */
-    int32_t reserved;
+    int32_t reserved;          /* choice 0's finish reason once finished: 0 length, 1 stop (rr_engine_submit_stop) */
 } rr_gateway_result;
 
 typedef struct rr_gateway_stats {
@@ -602,6 +643,19 @@ int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_id
                               const float* bias_vals, uint64_t* ticket);
 int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
                             int max_tokens_out, float* lp_out, int32_t* id_out);
+/* Stop sequences (rr_engine_submit_stop): stored with the request and handed to every engine it is admitted to, a fallback
+ * re-admission included (the bytes need no vocabulary check).  A gateway with a mock replica refuses n_stop > 0 at submit
+ * with RR_INVALID_ARGUMENT: a mock replica has no decode loop to cut.  The request is one ADMIT event and one DONE event
+ * carrying the tokens its choices return.  wait_stop: rr_gateway_wait_choices plus each choice's token count and finish
+ * reason, as rr_engine_wait_stop; rr_gateway_result.n_generated is the longest choice's count.  The other wait and peek
+ * calls keep working for such a request of one choice (rr_gateway_result.reserved = its finish reason). */
+int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                           int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                           float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                           const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
+                           uint64_t* ticket);
+int rr_gateway_wait_stop(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                         int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

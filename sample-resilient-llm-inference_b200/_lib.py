@@ -29,6 +29,7 @@ lib = _load()
 
 c_i32p = C.POINTER(C.c_int32)
 c_f32p = C.POINTER(C.c_float)
+c_u8p = C.POINTER(C.c_uint8)
 vp = C.c_void_p
 
 # ---------------------------------------------------------------- structs (mirror rr_b200.h)
@@ -159,6 +160,7 @@ PROTOTYPES = {
     "rr_op_logprobs": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp]),
     "rr_op_sample": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "rr_op_logit_penalties": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, vp]),
+    "rr_op_stop_match": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]),
     "rr_op_decode_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -198,6 +200,11 @@ PROTOTYPES = {
                                            C.POINTER(C.c_uint64)]),
     "rr_engine_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p,
                                          c_i32p]),
+    "rr_engine_submit_stop": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                        C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
+                                        C.POINTER(C.c_uint64)]),
+    "rr_engine_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p,
+                                      c_i32p, c_i32p]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
                                       C.POINTER(Completion), c_i32p]),
     "rr_engine_now": (C.c_double, [vp]),
@@ -228,6 +235,11 @@ PROTOTYPES = {
                                             C.POINTER(C.c_uint64)]),
     "rr_gateway_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
                                           c_i32p]),
+    "rr_gateway_submit_stop": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                         C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
+                                         C.POINTER(C.c_uint64)]),
+    "rr_gateway_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
+                                       c_i32p, c_i32p, c_i32p]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),
     "rr_gateway_quiesce": (C.c_int, [vp, C.c_double]),
     "rr_gateway_get_stats": (C.c_int, [vp, C.POINTER(GatewayStats)]),

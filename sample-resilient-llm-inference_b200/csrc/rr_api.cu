@@ -252,6 +252,20 @@ RR_API int rr_op_logit_penalties(float* logits, int ld, int rows, int vocab, con
     return check_last();
 }
 
+// Stop-sequence matching as the engine runs it at the end of the logits tail (StopArgs, rr_kernels.h), on caller buffers.
+RR_API int rr_op_stop_match(int32_t* hist, int hist_ld, const int32_t* tok, const int32_t* position,
+                            const int32_t* row_active, const int32_t* n_stop, const int32_t* gen0, const uint8_t* stop_len,
+                            const uint8_t* stop_bytes, int32_t* cut_out, int32_t* hold_out, int rows, void* stream) {
+    if (!hist || !tok || !position || !n_stop || !gen0 || !stop_len || !stop_bytes || !cut_out || !hold_out)
+        return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > 65535 || hist_ld < 1 || ((uintptr_t)stop_bytes & 3)) return RR_INVALID_ARGUMENT;
+    StopArgs a;
+    a.n_stop = n_stop; a.gen0 = gen0; a.len = stop_len; a.bytes = stop_bytes; a.hist = hist; a.hist_ld = hist_ld;
+    a.hist_row = nullptr; a.tok = tok; a.position = position; a.row_active = row_active; a.cut = cut_out; a.hold = hold_out;
+    launch_stop_match(a, rows, (cudaStream_t)stream);
+    return check_last();
+}
+
 RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_cache, void* out,
                              const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                              int n_kv_heads, int ctx_max, int n_slots, float scale, int kv_splits, void* stream) {

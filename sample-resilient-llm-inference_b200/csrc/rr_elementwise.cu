@@ -916,6 +916,77 @@ void launch_logit_penalties(float* logits, int ld, int rows, int vocab, const Pe
     launch_pdl(logit_penalties_kernel, dim3(rows), dim3(PEN_THREADS), 0, st, logits, ld, vocab, a, cnt_ws);
 }
 
+// ---- stop sequences (rr_op_stop_match) ---------------------------------------------------------------------------------
+// One warp per row.  The warp stores the new token in the history, then walks the history back in 32-token steps and
+// compacts (ballot + popc) the last <= STOP_MAX_LEN text bytes and the history index of each into shared memory, newest
+// first; byteless tokens (< 3) are skipped, so the walk is O(STOP_MAX_LEN) except through runs of them.  Lane k then tests,
+// for every sequence, "the last k + 1 (and k + 33) text bytes are the first k + 1 (k + 33) bytes of the sequence": the
+// full-length test is a hit, shorter ones are partial matches; warp maxima pick the longest of each.  Integer work only,
+// no atomics: the outputs are a function of the inputs.
+constexpr int STOP_WARPS = 4;
+
+__global__ void __launch_bounds__(32 * STOP_WARPS) stop_match_kernel(StopArgs a, int rows) {
+    griddep_launch();
+    griddep_wait();
+    __shared__ uint8_t s_txt[STOP_WARPS][STOP_MAX_LEN];
+    __shared__ int32_t s_idx[STOP_WARPS][STOP_MAX_LEN];
+    __shared__ uint32_t s_stop[STOP_WARPS][STOP_MAX_SEQS * STOP_MAX_LEN / 4];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int row = blockIdx.x * STOP_WARPS + warp;
+    if (row >= rows) return;
+    const int ns = min(a.n_stop[row], STOP_MAX_SEQS);
+    if (ns <= 0 || (a.row_active && a.row_active[row] < 0)) return;
+    const int i = a.position ? a.position[row] - a.gen0[row] : 0;
+    if (i < 0 || i >= a.hist_ld) {
+        if (lane == 0) { a.cut[row] = -1; a.hold[row] = 0; }
+        return;
+    }
+    int32_t* h = a.hist + (size_t)(a.hist_row ? a.hist_row[row] : row) * a.hist_ld;
+    const int newest = a.tok[row];
+    if (lane == 0) h[i] = newest;
+    const uint32_t* sb = reinterpret_cast<const uint32_t*>(a.bytes + (size_t)row * STOP_MAX_SEQS * STOP_MAX_LEN);
+    s_stop[warp][lane] = sb[lane];
+    s_stop[warp][lane + 32] = sb[lane + 32];
+    __syncwarp();
+    uint8_t* txt = s_txt[warp];
+    int32_t* idx = s_idx[warp];
+    int nb = 0;                                    // text bytes staged so far: txt[k] = the k-th newest, idx[k] its token
+    for (int base = i; base >= 0 && nb < STOP_MAX_LEN; base -= 32) {
+        const int j = base - lane;
+        const int t = j >= 0 ? h[j] : 0;
+        const unsigned m = __ballot_sync(0xffffffffu, t >= 3);
+        const int k = nb + __popc(m & ((1u << lane) - 1u));
+        if (t >= 3 && k < STOP_MAX_LEN) { txt[k] = (uint8_t)((t - 3) & 255); idx[k] = j; }
+        nb += __popc(m);
+    }
+    nb = min(nb, STOP_MAX_LEN);
+    __syncwarp();
+    const uint8_t* stop = reinterpret_cast<const uint8_t*>(s_stop[warp]);
+    int hit = 0, part = 0;                         // longest full / proper-prefix match this lane found, in bytes
+    for (int s = 0; s < ns; ++s) {
+        const int L = a.len[row * STOP_MAX_SEQS + s];
+        if (L < 1 || L > STOP_MAX_LEN) continue;
+        const uint8_t* q = stop + s * STOP_MAX_LEN;
+        for (int kl = lane + 1; kl <= min(L, nb); kl += 32) {
+            int j = 0;
+            while (j < kl && q[j] == txt[kl - 1 - j]) ++j;
+            if (j < kl) continue;
+            if (kl == L) hit = max(hit, kl);
+            else part = max(part, kl);
+        }
+    }
+    hit = __reduce_max_sync(0xffffffffu, hit);
+    part = __reduce_max_sync(0xffffffffu, part);
+    if (lane != 0) return;
+    if (hit > 0 && newest >= 3) { a.cut[row] = idx[hit - 1]; a.hold[row] = 0; }
+    else { a.cut[row] = -1; a.hold[row] = part > 0 ? i + 1 - idx[part - 1] : 0; }
+}
+
+void launch_stop_match(const StopArgs& a, int rows, cudaStream_t st) {
+    if (rows <= 0) return;
+    launch_pdl(stop_match_kernel, dim3((rows + STOP_WARPS - 1) / STOP_WARPS), dim3(32 * STOP_WARPS), 0, st, a, rows);
+}
+
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }
 
 }  // namespace rr

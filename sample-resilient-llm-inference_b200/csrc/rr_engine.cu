@@ -66,8 +66,9 @@ __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const
 }
 
 // One request of n_choices choices.  Choice c decodes in row rows[c] (== its KV slot); the prompt is prefilled once, into
-// rows[0], and its KV copied to the other rows.  All choices run in lockstep: admitted in one chunk, one token each per
-// step, released together.
+// rows[0], and its KV copied to the other rows.  The choices are admitted in one chunk and get one token each per step.  A
+// choice finishes when it holds max_new tokens or a stop sequence cuts it, and gives its row back at once; the request
+// finishes with its last choice.  Without stop sequences that is one step for all of them.
 struct Request {
     uint64_t ticket;
     std::vector<int32_t> prompt;
@@ -77,7 +78,9 @@ struct Request {
     int status = RR_OK;
     bool done = false;
     double t_submit = 0, t_first = 0, t_done = 0;
-    std::vector<int> rows;     // [n_choices] while admitted, else empty
+    std::vector<int> rows;     // [n_choices] while admitted (-1: the choice finished and freed its row), else empty
+    std::vector<int> finish;   // [n_choices] -1 running, else why the choice finished: 0 length, 1 stop
+    std::vector<int> hold;     // [n_choices] newest tokens of a running choice that a stop sequence may still take back
     uint64_t tag = 0;          // opaque caller value handed to the done hook (the gateway's request id)
     bool cancel = false;       // rr_engine_cancel: the worker drops the rows at the next step
     bool detached = false;     // nobody will call rr_engine_wait: the worker frees the request when it finishes
@@ -86,7 +89,19 @@ struct Request {
     std::vector<std::vector<int32_t>> lp_id;
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
 
-    int n_generated() const { return (int)out[0].size(); }      // tokens per choice
+    // Tokens of choice c a reader may see: all of a finished choice, else those no stop sequence can take back.
+    int visible(int c) const { return (int)out[c].size() - (finish[c] < 0 ? hold[c] : 0); }
+    int n_generated() const {          // the longest choice's visible tokens
+        int n = 0;
+        for (int c = 0; c < n_choices; ++c) n = std::max(n, visible(c));
+        return n;
+    }
+    int n_returned() const {           // over all choices
+        int n = 0;
+        for (int c = 0; c < n_choices; ++c) n += visible(c);
+        return n;
+    }
+    bool all_finished() const { return std::find(finish.begin(), finish.end(), -1) == finish.end(); }
 };
 
 // Prefix caching: the shortest shared prefix that counts as a hit -- one key tile of prefill attention.  Trivial shared
@@ -98,15 +113,20 @@ constexpr int PREFIX_MIN = 64;
 //   1 samp   seed u64[n] | temperature f32[n] (0: greedy) | top_p f32[n], with a position column also | position i32[n]
 //   2 pen    frequency_penalty f32[n] | presence_penalty f32[n] | gen0 i32[n] (the position of the first generated token)
 //            | n_bias i32[n] | bias ids i32[n][bias_ld] | bias values f32[n][bias_ld]
+//   3 stop   n_stop i32[n] | gen0 i32[n] | len u8[n][STOP_MAX_SEQS] | bytes u8[n][STOP_MAX_SEQS][STOP_MAX_LEN]
 // The decode rows use n = Bm and bias_ld = PEN_MAX_BIAS (fixed: the graphs hold it).  A prefill chunk uses n = n_seqs, the
 // largest bias count among its sequences and a position column, in buffers sized for Bm rows and PEN_MAX_BIAS.
 struct ParamBlocks {
-    char* blk[3] = {};            // pen stays null until the first processed request (ensure_pen_buffers)
+    char* blk[4] = {};            // pen / stop stay null until the first request that uses them (ensure_pen_buffers /
+                                  // ensure_stop_buffers)
     int n = 0, bias_ld = 0;
     bool has_pos = false;
 
     ParamBlocks at(int rows, int ld) const { ParamBlocks p = *this; p.n = rows; p.bias_ld = ld; return p; }
-    size_t bytes(int i) const { return (size_t)n * (i == 0 ? 4 : i == 1 ? (has_pos ? 20 : 16) : 16 + 8 * (size_t)bias_ld); }
+    static constexpr size_t STOP_ROW = 12 + STOP_MAX_SEQS * STOP_MAX_LEN;      // 268 B per row
+    size_t bytes(int i) const {
+        return (size_t)n * (i == 0 ? 4 : i == 1 ? (has_pos ? 20 : 16) : i == 2 ? 16 + 8 * (size_t)bias_ld : STOP_ROW);
+    }
     int32_t* top_n() const { return (int32_t*)blk[0]; }
     uint64_t* seed() const { return (uint64_t*)blk[1]; }
     float* temp() const { return (float*)(blk[1] + 8 * (size_t)n); }
@@ -118,6 +138,10 @@ struct ParamBlocks {
     int32_t* n_bias() const { return (int32_t*)(blk[2] + 12 * (size_t)n); }
     int32_t* bias_ids() const { return (int32_t*)(blk[2] + 16 * (size_t)n); }
     float* bias_vals() const { return (float*)(bias_ids() + (size_t)n * bias_ld); }
+    int32_t* n_stop() const { return (int32_t*)blk[3]; }
+    int32_t* stop_gen0() const { return (int32_t*)(blk[3] + 4 * (size_t)n); }
+    uint8_t* stop_len() const { return (uint8_t*)(blk[3] + 8 * (size_t)n); }
+    uint8_t* stop_bytes() const { return (uint8_t*)(blk[3] + 12 * (size_t)n); }
 
     PenaltyArgs pen_args() const {
         PenaltyArgs a;
@@ -126,20 +150,32 @@ struct ParamBlocks {
         a.hist = nullptr; a.hist_ld = 0; a.hist_len = nullptr; a.app_tok = nullptr; a.app_pos = nullptr;
         return a;
     }
+    StopArgs stop_args() const {
+        StopArgs a = {};
+        a.n_stop = n_stop(); a.gen0 = stop_gen0(); a.len = stop_len(); a.bytes = stop_bytes();
+        return a;
+    }
     // The step_mode bits of the blocks whose row i differs from the defaults.
     int row_mode(int i) const {
         return (top_n()[i] >= 0 ? 1 : 0) | (temp()[i] > 0.f ? 2 : 0) |
-               (blk[2] && (freq()[i] != 0.f || pres()[i] != 0.f || n_bias()[i] != 0) ? 4 : 0);
+               (blk[2] && (freq()[i] != 0.f || pres()[i] != 0.f || n_bias()[i] != 0) ? 4 : 0) |
+               (blk[3] && n_stop()[i] != 0 ? 8 : 0);
     }
     // Row i from p for its choice `choice`: drawn at `position` (with a position column) with seed p.seed + choice, p's
-    // bias, and penalties f / pr from position g0 on.
+    // bias, penalties f / pr and p's stop sequences; g0 = the position of the row's first generated token (penalty history
+    // and stop matching start there).
     void put_row(int i, const GenParams& p, int choice, int position, float f, float pr, int g0) const {
         top_n()[i] = p.top_lp;
         seed()[i] = p.sampled() ? p.seed + (uint64_t)choice : p.seed; temp()[i] = p.temp; top_p()[i] = p.top_p;
         if (has_pos) pos()[i] = position;
+        if (blk[3]) {
+            n_stop()[i] = p.n_stop; stop_gen0()[i] = p.stops() ? g0 : 0;
+            memcpy(stop_len() + (size_t)i * STOP_MAX_SEQS, p.stop_len, STOP_MAX_SEQS);
+            if (p.stops()) memcpy(stop_bytes() + (size_t)i * STOP_MAX_SEQS * STOP_MAX_LEN, p.stop, sizeof(p.stop));
+        }
         if (!blk[2]) return;
         const int nb = (int)p.bias_id.size();
-        freq()[i] = f; pres()[i] = pr; gen0()[i] = g0; n_bias()[i] = nb;
+        freq()[i] = f; pres()[i] = pr; gen0()[i] = p.processed() ? g0 : 0; n_bias()[i] = nb;
         if (nb) {
             memcpy(bias_ids() + (size_t)i * bias_ld, p.bias_id.data(), 4 * (size_t)nb);
             memcpy(bias_vals() + (size_t)i * bias_ld, p.bias_val.data(), 4 * (size_t)nb);
@@ -147,7 +183,7 @@ struct ParamBlocks {
     }
     // Copies the blocks whose bit is in `mask` from these (pinned) blocks to d, of the same n and bias_ld.
     cudaError_t upload(const ParamBlocks& d, int mask, cudaStream_t s, uint64_t* h2d_bytes) const {
-        for (int i = 0; i < 3; ++i) {
+        for (int i = 0; i < 4; ++i) {
             if (!(mask >> i & 1)) continue;
             const cudaError_t err = cudaMemcpyAsync(d.blk[i], blk[i], bytes(i), cudaMemcpyHostToDevice, s);
             if (err != cudaSuccess) return err;
@@ -158,7 +194,8 @@ struct ParamBlocks {
 };
 
 int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_, uint64_t seed_, float frequency_penalty,
-                   float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals) {
+                   float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop_,
+                   const uint8_t* stop_bytes, const int32_t* stop_off) {
     if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     if (!(temperature >= 0.f && temperature <= 2.f && top_p_ >= 0.f && top_p_ <= 1.f)) return RR_INVALID_ARGUMENT;
     if (!(frequency_penalty >= -2.f && frequency_penalty <= 2.f && presence_penalty >= -2.f && presence_penalty <= 2.f))
@@ -170,12 +207,21 @@ int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_,
     std::vector<int32_t> ids(bias_ids, bias_ids + n_bias);
     std::sort(ids.begin(), ids.end());
     if (std::adjacent_find(ids.begin(), ids.end()) != ids.end()) return RR_INVALID_ARGUMENT;
+    if (n_stop_ < 0 || n_stop_ > STOP_MAX_SEQS || (n_stop_ > 0 && (!stop_bytes || !stop_off))) return RR_INVALID_ARGUMENT;
+    for (int i = 0; i < n_stop_; ++i)
+        if (stop_off[i] < 0 || stop_off[i + 1] - stop_off[i] < 1 || stop_off[i + 1] - stop_off[i] > STOP_MAX_LEN)
+            return RR_INVALID_ARGUMENT;
     *this = GenParams();
     top_lp = top_logprobs;
     if (temperature > 0.f) { temp = temperature; top_p = top_p_; seed = seed_; }
     if (frequency_penalty != 0.f || presence_penalty != 0.f || n_bias > 0) {
         fpen = frequency_penalty; ppen = presence_penalty;
         bias_id.assign(bias_ids, bias_ids + n_bias); bias_val.assign(bias_vals, bias_vals + n_bias);
+    }
+    n_stop = n_stop_;
+    for (int i = 0; i < n_stop_; ++i) {
+        stop_len[i] = (uint8_t)(stop_off[i + 1] - stop_off[i]);
+        memcpy(stop[i], stop_bytes + stop_off[i], stop_len[i]);
     }
     return RR_OK;
 }
@@ -228,10 +274,10 @@ struct rr_engine {
     MlpItem* mlp_items = nullptr;     // device copy of the schedule (shared by all layers)
     unsigned* mlp_ready = nullptr;    // [n_slices] dependency counters, reset by the norm kernel before each launch
     int mlp_slices = 0, mlp_slice_kb = 0;
-    // decode step graphs by step_mode(): bit 0 + launch_logprobs, bit 1 + launch_sample, bit 2 + launch_logit_penalties.
-    // [0] (plain) is captured after the warm-up step, the others on first use: a step without logprobs, sampled or
-    // processed rows replays the plain graph.
-    cudaGraphExec_t graph[8] = {};
+    // decode step graphs by step_mode(): bit 0 + launch_logprobs, bit 1 + launch_sample, bit 2 + launch_logit_penalties,
+    // bit 3 + launch_stop_match.  [0] (plain) is captured after the warm-up step, the others on first use: a step without
+    // logprobs, sampled, processed or stop rows replays the plain graph.
+    cudaGraphExec_t graph[16] = {};
     bool warmed = false;
     // The decode rows' parameter blocks (d_rows) and their pinned host mirror (h_rows), which set_row_params keeps in step
     // with row_req, marking the blocks it changes in rows_dirty (step_mode bits); upload_row_params copies a dirty block
@@ -244,9 +290,10 @@ struct rr_engine {
     int32_t* d_lp_id = nullptr;
     void* sample_ws = nullptr;
     float* d_tok_lp = nullptr;                         // [Bm] the sampled token's logprob (sampled logprobs rows)
-    // penalties, allocated with the pen blocks on the first processed request (ensure_pen_buffers): the generated-token
-    // history [Bm][ctx_max] and the count workspace [Bm][vocab] (all zero between launches)
-    int32_t *d_hist = nullptr, *pen_ws = nullptr;
+    // the generated-token history [Bm][ctx_max], shared by the penalty and the stop kernels and allocated with the first
+    // of their buffers (ensure_hist); penalties (ensure_pen_buffers): the count workspace [Bm][vocab] (all zero between
+    // launches); stop sequences (ensure_stop_buffers): cut[Bm] | hold[Bm] of rr_op_stop_match and their pinned copy
+    int32_t *d_hist = nullptr, *pen_ws = nullptr, *d_stop = nullptr, *h_stop = nullptr;
 
     // prefill working set
     int Tmax;
@@ -285,7 +332,7 @@ struct rr_engine {
     std::chrono::steady_clock::time_point t0;
 
     rr_engine_stats st;                  // written under gpu_mu (launch / timing counters) or mu (queued, active_rows)
-    uint64_t step_launches[8] = {};              // launches of one decode step, by step_mode()
+    uint64_t step_launches[16] = {};              // launches of one decode step, by step_mode()
     // completion hook (the native gateway, rr_gateway.cu): called on the worker / submitting thread, outside `mu`
     rr::EngineDoneHook hook = nullptr;
     void* hook_ctx = nullptr;
@@ -339,36 +386,55 @@ static PartIn part_bf16(const __nv_bfloat16* p, int ld) {
 static PartIn part_none() { PartIn r; r.ptr = nullptr; r.is_bf16 = 0; r.n_splits = 1; r.split_stride = 0; r.ld = 0; return r; }
 
 // ---------------------------------------------------------------- decode step (enqueue only)
-// The step_mode bits a request needs: 1 logprobs, 2 sampling, 4 penalties / logit bias.  Over a step's rows or a chunk's
-// sequences they pick the parameter blocks to upload, the kernels of the logits tail and the decode graph.
+// The step_mode bits a request needs: 1 logprobs, 2 sampling, 4 penalties / logit bias, 8 stop sequences.  Over a step's
+// rows or a chunk's sequences they pick the parameter blocks to upload, the kernels of the logits tail and the decode graph.
 static int step_mode(const GenParams& p) {
-    return (p.logprobs() ? 1 : 0) | (p.sampled() ? 2 : 0) | (p.processed() ? 4 : 0);
+    return (p.logprobs() ? 1 : 0) | (p.sampled() ? 2 : 0) | (p.processed() ? 4 : 0) | (p.stops() ? 8 : 0);
+}
+
+// Caller holds gpu_mu.  The generated-token history, which the decode graphs of modes 4 and 8 hold: allocated once.
+static int ensure_hist(rr_engine* e) {
+    return e->d_hist ? RR_OK : dalloc(e, &e->d_hist, (size_t)e->Bm * e->o.ctx_max, false);
+}
+
+// Caller holds gpu_mu.  Decode rows' and prefill blocks of parameter block i (2 or 3), device and pinned, all zero: the
+// defaults of a row that does not use the block.
+static int ensure_block(rr_engine* e, int i) {
+    const size_t blk = e->d_rows.bytes(i);            // also the prefill blocks' size: Bm rows (of PEN_MAX_BIAS)
+    char *dp = nullptr, *dpf = nullptr, *hp = nullptr, *hpf = nullptr;
+    int rc = dalloc(e, &dp, blk, false);
+    if (rc == RR_OK) rc = dalloc(e, &dpf, blk, false);
+    if (rc != RR_OK) return rc;
+    CK(cudaMemsetAsync(dp, 0, blk, e->stream));       // on the engine's stream: ordered before the step that reads it
+    CK(cudaMallocHost(&hp, blk));
+    cudaError_t ce = cudaMallocHost(&hpf, blk);
+    if (ce != cudaSuccess) { cudaFreeHost(hp); rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
+    memset(hp, 0, blk);
+    e->d_pf.blk[i] = dpf; e->h_rows.blk[i] = hp; e->h_pf.blk[i] = hpf; e->d_rows.blk[i] = dp;
+    return RR_OK;
+}
+
+// Caller holds gpu_mu.  The stop-sequence buffers, allocated on the first request with stop sequences: 2 x 268 B x Bm of
+// parameter blocks, the history and 8 B x Bm of results.  An engine that never sees one allocates nothing.
+static int ensure_stop_buffers(rr_engine* e) {
+    if (e->d_rows.blk[3]) return RR_OK;
+    int rc = ensure_hist(e);
+    if (rc == RR_OK && !e->d_stop) rc = dalloc(e, &e->d_stop, 2 * (size_t)e->Bm);
+    if (rc != RR_OK) return rc;
+    if (!e->h_stop) CK(cudaMallocHost(&e->h_stop, sizeof(int32_t) * 2 * e->Bm));
+    return ensure_block(e, 3);
 }
 
 // Caller holds gpu_mu.  The penalty buffers, allocated on the first processed request, so an engine that never sees one
 // keeps its footprint.
 static int ensure_pen_buffers(rr_engine* e) {
     if (e->d_rows.blk[2]) return RR_OK;
-    const int B = e->Bm;
-    const size_t blk = e->d_rows.bytes(2);            // also the prefill blocks' size: Bm rows of PEN_MAX_BIAS
-    char *dp = nullptr, *dpf = nullptr;
-    int32_t *hist = nullptr, *ws = nullptr;
-    int rc = dalloc(e, &dp, blk);
-    if (rc == RR_OK) rc = dalloc(e, &dpf, blk, false);
-    if (rc == RR_OK) rc = dalloc(e, &hist, (size_t)B * e->o.ctx_max, false);
-    if (rc == RR_OK) rc = dalloc(e, &ws, (size_t)B * e->d.vocab, false);
-    if (rc != RR_OK) return rc;
-    CK(cudaMemsetAsync(dp, 0, blk, e->stream));
-    CK(cudaMemsetAsync(ws, 0, sizeof(int32_t) * B * (size_t)e->d.vocab, e->stream));
-    char *hp = nullptr, *hpf = nullptr;
-    CK(cudaMallocHost(&hp, blk));
-    cudaError_t ce = cudaMallocHost(&hpf, blk);
-    if (ce != cudaSuccess) { cudaFreeHost(hp); rr::note_cuda_error(ce); return RR_CUDA_ERROR; }
-    memset(hp, 0, blk);
-    CK(cudaStreamSynchronize(e->stream));
-    e->d_pf.blk[2] = dpf; e->d_hist = hist; e->pen_ws = ws; e->h_rows.blk[2] = hp; e->h_pf.blk[2] = hpf;
-    e->d_rows.blk[2] = dp;
-    return RR_OK;
+    int rc = ensure_hist(e);
+    if (rc == RR_OK && !e->pen_ws) {
+        rc = dalloc(e, &e->pen_ws, (size_t)e->Bm * e->d.vocab, false);
+        if (rc == RR_OK) CK(cudaMemsetAsync(e->pen_ws, 0, sizeof(int32_t) * e->Bm * (size_t)e->d.vocab, e->stream));
+    }
+    return rc != RR_OK ? rc : ensure_block(e, 2);
 }
 
 // The rest of layer l after attention on `rows` rows of the decode working set, with the unfused kernels: O GEMM,
@@ -395,9 +461,12 @@ static int enqueue_o_mlp(rr_engine* e, int l, int rows, cudaStream_t s, uint64_t
 //   mode & 2: rows with temperature > 0 replace the argmax token by rr_op_sample's draw at `position`.
 //   mode & 1: logprobs of the rows with top_n >= 0 (the logits are left as they were), with mode & 2 also the logprob of
 //             the token in tok into d_tok_lp.
+//   mode & 8: stop sequences over the picked token, into d_stop (cut[Bm] | hold[Bm]).  Decode: the token joins history row
+//             r at its position (pos_inc has advanced `position` to it) - gen0.  Prefill (hist null): it is token 0 of the
+//             history of its slot, stop_row[r].
 static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int mode, int32_t* tok,
                              const int32_t* row_active, int32_t* pos_inc, const int32_t* position, int32_t* hist,
-                             cudaStream_t s) {
+                             cudaStream_t s, const int32_t* stop_row = nullptr) {
     const int V = e->d.vocab;
     uint64_t nl = 0;
     if (mode & 4) {
@@ -415,14 +484,27 @@ static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int m
                         mode & 2 ? tok : nullptr, mode & 2 ? e->d_tok_lp : nullptr);
         nl += LP_LAUNCHES;
     }
+    if (mode & 8) {
+        StopArgs a = p.stop_args();
+        a.hist = e->d_hist; a.hist_ld = e->o.ctx_max; a.hist_row = stop_row; a.tok = tok;
+        a.position = hist ? position : nullptr; a.row_active = row_active;
+        a.cut = e->d_stop; a.hold = e->d_stop + e->Bm;
+        launch_stop_match(a, rows, s); ++nl;
+    }
     return nl;
 }
 
 // Reads a tail's results for `rows` rows back to the host: the tokens (h_tok), with mode & 1 the [rows][LP_MAX_TOP]
-// logprobs and ids (h_lp, h_lp_id), and with mode & 3 == 3 the drawn tokens' logprobs (h_tok_lp).
+// logprobs and ids (h_lp, h_lp_id), with mode & 3 == 3 the drawn tokens' logprobs (h_tok_lp), and with mode & 8 the stop
+// results (h_stop: cut[Bm] | hold[Bm]).
 static int enqueue_readback(rr_engine* e, const int32_t* tok, int rows, int mode, cudaStream_t s) {
     CK(cudaMemcpyAsync(e->h_tok, tok, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
     e->st.d2h_bytes += sizeof(int32_t) * rows;
+    if (mode & 8) {
+        for (int i = 0; i < 2; ++i)
+            CK(cudaMemcpyAsync(e->h_stop + i * e->Bm, e->d_stop + i * e->Bm, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += 2 * sizeof(int32_t) * rows;
+    }
     if (!(mode & 1)) return RR_OK;
     const size_t n = (size_t)rows * LP_MAX_TOP;
     CK(cudaMemcpyAsync(e->h_lp, e->d_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
@@ -479,7 +561,7 @@ static int capture_decode_step(rr_engine* e, int mode, cudaGraphExec_t* out, uin
 }
 
 // mode: the step_mode bits of the active rows (enqueue_tail).  Each combination has its own graph, captured on first use;
-// a step without logprobs, sampled or processed rows replays the plain graph.
+// a step without logprobs, sampled, processed or stop rows replays the plain graph.
 static int run_decode_step(rr_engine* e, int mode) {
     cudaStream_t s = e->stream;
     if (!e->warmed || !e->o.use_cuda_graph) {
@@ -566,7 +648,8 @@ struct PrefillTail {
 // activates the rows. Caller holds gpu_mu.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
-// tail (optional): the tail rows and their request parameters.  Only a logit bias applies (penalties count generated
+// tail (optional): the tail rows and their request parameters.  Stop sequences are matched over the first token (needs
+// ensure_stop_buffers; results in e->h_stop row j).  Only a logit bias applies (penalties count generated
 // tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position
 // pos0 + the sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's
 // logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
@@ -625,6 +708,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     for (int j = 0; (mode & 4) && j < nt; ++j) max_bias = std::max(max_bias, (int)tail->gen[j]->bias_id.size());
     if (max_bias == 0) mode &= ~4;
     else if (!e->d_pf.blk[2]) return RR_INTERNAL;
+    if ((mode & 8) && !e->d_pf.blk[3]) return RR_INTERNAL;
     const ParamBlocks hp = e->h_pf.at(nt, max_bias), dp = e->d_pf.at(nt, max_bias);
     for (int j = 0; mode && j < nt; ++j) {
         const int q = tail->seq[j];
@@ -689,7 +773,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ++nl;
     }
     if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..nt-1)
-    nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s);
+    nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s, p_tsl);
     launch_pdl(activate_rows_kernel, dim3((nt + 127) / 128), dim3(128), 0, s, p_tsl, (const int32_t*)e->p_first,
                (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
     const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
@@ -725,7 +809,7 @@ static void set_row_params(rr_engine* e, int b, const Request* r, int choice = 0
     static const GenParams plain;
     const GenParams& p = r ? r->gen : plain;
     e->rows_dirty |= e->h_rows.row_mode(b) | step_mode(p);
-    e->h_rows.put_row(b, p, choice, 0, p.fpen, p.ppen, p.processed() ? (int)r->prompt.size() : 0);
+    e->h_rows.put_row(b, p, choice, 0, p.fpen, p.ppen, r ? (int)r->prompt.size() : 0);
 }
 
 // Before a decode step: copy each parameter block the step reads (step_mode bits) whose mirror changed.
@@ -736,10 +820,17 @@ static void upload_row_params(rr_engine* e, int mode) {
 
 // Caller holds e->mu.  Returns the hook call to make once the lock is released (tag == 0 and no hook: nothing).
 static void finish_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes = nullptr) {
+    for (int c = 0; c < r->n_choices; ++c) {      // ended from outside: a running choice keeps what a reader may have seen
+        if (r->finish[c] >= 0) continue;
+        const size_t n = (size_t)r->visible(c);
+        r->out[c].resize(n);
+        if (r->gen.logprobs()) { r->lp[c].resize(n * r->gen.lp_width()); r->lp_id[c].resize(n * r->gen.lp_width()); }
+        r->hold[c] = 0;
+    }
     r->status = status;
     r->t_done = now_s(e);
     r->done = true;
-    if (notes && e->hook) notes->push_back(DoneNote{r->tag, r->ticket, status, r->n_generated() * r->n_choices});
+    if (notes && e->hook) notes->push_back(DoneNote{r->tag, r->ticket, status, r->n_returned()});
     if (r->detached) {                   // cancelled by its owner: nobody waits for it
         e->table.erase(r->ticket);
         delete r;
@@ -750,21 +841,28 @@ static void run_hooks(rr_engine* e, std::vector<DoneNote>& notes) {
     notes.clear();
 }
 
-// Caller holds e->mu.  Frees every decode row of r (inactive from the next step, parameters back to the defaults) and
-// finishes r with `status`.
-static void release_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes) {
-    for (int b : r->rows) {
-        e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1;
-        set_row_params(e, b, nullptr);
-    }
+// Caller holds e->mu.  Frees the decode row of choice c of r, if it still has one: inactive from the next step, parameters
+// back to the defaults, free for the next waiting prompt.
+static void release_row(rr_engine* e, Request* r, int c) {
+    const int b = r->rows[c];
+    if (b < 0) return;
+    e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1;
+    set_row_params(e, b, nullptr);
     e->slots_dirty = true;
+    r->rows[c] = -1;
+}
+
+// Caller holds e->mu.  Frees every decode row r still has and finishes r with `status`.
+static void release_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes) {
+    for (int c = 0; c < (int)r->rows.size(); ++c) release_row(e, r, c);
     r->rows.clear();
     finish_request(e, r, status, notes);
 }
 
 // Caller holds e->mu.  Appends the token read back for row `row` to choice c of r, with its pairs (h_lp / h_lp_id row
-// `row`, and for a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  True once every
-// choice of r has max_new tokens: the choices run in lockstep, so that is the step's last row of r.
+// `row`, and for a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  With stop sequences
+// it takes the row's cut / hold (h_stop): a hit finishes the choice with reason stop, its tokens and pairs truncated to the
+// cut.  Otherwise max_new tokens finish it with reason length.  True when the choice finished.
 static bool take_token(rr_engine* e, Request* r, int c, int row) {
     r->out[c].push_back(e->h_tok[row]);
     if (r->gen.logprobs()) {
@@ -776,9 +874,19 @@ static bool take_token(rr_engine* e, Request* r, int c, int row) {
         if (r->gen.sampled()) { r->lp[c].push_back(e->h_tok_lp[row]); r->lp_id[c].push_back(r->out[c].back()); }
     }
     e->st.generated_tokens += 1;
-    for (const std::vector<int32_t>& o : r->out)
-        if ((int)o.size() < r->max_new) return false;
-    return true;
+    const int cut = r->gen.stops() ? e->h_stop[row] : -1;
+    if (cut >= 0 && cut < (int)r->out[c].size()) {
+        r->out[c].resize(cut);
+        if (r->gen.logprobs()) {
+            r->lp[c].resize((size_t)cut * r->gen.lp_width()); r->lp_id[c].resize((size_t)cut * r->gen.lp_width());
+        }
+        r->finish[c] = 1;
+    } else if ((int)r->out[c].size() >= r->max_new) {
+        r->finish[c] = 0;
+    } else if (r->gen.stops()) {
+        r->hold[c] = std::min(std::max(e->h_stop[e->Bm + row], 0), (int)r->out[c].size());
+    }
+    return r->finish[c] >= 0;
 }
 
 // Caller holds e->mu.  Prefix caching: the slot a prompt p is admitted into and how many of its tokens are cached there.
@@ -929,6 +1037,7 @@ static void worker_main(rr_engine* e) {
             tail.n = (int)tail_seq.size(); tail.seq = tail_seq.data(); tail.slot = tail_slot.data();
             tail.choice = tail_choice.data(); tail.gen = tail_gen.data(); tail.mode = chunk_mode;
             int rc = (chunk_mode & 4) ? ensure_pen_buffers(e) : RR_OK;
+            if (rc == RR_OK && (chunk_mode & 8)) rc = ensure_stop_buffers(e);
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
                                  e->o.prefix_cache ? pos0.data() : nullptr, copies, &tail);
@@ -947,11 +1056,11 @@ static void worker_main(rr_engine* e) {
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
                 r->t_first = t;
-                bool done = false;
-                for (int c = 0; c < r->n_choices; ++c) done = take_token(e, r, c, row0 + c);
-                if (done) release_request(e, r, RR_OK, &notes);
-                else
-                    for (int c = 0; c < r->n_choices; ++c) set_row_params(e, r->rows[c], r, c);
+                for (int c = 0; c < r->n_choices; ++c) {
+                    if (take_token(e, r, c, row0 + c)) release_row(e, r, c);
+                    else set_row_params(e, r->rows[c], r, c);
+                }
+                if (r->all_finished()) release_request(e, r, RR_OK, &notes);
             }
             e->cv_done.notify_all();
             continue;   // look for more waiting prompts before decoding
@@ -982,8 +1091,11 @@ static void worker_main(rr_engine* e) {
             for (int b = 0; b < e->Bm; ++b) {              // a released request's later rows are already free
                 Request* r = e->row_req[b];
                 if (!r) continue;
-                if (rc != RR_OK) release_request(e, r, RR_INTERNAL, &notes);
-                else if (take_token(e, r, e->row_choice[b], b)) release_request(e, r, RR_OK, &notes);
+                if (rc != RR_OK) { release_request(e, r, RR_INTERNAL, &notes); continue; }
+                const int c = e->row_choice[b];
+                if (!take_token(e, r, c, b)) continue;
+                release_row(e, r, c);                      // the row is free for the next waiting prompt at once
+                if (r->all_finished()) release_request(e, r, RR_OK, &notes);
             }
         }
         e->cv_done.notify_all();
@@ -1178,6 +1290,7 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_lp) cudaFreeHost(e->h_lp);
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
+    if (e->h_stop) cudaFreeHost(e->h_stop);
     for (const ParamBlocks* p : {&e->h_rows, &e->h_pf})
         for (char* b : p->blk)
             if (b) cudaFreeHost(b);
@@ -1262,6 +1375,7 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     r->max_new = max_new_tokens;
     r->n_choices = n_choices;
     r->out.resize(n_choices);
+    r->finish.assign(n_choices, -1); r->hold.assign(n_choices, 0);
     r->lp.resize(n_choices); r->lp_id.resize(n_choices);
     for (int c = 0; c < n_choices; ++c) {
         r->out[c].reserve(max_new_tokens);
@@ -1305,15 +1419,24 @@ int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab
 }
 }  // namespace rr
 
+RR_API int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
+                                 int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                                 float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
+                                 int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off, uint64_t* ticket) {
+    if (!e) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off);
+    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
+}
+
 RR_API int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                                     int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
                                     float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
                                     const float* bias_vals, uint64_t* ticket) {
-    if (!e) return RR_INVALID_ARGUMENT;
-    rr::GenParams p;
-    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals);
-    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
+    return rr_engine_submit_stop(e, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature, top_p, seed,
+                                 frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, 0, nullptr, nullptr,
+                                 ticket);
 }
 
 RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
@@ -1342,14 +1465,14 @@ RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int
                                       0.f, 0, nullptr, nullptr, ticket);
 }
 
-// Caller holds e->mu.  The first min(n, max_tokens_out) tokens of each choice of r into tokens_out [n_choices]
-// [max_tokens_out], and of a logprobs request their pairs into lp_out / id_out [n_choices][max_tokens_out][K] (any may
-// be null).
+// Caller holds e->mu.  The first min(n, max_tokens_out) visible tokens of each choice of r (fewer for a shorter choice)
+// into tokens_out [n_choices][max_tokens_out], and of a logprobs request their pairs into lp_out / id_out [n_choices]
+// [max_tokens_out][K] (any may be null).
 static void copy_choices(const Request* r, int n, int max_tokens_out, int32_t* tokens_out, float* lp_out, int32_t* id_out) {
-    const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (t <= 0) return;
     const size_t k = (size_t)r->gen.lp_width();
     for (int c = 0; c < r->n_choices; ++c) {
+        const int t = std::min(std::min(n, max_tokens_out), r->visible(c));
+        if (t <= 0) continue;
         const size_t o = (size_t)c * max_tokens_out;
         if (tokens_out) memcpy(tokens_out + o, r->out[c].data(), sizeof(int32_t) * t);
         if (!r->gen.logprobs()) continue;
@@ -1425,10 +1548,11 @@ RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeou
                                    t_first_token_s, nullptr, nullptr);
 }
 
-// rr_engine_wait_choices, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
+// rr_engine_wait_stop, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
 // choices, which stays in flight.
 static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                       int max_tokens_out, float* lp_out, int32_t* id_out, bool choices) {
+                       int max_tokens_out, float* lp_out, int32_t* id_out, bool choices, int32_t* n_tokens_out = nullptr,
+                       int32_t* finish_out = nullptr) {
     if (!e || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1452,10 +1576,20 @@ static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_compl
     out->n_generated = r->n_generated(); out->n_cached = r->n_cached;
     out->t_submit_s = r->t_submit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
     copy_choices(r, r->n_generated(), max_tokens_out, tokens_out, lp_out, id_out);
+    for (int c = 0; c < r->n_choices; ++c) {
+        if (n_tokens_out) n_tokens_out[c] = r->visible(c);
+        if (finish_out) finish_out[c] = r->finish[c] > 0 ? 1 : 0;
+    }
     const int status = r->status;
     e->table.erase(ticket);
     delete r;
     return status == RR_OK ? RR_OK : status;
+}
+
+RR_API int rr_engine_wait_stop(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                               int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out,
+                               int32_t* finish_out) {
+    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true, n_tokens_out, finish_out);
 }
 
 RR_API int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,

@@ -18,6 +18,7 @@
 // config/config.yaml:100-108) for the call shape of reference src/demo_fallback.py:143-147.
 #include "rr_kernels.h"
 
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -47,15 +48,20 @@ struct GwReq {
     int deployment = -1, served_group = -1, chain_pos = 0, replica = -1;
     rr_engine* eng = nullptr;
     uint64_t eng_ticket = 0;
-    std::vector<int32_t> tokens;      // [n_choices][n_gen()]
+    std::vector<int32_t> tokens;      // the choices' returned tokens, one after the other: n_tok[c] of choice c
+    std::vector<int32_t> n_tok, fin;  // [n_choices] tokens returned and finish reason (0 length, 1 stop); empty until settled
     rr::GenParams gen;                // handed to every engine the request is admitted to
-    std::vector<float> lp;            // [n_choices][n_gen()][gen.lp_width()]
+    std::vector<float> lp;            // tokens' pairs, [gen.lp_width()] each
     std::vector<int32_t> lp_id;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;   // t_eng_submit: hand-off to the replica
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
 
-    int n_gen() const { return (int)tokens.size() / n_choices; }      // tokens per choice
+    int n_gen() const {               // tokens of the longest choice
+        int n = 0;
+        for (int32_t t : n_tok) n = t > n ? t : n;
+        return n;
+    }
 };
 
 struct Pending {
@@ -123,17 +129,20 @@ static void gw_finish(rr_gateway* g, GwReq* r, int status) {
 
 // caller holds g->mu.  Request r ended on the replica it was handed to with `status` (n_generated tokens by then, over all
 // choices).  When the replica's record of it was read (wrc RR_OK / RR_BACKEND_FAILED: comp, toks [n_choices][max_new],
-// and with logprobs lps / lp_ids [n_choices][max_new][K]), the result is stored.  Then DONE (with the latency sample) / FAIL / the cancel report is posted and the request finishes,
+// each choice's token count n_toks and finish reason fins, and with logprobs lps / lp_ids [n_choices][max_new][K]), the
+// result is stored.  Then DONE (with the latency sample) / FAIL / the cancel report is posted and the request finishes,
 // or after a backend failure goes back into the queue one step further down its fallback chain.
 static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int wrc, const rr_completion& comp,
-                      const int32_t* toks, const float* lps, const int32_t* lp_ids) {
+                      const int32_t* toks, const int32_t* n_toks, const int32_t* fins, const float* lps,
+                      const int32_t* lp_ids) {
     const int dep = r->deployment;
     if (wrc == RR_OK || wrc == RR_BACKEND_FAILED) {
-        int n = comp.n_generated < r->max_new ? comp.n_generated : r->max_new;
-        n = n > 0 ? n : 0;
         const size_t k = (size_t)r->gen.lp_width();
-        r->tokens.clear(); r->lp.clear(); r->lp_id.clear();
+        r->tokens.clear(); r->lp.clear(); r->lp_id.clear(); r->n_tok.clear(); r->fin.clear();
         for (int c = 0; c < r->n_choices; ++c) {
+            int n = n_toks[c] < r->max_new ? n_toks[c] : r->max_new;
+            n = n > 0 ? n : 0;
+            r->n_tok.push_back(n); r->fin.push_back(fins[c]);
             const size_t o = (size_t)c * r->max_new;
             r->tokens.insert(r->tokens.end(), toks + o, toks + o + n);
             if (r->gen.logprobs()) {
@@ -168,7 +177,7 @@ static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int 
             r->chain_start = r->chain_pos + 1;
             r->state = Q_ADMIT;
             r->eng = nullptr;
-            r->tokens.clear();
+            r->tokens.clear(); r->n_tok.clear(); r->fin.clear();
             r->lp.clear(); r->lp_id.clear();
             r->n_cached = 0;
             g->st.failed_over++;
@@ -203,15 +212,17 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     std::vector<int32_t> toks(n_ch * (size_t)(max_new > 0 ? max_new : 1));
     std::vector<float> lps(logprobs ? toks.size() * k : 0);
     std::vector<int32_t> lp_ids(lps.size());
+    std::vector<int32_t> n_toks(n_ch, 0), fins(n_ch, 0);
     int wrc = RR_INVALID_ARGUMENT;
     if (eng && status != RR_CANCELLED)
-        wrc = rr_engine_wait_choices(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
-                                     logprobs ? lp_ids.data() : nullptr);
+        wrc = rr_engine_wait_stop(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
+                                  logprobs ? lp_ids.data() : nullptr, n_toks.data(), fins.data());
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
         if (it == g->table.end()) return;
-        gw_settle(g, it->second, status, n_generated, wrc, comp, toks.data(), lps.data(), lp_ids.data());
+        gw_settle(g, it->second, status, n_generated, wrc, comp, toks.data(), n_toks.data(), fins.data(), lps.data(),
+                  lp_ids.data());
     }
     g->cv_work.notify_one();
     g->cv_done.notify_all();
@@ -232,7 +243,9 @@ static void gw_serve_stub(rr_gateway* g, GwReq* r, int rep) {
     comp.t_submit_s = r->t_eng_submit;
     comp.t_first_token_s = comp.t_done_s = gw_now_s(g);
     const int status = failed ? RR_BACKEND_FAILED : RR_OK;
-    gw_settle(g, r, status, comp.n_generated * r->n_choices, status, comp, toks.data(), nullptr, nullptr);
+    const std::vector<int32_t> n_toks((size_t)r->n_choices, comp.n_generated), fins((size_t)r->n_choices, 0);
+    gw_settle(g, r, status, comp.n_generated * r->n_choices, status, comp, toks.data(), n_toks.data(), fins.data(), nullptr,
+              nullptr);
 }
 
 static void gw_dispatch(rr_gateway* g) {
@@ -472,18 +485,29 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
 
 // The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
 // gets RR_INVALID_ARGUMENT.
+RR_API int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                  int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                  float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                  const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
+                                  uint64_t* ticket) {
+    if (!g) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off);
+    if (rc != RR_OK) return rc;
+    // a mock replica has no logits to fill the pairs from and no decode loop to cut
+    if ((p.logprobs() || p.stops()) && g->has_stub) return RR_INVALID_ARGUMENT;
+    const int32_t start[2] = {0, n_prompt};
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
+}
+
 RR_API int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                                      int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
                                      float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
                                      const float* bias_vals, uint64_t* ticket) {
-    if (!g) return RR_INVALID_ARGUMENT;
-    rr::GenParams p;
-    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals);
-    if (rc != RR_OK) return rc;
-    if (p.logprobs() && g->has_stub) return RR_INVALID_ARGUMENT;     // a mock replica has no logits to fill the pairs from
-    const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
+    return rr_gateway_submit_stop(g, group, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature,
+                                  top_p, seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, 0, nullptr,
+                                  nullptr, ticket);
 }
 
 RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
@@ -512,15 +536,16 @@ RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* pr
                                        0.f, 0.f, 0, nullptr, nullptr, ticket);
 }
 
-// caller holds g->mu.  The first min(n, max_tokens_out) tokens of each choice into tokens_out [n_choices][max_tokens_out],
-// and of a logprobs request their pairs into lp_out / id_out [n_choices][max_tokens_out][r->gen.lp_width()] (any may be
-// null).
+// caller holds g->mu.  The first min(n, max_tokens_out) tokens of each choice (fewer for a shorter choice) into tokens_out
+// [n_choices][max_tokens_out], and of a logprobs request their pairs into lp_out / id_out [n_choices][max_tokens_out]
+// [r->gen.lp_width()] (any may be null).
 static void gw_copy_choices(const GwReq* r, int n, int max_tokens_out, int32_t* tokens_out, float* lp_out, int32_t* id_out) {
-    const int t = n < max_tokens_out ? n : max_tokens_out;
-    if (t <= 0) return;
-    const size_t k = (size_t)r->gen.lp_width(), have = (size_t)r->n_gen();
-    for (int c = 0; c < r->n_choices; ++c) {
-        const size_t o = (size_t)c * max_tokens_out, src = (size_t)c * have;
+    const size_t k = (size_t)r->gen.lp_width();
+    size_t src = 0;
+    for (size_t c = 0; c < r->n_tok.size(); src += (size_t)r->n_tok[c], ++c) {
+        const int t = std::min(std::min(n, max_tokens_out), (int)r->n_tok[c]);
+        if (t <= 0) continue;
+        const size_t o = c * (size_t)max_tokens_out;
         if (tokens_out) memcpy(tokens_out + o, r->tokens.data() + src, sizeof(int32_t) * (size_t)t);
         if (!r->gen.logprobs()) continue;
         if (lp_out) memcpy(lp_out + o * k, r->lp.data() + src * k, sizeof(float) * t * k);
@@ -534,13 +559,14 @@ static void gw_fill(const GwReq* r, rr_gateway_result* out) {
     out->replica = r->replica; out->n_prompt = (int32_t)r->prompt.size(); out->n_generated = (int32_t)r->n_gen();
     out->attempts = r->attempts;
     out->t_submit_s = r->t_submit; out->t_admit_s = r->t_admit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
-    out->n_cached = r->n_cached; out->reserved = 0;
+    out->n_cached = r->n_cached; out->reserved = r->fin.empty() ? 0 : r->fin[0];
 }
 
 // rr_gateway_wait_choices, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
 // choices, which stays in flight.
 static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                   int max_tokens_out, float* lp_out, int32_t* id_out, bool choices) {
+                   int max_tokens_out, float* lp_out, int32_t* id_out, bool choices, int32_t* n_tokens_out = nullptr,
+                   int32_t* finish_out = nullptr) {
     if (!g || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(g->mu);
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
@@ -563,10 +589,20 @@ static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_
     }
     gw_fill(r, out);
     gw_copy_choices(r, r->n_gen(), max_tokens_out, tokens_out, lp_out, id_out);
+    for (int c = 0; c < r->n_choices; ++c) {      // a request that never reached a replica has no per-choice record
+        if (n_tokens_out) n_tokens_out[c] = (size_t)c < r->n_tok.size() ? r->n_tok[c] : 0;
+        if (finish_out) finish_out[c] = (size_t)c < r->fin.size() ? r->fin[c] : 0;
+    }
     const int status = r->status;
     g->table.erase(ticket);
     delete r;
     return status;
+}
+
+RR_API int rr_gateway_wait_stop(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                                int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out,
+                                int32_t* finish_out) {
+    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true, n_tokens_out, finish_out);
 }
 
 RR_API int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,

@@ -89,16 +89,25 @@ struct GenParams {
     bool logprobs() const { return top_lp >= 0; }
     bool sampled() const { return temp > 0.f; }
     bool processed() const { return fpen != 0.f || ppen != 0.f || !bias_id.empty(); }
+    // stop sequences (rr_op_stop_match): n_stop of them, sequence i = stop[i][0 .. stop_len[i]) bytes of reply text
+    int n_stop = 0;
+    uint8_t stop_len[4] = {};
+    uint8_t stop[4][64] = {};
+    bool stops() const { return n_stop > 0; }
     // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
     int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
     // The raw C arguments, checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and OpenAI's ranges
     // 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null arrays when
-    // n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails.  A greedy request keeps the
-    // default top_p and seed, an unprocessed one the default penalties.  RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
+    // n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails; 0 <= n_stop <= STOP_MAX_SEQS
+    // sequences of 1..STOP_MAX_LEN bytes each, sequence i = stop_bytes[stop_off[i] .. stop_off[i + 1]) (non-null arrays when
+    // n_stop > 0).  A greedy request keeps the default top_p and seed, an unprocessed one the default penalties.
+    // RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
     int set(int vocab, int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals);
+            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
+            const uint8_t* stop_bytes, const int32_t* stop_off);
 };
-// n_choices (1..max_batch): choices of the request (rr_engine_submit_choices); the done hook's n_generated is their total.
+// n_choices (1..max_batch): choices of the request (rr_engine_submit_choices); the done hook's n_generated is the total of
+// the tokens the choices return (a choice cut by a stop sequence counts what is left of it).
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, const GenParams& p, int n_choices);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
@@ -236,6 +245,27 @@ struct PenaltyArgs {
 };
 void launch_logit_penalties(float* logits, int ld, int rows, int vocab, const PenaltyArgs& a, int32_t* cnt_ws,
                             cudaStream_t st);
+// Stop sequences (rr_op_stop_match), one launch, one warp per row.  Row r has n_stop[r] sequences (0: the row is skipped and
+// its outputs are not written), sequence s = bytes[r][s][0 .. len[r][s]).  The kernel stores tok[r] (the token just picked)
+// in the row's history (hist + (hist_row ? hist_row[r] : r) * hist_ld) at index i = position[r] - gen0[r] (position null:
+// i = 0) and matches the reply text of history[0 .. i] (token t >= 3 is the byte (t - 3) % 256, t < 3 is no text):
+//   cut[r]  = -1, or when the text now ends in a sequence and tok[r] has a byte: the history index of the first token of the
+//             longest such sequence (= the tokens to keep)
+//   hold[r] = 0 on a hit, else the tokens from the first token of the longest text suffix that is a proper prefix of some
+//             sequence up to tok[r] (0: no such suffix)
+// Rows with row_active[r] < 0 (row_active optional) are skipped like rows without sequences.
+constexpr int STOP_MAX_SEQS = 4;
+constexpr int STOP_MAX_LEN = 64;
+struct StopArgs {
+    const int32_t *n_stop, *gen0;
+    const uint8_t* len;              // [rows][STOP_MAX_SEQS]
+    const uint8_t* bytes;            // [rows][STOP_MAX_SEQS][STOP_MAX_LEN]
+    int32_t* hist;
+    int hist_ld;
+    const int32_t *hist_row, *tok, *position, *row_active;
+    int32_t *cut, *hold;
+};
+void launch_stop_match(const StopArgs& a, int rows, cudaStream_t st);
 
 // ---- attention (rr_attn_decode.cu, rr_attn_tc.cu) ---------------------------------------------------
 struct DecodeAttnArgs {

@@ -15,7 +15,7 @@ import torch
 
 from . import _lib
 from .models import ModelSpec, Weights, make_weights
-from .router import gen_args, logprob_pairs
+from .router import FINISH_REASONS, check_stop, gen_args, logprob_pairs
 
 
 @dataclass
@@ -35,6 +35,9 @@ class CompletionRecord:
     # submit(n=k): every choice's tokens and, with top_logprobs, pairs ([k][tokens]); tokens / logprobs are choice 0's
     choices: List[List[int]] = field(default_factory=list)
     choice_logprobs: Optional[List[List[List[Tuple[int, float]]]]] = None
+    # every choice's finish reason: "stop" when a stop sequence of submit(stop=) cut it (its tokens end before the match),
+    # else "length"; with `stop` the choices have their own lengths
+    finish_reasons: List[str] = field(default_factory=list)
 
     @property
     def ttft(self) -> float:
@@ -105,7 +108,8 @@ class Engine:
                                1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
-        self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1
+        self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1 or with stop
+        self._stop: set = set()             # tickets of the requests submitted with stop
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -152,7 +156,7 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
                temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None,
                frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-               logit_bias: Optional[Dict[int, float]] = None, n: int = 1) -> int:
+               logit_bias: Optional[Dict[int, float]] = None, n: int = 1, stop=None) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
@@ -160,13 +164,22 @@ class Engine:
         {token id: bias in [-100, 100]} (at most 300 entries): applied to the logits before every token is picked, the
         penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing.
         n in 1..max_batch: n choices of the prompt, prefilled once (rr_engine_submit_choices); choice i is drawn with
-        seed + i.  wait() returns them all; peek() is for n = 1 only."""
+        seed + i.  wait() returns them all; peek() is for n = 1 only.
+        stop: a string or up to 4 strings (or bytes) of 1..64 bytes each: a choice ends where its reply text (the bytes of
+        its tokens) would contain one, returns the tokens before the match and frees its decode row at once
+        (rr_engine_submit_stop).  The tokens are a prefix of the same request's without `stop`."""
         ids = _i32(prompt_ids)
         bias = logit_bias or {}
+        stops = stop if isinstance(stop, (list, tuple)) and all(isinstance(b, bytes) for b in stop) else check_stop(stop)
         gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
-                       list(bias.values()))
+                       list(bias.values()), stop=stops)
         t = C.c_uint64()
-        if n == 1:
+        if gen.stop:
+            _lib.check(_lib.lib.rr_engine_submit_stop(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail, *gen.stop,
+                                                      C.byref(t)), "rr_engine_submit_stop")
+            self._n[t.value] = n
+            self._stop.add(t.value)
+        elif n == 1:
             _lib.check(_lib.lib.rr_engine_submit_processed(self._h, _p(ids), len(ids), max_new_tokens, *gen.tail,
                                                            C.byref(t)), "rr_engine_submit_processed")
         else:
@@ -189,18 +202,25 @@ class Engine:
         nc = self._n.get(ticket, 1)
         buf = np.zeros((nc, max_tokens), dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens, nc)
-        wait = _lib.lib.rr_engine_wait_choices if nc > 1 else _lib.lib.rr_engine_wait_logprobs
-        rc = wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
+        n_tok, fin = (C.c_int32 * nc)(), (C.c_int32 * nc)()
+        if ticket in self._stop:
+            rc = _lib.lib.rr_engine_wait_stop(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p,
+                                              n_tok, fin)
+        else:
+            wait = _lib.lib.rr_engine_wait_choices if nc > 1 else _lib.lib.rr_engine_wait_logprobs
+            rc = wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
+            n_tok[:] = [c.n_generated] * nc
         if rc != 6:
             self._lp_k.pop(ticket, None)
             self._n.pop(ticket, None)
+            self._stop.discard(ticket)
         if rc not in (0, 6, 7):
             _lib.check(rc, "rr_engine_wait")
-        n = min(c.n_generated, max_tokens)
-        toks = [row[:n].tolist() for row in buf]
-        pairs = [logprob_pairs(a, b, 0, n) for a, b in zip(lp, ids)] if lp is not None else None
+        ns = [min(k, max_tokens) for k in n_tok]
+        toks = [row[:k].tolist() for row, k in zip(buf, ns)]
+        pairs = [logprob_pairs(a, b, 0, k) for a, b, k in zip(lp, ids, ns)] if lp is not None else None
         return CompletionRecord(ticket, rc, c.n_prompt, toks[0], c.t_submit_s, c.t_first_token_s, c.t_done_s,
-                                pairs[0] if pairs else None, c.n_cached, toks, pairs)
+                                pairs[0] if pairs else None, c.n_cached, toks, pairs, [FINISH_REASONS[f] for f in fin])
 
     def peek(self, ticket: int, have: int, timeout: float = 0.05, max_tokens: int = 4096):
         """Streaming: wait until more than `have` tokens exist (or done / timeout). -> (tokens so far, done, ttft_s), and

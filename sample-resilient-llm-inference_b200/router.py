@@ -249,21 +249,52 @@ def check_n(n: Any) -> int:
     return n
 
 
+MAX_STOP = 4                 # OpenAI's limit on the number of `stop` sequences (STOP_MAX_SEQS of the engine)
+MAX_STOP_BYTES = 64          # this project's cap on one stop sequence, in bytes of UTF-8 (STOP_MAX_LEN of the engine)
+FINISH_REASONS = ("length", "stop")      # by the native finish code (rr_engine_wait_stop)
+
+
+def check_stop(stop: Any) -> List[bytes]:
+    """OpenAI's rules for the `stop` request field -> the stop sequences as UTF-8 bytes: none for None or [], one for a
+    string, else a list of 1..4 strings, each 1..64 bytes long.  They are matched on the bytes of the reply.  Raises
+    BadRequestError (HTTP 400) for anything else."""
+    if stop is None:
+        return []
+    seqs = [stop] if isinstance(stop, str) else stop
+    if not isinstance(seqs, (list, tuple)) or any(not isinstance(s, str) for s in seqs):
+        raise BadRequestError("`stop` must be a string or an array of strings")
+    if len(seqs) > MAX_STOP:
+        raise BadRequestError(f"`stop` may hold at most {MAX_STOP} sequences")
+    out = [s.encode("utf-8") for s in seqs]
+    if any(len(b) == 0 for b in out):
+        raise BadRequestError("`stop` sequences must not be empty: each is 1 to "
+                              f"{MAX_STOP_BYTES} bytes of UTF-8")
+    if any(len(b) > MAX_STOP_BYTES for b in out):
+        raise BadRequestError(f"a `stop` sequence may be at most {MAX_STOP_BYTES} bytes of UTF-8")
+    return out
+
+
 class GenArgs(NamedTuple):
     """A request's generation parameters in the form the native submit calls take them (gen_args)."""
     top: Optional[int]     # top_logprobs; None: no logprobs
     tail: tuple            # rr_engine_submit_processed / rr_gateway_submit_processed: top_logprobs .. bias_vals
     width: int             # (logprob, id) pairs per generated token; 0 without logprobs
+    stop: tuple = ()       # with stop sequences, what rr_*_submit_stop takes after the tail: n_stop, stop_bytes, stop_off
+
+
+class StreamItem(tuple):
+    """An item of Router.completion_stream; the closing one carries the choice's finish reason."""
+    finish_reason: Optional[str] = None
 
 
 def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
              seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
              presence_penalty: Optional[float] = None, bias_ids: Sequence[int] = (),
-             bias_vals: Sequence[float] = ()) -> GenArgs:
+             bias_vals: Sequence[float] = (), stop: Sequence[bytes] = ()) -> GenArgs:
     """None and absent fields take the defaults of a plain greedy request.  A sampled request (temperature > 0) without
     a seed gets a random one here, once, so that a fallback re-admission draws the same tokens; the seed is taken modulo
-    2^64.  Without bias entries the bias arrays are null pointers.  Ranges are checked by the native call (check_* raise
-    HTTP 400 first on the router's path)."""
+    2^64.  Without bias entries the bias arrays are null pointers.  `stop`: the stop sequences as bytes (check_stop).
+    Ranges are checked by the native call (check_* raise HTTP 400 first on the router's path)."""
     k = -1 if top_logprobs is None else int(top_logprobs)
     temp = float(temperature or 0.0)
     seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temp else 0
@@ -273,7 +304,13 @@ def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = 
         b_vals = np.ascontiguousarray(np.asarray(bias_vals, dtype=np.float32)).ctypes.data_as(C.POINTER(C.c_float))
     tail = (k, temp, 1.0 if top_p is None else float(top_p), seed, float(frequency_penalty or 0.0),
             float(presence_penalty or 0.0), len(bias_ids), b_ids, b_vals)
-    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0)
+    st = ()
+    if len(stop):
+        blob = np.frombuffer(b"".join(stop), dtype=np.uint8).copy()
+        off = np.zeros(len(stop) + 1, dtype=np.int32)
+        np.cumsum([len(b) for b in stop], out=off[1:])
+        st = (len(stop), blob.ctypes.data_as(C.POINTER(C.c_uint8)), off.ctypes.data_as(C.POINTER(C.c_int32)))
+    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0, st)
 
 
 def _token_entry(tok: int, logprob: float) -> dict:
@@ -430,15 +467,20 @@ class Router:
         details = {"cached_tokens": int(n_cached)} if self.cfg.deployments[dep].prefix_cache else None
         return Usage(n_prompt, n_gen, n_prompt + n_gen, details)
 
-    def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None) -> ModelResponse:
-        """toks [n choices][max_new] (or one row), logprobs: one `logprobs` object per choice (or None)."""
+    def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None, n_tokens=None,
+                     finish=None) -> ModelResponse:
+        """toks [n choices][max_new] (or one row), logprobs: one `logprobs` object per choice (or None).  With stop
+        sequences, n_tokens / finish: each choice's token count and finish code (else res.n_generated and length)."""
         d = self.cfg.deployments[res.deployment]
-        rows = [[int(t) for t in row[: res.n_generated]] for row in np.atleast_2d(toks)]
+        toks = np.atleast_2d(toks)
+        n_tokens = [res.n_generated] * len(toks) if n_tokens is None else n_tokens
+        finish = [0] * len(toks) if finish is None else finish
+        rows = [[int(t) for t in row[:k]] for row, k in zip(toks, n_tokens)]
         lps = logprobs if isinstance(logprobs, list) else [logprobs] * len(rows)
         return ModelResponse(
             id="chatcmpl-" + uuid.uuid4().hex[:24], model=d.response_model,
-            choices=[Choice(i, Message("assistant", detokenize(t) if detok else ""), logprobs=lp)
-                     for i, (t, lp) in enumerate(zip(rows, lps))],
+            choices=[Choice(i, Message("assistant", detokenize(t) if detok else ""), FINISH_REASONS[f], logprobs=lp)
+                     for i, (t, lp, f) in enumerate(zip(rows, lps, finish))],
             usage=self._usage(res.deployment, n_prompt, sum(len(t) for t in rows), res.n_cached), created=int(time.time()),
             _token_ids=rows[0], _deployment=res.deployment, _model_group=self.cfg.groups[res.served_group],
             _fell_back=res.chain_pos > 0, _ttft_s=res.t_first_token_s - res.t_submit_s,
@@ -480,13 +522,16 @@ class Router:
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
     def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs, n: int = 1) -> int:
-        """n > 1: rr_gateway_submit_choices; a request of one choice takes rr_gateway_submit_processed, as before."""
+        """With stop sequences: rr_gateway_submit_stop; else n > 1: rr_gateway_submit_choices and a request of one choice
+        rr_gateway_submit_processed."""
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
         p = ids.ctypes.data_as(C.POINTER(C.c_int32))
-        if n > 1:
+        if gen.stop:
+            rc = _lib.lib.rr_gateway_submit_stop(gw, g, p, len(ids), max_new, n, *gen.tail, *gen.stop, C.byref(t))
+        elif n > 1:
             rc = _lib.lib.rr_gateway_submit_choices(gw, g, p, len(ids), max_new, n, *gen.tail, C.byref(t))
         else:
             rc = _lib.lib.rr_gateway_submit_processed(gw, g, p, len(ids), max_new, *gen.tail, C.byref(t))
@@ -512,22 +557,30 @@ class Router:
         res = _lib.GatewayResult()
         toks = np.zeros(max_new if n == 1 else (n, max_new), dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new, n)
-        wait = _lib.lib.rr_gateway_wait_choices if n > 1 else _lib.lib.rr_gateway_wait_logprobs
-        rc = wait(gw, ticket, float(timeout or 0.0), C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
-                  lp_p, ids_p)
+        n_tok = fin = None
+        if gen.stop:                     # the choices end on their own: each has its token count and finish reason
+            n_tok, fin = (C.c_int32 * n)(), (C.c_int32 * n)()
+            rc = _lib.lib.rr_gateway_wait_stop(gw, ticket, float(timeout or 0.0), C.byref(res),
+                                               toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p, n_tok, fin)
+        else:
+            wait = _lib.lib.rr_gateway_wait_choices if n > 1 else _lib.lib.rr_gateway_wait_logprobs
+            rc = wait(gw, ticket, float(timeout or 0.0), C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
+                      lp_p, ids_p)
         if rc == 6:                      # client-side timeout: give the rows back, count a failure against the deployment
             _lib.lib.rr_gateway_cancel(gw, ticket, 1)
             raise self._gw_error(6, model, res, timeout)
         if rc != 0:
             raise self._gw_error(rc, model, res, timeout)
         content = None
+        n_tok = None if n_tok is None else [min(k, max_new) for k in n_tok]
         if gen.top is not None:
-            k = min(res.n_generated, max_new)
+            ks = [min(res.n_generated, max_new)] * n if n_tok is None else n_tok
             content = [{"content": logprobs_content(t[:k].tolist(), logprob_pairs(a, b, 0, k), gen.top), "refusal": None}
-                       for t, a, b in zip(np.atleast_2d(toks), lp.reshape(-1, max_new, gen.width),
-                                          ids.reshape(-1, max_new, gen.width))]
+                       for t, a, b, k in zip(np.atleast_2d(toks), lp.reshape(-1, max_new, gen.width),
+                                             ids.reshape(-1, max_new, gen.width), ks)]
             content = content[0] if n == 1 else content
-        return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content)
+        return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content, n_tokens=n_tok,
+                                 finish=None if fin is None else list(fin))
 
     def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
         ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
@@ -558,9 +611,11 @@ class Router:
                         raise self._gw_error(rc, model, res, timeout)
                     label = self.cfg.deployments[res.deployment].response_model
                     ttft = res.t_first_token_s - res.t_submit_s
-                    if res.n_generated > sent:
+                    if res.n_generated > sent:       # the last tokens, with any a pending partial stop match held back
                         yield item(label, sent, res.n_generated, ttft)
-                    yield (label, [], True, ttft) if top is None else (label, [], True, ttft, [])
+                    last = StreamItem((label, [], True, ttft) if top is None else (label, [], True, ttft, []))
+                    last.finish_reason = FINISH_REASONS[res.reserved]
+                    yield last
                     return
                 if n.value > sent and res.deployment >= 0:
                     label = self.cfg.deployments[res.deployment].response_model
@@ -653,22 +708,26 @@ class Router:
         return min((b.vocab for b in self.backends.values()), default=128256)
 
     def _params(self, logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                logit_bias) -> GenArgs:
-        """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs; bias ids
-        must be valid on every replica the request may fall back to."""
+                logit_bias, stop=None) -> GenArgs:
+        """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs and a decode
+        loop that stop sequences can end; bias ids must be valid on every replica the request may fall back to."""
         top = check_logprobs(logprobs, top_logprobs)
-        if top is not None and any(isinstance(b, StubBackend) for b in self.backends.values()):
+        stops = check_stop(stop)
+        mock = any(isinstance(b, StubBackend) for b in self.backends.values())
+        if stops and mock:
+            raise BadRequestError("`stop` is not available: the backends of this router are not model replicas")
+        if top is not None and mock:
             raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
         samp = check_sampling(temperature, top_p, seed) or (None, None, None)
         pen = check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab()) or (None, None, (), ())
-        return gen_args(top, *samp, *pen)
+        return gen_args(top, *samp, *pen, stop=stops)
 
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
                    logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                    top_p: Optional[float] = None, seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
                    presence_penalty: Optional[float] = None, logit_bias: Optional[Dict[str, float]] = None,
-                   n: Optional[int] = None, **_ignored) -> ModelResponse:
+                   n: Optional[int] = None, stop: Any = None, **_ignored) -> ModelResponse:
         """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
         (0..20) most likely alternatives, as the OpenAI API returns them.  temperature > 0: every token is drawn from
         the top_p nucleus of softmax(logits / temperature) with the request's seed (rr_op_sample); absent or 0 is
@@ -678,10 +737,14 @@ class Router:
         n (1..128, at most the decode rows of the smallest engine replica): n choices of the same prompt, prefilled once
         (rr_gateway_submit_choices).  Choice i of a sampled request is drawn with seed + i (mod 2^64), so it equals the
         n=1 response with that seed; greedy choices are all the greedy response.  usage.completion_tokens sums the
-        choices and `_choice_token_ids` holds each choice's tokens (`_token_ids`: choice 0's)."""
+        choices and `_choice_token_ids` holds each choice's tokens (`_token_ids`: choice 0's).
+        stop: a string or up to 4 strings of 1..64 bytes of UTF-8 each.  A choice ends where its reply would contain one
+        of them: the content stops before it and finish_reason is "stop" (rr_gateway_submit_stop).  They are matched on
+        the reply's bytes, so the tokens are a prefix of the same request's without `stop`; each choice ends on its own
+        and usage.completion_tokens counts the tokens returned."""
         n = check_n(n)
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                           logit_bias)
+                           logit_bias, stop)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -697,16 +760,17 @@ class Router:
                           logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                           top_p: Optional[float] = None, seed: Optional[int] = None,
                           frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-                          logit_bias: Optional[Dict[str, float]] = None, n: Optional[int] = None):
+                          logit_bias: Optional[Dict[str, float]] = None, n: Optional[int] = None, stop: Any = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
         (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
         fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties and logit
-        bias as in completion().  n > 1 is not streamed: BadRequestError."""
+        bias as in completion().  n > 1 is not streamed: BadRequestError.  With `stop`, a token is yielded only once no stop
+        sequence can take it back, and the closing item (a StreamItem) has finish_reason "stop" or "length"."""
         if check_n(n) > 1:
             raise BadRequestError("streaming is not available with `n` > 1: send the request without `stream`")
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                           logit_bias)
+                           logit_bias, stop)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")

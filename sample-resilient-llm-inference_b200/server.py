@@ -16,7 +16,7 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend, check_logprobs, check_n, check_penalties, check_sampling)
+                     StubBackend, check_logprobs, check_n, check_penalties, check_sampling, check_stop)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -60,7 +60,8 @@ def create_app(router: Router):
         def chunk(item):
             label, toks, done = item[:3]
             delta = {} if done else {"role": "assistant", "content": detokenize(toks)}
-            choice = {"index": 0, "delta": delta, "finish_reason": "length" if done else None}
+            choice = {"index": 0, "delta": delta,
+                      "finish_reason": (getattr(item, "finish_reason", None) or "length") if done else None}
             if lp_kw:
                 choice["logprobs"] = None if done else {"content": item[4], "refusal": None}
             return "data: " + _json.dumps({"id": cid, "object": "chat.completion.chunk", "created": int(time.time()),
@@ -97,6 +98,9 @@ def create_app(router: Router):
             samp_kw.update({k: body[k] for k in ("frequency_penalty", "presence_penalty", "logit_bias")
                             if body.get(k) is not None})
             check_penalties(**{k: v for k, v in samp_kw.items() if k not in ("temperature", "top_p", "seed")})
+            if body.get("stop") is not None:
+                check_stop(body["stop"])
+                samp_kw["stop"] = body["stop"]
             if "n" in body:
                 samp_kw["n"] = body["n"]
                 if check_n(body["n"]) > 1 and body.get("stream"):
