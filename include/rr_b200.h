@@ -264,6 +264,25 @@ int rr_op_logit_penalties(float* logits, int ld, int rows, int vocab, const int3
 int rr_op_stop_match(int32_t* hist, int hist_ld, const int32_t* tok, const int32_t* position, const int32_t* row_active,
                      const int32_t* n_stop, const int32_t* gen0, const uint8_t* stop_len, const uint8_t* stop_bytes,
                      int32_t* cut_out, int32_t* hold_out, int rows, void* stream);
+/* JSON mode, as the engine masks and advances a json_object row.  All arrays are device memory.  state is [rows] opaque
+ * 16-byte automaton states (all zero: the initial state, before the top-level '{'); the caller never interprets them.
+ * Token t >= 3 is the byte (t - 3) % 256; tokens 0..2 are never allowed.  The automaton accepts exactly the prefixes of JSON
+ * texts (RFC 8259) whose top-level value is an object, with strict UTF-8 in strings (no overlongs, no surrogates, nothing
+ * above U+10FFFF), no raw bytes < 0x20 in strings, at most 64 open containers ('{' and '[' are not allowed at 64) and runs
+ * of insignificant whitespace of at most 64 bytes; after the closing '}' it allows whitespace only.  No state allows no byte.
+ * Rows with fmt[r] == 0 or (row_active non-NULL and row_active[r] < 0) are skipped by both calls.
+ * mask: writes -inf to every column c < vocab of row r (logits + r * ld) that the row's state (state NULL: the initial
+ *   state) does not allow: c < 3, or byte (c - 3) % 256 not allowed.  It never reads the logits; allowed columns and
+ *   columns >= vocab are not touched.  Grid: one CTA per 8192 columns of a row.
+ * advance: state_out[out_row ? out_row[r] : r] = the state of row r (state_in NULL: the initial state) after tok[r], and
+ *   done[r] = 1 when that state is past the top-level object's closing '}', else 0.  A token the state does not allow
+ *   leaves the state as it was.  Integer work only: two calls agree bit for bit.
+ * RR_INVALID_ARGUMENT before touching the device for a null logits / fmt / tok / state_out / done pointer, rows outside
+ * 1..65535, or (mask) unless 1 <= vocab <= ld, vocab <= 524288 and ld % 4 == 0. */
+int rr_op_json_mask(float* logits, int ld, int rows, int vocab, const int32_t* fmt, const int32_t* row_active,
+                    const void* state, void* stream);
+int rr_op_json_advance(int rows, const int32_t* fmt, const int32_t* row_active, const int32_t* tok, const void* state_in,
+                       void* state_out, const int32_t* out_row, int32_t* done, void* stream);
 int rr_op_decode_attn(const void* q, const void* k_cache, const void* v_cache, void* out,
                       const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                       int n_kv_heads, int ctx_max /* % 64 == 0 */, int n_slots, float scale,
@@ -516,6 +535,19 @@ int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt,
 int rr_engine_wait_stop(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
                         int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out /* [n_choices] */,
                         int32_t* finish_out /* [n_choices] */);
+/* JSON mode (OpenAI `response_format: {"type": "json_object"}`): rr_engine_submit_stop with response_format 1.  Before
+ * every token is picked (after penalties and logit bias, before the argmax, the sampler and logprobs) rr_op_json_mask sets
+ * the logit of every token the JSON grammar does not allow next to -inf, so the reply's bytes are always a prefix of a JSON
+ * text whose top-level value is an object (rr_op_json_mask states the grammar), and logprobs describe the masked
+ * distribution (a masked token's logprob is -inf).  The choice whose token closes the top-level object finishes with reason
+ * 1 (stop), that token included, and frees its decode row at once; a stop-sequence cut on the same token wins, and
+ * max_new_tokens first gives reason 0 (length) and a valid prefix.  Results come back through rr_engine_wait_stop.
+ * response_format 0 is rr_engine_submit_stop.  RR_INVALID_ARGUMENT, before anything is queued, for response_format other
+ * than 0 or 1, 1 on an engine with vocab < 259 (some bytes have no token), and whatever rr_engine_submit_stop rejects. */
+int rr_engine_submit_format(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
+                            int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
+                            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
+                            const uint8_t* stop_bytes, const int32_t* stop_off, int response_format, uint64_t* ticket);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -656,6 +688,15 @@ int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, 
                            uint64_t* ticket);
 int rr_gateway_wait_stop(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
                          int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out);
+/* JSON mode (rr_engine_submit_format): the format is stored with the request and handed to every engine it is admitted to,
+ * a fallback re-admission included.  RR_INVALID_ARGUMENT at submit for response_format 1 when a mock replica is attached
+ * (it has no logits to mask) or the smallest vocabulary is below 259, and for a value other than 0 or 1.  Results come
+ * back through rr_gateway_wait_stop.  response_format 0 is rr_gateway_submit_stop. */
+int rr_gateway_submit_format(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                             int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                             float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                             const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
+                             int response_format, uint64_t* ticket);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

@@ -161,6 +161,8 @@ PROTOTYPES = {
     "rr_op_sample": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "rr_op_logit_penalties": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, vp]),
     "rr_op_stop_match": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp]),
+    "rr_op_json_mask": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]),
+    "rr_op_json_advance": (C.c_int, [C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]),
     "rr_op_decode_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                     C.c_float, C.c_int, vp]),
     "rr_op_prefill_attn": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -203,6 +205,9 @@ PROTOTYPES = {
     "rr_engine_submit_stop": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
                                         C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
                                         C.POINTER(C.c_uint64)]),
+    "rr_engine_submit_format": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                          C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
+                                          C.c_int, C.POINTER(C.c_uint64)]),
     "rr_engine_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p,
                                       c_i32p, c_i32p]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
@@ -238,6 +243,9 @@ PROTOTYPES = {
     "rr_gateway_submit_stop": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
                                          C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
                                          C.POINTER(C.c_uint64)]),
+    "rr_gateway_submit_format": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                           C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int,
+                                           c_u8p, c_i32p, C.c_int, C.POINTER(C.c_uint64)]),
     "rr_gateway_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
                                        c_i32p, c_i32p, c_i32p]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),

@@ -266,6 +266,24 @@ RR_API int rr_op_stop_match(int32_t* hist, int hist_ld, const int32_t* tok, cons
     return check_last();
 }
 
+// JSON mode as the engine runs it in the logits tail (rr_kernels.h, JsonState), on caller buffers.
+RR_API int rr_op_json_mask(float* logits, int ld, int rows, int vocab, const int32_t* fmt, const int32_t* row_active,
+                           const void* state, void* stream) {
+    if (!logits || !fmt) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > 65535 || vocab < 1 || vocab > ld || ld % 4 || vocab > LP_MAX_CHUNKS * LP_CHUNK)
+        return RR_INVALID_ARGUMENT;
+    launch_json_mask(logits, ld, rows, vocab, fmt, row_active, (const JsonState*)state, (cudaStream_t)stream);
+    return check_last();
+}
+
+RR_API int rr_op_json_advance(int rows, const int32_t* fmt, const int32_t* row_active, const int32_t* tok,
+                              const void* state_in, void* state_out, const int32_t* out_row, int32_t* done, void* stream) {
+    if (!fmt || !tok || !state_out || !done || rows < 1 || rows > 65535) return RR_INVALID_ARGUMENT;
+    launch_json_advance(rows, fmt, row_active, tok, (const JsonState*)state_in, (JsonState*)state_out, out_row, done,
+                        (cudaStream_t)stream);
+    return check_last();
+}
+
 RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_cache, void* out,
                              const int32_t* slot, const int32_t* pos, int rows, int n_heads,
                              int n_kv_heads, int ctx_max, int n_slots, float scale, int kv_splits, void* stream) {

@@ -536,7 +536,9 @@ logprobs_chunk_kernel(const float* __restrict__ logits, int ld, int vocab, const
     __syncthreads();
     const float m = block_max(mx, s_rv);
     float s = 0.f;
-    for (int j = threadIdx.x; j < n; j += LP_THREADS) s += expf(s_x[j] - m);
+    // a chunk of -inf columns only (a JSON-mode mask) has m = -inf: it adds s = 0, not expf(-inf - -inf) = NaN
+    if (m != -INFINITY)
+        for (int j = threadIdx.x; j < n; j += LP_THREADS) s += expf(s_x[j] - m);
     s = block_sum(s, s_rv);
     LpPart* out = ws + (size_t)row * gridDim.x + c;
     if (threadIdx.x == 0) { out->m = m; out->s = s; }
@@ -583,7 +585,8 @@ logprobs_merge_kernel(const int32_t* __restrict__ top_n, int max_top, int n_chun
         float m = -INFINITY;
         for (int c = 0; c < n_chunks; ++c) m = fmaxf(m, p[c].m);
         float s = 0.f;
-        for (int c = 0; c < n_chunks; ++c) s += p[c].s * expf(p[c].m - m);
+        for (int c = 0; c < n_chunks; ++c)
+            if (p[c].m != -INFINITY) s += p[c].s * expf(p[c].m - m);      // an all -inf chunk adds nothing
         s_lse = m + logf(s);
         // a sampled token may lie outside the top k: its own pair, from the same value and lse as the ranked entries
         if (tok) tok_lp[row] = logits[(size_t)row * ld + tok[row]] - s_lse;
@@ -802,7 +805,7 @@ sample_chunk_kernel(const float* __restrict__ logits, int ld, int vocab, const f
     int bi = 0x7fffffff;
     for (int j = threadIdx.x; j < n; j += LP_THREADS) {
         const float v = x[j];
-        if (!(v >= t)) continue;
+        if (!(v >= t) || v == -INFINITY) continue;        // with top_p = 1, tau = -inf: a masked column is never drawn
         const int id = c0 + j;
         const float s = v / T + sample_gumbel(philox_first((uint32_t)id, pos, key));
         if (lp_before(s, id, bv, bi)) { bv = s; bi = id; }
@@ -985,6 +988,229 @@ __global__ void __launch_bounds__(32 * STOP_WARPS) stop_match_kernel(StopArgs a,
 void launch_stop_match(const StopArgs& a, int rows, cudaStream_t st) {
     if (rows <= 0) return;
     launch_pdl(stop_match_kernel, dim3((rows + STOP_WARPS - 1) / STOP_WARPS), dim3(32 * STOP_WARPS), 0, st, a, rows);
+}
+
+// ---- JSON mode (rr_op_json_mask / rr_op_json_advance) -------------------------------------------------------------------
+// The automaton both kernels run (tests/json_oracle.py states the same one in Python).  A JsonState holds the node, the
+// depth and a bit per open container (array or object), the whitespace run and, in w1, the progress inside a literal, an
+// escape, a \u escape or a multi-byte UTF-8 character.  All zero is the initial state (JN_START).
+enum JsonNode : uint32_t {
+    JN_START = 0,   // before the top-level value: '{'
+    JN_OBJ_FIRST,   // after '{': a key or '}'
+    JN_OBJ_KEY,     // after ',' in an object: a key
+    JN_COLON,       // after a key: ':'
+    JN_VALUE,       // after ':', or after ',' in an array: a value
+    JN_ARR_FIRST,   // after '[': a value or ']'
+    JN_AFTER,       // after a value in a container: ',' or the container's close
+    JN_STR,         // in a string (w0 bit 24: it is a key)
+    JN_ESC,         // after '\' in a string
+    JN_HEX,         // in \uXXXX: w1 = hex digits still due
+    JN_UTF8,        // in a multi-byte character: w1 = bytes due | lo << 8 | hi << 16, the next byte's range
+    JN_LIT,         // in true / false / null: w1 = literal << 4 | bytes matched
+    JN_MINUS,       // number: after '-'
+    JN_ZERO,        //         after a leading '0'
+    JN_INT,         //         in the integer digits
+    JN_DOT,         //         after '.'
+    JN_FRAC,        //         in the fraction digits
+    JN_EXP,         //         after 'e' / 'E'
+    JN_EXP_SIGN,    //         after the exponent's sign
+    JN_EXP_DIG,     //         in the exponent digits
+    JN_DONE         // the top-level object is closed: only trailing whitespace, which RFC 8259 allows (the choice has ended)
+};
+
+__device__ __forceinline__ bool json_ws(int c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r'; }
+__device__ __forceinline__ bool json_digit(int c) { return c >= '0' && c <= '9'; }
+
+// One byte c: true and *s advanced when the state allows c, else false and *s unchanged.  Integer work only.
+__device__ bool json_step(JsonState* s, int c) {
+    uint64_t stack = s->stack;
+    uint32_t node = s->w0 & 0xff, depth = (s->w0 >> 8) & 0xff, ws = (s->w0 >> 16) & 0xff, key = (s->w0 >> 24) & 1;
+    uint32_t aux = s->w1;
+    bool ok = false, structural = false;
+    switch (node) {
+    case JN_MINUS:
+        if (json_digit(c)) { node = c == '0' ? JN_ZERO : JN_INT; ok = true; }
+        break;
+    case JN_ZERO:           // a byte that does not continue a number ends it and is read as in JN_AFTER
+    case JN_INT:
+        if (node == JN_INT && json_digit(c)) ok = true;
+        else if (c == '.') { node = JN_DOT; ok = true; }
+        else if (c == 'e' || c == 'E') { node = JN_EXP; ok = true; }
+        else { node = JN_AFTER; structural = true; }
+        break;
+    case JN_DOT:
+        if (json_digit(c)) { node = JN_FRAC; ok = true; }
+        break;
+    case JN_FRAC:
+        if (json_digit(c)) ok = true;
+        else if (c == 'e' || c == 'E') { node = JN_EXP; ok = true; }
+        else { node = JN_AFTER; structural = true; }
+        break;
+    case JN_EXP:
+        if (c == '+' || c == '-') { node = JN_EXP_SIGN; ok = true; }
+        else if (json_digit(c)) { node = JN_EXP_DIG; ok = true; }
+        break;
+    case JN_EXP_SIGN:
+        if (json_digit(c)) { node = JN_EXP_DIG; ok = true; }
+        break;
+    case JN_EXP_DIG:
+        if (json_digit(c)) ok = true;
+        else { node = JN_AFTER; structural = true; }
+        break;
+    case JN_STR:
+        if (c == '"') { node = key ? JN_COLON : JN_AFTER; key = 0; ok = true; }
+        else if (c == '\\') { node = JN_ESC; ok = true; }
+        else if (c >= 0x20 && c < 0x80) ok = true;
+        else if (c >= 0xC2 && c <= 0xF4) {   // a lead byte: no overlong (C0, C1, E0 80..9F, F0 80..8F), no surrogate
+            const uint32_t n = c < 0xE0 ? 1 : c < 0xF0 ? 2 : 3;                // (ED A0..BF), nothing above U+10FFFF
+            const uint32_t lo = c == 0xE0 ? 0xA0 : c == 0xF0 ? 0x90 : 0x80;
+            const uint32_t hi = c == 0xED ? 0x9F : c == 0xF4 ? 0x8F : 0xBF;
+            node = JN_UTF8; aux = n | lo << 8 | hi << 16; ok = true;
+        }
+        break;
+    case JN_UTF8:
+        if ((uint32_t)c >= ((aux >> 8) & 0xff) && (uint32_t)c <= (aux >> 16)) {
+            const uint32_t n = (aux & 0xff) - 1;
+            if (n == 0) node = JN_STR;
+            else aux = n | 0x80u << 8 | 0xBFu << 16;
+            ok = true;
+        }
+        break;
+    case JN_ESC:
+        if (c == '"' || c == '\\' || c == '/' || c == 'b' || c == 'f' || c == 'n' || c == 'r' || c == 't') {
+            node = JN_STR; ok = true;
+        } else if (c == 'u') { node = JN_HEX; aux = 4; ok = true; }
+        break;
+    case JN_HEX:
+        if (json_digit(c) || (c >= 'a' && c <= 'f') || (c >= 'A' && c <= 'F')) {
+            if (--aux == 0) node = JN_STR;
+            ok = true;
+        }
+        break;
+    case JN_LIT: {      // "true", "false", "null", little-endian
+        const uint32_t lit = aux >> 4, pos = aux & 15, len = lit == 1 ? 5 : 4;
+        const uint64_t w = lit == 0 ? 0x65757274ull : lit == 1 ? 0x65736c6166ull : 0x6c6c756eull;
+        if ((uint32_t)c == ((w >> (8 * pos)) & 0xff)) {
+            aux = lit << 4 | (pos + 1);
+            if (pos + 1 == len) node = JN_AFTER;
+            ok = true;
+        }
+        break;
+    }
+    case JN_DONE:
+        ok = json_ws(c);
+        break;
+    default:
+        structural = true;
+    }
+    if (structural) {
+        if (json_ws(c)) {
+            if (ws < JSON_MAX_WS) { ++ws; ok = true; }
+        } else {
+            const bool arr = depth > 0 && (stack >> (depth - 1) & 1);
+            int push = -1;                         // 0: open an object, 1: an array
+            bool pop = false;
+            switch (node) {
+            case JN_START:
+                if (c == '{') push = 0;
+                break;
+            case JN_OBJ_FIRST:
+            case JN_OBJ_KEY:
+                if (c == '"') { node = JN_STR; key = 1; ok = true; }
+                else if (c == '}' && node == JN_OBJ_FIRST) pop = true;
+                break;
+            case JN_COLON:
+                if (c == ':') { node = JN_VALUE; ok = true; }
+                break;
+            case JN_AFTER:
+                if (c == ',') { node = arr ? JN_VALUE : JN_OBJ_KEY; ok = true; }
+                else if (c == (arr ? ']' : '}')) pop = true;
+                break;
+            default:            // JN_VALUE, JN_ARR_FIRST: a value
+                if (c == ']' && node == JN_ARR_FIRST) pop = true;
+                else if (c == '{' || c == '[') { if (depth < JSON_MAX_DEPTH) push = c == '['; }
+                else if (c == '"') { node = JN_STR; key = 0; ok = true; }
+                else if (c == '-') { node = JN_MINUS; ok = true; }
+                else if (c == '0') { node = JN_ZERO; ok = true; }
+                else if (json_digit(c)) { node = JN_INT; ok = true; }
+                else if (c == 't' || c == 'f' || c == 'n') { node = JN_LIT; aux = (c == 't' ? 0 : c == 'f' ? 1 : 2) << 4 | 1; ok = true; }
+            }
+            if (push >= 0) {
+                stack = (stack & ~(1ull << depth)) | ((uint64_t)push << depth);
+                ++depth;
+                node = push ? JN_ARR_FIRST : JN_OBJ_FIRST;
+                ok = true;
+            } else if (pop) {
+                --depth;
+                node = depth == 0 ? JN_DONE : JN_AFTER;
+                ok = true;
+            }
+            if (ok) ws = 0;
+        }
+    }
+    if (!ok) return false;
+    if (node != JN_HEX && node != JN_UTF8 && node != JN_LIT) aux = 0;
+    s->stack = stack;
+    s->w0 = node | depth << 8 | ws << 16 | key << 24;
+    s->w1 = aux;
+    return true;
+}
+
+// Mask: LP_CHUNK is a multiple of JSON_THREADS = 256, so the columns of thread j in every chunk all carry the byte
+// (j - 3) mod 256: the thread steps a copy of the state by that one byte and, when it is not allowed, writes -inf to all of
+// its columns (and to columns 0..2, which carry no byte).  No shared memory, and the logits are never read.
+constexpr int JSON_THREADS = 256;
+static_assert(LP_CHUNK % JSON_THREADS == 0, "a chunk's columns repeat the byte pattern");
+
+__global__ void __launch_bounds__(JSON_THREADS)
+json_mask_kernel(float* __restrict__ logits, int ld, int vocab, const int32_t* __restrict__ fmt,
+                 const int32_t* __restrict__ row_active, const JsonState* __restrict__ state) {
+    griddep_launch();
+    griddep_wait();
+    const int row = blockIdx.y;
+    if (fmt[row] == 0 || (row_active && row_active[row] < 0)) return;
+    JsonState s = {0, 0, 0};
+    if (state) s = state[row];
+    const bool allowed = json_step(&s, (threadIdx.x + 253) & 255);
+    const int c0 = blockIdx.x * LP_CHUNK, n = min(LP_CHUNK, vocab - c0);
+    float* x = logits + (size_t)row * ld + c0;
+    if (!allowed) {
+#pragma unroll 4
+        for (int j = threadIdx.x; j < n; j += JSON_THREADS) x[j] = -INFINITY;
+    } else if (c0 == 0 && threadIdx.x < 3 && (int)threadIdx.x < n) {
+        x[threadIdx.x] = -INFINITY;
+    }
+}
+
+__global__ void __launch_bounds__(128)
+json_advance_kernel(int rows, const int32_t* __restrict__ fmt, const int32_t* __restrict__ row_active,
+                    const int32_t* __restrict__ tok, const JsonState* state_in, JsonState* state_out,
+                    const int32_t* __restrict__ out_row, int32_t* __restrict__ done) {
+    griddep_launch();
+    griddep_wait();
+    const int r = blockIdx.x * 128 + threadIdx.x;
+    if (r >= rows || fmt[r] == 0 || (row_active && row_active[r] < 0)) return;
+    JsonState s = {0, 0, 0};
+    if (state_in) s = state_in[r];
+    const int t = tok[r];
+    if (t >= 3) json_step(&s, (t - 3) & 255);
+    state_out[out_row ? out_row[r] : r] = s;
+    done[r] = (s.w0 & 0xff) == JN_DONE ? 1 : 0;
+}
+
+void launch_json_mask(float* logits, int ld, int rows, int vocab, const int32_t* fmt, const int32_t* row_active,
+                      const JsonState* state, cudaStream_t st) {
+    if (rows <= 0) return;
+    launch_pdl(json_mask_kernel, dim3((vocab + LP_CHUNK - 1) / LP_CHUNK, rows), dim3(JSON_THREADS), 0, st, logits, ld,
+               vocab, fmt, row_active, state);
+}
+
+void launch_json_advance(int rows, const int32_t* fmt, const int32_t* row_active, const int32_t* tok,
+                         const JsonState* state_in, JsonState* state_out, const int32_t* out_row, int32_t* done,
+                         cudaStream_t st) {
+    if (rows <= 0) return;
+    launch_pdl(json_advance_kernel, dim3((rows + 127) / 128), dim3(128), 0, st, rows, fmt, row_active, tok, state_in,
+               state_out, out_row, done);
 }
 
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }

@@ -67,8 +67,9 @@ __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const
 
 // One request of n_choices choices.  Choice c decodes in row rows[c] (== its KV slot); the prompt is prefilled once, into
 // rows[0], and its KV copied to the other rows.  The choices are admitted in one chunk and get one token each per step.  A
-// choice finishes when it holds max_new tokens or a stop sequence cuts it, and gives its row back at once; the request
-// finishes with its last choice.  Without stop sequences that is one step for all of them.
+// choice finishes when it holds max_new tokens, a stop sequence cuts it or (JSON mode) its top-level object closes, and
+// gives its row back at once; the request finishes with its last choice.  Without stop sequences or JSON mode that is one
+// step for all of them.
 struct Request {
     uint64_t ticket;
     std::vector<int32_t> prompt;
@@ -114,18 +115,20 @@ constexpr int PREFIX_MIN = 64;
 //   2 pen    frequency_penalty f32[n] | presence_penalty f32[n] | gen0 i32[n] (the position of the first generated token)
 //            | n_bias i32[n] | bias ids i32[n][bias_ld] | bias values f32[n][bias_ld]
 //   3 stop   n_stop i32[n] | gen0 i32[n] | len u8[n][STOP_MAX_SEQS] | bytes u8[n][STOP_MAX_SEQS][STOP_MAX_LEN]
+//   4 json   fmt i32[n] (0 text, 1 json_object)
 // The decode rows use n = Bm and bias_ld = PEN_MAX_BIAS (fixed: the graphs hold it).  A prefill chunk uses n = n_seqs, the
 // largest bias count among its sequences and a position column, in buffers sized for Bm rows and PEN_MAX_BIAS.
 struct ParamBlocks {
-    char* blk[4] = {};            // pen / stop stay null until the first request that uses them (ensure_pen_buffers /
-                                  // ensure_stop_buffers)
+    char* blk[5] = {};            // pen / stop / json stay null until the first request that uses them
+                                  // (ensure_pen_buffers / ensure_stop_buffers / ensure_json_buffers)
     int n = 0, bias_ld = 0;
     bool has_pos = false;
 
     ParamBlocks at(int rows, int ld) const { ParamBlocks p = *this; p.n = rows; p.bias_ld = ld; return p; }
     static constexpr size_t STOP_ROW = 12 + STOP_MAX_SEQS * STOP_MAX_LEN;      // 268 B per row
     size_t bytes(int i) const {
-        return (size_t)n * (i == 0 ? 4 : i == 1 ? (has_pos ? 20 : 16) : i == 2 ? 16 + 8 * (size_t)bias_ld : STOP_ROW);
+        return (size_t)n * (i == 0 || i == 4 ? 4 : i == 1 ? (has_pos ? 20 : 16) : i == 2 ? 16 + 8 * (size_t)bias_ld
+                                                                                          : STOP_ROW);
     }
     int32_t* top_n() const { return (int32_t*)blk[0]; }
     uint64_t* seed() const { return (uint64_t*)blk[1]; }
@@ -142,6 +145,7 @@ struct ParamBlocks {
     int32_t* stop_gen0() const { return (int32_t*)(blk[3] + 4 * (size_t)n); }
     uint8_t* stop_len() const { return (uint8_t*)(blk[3] + 8 * (size_t)n); }
     uint8_t* stop_bytes() const { return (uint8_t*)(blk[3] + 12 * (size_t)n); }
+    int32_t* fmt() const { return (int32_t*)blk[4]; }
 
     PenaltyArgs pen_args() const {
         PenaltyArgs a;
@@ -159,7 +163,7 @@ struct ParamBlocks {
     int row_mode(int i) const {
         return (top_n()[i] >= 0 ? 1 : 0) | (temp()[i] > 0.f ? 2 : 0) |
                (blk[2] && (freq()[i] != 0.f || pres()[i] != 0.f || n_bias()[i] != 0) ? 4 : 0) |
-               (blk[3] && n_stop()[i] != 0 ? 8 : 0);
+               (blk[3] && n_stop()[i] != 0 ? 8 : 0) | (blk[4] && fmt()[i] != 0 ? 16 : 0);
     }
     // Row i from p for its choice `choice`: drawn at `position` (with a position column) with seed p.seed + choice, p's
     // bias, penalties f / pr and p's stop sequences; g0 = the position of the row's first generated token (penalty history
@@ -173,6 +177,7 @@ struct ParamBlocks {
             memcpy(stop_len() + (size_t)i * STOP_MAX_SEQS, p.stop_len, STOP_MAX_SEQS);
             if (p.stops()) memcpy(stop_bytes() + (size_t)i * STOP_MAX_SEQS * STOP_MAX_LEN, p.stop, sizeof(p.stop));
         }
+        if (blk[4]) fmt()[i] = p.fmt;
         if (!blk[2]) return;
         const int nb = (int)p.bias_id.size();
         freq()[i] = f; pres()[i] = pr; gen0()[i] = p.processed() ? g0 : 0; n_bias()[i] = nb;
@@ -183,7 +188,7 @@ struct ParamBlocks {
     }
     // Copies the blocks whose bit is in `mask` from these (pinned) blocks to d, of the same n and bias_ld.
     cudaError_t upload(const ParamBlocks& d, int mask, cudaStream_t s, uint64_t* h2d_bytes) const {
-        for (int i = 0; i < 4; ++i) {
+        for (int i = 0; i < 5; ++i) {
             if (!(mask >> i & 1)) continue;
             const cudaError_t err = cudaMemcpyAsync(d.blk[i], blk[i], bytes(i), cudaMemcpyHostToDevice, s);
             if (err != cudaSuccess) return err;
@@ -195,8 +200,10 @@ struct ParamBlocks {
 
 int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_, uint64_t seed_, float frequency_penalty,
                    float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop_,
-                   const uint8_t* stop_bytes, const int32_t* stop_off) {
+                   const uint8_t* stop_bytes, const int32_t* stop_off, int response_format) {
     if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
+    if (response_format < 0 || response_format > 1 || (response_format == 1 && vocab < JSON_MIN_VOCAB))
+        return RR_INVALID_ARGUMENT;
     if (!(temperature >= 0.f && temperature <= 2.f && top_p_ >= 0.f && top_p_ <= 1.f)) return RR_INVALID_ARGUMENT;
     if (!(frequency_penalty >= -2.f && frequency_penalty <= 2.f && presence_penalty >= -2.f && presence_penalty <= 2.f))
         return RR_INVALID_ARGUMENT;
@@ -223,6 +230,7 @@ int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_,
         stop_len[i] = (uint8_t)(stop_off[i + 1] - stop_off[i]);
         memcpy(stop[i], stop_bytes + stop_off[i], stop_len[i]);
     }
+    fmt = response_format;
     return RR_OK;
 }
 
@@ -275,9 +283,9 @@ struct rr_engine {
     unsigned* mlp_ready = nullptr;    // [n_slices] dependency counters, reset by the norm kernel before each launch
     int mlp_slices = 0, mlp_slice_kb = 0;
     // decode step graphs by step_mode(): bit 0 + launch_logprobs, bit 1 + launch_sample, bit 2 + launch_logit_penalties,
-    // bit 3 + launch_stop_match.  [0] (plain) is captured after the warm-up step, the others on first use: a step without
-    // logprobs, sampled, processed or stop rows replays the plain graph.
-    cudaGraphExec_t graph[16] = {};
+    // bit 3 + launch_stop_match, bit 4 + launch_json_mask / launch_json_advance.  [0] (plain) is captured after the warm-up
+    // step, the others on first use: a step without logprobs, sampled, processed, stop or JSON rows replays the plain graph.
+    cudaGraphExec_t graph[32] = {};
     bool warmed = false;
     // The decode rows' parameter blocks (d_rows) and their pinned host mirror (h_rows), which set_row_params keeps in step
     // with row_req, marking the blocks it changes in rows_dirty (step_mode bits); upload_row_params copies a dirty block
@@ -294,6 +302,10 @@ struct rr_engine {
     // of their buffers (ensure_hist); penalties (ensure_pen_buffers): the count workspace [Bm][vocab] (all zero between
     // launches); stop sequences (ensure_stop_buffers): cut[Bm] | hold[Bm] of rr_op_stop_match and their pinned copy
     int32_t *d_hist = nullptr, *pen_ws = nullptr, *d_stop = nullptr, *h_stop = nullptr;
+    // JSON mode (ensure_json_buffers): each slot's automaton state [Bm], and done[Bm] of rr_op_json_advance with its pinned
+    // copy
+    JsonState* d_json = nullptr;
+    int32_t *d_json_done = nullptr, *h_json_done = nullptr;
 
     // prefill working set
     int Tmax;
@@ -332,7 +344,7 @@ struct rr_engine {
     std::chrono::steady_clock::time_point t0;
 
     rr_engine_stats st;                  // written under gpu_mu (launch / timing counters) or mu (queued, active_rows)
-    uint64_t step_launches[16] = {};              // launches of one decode step, by step_mode()
+    uint64_t step_launches[32] = {};              // launches of one decode step, by step_mode()
     // completion hook (the native gateway, rr_gateway.cu): called on the worker / submitting thread, outside `mu`
     rr::EngineDoneHook hook = nullptr;
     void* hook_ctx = nullptr;
@@ -386,10 +398,12 @@ static PartIn part_bf16(const __nv_bfloat16* p, int ld) {
 static PartIn part_none() { PartIn r; r.ptr = nullptr; r.is_bf16 = 0; r.n_splits = 1; r.split_stride = 0; r.ld = 0; return r; }
 
 // ---------------------------------------------------------------- decode step (enqueue only)
-// The step_mode bits a request needs: 1 logprobs, 2 sampling, 4 penalties / logit bias, 8 stop sequences.  Over a step's
-// rows or a chunk's sequences they pick the parameter blocks to upload, the kernels of the logits tail and the decode graph.
+// The step_mode bits a request needs: 1 logprobs, 2 sampling, 4 penalties / logit bias, 8 stop sequences, 16 JSON mode.
+// Over a step's rows or a chunk's sequences they pick the parameter blocks to upload, the kernels of the logits tail and
+// the decode graph.
 static int step_mode(const GenParams& p) {
-    return (p.logprobs() ? 1 : 0) | (p.sampled() ? 2 : 0) | (p.processed() ? 4 : 0) | (p.stops() ? 8 : 0);
+    return (p.logprobs() ? 1 : 0) | (p.sampled() ? 2 : 0) | (p.processed() ? 4 : 0) | (p.stops() ? 8 : 0) |
+           (p.json() ? 16 : 0);
 }
 
 // Caller holds gpu_mu.  The generated-token history, which the decode graphs of modes 4 and 8 hold: allocated once.
@@ -397,7 +411,7 @@ static int ensure_hist(rr_engine* e) {
     return e->d_hist ? RR_OK : dalloc(e, &e->d_hist, (size_t)e->Bm * e->o.ctx_max, false);
 }
 
-// Caller holds gpu_mu.  Decode rows' and prefill blocks of parameter block i (2 or 3), device and pinned, all zero: the
+// Caller holds gpu_mu.  Decode rows' and prefill blocks of parameter block i (2, 3 or 4), device and pinned, all zero: the
 // defaults of a row that does not use the block.
 static int ensure_block(rr_engine* e, int i) {
     const size_t blk = e->d_rows.bytes(i);            // also the prefill blocks' size: Bm rows (of PEN_MAX_BIAS)
@@ -423,6 +437,18 @@ static int ensure_stop_buffers(rr_engine* e) {
     if (rc != RR_OK) return rc;
     if (!e->h_stop) CK(cudaMallocHost(&e->h_stop, sizeof(int32_t) * 2 * e->Bm));
     return ensure_block(e, 3);
+}
+
+// Caller holds gpu_mu.  The JSON-mode buffers, allocated on the first JSON request: 2 x 4 B x Bm of parameter blocks,
+// 16 B x Bm of automaton state and 4 B x Bm of done flags.  An engine that never sees one allocates nothing.
+static int ensure_json_buffers(rr_engine* e) {
+    if (e->d_rows.blk[4]) return RR_OK;
+    int rc = RR_OK;
+    if (!e->d_json) rc = dalloc(e, &e->d_json, (size_t)e->Bm);
+    if (rc == RR_OK && !e->d_json_done) rc = dalloc(e, &e->d_json_done, (size_t)e->Bm);
+    if (rc != RR_OK) return rc;
+    if (!e->h_json_done) CK(cudaMallocHost(&e->h_json_done, sizeof(int32_t) * e->Bm));
+    return ensure_block(e, 4);
 }
 
 // Caller holds gpu_mu.  The penalty buffers, allocated on the first processed request, so an engine that never sees one
@@ -464,6 +490,11 @@ static int enqueue_o_mlp(rr_engine* e, int l, int rows, cudaStream_t s, uint64_t
 //   mode & 8: stop sequences over the picked token, into d_stop (cut[Bm] | hold[Bm]).  Decode: the token joins history row
 //             r at its position (pos_inc has advanced `position` to it) - gen0.  Prefill (hist null): it is token 0 of the
 //             history of its slot, stop_row[r].
+//   mode & 16: JSON mode.  After penalties and before the argmax, rr_op_json_mask sets the logits the grammar does not
+//             allow next to -inf, so everything after reads the masked logits; last of all rr_op_json_advance steps the
+//             state by the picked token into d_json and writes d_json_done.  Decode: row r's state is d_json[r] (row ==
+//             slot).  Prefill (pos_inc null): every tail row starts from the initial state and leaves its state in its
+//             slot, stop_row[r].
 static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int mode, int32_t* tok,
                              const int32_t* row_active, int32_t* pos_inc, const int32_t* position, int32_t* hist,
                              cudaStream_t s, const int32_t* stop_row = nullptr) {
@@ -474,6 +505,10 @@ static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int m
         if (hist) { a.hist = hist; a.hist_ld = e->o.ctx_max; a.app_tok = tok; a.app_pos = position; }
         launch_logit_penalties(e->logits, V, rows, V, a, e->pen_ws, s); ++nl;
     }
+    // decode (pos_inc set) steps each row's own state; prefill starts every tail row from the initial state.  (hist does not
+    // tell them apart: the history exists only once a penalty or stop request allocated it.)
+    const JsonState* json_in = pos_inc ? e->d_json : nullptr;
+    if (mode & 16) { launch_json_mask(e->logits, V, rows, V, p.fmt(), row_active, json_in, s); ++nl; }
     launch_argmax(part_f32(e->logits, 1, e->Bm, V), rows, V, tok, nullptr, row_active, pos_inc, s); ++nl;
     if (mode & 2) {
         launch_sample(e->logits, V, rows, V, p.temp(), p.top_p(), p.seed(), position, tok, e->sample_ws, s);
@@ -491,15 +526,24 @@ static uint64_t enqueue_tail(rr_engine* e, const ParamBlocks& p, int rows, int m
         a.cut = e->d_stop; a.hold = e->d_stop + e->Bm;
         launch_stop_match(a, rows, s); ++nl;
     }
+    if (mode & 16) {
+        launch_json_advance(rows, p.fmt(), row_active, tok, json_in, e->d_json, pos_inc ? nullptr : stop_row, e->d_json_done,
+                            s);
+        ++nl;
+    }
     return nl;
 }
 
 // Reads a tail's results for `rows` rows back to the host: the tokens (h_tok), with mode & 1 the [rows][LP_MAX_TOP]
-// logprobs and ids (h_lp, h_lp_id), with mode & 3 == 3 the drawn tokens' logprobs (h_tok_lp), and with mode & 8 the stop
-// results (h_stop: cut[Bm] | hold[Bm]).
+// logprobs and ids (h_lp, h_lp_id), with mode & 3 == 3 the drawn tokens' logprobs (h_tok_lp), with mode & 8 the stop
+// results (h_stop: cut[Bm] | hold[Bm]) and with mode & 16 the JSON done flags (h_json_done).
 static int enqueue_readback(rr_engine* e, const int32_t* tok, int rows, int mode, cudaStream_t s) {
     CK(cudaMemcpyAsync(e->h_tok, tok, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
     e->st.d2h_bytes += sizeof(int32_t) * rows;
+    if (mode & 16) {
+        CK(cudaMemcpyAsync(e->h_json_done, e->d_json_done, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += sizeof(int32_t) * rows;
+    }
     if (mode & 8) {
         for (int i = 0; i < 2; ++i)
             CK(cudaMemcpyAsync(e->h_stop + i * e->Bm, e->d_stop + i * e->Bm, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, s));
@@ -649,7 +693,8 @@ struct PrefillTail {
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
 // position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
 // tail (optional): the tail rows and their request parameters.  Stop sequences are matched over the first token (needs
-// ensure_stop_buffers; results in e->h_stop row j).  Only a logit bias applies (penalties count generated
+// ensure_stop_buffers; results in e->h_stop row j).  A JSON-mode row picks its first token from the initial state's mask
+// and leaves its state in its slot (needs ensure_json_buffers; done in e->h_json_done row j).  Only a logit bias applies (penalties count generated
 // tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position
 // pos0 + the sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's
 // logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
@@ -709,6 +754,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     if (max_bias == 0) mode &= ~4;
     else if (!e->d_pf.blk[2]) return RR_INTERNAL;
     if ((mode & 8) && !e->d_pf.blk[3]) return RR_INTERNAL;
+    if ((mode & 16) && !e->d_pf.blk[4]) return RR_INTERNAL;
     const ParamBlocks hp = e->h_pf.at(nt, max_bias), dp = e->d_pf.at(nt, max_bias);
     for (int j = 0; mode && j < nt; ++j) {
         const int q = tail->seq[j];
@@ -862,7 +908,8 @@ static void release_request(rr_engine* e, Request* r, int status, std::vector<Do
 // Caller holds e->mu.  Appends the token read back for row `row` to choice c of r, with its pairs (h_lp / h_lp_id row
 // `row`, and for a sampled request the drawn token's own pair from h_tok_lp) if r asked for logprobs.  With stop sequences
 // it takes the row's cut / hold (h_stop): a hit finishes the choice with reason stop, its tokens and pairs truncated to the
-// cut.  Otherwise max_new tokens finish it with reason length.  True when the choice finished.
+// cut.  Otherwise, in JSON mode, the token that closed the top-level object (h_json_done) finishes it with reason stop, and
+// otherwise max_new tokens finish it with reason length.  True when the choice finished.
 static bool take_token(rr_engine* e, Request* r, int c, int row) {
     r->out[c].push_back(e->h_tok[row]);
     if (r->gen.logprobs()) {
@@ -880,6 +927,8 @@ static bool take_token(rr_engine* e, Request* r, int c, int row) {
         if (r->gen.logprobs()) {
             r->lp[c].resize((size_t)cut * r->gen.lp_width()); r->lp_id[c].resize((size_t)cut * r->gen.lp_width());
         }
+        r->finish[c] = 1;
+    } else if (r->gen.json() && e->h_json_done[row]) {
         r->finish[c] = 1;
     } else if ((int)r->out[c].size() >= r->max_new) {
         r->finish[c] = 0;
@@ -1038,6 +1087,7 @@ static void worker_main(rr_engine* e) {
             tail.choice = tail_choice.data(); tail.gen = tail_gen.data(); tail.mode = chunk_mode;
             int rc = (chunk_mode & 4) ? ensure_pen_buffers(e) : RR_OK;
             if (rc == RR_OK && (chunk_mode & 8)) rc = ensure_stop_buffers(e);
+            if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
                                  e->o.prefix_cache ? pos0.data() : nullptr, copies, &tail);
@@ -1291,6 +1341,7 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
     if (e->h_stop) cudaFreeHost(e->h_stop);
+    if (e->h_json_done) cudaFreeHost(e->h_json_done);
     for (const ParamBlocks* p : {&e->h_rows, &e->h_pf})
         for (char* b : p->blk)
             if (b) cudaFreeHost(b);
@@ -1419,15 +1470,25 @@ int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab
 }
 }  // namespace rr
 
+RR_API int rr_engine_submit_format(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                   int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
+                                   float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
+                                   const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
+                                   int response_format, uint64_t* ticket) {
+    if (!e) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off, response_format);
+    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
+}
+
 RR_API int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
                                  int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
                                  float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
                                  int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off, uint64_t* ticket) {
-    if (!e) return RR_INVALID_ARGUMENT;
-    rr::GenParams p;
-    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off);
-    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
+    return rr_engine_submit_format(e, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature, top_p,
+                                   seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, n_stop, stop_bytes,
+                                   stop_off, 0, ticket);
 }
 
 RR_API int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,

@@ -485,20 +485,31 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
 
 // The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
 // gets RR_INVALID_ARGUMENT.
+RR_API int rr_gateway_submit_format(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
+                                    int max_new_tokens, int n_choices, int top_logprobs, float temperature, float top_p,
+                                    uint64_t seed, float frequency_penalty, float presence_penalty, int n_bias,
+                                    const int32_t* bias_ids, const float* bias_vals, int n_stop, const uint8_t* stop_bytes,
+                                    const int32_t* stop_off, int response_format, uint64_t* ticket) {
+    if (!g) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    // the format is checked against the smallest vocabulary: a fallback re-admission may take the request to any replica
+    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
+                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off, response_format);
+    if (rc != RR_OK) return rc;
+    // a mock replica has no logits to fill the pairs from or to mask, and no decode loop to cut
+    if ((p.logprobs() || p.stops() || p.json()) && g->has_stub) return RR_INVALID_ARGUMENT;
+    const int32_t start[2] = {0, n_prompt};
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
+}
+
 RR_API int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                                   int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
                                   float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
                                   const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
                                   uint64_t* ticket) {
-    if (!g) return RR_INVALID_ARGUMENT;
-    rr::GenParams p;
-    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off);
-    if (rc != RR_OK) return rc;
-    // a mock replica has no logits to fill the pairs from and no decode loop to cut
-    if ((p.logprobs() || p.stops()) && g->has_stub) return RR_INVALID_ARGUMENT;
-    const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
+    return rr_gateway_submit_format(g, group, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature,
+                                    top_p, seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, n_stop,
+                                    stop_bytes, stop_off, 0, ticket);
 }
 
 RR_API int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,

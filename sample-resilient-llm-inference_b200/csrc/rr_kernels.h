@@ -94,17 +94,20 @@ struct GenParams {
     uint8_t stop_len[4] = {};
     uint8_t stop[4][64] = {};
     bool stops() const { return n_stop > 0; }
+    // response format: 0 text, 1 json_object (every token is masked to the JSON grammar, rr_op_json_mask)
+    int fmt = 0;
+    bool json() const { return fmt == 1; }
     // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
     int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
     // The raw C arguments, checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and OpenAI's ranges
     // 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null arrays when
     // n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails; 0 <= n_stop <= STOP_MAX_SEQS
     // sequences of 1..STOP_MAX_LEN bytes each, sequence i = stop_bytes[stop_off[i] .. stop_off[i + 1]) (non-null arrays when
-    // n_stop > 0).  A greedy request keeps the default top_p and seed, an unprocessed one the default penalties.
-    // RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
+    // n_stop > 0); response_format 0 or 1, and 1 only with vocab >= JSON_MIN_VOCAB.  A greedy request keeps the default
+    // top_p and seed, an unprocessed one the default penalties.  RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
     int set(int vocab, int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
             float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
-            const uint8_t* stop_bytes, const int32_t* stop_off);
+            const uint8_t* stop_bytes, const int32_t* stop_off, int response_format = 0);
 };
 // n_choices (1..max_batch): choices of the request (rr_engine_submit_choices); the done hook's n_generated is the total of
 // the tokens the choices return (a choice cut by a stop sequence counts what is left of it).
@@ -266,6 +269,31 @@ struct StopArgs {
     int32_t *cut, *hold;
 };
 void launch_stop_match(const StopArgs& a, int rows, cudaStream_t st);
+// JSON mode (response_format json_object, rr_op_json_mask / rr_op_json_advance).  Each row has an opaque 16-byte state of
+// a byte-level automaton for a JSON text whose top-level value is an object (RFC 8259, strict UTF-8 in strings, at most
+// JSON_MAX_DEPTH open containers, whitespace runs of at most JSON_MAX_WS bytes); all zero is the initial state.  Token
+// t >= 3 is the byte (t - 3) % 256; tokens 0..2 are never allowed.  Rows with fmt[r] == 0 or row_active[r] < 0
+// (row_active optional) are skipped by both kernels.
+//   mask:    one CTA per (LP_CHUNK columns, row): tests each byte against state[r] (null: the initial state) and writes
+//            -inf to every disallowed column of the chunk; it never reads the logits.
+//   advance: one thread per row: next = step(state[r] (null: initial), byte of tok[r]) into state_out[out_row ? out_row[r]
+//            : r], and done[r] = 1 when the new state is past the top-level object's close, else 0.  A token the state
+//            does not allow leaves it unchanged.
+constexpr int JSON_MAX_DEPTH = 64;
+constexpr int JSON_MAX_WS = 64;
+constexpr int JSON_MIN_VOCAB = 259;   // every byte has a token
+struct JsonState {
+    uint64_t stack;                   // bit l: container at level l is an array (1) or an object (0)
+    uint32_t w0;                      // node | depth << 8 | whitespace run << 16 | string-is-a-key << 24
+    uint32_t w1;                      // literal / escape / \u-hex / UTF-8 progress of the node
+};
+static_assert(sizeof(JsonState) == 16, "JsonState is 16 bytes");
+constexpr int JSON_LAUNCHES = 2;
+void launch_json_mask(float* logits, int ld, int rows, int vocab, const int32_t* fmt, const int32_t* row_active,
+                      const JsonState* state, cudaStream_t st);
+void launch_json_advance(int rows, const int32_t* fmt, const int32_t* row_active, const int32_t* tok,
+                         const JsonState* state_in, JsonState* state_out, const int32_t* out_row, int32_t* done,
+                         cudaStream_t st);
 
 // ---- attention (rr_attn_decode.cu, rr_attn_tc.cu) ---------------------------------------------------
 struct DecodeAttnArgs {

@@ -15,7 +15,7 @@ import torch
 
 from . import _lib
 from .models import ModelSpec, Weights, make_weights
-from .router import FINISH_REASONS, check_stop, gen_args, logprob_pairs
+from .router import FINISH_REASONS, check_response_format, check_stop, gen_args, logprob_pairs
 
 
 @dataclass
@@ -109,7 +109,7 @@ class Engine:
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
         self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1 or with stop
-        self._stop: set = set()             # tickets of the requests submitted with stop
+        self._stop: set = set()             # tickets of the requests submitted with stop or JSON mode
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -156,7 +156,7 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
                temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None,
                frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-               logit_bias: Optional[Dict[int, float]] = None, n: int = 1, stop=None) -> int:
+               logit_bias: Optional[Dict[int, float]] = None, n: int = 1, stop=None, response_format=None) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
@@ -167,14 +167,22 @@ class Engine:
         seed + i.  wait() returns them all; peek() is for n = 1 only.
         stop: a string or up to 4 strings (or bytes) of 1..64 bytes each: a choice ends where its reply text (the bytes of
         its tokens) would contain one, returns the tokens before the match and frees its decode row at once
-        (rr_engine_submit_stop).  The tokens are a prefix of the same request's without `stop`."""
+        (rr_engine_submit_stop).  The tokens are a prefix of the same request's without `stop`.
+        response_format {"type": "json_object"}: JSON mode (rr_engine_submit_format): every token is picked from the
+        logits masked to the JSON grammar, and a choice ends with finish reason "stop" on the token that closes its
+        top-level object.  None and {"type": "text"} change nothing (check_response_format)."""
         ids = _i32(prompt_ids)
         bias = logit_bias or {}
         stops = stop if isinstance(stop, (list, tuple)) and all(isinstance(b, bytes) for b in stop) else check_stop(stop)
         gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
-                       list(bias.values()), stop=stops)
+                       list(bias.values()), stop=stops, json_object=check_response_format(response_format))
         t = C.c_uint64()
-        if gen.stop:
+        if gen.fmt:
+            _lib.check(_lib.lib.rr_engine_submit_format(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail,
+                                                        *gen.format_args(), C.byref(t)), "rr_engine_submit_format")
+            self._n[t.value] = n
+            self._stop.add(t.value)
+        elif gen.stop:
             _lib.check(_lib.lib.rr_engine_submit_stop(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail, *gen.stop,
                                                       C.byref(t)), "rr_engine_submit_stop")
             self._n[t.value] = n

@@ -252,6 +252,7 @@ def check_n(n: Any) -> int:
 MAX_STOP = 4                 # OpenAI's limit on the number of `stop` sequences (STOP_MAX_SEQS of the engine)
 MAX_STOP_BYTES = 64          # this project's cap on one stop sequence, in bytes of UTF-8 (STOP_MAX_LEN of the engine)
 FINISH_REASONS = ("length", "stop")      # by the native finish code (rr_engine_wait_stop)
+JSON_MIN_VOCAB = 259         # JSON mode needs a token for every byte (3 + 256; JSON_MIN_VOCAB of the engine)
 
 
 def check_stop(stop: Any) -> List[bytes]:
@@ -274,12 +275,37 @@ def check_stop(stop: Any) -> List[bytes]:
     return out
 
 
+def check_response_format(value: Any) -> bool:
+    """OpenAI's `response_format` request field -> True for JSON mode ({"type": "json_object"}), False for None and
+    {"type": "text"}.  Raises BadRequestError (HTTP 400) for `json_schema`, which is not supported, and anything else."""
+    if value is None:
+        return False
+    typ = value.get("type") if isinstance(value, dict) else None
+    if typ == "text":
+        return False
+    if typ == "json_object":
+        return True
+    if typ == "json_schema":
+        raise BadRequestError("`response_format` type `json_schema` is not supported: use {\"type\": \"json_object\"}")
+    raise BadRequestError("`response_format` must be {\"type\": \"text\"} or {\"type\": \"json_object\"}")
+
+
 class GenArgs(NamedTuple):
     """A request's generation parameters in the form the native submit calls take them (gen_args)."""
     top: Optional[int]     # top_logprobs; None: no logprobs
     tail: tuple            # rr_engine_submit_processed / rr_gateway_submit_processed: top_logprobs .. bias_vals
     width: int             # (logprob, id) pairs per generated token; 0 without logprobs
     stop: tuple = ()       # with stop sequences, what rr_*_submit_stop takes after the tail: n_stop, stop_bytes, stop_off
+    fmt: int = 0           # response format of rr_*_submit_format: 0 text, 1 json_object
+
+    @property
+    def ends_early(self) -> bool:
+        """The choices end on their own (stop sequences, JSON mode): results come back through rr_*_wait_stop."""
+        return bool(self.stop) or self.fmt != 0
+
+    def format_args(self) -> tuple:
+        """What rr_*_submit_format takes after the tail: n_stop, stop_bytes, stop_off, response_format."""
+        return (self.stop or (0, None, None)) + (self.fmt,)
 
 
 class StreamItem(tuple):
@@ -290,11 +316,12 @@ class StreamItem(tuple):
 def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
              seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
              presence_penalty: Optional[float] = None, bias_ids: Sequence[int] = (),
-             bias_vals: Sequence[float] = (), stop: Sequence[bytes] = ()) -> GenArgs:
+             bias_vals: Sequence[float] = (), stop: Sequence[bytes] = (), json_object: bool = False) -> GenArgs:
     """None and absent fields take the defaults of a plain greedy request.  A sampled request (temperature > 0) without
     a seed gets a random one here, once, so that a fallback re-admission draws the same tokens; the seed is taken modulo
     2^64.  Without bias entries the bias arrays are null pointers.  `stop`: the stop sequences as bytes (check_stop).
-    Ranges are checked by the native call (check_* raise HTTP 400 first on the router's path)."""
+    json_object: JSON mode (check_response_format).  Ranges are checked by the native call (check_* raise HTTP 400 first
+    on the router's path)."""
     k = -1 if top_logprobs is None else int(top_logprobs)
     temp = float(temperature or 0.0)
     seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temp else 0
@@ -310,7 +337,8 @@ def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = 
         off = np.zeros(len(stop) + 1, dtype=np.int32)
         np.cumsum([len(b) for b in stop], out=off[1:])
         st = (len(stop), blob.ctypes.data_as(C.POINTER(C.c_uint8)), off.ctypes.data_as(C.POINTER(C.c_int32)))
-    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0, st)
+    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0, st,
+                   1 if json_object else 0)
 
 
 def _token_entry(tok: int, logprob: float) -> dict:
@@ -320,12 +348,13 @@ def _token_entry(tok: int, logprob: float) -> dict:
 
 def logprobs_content(tokens: Sequence[int], pairs: Sequence[Sequence[Tuple[int, float]]], top: int) -> List[dict]:
     """`choices[0].logprobs.content` for the generated tokens: pairs[i] = the engine's (id, logprob) list of token i, best
-    first (a sampled request adds the token's own pair after them); `top` alternatives each."""
+    first (a sampled request adds the token's own pair after them); `top` alternatives each.  Alternatives of logprob -inf
+    (tokens JSON mode masked out, when fewer than `top` are allowed) are left out: JSON cannot encode -inf."""
     out = []
     for tok, p in zip(tokens, pairs):
         lp = next((v for i, v in p if i == tok), p[0][1])
         e = _token_entry(int(tok), lp)
-        e["top_logprobs"] = [_token_entry(i, v) for i, v in p[:top]]
+        e["top_logprobs"] = [_token_entry(i, v) for i, v in p[:top] if v != -math.inf]
         out.append(e)
     return out
 
@@ -522,14 +551,17 @@ class Router:
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
     def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs, n: int = 1) -> int:
-        """With stop sequences: rr_gateway_submit_stop; else n > 1: rr_gateway_submit_choices and a request of one choice
-        rr_gateway_submit_processed."""
+        """In JSON mode: rr_gateway_submit_format; else with stop sequences: rr_gateway_submit_stop; else n > 1:
+        rr_gateway_submit_choices and a request of one choice rr_gateway_submit_processed."""
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
         p = ids.ctypes.data_as(C.POINTER(C.c_int32))
-        if gen.stop:
+        if gen.fmt:
+            rc = _lib.lib.rr_gateway_submit_format(gw, g, p, len(ids), max_new, n, *gen.tail, *gen.format_args(),
+                                                   C.byref(t))
+        elif gen.stop:
             rc = _lib.lib.rr_gateway_submit_stop(gw, g, p, len(ids), max_new, n, *gen.tail, *gen.stop, C.byref(t))
         elif n > 1:
             rc = _lib.lib.rr_gateway_submit_choices(gw, g, p, len(ids), max_new, n, *gen.tail, C.byref(t))
@@ -558,7 +590,7 @@ class Router:
         toks = np.zeros(max_new if n == 1 else (n, max_new), dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new, n)
         n_tok = fin = None
-        if gen.stop:                     # the choices end on their own: each has its token count and finish reason
+        if gen.ends_early:               # the choices end on their own: each has its token count and finish reason
             n_tok, fin = (C.c_int32 * n)(), (C.c_int32 * n)()
             rc = _lib.lib.rr_gateway_wait_stop(gw, ticket, float(timeout or 0.0), C.byref(res),
                                                toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p, n_tok, fin)
@@ -708,26 +740,34 @@ class Router:
         return min((b.vocab for b in self.backends.values()), default=128256)
 
     def _params(self, logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                logit_bias, stop=None) -> GenArgs:
-        """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs and a decode
-        loop that stop sequences can end; bias ids must be valid on every replica the request may fall back to."""
+                logit_bias, stop=None, response_format=None) -> GenArgs:
+        """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs and to mask
+        for JSON mode, and a decode loop that stop sequences can end; bias ids must be valid on every replica the request
+        may fall back to, and JSON mode needs a token for every byte there."""
         top = check_logprobs(logprobs, top_logprobs)
         stops = check_stop(stop)
+        json_object = check_response_format(response_format)
         mock = any(isinstance(b, StubBackend) for b in self.backends.values())
         if stops and mock:
             raise BadRequestError("`stop` is not available: the backends of this router are not model replicas")
         if top is not None and mock:
             raise BadRequestError("`logprobs` is not available: the backends of this router are not model replicas")
+        if json_object and mock:
+            raise BadRequestError("`response_format` json_object is not available: the backends of this router are not "
+                                  "model replicas")
+        if json_object and self._vocab() < JSON_MIN_VOCAB:
+            raise BadRequestError(f"`response_format` json_object needs a vocabulary of at least {JSON_MIN_VOCAB} tokens")
         samp = check_sampling(temperature, top_p, seed) or (None, None, None)
         pen = check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab()) or (None, None, (), ())
-        return gen_args(top, *samp, *pen, stop=stops)
+        return gen_args(top, *samp, *pen, stop=stops, json_object=json_object)
 
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
                    logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                    top_p: Optional[float] = None, seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
                    presence_penalty: Optional[float] = None, logit_bias: Optional[Dict[str, float]] = None,
-                   n: Optional[int] = None, stop: Any = None, **_ignored) -> ModelResponse:
+                   n: Optional[int] = None, stop: Any = None, response_format: Any = None,
+                   **_ignored) -> ModelResponse:
         """logprobs=True: `choices[0].logprobs` carries the logprob of every generated token and its `top_logprobs`
         (0..20) most likely alternatives, as the OpenAI API returns them.  temperature > 0: every token is drawn from
         the top_p nucleus of softmax(logits / temperature) with the request's seed (rr_op_sample); absent or 0 is
@@ -741,10 +781,14 @@ class Router:
         stop: a string or up to 4 strings of 1..64 bytes of UTF-8 each.  A choice ends where its reply would contain one
         of them: the content stops before it and finish_reason is "stop" (rr_gateway_submit_stop).  They are matched on
         the reply's bytes, so the tokens are a prefix of the same request's without `stop`; each choice ends on its own
-        and usage.completion_tokens counts the tokens returned."""
+        and usage.completion_tokens counts the tokens returned.
+        response_format {"type": "json_object"}: JSON mode (rr_gateway_submit_format).  Every token is picked from the
+        logits masked to the JSON grammar, so each choice's content is a prefix of a JSON object; the choice whose object
+        closes ends there with finish_reason "stop", one that reaches max_tokens first with "length".  {"type": "text"}
+        and None change nothing; `json_schema` and anything else raise BadRequestError (check_response_format)."""
         n = check_n(n)
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                           logit_bias, stop)
+                           logit_bias, stop, response_format)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -760,17 +804,19 @@ class Router:
                           logprobs: bool = False, top_logprobs: Optional[int] = None, temperature: Optional[float] = None,
                           top_p: Optional[float] = None, seed: Optional[int] = None,
                           frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-                          logit_bias: Optional[Dict[str, float]] = None, n: Optional[int] = None, stop: Any = None):
+                          logit_bias: Optional[Dict[str, float]] = None, n: Optional[int] = None, stop: Any = None,
+                          response_format: Any = None):
         """Streaming variant (SSE in server.py): admission exactly like completion(); yields
         (model_label, new_token_ids, done, ttft_s) as tokens arrive, with logprobs=True a fifth element: the OpenAI
         `logprobs.content` entries of those tokens.  A backend failure before the first token walks the
-        fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties and logit
-        bias as in completion().  n > 1 is not streamed: BadRequestError.  With `stop`, a token is yielded only once no stop
-        sequence can take it back, and the closing item (a StreamItem) has finish_reason "stop" or "length"."""
+        fallback chain; rate limiting raises RateLimitError before anything is yielded.  Sampling, penalties, logit
+        bias and response_format as in completion().  n > 1 is not streamed: BadRequestError.  With `stop`, a token is
+        yielded only once no stop sequence can take it back; the closing item (a StreamItem) has finish_reason "stop" or
+        "length"."""
         if check_n(n) > 1:
             raise BadRequestError("streaming is not available with `n` > 1: send the request without `stream`")
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                           logit_bias, stop)
+                           logit_bias, stop, response_format)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")

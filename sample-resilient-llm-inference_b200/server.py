@@ -16,7 +16,8 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend, check_logprobs, check_n, check_penalties, check_sampling, check_stop)
+                     StubBackend, check_logprobs, check_n, check_penalties, check_response_format, check_sampling,
+                     check_stop)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -101,6 +102,8 @@ def create_app(router: Router):
             if body.get("stop") is not None:
                 check_stop(body["stop"])
                 samp_kw["stop"] = body["stop"]
+            if body.get("response_format") is not None and check_response_format(body["response_format"]):
+                samp_kw["response_format"] = body["response_format"]      # {"type": "text"} is the default: not passed
             if "n" in body:
                 samp_kw["n"] = body["n"]
                 if check_n(body["n"]) > 1 and body.get("stream"):
