@@ -444,110 +444,98 @@ typedef struct rr_completion {
     double t_submit_s, t_first_token_s, t_done_s;   /* engine monotonic clock */
 } rr_completion;
 
-int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+/* Generation parameters of one request: the fields of chat.completions.create that steer decoding.  rr_engine_submit
+ * states what each does; the field comments give the encodings.  A NULL rr_gen_params* is a plain greedy request of one
+ * choice.  A non-NULL struct is read in full: zero is a value, never "use the default". */
+typedef struct rr_gen_params {
+    int32_t n_choices;                   /* 1..max_batch (OpenAI n) */
+    int32_t top_logprobs;                /* -1: off; 0..20 */
+    float temperature, top_p;            /* temperature 0: greedy (top_p and seed unused) */
+    uint64_t seed;
+    float frequency_penalty, presence_penalty;
+    int32_t n_bias, n_stop;
+    const int32_t* bias_ids;  const float* bias_vals;      /* [n_bias] */
+    const uint8_t* stop_bytes; const int32_t* stop_off;    /* sequence i = stop_bytes[stop_off[i] .. stop_off[i+1]) */
+    int32_t response_format;             /* 0 text, 1 json_object */
+    int32_t reserved;                    /* pass 0 */
+} rr_gen_params;                         /* 80 bytes; the offsets are pinned by tests/test_abi.py */
+
+/* Queue one request and write its ticket to *ticket; finish it with rr_engine_wait or rr_engine_cancel.  p = NULL is a
+ * greedy request of one choice.  The tokens depend only on the prompt, the weights and p: not on the batch, the slot, the
+ * prefix cache or the replica.
+ * - top_logprobs (OpenAI `logprobs` / `top_logprobs`) 0..20: for every generated token the engine records K =
+ *   max(1, top_logprobs) (logprob, token id) pairs, the K most likely tokens of that step ordered by logprob descending then
+ *   id ascending (pair 0 is the greedy token), computed on the GPU from the same fp32 logits the pick reads
+ *   (rr_op_logprobs).  With temperature > 0 a token has K + 1 pairs, the last being (the generated token's logprob, its
+ *   id).  Logprobs change no token.
+ * - temperature > 0 (seeded sampling, OpenAI `temperature` / `top_p` / `seed`): every token is drawn by rr_op_sample with
+ *   (temperature, top_p, seed) at its own position (n_prompt for the first generated token, n_prompt + j for the j-th after
+ *   it).  temperature = 0 is greedy.
+ * - frequency_penalty / presence_penalty / logit bias (bias_ids[i] gets bias_vals[i]): before every token is picked
+ *   (argmax, or the draw), its logits go through rr_op_logit_penalties with the tokens the choice generated so far as the
+ *   history (prompt tokens do not count, so the first token gets the bias only).  Logprobs describe the processed logits.
+ *   Penalties 0 and n_bias = 0 change nothing.
+ * - n_choices (OpenAI `n`): completions of the same prompt.  The prompt is prefilled once; its KV is then copied into
+ *   n_choices - 1 further KV slots, and every choice decodes in a row of its own.  Choice i is exactly what the request of
+ *   one choice gives with seed (seed + i) mod 2^64 and the same other parameters (greedy: every choice is the greedy
+ *   completion); penalties count the choice's own tokens.  The choices run in lockstep: they are admitted together (a
+ *   request waits at the head of the queue until n_choices rows are free; nothing overtakes it) and get one token each per
+ *   step.  Without stop sequences or JSON mode they end together.  Cancellation, an injected failure or an internal error
+ *   ends every choice.
+ * - stop sequences (OpenAI `stop`): n_stop sequences, sequence i = stop_bytes[stop_off[i] .. stop_off[i + 1]).  They are
+ *   matched on the reply text (a generated token t >= 3 is the byte (t - 3) % 256, a token < 3 is no text) by
+ *   rr_op_stop_match after every generated token, the first included.  A choice whose text comes to end in a sequence
+ *   finishes with reason 1 (stop): it returns the tokens before the first token of the match (of the longest sequence when
+ *   several end there), its logprob pairs likewise, and its decode row is free from the next step on, while the request's
+ *   other choices go on.  Stop sequences change no logit and no draw: the tokens returned are a prefix of those of the
+ *   same request without them.
+ * - response_format 1 (JSON mode, OpenAI `response_format: {"type": "json_object"}`): before every token is picked (after
+ *   penalties and logit bias, before the argmax, the sampler and logprobs) rr_op_json_mask sets the logit of every token
+ *   the JSON grammar does not allow next to -inf, so the reply's bytes are always a prefix of a JSON text whose top-level
+ *   value is an object (rr_op_json_mask states the grammar), and logprobs describe the masked distribution (a masked
+ *   token's logprob is -inf).  The choice whose token closes the top-level object finishes with reason 1 (stop), that token
+ *   included, and frees its decode row at once; a stop-sequence cut on the same token wins.
+ * A choice that reaches max_new_tokens first finishes with reason 0 (length), in JSON mode with a valid prefix.  The
+ * request is done when every choice has finished.
+ * RR_INVALID_ARGUMENT, before anything is queued and with *ticket untouched, for a NULL engine, prompt or ticket,
+ * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max, a prompt longer than a prefill chunk, a
+ * prompt token outside [0, vocab), and for parameters outside these ranges (NaN is outside every range):
+ * 1 <= n_choices <= max_batch; -1 <= top_logprobs <= 20; 0 <= temperature <= 2; 0 <= top_p <= 1; -2 <= penalties <= 2;
+ * 0 <= n_bias <= 300 with non-null arrays when n_bias > 0, unique bias ids in [0, vocab) and -100 <= bias values <= 100;
+ * 0 <= n_stop <= 4 sequences of 1..64 bytes with non-null arrays when n_stop > 0; response_format 0 or 1, and 1 only with
+ * vocab >= 259 (some bytes have no token otherwise).  top_logprobs >= 0 and temperature > 0 need a vocabulary that is a
+ * multiple of 4.
+ * Stats: prefill_tokens counts the prompt once, kv_copy_tokens grows by (n_choices - 1) x the prompt length,
+ * generated_tokens counts every token produced, the ones a stop sequence cut included. */
+int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, const rr_gen_params* p,
                      uint64_t* ticket);
-int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
-                   int32_t* tokens_out, int max_tokens_out);
+/* Block (release the GIL) until the request is done, or timeout_s (<= 0: no limit) elapses.  RR_TIMEOUT: still in flight
+ * (out->status = RR_TIMEOUT), wait again or rr_engine_cancel.  Otherwise the ticket is consumed and the request's status
+ * returned (RR_OK / RR_BACKEND_FAILED / ...), with `out` filled and for every choice c of its n_choices:
+ *   n_tokens_out[c] = the tokens choice c returned, finish_out[c] = its finish reason (0 length, 1 stop);
+ *   row c of tokens_out [n_choices][max_tokens_out] = its first min(n_tokens_out[c], max_tokens_out) tokens;
+ *   with top_logprobs >= 0, row c of lp_out / id_out [n_choices][max_tokens_out][K] = their pairs (K as rr_engine_submit
+ *   describes); nothing is written there for a request without logprobs.
+ * tokens_out, lp_out, id_out, n_tokens_out and finish_out may each be NULL.  rr_completion.n_generated is the longest
+ * choice's count.  RR_INVALID_ARGUMENT for a NULL engine or out, and for an unknown, consumed or cancelled ticket. */
+int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                   int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out /* [n_choices] */,
+                   int32_t* finish_out /* [n_choices] */);
 /* Abandon a request: queued -> dropped; running -> its decode row is freed at the next step; finished -> freed.
  * Consumes the ticket (do not wait on it afterwards).  Replaces the client-side `timeout=` of the reference's
  * chat.completions.create calls (reference src/demo_fallback.py:146) as seen from the backend. */
 int rr_engine_cancel(rr_engine* e, uint64_t ticket);
-/* Streaming (SSE): block until the request holds more than `have` tokens, is done, or `timeout_s` elapses;
- * copies the tokens generated so far.  Does not consume the request — finish with rr_engine_wait. */
-int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                   int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s);
-/* Per-token log-probabilities (OpenAI `logprobs` / `top_logprobs`).  top_logprobs = -1: off (rr_engine_submit);
- * 0..20: for every generated token the engine records K = max(1, top_logprobs) (logprob, token id) pairs, the K most
- * likely tokens of that step ordered by logprob descending then id ascending (pair 0 is the greedy token), computed on
- * the GPU from the same fp32 logits the greedy pick reads (rr_op_logprobs).  Tokens are the same as without logprobs.
- * RR_INVALID_ARGUMENT for top_logprobs outside -1..20 (or >= 0 with a vocabulary that is not a multiple of 4).
- * wait / peek behave like rr_engine_wait / rr_engine_peek and also fill lp_out / id_out [max_tokens_out][K] (either may be
- * NULL; nothing is written for a request submitted with top_logprobs = -1). */
-int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                              int top_logprobs, uint64_t* ticket);
-int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                            int max_tokens_out, float* lp_out, int32_t* id_out);
-int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                            int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
-                            float* lp_out, int32_t* id_out);
-/* Seeded sampling (OpenAI `temperature` / `top_p` / `seed`): every token of the request is drawn by rr_op_sample with
- * these parameters at its own position (n_prompt for the first generated token, n_prompt + j for the j-th after it), so
- * the tokens depend only on the prompt, the weights and (temperature, top_p, seed): not on the batch, the slot, the prefix
- * cache or the replica.  temperature = 0 is greedy, exactly as rr_engine_submit_logprobs.  top_logprobs as in
- * rr_engine_submit_logprobs; for a request with temperature > 0 and top_logprobs >= 0 the pair buffers of
- * rr_engine_wait_logprobs / rr_engine_peek_logprobs are [max_tokens_out][max(1, top_logprobs) + 1], the last column
- * being (the generated token's logprob, its id).  RR_INVALID_ARGUMENT unless 0 <= temperature <= 2 and
- * 0 <= top_p <= 1. */
-int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int top_logprobs,
-                             float temperature, float top_p, uint64_t seed, uint64_t* ticket);
-/* Penalties and logit bias (OpenAI `frequency_penalty` / `presence_penalty` / `logit_bias`) on top of
- * rr_engine_submit_sampled: before every token of the request is picked (argmax, or the draw with temperature > 0), its
- * logits go through rr_op_logit_penalties with the tokens the request generated so far as the history (prompt tokens do
- * not count, so the first token gets the bias only).  Logprobs describe the processed logits.  Tokens depend only on the
- * prompt, the weights and the parameters.  Penalties 0 and n_bias = 0 behave exactly as rr_engine_submit_sampled.
- * RR_INVALID_ARGUMENT unless rr_engine_submit_sampled's ranges hold, -2 <= penalties <= 2, 0 <= n_bias <= 300, the
- * bias ids are unique and in [0, vocab) and -100 <= bias values <= 100. */
-int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int top_logprobs,
-                               float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                               float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
-                               uint64_t* ticket);
-/* Several choices per request (OpenAI `n`): rr_engine_submit_processed with n_choices (1..max_batch) completions of the same
- * prompt.  The prompt is prefilled once; its KV is then copied into n_choices - 1 further KV slots, and every choice decodes
- * in a row of its own.  Choice i is exactly what rr_engine_submit_processed gives with seed (seed + i) mod 2^64 and the same
- * other parameters (greedy: every choice is the greedy completion); penalties count the choice's own tokens.  The choices
- * run in lockstep: they are admitted together (a request waits at the head of the queue until n_choices rows are free;
- * nothing overtakes it), get one token each per step and, without stop sequences (rr_engine_submit_stop), end together,
- * so rr_completion.n_generated counts the tokens of each choice.  Cancellation, an injected failure or an internal error ends every choice.  n_choices = 1 is
- * rr_engine_submit_processed.  RR_INVALID_ARGUMENT, before anything is queued, for n_choices outside 1..max_batch and
- * whatever rr_engine_submit_processed rejects.
- * wait_choices: rr_engine_wait_logprobs for any n_choices, with tokens_out [n_choices][max_tokens_out] and lp_out / id_out
- * [n_choices][max_tokens_out][K] (K as rr_engine_submit_sampled describes).  rr_engine_wait / _wait_logprobs / _peek /
- * _peek_logprobs return RR_INVALID_ARGUMENT for a request of n_choices > 1 (it stays in flight).
- * Stats: prefill_tokens counts the prompt once, kv_copy_tokens grows by (n_choices - 1) x the prompt length,
- * generated_tokens counts every choice's tokens. */
-int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
-                             int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                             float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
-                             uint64_t* ticket);
-int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                           int max_tokens_out, float* lp_out, int32_t* id_out);
-/* Stop sequences (OpenAI `stop`): rr_engine_submit_choices with n_stop (0..4) sequences of 1..64 bytes each, sequence i =
- * stop_bytes[stop_off[i] .. stop_off[i + 1]).  They are matched on the reply text (a generated token t >= 3 is the byte
- * (t - 3) % 256, a token < 3 is no text) by rr_op_stop_match after every generated token, the first included.  A choice
- * whose text comes to end in a sequence finishes with reason 1 (stop): it returns the tokens before the first token of the
- * match (of the longest sequence when several end there), its logprob pairs likewise, and its decode row is free from the
- * next step on, while the request's other choices go on.  A choice that reaches max_new_tokens finishes with reason 0
- * (length).  The request is done when every choice has finished.  Stop sequences change no logit and no draw: the tokens
- * returned are a prefix of those of the same request without them.  n_stop = 0 is rr_engine_submit_choices.
- * RR_INVALID_ARGUMENT, before anything is queued, for n_stop outside 0..4, a length outside 1..64, null arrays with
- * n_stop > 0, and whatever rr_engine_submit_choices rejects.
- * wait_stop: rr_engine_wait_choices, and n_tokens_out[c] = the tokens choice c returned, finish_out[c] = its reason (either
- * may be NULL).  Row c of tokens_out / lp_out / id_out holds min(n_tokens_out[c], max_tokens_out) entries.
- * rr_completion.n_generated is the longest choice's count; the other wait calls report the same.  While a request runs,
- * rr_engine_peek[_logprobs] shows a token only once no stop sequence can take it back (hold_out of rr_op_stop_match), so
- * n_generated there never shrinks; a request that ends by length releases the held tokens with its last ones.  After a
- * cancel, an injected failure or an internal error the tokens shown so far are what is kept.
- * Stats: generated_tokens counts every token produced, the cut ones included. */
-int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
-                          int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                          float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
-                          const uint8_t* stop_bytes, const int32_t* stop_off, uint64_t* ticket);
-int rr_engine_wait_stop(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                        int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out /* [n_choices] */,
-                        int32_t* finish_out /* [n_choices] */);
-/* JSON mode (OpenAI `response_format: {"type": "json_object"}`): rr_engine_submit_stop with response_format 1.  Before
- * every token is picked (after penalties and logit bias, before the argmax, the sampler and logprobs) rr_op_json_mask sets
- * the logit of every token the JSON grammar does not allow next to -inf, so the reply's bytes are always a prefix of a JSON
- * text whose top-level value is an object (rr_op_json_mask states the grammar), and logprobs describe the masked
- * distribution (a masked token's logprob is -inf).  The choice whose token closes the top-level object finishes with reason
- * 1 (stop), that token included, and frees its decode row at once; a stop-sequence cut on the same token wins, and
- * max_new_tokens first gives reason 0 (length) and a valid prefix.  Results come back through rr_engine_wait_stop.
- * response_format 0 is rr_engine_submit_stop.  RR_INVALID_ARGUMENT, before anything is queued, for response_format other
- * than 0 or 1, 1 on an engine with vocab < 259 (some bytes have no token), and whatever rr_engine_submit_stop rejects. */
-int rr_engine_submit_format(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
-                            int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
-                            const uint8_t* stop_bytes, const int32_t* stop_off, int response_format, uint64_t* ticket);
+/* Streaming (SSE): block until the request shows more than `have` tokens, is done, or `timeout_s` elapses; then
+ * *n_generated = the tokens shown, *done = 1 once the request is done, *t_first_token_s = its time to the first token, and
+ * the first min(*n_generated, max_tokens_out) tokens go to tokens_out, with top_logprobs >= 0 their pairs to lp_out /
+ * id_out [max_tokens_out][K] (tokens_out, t_first_token_s, lp_out and id_out may each be NULL).  Does not consume the
+ * request: finish with rr_engine_wait.  While a request runs, a token is shown only once no stop sequence can take it back
+ * (hold_out of rr_op_stop_match), so *n_generated never shrinks; a request that ends by length releases the held tokens
+ * with its last ones.  After a cancel, an injected failure or an internal error the tokens shown so far are what is kept.
+ * RR_INVALID_ARGUMENT for a NULL engine, n_generated or done, for a request of n_choices > 1 (it stays in flight) and for
+ * an unknown or consumed ticket. */
+int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
+                   int32_t* n_generated, int32_t* done, double* t_first_token_s, float* lp_out, int32_t* id_out);
 /* Closed-batch convenience used by bench.py: submit all, wait all. prompts are host buffers
  * (pinned or pageable); the H2D copies happen inside. */
 int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start,
@@ -596,7 +584,7 @@ typedef struct rr_gateway_result {
     int32_t attempts;          /* admissions this request went through (1 + backends that failed under it) */
     double t_submit_s, t_admit_s, t_first_token_s, t_done_s;   /* gateway monotonic clock, seconds */
     int32_t n_cached;          /* rr_completion.n_cached of the engine that served the request */
-    int32_t reserved;          /* choice 0's finish reason once finished: 0 length, 1 stop (rr_engine_submit_stop) */
+    int32_t finish;            /* choice 0's finish reason once finished: 0 length, 1 stop (rr_engine_wait) */
 } rr_gateway_result;
 
 typedef struct rr_gateway_stats {
@@ -619,84 +607,44 @@ typedef struct rr_stub_desc {
  * replica a mock one described by stubs[i] (stubs is read only there and may be NULL when no engine is NULL).
  * RR_INVALID_ARGUMENT, with nothing created, for a NULL engine without a descriptor, reply_tokens < 0, fail_every < 0 or
  * vocab < 1.  A mock replica's vocab counts toward the smallest vocabulary; it sets no context or prefill limit.  A
- * gateway with a mock replica refuses logprobs (top_logprobs >= 0) at submit with RR_INVALID_ARGUMENT.  The router and
+ * gateway with a mock replica refuses logprobs, stop sequences and JSON mode at submit (rr_gateway_submit).  The router and
  * the engines must outlive the gateway; the engines' completion hooks are taken by the gateway until it is destroyed. */
 int rr_gateway_create(rr_router* router, rr_engine* const* engines, const int32_t* replica_ids, int n_engines,
                       const rr_stub_desc* stubs, const rr_gateway_opts* opts, rr_gateway** out);
 void rr_gateway_destroy(rr_gateway* g);
 int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
-/* group = index of the model group (model_name) the client asked for.  Returns RR_NO_GROUP / RR_INVALID_ARGUMENT
- * (prompt + max_new_tokens beyond a replica's context, bad token id: HTTP 400) before anything is debited. */
+/* Queue one request for model group `group` (index of the model_name the client asked for) and write its ticket to
+ * *ticket.  p as rr_engine_submit describes it (NULL: greedy, one choice).  The parameters are stored with the request and
+ * handed to every engine it is admitted to, a fallback re-admission included (all choices restart there), so a
+ * re-admitted sampled request draws the same tokens on a replica with the same weights.  The request is one ADMIT event
+ * (the prompt's tokens) and one DONE event carrying the tokens its choices return, whatever p holds.
+ * Refusals, before anything is debited and with *ticket untouched, in this order: RR_INVALID_ARGUMENT for a NULL gateway
+ * or for parameters rr_engine_submit rejects, bias ids and JSON mode judged against the smallest vocabulary of the
+ * gateway's replicas (stop bytes need no vocabulary check); RR_INVALID_ARGUMENT when a mock replica is attached and p asks
+ * for logprobs (top_logprobs >= 0), stop sequences (n_stop > 0) or JSON mode (response_format 1): a mock replica has no
+ * logits to fill pairs from or to mask and no decode loop to cut; RR_INVALID_ARGUMENT for a NULL prompt or ticket;
+ * RR_NO_GROUP for an unknown group; RR_INVALID_ARGUMENT (HTTP 400) for n_prompt or max_new_tokens below 1, n_choices
+ * outside 1..the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices
+ * copies of its reply), prompt + max_new_tokens beyond a replica's context, a prompt beyond its prefill chunk and a bad
+ * token id. */
 int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                      uint64_t* ticket);
-/* A closed burst as one contiguous block of the admission trace (declare_burst != 0 prepends RR_EV_BURST). */
+                      const rr_gen_params* p, uint64_t* ticket);
+/* A closed burst of plain requests (greedy, one choice) as one contiguous block of the admission trace (declare_burst != 0
+ * prepends RR_EV_BURST). */
 int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
                             int max_new_tokens, int declare_burst, uint64_t* tickets);
 /* Blocks (release the GIL) until the request is finished; returns its status and consumes the ticket.
- * RR_TIMEOUT: still in flight -- wait again or rr_gateway_cancel. */
+ * RR_TIMEOUT: still in flight -- wait again or rr_gateway_cancel.  The buffers as rr_engine_wait fills them (each may be
+ * NULL); a request that never reached a replica reports 0 tokens and reason 0 for every choice.
+ * rr_gateway_result.n_generated is the longest choice's count and .finish choice 0's reason. */
 int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                    int max_tokens_out);
-/* Streaming: returns once more than `have` tokens exist, the request is finished, or timeout_s elapsed. */
+                    int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out /* [n_choices] */,
+                    int32_t* finish_out /* [n_choices] */);
+/* Streaming: returns once more than `have` tokens are shown, the request is finished, or timeout_s elapsed; the tokens
+ * and pairs as rr_engine_peek shows them (a token a stop sequence may still take back is held), and `out` (may be NULL)
+ * gets the request's record so far (status -1 while in flight).  RR_INVALID_ARGUMENT for a request of n_choices > 1. */
 int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
-                    int32_t* n_generated, int32_t* done, rr_gateway_result* out);
-/* The same with per-token log-probabilities (rr_engine_submit_logprobs): top_logprobs -1..20 travels with the request,
- * a fallback re-admission included; wait / peek also fill lp_out / id_out [max_tokens_out][max(1, top_logprobs)].  The
- * admission trace is the same as rr_gateway_submit's. */
-int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                               int top_logprobs, uint64_t* ticket);
-int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                             int max_tokens_out, float* lp_out, int32_t* id_out);
-int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                             int max_tokens_out, int32_t* n_generated, int32_t* done, rr_gateway_result* out,
-                             float* lp_out, int32_t* id_out);
-/* Seeded sampling (rr_engine_submit_sampled): the parameters travel with the request, a fallback re-admission included,
- * so a re-admitted request draws the same tokens on a replica with the same weights.  Results through
- * rr_gateway_wait_logprobs / rr_gateway_peek_logprobs, pair buffers as rr_engine_submit_sampled describes.  The admission
- * trace is the same as rr_gateway_submit's. */
-int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                              int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket);
-/* Penalties and logit bias (rr_engine_submit_processed): stored with the request and handed to every engine it is admitted
- * to, a fallback re-admission included.  Bias ids must lie in [0, the smallest vocabulary of the gateway's engines).  The
- * admission trace is the same as rr_gateway_submit's. */
-int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                                float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
-                                uint64_t* ticket);
-/* Several choices per request (rr_engine_submit_choices): n_choices is stored with the request and travels with it, a
- * fallback re-admission included (all choices restart there).  The request is one ADMIT event (the prompt's tokens) and
- * one DONE event carrying the tokens of all choices.  RR_INVALID_ARGUMENT before anything is debited for n_choices below 1
- * or above the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices copies
- * of its reply).  wait_choices: rr_gateway_wait_logprobs for any n_choices, with tokens_out [n_choices][max_tokens_out]
- * and lp_out / id_out [n_choices][max_tokens_out][K]; rr_gateway_result.n_generated counts the tokens of each choice.
- * rr_gateway_wait / _wait_logprobs / _peek / _peek_logprobs return RR_INVALID_ARGUMENT for a request of n_choices > 1. */
-int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                              int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                              float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                              const float* bias_vals, uint64_t* ticket);
-int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                            int max_tokens_out, float* lp_out, int32_t* id_out);
-/* Stop sequences (rr_engine_submit_stop): stored with the request and handed to every engine it is admitted to, a fallback
- * re-admission included (the bytes need no vocabulary check).  A gateway with a mock replica refuses n_stop > 0 at submit
- * with RR_INVALID_ARGUMENT: a mock replica has no decode loop to cut.  The request is one ADMIT event and one DONE event
- * carrying the tokens its choices return.  wait_stop: rr_gateway_wait_choices plus each choice's token count and finish
- * reason, as rr_engine_wait_stop; rr_gateway_result.n_generated is the longest choice's count.  The other wait and peek
- * calls keep working for such a request of one choice (rr_gateway_result.reserved = its finish reason). */
-int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                           int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                           float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                           const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
-                           uint64_t* ticket);
-int rr_gateway_wait_stop(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                         int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out);
-/* JSON mode (rr_engine_submit_format): the format is stored with the request and handed to every engine it is admitted to,
- * a fallback re-admission included.  RR_INVALID_ARGUMENT at submit for response_format 1 when a mock replica is attached
- * (it has no logits to mask) or the smallest vocabulary is below 259, and for a value other than 0 or 1.  Results come
- * back through rr_gateway_wait_stop.  response_format 0 is rr_gateway_submit_stop. */
-int rr_gateway_submit_format(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                             int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                             float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                             const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
-                             int response_format, uint64_t* ticket);
+                    int32_t* n_generated, int32_t* done, rr_gateway_result* out, float* lp_out, int32_t* id_out);
 /* Abandon a request (consumes the ticket).  count_as_failure != 0: a client-side timeout -- the deployment gets a FAIL
  * event (allowed_fails / cooldown, reference config/config.yaml:103-104); 0: a disconnect -- a DONE event. */
 int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure);

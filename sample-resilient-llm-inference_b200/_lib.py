@@ -113,7 +113,14 @@ class GatewayResult(C.Structure):
                 ("chain_pos", C.c_int32), ("replica", C.c_int32), ("n_prompt", C.c_int32), ("n_generated", C.c_int32),
                 ("attempts", C.c_int32), ("t_submit_s", C.c_double), ("t_admit_s", C.c_double),
                 ("t_first_token_s", C.c_double), ("t_done_s", C.c_double), ("n_cached", C.c_int32),
-                ("reserved", C.c_int32)]
+                ("finish", C.c_int32)]
+
+
+class GenParams(C.Structure):
+    _fields_ = [("n_choices", C.c_int32), ("top_logprobs", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
+                ("seed", C.c_uint64), ("frequency_penalty", C.c_float), ("presence_penalty", C.c_float),
+                ("n_bias", C.c_int32), ("n_stop", C.c_int32), ("bias_ids", c_i32p), ("bias_vals", c_f32p),
+                ("stop_bytes", c_u8p), ("stop_off", c_i32p), ("response_format", C.c_int32), ("reserved", C.c_int32)]
 
 
 class GatewayStats(C.Structure):
@@ -183,33 +190,11 @@ PROTOTYPES = {
     "rr_engine_destroy": (None, [vp]),
     "rr_engine_prefill": (C.c_int, [vp, c_i32p, c_i32p, c_i32p, C.c_int, c_i32p, c_f32p]),
     "rr_engine_decode_step": (C.c_int, [vp, c_i32p, c_i32p, c_i32p, C.c_int, c_i32p, c_f32p]),
-    "rr_engine_submit": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_engine_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p,
-                                 C.c_int]),
+    "rr_engine_submit": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.POINTER(C.c_uint64)]),
+    "rr_engine_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p, c_i32p,
+                                 c_i32p]),
     "rr_engine_peek": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
-                                 C.POINTER(C.c_double)]),
-    "rr_engine_submit_logprobs": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_engine_wait_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p,
-                                          c_i32p]),
-    "rr_engine_peek_logprobs": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
-                                          C.POINTER(C.c_double), c_f32p, c_i32p]),
-    "rr_engine_submit_sampled": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
-                                           C.POINTER(C.c_uint64)]),
-    "rr_engine_submit_processed": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_uint64,
-                                             C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.POINTER(C.c_uint64)]),
-    "rr_engine_submit_choices": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                           C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
-                                           C.POINTER(C.c_uint64)]),
-    "rr_engine_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p,
-                                         c_i32p]),
-    "rr_engine_submit_stop": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                        C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
-                                        C.POINTER(C.c_uint64)]),
-    "rr_engine_submit_format": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                          C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
-                                          C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_engine_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p,
-                                      c_i32p, c_i32p]),
+                                 C.POINTER(C.c_double), c_f32p, c_i32p]),
     "rr_engine_run_batch": (C.c_int, [vp, c_i32p, c_i32p, C.c_int, C.c_int,
                                       C.POINTER(Completion), c_i32p]),
     "rr_engine_now": (C.c_double, [vp]),
@@ -220,34 +205,12 @@ PROTOTYPES = {
                                     C.POINTER(vp)]),
     "rr_gateway_destroy": (None, [vp]),
     "rr_gateway_set_now": (C.c_int, [vp, C.c_int64]),
-    "rr_gateway_submit": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
+    "rr_gateway_submit": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.POINTER(C.c_uint64)]),
     "rr_gateway_submit_batch": (C.c_int, [vp, C.c_int, c_i32p, c_i32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_gateway_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int]),
+    "rr_gateway_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p, c_i32p,
+                                  c_i32p, c_i32p]),
     "rr_gateway_peek": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
-                                  C.POINTER(GatewayResult)]),
-    "rr_gateway_submit_logprobs": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_gateway_wait_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
-                                           c_i32p]),
-    "rr_gateway_peek_logprobs": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
-                                           C.POINTER(GatewayResult), c_f32p, c_i32p]),
-    "rr_gateway_submit_sampled": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                            C.c_uint64, C.POINTER(C.c_uint64)]),
-    "rr_gateway_submit_processed": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                              C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
-                                              C.POINTER(C.c_uint64)]),
-    "rr_gateway_submit_choices": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                            C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p,
-                                            C.POINTER(C.c_uint64)]),
-    "rr_gateway_wait_choices": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
-                                          c_i32p]),
-    "rr_gateway_submit_stop": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
-                                         C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int, c_u8p, c_i32p,
-                                         C.POINTER(C.c_uint64)]),
-    "rr_gateway_submit_format": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
-                                           C.c_float, C.c_uint64, C.c_float, C.c_float, C.c_int, c_i32p, c_f32p, C.c_int,
-                                           c_u8p, c_i32p, C.c_int, C.POINTER(C.c_uint64)]),
-    "rr_gateway_wait_stop": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p,
-                                       c_i32p, c_i32p, c_i32p]),
+                                  C.POINTER(GatewayResult), c_f32p, c_i32p]),
     "rr_gateway_cancel": (C.c_int, [vp, C.c_uint64, C.c_int]),
     "rr_gateway_quiesce": (C.c_int, [vp, C.c_double]),
     "rr_gateway_get_stats": (C.c_int, [vp, C.POINTER(GatewayStats)]),

@@ -198,39 +198,43 @@ struct ParamBlocks {
     }
 };
 
-int GenParams::set(int vocab, int top_logprobs, float temperature, float top_p_, uint64_t seed_, float frequency_penalty,
-                   float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop_,
-                   const uint8_t* stop_bytes, const int32_t* stop_off, int response_format) {
-    if (top_logprobs < -1 || top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
-    if (response_format < 0 || response_format > 1 || (response_format == 1 && vocab < JSON_MIN_VOCAB))
+static_assert(sizeof(rr_gen_params) == 80 && offsetof(rr_gen_params, seed) == 16 && offsetof(rr_gen_params, bias_ids) == 40 &&
+                  offsetof(rr_gen_params, response_format) == 72,
+              "rr_gen_params layout: _lib.GenParams and tests/test_abi.py mirror it");
+int GenParams::set(int vocab, const rr_gen_params* p) {
+    if (!p) { *this = GenParams(); return RR_OK; }
+    if (p->top_logprobs < -1 || p->top_logprobs > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
+    if (p->response_format < 0 || p->response_format > 1 || (p->response_format == 1 && vocab < JSON_MIN_VOCAB))
         return RR_INVALID_ARGUMENT;
-    if (!(temperature >= 0.f && temperature <= 2.f && top_p_ >= 0.f && top_p_ <= 1.f)) return RR_INVALID_ARGUMENT;
-    if (!(frequency_penalty >= -2.f && frequency_penalty <= 2.f && presence_penalty >= -2.f && presence_penalty <= 2.f))
+    if (!(p->temperature >= 0.f && p->temperature <= 2.f && p->top_p >= 0.f && p->top_p <= 1.f)) return RR_INVALID_ARGUMENT;
+    if (!(p->frequency_penalty >= -2.f && p->frequency_penalty <= 2.f && p->presence_penalty >= -2.f &&
+          p->presence_penalty <= 2.f))
         return RR_INVALID_ARGUMENT;
-    if (n_bias < 0 || n_bias > PEN_MAX_BIAS || (n_bias > 0 && (!bias_ids || !bias_vals))) return RR_INVALID_ARGUMENT;
+    const int n_bias = p->n_bias;
+    if (n_bias < 0 || n_bias > PEN_MAX_BIAS || (n_bias > 0 && (!p->bias_ids || !p->bias_vals))) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_bias; ++i)
-        if (bias_ids[i] < 0 || bias_ids[i] >= vocab || !(bias_vals[i] >= -100.f && bias_vals[i] <= 100.f))
+        if (p->bias_ids[i] < 0 || p->bias_ids[i] >= vocab || !(p->bias_vals[i] >= -100.f && p->bias_vals[i] <= 100.f))
             return RR_INVALID_ARGUMENT;
-    std::vector<int32_t> ids(bias_ids, bias_ids + n_bias);
+    std::vector<int32_t> ids(p->bias_ids, p->bias_ids + n_bias);
     std::sort(ids.begin(), ids.end());
     if (std::adjacent_find(ids.begin(), ids.end()) != ids.end()) return RR_INVALID_ARGUMENT;
-    if (n_stop_ < 0 || n_stop_ > STOP_MAX_SEQS || (n_stop_ > 0 && (!stop_bytes || !stop_off))) return RR_INVALID_ARGUMENT;
-    for (int i = 0; i < n_stop_; ++i)
-        if (stop_off[i] < 0 || stop_off[i + 1] - stop_off[i] < 1 || stop_off[i + 1] - stop_off[i] > STOP_MAX_LEN)
-            return RR_INVALID_ARGUMENT;
+    const int32_t* off = p->stop_off;
+    if (p->n_stop < 0 || p->n_stop > STOP_MAX_SEQS || (p->n_stop > 0 && (!p->stop_bytes || !off))) return RR_INVALID_ARGUMENT;
+    for (int i = 0; i < p->n_stop; ++i)
+        if (off[i] < 0 || off[i + 1] - off[i] < 1 || off[i + 1] - off[i] > STOP_MAX_LEN) return RR_INVALID_ARGUMENT;
     *this = GenParams();
-    top_lp = top_logprobs;
-    if (temperature > 0.f) { temp = temperature; top_p = top_p_; seed = seed_; }
-    if (frequency_penalty != 0.f || presence_penalty != 0.f || n_bias > 0) {
-        fpen = frequency_penalty; ppen = presence_penalty;
-        bias_id.assign(bias_ids, bias_ids + n_bias); bias_val.assign(bias_vals, bias_vals + n_bias);
+    top_lp = p->top_logprobs;
+    if (p->temperature > 0.f) { temp = p->temperature; top_p = p->top_p; seed = p->seed; }
+    if (p->frequency_penalty != 0.f || p->presence_penalty != 0.f || n_bias > 0) {
+        fpen = p->frequency_penalty; ppen = p->presence_penalty;
+        bias_id.assign(p->bias_ids, p->bias_ids + n_bias); bias_val.assign(p->bias_vals, p->bias_vals + n_bias);
     }
-    n_stop = n_stop_;
-    for (int i = 0; i < n_stop_; ++i) {
-        stop_len[i] = (uint8_t)(stop_off[i + 1] - stop_off[i]);
-        memcpy(stop[i], stop_bytes + stop_off[i], stop_len[i]);
+    n_stop = p->n_stop;
+    for (int i = 0; i < n_stop; ++i) {
+        stop_len[i] = (uint8_t)(off[i + 1] - off[i]);
+        memcpy(stop[i], p->stop_bytes + off[i], stop_len[i]);
     }
-    fmt = response_format;
+    fmt = p->response_format;
     return RR_OK;
 }
 
@@ -1470,60 +1474,13 @@ int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab
 }
 }  // namespace rr
 
-RR_API int rr_engine_submit_format(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                   int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                   float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                   const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
-                                   int response_format, uint64_t* ticket) {
+RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                            const rr_gen_params* params, uint64_t* ticket) {
     if (!e) return RR_INVALID_ARGUMENT;
     rr::GenParams p;
-    const int rc = p.set(e->d.vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off, response_format);
-    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, n_choices);
-}
-
-RR_API int rr_engine_submit_stop(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, int n_choices,
-                                 int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-                                 float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals,
-                                 int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off, uint64_t* ticket) {
-    return rr_engine_submit_format(e, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature, top_p,
-                                   seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, n_stop, stop_bytes,
-                                   stop_off, 0, ticket);
-}
-
-RR_API int rr_engine_submit_choices(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                    int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                    float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                    const float* bias_vals, uint64_t* ticket) {
-    return rr_engine_submit_stop(e, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature, top_p, seed,
-                                 frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, 0, nullptr, nullptr,
-                                 ticket);
-}
-
-RR_API int rr_engine_submit_processed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                      int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                      float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                      const float* bias_vals, uint64_t* ticket) {
-    return rr_engine_submit_choices(e, prompt_ids, n_prompt, max_new_tokens, 1, top_logprobs, temperature, top_p, seed,
-                                    frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, ticket);
-}
-
-RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                            uint64_t* ticket) {
-    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, -1, 0.f, 1.f, 0, 0.f, 0.f, 0, nullptr,
-                                      nullptr, ticket);
-}
-
-RR_API int rr_engine_submit_logprobs(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                     int top_logprobs, uint64_t* ticket) {
-    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, top_logprobs, 0.f, 1.f, 0, 0.f, 0.f, 0,
-                                      nullptr, nullptr, ticket);
-}
-
-RR_API int rr_engine_submit_sampled(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                    int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
-    return rr_engine_submit_processed(e, prompt_ids, n_prompt, max_new_tokens, top_logprobs, temperature, top_p, seed, 0.f,
-                                      0.f, 0, nullptr, nullptr, ticket);
+    const int rc = p.set(e->d.vocab, params);
+    return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p,
+                                                       params ? params->n_choices : 1);
 }
 
 // Caller holds e->mu.  The first min(n, max_tokens_out) visible tokens of each choice of r (fewer for a shorter choice)
@@ -1573,9 +1530,9 @@ RR_API int rr_engine_cancel(rr_engine* e, uint64_t ticket) {
 // Streaming support: block until the request has more than `have` tokens (or is done / the wait times out), then
 // copy the tokens generated so far.  Does not consume the request; finish with rr_engine_wait.  A request of several
 // choices gets RR_INVALID_ARGUMENT.
-RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                                   int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s,
-                                   float* lp_out, int32_t* id_out) {
+RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
+                          int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s, float* lp_out,
+                          int32_t* id_out) {
     if (!e || !n_generated || !done) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1603,17 +1560,8 @@ RR_API int rr_engine_peek_logprobs(rr_engine* e, uint64_t ticket, int have, doub
     return RR_OK;
 }
 
-RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                          int max_tokens_out, int32_t* n_generated, int32_t* done, double* t_first_token_s) {
-    return rr_engine_peek_logprobs(e, ticket, have, timeout_s, tokens_out, max_tokens_out, n_generated, done,
-                                   t_first_token_s, nullptr, nullptr);
-}
-
-// rr_engine_wait_stop, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
-// choices, which stays in flight.
-static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                       int max_tokens_out, float* lp_out, int32_t* id_out, bool choices, int32_t* n_tokens_out = nullptr,
-                       int32_t* finish_out = nullptr) {
+RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
+                          int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out) {
     if (!e || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
     const auto deadline = std::chrono::steady_clock::now() +
@@ -1623,7 +1571,6 @@ static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_compl
         auto it = e->table.find(ticket);
         if (it == e->table.end()) return RR_INVALID_ARGUMENT;      // unknown, already consumed, or cancelled
         r = it->second;
-        if (!choices && r->n_choices > 1) return RR_INVALID_ARGUMENT;
         if (r->done) break;
         if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
             it = e->table.find(ticket);
@@ -1647,40 +1594,19 @@ static int engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_compl
     return status == RR_OK ? RR_OK : status;
 }
 
-RR_API int rr_engine_wait_stop(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                               int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out,
-                               int32_t* finish_out) {
-    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true, n_tokens_out, finish_out);
-}
-
-RR_API int rr_engine_wait_choices(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
-                                  int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
-    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true);
-}
-
-RR_API int rr_engine_wait_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out,
-                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
-    return engine_wait(e, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, false);
-}
-
-RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_completion* out, int32_t* tokens_out,
-                          int max_tokens_out) {
-    return rr_engine_wait_logprobs(e, ticket, timeout_s, out, tokens_out, max_tokens_out, nullptr, nullptr);
-}
-
 RR_API int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const int32_t* prompt_start, int n_requests,
                                int max_new_tokens, rr_completion* out, int32_t* tokens_out) {
     if (!e || !prompt_ids || !prompt_start || n_requests < 1 || !out) return RR_INVALID_ARGUMENT;
     std::vector<uint64_t> tk(n_requests);
     for (int i = 0; i < n_requests; ++i) {
         int rc = rr_engine_submit(e, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i],
-                                  max_new_tokens, &tk[i]);
+                                  max_new_tokens, nullptr, &tk[i]);
         if (rc != RR_OK) return rc;
     }
     int worst = RR_OK;
     for (int i = 0; i < n_requests; ++i) {
         int rc = rr_engine_wait(e, tk[i], 0, &out[i], tokens_out ? tokens_out + (size_t)i * max_new_tokens : nullptr,
-                                max_new_tokens);
+                                max_new_tokens, nullptr, nullptr, nullptr, nullptr);
         if (rc != RR_OK) worst = rc;
     }
     return worst;

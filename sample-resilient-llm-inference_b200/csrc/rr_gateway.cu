@@ -215,8 +215,8 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     std::vector<int32_t> n_toks(n_ch, 0), fins(n_ch, 0);
     int wrc = RR_INVALID_ARGUMENT;
     if (eng && status != RR_CANCELLED)
-        wrc = rr_engine_wait_stop(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
-                                  logprobs ? lp_ids.data() : nullptr, n_toks.data(), fins.data());
+        wrc = rr_engine_wait(eng, eng_ticket, 0.001, &comp, toks.data(), max_new, logprobs ? lps.data() : nullptr,
+                             logprobs ? lp_ids.data() : nullptr, n_toks.data(), fins.data());
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -485,66 +485,17 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
 
 // The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
 // gets RR_INVALID_ARGUMENT.
-RR_API int rr_gateway_submit_format(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
-                                    int max_new_tokens, int n_choices, int top_logprobs, float temperature, float top_p,
-                                    uint64_t seed, float frequency_penalty, float presence_penalty, int n_bias,
-                                    const int32_t* bias_ids, const float* bias_vals, int n_stop, const uint8_t* stop_bytes,
-                                    const int32_t* stop_off, int response_format, uint64_t* ticket) {
+RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                             const rr_gen_params* params, uint64_t* ticket) {
     if (!g) return RR_INVALID_ARGUMENT;
     rr::GenParams p;
     // the format is checked against the smallest vocabulary: a fallback re-admission may take the request to any replica
-    const int rc = p.set(g->min_vocab, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, n_bias,
-                         bias_ids, bias_vals, n_stop, stop_bytes, stop_off, response_format);
+    const int rc = p.set(g->min_vocab, params);
     if (rc != RR_OK) return rc;
     // a mock replica has no logits to fill the pairs from or to mask, and no decode loop to cut
     if ((p.logprobs() || p.stops() || p.json()) && g->has_stub) return RR_INVALID_ARGUMENT;
     const int32_t start[2] = {0, n_prompt};
-    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, n_choices, ticket);
-}
-
-RR_API int rr_gateway_submit_stop(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                  int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                  float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                  const float* bias_vals, int n_stop, const uint8_t* stop_bytes, const int32_t* stop_off,
-                                  uint64_t* ticket) {
-    return rr_gateway_submit_format(g, group, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature,
-                                    top_p, seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, n_stop,
-                                    stop_bytes, stop_off, 0, ticket);
-}
-
-RR_API int rr_gateway_submit_choices(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                     int n_choices, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                     float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                     const float* bias_vals, uint64_t* ticket) {
-    return rr_gateway_submit_stop(g, group, prompt_ids, n_prompt, max_new_tokens, n_choices, top_logprobs, temperature,
-                                  top_p, seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, 0, nullptr,
-                                  nullptr, ticket);
-}
-
-RR_API int rr_gateway_submit_processed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt,
-                                       int max_new_tokens, int top_logprobs, float temperature, float top_p, uint64_t seed,
-                                       float frequency_penalty, float presence_penalty, int n_bias, const int32_t* bias_ids,
-                                       const float* bias_vals, uint64_t* ticket) {
-    return rr_gateway_submit_choices(g, group, prompt_ids, n_prompt, max_new_tokens, 1, top_logprobs, temperature, top_p,
-                                     seed, frequency_penalty, presence_penalty, n_bias, bias_ids, bias_vals, ticket);
-}
-
-RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                             uint64_t* ticket) {
-    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, -1, 0.f, 1.f, 0, 0.f, 0.f, 0, nullptr,
-                                       nullptr, ticket);
-}
-
-RR_API int rr_gateway_submit_logprobs(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                      int top_logprobs, uint64_t* ticket) {
-    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, top_logprobs, 0.f, 1.f, 0, 0.f, 0.f, 0,
-                                       nullptr, nullptr, ticket);
-}
-
-RR_API int rr_gateway_submit_sampled(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                                     int top_logprobs, float temperature, float top_p, uint64_t seed, uint64_t* ticket) {
-    return rr_gateway_submit_processed(g, group, prompt_ids, n_prompt, max_new_tokens, top_logprobs, temperature, top_p, seed,
-                                       0.f, 0.f, 0, nullptr, nullptr, ticket);
+    return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, params ? params->n_choices : 1, ticket);
 }
 
 // caller holds g->mu.  The first min(n, max_tokens_out) tokens of each choice (fewer for a shorter choice) into tokens_out
@@ -570,14 +521,11 @@ static void gw_fill(const GwReq* r, rr_gateway_result* out) {
     out->replica = r->replica; out->n_prompt = (int32_t)r->prompt.size(); out->n_generated = (int32_t)r->n_gen();
     out->attempts = r->attempts;
     out->t_submit_s = r->t_submit; out->t_admit_s = r->t_admit; out->t_first_token_s = r->t_first; out->t_done_s = r->t_done;
-    out->n_cached = r->n_cached; out->reserved = r->fin.empty() ? 0 : r->fin[0];
+    out->n_cached = r->n_cached; out->finish = r->fin.empty() ? 0 : r->fin[0];
 }
 
-// rr_gateway_wait_choices, and with `choices` false (the single-choice calls) RR_INVALID_ARGUMENT for a request of several
-// choices, which stays in flight.
-static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                   int max_tokens_out, float* lp_out, int32_t* id_out, bool choices, int32_t* n_tokens_out = nullptr,
-                   int32_t* finish_out = nullptr) {
+RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
+                           int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out) {
     if (!g || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(g->mu);
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
@@ -586,7 +534,6 @@ static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_
         auto it = g->table.find(ticket);
         if (it == g->table.end()) return RR_INVALID_ARGUMENT;
         r = it->second;
-        if (!choices && r->n_choices > 1) return RR_INVALID_ARGUMENT;
         if (r->state == FINISHED) break;
         if (g->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
             it = g->table.find(ticket);
@@ -610,30 +557,8 @@ static int gw_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_
     return status;
 }
 
-RR_API int rr_gateway_wait_stop(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                                int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out,
-                                int32_t* finish_out) {
-    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true, n_tokens_out, finish_out);
-}
-
-RR_API int rr_gateway_wait_choices(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
-                                   int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
-    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, true);
-}
-
-RR_API int rr_gateway_wait_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out,
-                                    int32_t* tokens_out, int max_tokens_out, float* lp_out, int32_t* id_out) {
-    return gw_wait(g, ticket, timeout_s, out, tokens_out, max_tokens_out, lp_out, id_out, false);
-}
-
-RR_API int rr_gateway_wait(rr_gateway* g, uint64_t ticket, double timeout_s, rr_gateway_result* out, int32_t* tokens_out,
-                           int max_tokens_out) {
-    return rr_gateway_wait_logprobs(g, ticket, timeout_s, out, tokens_out, max_tokens_out, nullptr, nullptr);
-}
-
-RR_API int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out,
-                                    int max_tokens_out, int32_t* n_generated, int32_t* done, rr_gateway_result* out,
-                                    float* lp_out, int32_t* id_out) {
+RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
+                           int32_t* n_generated, int32_t* done, rr_gateway_result* out, float* lp_out, int32_t* id_out) {
     if (!g || !n_generated || !done) return RR_INVALID_ARGUMENT;
     const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
     for (;;) {
@@ -659,20 +584,14 @@ RR_API int rr_gateway_peek_logprobs(rr_gateway* g, uint64_t ticket, int have, do
         }
         const double left = std::chrono::duration<double>(deadline - std::chrono::steady_clock::now()).count();
         int32_t n = 0, d = 0;
-        const int rc = rr_engine_peek_logprobs(eng, tk, have, left > 0.001 ? left : 0.001, tokens_out, max_tokens_out, &n, &d,
-                                               nullptr, lp_out, id_out);
+        const int rc = rr_engine_peek(eng, tk, have, left > 0.001 ? left : 0.001, tokens_out, max_tokens_out, &n, &d, nullptr,
+                                      lp_out, id_out);
         if (rc == RR_OK && !d) { *n_generated = n; *done = 0; return RR_OK; }
         // finished (the hook is consuming / has consumed the engine's record) or failed over: look at our own record again
         if (std::chrono::steady_clock::now() >= deadline) { *n_generated = rc == RR_OK ? n : 0; *done = 0; return RR_OK; }
         std::unique_lock<std::mutex> lk(g->mu);
         g->cv_done.wait_for(lk, std::chrono::milliseconds(1));
     }
-}
-
-RR_API int rr_gateway_peek(rr_gateway* g, uint64_t ticket, int have, double timeout_s, int32_t* tokens_out, int max_tokens_out,
-                           int32_t* n_generated, int32_t* done, rr_gateway_result* out) {
-    return rr_gateway_peek_logprobs(g, ticket, have, timeout_s, tokens_out, max_tokens_out, n_generated, done, out, nullptr,
-                                    nullptr);
 }
 
 RR_API int rr_gateway_cancel(rr_gateway* g, uint64_t ticket, int count_as_failure) {

@@ -77,8 +77,8 @@ int num_sms();
 
 // ---- engine / router internals used by the native gateway (rr_gateway.cu)
 typedef void (*EngineDoneHook)(void* ctx, uint64_t tag, uint64_t ticket, int status, int n_generated);
-// What a request asks the decoder to do (the parameters of rr_engine_submit_processed / rr_gateway_submit_processed;
-// the defaults are a plain greedy request).  The gateway hands it unchanged to every engine the request is admitted to.
+// What a request asks the decoder to do (an rr_gen_params of rr_engine_submit / rr_gateway_submit, less n_choices; the
+// defaults are a plain greedy request).  The gateway hands it unchanged to every engine the request is admitted to.
 struct GenParams {
     int top_lp = -1;                  // -1: no logprobs, else max(1, top_lp) (logprob, id) pairs per token
     float temp = 0.f, top_p = 1.f;    // temp > 0 draws every token with rr_op_sample
@@ -99,17 +99,16 @@ struct GenParams {
     bool json() const { return fmt == 1; }
     // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
     int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
-    // The raw C arguments, checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and OpenAI's ranges
-    // 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null arrays when
-    // n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails; 0 <= n_stop <= STOP_MAX_SEQS
-    // sequences of 1..STOP_MAX_LEN bytes each, sequence i = stop_bytes[stop_off[i] .. stop_off[i + 1]) (non-null arrays when
-    // n_stop > 0); response_format 0 or 1, and 1 only with vocab >= JSON_MIN_VOCAB.  A greedy request keeps the default
-    // top_p and seed, an unprocessed one the default penalties.  RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
-    int set(int vocab, int top_logprobs, float temperature, float top_p, uint64_t seed, float frequency_penalty,
-            float presence_penalty, int n_bias, const int32_t* bias_ids, const float* bias_vals, int n_stop,
-            const uint8_t* stop_bytes, const int32_t* stop_off, int response_format = 0);
+    // The raw C struct (NULL: the defaults), checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and
+    // OpenAI's ranges 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null
+    // arrays when n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails; 0 <= n_stop <=
+    // STOP_MAX_SEQS sequences of 1..STOP_MAX_LEN bytes each, sequence i = stop_bytes[stop_off[i] .. stop_off[i + 1])
+    // (non-null arrays when n_stop > 0); response_format 0 or 1, and 1 only with vocab >= JSON_MIN_VOCAB.  n_choices is
+    // the caller's to check.  A greedy request keeps the default top_p and seed, an unprocessed one the default penalties.
+    // RR_INVALID_ARGUMENT (nothing stored) or RR_OK.
+    int set(int vocab, const rr_gen_params* p);
 };
-// n_choices (1..max_batch): choices of the request (rr_engine_submit_choices); the done hook's n_generated is the total of
+// n_choices (1..max_batch): choices of the request (rr_gen_params.n_choices); the done hook's n_generated is the total of
 // the tokens the choices return (a choice cut by a stop sequence counts what is left of it).
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, const GenParams& p, int n_choices);

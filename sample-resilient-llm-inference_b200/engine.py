@@ -108,8 +108,7 @@ class Engine:
                                1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
-        self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1 or with stop
-        self._stop: set = set()             # tickets of the requests submitted with stop or JSON mode
+        self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -160,39 +159,26 @@ class Engine:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
-        rr_engine_submit_sampled; None or 0 is greedy.  frequency_penalty / presence_penalty in [-2, 2] and logit_bias
+        rr_engine_submit; None or 0 is greedy.  frequency_penalty / presence_penalty in [-2, 2] and logit_bias
         {token id: bias in [-100, 100]} (at most 300 entries): applied to the logits before every token is picked, the
-        penalties over the tokens generated so far (rr_engine_submit_processed); None, 0 or {} change nothing.
-        n in 1..max_batch: n choices of the prompt, prefilled once (rr_engine_submit_choices); choice i is drawn with
-        seed + i.  wait() returns them all; peek() is for n = 1 only.
+        penalties over the tokens generated so far; None, 0 or {} change nothing.
+        n in 1..max_batch: n choices of the prompt, prefilled once; choice i is drawn with seed + i.  wait() returns
+        them all; peek() is for n = 1 only.
         stop: a string or up to 4 strings (or bytes) of 1..64 bytes each: a choice ends where its reply text (the bytes of
-        its tokens) would contain one, returns the tokens before the match and frees its decode row at once
-        (rr_engine_submit_stop).  The tokens are a prefix of the same request's without `stop`.
-        response_format {"type": "json_object"}: JSON mode (rr_engine_submit_format): every token is picked from the
-        logits masked to the JSON grammar, and a choice ends with finish reason "stop" on the token that closes its
-        top-level object.  None and {"type": "text"} change nothing (check_response_format)."""
+        its tokens) would contain one, returns the tokens before the match and frees its decode row at once.  The
+        tokens are a prefix of the same request's without `stop`.
+        response_format {"type": "json_object"}: JSON mode: every token is picked from the logits masked to the JSON
+        grammar, and a choice ends with finish reason "stop" on the token that closes its top-level object.  None and
+        {"type": "text"} change nothing (check_response_format)."""
         ids = _i32(prompt_ids)
         bias = logit_bias or {}
         stops = stop if isinstance(stop, (list, tuple)) and all(isinstance(b, bytes) for b in stop) else check_stop(stop)
         gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
-                       list(bias.values()), stop=stops, json_object=check_response_format(response_format))
+                       list(bias.values()), stop=stops, json_object=check_response_format(response_format), n=n)
         t = C.c_uint64()
-        if gen.fmt:
-            _lib.check(_lib.lib.rr_engine_submit_format(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail,
-                                                        *gen.format_args(), C.byref(t)), "rr_engine_submit_format")
-            self._n[t.value] = n
-            self._stop.add(t.value)
-        elif gen.stop:
-            _lib.check(_lib.lib.rr_engine_submit_stop(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail, *gen.stop,
-                                                      C.byref(t)), "rr_engine_submit_stop")
-            self._n[t.value] = n
-            self._stop.add(t.value)
-        elif n == 1:
-            _lib.check(_lib.lib.rr_engine_submit_processed(self._h, _p(ids), len(ids), max_new_tokens, *gen.tail,
-                                                           C.byref(t)), "rr_engine_submit_processed")
-        else:
-            _lib.check(_lib.lib.rr_engine_submit_choices(self._h, _p(ids), len(ids), max_new_tokens, n, *gen.tail,
-                                                         C.byref(t)), "rr_engine_submit_choices")
+        _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(gen.params), C.byref(t)),
+                   "rr_engine_submit")
+        if n > 1:
             self._n[t.value] = n
         if gen.width:
             self._lp_k[t.value] = gen.width
@@ -211,17 +197,11 @@ class Engine:
         buf = np.zeros((nc, max_tokens), dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens, nc)
         n_tok, fin = (C.c_int32 * nc)(), (C.c_int32 * nc)()
-        if ticket in self._stop:
-            rc = _lib.lib.rr_engine_wait_stop(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p,
-                                              n_tok, fin)
-        else:
-            wait = _lib.lib.rr_engine_wait_choices if nc > 1 else _lib.lib.rr_engine_wait_logprobs
-            rc = wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p)
-            n_tok[:] = [c.n_generated] * nc
+        rc = _lib.lib.rr_engine_wait(self._h, ticket, float(timeout), C.byref(c), _p(buf), max_tokens, lp_p, ids_p, n_tok,
+                                     fin)
         if rc != 6:
             self._lp_k.pop(ticket, None)
             self._n.pop(ticket, None)
-            self._stop.discard(ticket)
         if rc not in (0, 6, 7):
             _lib.check(rc, "rr_engine_wait")
         ns = [min(k, max_tokens) for k in n_tok]
@@ -237,8 +217,8 @@ class Engine:
         n, done, ttft = C.c_int32(), C.c_int32(), C.c_double()
         lp, ids, lp_p, ids_p = self._lp_bufs(ticket, max_tokens)
         lp, ids = (None, None) if lp is None else (lp[0], ids[0])
-        _lib.check(_lib.lib.rr_engine_peek_logprobs(self._h, ticket, have, float(timeout), _p(buf), max_tokens, C.byref(n),
-                                                    C.byref(done), C.byref(ttft), lp_p, ids_p), "rr_engine_peek")
+        _lib.check(_lib.lib.rr_engine_peek(self._h, ticket, have, float(timeout), _p(buf), max_tokens, C.byref(n),
+                                           C.byref(done), C.byref(ttft), lp_p, ids_p), "rr_engine_peek")
         if lp is None:
             return buf[: n.value].tolist(), bool(done.value), ttft.value
         m = min(n.value, max_tokens)

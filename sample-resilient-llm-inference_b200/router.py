@@ -251,7 +251,7 @@ def check_n(n: Any) -> int:
 
 MAX_STOP = 4                 # OpenAI's limit on the number of `stop` sequences (STOP_MAX_SEQS of the engine)
 MAX_STOP_BYTES = 64          # this project's cap on one stop sequence, in bytes of UTF-8 (STOP_MAX_LEN of the engine)
-FINISH_REASONS = ("length", "stop")      # by the native finish code (rr_engine_wait_stop)
+FINISH_REASONS = ("length", "stop")      # by the native finish code (rr_engine_wait)
 JSON_MIN_VOCAB = 259         # JSON mode needs a token for every byte (3 + 256; JSON_MIN_VOCAB of the engine)
 
 
@@ -292,20 +292,9 @@ def check_response_format(value: Any) -> bool:
 
 class GenArgs(NamedTuple):
     """A request's generation parameters in the form the native submit calls take them (gen_args)."""
+    params: _lib.GenParams  # rr_gen_params, passed by reference to rr_engine_submit / rr_gateway_submit
     top: Optional[int]     # top_logprobs; None: no logprobs
-    tail: tuple            # rr_engine_submit_processed / rr_gateway_submit_processed: top_logprobs .. bias_vals
     width: int             # (logprob, id) pairs per generated token; 0 without logprobs
-    stop: tuple = ()       # with stop sequences, what rr_*_submit_stop takes after the tail: n_stop, stop_bytes, stop_off
-    fmt: int = 0           # response format of rr_*_submit_format: 0 text, 1 json_object
-
-    @property
-    def ends_early(self) -> bool:
-        """The choices end on their own (stop sequences, JSON mode): results come back through rr_*_wait_stop."""
-        return bool(self.stop) or self.fmt != 0
-
-    def format_args(self) -> tuple:
-        """What rr_*_submit_format takes after the tail: n_stop, stop_bytes, stop_off, response_format."""
-        return (self.stop or (0, None, None)) + (self.fmt,)
 
 
 class StreamItem(tuple):
@@ -316,29 +305,30 @@ class StreamItem(tuple):
 def gen_args(top_logprobs: Optional[int] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
              seed: Optional[int] = None, frequency_penalty: Optional[float] = None,
              presence_penalty: Optional[float] = None, bias_ids: Sequence[int] = (),
-             bias_vals: Sequence[float] = (), stop: Sequence[bytes] = (), json_object: bool = False) -> GenArgs:
+             bias_vals: Sequence[float] = (), stop: Sequence[bytes] = (), json_object: bool = False, n: int = 1) -> GenArgs:
     """None and absent fields take the defaults of a plain greedy request.  A sampled request (temperature > 0) without
     a seed gets a random one here, once, so that a fallback re-admission draws the same tokens; the seed is taken modulo
-    2^64.  Without bias entries the bias arrays are null pointers.  `stop`: the stop sequences as bytes (check_stop).
-    json_object: JSON mode (check_response_format).  Ranges are checked by the native call (check_* raise HTTP 400 first
-    on the router's path)."""
+    2^64.  Without bias entries or stop sequences their arrays are null pointers; otherwise the struct holds the arrays
+    (ctypes keeps what a pointer field is assigned).  `stop`: the stop sequences as bytes (check_stop).  json_object:
+    JSON mode (check_response_format).  n: the number of choices.  Ranges are checked by the native call (check_* raise
+    HTTP 400 first on the router's path)."""
     k = -1 if top_logprobs is None else int(top_logprobs)
     temp = float(temperature or 0.0)
     seed = (secrets.randbits(64) if seed is None else int(seed) % 2**64) if temp else 0
-    b_ids = b_vals = None
+    p = _lib.GenParams(n_choices=n, top_logprobs=k, temperature=temp, top_p=1.0 if top_p is None else float(top_p),
+                       seed=seed, frequency_penalty=float(frequency_penalty or 0.0),
+                       presence_penalty=float(presence_penalty or 0.0), n_bias=len(bias_ids), n_stop=len(stop),
+                       response_format=1 if json_object else 0)
     if len(bias_ids):
-        b_ids = np.ascontiguousarray(np.asarray(bias_ids, dtype=np.int32)).ctypes.data_as(C.POINTER(C.c_int32))
-        b_vals = np.ascontiguousarray(np.asarray(bias_vals, dtype=np.float32)).ctypes.data_as(C.POINTER(C.c_float))
-    tail = (k, temp, 1.0 if top_p is None else float(top_p), seed, float(frequency_penalty or 0.0),
-            float(presence_penalty or 0.0), len(bias_ids), b_ids, b_vals)
-    st = ()
+        p.bias_ids = np.ctypeslib.as_ctypes(np.ascontiguousarray(bias_ids, dtype=np.int32))
+        p.bias_vals = np.ctypeslib.as_ctypes(np.ascontiguousarray(bias_vals, dtype=np.float32))
     if len(stop):
-        blob = np.frombuffer(b"".join(stop), dtype=np.uint8).copy()
+        blob = b"".join(stop)
         off = np.zeros(len(stop) + 1, dtype=np.int32)
         np.cumsum([len(b) for b in stop], out=off[1:])
-        st = (len(stop), blob.ctypes.data_as(C.POINTER(C.c_uint8)), off.ctypes.data_as(C.POINTER(C.c_int32)))
-    return GenArgs(None if k < 0 else k, tail, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0, st,
-                   1 if json_object else 0)
+        p.stop_bytes = (C.c_uint8 * len(blob)).from_buffer_copy(blob)
+        p.stop_off = np.ctypeslib.as_ctypes(off)
+    return GenArgs(p, None if k < 0 else k, (max(1, k) + (1 if temp else 0)) if k >= 0 else 0)
 
 
 def _token_entry(tok: int, logprob: float) -> dict:
@@ -498,8 +488,8 @@ class Router:
 
     def _gw_response(self, res, toks, n_prompt, t_start, detok=True, logprobs=None, n_tokens=None,
                      finish=None) -> ModelResponse:
-        """toks [n choices][max_new] (or one row), logprobs: one `logprobs` object per choice (or None).  With stop
-        sequences, n_tokens / finish: each choice's token count and finish code (else res.n_generated and length)."""
+        """toks [n choices][max_new] (or one row), logprobs: one `logprobs` object per choice (or None).  n_tokens /
+        finish: each choice's token count and finish code (None: res.n_generated and length, as for a plain request)."""
         d = self.cfg.deployments[res.deployment]
         toks = np.atleast_2d(toks)
         n_tokens = [res.n_generated] * len(toks) if n_tokens is None else n_tokens
@@ -550,25 +540,15 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs, n: int = 1) -> int:
-        """In JSON mode: rr_gateway_submit_format; else with stop sequences: rr_gateway_submit_stop; else n > 1:
-        rr_gateway_submit_choices and a request of one choice rr_gateway_submit_processed."""
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs) -> int:
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        p = ids.ctypes.data_as(C.POINTER(C.c_int32))
-        if gen.fmt:
-            rc = _lib.lib.rr_gateway_submit_format(gw, g, p, len(ids), max_new, n, *gen.tail, *gen.format_args(),
-                                                   C.byref(t))
-        elif gen.stop:
-            rc = _lib.lib.rr_gateway_submit_stop(gw, g, p, len(ids), max_new, n, *gen.tail, *gen.stop, C.byref(t))
-        elif n > 1:
-            rc = _lib.lib.rr_gateway_submit_choices(gw, g, p, len(ids), max_new, n, *gen.tail, C.byref(t))
-        else:
-            rc = _lib.lib.rr_gateway_submit_processed(gw, g, p, len(ids), max_new, *gen.tail, C.byref(t))
+        rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                        C.byref(gen.params), C.byref(t))
         if rc == 4:
-            raise self._invalid(len(ids), max_new, n)
+            raise self._invalid(len(ids), max_new, gen.params.n_choices)
         if rc != 0:
             raise self._gw_error(rc, model)
         return t.value
@@ -583,36 +563,29 @@ class Router:
         ids = np.zeros(shape, dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), ids.ctypes.data_as(C.POINTER(C.c_int32))
 
-    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs, n: int = 1):
+    def _completion_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
         t_start = time.perf_counter()
-        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen, n)
+        ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
+        n = gen.params.n_choices
         res = _lib.GatewayResult()
         toks = np.zeros(max_new if n == 1 else (n, max_new), dtype=np.int32)
         lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new, n)
-        n_tok = fin = None
-        if gen.ends_early:               # the choices end on their own: each has its token count and finish reason
-            n_tok, fin = (C.c_int32 * n)(), (C.c_int32 * n)()
-            rc = _lib.lib.rr_gateway_wait_stop(gw, ticket, float(timeout or 0.0), C.byref(res),
-                                               toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p, n_tok, fin)
-        else:
-            wait = _lib.lib.rr_gateway_wait_choices if n > 1 else _lib.lib.rr_gateway_wait_logprobs
-            rc = wait(gw, ticket, float(timeout or 0.0), C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
-                      lp_p, ids_p)
+        n_tok, fin = (C.c_int32 * n)(), (C.c_int32 * n)()
+        rc = _lib.lib.rr_gateway_wait(gw, ticket, float(timeout or 0.0), C.byref(res),
+                                      toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p, n_tok, fin)
         if rc == 6:                      # client-side timeout: give the rows back, count a failure against the deployment
             _lib.lib.rr_gateway_cancel(gw, ticket, 1)
             raise self._gw_error(6, model, res, timeout)
         if rc != 0:
             raise self._gw_error(rc, model, res, timeout)
         content = None
-        n_tok = None if n_tok is None else [min(k, max_new) for k in n_tok]
+        n_tok = [min(k, max_new) for k in n_tok]
         if gen.top is not None:
-            ks = [min(res.n_generated, max_new)] * n if n_tok is None else n_tok
             content = [{"content": logprobs_content(t[:k].tolist(), logprob_pairs(a, b, 0, k), gen.top), "refusal": None}
                        for t, a, b, k in zip(np.atleast_2d(toks), lp.reshape(-1, max_new, gen.width),
-                                             ids.reshape(-1, max_new, gen.width), ks)]
+                                             ids.reshape(-1, max_new, gen.width), n_tok)]
             content = content[0] if n == 1 else content
-        return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content, n_tokens=n_tok,
-                                 finish=None if fin is None else list(fin))
+        return self._gw_response(res, toks, len(prompt_ids), t_start, logprobs=content, n_tokens=n_tok, finish=list(fin))
 
     def _stream_gw(self, gw, model, g, prompt_ids, max_new, timeout, gen: GenArgs):
         ticket = self._gw_submit(gw, g, prompt_ids, max_new, model, gen)
@@ -632,12 +605,11 @@ class Router:
             return label, new, False, ttft, logprobs_content(new, logprob_pairs(lp, ids, a, b), top)
         try:
             while True:
-                _lib.check(_lib.lib.rr_gateway_peek_logprobs(gw, ticket, sent, 0.05, toks.ctypes.data_as(C.POINTER(C.c_int32)),
-                                                             max_new, C.byref(n), C.byref(done), C.byref(res), lp_p, ids_p),
-                           "rr_gateway_peek")
+                _lib.check(_lib.lib.rr_gateway_peek(gw, ticket, sent, 0.05, toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new,
+                                                    C.byref(n), C.byref(done), C.byref(res), lp_p, ids_p), "rr_gateway_peek")
                 if done.value:
-                    rc = _lib.lib.rr_gateway_wait_logprobs(gw, ticket, 1.0, C.byref(res),
-                                                           toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p)
+                    rc = _lib.lib.rr_gateway_wait(gw, ticket, 1.0, C.byref(res), toks.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                  max_new, lp_p, ids_p, None, None)
                     finished = True
                     if rc != 0:
                         raise self._gw_error(rc, model, res, timeout)
@@ -646,7 +618,7 @@ class Router:
                     if res.n_generated > sent:       # the last tokens, with any a pending partial stop match held back
                         yield item(label, sent, res.n_generated, ttft)
                     last = StreamItem((label, [], True, ttft) if top is None else (label, [], True, ttft, []))
-                    last.finish_reason = FINISH_REASONS[res.reserved]
+                    last.finish_reason = FINISH_REASONS[res.finish]
                     yield last
                     return
                 if n.value > sent and res.deployment >= 0:
@@ -683,7 +655,7 @@ class Router:
             res = _lib.GatewayResult()
             left = None if not timeout else max(0.001, timeout - (time.perf_counter() - t0))
             rc = _lib.lib.rr_gateway_wait(gw, tk[i], float(left or 0.0), C.byref(res),
-                                          toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new)
+                                          toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, None, None, None, None)
             if rc == 6:
                 _lib.lib.rr_gateway_cancel(gw, tk[i], 1)
             out[i] = self._gw_response(res, toks, len(prompts[i]), t0, detok=False) if rc == 0 \
@@ -740,7 +712,7 @@ class Router:
         return min((b.vocab for b in self.backends.values()), default=128256)
 
     def _params(self, logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                logit_bias, stop=None, response_format=None) -> GenArgs:
+                logit_bias, stop=None, response_format=None, n: int = 1) -> GenArgs:
         """The request's validated generation parameters.  Only engine replicas have logits to serve logprobs and to mask
         for JSON mode, and a decode loop that stop sequences can end; bias ids must be valid on every replica the request
         may fall back to, and JSON mode needs a token for every byte there."""
@@ -759,7 +731,7 @@ class Router:
             raise BadRequestError(f"`response_format` json_object needs a vocabulary of at least {JSON_MIN_VOCAB} tokens")
         samp = check_sampling(temperature, top_p, seed) or (None, None, None)
         pen = check_penalties(frequency_penalty, presence_penalty, logit_bias, self._vocab()) or (None, None, (), ())
-        return gen_args(top, *samp, *pen, stop=stops, json_object=json_object)
+        return gen_args(top, *samp, *pen, stop=stops, json_object=json_object, n=n)
 
     def completion(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                    max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,
@@ -775,20 +747,20 @@ class Router:
         (rr_op_logit_penalties; the penalties count the tokens generated so far).  Stub backends validate these and keep
         their fixed reply.
         n (1..128, at most the decode rows of the smallest engine replica): n choices of the same prompt, prefilled once
-        (rr_gateway_submit_choices).  Choice i of a sampled request is drawn with seed + i (mod 2^64), so it equals the
+        (rr_gen_params.n_choices).  Choice i of a sampled request is drawn with seed + i (mod 2^64), so it equals the
         n=1 response with that seed; greedy choices are all the greedy response.  usage.completion_tokens sums the
         choices and `_choice_token_ids` holds each choice's tokens (`_token_ids`: choice 0's).
         stop: a string or up to 4 strings of 1..64 bytes of UTF-8 each.  A choice ends where its reply would contain one
-        of them: the content stops before it and finish_reason is "stop" (rr_gateway_submit_stop).  They are matched on
+        of them: the content stops before it and finish_reason is "stop" (rr_gen_params.n_stop).  They are matched on
         the reply's bytes, so the tokens are a prefix of the same request's without `stop`; each choice ends on its own
         and usage.completion_tokens counts the tokens returned.
-        response_format {"type": "json_object"}: JSON mode (rr_gateway_submit_format).  Every token is picked from the
-        logits masked to the JSON grammar, so each choice's content is a prefix of a JSON object; the choice whose object
+        response_format {"type": "json_object"}: JSON mode (rr_gen_params.response_format).  Every token is picked from
+        the logits masked to the JSON grammar, so each choice's content is a prefix of a JSON object; the choice whose object
         closes ends there with finish_reason "stop", one that reaches max_tokens first with "length".  {"type": "text"}
         and None change nothing; `json_schema` and anything else raise BadRequestError (check_response_format)."""
         n = check_n(n)
         gen = self._params(logprobs, top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty,
-                           logit_bias, stop, response_format)
+                           logit_bias, stop, response_format, n)
         g = self.cfg.group_index(model)
         if g < 0:
             raise BadRequestError(f"Invalid model name passed in model={model}")
@@ -797,7 +769,7 @@ class Router:
         max_new = max_tokens or self.default_max_tokens
         if n > self._limits()[2]:
             raise self._invalid(n=n)
-        return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen, n)
+        return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen)
 
     def completion_stream(self, model: str, messages: Optional[Sequence[dict]] = None, timeout: Optional[float] = None,
                           max_tokens: Optional[int] = None, prompt_ids: Optional[Sequence[int]] = None,

@@ -1,4 +1,4 @@
-"""Pure-Python statement of the stop-sequence contract (rr_op_stop_match, rr_engine_submit_stop), for the tests.
+"""Pure-Python statement of the stop-sequence contract (rr_op_stop_match, rr_gen_params.n_stop), for the tests.
 
 The reply text of a token list is what `detokenize` makes of it before decoding: a token t >= 3 is the byte (t - 3) % 256,
 a token < 3 is no text.  Stop sequences are byte strings matched on that text."""

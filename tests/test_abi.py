@@ -36,6 +36,18 @@ def test_struct_sizes_match_header():
     assert C.sizeof(_lib.StubDesc) == 16
 
 
+def test_gen_params_layout_matches_header():
+    """rr_gen_params is 80 bytes with these offsets on every LP64 platform; the library reads it by the header's layout."""
+    from rr_b200 import _lib
+    P = _lib.GenParams
+    assert C.sizeof(P) == 80
+    want = {"n_choices": 0, "top_logprobs": 4, "temperature": 8, "top_p": 12, "seed": 16, "frequency_penalty": 24,
+            "presence_penalty": 28, "n_bias": 32, "n_stop": 36, "bias_ids": 40, "bias_vals": 48, "stop_bytes": 56,
+            "stop_off": 64, "response_format": 72, "reserved": 76}
+    assert {f: getattr(P, f).offset for f, _ in P._fields_} == want
+    assert _lib.GatewayResult.finish.offset == 76 and C.sizeof(_lib.GatewayResult) == 80
+
+
 def test_mt19937_seeding_matches_cpython():
     from rr_b200 import _lib
     for seed in [0, 1, 42, 1234, 2**31 - 1, 2**32 - 1, 2**32, 2**40 + 12345, 2**64 - 1]:

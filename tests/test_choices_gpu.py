@@ -87,7 +87,7 @@ def test_mixed_burst_counts_the_prompt_once():
         eng.close()
 
 
-def test_rows_admission_order_and_cancel():
+def test_rows_admission_order_cancel_and_peek_refusal():
     from rr_b200 import _lib
     B = 8
     eng = _engine(B=B, ctx_max=8192)
@@ -102,12 +102,10 @@ def test_rows_admission_order_and_cancel():
         r1, rx, rq = eng.wait(t1), eng.wait(tx), eng.wait(tq)
         assert r1.status == rx.status == rq.status == 0 and len(rx.choices) == B
         assert rx.t_first_token >= r1.t_done and rq.t_first_token > rx.t_first_token
-        # the single-choice calls refuse an n-choice ticket, which stays in flight
+        # peek refuses an n-choice ticket, which stays in flight
         tc = eng.submit(_prompt(30), 8000, n=4)                     # long enough to be cancelled mid-decode
-        c = _lib.Completion()
-        assert _lib.lib.rr_engine_wait_logprobs(eng._h, tc, 0.01, C.byref(c), None, 0, None, None) == 4
         n, d = C.c_int32(), C.c_int32()
-        assert _lib.lib.rr_engine_peek(eng._h, tc, 0, 0.01, None, 0, C.byref(n), C.byref(d), None) == 4
+        assert _lib.lib.rr_engine_peek(eng._h, tc, 0, 0.01, None, 0, C.byref(n), C.byref(d), None, None, None) == 4
         eng.reset_stats()
         deadline = time.time() + 30
         while eng.stats()["active_rows"] != 4 and time.time() < deadline:
@@ -155,7 +153,7 @@ def _router(backends, **kw):
     return r
 
 
-def test_fallback_readmission_gives_the_same_choices_and_the_trace_replays():
+def test_fallback_readmission_gives_the_same_choices_and_the_gateway_caps_n():
     from rr_b200 import BadRequestError, EngineBackend, _lib
     from test_gateway_gpu import _replay
     bad, good, ref = _engine(fail_prob=0.5, fail_seed=42), _engine(), _engine()
@@ -183,8 +181,8 @@ def test_fallback_readmission_gives_the_same_choices_and_the_trace_replays():
         assert "`n`" in str(ei.value)
         t = C.c_uint64()
         ids = (C.c_int32 * 2)(5, 6)
-        assert _lib.lib.rr_gateway_submit_choices(r._gateway(), 0, ids, 2, 2, 9, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None,
-                                                  C.byref(t)) == 4
+        p = _lib.GenParams(n_choices=9, top_logprobs=-1, top_p=1.0)
+        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 2, 2, C.byref(p), C.byref(t)) == 4
         with pytest.raises(BadRequestError):
             next(r.completion_stream(model="primary", prompt_ids=[5, 6], max_tokens=2, n=2))
     finally:

@@ -134,7 +134,7 @@ def test_mock_replica_failures_walk_the_chain_inside_the_library():
     assert _failures_walk_the_chain(StubBackend(fail_every=2), StubBackend()) == 20
 
 
-def test_mock_replica_descriptors_are_checked_and_logprobs_refused():
+def test_mock_replica_descriptors_are_checked_and_a_logprobs_struct_refused():
     """rr_gateway_create refuses a NULL engine without a valid rr_stub_desc and creates nothing; a gateway with a mock
     replica refuses logprobs at submit (no logits to fill the pairs from) and serves its fixed reply."""
     import ctypes as C
@@ -149,10 +149,11 @@ def test_mock_replica_descriptors_are_checked_and_logprobs_refused():
             assert _lib.lib.rr_gateway_create(r._h, engs, reps, 1, stubs, None, C.byref(gw)) == 4
         assert not gw.value
         ids, t = (C.c_int32 * 3)(5, 6, 7), C.c_uint64()
-        assert _lib.lib.rr_gateway_submit_logprobs(r._gateway(), 0, ids, 3, 4, 0, C.byref(t)) == 4
-        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 3, 4, C.byref(t)) == 0
+        lp = _lib.GenParams(n_choices=1, top_logprobs=0, top_p=1.0)
+        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 3, 4, C.byref(lp), C.byref(t)) == 4
+        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 3, 4, None, C.byref(t)) == 0
         res, toks = _lib.GatewayResult(), (C.c_int32 * 4)()
-        assert _lib.lib.rr_gateway_wait(r._gateway(), t.value, 30.0, C.byref(res), toks, 4) == 0
+        assert _lib.lib.rr_gateway_wait(r._gateway(), t.value, 30.0, C.byref(res), toks, 4, None, None, None, None) == 0
         assert list(toks) == [3, 4, 5, 6] and res.n_generated == 4 and res.deployment == 0
     finally:
         r.close()

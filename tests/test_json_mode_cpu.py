@@ -176,13 +176,15 @@ def test_check_response_format():
         assert ei.value.status_code == 400 and "response_format" in ei.value.message, bad
 
 
-def test_gen_args_json_object():
-    g = gen_args(json_object=True)
-    assert g.fmt == 1 and g.tail == gen_args().tail and g.stop == ()
-    assert g.ends_early and not gen_args().ends_early and gen_args(stop=[b"x"]).ends_early
-    assert g.format_args() == (0, None, None, 1)
-    st = gen_args(stop=[b"ab"], json_object=True)
-    assert st.format_args()[0] == 1 and st.format_args()[-1] == 1
+def test_gen_args_json_object_fills_response_format():
+    g, plain = gen_args(json_object=True).params, gen_args().params
+    assert g.response_format == 1 and plain.response_format == 0
+    for p in (g, plain):              # otherwise a plain request: greedy, one choice, nothing else asked for
+        assert (p.n_choices, p.top_logprobs, p.temperature, p.top_p, p.seed, p.frequency_penalty, p.presence_penalty,
+                p.n_bias, p.n_stop) == (1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, 0)
+        assert not (p.bias_ids or p.bias_vals or p.stop_bytes or p.stop_off)
+    st = gen_args(stop=[b"ab"], json_object=True).params
+    assert st.n_stop == 1 and st.response_format == 1
 
 
 def test_top_logprobs_drop_minus_infinity():
@@ -254,18 +256,17 @@ def test_http_forwards_response_format_only_when_present_and_not_text():
     assert _chunks(res)[-1]["choices"][0]["finish_reason"] == "length" and r.calls[-1] == {}
 
 
-def test_ctypes_table_of_the_json_calls():
+def test_submit_takes_the_format_in_the_param_struct():
     from rr_b200 import _lib
     P = _lib.PROTOTYPES
-    for name, base in (("rr_engine_submit_format", "rr_engine_submit_stop"),
-                       ("rr_gateway_submit_format", "rr_gateway_submit_stop")):
-        assert P[name][0] is C.c_int and P[name][1] == P[base][1][:-1] + [C.c_int] + P[base][1][-1:]
+    # the format goes in through the parameter struct (its layout: tests/test_abi.py)
+    for name in ("rr_engine_submit", "rr_gateway_submit"):
+        assert P[name][0] is C.c_int and C.POINTER(_lib.GenParams) in P[name][1]
     assert len(P["rr_op_json_mask"][1]) == 8 and len(P["rr_op_json_advance"][1]) == 9
     # the raw arguments are checked before anything is queued or launched: no engine or GPU is needed to be refused
-    t = C.c_uint64()
-    assert _lib.lib.rr_engine_submit_format(None, None, 0, 0, 1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None, 0, None, None,
-                                            1, C.byref(t)) == 4
-    assert _lib.lib.rr_gateway_submit_format(None, 0, None, 0, 0, 1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None, 0, None,
-                                             None, 1, C.byref(t)) == 4
+    t = C.c_uint64(77)
+    p = _lib.GenParams(n_choices=1, top_logprobs=-1, top_p=1.0, response_format=1)
+    assert _lib.lib.rr_engine_submit(None, None, 0, 0, C.byref(p), C.byref(t)) == 4
+    assert _lib.lib.rr_gateway_submit(None, 0, None, 0, 0, C.byref(p), C.byref(t)) == 4 and t.value == 77
     assert _lib.lib.rr_op_json_mask(None, 8, 1, 8, None, None, None, None) == 4
     assert _lib.lib.rr_op_json_advance(0, None, None, None, None, None, None, None, None) == 4

@@ -522,7 +522,7 @@ def test_fallback_readmission_gives_the_same_reply_and_the_trace_replays():
         r.close(); bad.close(); good.close(); ref.close()
 
 
-def test_refusals_mock_replicas_and_small_vocabularies():
+def test_refusals_mock_replicas_and_small_vocabularies_via_gen_params():
     from rr_b200 import BadRequestError, EngineBackend, SPECS, StubBackend, _lib as L
     r = _router({0: StubBackend(), 1: StubBackend()})
     try:
@@ -530,8 +530,8 @@ def test_refusals_mock_replicas_and_small_vocabularies():
             r.completion(model="primary", prompt_ids=[5, 6, 7], max_tokens=4, response_format=JS)
         assert ei.value.status_code == 400 and "response_format" in ei.value.message
         t, ids = C.c_uint64(), (C.c_int32 * 2)(5, 6)
-        assert L.lib.rr_gateway_submit_format(r._gateway(), 0, ids, 2, 2, 1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None, 0,
-                                              None, None, 1, C.byref(t)) == 4
+        p = L.GenParams(n_choices=1, top_logprobs=-1, top_p=1.0, response_format=1)
+        assert L.lib.rr_gateway_submit(r._gateway(), 0, ids, 2, 2, C.byref(p), C.byref(t)) == 4
         assert len(r.completion(model="primary", prompt_ids=[5, 6, 7], max_tokens=4,
                                 response_format={"type": "text"})._token_ids) == 4
     finally:

@@ -14,7 +14,7 @@ from rr_b200.server import create_app
 RR_INVALID_ARGUMENT = 4
 
 
-def test_logprobs_entry_points_validate_before_touching_the_device():
+def test_logprobs_entry_points_and_unified_calls_validate_before_touching_the_device():
     from rr_b200 import _lib
     L = _lib.lib
     dummy = C.c_void_p(16)                       # never dereferenced: every call below is rejected first
@@ -30,13 +30,15 @@ def test_logprobs_entry_points_validate_before_touching_the_device():
         assert op(**bad) == RR_INVALID_ARGUMENT, bad
     t = C.c_uint64(77)
     ids = (C.c_int32 * 4)(1, 2, 3, 4)
-    assert L.rr_engine_submit_logprobs(None, ids, 4, 8, 3, C.byref(t)) == RR_INVALID_ARGUMENT
-    assert L.rr_engine_wait_logprobs(None, 1, 0.0, None, None, 0, None, None) == RR_INVALID_ARGUMENT
+    p = _lib.GenParams(n_choices=1, top_logprobs=3, top_p=1.0)
+    for params in (None, C.byref(p)):
+        assert L.rr_engine_submit(None, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
+        assert L.rr_gateway_submit(None, 0, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
+    assert L.rr_engine_wait(None, 1, 0.0, None, None, 0, None, None, None, None) == RR_INVALID_ARGUMENT
     n, d = C.c_int32(-1), C.c_int32(-1)
-    assert L.rr_engine_peek_logprobs(None, 1, 0, 0.0, None, 0, C.byref(n), C.byref(d), None, None, None) == RR_INVALID_ARGUMENT
-    assert L.rr_gateway_submit_logprobs(None, 0, ids, 4, 8, 3, C.byref(t)) == RR_INVALID_ARGUMENT
-    assert L.rr_gateway_wait_logprobs(None, 1, 0.0, None, None, 0, None, None) == RR_INVALID_ARGUMENT
-    assert L.rr_gateway_peek_logprobs(None, 1, 0, 0.0, None, 0, C.byref(n), C.byref(d), None, None, None) == RR_INVALID_ARGUMENT
+    assert L.rr_engine_peek(None, 1, 0, 0.0, None, 0, C.byref(n), C.byref(d), None, None, None) == RR_INVALID_ARGUMENT
+    assert L.rr_gateway_wait(None, 1, 0.0, None, None, 0, None, None, None, None) == RR_INVALID_ARGUMENT
+    assert L.rr_gateway_peek(None, 1, 0, 0.0, None, 0, C.byref(n), C.byref(d), None, None, None) == RR_INVALID_ARGUMENT
     assert t.value == 77 and (n.value, d.value) == (-1, -1)
 
 

@@ -126,7 +126,7 @@ def test_http_rejects_invalid_values_with_400(stream, extra):
 
 
 # ---------------------------------------------------------------- C entry points
-def test_penalty_entry_points_validate_before_touching_the_device():
+def test_penalty_entry_points_and_unified_submit_validate_before_touching_the_device():
     from rr_b200 import _lib
     L = _lib.lib
     dummy = C.c_void_p(16)                       # never dereferenced: every call below is rejected first
@@ -145,8 +145,9 @@ def test_penalty_entry_points_validate_before_touching_the_device():
     t = C.c_uint64(77)
     ids = (C.c_int32 * 4)(1, 2, 3, 4)
     b_ids, b_vals = (C.c_int32 * 1)(5), (C.c_float * 1)(1.0)
-    assert L.rr_engine_submit_processed(None, ids, 4, 8, -1, 0.0, 1.0, 0, 0.5, 0.0, 1, b_ids, b_vals,
-                                        C.byref(t)) == RR_INVALID_ARGUMENT
-    assert L.rr_gateway_submit_processed(None, 0, ids, 4, 8, -1, 0.0, 1.0, 0, 0.5, 0.0, 1, b_ids, b_vals,
-                                         C.byref(t)) == RR_INVALID_ARGUMENT
+    p = _lib.GenParams(n_choices=1, top_logprobs=-1, top_p=1.0, frequency_penalty=0.5, n_bias=1, bias_ids=b_ids,
+                       bias_vals=b_vals)
+    for params in (None, C.byref(p)):
+        assert L.rr_engine_submit(None, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
+        assert L.rr_gateway_submit(None, 0, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
     assert t.value == 77

@@ -227,7 +227,7 @@ def _tiny(**kw):
                   ctx_max=512, max_prefill_tokens=4096, **kw)
 
 
-def test_no_leaks_between_requests_and_no_effect_on_plain_rows():
+def test_no_leaks_between_requests_and_no_effect_on_plain_or_zero_param_rows():
     from rr_b200 import SPECS
     vocab = SPECS["tiny"].vocab
     prompt = _prompts(1, vocab, 3, 20, 30)[0]
@@ -250,9 +250,12 @@ def test_no_leaks_between_requests_and_no_effect_on_plain_rows():
         assert eng.wait(eng.submit(prompt, N, frequency_penalty=0, presence_penalty=0.0, logit_bias={})).tokens == plain
         ids = np.asarray(prompt, dtype=np.int32)
         t = C.c_uint64()
-        assert _lib().rr_engine_submit_processed(eng._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), N, -1, 0.0,
-                                                 1.0, 0, 0.0, 0.0, 0, None, None, C.byref(t)) == 0
-        assert eng.wait(t.value).tokens == plain
+        from rr_b200._lib import GenParams
+        zero = GenParams(n_choices=1, top_logprobs=-1, top_p=1.0)
+        for p in (None, C.byref(zero)):
+            assert _lib().rr_engine_submit(eng._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), N, p,
+                                           C.byref(t)) == 0
+            assert eng.wait(t.value).tokens == plain
         # a 64-request burst: plain rows bit-identical with and without processed rows beside them
         burst = _prompts(64, vocab, 17, 5, 40)
         base = [eng.submit(p, N) for p in burst]

@@ -135,7 +135,7 @@ def test_http_rejects_invalid_values_with_400(stream, extra):
 
 
 # ---------------------------------------------------------------- C entry points
-def test_sampling_entry_points_validate_before_touching_the_device():
+def test_sampling_entry_points_and_unified_submit_validate_before_touching_the_device():
     from rr_b200 import _lib
     L = _lib.lib
     dummy = C.c_void_p(16)                       # never dereferenced: every call below is rejected first
@@ -151,6 +151,8 @@ def test_sampling_entry_points_validate_before_touching_the_device():
         assert op(**bad) == RR_INVALID_ARGUMENT, bad
     t = C.c_uint64(77)
     ids = (C.c_int32 * 4)(1, 2, 3, 4)
-    assert L.rr_engine_submit_sampled(None, ids, 4, 8, -1, 0.7, 0.9, 1, C.byref(t)) == RR_INVALID_ARGUMENT
-    assert L.rr_gateway_submit_sampled(None, 0, ids, 4, 8, -1, 0.7, 0.9, 1, C.byref(t)) == RR_INVALID_ARGUMENT
+    p = _lib.GenParams(n_choices=1, top_logprobs=-1, temperature=0.7, top_p=0.9, seed=1)
+    for params in (None, C.byref(p)):
+        assert L.rr_engine_submit(None, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
+        assert L.rr_gateway_submit(None, 0, ids, 4, 8, params, C.byref(t)) == RR_INVALID_ARGUMENT
     assert t.value == 77

@@ -1,8 +1,10 @@
 """CPU: the `stop` request field -- its validation, the oracle of the byte-matching contract on hand-written cases, the
 HTTP front with a recording router, and the ctypes side of the calls it added."""
 import ctypes as C
+import gc
 import json
 
+import numpy as np
 import pytest
 from starlette.testclient import TestClient
 
@@ -27,12 +29,23 @@ def test_check_stop_accepts_openai_shapes_only():
         assert ei.value.status_code == 400 and word in ei.value.message, bad
 
 
-def test_gen_args_keeps_the_plain_tail_and_adds_the_stop_arrays():
-    assert gen_args().stop == () and gen_args(stop=[]).stop == ()
-    g = gen_args(stop=[b"ab", b"c"])
-    assert g.tail == gen_args().tail
-    n, blob, off = g.stop
-    assert n == 2 and bytes(blob[:3]) == b"abc" and off[:3] == [0, 2, 3]
+def test_gen_args_fills_the_stop_fields_and_keeps_the_rest_plain():
+    plain = gen_args().params
+    for p in (plain, gen_args(stop=[]).params):
+        assert p.n_stop == 0 and not p.stop_bytes and not p.stop_off
+    g = gen_args(stop=[b"ab", b"c"]).params
+    same = ("n_choices", "top_logprobs", "temperature", "top_p", "seed", "frequency_penalty", "presence_penalty", "n_bias",
+            "response_format")
+    assert [getattr(g, f) for f in same] == [getattr(plain, f) for f in same] and not g.bias_ids
+    assert g.n_stop == 2 and bytes(g.stop_bytes[:3]) == b"abc" and g.stop_off[:3] == [0, 2, 3]
+
+
+def test_gen_args_struct_keeps_its_arrays_alive():
+    g = gen_args(stop=[b"ab", b"c"], bias_ids=[5, 9], bias_vals=[1.5, -2.0]).params
+    gc.collect()
+    junk = [np.full(64, -1, dtype=np.int32) for _ in range(256)]      # takes the memory of any array freed above
+    assert g.bias_ids[:2] == [5, 9] and g.bias_vals[:2] == [1.5, -2.0] and len(junk) == 256
+    assert bytes(g.stop_bytes[:3]) == b"abc" and g.stop_off[:3] == [0, 2, 3]
 
 
 def test_oracle_cuts_at_the_first_match_and_keeps_what_precedes_it():
@@ -139,19 +152,20 @@ def test_http_forwards_stop_only_when_present_and_reports_the_finish_reason():
     assert _chunks(res)[-1]["choices"][0]["finish_reason"] == "length" and r.calls[-1] == {}
 
 
-def test_ctypes_table_of_the_stop_calls():
+def test_submit_takes_the_stops_in_the_param_struct_and_wait_returns_each_choice():
     from rr_b200 import _lib
     P = _lib.PROTOTYPES
-    u8p, i32p = C.POINTER(C.c_uint8), C.POINTER(C.c_int32)
-    for name, base in (("rr_engine_submit_stop", "rr_engine_submit_choices"),
-                       ("rr_gateway_submit_stop", "rr_gateway_submit_choices")):
-        assert P[name][0] is C.c_int and P[name][1] == P[base][1][:-1] + [C.c_int, u8p, i32p] + P[base][1][-1:]
-    for name, base in (("rr_engine_wait_stop", "rr_engine_wait_choices"), ("rr_gateway_wait_stop", "rr_gateway_wait_choices")):
-        assert P[name] == (C.c_int, P[base][1] + [i32p, i32p])
+    i32p = C.POINTER(C.c_int32)
+    # the sequences go in through the parameter struct; every choice's token count and finish reason come back from wait
+    for name in ("rr_engine_submit", "rr_gateway_submit"):
+        assert P[name][0] is C.c_int and P[name][1][-2:] == [C.POINTER(_lib.GenParams), C.POINTER(C.c_uint64)]
+    for name in ("rr_engine_wait", "rr_gateway_wait"):
+        assert P[name][0] is C.c_int and P[name][1][-4:] == [C.POINTER(C.c_float), i32p, i32p, i32p]
     assert len(P["rr_op_stop_match"][1]) == 13
     assert C.sizeof(_lib.Completion) == 48 and C.sizeof(_lib.GatewayResult) == 80
     # the raw arguments are checked before anything is queued: no engine is needed to be refused
-    t = C.c_uint64()
-    assert _lib.lib.rr_engine_submit_stop(None, None, 0, 0, 1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None, 1, None, None,
-                                          C.byref(t)) == 4
+    t = C.c_uint64(77)
+    p = _lib.GenParams(n_choices=1, top_logprobs=-1, top_p=1.0, n_stop=1)
+    assert _lib.lib.rr_engine_submit(None, None, 0, 0, C.byref(p), C.byref(t)) == 4
+    assert _lib.lib.rr_gateway_submit(None, 0, None, 0, 0, C.byref(p), C.byref(t)) == 4 and t.value == 77
     assert _lib.lib.rr_op_stop_match(None, 8, None, None, None, None, None, None, None, None, None, 1, None) == 4

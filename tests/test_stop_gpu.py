@@ -434,7 +434,7 @@ def test_fallback_readmission_gives_the_same_cut_reply_and_the_trace_replays():
         r.close(); bad.close(); good.close(); ref.close()
 
 
-def test_mock_replicas_refuse_stop_and_the_prefix_cache_does_not_change_the_cut():
+def test_mock_replicas_refuse_a_stop_struct_and_the_prefix_cache_does_not_change_the_cut():
     from rr_b200 import BadRequestError, EngineBackend, StubBackend, _lib
     r = _router({0: StubBackend(), 1: StubBackend()})
     try:
@@ -443,8 +443,8 @@ def test_mock_replicas_refuse_stop_and_the_prefix_cache_does_not_change_the_cut(
         assert ei.value.status_code == 400 and "`stop`" in ei.value.message
         t, ids, off = C.c_uint64(), (C.c_int32 * 2)(5, 6), (C.c_int32 * 2)(0, 1)
         by = (C.c_uint8 * 1)(97)
-        assert _lib.lib.rr_gateway_submit_stop(r._gateway(), 0, ids, 2, 2, 1, -1, 0.0, 1.0, 0, 0.0, 0.0, 0, None, None, 1, by,
-                                               off, C.byref(t)) == 4
+        p = _lib.GenParams(n_choices=1, top_logprobs=-1, top_p=1.0, n_stop=1, stop_bytes=by, stop_off=off)
+        assert _lib.lib.rr_gateway_submit(r._gateway(), 0, ids, 2, 2, C.byref(p), C.byref(t)) == 4
         assert len(r.completion(model="primary", prompt_ids=[5, 6, 7], max_tokens=4)._token_ids) == 4
     finally:
         r.close()
