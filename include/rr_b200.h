@@ -308,6 +308,30 @@ int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const void* v_
  * destination that is also a source in the same call. */
 int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
                          const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies, void* stream);
+/* Paged KV cache, as the engine runs it: the four entry points below take the arguments of rr_op_decode_attn_qkv,
+ * rr_op_prefill_qkv, rr_op_prefill_attn_cached and rr_op_kv_copy_prefix plus a page table.  The caches are
+ * [n_pages][n_kv_heads][64][128] bf16 (per layer for the copy), and position p of slot s lives on page
+ * page_table[s * pages_per_slot + p / 64] (device int32 [n_slots][pages_per_slot]), at row p % 64 of the page.  ctx_max
+ * must be 64 x pages_per_slot.  Table entries are trusted, as slot indices are: each must be in [0, n_pages).  Only the
+ * table rows of the slots named (slot >= 0, seq_slot, src / dst) are read, so the table needs n_slots rows.  Returns
+ * RR_INVALID_ARGUMENT before touching the device for a null page_table, pages_per_slot or n_pages below 1, or ctx_max
+ * other than 64 x pages_per_slot; otherwise for whatever the counterpart rejects.  Results, bit for bit: the
+ * counterpart's over the cache gathered through the table. */
+int rr_op_decode_attn_qkv_paged(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads,
+                                int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
+                                const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
+int rr_op_prefill_qkv_paged(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                            int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
+                            const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
+                            const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
+int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                    const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                                    int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
+                                    const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
+int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                               const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies,
+                               const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
 /* Fused decode MLP, one launch exactly as the engine runs it for a batch of `rows` (tile width, K slices, grid and
  * schedule from the engine's rules; env RR_MLP_STATIC / RR_NO_TMA_EPI are read per call):
  *   act[b, n]       = bf16(SiLU(xn[b] . gate[n]) * (xn[b] . up[n]))                        bf16 [rows, inter]
@@ -405,12 +429,19 @@ typedef struct rr_engine rr_engine;
 typedef struct rr_engine_opts {
     int32_t device;
     int32_t max_batch;            /* decode rows / KV slots (<= 256) */
-    int32_t ctx_max;              /* tokens per KV slot */
+    int32_t ctx_max;              /* tokens per request (prompt + max_new_tokens), a multiple of 64 */
     int32_t max_prefill_tokens;   /* tokens per prefill chunk */
     int32_t use_cuda_graph;       /* capture the decode step */
     int32_t fail_seed;            /* fault injection: seed of the Bernoulli failure mask */
     float fail_prob;              /* fault injection: P(request fails) (BASELINE config #4) */
-    int32_t reserved[4];          /* ignored (pass zeros); keeps prefix_cache at offset 44 */
+    int32_t kv_cache_tokens;      /* offset 28: the KV cache, a pool of 64-token pages shared by the decode rows.  0 =
+                                     max_batch x ctx_max (every row can hold ctx_max tokens at once, the pool never binds);
+                                     otherwise a multiple of 64 in [ctx_max, max_batch x ctx_max], else rr_engine_create
+                                     returns RR_INVALID_ARGUMENT before any CUDA call.  Each choice of a request reserves
+                                     ceil((n_prompt + max_new_tokens) / 64) pages when it is admitted; a request that does
+                                     not fit waits at the head of the queue (nothing overtakes it).  Memory: 2 x n_layers x
+                                     kv_cache_tokens x n_kv_heads x 256 B. */
+    int32_t reserved[3];          /* ignored (pass zeros); keeps prefix_cache at offset 44 */
     int32_t prefix_cache;         /* 1: prompt prefix caching.  A slot keeps the prompt KV its last prefill wrote; a new prompt
                                      sharing >= 64 leading tokens with one is prefilled from there on (the prefix is copied
                                      when that slot is busy).  Tokens and logits are bit-identical to a cold prefill.  Off
@@ -421,7 +452,9 @@ int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w,
                      const rr_engine_opts* opts, rr_engine** out);
 void rr_engine_destroy(rr_engine* e);
 
-/* Low-level synchronous steps (parity tests).  Host buffers.  Both forget every retained prompt prefix (prefix_cache).
+/* Low-level synchronous steps (parity tests).  Host buffers.  Both forget every retained prompt prefix (prefix_cache), and
+ * both first give each named slot the KV pages of the positions they write (positions [0, prompt length) / [0, pos]); they
+ * return RR_INVALID_ARGUMENT when the free pages do not cover that.  A slot keeps those pages until a request takes it.
  * prefill: n_seqs prompts concatenated in `ids`; seq_start[n_seqs+1]; slots[n_seqs] = KV slots.
  *          Writes first generated token per prompt to first_tok[n_seqs].
  *          If logits_out != NULL: fp32 [n_seqs, vocab] last-position logits. */
@@ -498,7 +531,8 @@ typedef struct rr_gen_params {
  * A choice that reaches max_new_tokens first finishes with reason 0 (length), in JSON mode with a valid prefix.  The
  * request is done when every choice has finished.
  * RR_INVALID_ARGUMENT, before anything is queued and with *ticket untouched, for a NULL engine, prompt or ticket,
- * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max, a prompt longer than a prefill chunk, a
+ * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max, a prompt longer than a prefill chunk,
+ * n_choices x ceil((n_prompt + max_new_tokens) / 64) x 64 above kv_cache_tokens (the request could never be admitted), a
  * prompt token outside [0, vocab), and for parameters outside these ranges (NaN is outside every range):
  * 1 <= n_choices <= max_batch; -1 <= top_logprobs <= 20; 0 <= temperature <= 2; 0 <= top_p <= 1; -2 <= penalties <= 2;
  * 0 <= n_bias <= 300 with non-null arrays when n_bias > 0, unique bias ids in [0, vocab) and -100 <= bias values <= 100;
@@ -553,6 +587,10 @@ typedef struct rr_engine_stats {
     uint64_t prefix_hits, prefix_cached_tokens, kv_copy_tokens;
 } rr_engine_stats;
 int rr_engine_get_stats(rr_engine* e, rr_engine_stats* out);
+/* The KV page pool: *pages_total = kv_cache_tokens / 64, *pages_free = pages no slot holds.  A slot keeps the pages of its
+ * retained prompt prefix (prefix_cache) after its request; otherwise every page is free once the engine is idle.
+ * RR_INVALID_ARGUMENT for a NULL argument. */
+int rr_engine_kv_usage(rr_engine* e, int32_t* pages_total, int32_t* pages_free);
 int rr_engine_reset_stats(rr_engine* e);
 
 /* ================================================================================================
@@ -625,8 +663,9 @@ int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
  * logits to fill pairs from or to mask and no decode loop to cut; RR_INVALID_ARGUMENT for a NULL prompt or ticket;
  * RR_NO_GROUP for an unknown group; RR_INVALID_ARGUMENT (HTTP 400) for n_prompt or max_new_tokens below 1, n_choices
  * outside 1..the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices
- * copies of its reply), prompt + max_new_tokens beyond a replica's context, a prompt beyond its prefill chunk and a bad
- * token id. */
+ * copies of its reply), prompt + max_new_tokens beyond a replica's context, a prompt beyond its prefill chunk,
+ * n_choices x ceil((prompt + max_new_tokens) / 64) x 64 beyond the smallest KV pool of the gateway's engines (a mock
+ * replica sets no KV limit) and a bad token id. */
 int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                       const rr_gen_params* p, uint64_t* ticket);
 /* A closed burst of plain requests (greedy, one choice) as one contiguous block of the admission trace (declare_burst != 0

@@ -79,7 +79,8 @@ class ModelWeights(C.Structure):
 class EngineOpts(C.Structure):
     _fields_ = [("device", C.c_int32), ("max_batch", C.c_int32), ("ctx_max", C.c_int32),
                 ("max_prefill_tokens", C.c_int32), ("use_cuda_graph", C.c_int32),
-                ("fail_seed", C.c_int32), ("fail_prob", C.c_float), ("reserved", C.c_int32 * 4),
+                ("fail_seed", C.c_int32), ("fail_prob", C.c_float), ("kv_cache_tokens", C.c_int32),
+                ("reserved", C.c_int32 * 3),
                 ("prefix_cache", C.c_int32)]
 
 
@@ -177,12 +178,21 @@ PROTOTYPES = {
     "rr_op_prefill_attn_cached": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.c_int, C.c_float, vp]),
     "rr_op_kv_copy_prefix": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int, vp]),
+    "rr_op_prefill_attn_cached_paged": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                  C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]),
+    "rr_op_kv_copy_prefix_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int,
+                                             vp, C.c_int, C.c_int, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp]),
+    "rr_op_decode_attn_qkv_paged": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
+                                              C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp, C.c_int, C.c_int,
+                                              vp]),
     "rr_op_add_rmsnorm_pf": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp]),
     "rr_op_prefill_qkv": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                     C.c_float, vp, vp, vp, vp, vp, c_i32p, vp]),
+    "rr_op_prefill_qkv_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                          C.c_float, C.c_float, vp, vp, vp, vp, vp, c_i32p, vp, C.c_int, C.c_int, vp]),
     "rr_op_prefill_gemm": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp,
                                      C.c_int, C.c_int, C.c_float, vp, vp, vp, C.c_int, vp]),
     "rr_engine_create": (C.c_int, [C.POINTER(ModelDesc), C.POINTER(ModelWeights),
@@ -200,6 +210,7 @@ PROTOTYPES = {
     "rr_engine_now": (C.c_double, [vp]),
     "rr_engine_get_stats": (C.c_int, [vp, C.POINTER(EngineStats)]),
     "rr_engine_reset_stats": (C.c_int, [vp]),
+    "rr_engine_kv_usage": (C.c_int, [vp, c_i32p, c_i32p]),
     "rr_engine_cancel": (C.c_int, [vp, C.c_uint64]),
     "rr_gateway_create": (C.c_int, [vp, C.POINTER(vp), c_i32p, C.c_int, C.POINTER(StubDesc), C.POINTER(GatewayOpts),
                                     C.POINTER(vp)]),

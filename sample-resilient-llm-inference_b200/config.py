@@ -8,7 +8,10 @@ YAML anchors / merge keys (`<<: *aws-defaults`, :40) are resolved by PyYAML.  AW
 `router_settings.routing_strategy_args` takes litellm's latency-based-routing keys (`lowest_latency_buffer`,
 `max_latency_list_size`, `ttl`).  Local extensions: `litellm_params.gpu: N` pins a deployment to a replica; `litellm_params.model:
 b200/<spec>` names an on-box model (models.SPECS) instead of `bedrock/<id>`; `litellm_params.prefix_cache: true` turns on
-prompt prefix caching in the replica (deployments on one GPU share its engine, so they must agree).
+prompt prefix caching in the replica; `litellm_params.context_window: N` is the longest request (prompt + max_tokens, in
+tokens) the replica serves, a positive multiple of 64, default 1024; `litellm_params.kv_cache_tokens: N` sizes the replica's
+KV cache, a pool of 64-token pages its decode rows share: a multiple of 64 in [context_window, max_batch x context_window],
+default the full max_batch x context_window.  Deployments on one GPU share its engine, so they must agree on all three.
 """
 from __future__ import annotations
 
@@ -43,6 +46,8 @@ class DeploymentCfg:
     weight: int = -1           # simple-shuffle weight (litellm_params.weight / rpm / tpm), -1 = unset
     gpu: int = 0
     prefix_cache: bool = False  # litellm_params.prefix_cache: the replica reuses cached prompt prefixes
+    context_window: int = 1024  # litellm_params.context_window: prompt + max_tokens of one request, a multiple of 64
+    kv_cache_tokens: Optional[int] = None   # litellm_params.kv_cache_tokens: the KV pool; None = max_batch x context_window
     params: Dict[str, Any] = field(default_factory=dict)
 
     @property
@@ -130,13 +135,22 @@ def build_config(model_list: List[dict], router_settings: Optional[dict] = None,
         pc = lp.get("prefix_cache", False)
         if not isinstance(pc, bool):
             raise ValueError(f"model_list[{i}].litellm_params.prefix_cache must be true or false, got {pc!r}")
+        cw = lp.get("context_window", 1024)
+        if isinstance(cw, bool) or not isinstance(cw, int) or cw < 64 or cw % 64:
+            raise ValueError(f"model_list[{i}].litellm_params.context_window must be a positive multiple of 64, got {cw!r}")
+        kv = lp.get("kv_cache_tokens")
+        if kv is not None and (isinstance(kv, bool) or not isinstance(kv, int) or kv < cw or kv % 64):
+            raise ValueError(f"model_list[{i}].litellm_params.kv_cache_tokens must be a multiple of 64 of at least "
+                             f"context_window ({cw}), got {kv!r}")
         deps.append(DeploymentCfg(index=i, model_name=name, model=lp["model"], group=groups.index(name),
-                                  rpm=rpm, tpm=tpm, gpu=int(lp.get("gpu", 0)), prefix_cache=pc, params=lp))
-    for d in deps:                       # one engine per GPU: its deployments share the setting
+                                  rpm=rpm, tpm=tpm, gpu=int(lp.get("gpu", 0)), prefix_cache=pc, context_window=cw,
+                                  kv_cache_tokens=kv, params=lp))
+    for d in deps:                       # one engine per GPU: its deployments share the settings
         first = next(x for x in deps if x.gpu == d.gpu)
-        if d.prefix_cache != first.prefix_cache:
-            raise ValueError(f"model_list[{first.index}] and model_list[{d.index}] share gpu {d.gpu} but disagree on "
-                             "litellm_params.prefix_cache")
+        for key in ("prefix_cache", "context_window", "kv_cache_tokens"):
+            if getattr(d, key) != getattr(first, key):
+                raise ValueError(f"model_list[{first.index}] and model_list[{d.index}] share gpu {d.gpu} but disagree on "
+                                 f"litellm_params.{key}")
     # simple-shuffle weights: the first of weight / rpm / tpm present in the litellm_params of the
     # group's first deployment decides the key for the whole group (oracle/router.py header).
     for g in range(len(groups)):

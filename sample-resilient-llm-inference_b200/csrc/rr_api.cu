@@ -312,10 +312,11 @@ RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_ca
 // Decode attention as the engine runs it (rr_engine_create): RoPE and the KV append fused in, q / k / v summed from the QKV
 // GEMM's fp32 split-K planes, the engine's scale, kv-split rule and RoPE table; RR_ATTN_NO_TRIM is read per call.  The
 // table and the split-KV workspace live in stream-ordered scratch memory.
-RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
-                                 void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads,
-                                 int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
-                                 void* stream) {
+// page_table == nullptr: the slot-contiguous cache of n_slots slots; else n_pages 64-token pages (kv_row).
+static int decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache, void* v_cache,
+                           void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads, int n_kv_heads,
+                           int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits, const int32_t* page_table,
+                           int pages_per_slot, int n_pages, void* stream) {
     if (!qkv || !k_cache || !v_cache || !out || !slot || !pos || !kv_splits) return RR_INVALID_ARGUMENT;
     if (rows < 1 || n_slots < 1 || n_splits < 1) return RR_INVALID_ARGUMENT;
     if (n_kv_heads <= 0 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
@@ -331,7 +332,8 @@ RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split
     a.scale = 1.0f / sqrtf((float)head_dim);
     a.kv_splits = pick_kv_splits(rows, n_kv_heads); a.ws = nullptr;
     a.fuse_rope = 1; a.qkv = mk_part(qkv, 0, n_splits, split_stride, ld); a.head_dim = head_dim;
-    { int rcm = decode_attn_make_maps(&a, n_slots); if (rcm != RR_OK) return rcm; }
+    a.page_table = page_table; a.pages_per_slot = pages_per_slot;
+    { int rcm = decode_attn_make_maps(&a, page_table ? n_pages : n_slots); if (rcm != RR_OK) return rcm; }
     cudaStream_t st = (cudaStream_t)stream;
     float2* table = nullptr;
     float* ws = nullptr;
@@ -351,6 +353,30 @@ RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split
     return check_last();
 }
 
+RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                 void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads,
+                                 int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
+                                 void* stream) {
+    return decode_attn_qkv(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads, n_kv_heads,
+                           head_dim, ctx_max, n_slots, theta, kv_splits, nullptr, 0, 0, stream);
+}
+
+// The paged entry points' own checks, made before their counterpart's: a page table, at least one page per slot and in the
+// pool, and ctx_max = KV_PAGE x pages_per_slot.
+static bool paged_ok(const int32_t* page_table, int pages_per_slot, int n_pages, int ctx_max) {
+    return page_table && pages_per_slot >= 1 && n_pages >= 1 && (long long)ctx_max == (long long)KV_PAGE * pages_per_slot;
+}
+
+RR_API int rr_op_decode_attn_qkv_paged(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                       void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows,
+                                       int n_heads, int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta,
+                                       int* kv_splits, const int32_t* page_table, int pages_per_slot, int n_pages,
+                                       void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return decode_attn_qkv(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads, n_kv_heads,
+                           head_dim, ctx_max, n_slots, theta, kv_splits, page_table, pages_per_slot, n_pages, stream);
+}
+
 // Layer 0's RMSNorm of a prefill chunk in the deferred form, the only form run_prefill launches.
 RR_API int rr_op_add_rmsnorm_pf(float* x, const void* w, void* xn, int rows, int hidden, float eps, float* rowss_out,
                                 int n_part_out, void* stream) {
@@ -364,10 +390,10 @@ RR_API int rr_op_add_rmsnorm_pf(float* x, const void* w, void* xn, int rows, int
 // The prefill QKV projection as run_prefill runs it: the plan is made for plan_rows rows and launched for T, the deferred
 // norm scale comes from rowss, and RoPE + KV append run in the epilogue (head_dim 128) or in rope_kv_kernel from a bf16
 // qkv matrix.  The RoPE table and that matrix live in stream-ordered scratch memory.
-RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
-                             int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
-                             const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
-                             void* stream) {
+static int prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                       int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps, const int32_t* slot,
+                       const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
+                       const int32_t* page_table, int pages_per_slot, void* stream) {
     if (!xhat || !rowss || !wqkv || !slot || !pos || !q_out || !k_cache || !v_cache || !fused) return RR_INVALID_ARGUMENT;
     if (T < 1 || T > plan_rows || hidden < 64 || hidden % 64 || hidden > 8192) return RR_INVALID_ARGUMENT;
     if (n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
@@ -394,6 +420,7 @@ RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows
             RopeEpi& r = p.rope;
             r.q_out = (__nv_bfloat16*)q_out; r.k_cache = (__nv_bfloat16*)k_cache; r.v_cache = (__nv_bfloat16*)v_cache;
             r.slot = slot; r.pos = pos; r.table = table; r.n_heads = n_heads; r.n_kv_heads = n_kv_heads; r.ctx_max = ctx_max;
+            r.page_table = page_table; r.pages_per_slot = pages_per_slot;
         } else {
             p.out = qkv;
         }
@@ -404,6 +431,7 @@ RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows
             ra.q_out = (__nv_bfloat16*)q_out; ra.k_cache = (__nv_bfloat16*)k_cache; ra.v_cache = (__nv_bfloat16*)v_cache;
             ra.slot = slot; ra.pos = pos; ra.rows = T; ra.n_heads = n_heads; ra.n_kv_heads = n_kv_heads; ra.ctx_max = ctx_max;
             ra.theta = theta; ra.table = table; ra.head_dim = head_dim;
+            ra.page_table = page_table; ra.pages_per_slot = pages_per_slot;
             launch_rope_kv(ra, st);
         }
         if (rc != RR_OK) note_cuda_error(cudaPeekAtLastError());
@@ -415,6 +443,23 @@ RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows
     if (rc != RR_OK) return rc;
     *fused = fuse ? 1 : 0;
     return check_last();
+}
+
+RR_API int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                             int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
+                             const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache, int* fused,
+                             void* stream) {
+    return prefill_qkv(xhat, rowss, plan_rows, T, hidden, wqkv, n_heads, n_kv_heads, head_dim, ctx_max, theta, eps, slot, pos,
+                       q_out, k_cache, v_cache, fused, nullptr, 0, stream);
+}
+
+RR_API int rr_op_prefill_qkv_paged(const void* xhat, const float* rowss, int plan_rows, int T, int hidden, const void* wqkv,
+                                   int n_heads, int n_kv_heads, int head_dim, int ctx_max, float theta, float eps,
+                                   const int32_t* slot, const int32_t* pos, void* q_out, void* k_cache, void* v_cache,
+                                   int* fused, const int32_t* page_table, int pages_per_slot, int n_pages, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return prefill_qkv(xhat, rowss, plan_rows, T, hidden, wqkv, n_heads, n_kv_heads, head_dim, ctx_max, theta, eps, slot, pos,
+                       q_out, k_cache, v_cache, fused, page_table, pages_per_slot, stream);
 }
 
 // The O, gate/up and down projections of a prefill chunk as run_prefill runs them: planned for plan_rows rows, launched
@@ -522,9 +567,10 @@ RR_API int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_
 // Prefill attention with a cached prefix per sequence (seq_pos0): the engine's launch.  Like rr_op_prefill_attn, the TMA
 // maps need the extents of q and of the caches, read back from the caller's index arrays; the positions are checked
 // against ctx_max on the way.
-RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out,
-                                     const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
-                                     int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream) {
+static int prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* seq_start,
+                               const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs, int max_len, int n_heads,
+                               int n_kv_heads, int ctx_max, float scale, const int32_t* page_table, int pages_per_slot,
+                               int n_pages, void* stream) {
     if (!q || !k_cache || !v_cache || !out || !seq_start || !seq_slot || !seq_pos0) return RR_INVALID_ARGUMENT;
     if (n_seqs < 1 || max_len < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
     if (ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
@@ -546,16 +592,35 @@ RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const v
     a.v_cache = (const __nv_bfloat16*)v_cache; a.out = (__nv_bfloat16*)out; a.seq_start = seq_start;
     a.seq_slot = seq_slot; a.seq_pos0 = seq_pos0; a.n_seqs = n_seqs; a.max_len = max_len; a.n_heads = n_heads;
     a.n_kv_heads = n_kv_heads; a.ctx_max = ctx_max; a.scale = scale; a.head_dim = 128;
-    (void)prefill_attn_make_maps(&a, h[n_seqs], (long long)(max_slot + 1) * n_kv_heads * ctx_max);
+    a.page_table = page_table; a.pages_per_slot = pages_per_slot;
+    (void)prefill_attn_make_maps(&a, h[n_seqs], page_table ? (long long)n_pages * n_kv_heads * KV_PAGE
+                                                           : (long long)(max_slot + 1) * n_kv_heads * ctx_max);
     const int rcl = launch_prefill_attn(a, st);
     if (rcl != RR_OK) return rcl;
     return check_last();
 }
 
+RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                     const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                                     int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream) {
+    return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
+                               ctx_max, scale, nullptr, 0, 0, stream);
+}
+
+RR_API int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                           const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0,
+                                           int n_seqs, int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
+                                           const int32_t* page_table, int pages_per_slot, int n_pages, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
+                               ctx_max, scale, page_table, pages_per_slot, n_pages, stream);
+}
+
 // Prefix copy between KV slots as the engine runs it at the start of a prefill chunk.  The lists are host arrays, checked
 // before the device is touched.
-RR_API int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
-                                const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies, void* stream) {
+static int kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                          const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies,
+                          const int32_t* page_table, int pages_per_slot, int n_pages, void* stream) {
     if (!k_cache || !v_cache || !src || !dst || !n_tok) return RR_INVALID_ARGUMENT;
     if (n_layers < 1 || n_slots < 1 || n_kv_heads < 1 || ctx_max < 1 || n_copies < 1 || n_copies > KV_COPY_MAX)
         return RR_INVALID_ARGUMENT;
@@ -563,8 +628,23 @@ RR_API int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int 
     c.count = n_copies;
     for (int i = 0; i < n_copies; ++i) { c.src[i] = src[i]; c.dst[i] = dst[i]; c.n[i] = n_tok[i]; }
     if (kv_copy_check(c, n_slots, ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
-    if (launch_kv_copy((__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, n_layers, n_slots, n_kv_heads, ctx_max, c,
-                       (cudaStream_t)stream) != RR_OK)
+    const long long layer_rows = page_table ? (long long)n_pages * n_kv_heads * KV_PAGE : (long long)n_slots * n_kv_heads * ctx_max;
+    if (launch_kv_copy((__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, n_layers, layer_rows, n_kv_heads, ctx_max, page_table,
+                       pages_per_slot, c, (cudaStream_t)stream) != RR_OK)
         note_cuda_error(cudaPeekAtLastError());
     return check_last();
+}
+
+RR_API int rr_op_kv_copy_prefix(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                                const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies, void* stream) {
+    return kv_copy_prefix(k_cache, v_cache, n_layers, n_slots, n_kv_heads, ctx_max, src, dst, n_tok, n_copies, nullptr, 0, 0,
+                          stream);
+}
+
+RR_API int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
+                                      const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies,
+                                      const int32_t* page_table, int pages_per_slot, int n_pages, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return kv_copy_prefix(k_cache, v_cache, n_layers, n_slots, n_kv_heads, ctx_max, src, dst, n_tok, n_copies, page_table,
+                          pages_per_slot, n_pages, stream);
 }

@@ -1,5 +1,5 @@
-// rr_attn_decode.cu — K8: decode attention over the slot-contiguous KV cache
-// [slot][kv_head][ctx_max][128] bf16.  One query token per row; the G query heads of a GQA group
+// rr_attn_decode.cu — K8: decode attention over the KV cache, [page][kv_head][P][128] bf16 addressed by kv_row
+// (rr_kernels.h): 64-token pages through a page table, or one ctx_max-token page per slot.  One query token per row; the G query heads of a GQA group
 // share each KV head, so one CTA = (row, kv_head[, kv split]) streams ctx * 512 B exactly once.
 //
 // HBM-bound by design (SURVEY.md §8d: 128 KiB/token/step for Llama-3-8B):
@@ -29,6 +29,14 @@ constexpr int UNIT_BYTES = DT * HD * 2; // 16 KB
 constexpr int RING = 3;
 constexpr int DEC_THREADS = 160;        // 4 consumer warps + 1 producer warp
 constexpr int DEC_SMEM = RING * UNIT_BYTES + 1024 /*align*/ + 128 /*barriers*/ + 512 /*new k, v row*/ + 2048 /*q*/;
+// + the cache row of each of the CTA's tiles, int32: room for at least DEC_TBL tiles (8192 tokens), so contexts up to that
+// run every kv-split count with one shared-memory size and 4 CTAs/SM
+constexpr int DEC_TBL = 128;
+static_assert(DT == KV_PAGE, "a decode tile never crosses a page");
+static int dec_smem(const DecodeAttnArgs& a) {
+    const int tiles = (a.ctx_max / DT + a.kv_splits - 1) / a.kv_splits;
+    return DEC_SMEM + 4 * (tiles > DEC_TBL ? tiles : DEC_TBL);
+}
 
 __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
     asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
@@ -65,6 +73,7 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
     uint64_t* newkv_bar = empty_bar + RING;
     __nv_bfloat16* newkv = reinterpret_cast<__nv_bfloat16*>(ring + RING * UNIT_BYTES + 128);   // [k 128 | v 128]
     __nv_bfloat16* q_s = newkv + 2 * HD;                                                          // [8 heads][128]
+    int* tile_row_s = reinterpret_cast<int*>(q_s + 8 * HD);      // [tiles] cache row of tile tile0 + j (dec_smem)
 
     griddep_launch();
     const int tr_slot = trace_begin(TR_ATTN_DEC);
@@ -100,13 +109,18 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
     const int tile0 = split * tiles_per;
     const int tile1 = min(n_tiles_all, tile0 + tiles_per);
     const int n_units = 2 * max(0, tile1 - tile0);
-    const int row_base = (slot * a.n_kv_heads + kvh) * a.ctx_max;      // row in the [slots*kvh*ctx, 128] view
 
     const int pos = ctx - 1;
     const bool owns_new = a.fuse_rope && tile1 == n_tiles_all && tile1 > tile0;   // this split holds token `pos`
 
     if (warp == 4) {
         // ===================== producer: TMA units K0 V0 K1 V1 ... =====================
+        // The page table, like slot and pos, only changes between steps: the rows of this CTA's tiles are read before the PDL
+        // wait, once, so the steady state issues no dependent global load per tile.
+        // Row of the first token of tile tile0 + j in the [n_pages*kvh*P, 128] view; a 64-token tile never crosses a page.
+        for (int j = lane; j < tile1 - tile0; j += 32)
+            tile_row_s[j] = (int)kv_row(a.page_table, a.pages_per_slot, a.n_kv_heads, a.ctx_max, slot, kvh, (tile0 + j) * DT);
+        __syncwarp();
         const bool leader = elect_one();
         // The last tile of a row usually holds fewer than 64 tokens: it is requested as 16-row boxes covering only the rows in use
         // (ncu: the kernel read 1.14 x its algorithmic bytes with whole tiles).  The rows of the slot that are not rewritten keep
@@ -115,7 +129,7 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
             const int s = u % RING;
             const bool is_v = (u & 1) != 0;
             const int tile = tile0 + (u >> 1);
-            const int r0 = row_base + tile * DT;
+            const int r0 = tile_row_s[u >> 1];
             const int valid = ctx - tile * DT;                        // > 0; >= DT for all but the last tile
             if (a.trim_tail && valid <= DT - 16 && u >= RING) {
                 const int nb = (valid + 15) >> 4;
@@ -210,8 +224,9 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
                 uint2 vv;
                 vv.x = pack_bf16(v0.x, v0.y);
                 vv.y = pack_bf16(v1.x, v1.y);
-                __nv_bfloat16* kdst = const_cast<__nv_bfloat16*>(a.k_cache) + ((size_t)row_base + pos) * HD;
-                __nv_bfloat16* vdst = const_cast<__nv_bfloat16*>(a.v_cache) + ((size_t)row_base + pos) * HD;
+                const size_t prow = (size_t)tile_row_s[pos / DT - tile0] + pos % DT;   // the append goes through the same rule
+                __nv_bfloat16* kdst = const_cast<__nv_bfloat16*>(a.k_cache) + prow * HD;
+                __nv_bfloat16* vdst = const_cast<__nv_bfloat16*>(a.v_cache) + prow * HD;
                 if (lane_on) {
                     *reinterpret_cast<uint32_t*>(kdst + i) = k_lo;
                     *reinterpret_cast<uint32_t*>(kdst + half + i) = k_hi;
@@ -425,8 +440,8 @@ size_t decode_attn_ws_bytes(int rows, int n_heads, int kv_splits) {
     return kv_splits > 1 ? (size_t)rows * n_heads * kv_splits * (HD + 2) * sizeof(float) : 0;
 }
 
-int decode_attn_make_maps(DecodeAttnArgs* a, int n_slots) {
-    const long long rows = (long long)n_slots * a->n_kv_heads * a->ctx_max;
+int decode_attn_make_maps(DecodeAttnArgs* a, int n_pages) {
+    const long long rows = (long long)n_pages * a->n_kv_heads * (a->page_table ? KV_PAGE : a->ctx_max);
     if (rows <= 0 || rows > 0x7fffffffLL || a->ctx_max % DT) return RR_ERR_ARG;
     int rc = make_tmap_bf16_2d(&a->tmK, a->k_cache, (int)rows, HD, HD, DT);
     if (rc == RR_OK) rc = make_tmap_bf16_2d(&a->tmV, a->v_cache, (int)rows, HD, HD, DT);
@@ -439,9 +454,9 @@ int decode_attn_make_maps(DecodeAttnArgs* a, int n_slots) {
 template <int G>
 static void launch_dec(const DecodeAttnArgs& a, cudaStream_t st) {
     static std::atomic<uint64_t> attr{0};
-    if (ensure_dyn_smem(decode_attn_mma_kernel<G>, DEC_SMEM, attr) != cudaSuccess) return;
+    if (ensure_dyn_smem(decode_attn_mma_kernel<G>, 227 * 1024, attr) != cudaSuccess) return;
     dim3 grid(a.n_kv_heads, a.rows, a.kv_splits);
-    launch_pdl(decode_attn_mma_kernel<G>, grid, dim3(DEC_THREADS), (size_t)DEC_SMEM, st, a);
+    launch_pdl(decode_attn_mma_kernel<G>, grid, dim3(DEC_THREADS), (size_t)dec_smem(a), st, a);
     if (a.kv_splits > 1)
         launch_pdl(decode_attn_combine_kernel, dim3(a.n_heads, a.rows), dim3(64), 0, st, (const float*)a.ws, a.out,
                    a.slot, a.n_heads, a.kv_splits, a.head_dim);

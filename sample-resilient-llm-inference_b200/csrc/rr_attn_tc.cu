@@ -14,6 +14,8 @@
 // tile of warpgroup 0) is only waited for and released.
 //
 // Work item = (sequence, query head, 128-row query tile), heaviest (last) query tiles first, strided over the CTAs.
+// KV addresses follow kv_row (rr_kernels.h): with a page table the producer looks up each key tile's page, else the tiles
+// of a slot are consecutive.
 // Prefix caching: a sequence's `len` query rows may sit at positions pos0 .. pos0 + len - 1 of its slot (seq_pos0; the
 // prefix 0 .. pos0 - 1 is already in the cache).  They attend to positions 0 .. own position; the key tiles, the causal
 // mask and the skip test use absolute positions, Q stays at the sequence's rows of q.  A query row visits key tiles
@@ -124,20 +126,30 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                 const WorkFetch f = nf;
                 fetch_work(a, w + gridDim.x, n_work, true, nf);
                 if (!decode_work(a, w, max_qt, f, k)) continue;
-                const int kv_row0 = (f.slot * a.n_kv_heads + k.head / G) * a.ctx_max;
+                const int kvh = k.head / G;
+                const bool paged = a.page_table != nullptr;
                 mbar_wait(&bars->q_empty, (q_it & 1) ^ 1);
                 mbar_arrive_expect_tx(&bars->q_full, Q_BYTES);
                 for (int c = 0; c < 2; ++c)
                     tma_load_2d(smem + OFF_Q + c * 16384, &tmQ, &bars->q_full, k.head * 128 + c * 64, k.tok0 + k.qt * TQ);
                 ++q_it;
+                // a 64-key tile never crosses a page: one table lookup per tile, the next tile's issued before this tile's
+                // ring-slot wait so that its latency hides under the wait
+                auto kv_tile_row = [&](int j) {
+                    return (int)kv_page_row(paged, kv_page(a.page_table, a.pages_per_slot, f.slot, j * TKV), a.n_kv_heads,
+                                            a.ctx_max, kvh, j * TKV);
+                };
+                int kv_next = kv_tile_row(0);
                 for (int j = 0; j < k.n_kt; ++j, ++kv_it) {
                     const uint32_t s = kv_it % NS;
+                    const int kv_r = kv_next;
+                    if (j + 1 < k.n_kt) kv_next = kv_tile_row(j + 1);
                     mbar_wait(&bars->kv_empty[s], ((kv_it / NS) & 1) ^ 1);
                     mbar_arrive_expect_tx(&bars->kv_full[s], 2 * KV_BYTES);
                     uint8_t* dst = smem + OFF_KV + s * 2 * KV_BYTES;
                     for (int c = 0; c < 2; ++c) {
-                        tma_load_2d(dst + c * 8192, &tmK, &bars->kv_full[s], c * 64, kv_row0 + j * TKV);
-                        tma_load_2d(dst + KV_BYTES + c * 8192, &tmV, &bars->kv_full[s], c * 64, kv_row0 + j * TKV);
+                        tma_load_2d(dst + c * 8192, &tmK, &bars->kv_full[s], c * 64, kv_r);
+                        tma_load_2d(dst + KV_BYTES + c * 8192, &tmV, &bars->kv_full[s], c * 64, kv_r);
                     }
                 }
             }
@@ -272,7 +284,7 @@ bool prefill_attn_tc_eligible(const PrefillAttnArgs& a) {
     return a.has_maps && G >= 1 && a.n_heads % a.n_kv_heads == 0 && a.ctx_max % TKV == 0 && a.head_dim % 8 == 0;
 }
 
-// q: [q_rows, n_heads*128]; caches: [kv_rows = n_slots*n_kv_heads*ctx_max, 128].  Boxes: Q 64 x 128 rows,
+// q: [q_rows, n_heads*128]; caches: [kv_rows = n_pages*n_kv_heads*P, 128] (kv_row).  Boxes: Q 64 x 128 rows,
 // K/V 64 x 64 rows, 128-byte swizzle.
 int prefill_attn_make_maps(PrefillAttnArgs* a, long long q_rows, long long kv_rows) {
     a->has_maps = 0;

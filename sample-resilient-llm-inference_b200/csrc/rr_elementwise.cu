@@ -334,6 +334,8 @@ rope_kv_kernel(RopeArgs a) {
     const int slot = a.slot[row];
     if (slot < 0) return;
     const int pos = a.pos[row];
+    const int page = kv_page(a.page_table, a.pages_per_slot, slot, pos);        // one lookup per token row
+    const bool paged = a.page_table != nullptr;
     // work items of 2 rotation pairs: (head, i..i+1) for q heads then k heads, then v copies (4 elements).
     // hd = true head dim: rotation pairs (i, i + hd/2); destination rows are padded to 128 (pad stays zero).
     const int hd = a.head_dim, half = hd >> 1, ipw = half >> 1, vpw = hd >> 2;      // items per head
@@ -360,7 +362,7 @@ rope_kv_kernel(RopeArgs a) {
             const uint32_t o_hi = pack_bf16(hi.x * c0 + lo.x * s0, hi.y * c1 + lo.y * s1);
             __nv_bfloat16* dst = is_q
                 ? a.q_out + (size_t)row * (a.n_heads * 128) + head * 128 + i
-                : a.k_cache + (((size_t)slot * a.n_kv_heads + head) * a.ctx_max + pos) * 128 + i;
+                : a.k_cache + kv_page_row(paged, page, a.n_kv_heads, a.ctx_max, head, pos) * 128 + i;
             *reinterpret_cast<uint32_t*>(dst) = o_lo;
             *reinterpret_cast<uint32_t*>(dst + half) = o_hi;
         } else {
@@ -368,7 +370,7 @@ rope_kv_kernel(RopeArgs a) {
             const int head = j / vpw, i4 = (j % vpw) * 4;
             const int col = (a.n_heads + a.n_kv_heads) * hd + head * hd + i4;
             const float4 v = part_load4(a.qkv, row, col);
-            __nv_bfloat16* dst = a.v_cache + (((size_t)slot * a.n_kv_heads + head) * a.ctx_max + pos) * 128 + i4;
+            __nv_bfloat16* dst = a.v_cache + kv_page_row(paged, page, a.n_kv_heads, a.ctx_max, head, pos) * 128 + i4;
             uint2 o;
             o.x = pack_bf16(v.x, v.y);
             o.y = pack_bf16(v.z, v.w);

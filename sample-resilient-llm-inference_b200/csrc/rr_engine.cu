@@ -6,9 +6,9 @@
 // (submit -> wait -> tokens + timestamps) is what chat.completions.create needs
 // (src/demo_load_balancing.py:106-116).
 //
-// Layout in HBM (one replica): bf16 weights (caller-owned), KV cache
-// [layer][slot][kv_head][ctx_max][128] bf16 for K and for V, a decode working set of max_batch
-// rows (row b == KV slot b) and a prefill working set of max_prefill_tokens rows.
+// Layout in HBM (one replica): bf16 weights (caller-owned), a paged KV cache [layer][page][kv_head][64][128] bf16 for K and
+// for V (a pool of kv_cache_tokens / 64 pages, addressed through the page table [slot][ctx_max / 64], kv_row), a decode
+// working set of max_batch rows (row b == KV slot b) and a prefill working set of max_prefill_tokens rows.
 // The decode step is a fixed sequence of 6 launches per layer + 4, captured once in a CUDA graph
 // and replayed; per-row metadata (token, position, active flag) lives on the device so replays
 // need no parameter changes.
@@ -269,6 +269,15 @@ struct rr_engine {
     float2* rope_table;
     __nv_bfloat16 *kcache, *vcache;
     size_t kv_layer_stride;
+    // The KV page pool, under mu: n_pages pages of KV_PAGE positions.  slot_pages[b] = the pages slot b holds, in position
+    // order (a slot keeps them after its request; see take_pages / trim_pages / reclaim_pages); free_pages = a stack.  The
+    // device table d_table [Bm][pps] has a fixed address (the decode graphs hold it); h_table is its pinned mirror, and
+    // table_dirty[b] marks the rows upload_table copies before the next prefill chunk or decode step.
+    int n_pages = 0, pps = 0;
+    int32_t *d_table = nullptr, *h_table = nullptr;
+    std::vector<std::vector<int32_t>> slot_pages;
+    std::vector<int32_t> free_pages;
+    std::vector<char> table_dirty;
     int kv_splits;
     std::vector<GemmPlan> pl_qkv, pl_o, pl_gu, pl_down;
     std::vector<DecodeAttnArgs> attn_args;   // per layer (TMA maps of that layer's K / V cache)
@@ -657,6 +666,7 @@ static int init_pf_plans(rr_engine* e) {
             r.v_cache = e->vcache + (size_t)l * e->kv_layer_stride;
             r.slot = nullptr; r.pos = nullptr;                     // set per chunk (offsets inside the staging buffer)
             r.table = e->rope_table; r.n_heads = d.n_heads; r.n_kv_heads = d.n_kv_heads; r.ctx_max = e->o.ctx_max;
+            r.page_table = e->d_table; r.pages_per_slot = e->pps;
         }
         rc = gemm_plan_init(&P.o[l], e->pattn, T, e->nq, e->wo[l], d.hidden, e->nq, e->nq, e->px, d.hidden, 0, 1,
                             OUT_ROWMAJOR_RESID, PF_BN);                // residual add in the epilogue
@@ -778,7 +788,8 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     auto launch_rows = [&](const GemmPlan& pl) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s); };
     uint64_t nl = 0;
     if (copies && copies->count > 0) {   // cached prefixes of busy slots into this chunk's slots, before any layer reads them
-        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, e->Bm, d.n_kv_heads, e->o.ctx_max, *copies, s) != RR_OK)
+        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, (long long)e->n_pages * d.n_kv_heads * KV_PAGE, d.n_kv_heads,
+                           e->o.ctx_max, e->d_table, e->pps, *copies, s) != RR_OK)
             return RR_CUDA_ERROR;
         ++nl;
     }
@@ -797,7 +808,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ra.qkv = part_bf16(e->pqkv, e->nqkv);
         ra.q_out = e->pq; ra.k_cache = kc; ra.v_cache = vc; ra.slot = p_slt; ra.pos = p_pos; ra.rows = T;
         ra.n_heads = d.n_heads; ra.n_kv_heads = d.n_kv_heads; ra.ctx_max = e->o.ctx_max; ra.theta = d.rope_theta;
-        ra.table = e->rope_table; ra.head_dim = d.head_dim;
+        ra.table = e->rope_table; ra.head_dim = d.head_dim; ra.page_table = e->d_table; ra.pages_per_slot = e->pps;
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer TMA maps made at create
         pa.q = e->pq; pa.k_cache = kc; pa.v_cache = vc; pa.out = e->pattn; pa.seq_start = p_ss; pa.seq_slot = p_sl;
@@ -818,7 +829,8 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (launch_rows(P.down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
     }
     if (fan_copies.count) {     // every layer's KV of the prompts is written: fan it out before any decode step reads it
-        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, e->Bm, d.n_kv_heads, e->o.ctx_max, fan_copies, s) != RR_OK)
+        if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, (long long)e->n_pages * d.n_kv_heads * KV_PAGE, d.n_kv_heads,
+                           e->o.ctx_max, e->d_table, e->pps, fan_copies, s) != RR_OK)
             return RR_CUDA_ERROR;
         ++nl;
     }
@@ -845,6 +857,95 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         const int sl = fan ? h_tsl[j] : slots[j];
         e->h_slot_mirror[sl] = sl;
     }
+    return RR_OK;
+}
+
+// ---------------------------------------------------------------- KV page pool (caller holds e->mu)
+static int pages_for(int tokens) { return (tokens + KV_PAGE - 1) / KV_PAGE; }
+
+// Slot b holds exactly n pages: it keeps its first ones, returns extra ones from the end and takes missing ones from the free
+// stack (the caller made sure there are enough).  Pages go back in the reverse of the order they were taken, so a slot
+// that returns its pages and takes as many again gets the same ones: its table row does not change and is not copied.
+static void resize_pages(rr_engine* e, int b, int n) {
+    std::vector<int32_t>& P = e->slot_pages[b];
+    while ((int)P.size() > n) { e->free_pages.push_back(P.back()); P.pop_back(); }
+    while ((int)P.size() < n) {
+        const int32_t pg = e->free_pages.back();
+        e->free_pages.pop_back();
+        int32_t& t = e->h_table[(size_t)b * e->pps + P.size()];
+        if (t != pg) { t = pg; e->table_dirty[b] = 1; }
+        P.push_back(pg);
+    }
+}
+
+// Pages a request could get now: the free ones and those of the free slots.
+static int pages_available(const rr_engine* e) {
+    int n = (int)e->free_pages.size();
+    for (int b = 0; b < e->Bm; ++b)
+        if (!e->row_req[b]) n += (int)e->slot_pages[b].size();
+    return n;
+}
+
+// Until `need` pages are free: take back every page of a free slot, first of slots with no retained prefix (lowest index
+// first), then least recently used by retained_used, and forget each such slot's prefix.
+static void reclaim_pages(rr_engine* e, int need) {
+    while ((int)e->free_pages.size() < need) {
+        int pick = -1;
+        for (int b = 0; b < e->Bm; ++b) {
+            if (e->row_req[b] || e->slot_pages[b].empty()) continue;
+            const bool empty = !e->o.prefix_cache || e->retained[b].empty();
+            if (empty) { pick = b; break; }
+            if (pick < 0 || e->retained_used[b] < e->retained_used[pick]) pick = b;
+        }
+        if (pick < 0) return;                              // cannot happen: the caller checked pages_available
+        if (e->o.prefix_cache) e->retained[pick].clear();
+        resize_pages(e, pick, 0);
+    }
+}
+
+// The request just took the slots r->rows: give each ceil((prompt + max_new) / 64) pages, shrinking before growing so the
+// pages a slot returns serve the others first.
+static void take_pages(rr_engine* e, const Request* r) {
+    const int need = pages_for((int)r->prompt.size() + r->max_new);
+    int missing = 0;
+    for (int b : r->rows) {
+        if ((int)e->slot_pages[b].size() > need) resize_pages(e, b, need);
+        missing += need - (int)e->slot_pages[b].size();
+    }
+    reclaim_pages(e, missing);
+    for (int b : r->rows) resize_pages(e, b, need);
+}
+
+// Slot b's request is done with it: keep the pages of its retained prefix (none without prefix caching), return the rest.
+static void trim_pages(rr_engine* e, int b) {
+    resize_pages(e, b, e->o.prefix_cache ? pages_for((int)e->retained[b].size()) : 0);
+}
+
+// Caller holds gpu_mu.  Copies the changed rows of the page table to the device on the engine stream, ahead of the work
+// that reads them.
+static int upload_table(rr_engine* e) {
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (int b = 0; b < e->Bm; ++b) {
+        if (!e->table_dirty[b]) continue;
+        const size_t off = (size_t)b * e->pps, bytes = sizeof(int32_t) * e->pps;
+        CK(cudaMemcpyAsync(e->d_table + off, e->h_table + off, bytes, cudaMemcpyHostToDevice, e->stream));
+        e->st.h2d_bytes += bytes;
+        e->table_dirty[b] = 0;
+    }
+    return RR_OK;
+}
+
+// Caller holds gpu_mu.  Low-level calls: slot slots[i] must hold the pages of positions [0, n_pos[i]).  RR_INVALID_ARGUMENT,
+// nothing changed, when the free pages do not cover that.
+static int grow_pages(rr_engine* e, const int32_t* slots, const int* n_pos, int n) {
+    std::lock_guard<std::mutex> lk(e->mu);
+    std::vector<int> want(e->Bm, 0);
+    for (int i = 0; i < n; ++i) want[slots[i]] = std::max(want[slots[i]], pages_for(n_pos[i]));
+    int missing = 0;
+    for (int b = 0; b < e->Bm; ++b) missing += std::max(0, want[b] - (int)e->slot_pages[b].size());
+    if (missing > (int)e->free_pages.size()) return RR_INVALID_ARGUMENT;
+    for (int b = 0; b < e->Bm; ++b)
+        if (want[b] > (int)e->slot_pages[b].size()) resize_pages(e, b, want[b]);
     return RR_OK;
 }
 
@@ -897,6 +998,7 @@ static void release_row(rr_engine* e, Request* r, int c) {
     const int b = r->rows[c];
     if (b < 0) return;
     e->row_req[b] = nullptr; e->h_slot_mirror[b] = -1;
+    trim_pages(e, b);
     set_row_params(e, b, nullptr);
     e->slots_dirty = true;
     r->rows[c] = -1;
@@ -1037,6 +1139,8 @@ static void worker_main(rr_engine* e) {
                     if (b >= e->Bm) break;
                 }
                 if ((int)ids.size() + (int)r->prompt.size() - m > e->Tmax) break;   // a chunk holds Tmax uncached tokens
+                // every choice reserves its pages now; a request that does not fit waits at the head of the queue
+                if (r->n_choices * pages_for((int)r->prompt.size() + r->max_new) > pages_available(e)) break;
                 e->waiting.pop_front();
                 r->n_cached = m;
                 if (e->o.prefix_cache) {
@@ -1059,6 +1163,7 @@ static void worker_main(rr_engine* e) {
                     tail_seq.push_back((int)chunk.size()); tail_slot.push_back(b); tail_choice.push_back(c);
                     tail_gen.push_back(&r->gen);
                 }
+                take_pages(e, r);
                 chunk.push_back(r);
                 slots.push_back(r->rows[0]);
                 chunk_mode |= step_mode(r->gen);
@@ -1078,7 +1183,7 @@ static void worker_main(rr_engine* e) {
             if (e->index_epoch != epoch) {
                 for (size_t i = chunk.size(); i-- > 0;) {
                     Request* r = chunk[i];
-                    for (int b : r->rows) e->row_req[b] = nullptr;
+                    for (int b : r->rows) { e->row_req[b] = nullptr; resize_pages(e, b, 0); }   // nothing retained
                     r->rows.clear(); r->n_cached = 0;
                     e->waiting.push_front(r);
                 }
@@ -1089,7 +1194,8 @@ static void worker_main(rr_engine* e) {
             PrefillTail tail;
             tail.n = (int)tail_seq.size(); tail.seq = tail_seq.data(); tail.slot = tail_slot.data();
             tail.choice = tail_choice.data(); tail.gen = tail_gen.data(); tail.mode = chunk_mode;
-            int rc = (chunk_mode & 4) ? ensure_pen_buffers(e) : RR_OK;
+            int rc = upload_table(e);
+            if (rc == RR_OK && (chunk_mode & 4)) rc = ensure_pen_buffers(e);
             if (rc == RR_OK && (chunk_mode & 8)) rc = ensure_stop_buffers(e);
             if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
             if (rc == RR_OK)
@@ -1129,8 +1235,9 @@ static void worker_main(rr_engine* e) {
             e->slots_dirty = false;
         }
         upload_row_params(e, step);
+        int rc = upload_table(e);
         cudaEventRecord(e->ev0, s);
-        int rc = run_decode_step(e, step);
+        if (rc == RR_OK) rc = run_decode_step(e, step);
         cudaEventRecord(e->ev1, s);
         const int rb = enqueue_readback(e, e->d_tok, e->Bm, step, s);     // outside ev0 .. ev1: decode_ms_total excludes it
         if (rc == RR_OK) rc = rb;
@@ -1172,6 +1279,10 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     if (d.hidden > 8192) return RR_INVALID_ARGUMENT;      // add_rmsnorm_kernel keeps one row in registers (rr_elementwise.cu)
     if (opts->max_batch < 1 || opts->max_batch > 256 || opts->ctx_max < 64 || opts->ctx_max % 64)
         return RR_INVALID_ARGUMENT;
+    // the KV pool: 0 = one ctx_max per decode row, else a multiple of 64 in [ctx_max, max_batch x ctx_max]
+    const long long kv_full = (long long)opts->max_batch * opts->ctx_max;
+    const long long kv_tokens = opts->kv_cache_tokens == 0 ? kv_full : opts->kv_cache_tokens;
+    if (kv_tokens % KV_PAGE || kv_tokens < opts->ctx_max || kv_tokens > kv_full) return RR_INVALID_ARGUMENT;
     CK(cudaSetDevice(opts->device));
     rr_engine* e = new (std::nothrow) rr_engine();
     if (!e) return RR_INTERNAL;
@@ -1222,9 +1333,15 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     TRY(dalloc(e, &e->logits, (size_t)B * d.vocab));
     TRY(dalloc(e, &e->rope_table, (size_t)opts->ctx_max * 64));
     launch_rope_table(e->rope_table, opts->ctx_max, d.rope_theta, d.head_dim, e->stream);
-    e->kv_layer_stride = (size_t)B * d.n_kv_heads * opts->ctx_max * 128;
+    // zeroed like the rest: decode attention reads stale rows of a partly used tile, whose masked scores must meet finite K/V
+    e->n_pages = (int)(kv_tokens / KV_PAGE); e->pps = opts->ctx_max / KV_PAGE;
+    e->o.kv_cache_tokens = (int32_t)kv_tokens;
+    e->kv_layer_stride = (size_t)e->n_pages * d.n_kv_heads * KV_PAGE * 128;
     TRY(dalloc(e, &e->kcache, e->kv_layer_stride * L));
     TRY(dalloc(e, &e->vcache, e->kv_layer_stride * L));
+    TRY(dalloc(e, &e->d_table, (size_t)B * e->pps));
+    TRYC(cudaMallocHost(&e->h_table, sizeof(int32_t) * B * e->pps));
+    memset(e->h_table, 0, sizeof(int32_t) * B * e->pps);
     {   // split-KV only when the grid would not fill the GPU
         const int ks = pick_kv_splits(B, d.n_kv_heads);
         e->kv_splits = ks;
@@ -1271,7 +1388,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
             pa.q = e->pq; pa.k_cache = e->kcache + (size_t)l * e->kv_layer_stride;
             pa.v_cache = e->vcache + (size_t)l * e->kv_layer_stride; pa.n_heads = d.n_heads;
             pa.n_kv_heads = d.n_kv_heads; pa.ctx_max = opts->ctx_max; pa.head_dim = d.head_dim;
-            TRY(prefill_attn_make_maps(&pa, T, (long long)B * d.n_kv_heads * opts->ctx_max));   // ctx_max % 64 == 0 (checked above)
+            pa.page_table = e->d_table; pa.pages_per_slot = e->pps;
+            TRY(prefill_attn_make_maps(&pa, T, (long long)e->n_pages * d.n_kv_heads * KV_PAGE));
         }
         DecodeAttnArgs& da = e->attn_args[l];
         da.q = e->qbuf; da.k_cache = e->kcache + (size_t)l * e->kv_layer_stride;
@@ -1280,8 +1398,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         da.ctx_max = opts->ctx_max; da.scale = 1.0f / sqrtf((float)d.head_dim); da.ws = e->attn_ws;
         da.kv_splits = e->kv_splits;
         da.fuse_rope = 1; da.qkv = part_f32(e->part_qkv, e->s_qkv, B, e->nqkv); da.rope_table = e->rope_table;
-        da.head_dim = d.head_dim;
-        TRY(decode_attn_make_maps(&da, B));
+        da.head_dim = d.head_dim; da.page_table = e->d_table; da.pages_per_slot = e->pps;
+        TRY(decode_attn_make_maps(&da, e->n_pages));
         TRY(gemm_plan_init(&e->pl_qkv[l], e->wqkv[l], e->nqkv, d.hidden, e->xn, B, d.hidden, d.hidden, e->part_qkv,
                            e->nqkv, B, e->s_qkv, OUT_TRANSPOSED_F32, e->bn_dec));
         TRY(gemm_plan_init(&e->pl_o[l], e->wo[l], d.hidden, e->nq, e->attn_out, B, e->nq, e->nq, e->part_o, d.hidden,
@@ -1321,6 +1439,9 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->row_req.assign(B, nullptr);
     e->row_choice.assign(B, 0);
     e->h_slot_mirror.assign(B, -1);
+    e->slot_pages.assign(B, {});
+    e->table_dirty.assign(B, 0);
+    for (int pg = e->n_pages; pg-- > 0;) e->free_pages.push_back(pg);      // pages 0, 1, ... come off the stack first
     if (e->o.prefix_cache) { e->retained.assign(B, {}); e->retained_used.assign(B, 0); }
     e->worker = std::thread(worker_main, e);
     *out = e;
@@ -1340,6 +1461,7 @@ RR_API void rr_engine_destroy(rr_engine* e) {
         if (g) cudaGraphExecDestroy(g);
     for (void* p : e->allocs) cudaFree(p);
     if (e->h_stage) cudaFreeHost(e->h_stage);
+    if (e->h_table) cudaFreeHost(e->h_table);
     if (e->h_tok) cudaFreeHost(e->h_tok);
     if (e->h_lp) cudaFreeHost(e->h_lp);
     if (e->h_lp_id) cudaFreeHost(e->h_lp_id);
@@ -1363,7 +1485,14 @@ RR_API int rr_engine_prefill(rr_engine* e, const int32_t* ids, const int32_t* se
     std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
     forget_prefixes(e);
     CK(cudaSetDevice(e->o.device));
-    return run_prefill(e, ids, seq_start, slots, n_seqs, first_tok, logits_out);
+    std::vector<int> n_pos(n_seqs);
+    for (int i = 0; i < n_seqs; ++i) {                 // run_prefill checks the rest
+        if (slots[i] < 0 || slots[i] >= e->Bm || seq_start[i + 1] - seq_start[i] > e->o.ctx_max) return RR_INVALID_ARGUMENT;
+        n_pos[i] = std::max(0, seq_start[i + 1] - seq_start[i]);
+    }
+    int rc = grow_pages(e, slots, n_pos.data(), n_seqs);
+    if (rc == RR_OK) rc = upload_table(e);
+    return rc != RR_OK ? rc : run_prefill(e, ids, seq_start, slots, n_seqs, first_tok, logits_out);
 }
 
 RR_API int rr_engine_decode_step(rr_engine* e, const int32_t* slots, const int32_t* tok, const int32_t* pos, int n,
@@ -1380,6 +1509,13 @@ RR_API int rr_engine_decode_step(rr_engine* e, const int32_t* slots, const int32
         const int s = slots[i];
         if (s < 0 || s >= B || pos[i] < 0 || pos[i] >= e->o.ctx_max) return RR_INVALID_ARGUMENT;
         h[s] = tok[i]; h[B + s] = pos[i]; h[2 * B + s] = s;
+    }
+    {
+        std::vector<int> n_pos(n);
+        for (int i = 0; i < n; ++i) n_pos[i] = pos[i] + 1;
+        int rc = grow_pages(e, slots, n_pos.data(), n);
+        if (rc == RR_OK) rc = upload_table(e);
+        if (rc != RR_OK) return rc;
     }
     cudaStream_t st = e->stream;
     CK(cudaMemcpyAsync(e->d_tok, h, sizeof(int32_t) * B, cudaMemcpyHostToDevice, st));
@@ -1422,6 +1558,7 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
+    if ((long long)n_choices * pages_for(n_prompt + max_new_tokens) > e->n_pages) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
         if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
     Request* r = new (std::nothrow) Request();
@@ -1464,8 +1601,9 @@ void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx) {
     std::lock_guard<std::mutex> lk(e->mu);
     e->hook = fn; e->hook_ctx = ctx;
 }
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch) {
+int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch, int* kv_tokens) {
     if (!e) return RR_INVALID_ARGUMENT;
+    if (kv_tokens) *kv_tokens = e->n_pages * KV_PAGE;
     if (max_batch) *max_batch = e->Bm;
     if (ctx_max) *ctx_max = e->o.ctx_max;
     if (max_prefill) *max_prefill = e->Tmax;
@@ -1613,6 +1751,14 @@ RR_API int rr_engine_run_batch(rr_engine* e, const int32_t* prompt_ids, const in
 }
 
 RR_API double rr_engine_now(rr_engine* e) { return e ? now_s(e) : 0.0; }
+
+RR_API int rr_engine_kv_usage(rr_engine* e, int32_t* pages_total, int32_t* pages_free) {
+    if (!e || !pages_total || !pages_free) return RR_INVALID_ARGUMENT;
+    std::lock_guard<std::mutex> lk(e->mu);
+    *pages_total = e->n_pages;
+    *pages_free = (int32_t)e->free_pages.size();
+    return RR_OK;
+}
 
 RR_API int rr_engine_get_stats(rr_engine* e, rr_engine_stats* out) {
     if (!e || !out) return RR_INVALID_ARGUMENT;

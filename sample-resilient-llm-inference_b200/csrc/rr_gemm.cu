@@ -573,6 +573,7 @@ __device__ __forceinline__ void pf_epilogue(const float (&acc)[128], int row0, i
                 if (slot < 0) continue;
                 const int pos = rope.pos[row];
                 const float2* tab = rope.table + (size_t)pos * 64;
+                const int page = kv_page(rope.page_table, rope.pages_per_slot, slot, pos);    // one lookup per token row
 #pragma unroll
                 for (int hb = 0; hb < 2; ++hb) {
                     const int H = b_tile * 2 + hb;
@@ -580,7 +581,8 @@ __device__ __forceinline__ void pf_epilogue(const float (&acc)[128], int row0, i
                     if (H < rope.n_heads + rope.n_kv_heads) {
                         __nv_bfloat16* dst = H < rope.n_heads
                             ? rope.q_out + (size_t)row * (rope.n_heads * 128) + H * 128
-                            : rope.k_cache + (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads)) * rope.ctx_max + pos) * 128;
+                            : rope.k_cache + kv_page_row(rope.page_table != nullptr, page, rope.n_kv_heads, rope.ctx_max,
+                                                         H - rope.n_heads, pos) * 128;
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const int d = 8 * j + cq;
@@ -592,8 +594,8 @@ __device__ __forceinline__ void pf_epilogue(const float (&acc)[128], int row0, i
                             *reinterpret_cast<uint32_t*>(dst + 64 + d) = pack_bf16(h0 * cs.x + l0 * cs.y, h1 * cs.z + l1 * cs.w);
                         }
                     } else {
-                        __nv_bfloat16* dst = rope.v_cache +
-                            (((size_t)slot * rope.n_kv_heads + (H - rope.n_heads - rope.n_kv_heads)) * rope.ctx_max + pos) * 128;
+                        __nv_bfloat16* dst = rope.v_cache + kv_page_row(rope.page_table != nullptr, page, rope.n_kv_heads,
+                                                                        rope.ctx_max, H - rope.n_heads - rope.n_kv_heads, pos) * 128;
 #pragma unroll
                         for (int j = 0; j < 16; ++j) {
                             const int jj = 16 * hb + j;

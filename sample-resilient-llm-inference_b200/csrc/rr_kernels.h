@@ -14,6 +14,25 @@ namespace rr {
 #define RR_ERR_ARG RR_INVALID_ARGUMENT
 #define RR_ERR_CUDA RR_CUDA_ERROR
 
+// ---- the KV cache address rule, the one formula every kernel that reads or writes the cache goes through.  A page holds P
+// consecutive positions of one slot for every kv head, [page][kv_head][P][128] bf16 per layer for K and for V.  With a page
+// table ([n_slots][pages_per_slot], the engine's layout) P = KV_PAGE and position pos of slot s lies on page
+// table[s * pages_per_slot + pos / KV_PAGE]; without one (table == nullptr) P = ctx_max and the page is the slot, which is
+// the slot-contiguous layout [slot][kv_head][ctx_max][128].  Table entries are trusted, like slot indices.
+constexpr int KV_PAGE = 64;
+__host__ __device__ __forceinline__ int kv_page(const int32_t* table, int pages_per_slot, int slot, int pos) {
+    return table ? table[slot * pages_per_slot + pos / KV_PAGE] : slot;
+}
+// Row of (page, kv head, pos) in the [n_pages * n_kv_heads * P, 128] view of one layer's cache.
+__host__ __device__ __forceinline__ long long kv_page_row(bool paged, int page, int n_kv_heads, int ctx_max, int kvh, int pos) {
+    return paged ? ((long long)page * n_kv_heads + kvh) * KV_PAGE + (pos & (KV_PAGE - 1))
+                 : ((long long)page * n_kv_heads + kvh) * ctx_max + pos;
+}
+__host__ __device__ __forceinline__ long long kv_row(const int32_t* table, int pages_per_slot, int n_kv_heads, int ctx_max,
+                                                     int slot, int kvh, int pos) {
+    return kv_page_row(table != nullptr, kv_page(table, pages_per_slot, slot, pos), n_kv_heads, ctx_max, kvh, pos);
+}
+
 enum GemmOutMode { OUT_ROWMAJOR_BF16 = 0, OUT_TRANSPOSED_F32 = 1, OUT_TRANSPOSED_SILU = 2, OUT_ROWMAJOR_SILU = 3,
                    OUT_ROWMAJOR_ROPE = 4, OUT_ROWMAJOR_RESID = 5 };
 // OUT_ROWMAJOR_RESID (prefill O / down projections): out is the fp32 residual stream, out[a*ldo + b] += acc —
@@ -29,6 +48,8 @@ struct RopeEpi {
     const int32_t* pos;
     const float2* table;      // [ctx_max][64] (cos, sin)
     int n_heads, n_kv_heads, ctx_max;
+    const int32_t* page_table = nullptr;   // KV address rule (kv_row): null = [slot][kv_head][ctx_max][128]
+    int pages_per_slot = 0;
     // ---- deferred RMSNorm (prefill): the GEMM that writes the residual also emits the next GEMM's operand
     // xhat = bf16(x * gamma) (NOT normalised) and per-row partial sums of squares; the next GEMM scales its
     // accumulators by rsqrt(mean(x^2) + eps) of the row in its epilogue (the projection is linear).  No norm kernel,
@@ -113,7 +134,8 @@ struct GenParams {
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, const GenParams& p, int n_choices);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch);
+// kv_tokens: the KV pool (rr_engine_opts.kv_cache_tokens after its default is applied)
+int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch, int* kv_tokens = nullptr);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
 int router_strategy(const rr_router* r);
@@ -203,6 +225,8 @@ struct RopeArgs {
     float theta;
     const float2* table;      // [ctx_max][64] (cos, sin) or null: compute inline
     int head_dim;             // true head dim (<= 128, % 8 == 0): column stride inside qkv; q_out / caches are padded to 128
+    const int32_t* page_table = nullptr;   // KV address rule (kv_row)
+    int pages_per_slot = 0;
 };
 void launch_rope_kv(const RopeArgs& a, cudaStream_t st);
 void launch_rope_table(float2* table, int ctx_max, float theta, int head_dim, cudaStream_t st);
@@ -316,8 +340,13 @@ struct DecodeAttnArgs {
     PartIn qkv;
     const float2* rope_table;
     int head_dim;             // true head dim: qkv column stride and `out` head stride; q / caches padded to 128
+    // KV address rule (kv_row).  The page table changes only between launches, like slot and pos: the producer reads the
+    // pages of its tiles before the PDL wait.
+    const int32_t* page_table = nullptr;
+    int pages_per_slot = 0;
 };
-int decode_attn_make_maps(DecodeAttnArgs* a, int n_slots);   // fills tmK / tmV (ctx_max % 64 == 0)
+// Fills tmK / tmV (ctx_max % 64 == 0) over n_pages pages: n_slots without a page table.
+int decode_attn_make_maps(DecodeAttnArgs* a, int n_pages);
 void launch_decode_attn(const DecodeAttnArgs& a, cudaStream_t st);
 size_t decode_attn_ws_bytes(int rows, int n_heads, int kv_splits);
 
@@ -334,6 +363,8 @@ struct PrefillAttnArgs {
     int head_dim;             // true head dim: `out` head stride; q / caches padded to 128
     int has_maps = 0;         // tmQ/tmK/tmV valid (prefill_attn_make_maps): required
     CUtensorMap tmQ, tmK, tmV;
+    const int32_t* page_table = nullptr;   // KV address rule (kv_row): the producer looks up the page of each key tile
+    int pages_per_slot = 0;
 };
 int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st);   // RR_ERR_ARG when the maps are missing / shape unsupported
 // wgmma kernel (rr_attn_tc.cu): one (sequence, head, 128-row query tile) per work item.
@@ -342,7 +373,8 @@ bool prefill_attn_tc_eligible(const PrefillAttnArgs& a);
 int launch_prefill_attn_tc(const PrefillAttnArgs& a, cudaStream_t st);
 
 // ---- prompt prefix caching (rr_kv_copy.cu): positions [0, n[i]) of slot src[i] -> slot dst[i], every layer and kv head,
-// K and V, one launch for the whole list (passed by value as a kernel parameter).
+// K and V, one launch for the whole list (passed by value as a kernel parameter).  Each layer's cache is layer_rows rows of
+// 128 (n_pages * n_kv_heads * P); positions are addressed by kv_row through page_table (null: slot-contiguous).
 constexpr int KV_COPY_MAX = 256;      // = the largest max_batch
 struct KvCopyList {
     int32_t src[KV_COPY_MAX], dst[KV_COPY_MAX], n[KV_COPY_MAX];
@@ -351,7 +383,7 @@ struct KvCopyList {
 // RR_ERR_ARG unless 1 <= count <= KV_COPY_MAX, every slot is in [0, n_slots), every n in [1, ctx_max], no destination
 // repeats and no destination is also a source.
 int kv_copy_check(const KvCopyList& c, int n_slots, int ctx_max);
-int launch_kv_copy(__nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
-                   const KvCopyList& c, cudaStream_t st);
+int launch_kv_copy(__nv_bfloat16* k_cache, __nv_bfloat16* v_cache, int n_layers, long long layer_rows, int n_kv_heads,
+                   int ctx_max, const int32_t* page_table, int pages_per_slot, const KvCopyList& c, cudaStream_t st);
 
 }  // namespace rr

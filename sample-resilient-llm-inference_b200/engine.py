@@ -59,10 +59,16 @@ def _p(a: np.ndarray):
 class Engine:
     def __init__(self, weights: Weights, device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
                  max_prefill_tokens: int = 8192, use_cuda_graph: bool = True,
-                 fail_prob: float = 0.0, fail_seed: int = 0, prefix_cache: bool = False):
+                 fail_prob: float = 0.0, fail_seed: int = 0, prefix_cache: bool = False,
+                 kv_cache_tokens: Optional[int] = None):
         """prefix_cache=True: a KV slot keeps the prompt its last prefill wrote, and a prompt that shares at least 64
         leading tokens with one is prefilled from there on (tokens and logits bit-identical to a cold prefill).  Off by
-        default: a resident prefix is a timing side channel between the engine's users."""
+        default: a resident prefix is a timing side channel between the engine's users.
+
+        kv_cache_tokens: the KV cache, a pool of 64-token pages the decode rows share; None = max_batch x ctx_max (the pool
+        never binds).  Otherwise a multiple of 64 in [ctx_max, max_batch x ctx_max].  ctx_max is then the limit of one
+        request (prompt + max_new_tokens), and each choice reserves ceil((prompt + max_new_tokens) / 64) pages while it
+        runs; a request that does not fit waits, and one that never could is refused at submit."""
         if not torch.cuda.is_available():
             raise RuntimeError("rr_b200.Engine needs a CUDA device (no CPU fallback)")
         self.spec: ModelSpec = weights.spec
@@ -72,6 +78,7 @@ class Engine:
         self.ctx_max = ctx_max
         self.max_prefill_tokens = max_prefill_tokens
         self.prefix_cache = bool(prefix_cache)
+        self.kv_cache_tokens = int(kv_cache_tokens or max_batch * ctx_max)
         s = self.spec
         desc = _lib.ModelDesc(s.vocab, s.hidden, s.inter, s.n_layers, s.n_heads, s.n_kv_heads,
                               s.head_dim, s.rope_theta, s.rms_eps)
@@ -104,7 +111,7 @@ class Engine:
                                weights.final_norm.data_ptr(), *self._arrs, 1 if interleave else 0, 0)
         opts = _lib.EngineOpts(device, max_batch, ctx_max, max_prefill_tokens,
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
-                               (C.c_int32 * 4)(),
+                               int(kv_cache_tokens or 0), (C.c_int32 * 3)(),
                                1 if prefix_cache else 0)
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
@@ -241,6 +248,12 @@ class Engine:
 
     def now(self) -> float:
         return _lib.lib.rr_engine_now(self._h)
+
+    def kv_usage(self) -> Tuple[int, int]:
+        """(pages_total, pages_free) of the KV page pool (64 tokens a page)."""
+        tot, free = C.c_int32(), C.c_int32()
+        _lib.check(_lib.lib.rr_engine_kv_usage(self._h, C.byref(tot), C.byref(free)), "rr_engine_kv_usage")
+        return tot.value, free.value
 
     def stats(self) -> dict:
         s = _lib.EngineStats()

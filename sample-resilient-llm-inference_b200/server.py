@@ -155,9 +155,18 @@ def create_app(router: Router):
 
 
 def build_backends(cfg: RouterConfig, stub: bool, spec_override: Optional[str] = None, max_batch: int = 64,
-                   ctx_max: int = 1024) -> Dict[int, object]:
-    """One backend per replica (GPU) named in the config; deployments on the same GPU share it."""
+                   ctx_max: Optional[int] = None) -> Dict[int, object]:
+    """One backend per replica (GPU) named in the config; deployments on the same GPU share it.  Each engine serves the
+    deployment's litellm_params.context_window (ctx_max overrides it) with its kv_cache_tokens pool (None: the full
+    max_batch x context window).  A pool outside [context window, max_batch x context window] raises ValueError before
+    any engine is created."""
     backends: Dict[int, object] = {}
+    for d in cfg.deployments:
+        ctx = ctx_max if ctx_max is not None else d.context_window
+        kv = d.kv_cache_tokens
+        if not stub and kv is not None and not ctx <= kv <= max_batch * ctx:
+            raise ValueError(f"model_list[{d.index}].litellm_params.kv_cache_tokens = {kv} is outside "
+                             f"[{ctx}, {max_batch * ctx}] (context window {ctx}, {max_batch} decode rows)")
     for d in cfg.deployments:
         if d.gpu in backends:
             continue
@@ -166,8 +175,10 @@ def build_backends(cfg: RouterConfig, stub: bool, spec_override: Optional[str] =
             continue
         from .engine import Engine
         spec = resolve_spec(spec_override or d.model)
+        ctx = ctx_max if ctx_max is not None else d.context_window
         backends[d.gpu] = EngineBackend(Engine.synthetic(spec, seed=0, device=d.gpu, max_batch=max_batch,
-                                                         ctx_max=ctx_max, prefix_cache=d.prefix_cache))
+                                                         ctx_max=ctx, prefix_cache=d.prefix_cache,
+                                                         kv_cache_tokens=d.kv_cache_tokens))
     return backends
 
 
