@@ -430,7 +430,11 @@ typedef struct rr_engine_opts {
     int32_t device;
     int32_t max_batch;            /* decode rows / KV slots (<= 256) */
     int32_t ctx_max;              /* tokens per request (prompt + max_new_tokens), a multiple of 64 */
-    int32_t max_prefill_tokens;   /* tokens per prefill chunk */
+    int32_t max_prefill_tokens;   /* tokens per prefill chunk.  A prompt whose uncached part does not fit the room left in a
+                                     chunk is prefilled in pieces: its first piece fills that room, each later piece
+                                     (up to this many tokens) leads the next chunk, and after every chunk that leaves it
+                                     in progress the worker runs one decode step for the rows already decoding.  One
+                                     prompt is in progress at a time, and nothing overtakes it. */
     int32_t use_cuda_graph;       /* capture the decode step */
     int32_t fail_seed;            /* fault injection: seed of the Bernoulli failure mask */
     float fail_prob;              /* fault injection: P(request fails) (BASELINE config #4) */
@@ -531,7 +535,7 @@ typedef struct rr_gen_params {
  * A choice that reaches max_new_tokens first finishes with reason 0 (length), in JSON mode with a valid prefix.  The
  * request is done when every choice has finished.
  * RR_INVALID_ARGUMENT, before anything is queued and with *ticket untouched, for a NULL engine, prompt or ticket,
- * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max, a prompt longer than a prefill chunk,
+ * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max,
  * n_choices x ceil((n_prompt + max_new_tokens) / 64) x 64 above kv_cache_tokens (the request could never be admitted), a
  * prompt token outside [0, vocab), and for parameters outside these ranges (NaN is outside every range):
  * 1 <= n_choices <= max_batch; -1 <= top_logprobs <= 20; 0 <= temperature <= 2; 0 <= top_p <= 1; -2 <= penalties <= 2;
@@ -539,7 +543,7 @@ typedef struct rr_gen_params {
  * 0 <= n_stop <= 4 sequences of 1..64 bytes with non-null arrays when n_stop > 0; response_format 0 or 1, and 1 only with
  * vocab >= 259 (some bytes have no token otherwise).  top_logprobs >= 0 and temperature > 0 need a vocabulary that is a
  * multiple of 4.
- * Stats: prefill_tokens counts the prompt once, kv_copy_tokens grows by (n_choices - 1) x the prompt length,
+ * Stats: prefill_tokens counts the prompt once (over all its pieces), kv_copy_tokens grows by (n_choices - 1) x the prompt length,
  * generated_tokens counts every token produced, the ones a stop sequence cut included. */
 int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, const rr_gen_params* p,
                      uint64_t* ticket);
@@ -663,7 +667,7 @@ int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
  * logits to fill pairs from or to mask and no decode loop to cut; RR_INVALID_ARGUMENT for a NULL prompt or ticket;
  * RR_NO_GROUP for an unknown group; RR_INVALID_ARGUMENT (HTTP 400) for n_prompt or max_new_tokens below 1, n_choices
  * outside 1..the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices
- * copies of its reply), prompt + max_new_tokens beyond a replica's context, a prompt beyond its prefill chunk,
+ * copies of its reply), prompt + max_new_tokens beyond a replica's context,
  * n_choices x ceil((prompt + max_new_tokens) / 64) x 64 beyond the smallest KV pool of the gateway's engines (a mock
  * replica sets no KV limit) and a bad token id. */
 int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,

@@ -66,10 +66,11 @@ __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const
 }
 
 // One request of n_choices choices.  Choice c decodes in row rows[c] (== its KV slot); the prompt is prefilled once, into
-// rows[0], and its KV copied to the other rows.  The choices are admitted in one chunk and get one token each per step.  A
+// rows[0], and its KV copied to the other rows.  The choices are admitted together and get one token each per step.  A
 // choice finishes when it holds max_new tokens, a stop sequence cuts it or (JSON mode) its top-level object closes, and
 // gives its row back at once; the request finishes with its last choice.  Without stop sequences or JSON mode that is one
-// step for all of them.
+// step for all of them.  A prompt whose uncached part does not fit the room in a chunk is prefilled in pieces over several
+// chunks (rr_engine::in_progress); its rows are held but do not decode until its last piece has run.
 struct Request {
     uint64_t ticket;
     std::vector<int32_t> prompt;
@@ -89,6 +90,8 @@ struct Request {
     std::vector<std::vector<float>> lp;        // [n_choices][out[c].size()][gen.lp_width()]
     std::vector<std::vector<int32_t>> lp_id;
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
+    int n_done = 0;            // prompt tokens whose KV is in its slot (cached or prefilled), while it is admitted
+    uint64_t epoch = 0;        // prefix caching: rr_engine::index_epoch when its first piece was admitted
 
     // Tokens of choice c a reader may see: all of a finished choice, else those no stop sequence can take back.
     int visible(int c) const { return (int)out[c].size() - (finish[c] < 0 ? hold[c] : 0); }
@@ -345,6 +348,9 @@ struct rr_engine {
     std::vector<int> row_choice;         // [Bm] the choice of row_req[b] that row b decodes
     std::vector<int32_t> h_slot_mirror;  // host mirror of d_slot
     bool slots_dirty = false;
+    // The request whose prompt will still be in progress after the chunk being built (some pieces done, no token yet), or
+    // null.  At most one: it holds its rows and pages, and its next piece leads the next chunk.
+    Request* in_progress = nullptr;
     // prefix caching (o.prefix_cache), under mu: retained[b] = the prompt tokens whose KV the last successful prefill into
     // slot b wrote (computed or copied; never a position decode wrote, since decode rounds differently), kept after the
     // request ends; retained_used[b] = LRU stamp.  index_epoch counts the low-level calls that cleared every list.
@@ -694,7 +700,8 @@ static int init_pf_plans(rr_engine* e) {
 // The tail rows of a prefill chunk: the rows the trimmed last layer, lm_head and the logits tail run on, one per choice of
 // each request.  Row j reads the last token of sequence seq[j], decodes in slot[j] and is choice choice[j] of the request
 // whose parameters are gen[j]; mode = the step_mode bits over gen.  Rows of the same sequence in other slots than the
-// sequence's get its prompt KV copied there.  Without a tail, row i is sequence i in slots[i], plain greedy.
+// sequence's get its prompt KV copied there.  A sequence may have no tail row (a piece of a long prompt that is not its
+// last).  Without a tail, row i is sequence i in slots[i], plain greedy.
 struct PrefillTail {
     int n = 0;
     const int32_t *seq = nullptr, *slot = nullptr, *choice = nullptr;
@@ -712,16 +719,20 @@ struct PrefillTail {
 // tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position
 // pos0 + the sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's
 // logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
-// slots, one launch after the last layer copies positions [0, prompt length) of its slot to each of them.
+// slots, one launch after the last layer copies positions [0, pos0 + its length) of its slot to each of them.
+// A chunk without tail rows (tail->n == 0) stops after the last layer's QKV projection and KV append: nothing after reads
+// its other outputs, and nothing is read back.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
                        const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     const int nt = tail ? tail->n : n_seqs;
-    const bool fan = nt != n_seqs;                     // some sequence has more than one tail row
+    // the tail rows' slots and last tokens are listed apart (h_tsl / h_tlast) unless row j is sequence j in its own slot
+    bool fan = nt != n_seqs;
+    for (int j = 0; tail && !fan && j < nt; ++j) fan = tail->seq[j] != j || tail->slot[j] != slots[j];
     int mode = tail ? tail->mode : 0;
-    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < n_seqs || nt > e->Bm) return RR_INVALID_ARGUMENT;
+    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < 0 || nt > e->Bm) return RR_INVALID_ARGUMENT;
     cudaStream_t s = e->stream;
     // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n] (| pos0[n])
     //                 (| tail_slot[nt] | tail_last[nt] with fan-out)
@@ -750,10 +761,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     for (int j = 0; tail && j < nt; ++j) {
         const int q = tail->seq[j], sl = tail->slot[j];
         if (q < 0 || q >= n_seqs || sl < 0 || sl >= e->Bm) return RR_INVALID_ARGUMENT;
-        if (!fan) {
-            if (q != j || sl != slots[j]) return RR_INVALID_ARGUMENT;
-            continue;
-        }
+        if (!fan) continue;
         h_tsl[j] = sl; h_tlast[j] = h_last[q];
         if (sl == slots[q]) continue;
         const int c = fan_copies.count++;              // < nt <= Bm <= KV_COPY_MAX
@@ -810,6 +818,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ra.n_heads = d.n_heads; ra.n_kv_heads = d.n_kv_heads; ra.ctx_max = e->o.ctx_max; ra.theta = d.rope_theta;
         ra.table = e->rope_table; ra.head_dim = d.head_dim; ra.page_table = e->d_table; ra.pages_per_slot = e->pps;
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
+        if (nt == 0 && l + 1 == d.n_layers) break;    // every layer's KV is written
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer TMA maps made at create
         pa.q = e->pq; pa.k_cache = kc; pa.v_cache = vc; pa.out = e->pattn; pa.seq_start = p_ss; pa.seq_slot = p_sl;
         pa.seq_pos0 = pos0 ? p_p0 : nullptr; pa.n_seqs = n_seqs; pa.max_len = max_len; pa.n_heads = d.n_heads; pa.n_kv_heads = d.n_kv_heads;
@@ -834,12 +843,14 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
             return RR_CUDA_ERROR;
         ++nl;
     }
-    if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..nt-1)
-    nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s, p_tsl);
-    launch_pdl(activate_rows_kernel, dim3((nt + 127) / 128), dim3(128), 0, s, p_tsl, (const int32_t*)e->p_first,
-               (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
-    const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
-    if (rc != RR_OK) return rc;
+    if (nt > 0) {
+        if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..nt-1)
+        nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s, p_tsl);
+        launch_pdl(activate_rows_kernel, dim3((nt + 127) / 128), dim3(128), 0, s, p_tsl, (const int32_t*)e->p_first,
+                   (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
+        const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
+        if (rc != RR_OK) return rc;
+    }
     if (logits_host) {
         CK(cudaMemcpyAsync(logits_host, e->logits, sizeof(float) * (size_t)n_seqs * d.vocab, cudaMemcpyDeviceToHost, s));
     }
@@ -1008,7 +1019,18 @@ static void release_row(rr_engine* e, Request* r, int c) {
 static void release_request(rr_engine* e, Request* r, int status, std::vector<DoneNote>* notes) {
     for (int c = 0; c < (int)r->rows.size(); ++c) release_row(e, r, c);
     r->rows.clear();
+    if (e->in_progress == r) e->in_progress = nullptr;
     finish_request(e, r, status, notes);
+}
+
+// Caller holds e->mu.  Prefix caching: a low-level call cleared the index after r was admitted, so its match and the KV of
+// its done pieces may be stale.  r gives its rows and pages back (nothing retained) and goes back to the head of the queue,
+// to start again from position 0.
+static void requeue(rr_engine* e, Request* r) {
+    for (int b : r->rows) { e->row_req[b] = nullptr; resize_pages(e, b, 0); }
+    r->rows.clear(); r->n_cached = 0; r->n_done = 0;
+    if (e->in_progress == r) e->in_progress = nullptr;
+    e->waiting.push_front(r);
 }
 
 // Caller holds e->mu.  Appends the token read back for row `row` to choice c of r, with its pairs (h_lp / h_lp_id row
@@ -1099,17 +1121,22 @@ static void worker_main(rr_engine* e) {
     KvCopyList* copies = new KvCopyList();
     std::vector<int32_t> tail_seq, tail_slot, tail_choice;      // the chunk's tail rows (PrefillTail), one per choice
     std::vector<const GenParams*> tail_gen;
+    bool decode_due = false;         // the last chunk left a prompt in progress: one decode step goes before the next chunk
     while (!e->stop.load()) {
         run_hooks(e, notes);
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
         chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
         tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear();
         copies->count = 0;
-        int active = 0;
-        int step = 0, chunk_mode = 0;                      // step_mode bits of the active rows / of the chunk's requests
+        int active = 0, decoding = 0;                      // rows held / rows decoding (not the prompt in progress's)
+        int step = 0, chunk_mode = 0;                      // step_mode bits of the decoding rows / of the chunk's tail rows
+        bool resumed = false;                              // the chunk continues a prompt in progress
         uint64_t epoch = 0;
         {
             std::unique_lock<std::mutex> lk(e->mu);
+            epoch = e->index_epoch;
+            Request* ip = e->in_progress;
+            if (ip && !ip->cancel && e->o.prefix_cache && ip->epoch != epoch) { requeue(e, ip); ip = nullptr; }
             for (int b = 0; b < e->Bm; ++b) {
                 Request* r = e->row_req[b];
                 if (!r) continue;
@@ -1118,19 +1145,41 @@ static void worker_main(rr_engine* e) {
                     continue;
                 }
                 ++active;
+                if (r == e->in_progress) continue;         // held for its next piece: no token yet
+                ++decoding;
                 step |= step_mode(r->gen);
             }
+            ip = e->in_progress;
             if (e->waiting.empty() && active == 0) {
                 if (!notes.empty()) continue;              // report the requests a cancel just ended before idling
                 e->st.queued = 0; e->st.active_rows = 0;   // idle: every row is free and every done hook has run
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
                 continue;
             }
+            // a running reply waits at most one chunk between tokens, however many pieces a long prompt takes
+            const bool decode_first = decode_due && decoding > 0;
+            decode_due = false;
+            if (ip && !decode_first) {                     // its next piece goes first: min(Tmax, remaining) tokens
+                const int n = std::min(e->Tmax, (int)ip->prompt.size() - ip->n_done);
+                chunk.push_back(ip);
+                slots.push_back(ip->rows[0]);
+                pos0.push_back(ip->n_done);
+                ids.insert(ids.end(), ip->prompt.begin() + ip->n_done, ip->prompt.begin() + ip->n_done + n);
+                seq_start.push_back((int)ids.size());
+                resumed = true;
+                if (ip->n_done + n == (int)ip->prompt.size()) {     // its last piece: the tail rows of its choices
+                    for (int c = 0; c < ip->n_choices; ++c) {
+                        tail_seq.push_back(0); tail_slot.push_back(ip->rows[c]); tail_choice.push_back(c);
+                        tail_gen.push_back(&ip->gen);
+                    }
+                    chunk_mode |= step_mode(ip->gen);
+                    e->in_progress = nullptr;
+                }
+            }
             int b = 0;
-            epoch = e->index_epoch;
-            while (!e->waiting.empty()) {
+            while (!decode_first && !e->waiting.empty()) {
                 Request* r = e->waiting.front();
-                if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all in this chunk
+                if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all at its admission
                 int m = 0, src = -1;
                 if (e->o.prefix_cache) {
                     if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
@@ -1138,19 +1187,28 @@ static void worker_main(rr_engine* e) {
                     while (b < e->Bm && e->row_req[b] != nullptr) ++b;
                     if (b >= e->Bm) break;
                 }
-                if ((int)ids.size() + (int)r->prompt.size() - m > e->Tmax) break;   // a chunk holds Tmax uncached tokens
+                // a chunk holds Tmax uncached tokens; with no prompt in progress, one that does not fit the room left
+                // starts with a piece that fills it
+                int n = (int)r->prompt.size() - m;
+                const int room = e->Tmax - (int)ids.size();
+                if (n > room) {
+                    if (e->in_progress || room == 0) break;
+                    n = room;
+                }
                 // every choice reserves its pages now; a request that does not fit waits at the head of the queue
                 if (r->n_choices * pages_for((int)r->prompt.size() + r->max_new) > pages_available(e)) break;
                 e->waiting.pop_front();
                 r->n_cached = m;
+                r->n_done = m;
                 if (e->o.prefix_cache) {
                     if (m > 0) e->retained_used[src >= 0 ? src : b] = ++e->lru_clock;
                     if (src >= 0) {
                         const int c = copies->count++;
                         copies->src[c] = src; copies->dst[c] = b; copies->n[c] = m;
                     }
-                    pos0.push_back(m);
                 }
+                pos0.push_back(m);
+                const bool last = m + n == (int)r->prompt.size();
                 for (int c = 0; c < r->n_choices; ++c) {   // choice 0 in the prompt's slot, the others in free ones
                     if (c > 0) {
                         if (e->o.prefix_cache) b = pick_slot_miss(e);
@@ -1159,15 +1217,17 @@ static void worker_main(rr_engine* e) {
                     e->row_req[b] = r;
                     e->row_choice[b] = c;
                     r->rows.push_back(b);
-                    if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this chunk; set again once it succeeds
+                    if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this prompt; set again once it succeeds
+                    if (!last) continue;
                     tail_seq.push_back((int)chunk.size()); tail_slot.push_back(b); tail_choice.push_back(c);
                     tail_gen.push_back(&r->gen);
                 }
                 take_pages(e, r);
                 chunk.push_back(r);
                 slots.push_back(r->rows[0]);
-                chunk_mode |= step_mode(r->gen);
-                ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.end());
+                if (last) chunk_mode |= step_mode(r->gen);
+                else { e->in_progress = r; r->epoch = epoch; }
+                ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.begin() + m + n);
                 seq_start.push_back((int)ids.size());
                 active += r->n_choices;
             }
@@ -1178,15 +1238,10 @@ static void worker_main(rr_engine* e) {
         std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
         if (!chunk.empty() && e->o.prefix_cache) {
             // a low-level call took the GPU between admission and here and cleared the index: its matches may be stale,
-            // so the chunk goes back to the head of the queue and is admitted again
+            // so the chunk goes back to the head of the queue and is admitted again (a prompt in progress from position 0)
             std::lock_guard<std::mutex> lk(e->mu);
             if (e->index_epoch != epoch) {
-                for (size_t i = chunk.size(); i-- > 0;) {
-                    Request* r = chunk[i];
-                    for (int b : r->rows) { e->row_req[b] = nullptr; resize_pages(e, b, 0); }   // nothing retained
-                    r->rows.clear(); r->n_cached = 0;
-                    e->waiting.push_front(r);
-                }
+                for (size_t i = chunk.size(); i-- > 0;) requeue(e, chunk[i]);
                 continue;
             }
         }
@@ -1200,17 +1255,21 @@ static void worker_main(rr_engine* e) {
             if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache ? pos0.data() : nullptr, copies, &tail);
+                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail);
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             int j = 0;                                     // the request's first tail row
-            for (Request* r : chunk) {
+            for (size_t i = 0; i < chunk.size(); ++i) {
+                Request* r = chunk[i];
                 const int row0 = j;
-                j += r->n_choices;
+                const bool last = pos0[i] + seq_start[i + 1] - seq_start[i] == (int)r->prompt.size();
+                if (last) j += r->n_choices;
                 if (rc != RR_OK) {
                     release_request(e, r, RR_INTERNAL, &notes);
                     continue;
                 }
+                r->n_done = pos0[i] + seq_start[i + 1] - seq_start[i];
+                if (!last) continue;                       // the prompt in progress: its next piece leads the next chunk
                 if (e->o.prefix_cache) {                   // every choice's slot holds the prompt's prefill-written KV
                     for (int b : r->rows) { e->retained[b] = r->prompt; e->retained_used[b] = ++e->lru_clock; }
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
@@ -1222,10 +1281,11 @@ static void worker_main(rr_engine* e) {
                 }
                 if (r->all_finished()) release_request(e, r, RR_OK, &notes);
             }
+            decode_due = e->in_progress != nullptr;
             e->cv_done.notify_all();
             continue;   // look for more waiting prompts before decoding
         }
-        if (active == 0) continue;
+        if (decoding == 0) continue;
         // ---- one decode step for all active rows
         cudaStream_t s = e->stream;
         if (e->slots_dirty) {
@@ -1253,6 +1313,7 @@ static void worker_main(rr_engine* e) {
                 Request* r = e->row_req[b];
                 if (!r) continue;
                 if (rc != RR_OK) { release_request(e, r, RR_INTERNAL, &notes); continue; }
+                if (r == e->in_progress) continue;         // its rows are inactive on the device
                 const int c = e->row_choice[b];
                 if (!take_token(e, r, c, b)) continue;
                 release_row(e, r, c);                      // the row is free for the next waiting prompt at once
@@ -1557,7 +1618,7 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     // the vocabularies the logprobs / sampling kernels handle
     if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
-    if (n_prompt + max_new_tokens > e->o.ctx_max || n_prompt > e->Tmax) return RR_INVALID_ARGUMENT;
+    if (n_prompt + max_new_tokens > e->o.ctx_max) return RR_INVALID_ARGUMENT;
     if ((long long)n_choices * pages_for(n_prompt + max_new_tokens) > e->n_pages) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
         if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
@@ -1601,12 +1662,11 @@ void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx) {
     std::lock_guard<std::mutex> lk(e->mu);
     e->hook = fn; e->hook_ctx = ctx;
 }
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch, int* kv_tokens) {
+int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens) {
     if (!e) return RR_INVALID_ARGUMENT;
     if (kv_tokens) *kv_tokens = e->n_pages * KV_PAGE;
     if (max_batch) *max_batch = e->Bm;
     if (ctx_max) *ctx_max = e->o.ctx_max;
-    if (max_prefill) *max_prefill = e->Tmax;
     if (vocab) *vocab = e->d.vocab;
     return RR_OK;
 }

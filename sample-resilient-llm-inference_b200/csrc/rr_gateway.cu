@@ -83,7 +83,7 @@ struct rr_gateway {
     std::unordered_map<int, int> by_replica;   // replica id -> index into engines
     int n_deps = 0, n_groups = 0;
     bool latency = false;                   // the router is latency-based: DONE / FAIL events carry samples
-    int min_ctx = 0, min_pf = 0, min_vocab = 0, min_rows = 0;     // min_rows: decode rows, the limit of n_choices
+    int min_ctx = 0, min_vocab = 0, min_rows = 0;     // min_rows: decode rows, the limit of n_choices
     int min_kv = 0;                                               // the smallest KV pool in tokens (rr_engine_opts.kv_cache_tokens)
     rr_gateway_opts opts;
 
@@ -379,15 +379,15 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
     memset(&g->st, 0, sizeof(g->st));
     rr::router_shape(router, &g->n_deps, &g->n_groups);
     g->latency = rr::router_strategy(router) == RR_STRATEGY_LATENCY_BASED;
-    g->min_ctx = g->min_pf = g->min_vocab = g->min_rows = g->min_kv = 0x7fffffff;
+    g->min_ctx = g->min_vocab = g->min_rows = g->min_kv = 0x7fffffff;
     g->stubs.assign((size_t)n_engines, rr_stub_desc{0, 0, 0, 0});
     g->stub_handed.assign((size_t)n_engines, 0);
     for (int i = 0; i < n_engines; ++i) {
         g->engines.push_back(engines[i]);
         g->by_replica[replica_ids[i]] = i;
-        int c = 0x7fffffff, p = 0x7fffffff, v = 0, rows = 0x7fffffff, kv = 0x7fffffff;   // a mock replica: no KV limit
+        int c = 0x7fffffff, v = 0, rows = 0x7fffffff, kv = 0x7fffffff;   // a mock replica: no KV limit
         if (engines[i]) {
-            rr::engine_limits(engines[i], &c, &p, &v, &rows, &kv);
+            rr::engine_limits(engines[i], &c, &v, &rows, &kv);
         } else {
             if (!stubs || stubs[i].reply_tokens < 0 || stubs[i].fail_every < 0 || stubs[i].vocab < 1) {
                 delete g;
@@ -398,7 +398,6 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
             v = stubs[i].vocab;
         }
         if (c < g->min_ctx) g->min_ctx = c;
-        if (p < g->min_pf) g->min_pf = p;
         if (v < g->min_vocab) g->min_vocab = v;
         if (rows < g->min_rows) g->min_rows = rows;
         if (kv < g->min_kv) g->min_kv = kv;
@@ -439,7 +438,7 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
     if (group < 0 || group >= g->n_groups) return RR_NO_GROUP;
     if (!ids || n_prompt < 1 || max_new < 1) return RR_INVALID_ARGUMENT;
     if (n_choices < 1 || n_choices > g->min_rows) return RR_INVALID_ARGUMENT;     // every choice takes a decode row
-    if (n_prompt + max_new > g->min_ctx || n_prompt > g->min_pf) return RR_INVALID_ARGUMENT;   // -> HTTP 400, before any debit
+    if (n_prompt + max_new > g->min_ctx) return RR_INVALID_ARGUMENT;   // -> HTTP 400, before any debit
     // every choice reserves whole 64-token KV pages of the smallest pool (rr_engine_submit)
     if ((long long)n_choices * ((n_prompt + max_new + 63) / 64) * 64 > g->min_kv) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)

@@ -135,7 +135,7 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
                          uint64_t* ticket, const GenParams& p, int n_choices);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 // kv_tokens: the KV pool (rr_engine_opts.kv_cache_tokens after its default is applied)
-int engine_limits(const rr_engine* e, int* ctx_max, int* max_prefill, int* vocab, int* max_batch, int* kv_tokens = nullptr);
+int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens = nullptr);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
 int router_strategy(const rr_router* r);

@@ -505,25 +505,22 @@ class Router:
             _fell_back=res.chain_pos > 0, _ttft_s=res.t_first_token_s - res.t_submit_s,
             _latency_s=time.perf_counter() - t_start, _choice_token_ids=rows)
 
-    def _limits(self) -> Tuple[int, int, int, int]:
-        """(context window, prefill chunk, decode rows, KV cache tokens) of the smallest engine replica attached; a mock
-        replica sets none."""
+    def _limits(self) -> Tuple[int, int, int]:
+        """(context window, decode rows, KV cache tokens) of the smallest engine replica attached; a mock replica sets
+        none."""
         engs = [b.engine for b in self.backends.values() if isinstance(b, EngineBackend)]
         big = 2**31 - 1
-        return (min((e.ctx_max for e in engs), default=big), min((e.max_prefill_tokens for e in engs), default=big),
-                min((e.max_batch for e in engs), default=big), min((e.kv_cache_tokens for e in engs), default=big))
+        return (min((e.ctx_max for e in engs), default=big), min((e.max_batch for e in engs), default=big),
+                min((e.kv_cache_tokens for e in engs), default=big))
 
     def _invalid(self, n_prompt: int = 0, max_new: int = 0, n: int = 1) -> BadRequestError:
         """The HTTP 400 of a request the gateway refused with RR_INVALID_ARGUMENT, naming the limit it broke."""
-        ctx, pf, rows, kv = self._limits()
+        ctx, rows, kv = self._limits()
         if n > rows:
             return BadRequestError(f"`n` = {n} exceeds the {rows} decode rows of the smallest replica")
         if n_prompt + max_new > ctx:
             return BadRequestError(f"prompt ({n_prompt} tokens) + max_tokens ({max_new}) exceed the context window "
                                    f"({ctx} tokens) of the deployment")
-        if n_prompt > pf:
-            return BadRequestError(f"the prompt ({n_prompt} tokens) exceeds the prefill chunk ({pf} tokens) of the "
-                                   "deployment")
         if n * -(-(n_prompt + max_new) // 64) * 64 > kv:
             return BadRequestError(f"`n` ({n}) x (prompt ({n_prompt} tokens) + max_tokens ({max_new})), in 64-token pages, "
                                    f"exceed the KV cache ({kv} tokens) of the deployment")
@@ -771,7 +768,7 @@ class Router:
         if prompt_ids is None:
             prompt_ids = tokenize(messages_to_text(messages or []), self._vocab())
         max_new = max_tokens or self.default_max_tokens
-        if n > self._limits()[2]:
+        if n > self._limits()[1]:
             raise self._invalid(n=n)
         return self._completion_gw(self._gateway(), model, g, prompt_ids, max_new, timeout, gen)
 
