@@ -198,6 +198,24 @@ enum { RR_OUT_ROWMAJOR_BF16 = 0, RR_OUT_TRANSPOSED_F32 = 1,
 int rr_gemm_bf16(const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
                  void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream);
 
+/* FP8 weights.  A weight W [rows, K] bf16 is stored as Q [rows, K] e4m3 (row pitch K bytes) and one fp32 scale per row,
+ * scale[n] = 2^e[n], e[n] = the smallest integer with max_k |W[n, k]| <= 448 * 2^e, clamped to [-117, 127] (0 for an
+ * all-zero row); Q = e4m3 round-to-nearest-even of W / 2^e[n], subnormals included (it never saturates).
+ * D = bf16(Q * scale) is exact for every row the quantizer accepts.  Q pointers must be 16-byte aligned and K a positive
+ * multiple of 16.
+ * quantize: w bf16 [rows, ld] (16-byte aligned, ld % 8 == 0, ld >= K).  Synchronises the stream.  RR_INVALID_ARGUMENT
+ *   before touching the device for a bad argument, and after the kernel when a row holds Inf or NaN, or has a largest
+ *   magnitude within 2^-4 of bf16's largest finite value (its e4m3 code times 2^e would be inf); those rows of q_out and
+ *   scale_out are not written.
+ * dequantize: out bf16 [rows, ld_out] = bf16(Q * scale) exactly (16-byte aligned, ld_out % 8 == 0, ld_out >= K). */
+int rr_op_quantize_fp8_weight(const void* w, int rows, int K, int ld, void* q_out, float* scale_out, void* stream);
+int rr_op_dequantize_fp8_weight(const void* q, const float* scale, int rows, int K, void* out, int ld_out, void* stream);
+/* rr_gemm_bf16's decode modes (RR_OUT_TRANSPOSED_F32 / _SILU) with A an e4m3 weight [rowsA, K] (pitch ldA bytes, a
+ * multiple of 16) and its row scales: the same tiles, splits, summation order and epilogues as rr_gemm_bf16 on
+ * D = bf16(A * scale), so the same output bits.  RR_INVALID_ARGUMENT for a row-major mode or a null scale. */
+int rr_gemm_fp8w(const void* A, const float* scale, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
+                 void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream);
+
 int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows, int hidden,
                 const int32_t* row_active, void* stream);
 int rr_op_add_rmsnorm(float* x, const void* part, int part_is_bf16, int n_splits,
@@ -342,6 +360,11 @@ int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers, int n
  * ld_rows >= rows, hidden and inter are positive multiples of 64, hidden <= 8192 and no pointer is null. */
 int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
                      void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream);
+/* The same with e4m3 weights (rr_op_quantize_fp8_weight) and their row scales (wgu_scale interleaved like the rows):
+ * bit for bit rr_op_decode_mlp on the dequantized weights.  Also RR_INVALID_ARGUMENT for a null scale. */
+int rr_op_decode_mlp_fp8(const void* wgu_il, const float* wgu_scale, const void* wdown, const float* wdown_scale,
+                         const void* xn, int rows, int hidden, int inter, void* act, void* planes, int ld_rows,
+                         int* n_slices, int* slice_kb, void* stream);
 /* Decode attention, one step exactly as the engine runs it: RoPE and the KV append fused in, scale 1 / sqrt(head_dim), the
  * engine's kv-split rule (returned in *kv_splits) and RoPE table (theta); env RR_ATTN_NO_TRIM is read per call.
  *   qkv      fp32 split-K planes [n_splits][..][ld], plane z of row b at qkv + z * split_stride + b * ld; columns are the
@@ -419,10 +442,22 @@ typedef struct rr_model_weights {
     const void* const* norm_mlp;  /* n_layers x [hidden] */
     int32_t flags;                /* RR_WEIGHTS_* */
     int32_t reserved;
+    /* RR_WEIGHTS_FP8_E4M3 only (ignored otherwise): n_layers x fp32 [out_features] row scales of wqkv / wo / wgu / wdown */
+    const void* const* wqkv_scale;
+    const void* const* wo_scale;
+    const void* const* wgu_scale;
+    const void* const* wdown_scale;
 } rr_model_weights;
 /* wgu rows are interleaved in 64-row gate/up blocks [g0..g63, u0..u63, g64.., u64.., ...] instead of
  * [gate; up]: enables the fused SiLU*mul GEMM epilogues (no separate activation kernel). */
 #define RR_WEIGHTS_WGU_INTERLEAVED64 1
+/* wqkv / wo / wgu / wdown are e4m3 [out_features, in_features] (rr_op_quantize_fp8_weight: 16-byte aligned) with the row
+ * scales above (with RR_WEIGHTS_WGU_INTERLEAVED64 the wgu rows and their scales are interleaved alike); embed, lm_head
+ * and the norms stay bf16.  The engine computes exactly what a bf16 engine computes on D = bf16(Q * scale): decode
+ * converts the e4m3 tiles in its GEMMs, prefill dequantizes each layer into an engine-owned bf16 scratch of one layer's
+ * four projections (2 x (nqkv + nq + 3 inter) x hidden bytes) before the layer's GEMMs.  rr_engine_create returns
+ * RR_INVALID_ARGUMENT before any CUDA call for a null or misaligned e4m3 pointer or a null scale pointer. */
+#define RR_WEIGHTS_FP8_E4M3 2
 
 typedef struct rr_engine rr_engine;
 

@@ -69,11 +69,17 @@ class ModelDesc(C.Structure):
                 ("head_dim", C.c_int32), ("rope_theta", C.c_float), ("rms_eps", C.c_float)]
 
 
+RR_WEIGHTS_WGU_INTERLEAVED64 = 1
+RR_WEIGHTS_FP8_E4M3 = 2
+
+
 class ModelWeights(C.Structure):
     _fields_ = [("embed", vp), ("lm_head", vp), ("final_norm", vp),
                 ("wqkv", C.POINTER(vp)), ("wo", C.POINTER(vp)), ("wgu", C.POINTER(vp)),
                 ("wdown", C.POINTER(vp)), ("norm_attn", C.POINTER(vp)),
-                ("norm_mlp", C.POINTER(vp)), ("flags", C.c_int32), ("reserved", C.c_int32)]
+                ("norm_mlp", C.POINTER(vp)), ("flags", C.c_int32), ("reserved", C.c_int32),
+                ("wqkv_scale", C.POINTER(vp)), ("wo_scale", C.POINTER(vp)), ("wgu_scale", C.POINTER(vp)),
+                ("wdown_scale", C.POINTER(vp))]
 
 
 class EngineOpts(C.Structure):
@@ -157,6 +163,10 @@ PROTOTYPES = {
     "rr_tokenize_batch_device": (C.c_int, [vp, vp, C.c_int, C.c_int64, C.c_int32, vp, vp, vp, vp]),
     "rr_gemm_bf16": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int,
                                C.c_int, C.c_int, C.c_int, C.c_int, vp]),
+    "rr_gemm_fp8w": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int,
+                               C.c_int, C.c_int, C.c_int, C.c_int, vp]),
+    "rr_op_quantize_fp8_weight": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
+    "rr_op_dequantize_fp8_weight": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
     "rr_op_embed": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "rr_op_add_rmsnorm": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp, vp,
                                     C.c_int, C.c_int, C.c_float, vp]),
@@ -183,6 +193,7 @@ PROTOTYPES = {
     "rr_op_kv_copy_prefix_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int,
                                              vp, C.c_int, C.c_int, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
+    "rr_op_decode_mlp_fp8": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp]),
     "rr_op_decode_attn_qkv_paged": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,

@@ -11,7 +11,9 @@ b200/<spec>` names an on-box model (models.SPECS) instead of `bedrock/<id>`; `li
 prompt prefix caching in the replica; `litellm_params.context_window: N` is the longest request (prompt + max_tokens, in
 tokens) the replica serves, a positive multiple of 64, default 1024; `litellm_params.kv_cache_tokens: N` sizes the replica's
 KV cache, a pool of 64-token pages its decode rows share: a multiple of 64 in [context_window, max_batch x context_window],
-default the full max_batch x context_window.  Deployments on one GPU share its engine, so they must agree on all three.
+default the full max_batch x context_window; `litellm_params.quantization: fp8` stores the replica's layer projections as
+e4m3 weights with power-of-two row scales (absent or null: bf16).  Deployments on one GPU share its engine, so they must
+agree on all four.
 """
 from __future__ import annotations
 
@@ -24,6 +26,10 @@ STRATEGIES = {"simple-shuffle": 0, "least-busy": 1, "round-robin": 2, "split": 3
               "latency-based-routing": 5}
 _INT32_MAX = 2**31 - 1
 _PROVIDER_PREFIXES = ("bedrock/", "b200/", "openai/", "azure/")
+
+
+# litellm_params.quantization values: None = bf16 weights
+QUANTIZATIONS = (None, "fp8")
 
 
 def strip_provider(model: str) -> str:
@@ -48,6 +54,7 @@ class DeploymentCfg:
     prefix_cache: bool = False  # litellm_params.prefix_cache: the replica reuses cached prompt prefixes
     context_window: int = 1024  # litellm_params.context_window: prompt + max_tokens of one request, a multiple of 64
     kv_cache_tokens: Optional[int] = None   # litellm_params.kv_cache_tokens: the KV pool; None = max_batch x context_window
+    quantization: Optional[str] = None      # litellm_params.quantization: None (bf16 weights) or "fp8" (e4m3 projections)
     params: Dict[str, Any] = field(default_factory=dict)
 
     @property
@@ -142,12 +149,16 @@ def build_config(model_list: List[dict], router_settings: Optional[dict] = None,
         if kv is not None and (isinstance(kv, bool) or not isinstance(kv, int) or kv < cw or kv % 64):
             raise ValueError(f"model_list[{i}].litellm_params.kv_cache_tokens must be a multiple of 64 of at least "
                              f"context_window ({cw}), got {kv!r}")
+        qz = lp.get("quantization")
+        if qz not in QUANTIZATIONS:
+            raise ValueError(f"model_list[{i}].litellm_params.quantization must be null or one of "
+                             f"{sorted(q for q in QUANTIZATIONS if q)}, got {qz!r}")
         deps.append(DeploymentCfg(index=i, model_name=name, model=lp["model"], group=groups.index(name),
                                   rpm=rpm, tpm=tpm, gpu=int(lp.get("gpu", 0)), prefix_cache=pc, context_window=cw,
-                                  kv_cache_tokens=kv, params=lp))
+                                  kv_cache_tokens=kv, quantization=qz, params=lp))
     for d in deps:                       # one engine per GPU: its deployments share the settings
         first = next(x for x in deps if x.gpu == d.gpu)
-        for key in ("prefix_cache", "context_window", "kv_cache_tokens"):
+        for key in ("prefix_cache", "context_window", "kv_cache_tokens", "quantization"):
             if getattr(d, key) != getattr(first, key):
                 raise ValueError(f"model_list[{first.index}] and model_list[{d.index}] share gpu {d.gpu} but disagree on "
                                  f"litellm_params.{key}")

@@ -140,6 +140,45 @@ RR_API int rr_gemm_bf16(const void* A, int rowsA, int ldA, const void* B, int ro
     return rc;
 }
 
+RR_API int rr_gemm_fp8w(const void* A, const float* scale, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
+                        void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream) {
+    GemmPlan p;
+    int rc = gemm_plan_init_fp8w(&p, A, scale, rowsA, ldA, B, rowsB, ldB, K, out, ldo, ld_rows, splits, mode, bn);
+    if (rc != RR_OK) return rc;
+    rc = gemm_launch(p, (cudaStream_t)stream);
+    if (rc != RR_OK) note_cuda_error(cudaPeekAtLastError());
+    return rc;
+}
+
+RR_API int rr_op_quantize_fp8_weight(const void* w, int rows, int K, int ld, void* q_out, float* scale_out, void* stream) {
+    if (!w || !scale_out || rows < 1 || ld < K || ld % 8 || ((uintptr_t)w & 15) || !fp8_weight_ok(q_out, K))
+        return RR_INVALID_ARGUMENT;
+    cudaStream_t st = (cudaStream_t)stream;
+    int* bad = nullptr;
+    int h_bad = 0;
+    cudaError_t e = cudaMallocAsync(&bad, sizeof(int), st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(bad, 0, sizeof(int), st);
+    int rc = RR_CUDA_ERROR;
+    if (e == cudaSuccess)
+        rc = launch_quantize_fp8((const __nv_bfloat16*)w, rows, K, ld, (uint8_t*)q_out, scale_out, bad, st);
+    if (rc == RR_OK) e = cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (bad) cudaFreeAsync(bad, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { note_cuda_error(e); return RR_CUDA_ERROR; }
+    if (rc != RR_OK) { note_cuda_error(cudaPeekAtLastError()); return rc; }
+    return h_bad ? RR_INVALID_ARGUMENT : check_last();
+}
+
+RR_API int rr_op_dequantize_fp8_weight(const void* q, const float* scale, int rows, int K, void* out, int ld_out, void* stream) {
+    if (!scale || !out || rows < 1 || !fp8_weight_ok(q, K) || ld_out < K || ld_out % 8 || ((uintptr_t)out & 15))
+        return RR_INVALID_ARGUMENT;
+    Fp8DequantJobs J;
+    fp8_dequant_job(&J, q, scale, rows, K, (__nv_bfloat16*)out, ld_out);
+    const int rc = launch_dequantize_fp8(J, (cudaStream_t)stream);
+    if (rc != RR_OK) { note_cuda_error(cudaPeekAtLastError()); return rc; }
+    return check_last();
+}
+
 static PartIn mk_part(const void* p, int is_bf16, int n_splits, long long split_stride, int ld) {
     PartIn r;
     r.ptr = p; r.is_bf16 = is_bf16; r.n_splits = n_splits < 1 ? 1 : n_splits;
@@ -489,8 +528,8 @@ RR_API int rr_op_prefill_gemm(const void* A, int plan_rows, int T, int ldA, cons
 
 // The fused decode MLP as the engine runs it (rr_engine_create): tile width, K slices, grid and schedule come from the same
 // helpers and environment switches; the schedule and the dependency counters live in stream-ordered scratch memory.
-RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
-                            void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream) {
+static int decode_mlp(const void* wgu_il, const float* sc_gu, const void* wdown, const float* sc_down, const void* xn, int rows,
+                      int hidden, int inter, void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream) {
     if (!wgu_il || !wdown || !xn || !act || !planes || !n_slices || !slice_kb) return RR_INVALID_ARGUMENT;
     // the engine fuses the MLP for batches of 17..MAX_BN rows (tile width >= 32, one batch tile)
     if (rows <= 16 || rows > MAX_BN || ld_rows < rows) return RR_INVALID_ARGUMENT;
@@ -512,7 +551,7 @@ RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* x
     if (e == cudaSuccess) {
         MlpPlan p;
         rc = mlp_plan_init(&p, wgu_il, wdown, inter, hidden, xn, rows, act, planes, ld_rows, pick_bn(rows), items, max_items,
-                           grid, ready, skb, dyn);
+                           grid, ready, skb, dyn, sc_gu, sc_down);
         if (rc == RR_OK) rc = mlp_launch(p, st);
     }
     if (e != cudaSuccess) note_cuda_error(e);
@@ -523,6 +562,19 @@ RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* x
     *n_slices = ns;
     *slice_kb = skb;
     return check_last();
+}
+
+RR_API int rr_op_decode_mlp(const void* wgu_il, const void* wdown, const void* xn, int rows, int hidden, int inter,
+                            void* act, void* planes, int ld_rows, int* n_slices, int* slice_kb, void* stream) {
+    return decode_mlp(wgu_il, nullptr, wdown, nullptr, xn, rows, hidden, inter, act, planes, ld_rows, n_slices, slice_kb, stream);
+}
+
+RR_API int rr_op_decode_mlp_fp8(const void* wgu_il, const float* wgu_scale, const void* wdown, const float* wdown_scale,
+                                const void* xn, int rows, int hidden, int inter, void* act, void* planes, int ld_rows,
+                                int* n_slices, int* slice_kb, void* stream) {
+    if (!wgu_scale || !wdown_scale || !fp8_weight_ok(wgu_il, hidden) || !fp8_weight_ok(wdown, inter)) return RR_INVALID_ARGUMENT;
+    return decode_mlp(wgu_il, wgu_scale, wdown, wdown_scale, xn, rows, hidden, inter, act, planes, ld_rows, n_slices,
+                      slice_kb, stream);
 }
 
 RR_API int rr_debug_mlp_schedule(int grid, int inter, int hidden, int slice_kb, int32_t* items_out, int capacity,

@@ -260,6 +260,11 @@ struct rr_engine {
     int Bm, bn_dec, nq, nkv_dim, nqkv;
     std::vector<const void*> wqkv, wo, wgu, wdown, norm_attn, norm_mlp;
     const void *embed, *lm_head, *final_norm;
+    // RR_WEIGHTS_FP8_E4M3: the projections are e4m3 with these row scales; prefill dequantizes layer l into deq (one layer's
+    // wqkv | wo | wgu | wdown, bf16) before its GEMMs, and the prefill plans read deq
+    bool fp8 = false;
+    std::vector<const float*> sqkv, so, sgu, sdown;
+    __nv_bfloat16* deq = nullptr;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     std::vector<void*> allocs;
@@ -655,6 +660,21 @@ static int run_decode_step(rr_engine* e, int mode) {
 }
 
 // ---------------------------------------------------------------- prefill chunk
+// FP8 weights: layer l's four projections dequantized into the prefill scratch (the layout init_pf_plans reads), one launch.
+// The last layer needs wqkv only: its O projection and MLP run on the chunk's tail rows through the decode kernels, which
+// read the e4m3 weights themselves.
+static int launch_dequant_layer(rr_engine* e, int l, cudaStream_t s) {
+    const rr_model_desc& d = e->d;
+    Fp8DequantJobs J;
+    __nv_bfloat16* p = e->deq;
+    fp8_dequant_job(&J, e->wqkv[l], e->sqkv[l], e->nqkv, d.hidden, p, d.hidden); p += (size_t)e->nqkv * d.hidden;
+    if (l + 1 == d.n_layers) return launch_dequantize_fp8(J, s);
+    fp8_dequant_job(&J, e->wo[l], e->so[l], d.hidden, e->nq, p, e->nq); p += (size_t)d.hidden * e->nq;
+    fp8_dequant_job(&J, e->wgu[l], e->sgu[l], 2 * d.inter, d.hidden, p, d.hidden); p += (size_t)2 * d.inter * d.hidden;
+    fp8_dequant_job(&J, e->wdown[l], e->sdown[l], d.hidden, d.inter, p, d.inter);
+    return launch_dequantize_fp8(J, s);
+}
+
 // One set of plans (4 L TMA descriptors) built for Tmax rows; the live row count is a launch argument: TMA reads of
 // rows >= T stay inside the Tmax-row buffers and every store is guarded by rowsA.
 static int init_pf_plans(rr_engine* e) {
@@ -663,7 +683,13 @@ static int init_pf_plans(rr_engine* e) {
     const int L = d.n_layers, T = e->Tmax;
     P.qkv.resize(L); P.o.resize(L); P.gu.resize(L); P.down.resize(L);
     for (int l = 0; l < L; ++l) {
-        int rc = gemm_plan_init(&P.qkv[l], e->pxn, T, d.hidden, e->wqkv[l], e->nqkv, d.hidden, d.hidden, e->pqkv,
+        const void *wqkv = e->wqkv[l], *wo = e->wo[l], *wgu = e->wgu[l], *wdown = e->wdown[l];
+        if (e->fp8) {
+            const __nv_bfloat16* base = e->deq;
+            wqkv = base; wo = base + (size_t)e->nqkv * d.hidden; wgu = (const __nv_bfloat16*)wo + (size_t)d.hidden * e->nq;
+            wdown = (const __nv_bfloat16*)wgu + (size_t)2 * d.inter * d.hidden;
+        }
+        int rc = gemm_plan_init(&P.qkv[l], e->pxn, T, d.hidden, wqkv, e->nqkv, d.hidden, d.hidden, e->pqkv,
                                 e->nqkv, 0, 1, e->fuse_rope_pf ? OUT_ROWMAJOR_ROPE : OUT_ROWMAJOR_BF16, PF_BN);
         if (rc) return rc;
         if (e->fuse_rope_pf) {
@@ -674,20 +700,20 @@ static int init_pf_plans(rr_engine* e) {
             r.table = e->rope_table; r.n_heads = d.n_heads; r.n_kv_heads = d.n_kv_heads; r.ctx_max = e->o.ctx_max;
             r.page_table = e->d_table; r.pages_per_slot = e->pps;
         }
-        rc = gemm_plan_init(&P.o[l], e->pattn, T, e->nq, e->wo[l], d.hidden, e->nq, e->nq, e->px, d.hidden, 0, 1,
+        rc = gemm_plan_init(&P.o[l], e->pattn, T, e->nq, wo, d.hidden, e->nq, e->nq, e->px, d.hidden, 0, 1,
                             OUT_ROWMAJOR_RESID, PF_BN);                // residual add in the epilogue
         if (rc) return rc;
         // deferred RMSNorm: the residual GEMMs (O, down) produce the next operand and its sum(x^2); QKV and gate/up apply 1 / rms
         pf_norm_consumer(&P.qkv[l].rope, e->p_rowss, d.hidden, d.rms_eps);
         pf_norm_producer(&P.o[l].rope, (const __nv_bfloat16*)e->norm_mlp[l], e->pxn, e->p_rowss, d.hidden);
         if (e->fuse_silu)
-            rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pact,
+            rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, wgu, 2 * d.inter, d.hidden, d.hidden, e->pact,
                                 d.inter, 0, 1, OUT_ROWMAJOR_SILU, PF_BN);
         else
-            rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, e->wgu[l], 2 * d.inter, d.hidden, d.hidden, e->pgu,
+            rc = gemm_plan_init(&P.gu[l], e->pxn, T, d.hidden, wgu, 2 * d.inter, d.hidden, d.hidden, e->pgu,
                                 2 * d.inter, 0, 1, OUT_ROWMAJOR_BF16, PF_BN);
         if (rc) return rc;
-        rc = gemm_plan_init(&P.down[l], e->pact, T, d.inter, e->wdown[l], d.hidden, d.inter, d.inter, e->px,
+        rc = gemm_plan_init(&P.down[l], e->pact, T, d.inter, wdown, d.hidden, d.inter, d.inter, e->px,
                             d.hidden, 0, 1, OUT_ROWMAJOR_RESID, PF_BN);
         if (rc) return rc;
         pf_norm_consumer(&P.gu[l].rope, e->p_rowss, d.hidden, d.rms_eps);
@@ -793,7 +819,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     const int32_t* p_tlast = fan ? p_ids + (h_tlast - h) : p_last;
 
     rr_engine::PfPlans& P = e->pf;
-    auto launch_rows = [&](const GemmPlan& pl) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s); };
+    auto launch_rows = [&](const GemmPlan& pl, bool pdl = true) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s, pdl); };
     uint64_t nl = 0;
     if (copies && copies->count > 0) {   // cached prefixes of busy slots into this chunk's slots, before any layer reads them
         if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, (long long)e->n_pages * d.n_kv_heads * KV_PAGE, d.n_kv_heads,
@@ -811,7 +837,13 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (e->fuse_rope_pf) {
             P.qkv[l].rope.slot = p_slt; P.qkv[l].rope.pos = p_pos;
         }
-        if (launch_rows(P.qkv[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        // FP8: layer l's weights into the scratch.  The dequantize and the QKV GEMM after it are plain launches: the
+        // dequantize starts after the previous layer's GEMMs have finished reading the scratch, and the QKV GEMM (and so
+        // every later kernel, whose PDL weight prefetch runs before griddepcontrol.wait) after the scratch is complete.
+        if (e->fp8) {
+            if (launch_dequant_layer(e, l, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
+        }
+        if (launch_rows(P.qkv[l], !e->fp8) != RR_OK) return RR_CUDA_ERROR; ++nl;
         RopeArgs ra;
         ra.qkv = part_bf16(e->pqkv, e->nqkv);
         ra.q_out = e->pq; ra.k_cache = kc; ra.v_cache = vc; ra.slot = p_slt; ra.pos = p_pos; ra.rows = T;
@@ -1344,6 +1376,17 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     const long long kv_full = (long long)opts->max_batch * opts->ctx_max;
     const long long kv_tokens = opts->kv_cache_tokens == 0 ? kv_full : opts->kv_cache_tokens;
     if (kv_tokens % KV_PAGE || kv_tokens < opts->ctx_max || kv_tokens > kv_full) return RR_INVALID_ARGUMENT;
+    const bool fp8 = (w->flags & RR_WEIGHTS_FP8_E4M3) != 0;
+    if (fp8) {      // e4m3 projections the decode GEMMs can stream, and their scales
+        if (!w->wqkv_scale || !w->wo_scale || !w->wgu_scale || !w->wdown_scale) return RR_INVALID_ARGUMENT;
+        const int nq = d.n_heads * d.head_dim;
+        for (int l = 0; l < d.n_layers; ++l) {
+            if (!fp8_weight_ok(w->wqkv[l], d.hidden) || !fp8_weight_ok(w->wo[l], nq) || !fp8_weight_ok(w->wgu[l], d.hidden) ||
+                !fp8_weight_ok(w->wdown[l], d.inter))
+                return RR_INVALID_ARGUMENT;
+            if (!w->wqkv_scale[l] || !w->wo_scale[l] || !w->wgu_scale[l] || !w->wdown_scale[l]) return RR_INVALID_ARGUMENT;
+        }
+    }
     CK(cudaSetDevice(opts->device));
     rr_engine* e = new (std::nothrow) rr_engine();
     if (!e) return RR_INTERNAL;
@@ -1358,7 +1401,12 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     for (int l = 0; l < L; ++l) {
         e->wqkv.push_back(w->wqkv[l]); e->wo.push_back(w->wo[l]); e->wgu.push_back(w->wgu[l]);
         e->wdown.push_back(w->wdown[l]); e->norm_attn.push_back(w->norm_attn[l]); e->norm_mlp.push_back(w->norm_mlp[l]);
+        if (fp8) {
+            e->sqkv.push_back((const float*)w->wqkv_scale[l]); e->so.push_back((const float*)w->wo_scale[l]);
+            e->sgu.push_back((const float*)w->wgu_scale[l]); e->sdown.push_back((const float*)w->wdown_scale[l]);
+        }
     }
+    e->fp8 = fp8;
     memset(&e->st, 0, sizeof(e->st));
     e->t0 = std::chrono::steady_clock::now();
     int rc = RR_OK;
@@ -1461,18 +1509,24 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         da.fuse_rope = 1; da.qkv = part_f32(e->part_qkv, e->s_qkv, B, e->nqkv); da.rope_table = e->rope_table;
         da.head_dim = d.head_dim; da.page_table = e->d_table; da.pages_per_slot = e->pps;
         TRY(decode_attn_make_maps(&da, e->n_pages));
-        TRY(gemm_plan_init(&e->pl_qkv[l], e->wqkv[l], e->nqkv, d.hidden, e->xn, B, d.hidden, d.hidden, e->part_qkv,
-                           e->nqkv, B, e->s_qkv, OUT_TRANSPOSED_F32, e->bn_dec));
-        TRY(gemm_plan_init(&e->pl_o[l], e->wo[l], d.hidden, e->nq, e->attn_out, B, e->nq, e->nq, e->part_o, d.hidden,
-                           B, e->s_o, OUT_TRANSPOSED_F32, e->bn_dec));
+        // the decode projections: the same plans on e4m3 weights with FP8 (gemm_plan_init_fp8w)
+        auto plan = [&](GemmPlan* p, const void* A, const float* sc, int rowsA, int K, const void* Bop, void* out, int ldo,
+                        int splits, int mode) {
+            return fp8 ? gemm_plan_init_fp8w(p, A, sc, rowsA, K, Bop, B, K, K, out, ldo, B, splits, mode, e->bn_dec)
+                       : gemm_plan_init(p, A, rowsA, K, Bop, B, K, K, out, ldo, B, splits, mode, e->bn_dec);
+        };
+        TRY(plan(&e->pl_qkv[l], e->wqkv[l], fp8 ? e->sqkv[l] : nullptr, e->nqkv, d.hidden, e->xn, e->part_qkv, e->nqkv,
+                 e->s_qkv, OUT_TRANSPOSED_F32));
+        TRY(plan(&e->pl_o[l], e->wo[l], fp8 ? e->so[l] : nullptr, d.hidden, e->nq, e->attn_out, e->part_o, d.hidden, e->s_o,
+                 OUT_TRANSPOSED_F32));
         if (e->fuse_silu)
-            TRY(gemm_plan_init(&e->pl_gu[l], e->wgu[l], 2 * d.inter, d.hidden, e->xn, B, d.hidden, d.hidden, e->act,
-                               d.inter, B, 1, OUT_TRANSPOSED_SILU, e->bn_dec));
+            TRY(plan(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, e->act, d.inter, 1,
+                     OUT_TRANSPOSED_SILU));
         else
-            TRY(gemm_plan_init(&e->pl_gu[l], e->wgu[l], 2 * d.inter, d.hidden, e->xn, B, d.hidden, d.hidden, e->part_gu,
-                               2 * d.inter, B, e->s_gu, OUT_TRANSPOSED_F32, e->bn_dec));
-        TRY(gemm_plan_init(&e->pl_down[l], e->wdown[l], d.hidden, d.inter, e->act, B, d.inter, d.inter, e->part_down,
-                           d.hidden, B, e->s_down, OUT_TRANSPOSED_F32, e->bn_dec));
+            TRY(plan(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, e->part_gu,
+                     2 * d.inter, e->s_gu, OUT_TRANSPOSED_F32));
+        TRY(plan(&e->pl_down[l], e->wdown[l], fp8 ? e->sdown[l] : nullptr, d.hidden, d.inter, e->act, e->part_down, d.hidden,
+                 e->s_down, OUT_TRANSPOSED_F32));
     }
     TRY(gemm_plan_init(&e->pl_head, e->lm_head, d.vocab, d.hidden, e->xn, B, d.hidden, d.hidden, e->logits, d.vocab,
                        B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
@@ -1481,6 +1535,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     // sums per row that the residual epilogue writes
     e->pf_parts = pf_norm_parts(d.hidden);
     TRY(dalloc(e, &e->p_rowss, (size_t)e->Tmax * e->pf_parts));
+    if (fp8) TRY(dalloc(e, &e->deq, (size_t)(e->nqkv + e->nq + 3 * d.inter) * d.hidden, false));
     TRY(init_pf_plans(e));
     if (e->fuse_mlp) {
         std::vector<MlpItem> sched;
@@ -1493,7 +1548,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         e->mlp.resize(L);
         for (int l = 0; l < L; ++l) {
             TRY(mlp_plan_init(&e->mlp[l], e->wgu[l], e->wdown[l], d.inter, d.hidden, e->xn, B, e->act, e->part_down, B,
-                              e->bn_dec, e->mlp_items, max_items, grid, e->mlp_ready, e->mlp_slice_kb, dyn));
+                              e->bn_dec, e->mlp_items, max_items, grid, e->mlp_ready, e->mlp_slice_kb, dyn,
+                              fp8 ? e->sgu[l] : nullptr, fp8 ? e->sdown[l] : nullptr));
         }
     }
     TRYC(cudaDeviceSynchronize());

@@ -18,6 +18,12 @@
 // PDL: the weight operand is constant, its first pipeline stages are requested before
 // griddepcontrol.wait; only the activation operand and the output wait for the preceding kernel.
 //
+// FP8 weights (template flag FP8 of the decode kernels): A is e4m3 [N, K] with one power-of-two scale per row (rr_fp8.cu).
+// The TMA producer streams 128 x 64-byte e4m3 slices (no swizzle) into a ring of half the bf16 stage size; the consumer
+// warpgroup converts each slice exactly into bf16(Q * s), written into one of three 128B-swizzled 16 KB tiles (the layout
+// TMA gives a bf16 A stage), fences the generic-proxy writes against the async proxy, and runs the same wgmma sequence,
+// k order, split-K planes and epilogues as the bf16 kernel: the output bits equal the bf16 kernel's on D = bf16(Q * s).
+//
 // Replaces: the remote bedrock:InvokeModel call (reference iam/policy.json:8,
 // src/demo_cris.py:233-238) — there is no reference kernel; see DESIGN.md §kernels.
 #include "rr_ptx.cuh"
@@ -47,21 +53,27 @@ constexpr int GROUP_A = 16;    // raster group: 16 A tiles share the streamed B 
 
 constexpr int cmax(int a, int b) { return a > b ? a : b; }
 
-// CAP bounds the smem ring.  Shared memory: [ring A][ring B][barriers 256 B][staged accumulators][epilogue staging];
-// the ring gets what the 227 KB of an H100 SM leave after the largest epilogue staging of any mode.
-template <int BN, int CAP = 8>
+// CAP bounds the smem ring.  Shared memory: [converted tiles (FP8)][ring A][ring B][barriers 256 B][staged accumulators]
+// [epilogue staging]; the ring gets what the 227 KB of an H100 SM leave after the largest epilogue staging of any mode and,
+// with FP8 weights, the three converted bf16 A tiles (48 KB).  An e4m3 A stage is 8 KB instead of 16 KB.  Stages, bf16 ->
+// FP8: BN 16: 8 -> 8, BN 32: 8 -> 8, BN 64: 6 -> 6, BN 128: 4 -> 3.
+template <int BN, int CAP = 8, bool FP8 = false>
 struct GemmCfg {
     static_assert(BN >= 16 && BN <= MAX_BN, "tile width");
-    static constexpr int kStageBytesA = BLOCK_A * BLOCK_K * 2;
+    static constexpr int kStageBytesA = BLOCK_A * BLOCK_K * (FP8 ? 1 : 2);
     static constexpr int kStageBytesB = BN * BLOCK_K * 2;
     static constexpr int kStageBytes = kStageBytesA + kStageBytesB;
+    static constexpr int kCvtTiles = FP8 ? 3 : 0;          // converted A tiles: wgmma k-block i reads tile i % 3
+    static constexpr int kCvtBytes = kCvtTiles * BLOCK_A * BLOCK_K * 2;
     static constexpr int kAccPitch = BN + 4;               // fp32 words per staged row: conflict-free 16-byte row reads
     static constexpr int kAccBytes = BLOCK_A * kAccPitch * 4;
     static constexpr int kSiluStageBytes = 2 * 32 * 64 * 4;   // OUT_TRANSPOSED_SILU: up-row exchange, 2 x [32 cols][64 rows] fp32
     static constexpr int kEpiMax = cmax(BN <= 64 ? BN * 512 : 0, kSiluStageBytes + (BN <= 64 ? BN * 128 : 0));
-    static constexpr int kStagesRaw = (224 * 1024 - 1024 - 256 - kAccBytes - kEpiMax) / kStageBytes;
+    static constexpr int kStagesRaw = (224 * 1024 - 1024 - 256 - kAccBytes - kEpiMax - kCvtBytes) / kStageBytes;
     static constexpr int kStages = kStagesRaw > CAP ? CAP : kStagesRaw;
-    static constexpr int kAccOff = kStages * kStageBytes + 256;         // staged accumulator tile
+    static constexpr int kRingOff = kCvtBytes;                          // ring A, then ring B
+    static constexpr int kBarOff = kRingOff + kStages * kStageBytes;    // full / empty barriers (+ the MLP's item queue)
+    static constexpr int kAccOff = kBarOff + 256;                       // staged accumulator tile
     static constexpr int kEpiOff = kAccOff + kAccBytes;                 // epilogue staging (mode dependent)
     static constexpr int kSmemBytes = kEpiOff + 1024 /*align slack*/;
 };
@@ -74,19 +86,62 @@ constexpr int mlp_stage_bytes() {
     constexpr int a = planes_stage_bytes<BN>(), b = GemmCfg<BN>::kSiluStageBytes + (BN <= 64 ? BN * 64 * 2 : 0);
     return a > b ? a : b;
 }
-template <int BN, int MODE, int CAP = 8>
+template <int BN, int MODE, int CAP = 8, bool FP8 = false>
 constexpr int gemm_smem_bytes() {
     // SILU: up-row exchange; F32: the planes tile of the TMA-store epilogue
-    return GemmCfg<BN, CAP>::kSmemBytes +
+    return GemmCfg<BN, CAP, FP8>::kSmemBytes +
            (MODE == OUT_TRANSPOSED_SILU ? GemmCfg<BN, CAP>::kSiluStageBytes : MODE == OUT_TRANSPOSED_F32 ? planes_stage_bytes<BN>() : 0);
 }
+// ---- FP8 weights: the consumer warpgroup's converter ------------------------------------------------------------------
+// Lane l of warp w converts 16 bytes (k 16 (l % 4) ..) of rows 32 w + l / 4 + 8 i, i < 4: each read instruction of a warp
+// covers 512 contiguous bytes of the slice, and the two 16-byte writes per row land on 128B-swizzle chunks that cover all
+// eight bank groups of a row block (no bank conflicts either way).
+struct Fp8Conv {
+    const uint8_t* ring;      // e4m3 ring A
+    uint8_t* tiles;           // kCvtTiles converted bf16 tiles, 16 KB each, 1024-byte aligned
+    int tile;                 // the tile the next k-block is converted into
+    float sc[4];              // scales of this lane's rows for the current item (1 for rows >= rowsA, which TMA zero-fills)
+    __device__ __forceinline__ void load_scales(const float* scale, int a_tile, int rowsA) {
+        const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int r = a_tile * BLOCK_A + 32 * w + (l >> 2) + 8 * i;
+            sc[i] = r < rowsA ? __ldg(scale + r) : 1.f;
+        }
+    }
+    // ring slot -> tile; returns the tile's shared-memory address.  Tile t is rewritten three k-blocks after it was read:
+    // every warp has passed the wgmma_wait<1> that retires that read before it reached the barrier of the k-block between.
+    __device__ __forceinline__ uint32_t convert(int stage) {
+        const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+        const uint8_t* src = ring + stage * (BLOCK_A * BLOCK_K);
+        uint8_t* dst = tiles + tile * (BLOCK_A * BLOCK_K * 2);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int r = 32 * w + (l >> 2) + 8 * i;
+            const uint4 q = *reinterpret_cast<const uint4*>(src + r * BLOCK_K + 16 * (l & 3));
+            const uint2 a = e4m3x4_to_bf16x4(q.x, sc[i]), b = e4m3x4_to_bf16x4(q.y, sc[i]);
+            const uint2 c = e4m3x4_to_bf16x4(q.z, sc[i]), d = e4m3x4_to_bf16x4(q.w, sc[i]);
+            const int c0 = 2 * (l & 3);                  // 16-byte bf16 chunks c0, c0 + 1 of row r, swizzled by r % 8
+            *reinterpret_cast<uint4*>(dst + r * 128 + ((c0 ^ (r & 7)) << 4)) = make_uint4(a.x, a.y, b.x, b.y);
+            *reinterpret_cast<uint4*>(dst + r * 128 + (((c0 + 1) ^ (r & 7)) << 4)) = make_uint4(c.x, c.y, d.x, d.y);
+        }
+        fence_proxy_async();                             // generic-proxy writes -> the wgmma's async-proxy reads
+        asm volatile("bar.sync 5, 128;" ::: "memory");
+        const uint32_t t = smem_u32(dst);
+        tile = tile == 2 ? 0 : tile + 1;
+        return t;
+    }
+};
+
 // ---- consumer warpgroup ------------------------------------------------------------------------------------------------
 // Accumulate the next `nkb` ring slots into acc (acc[0]: tile rows 0..63, acc[1]: rows 64..127).  The first k step
 // overwrites the accumulators.  One k-block stays in flight: a slot is released (one arrival per consumer warp on its
 // empty barrier) once the wgmma group that read it has retired.
-template <int BN>
+// FP8: cv converts each ring slot first and the wgmma read the converted tile.
+template <int BN, bool FP8 = false>
 __device__ __forceinline__ void gmma_mainloop(float (&acc)[2][BN / 2], uint32_t smemA, uint32_t smemB, uint64_t* full_bar,
-                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int nkb, int depth) {
+                                              uint64_t* empty_bar, int& stage, uint32_t& phase, int nkb, int depth,
+                                              Fp8Conv* cv = nullptr) {
     constexpr int kStageA = BLOCK_A * BLOCK_K * 2, kStageB = BN * BLOCK_K * 2;
     const bool arrive = (threadIdx.x & 31) == 0;
     int prev = -1;
@@ -94,7 +149,9 @@ __device__ __forceinline__ void gmma_mainloop(float (&acc)[2][BN / 2], uint32_t 
     wgmma_fence_regs(acc[1]);
     for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        const uint64_t da = gmma_desc_sw128(smemA + stage * kStageA);
+        uint64_t da;
+        if constexpr (FP8) da = gmma_desc_sw128(cv->convert(stage));
+        else da = gmma_desc_sw128(smemA + stage * kStageA);
         const uint64_t db = gmma_desc_sw128(smemB + stage * kStageB);
         wgmma_fence();
 #pragma unroll
@@ -333,19 +390,19 @@ __device__ __forceinline__ void epilogue_silu_tma(const float* arow, const WorkI
     }
 }
 
-template <int BN, int MODE, int CAP = 8>
+template <int BN, int MODE, int CAP = 8, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 void* __restrict__ out, int rowsA, int rowsB, int K, int splits, int ldo,
-                int ld_rows, const __grid_constant__ CUtensorMap tmOut, int tma_epi) {
-    using Cfg = GemmCfg<BN, CAP>;
+                int ld_rows, const __grid_constant__ CUtensorMap tmOut, int tma_epi, const float* __restrict__ scaleA) {
+    using Cfg = GemmCfg<BN, CAP, FP8>;
     constexpr int kStages = Cfg::kStages;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem_1024(smem_raw);
-    uint8_t* smemA = smem;
-    uint8_t* smemB = smem + kStages * Cfg::kStageBytesA;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+    uint8_t* smemA = smem + Cfg::kRingOff;
+    uint8_t* smemB = smemA + kStages * Cfg::kStageBytesA;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
     uint64_t* empty_bar = full_bar + kStages;
     float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOff);
 
@@ -432,9 +489,11 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         trace_dep(tr_slot);
         int stage = 0;
         uint32_t phase = 0;
+        Fp8Conv cv{smemA, smem, 0, {}};
         for (int it = 0; sched.next(t); ++it) {
             float acc[2][BN / 2];
-            gmma_mainloop<BN>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages);
+            if constexpr (FP8) cv.load_scales(scaleA, t.a_tile, rowsA);
+            gmma_mainloop<BN, FP8>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages, &cv);
             if (tsm >= 0 && etid == 0) trace_mark_at(TR_GEMM_MARK + 4, tsm, 16 + 2 * it);
             acc_bar();                                // the previous item's epilogue is done with the staged tile
             stage_acc<BN>(acc, acc_tile);
@@ -772,19 +831,19 @@ __device__ __forceinline__ unsigned ld_acquire_gpu_u32(const unsigned* p) {
     return v;
 }
 
-template <int BN>
+template <int BN, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_mlp_wgmma(const __grid_constant__ MlpArgs a) {
-    using Cfg = GemmCfg<BN>;
+    using Cfg = GemmCfg<BN, 8, FP8>;
     constexpr int kStages = Cfg::kStages;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = align_smem_1024(smem_raw);
-    uint8_t* smemA = smem;
-    uint8_t* smemB = smem + kStages * Cfg::kStageBytesA;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);
+    uint8_t* smemA = smem + Cfg::kRingOff;
+    uint8_t* smemB = smemA + kStages * Cfg::kStageBytesA;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOff);
     uint64_t* empty_bar = full_bar + kStages;
-    volatile int* dyn_q = reinterpret_cast<volatile int*>(smem + kStages * Cfg::kStageBytes + 176);   // [16] dynamic down items of this CTA
+    volatile int* dyn_q = reinterpret_cast<volatile int*>(smem + Cfg::kBarOff + 176);   // [16] dynamic down items of this CTA
     float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOff);
     float* silu_stage = reinterpret_cast<float*>(smem + Cfg::kEpiOff);    // exchange; aliased by the planes tile
     __nv_bfloat16* act_stage = reinterpret_cast<__nv_bfloat16*>(smem + Cfg::kEpiOff + Cfg::kSiluStageBytes);
@@ -917,10 +976,12 @@ gemm_mlp_wgmma(const __grid_constant__ MlpArgs a) {
         griddep_wait();
         trace_dep(tr_slot);
         int nstat = -1;
+        Fp8Conv cv{smemA, smem, 0, {}};
         for (int it = 0; next_consumer(it, nstat, t, ph); ++it) {
             if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 4 + ph, 64 + it);
             float acc[2][BN / 2];
-            gmma_mainloop<BN>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages);
+            if constexpr (FP8) cv.load_scales(ph ? a.sc1 : a.sc0, t.a_tile, ph ? a.hidden : 2 * a.inter);
+            gmma_mainloop<BN, FP8>(acc, smemA_u, smemB_u, full_bar, empty_bar, stage, phase, t.kb1 - t.kb0, kStages, &cv);
             if (etid == 0) trace_mark_fixed(TR_MLP_MARK + 6 + ph, 128 + 4 * it);
             acc_bar();
             stage_acc<BN>(acc, acc_tile);
@@ -1004,6 +1065,22 @@ int make_tmap_bf16_2d(CUtensorMap* map, const void* base, int rows, int K, int l
     return r == CUDA_SUCCESS ? RR_OK : RR_ERR_CUDA;
 }
 
+// [rows, K] e4m3 row-major (row pitch ld bytes) -> TMA map with box {64 bytes, box_rows}, no swizzle (the FP8 ring slot).
+// The caller has checked fp8_weight_ok and ld % 16 == 0: TMA needs a 16-byte aligned base and pitch, and a box row of 64
+// bytes is a multiple of 16.
+static int make_tmap_e4m3_2d(CUtensorMap* map, const void* base, int rows, int K, int ld, int box_rows) {
+    PFN_encodeTiled enc = get_encode_fn();
+    if (!enc) return RR_ERR_CUDA;
+    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)ld};
+    cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS ? RR_OK : RR_ERR_CUDA;
+}
+
 // planes P[z][b][n] fp32 (n contiguous, row pitch ldo, plane pitch ld_rows * ldo), valid n < n_valid, b < rows_valid:
 // 3-D map {n, b, z}, box {128, box_rows, 1}, no swizzle -- the destination of epilogue_planes_tma
 int make_tmap_planes_f32(CUtensorMap* map, const void* base, int n_valid, int ldo, int rows_valid, int ld_rows, int splits, int box_rows) {
@@ -1048,23 +1125,24 @@ int num_sms() {                         // of the current device (one process ma
     return n;
 }
 
-template <int BN, int MODE>
+template <int BN, int MODE, bool FP8 = false>
 static int launch_one(const GemmPlan& p, cudaStream_t st) {
     constexpr int CAP = 8;
-    auto kern = gemm_bf16_wgmma<BN, MODE, CAP>;
+    auto kern = gemm_bf16_wgmma<BN, MODE, CAP, FP8>;
     static std::atomic<uint64_t> attr_set{0};
-    if (ensure_dyn_smem(kern, (int)gemm_smem_bytes<BN, MODE, CAP>(), attr_set) != cudaSuccess) return RR_ERR_CUDA;
+    static_assert(gemm_smem_bytes<BN, MODE, CAP, FP8>() <= 227 * 1024, "decode GEMM: shared memory budget");
+    if (ensure_dyn_smem(kern, (int)gemm_smem_bytes<BN, MODE, CAP, FP8>(), attr_set) != cudaSuccess) return RR_ERR_CUDA;
     const int tilesA = (p.rowsA + BLOCK_A - 1) / BLOCK_A;
     const int tilesB = (p.rowsB + BN - 1) / BN;
     const int n_work = tilesA * tilesB * p.splits;
     const int grid = n_work < num_sms() ? n_work : num_sms();
-    cudaError_t le = launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)gemm_smem_bytes<BN, MODE, CAP>(), st, p.tmA, p.tmB,
-                                p.out, p.rowsA, p.rowsB, p.K, p.splits, p.ldo, p.ld_rows, p.tmOut, p.tma_epi);
+    cudaError_t le = launch_pdl(kern, dim3(grid), dim3(GEMM_THREADS), (size_t)gemm_smem_bytes<BN, MODE, CAP, FP8>(), st, p.tmA,
+                                p.tmB, p.out, p.rowsA, p.rowsB, p.K, p.splits, p.ldo, p.ld_rows, p.tmOut, p.tma_epi, p.scaleA);
     return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
 }
 
 template <int MODE>
-static int launch_pf(const GemmPlan& p, cudaStream_t st) {
+static int launch_pf(const GemmPlan& p, cudaStream_t st, bool pdl) {
     auto kern = gemm_pf_wgmma<MODE>;
     static std::atomic<uint64_t> attr_set{0};
     if (ensure_dyn_smem(kern, PfCfg::kSmemBytes, attr_set) != cudaSuccess) return RR_ERR_CUDA;
@@ -1072,8 +1150,8 @@ static int launch_pf(const GemmPlan& p, cudaStream_t st) {
     const int tilesB = (p.rowsB + PfCfg::kTileB - 1) / PfCfg::kTileB;
     const int n_work = tilesA * tilesB;
     const int grid = n_work < num_sms() ? n_work : num_sms();
-    cudaError_t le = launch_pdl(kern, dim3(grid), dim3(PfCfg::kThreads), (size_t)PfCfg::kSmemBytes, st, p.tmA, p.tmB, p.out,
-                                p.rowsA, p.rowsB, p.K, p.ldo, p.rope);
+    cudaError_t le = launch_ex(pdl ? g_use_pdl : 0, kern, dim3(grid), dim3(PfCfg::kThreads), (size_t)PfCfg::kSmemBytes, st, p.tmA,
+                               p.tmB, p.out, p.rowsA, p.rowsB, p.K, p.ldo, p.rope);
     return (le == cudaSuccess && cudaGetLastError() == cudaSuccess) ? RR_OK : RR_ERR_CUDA;
 }
 
@@ -1097,7 +1175,7 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
     if (mode < 0 || mode > OUT_ROWMAJOR_RESID) return RR_ERR_ARG;
     memset(&p->rope, 0, sizeof(p->rope));
     p->rowsA = rowsA; p->rowsB = rowsB; p->K = K; p->out = out; p->ldo = ldo; p->ld_rows = ld_rows;
-    p->splits = splits; p->mode = mode; p->bn = bn; p->max_ctas = 0;
+    p->splits = splits; p->mode = mode; p->bn = bn; p->max_ctas = 0; p->scaleA = nullptr;
     int rc = make_tmap_bf16_2d(&p->tmA, A, rowsA, K, ldA, BLOCK_A);
     if (rc != RR_OK) return rc;
     // decode planes through one TMA store per item: needs 16-byte pitches and at most 64 batch columns per tile
@@ -1110,19 +1188,39 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
     return make_tmap_bf16_2d(&p->tmB, B, rowsB, K, ldB, rowmajor(mode) ? PfCfg::kTileB : bn);
 }
 
-int gemm_launch(const GemmPlan& p, cudaStream_t st) {
+int gemm_plan_init_fp8w(GemmPlan* p, const void* A, const float* scale, int rowsA, int ldA, const void* B, int rowsB,
+                        int ldB, int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn) {
+    if (mode != OUT_TRANSPOSED_F32 && mode != OUT_TRANSPOSED_SILU) return RR_ERR_ARG;
+    if (!scale || !fp8_weight_ok(A, K) || ldA < K || ldA % 16 != 0 || rowsA < 1) return RR_ERR_ARG;
+    // the bf16 plan on a stand-in A of the same shape, then the e4m3 map of the real one
+    int rc = gemm_plan_init(p, A, rowsA, ldA, B, rowsB, ldB, K, out, ldo, ld_rows, splits, mode, bn);
+    if (rc != RR_OK) return rc;
+    rc = make_tmap_e4m3_2d(&p->tmA, A, rowsA, K, ldA, BLOCK_A);
+    if (rc != RR_OK) return rc;
+    p->scaleA = scale;
+    return RR_OK;
+}
+
+int gemm_launch(const GemmPlan& p, cudaStream_t st, bool pdl) {
     switch (p.mode) {
-        case OUT_ROWMAJOR_BF16: return launch_pf<OUT_ROWMAJOR_BF16>(p, st);
-        case OUT_ROWMAJOR_SILU: return launch_pf<OUT_ROWMAJOR_SILU>(p, st);
-        case OUT_ROWMAJOR_ROPE: return launch_pf<OUT_ROWMAJOR_ROPE>(p, st);
-        case OUT_ROWMAJOR_RESID: return launch_pf<OUT_ROWMAJOR_RESID>(p, st);
+        case OUT_ROWMAJOR_BF16: return launch_pf<OUT_ROWMAJOR_BF16>(p, st, pdl);
+        case OUT_ROWMAJOR_SILU: return launch_pf<OUT_ROWMAJOR_SILU>(p, st, pdl);
+        case OUT_ROWMAJOR_ROPE: return launch_pf<OUT_ROWMAJOR_ROPE>(p, st, pdl);
+        case OUT_ROWMAJOR_RESID: return launch_pf<OUT_ROWMAJOR_RESID>(p, st, pdl);
     }
-#define RR_CASE(BN_)                                                                                  \
-    case BN_:                                                                                         \
-        if (p.mode == OUT_TRANSPOSED_F32) return launch_one<BN_, OUT_TRANSPOSED_F32>(p, st);           \
-        if constexpr (BN_ >= 32) {                                                                    \
-            if (p.mode == OUT_TRANSPOSED_SILU) return launch_one<BN_, OUT_TRANSPOSED_SILU>(p, st);     \
-        }                                                                                             \
+#define RR_CASE(BN_)                                                                                            \
+    case BN_:                                                                                                   \
+        if (p.scaleA) {                                                                                         \
+            if (p.mode == OUT_TRANSPOSED_F32) return launch_one<BN_, OUT_TRANSPOSED_F32, true>(p, st);           \
+            if constexpr (BN_ >= 32) {                                                                          \
+                if (p.mode == OUT_TRANSPOSED_SILU) return launch_one<BN_, OUT_TRANSPOSED_SILU, true>(p, st);     \
+            }                                                                                                   \
+            return RR_ERR_ARG;                                                                                  \
+        }                                                                                                       \
+        if (p.mode == OUT_TRANSPOSED_F32) return launch_one<BN_, OUT_TRANSPOSED_F32>(p, st);                     \
+        if constexpr (BN_ >= 32) {                                                                              \
+            if (p.mode == OUT_TRANSPOSED_SILU) return launch_one<BN_, OUT_TRANSPOSED_SILU>(p, st);               \
+        }                                                                                                       \
         return RR_ERR_ARG;
     switch (p.bn) {
         RR_CASE(16)
@@ -1203,21 +1301,26 @@ int mlp_schedule(int grid, int inter, int hidden, int slice_kb, std::vector<MlpI
 
 int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hidden, const void* xn, int rows,
                   void* act, void* planes, int ld_rows, int bn, const MlpItem* items_dev, int max_items, int grid,
-                  unsigned* ready, int slice_kb, int dynamic) {
+                  unsigned* ready, int slice_kb, int dynamic, const float* sc_gu, const float* sc_down) {
     if (!p || !Wgu || !Wd || !xn || !act || !planes || !items_dev || !ready) return RR_ERR_ARG;
     if (inter % 64 || (2 * inter) % BLOCK_A || hidden % 8 || rows > bn || bn < 32 || bn > MAX_BN || slice_kb < 1) return RR_ERR_ARG;
     if ((2 * inter) / BLOCK_A > 0xffff || grid < 1 || grid > num_sms()) return RR_ERR_ARG;
+    const bool fp8 = sc_gu || sc_down;
+    if (fp8 && (!sc_gu || !sc_down || !fp8_weight_ok(Wgu, hidden) || !fp8_weight_ok(Wd, inter))) return RR_ERR_ARG;
     MlpArgs& a = p->args;
-    int rc = make_tmap_bf16_2d(&a.tmA0, Wgu, 2 * inter, hidden, hidden, BLOCK_A);
+    int rc = fp8 ? make_tmap_e4m3_2d(&a.tmA0, Wgu, 2 * inter, hidden, hidden, BLOCK_A)
+                 : make_tmap_bf16_2d(&a.tmA0, Wgu, 2 * inter, hidden, hidden, BLOCK_A);
     if (rc == RR_OK) rc = make_tmap_bf16_2d(&a.tmB0, xn, rows, hidden, hidden, bn);
-    if (rc == RR_OK) rc = make_tmap_bf16_2d(&a.tmA1, Wd, hidden, inter, inter, BLOCK_A);
+    if (rc == RR_OK) rc = fp8 ? make_tmap_e4m3_2d(&a.tmA1, Wd, hidden, inter, inter, BLOCK_A)
+                              : make_tmap_bf16_2d(&a.tmA1, Wd, hidden, inter, inter, BLOCK_A);
     if (rc == RR_OK) rc = make_tmap_bf16_2d(&a.tmB1, act, rows, inter, inter, bn);
     if (rc != RR_OK) return rc;
     a.act = (__nv_bfloat16*)act; a.out1 = (float*)planes; a.inter = inter; a.hidden = hidden; a.rows = rows;
     a.ld_rows = ld_rows; a.items = items_dev; a.max_items = max_items; a.ready = ready; a.slice_kb = slice_kb;
     a.kb1n = inter / BLOCK_K; a.tiles1 = (hidden + BLOCK_A - 1) / BLOCK_A;
     a.n_slices = (a.kb1n + slice_kb - 1) / slice_kb; a.n_down = a.n_slices * a.tiles1; a.dyn = dynamic ? 1 : 0;
-    p->grid = grid; p->bn = bn; p->n_slices = (inter / BLOCK_K + slice_kb - 1) / slice_kb;
+    a.sc0 = sc_gu; a.sc1 = sc_down;
+    p->grid = grid; p->bn = bn; p->n_slices = (inter / BLOCK_K + slice_kb - 1) / slice_kb; p->fp8 = fp8 ? 1 : 0;
     a.tma_epi = 0;
     if (bn <= 64 && hidden % 4 == 0 && inter % 8 == 0 && ((uintptr_t)planes & 15) == 0 && ((uintptr_t)act & 15) == 0 &&
         !getenv("RR_NO_TMA_EPI")) {
@@ -1229,11 +1332,11 @@ int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hi
     return RR_OK;
 }
 
-template <int BN>
+template <int BN, bool FP8 = false>
 static int launch_mlp_bn(const MlpPlan& p, cudaStream_t st) {
-    auto kern = gemm_mlp_wgmma<BN>;
+    auto kern = gemm_mlp_wgmma<BN, FP8>;
     static std::atomic<uint64_t> attr_set{0};
-    constexpr int smem = GemmCfg<BN>::kSmemBytes + mlp_stage_bytes<BN>();
+    constexpr int smem = GemmCfg<BN, 8, FP8>::kSmemBytes + mlp_stage_bytes<BN>();
     static_assert(smem <= 227 * 1024, "fused MLP kernel: shared memory budget");
     if (ensure_dyn_smem(kern, smem, attr_set) != cudaSuccess) return RR_ERR_CUDA;
     cudaError_t e = launch_pdl(kern, dim3(p.grid), dim3(GEMM_THREADS), (size_t)smem, st, p.args);
@@ -1241,6 +1344,14 @@ static int launch_mlp_bn(const MlpPlan& p, cudaStream_t st) {
 }
 // Requires all CTAs co-resident (grid <= SM count; one CTA per SM by shared memory) and ready[] zero at launch.
 int mlp_launch(const MlpPlan& p, cudaStream_t st) {
+    if (p.fp8) {
+        switch (p.bn) {
+            case 32: return launch_mlp_bn<32, true>(p, st);
+            case 64: return launch_mlp_bn<64, true>(p, st);
+            case 128: return launch_mlp_bn<128, true>(p, st);
+        }
+        return RR_ERR_ARG;
+    }
     switch (p.bn) {
         case 32: return launch_mlp_bn<32>(p, st);
         case 64: return launch_mlp_bn<64>(p, st);

@@ -76,6 +76,7 @@ struct GemmPlan {
     RopeEpi rope;             // OUT_ROWMAJOR_ROPE only
     CUtensorMap tmOut;        // OUT_TRANSPOSED_F32: planes [splits][rowsB][rowsA] (3-D, box {128, bn, 1}) for the TMA-store epilogue
     int tma_epi;              // 1: the epilogue stages the tile in shared memory and issues ONE TMA store per item
+    const float* scaleA;      // FP8 weights (gemm_plan_init_fp8w): A is e4m3 [rowsA, K] with one power-of-two scale per row
 };
 
 // ---- prefill decisions shared by the engine (init_pf_plans, run_prefill) and the kernel-level entry points (rr_api.cu)
@@ -142,7 +143,33 @@ int router_strategy(const rr_router* r);
 int make_tmap_bf16_2d(CUtensorMap* map, const void* base, int rows, int K, int ld, int box_rows);
 int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B, int rowsB, int ldB,
                    int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn);
-int gemm_launch(const GemmPlan& p, cudaStream_t st);
+// Decode orientation (OUT_TRANSPOSED_F32 / _SILU) on an e4m3 weight A [rowsA, K] (row pitch ldA bytes) with scale[rowsA]:
+// the same tiles, splits, k order and epilogues as gemm_plan_init on D = bf16(A * scale), so the same bits.  RR_ERR_ARG
+// for another mode, a null scale, or an A the TMA cannot stream (16-byte aligned base and pitch, K % 16 == 0).
+int gemm_plan_init_fp8w(GemmPlan* p, const void* A, const float* scale, int rowsA, int ldA, const void* B, int rowsB,
+                        int ldB, int K, void* out, int ldo, int ld_rows, int splits, int mode, int bn);
+// pdl = false: a plain stream-ordered launch (the first GEMM after the prefill dequantize, rr_fp8.cu)
+int gemm_launch(const GemmPlan& p, cudaStream_t st, bool pdl = true);
+
+// ---- FP8 weights (rr_fp8.cu)
+// An e4m3 weight the decode GEMMs can stream: non-null, 16-byte aligned, K a positive multiple of 16.
+bool fp8_weight_ok(const void* q, int K);
+// Per-row quantizer (rr_op_quantize_fp8_weight); a row with Inf or NaN sets *bad and writes nothing.
+int launch_quantize_fp8(const __nv_bfloat16* w, int rows, int K, int ld, uint8_t* q, float* scale, int* bad, cudaStream_t st);
+struct Fp8DequantJob {
+    const uint8_t* q;         // [rows, K] e4m3
+    const float* scale;       // [rows]
+    __nv_bfloat16* out;       // [rows, ld_out]
+    int rows, K, ld_out;
+};
+struct Fp8DequantJobs {       // up to four matrices in one launch (a layer's wqkv, wo, wgu, wdown)
+    Fp8DequantJob job[4];
+    long long end[4];         // cumulative 16-byte chunks
+    int n = 0;
+};
+void fp8_dequant_job(Fp8DequantJobs* J, const void* q, const float* scale, int rows, int K, __nv_bfloat16* out, int ld_out);
+// out = bf16(q * scale) for every job, as a plain stream-ordered launch that does not trigger its dependents.
+int launch_dequantize_fp8(const Fp8DequantJobs& J, cudaStream_t st);
 
 // ---- fused decode MLP (rr_gemm.cu): gate/up GEMM (+SiLU*mul) and down GEMM in one persistent launch.
 // Per-CTA work lists (built once on the host) replace the kernel boundary: a down item covers one K-slice of
@@ -166,10 +193,12 @@ struct MlpArgs {
     int dyn, n_down, tiles1, kb1n, n_slices;   // dyn: down items drawn from ready[n_slices] in slice-major order (not in `items`)
     CUtensorMap tmAct, tmPlanes;   // TMA-store epilogues: act [rows][inter] bf16 (box {64, bn}), planes (3-D, box {128, bn, 1})
     int tma_epi;
+    const float* sc0;         // FP8 weights: the e4m3 rows' scales of Wgu (interleaved like its rows) and of Wd
+    const float* sc1;
 };
 struct MlpPlan {
     MlpArgs args;
-    int grid, bn, n_slices;
+    int grid, bn, n_slices, fp8;
 };
 // Decode tile width along the batch rows: the narrowest of 16 / 32 / 64 / MAX_BN that holds `rows`; wider batches run
 // several MAX_BN tiles per weight tile.
@@ -185,7 +214,7 @@ int pick_kv_splits(int rows, int n_kv_heads);
 int mlp_schedule(int grid, int inter, int hidden, int slice_kb, std::vector<MlpItem>* items, int dynamic = 0);
 int mlp_plan_init(MlpPlan* p, const void* Wgu, const void* Wd, int inter, int hidden, const void* xn, int rows,
                   void* act, void* planes, int ld_rows, int bn, const MlpItem* items_dev, int max_items, int grid,
-                  unsigned* ready, int slice_kb, int dynamic = 0);
+                  unsigned* ready, int slice_kb, int dynamic = 0, const float* sc_gu = nullptr, const float* sc_down = nullptr);
 int mlp_launch(const MlpPlan& p, cudaStream_t st);
 
 // ---- elementwise / normalisation (rr_elementwise.cu) -------------------------------------------

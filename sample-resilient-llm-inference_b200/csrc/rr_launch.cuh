@@ -96,9 +96,10 @@ inline cudaError_t ensure_dyn_smem(K kern, int bytes, std::atomic<uint64_t>& don
 
 extern int g_use_pdl;   // rr_api.cu; env RR_NO_PDL=1 or rr_set_pdl(0) turns it off
 
+// pdl = 0: a plain stream-ordered launch
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                              Args&&... args) {
+inline cudaError_t launch_ex(int pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                             Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
@@ -106,10 +107,15 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = g_use_pdl ? 1 : 0;
+    at[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
     cfg.attrs = at;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                              Args&&... args) {
+    return launch_ex(g_use_pdl, kern, grid, block, smem, st, std::forward<Args>(args)...);
 }
 
 }  // namespace rr

@@ -6,6 +6,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda.h>
 #include <stdint.h>
 
@@ -259,6 +260,19 @@ __device__ __forceinline__ float bf16_hi(uint32_t packed) {
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// FP8 weights: four e4m3 values (byte i = element i) times the power of two s -> four bf16 (x: elements 0, 1; y: 2, 3),
+// exactly.  e4m3 -> f16 is exact (subnormals included), f16 -> f32 is exact, the product is exact while it stays a normal
+// fp32 number, and the bf16 rounding is exact because an e4m3 value has at most 4 significant bits.
+__device__ __forceinline__ uint2 e4m3x4_to_bf16x4(uint32_t q, float s) {
+    uint32_t h01, h23;
+    asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %2;\n\t"
+        "cvt.rn.f16x2.e4m3x2 %0, lo;\n\tcvt.rn.f16x2.e4m3x2 %1, hi;\n\t}"
+        : "=r"(h01), "=r"(h23) : "r"(q));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&h01));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&h23));
+    return make_uint2(pack_bf16(a.x * s, a.y * s), pack_bf16(b.x * s, b.y * s));
 }
 
 }  // namespace rr

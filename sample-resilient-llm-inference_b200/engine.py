@@ -8,13 +8,13 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
 from . import _lib
-from .models import ModelSpec, Weights, make_weights
+from .models import Fp8Weights, ModelSpec, Weights, make_weights, quantize_fp8
 from .router import FINISH_REASONS, check_response_format, check_stop, gen_args, logprob_pairs
 
 
@@ -57,7 +57,7 @@ def _p(a: np.ndarray):
 
 
 class Engine:
-    def __init__(self, weights: Weights, device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
+    def __init__(self, weights: Union[Weights, Fp8Weights], device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
                  max_prefill_tokens: int = 8192, use_cuda_graph: bool = True,
                  fail_prob: float = 0.0, fail_seed: int = 0, prefix_cache: bool = False,
                  kv_cache_tokens: Optional[int] = None):
@@ -68,7 +68,10 @@ class Engine:
         kv_cache_tokens: the KV cache, a pool of 64-token pages the decode rows share; None = max_batch x ctx_max (the pool
         never binds).  Otherwise a multiple of 64 in [ctx_max, max_batch x ctx_max].  ctx_max is then the limit of one
         request (prompt + max_new_tokens), and each choice reserves ceil((prompt + max_new_tokens) / 64) pages while it
-        runs; a request that does not fit waits, and one that never could is refused at submit."""
+        runs; a request that does not fit waits, and one that never could is refused at submit.
+
+        weights: bf16 Weights, or Fp8Weights (models.quantize_fp8): e4m3 layer projections, computing exactly what a bf16
+        engine computes on weights.dequantize().  Prefill then also holds a bf16 scratch of one layer's projections."""
         if not torch.cuda.is_available():
             raise RuntimeError("rr_b200.Engine needs a CUDA device (no CPU fallback)")
         self.spec: ModelSpec = weights.spec
@@ -96,19 +99,32 @@ class Engine:
         while gu_splits > 1 and kb // gu_splits < 8:
             gu_splits -= 1
         interleave = s.inter % 64 == 0 and gu_splits == 1 and max_batch > 16
+        fp8 = isinstance(weights, Fp8Weights)
         wgu = weights.wgu
+        wgu_scale = weights.wgu_scale if fp8 else []
+
+        def il(t):                  # [gate; up] -> 64-row blocks [g0..g63, u0..u63, ...] (rows, or their scales)
+            g, u = t[: s.inter].reshape(-1, 64, *t.shape[1:]), t[s.inter:].reshape(-1, 64, *t.shape[1:])
+            return torch.stack([g, u], 1).reshape(2 * s.inter, *t.shape[1:]).contiguous()
+
         if interleave:
-            self._wgu_il = []
-            for t in weights.wgu:
-                g, u = t[: s.inter].view(-1, 64, s.hidden), t[s.inter:].view(-1, 64, s.hidden)
-                self._wgu_il.append(torch.stack([g, u], 1).reshape(2 * s.inter, s.hidden).contiguous())
+            self._wgu_il = [il(t.view(torch.uint8)).view(t.dtype) if fp8 else il(t) for t in weights.wgu]
             wgu = self._wgu_il
+            if fp8:
+                self._wgu_scale_il = [il(t) for t in weights.wgu_scale]
+                wgu_scale = self._wgu_scale_il
         self._arrs = [arr(weights.wqkv), arr(weights.wo), arr(wgu), arr(weights.wdown),
                       arr(weights.norm_attn), arr(weights.norm_mlp)]
+        dtypes = (torch.bfloat16, torch.float8_e4m3fn, torch.float32) if fp8 else (torch.bfloat16,)
         for t in weights.tensors():
-            assert t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()
+            assert t.is_cuda and t.dtype in dtypes and t.is_contiguous()
+        scales = [None] * 4
+        if fp8:
+            self._arrs += [arr(weights.wqkv_scale), arr(weights.wo_scale), arr(wgu_scale), arr(weights.wdown_scale)]
+            scales = self._arrs[6:]
+        flags = (_lib.RR_WEIGHTS_WGU_INTERLEAVED64 if interleave else 0) | (_lib.RR_WEIGHTS_FP8_E4M3 if fp8 else 0)
         mw = _lib.ModelWeights(weights.embed.data_ptr(), weights.lm_head.data_ptr(),
-                               weights.final_norm.data_ptr(), *self._arrs, 1 if interleave else 0, 0)
+                               weights.final_norm.data_ptr(), *self._arrs[:6], flags, 0, *scales)
         opts = _lib.EngineOpts(device, max_batch, ctx_max, max_prefill_tokens,
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
                                int(kv_cache_tokens or 0), (C.c_int32 * 3)(),
@@ -121,8 +137,20 @@ class Engine:
                                              C.byref(self._h)), "rr_engine_create")
 
     @classmethod
-    def synthetic(cls, spec: ModelSpec, seed: int = 0, device: int = 0, **kw) -> "Engine":
-        return cls(make_weights(spec, seed=seed, device=f"cuda:{device}"), device=device, **kw)
+    def synthetic(cls, spec: ModelSpec, seed: int = 0, device: int = 0, quantization: Optional[str] = None,
+                  **kw) -> "Engine":
+        """An engine on the seeded weights of make_weights.  quantization="fp8": those weights through quantize_fp8, the
+        bf16 copy freed before the engine is created (peak memory while quantizing: both copies, about 16 + 9.5 GB for
+        Llama-3-8B)."""
+        if quantization not in (None, "fp8"):
+            raise ValueError(f"quantization must be None or 'fp8', got {quantization!r}")
+        w = make_weights(spec, seed=seed, device=f"cuda:{device}")
+        if quantization == "fp8":
+            q = quantize_fp8(w)
+            del w
+            torch.cuda.empty_cache()     # the engine allocates its buffers with cudaMalloc, outside torch's cache
+            w = q
+        return cls(w, device=device, **kw)
 
     def close(self):
         if getattr(self, "_h", None):

@@ -171,6 +171,78 @@ def make_weights(spec: ModelSpec, seed: int = 0, sigma: float = 0.02, device="cu
     return w
 
 
+@dataclass
+class Fp8Weights:
+    """Weights with e4m3 layer projections (`litellm_params.quantization: fp8`): each of wqkv / wo / wgu / wdown is
+    Q [N, K] torch.float8_e4m3fn with one fp32 row scale s[n] = 2^e[n] (`*_scale`, [N]); embed, lm_head and the norms
+    stay bf16.  The engine computes exactly what a bf16 engine computes on dequantize() = bf16(Q * s)
+    (include/rr_b200.h, RR_WEIGHTS_FP8_E4M3)."""
+    spec: ModelSpec
+    embed: torch.Tensor
+    lm_head: torch.Tensor
+    final_norm: torch.Tensor
+    wqkv: List[torch.Tensor] = field(default_factory=list)
+    wo: List[torch.Tensor] = field(default_factory=list)
+    wgu: List[torch.Tensor] = field(default_factory=list)
+    wdown: List[torch.Tensor] = field(default_factory=list)
+    norm_attn: List[torch.Tensor] = field(default_factory=list)
+    norm_mlp: List[torch.Tensor] = field(default_factory=list)
+    wqkv_scale: List[torch.Tensor] = field(default_factory=list)
+    wo_scale: List[torch.Tensor] = field(default_factory=list)
+    wgu_scale: List[torch.Tensor] = field(default_factory=list)
+    wdown_scale: List[torch.Tensor] = field(default_factory=list)
+
+    PROJ = ("wqkv", "wo", "wgu", "wdown")
+
+    def tensors(self) -> List[torch.Tensor]:
+        out = [self.embed, self.lm_head, self.final_norm]
+        for name in self.PROJ:
+            out.extend(getattr(self, name))
+            out.extend(getattr(self, name + "_scale"))
+        out.extend(self.norm_attn)
+        out.extend(self.norm_mlp)
+        return out
+
+    def nbytes(self) -> int:
+        return sum(t.numel() * t.element_size() for t in self.tensors())
+
+    def dequantize(self) -> Weights:
+        """bf16(Q * s) of every projection (rr_op_dequantize_fp8_weight), exact; embed, lm_head and the norms are shared."""
+        from . import _lib
+        stream = torch.cuda.current_stream(self.embed.device).cuda_stream
+        w = Weights(self.spec, self.embed, self.lm_head, self.final_norm,
+                    norm_attn=list(self.norm_attn), norm_mlp=list(self.norm_mlp))
+        for name in self.PROJ:
+            for q, sc in zip(getattr(self, name), getattr(self, name + "_scale")):
+                d = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
+                _lib.check(_lib.lib.rr_op_dequantize_fp8_weight(q.data_ptr(), sc.data_ptr(), q.shape[0], q.shape[1],
+                                                                d.data_ptr(), q.shape[1], stream),
+                           "rr_op_dequantize_fp8_weight")
+                getattr(w, name).append(d)
+        return w
+
+
+def quantize_fp8(w: Weights) -> Fp8Weights:
+    """Per-row power-of-two e4m3 quantization of the layer projections on the GPU (rr_op_quantize_fp8_weight): row n gets
+    e[n] = the smallest integer with max |W[n]| <= 448 * 2^e, clamped to [-117, 127] (0 for a zero row), and
+    Q = e4m3_rne(W / 2^e).  embed, lm_head and the norms are cloned into allocations of their own, so the result keeps no
+    reference to `w` and dropping `w` frees all of its memory.  Raises for a row with Inf or NaN."""
+    from . import _lib
+    stream = torch.cuda.current_stream(w.embed.device).cuda_stream
+    out = Fp8Weights(w.spec, w.embed.clone(), w.lm_head.clone(), w.final_norm.clone(),
+                     norm_attn=[t.clone() for t in w.norm_attn], norm_mlp=[t.clone() for t in w.norm_mlp])
+    for name in Fp8Weights.PROJ:
+        for t in getattr(w, name):
+            assert t.dtype == torch.bfloat16 and t.is_contiguous() and t.dim() == 2
+            q = torch.empty(t.shape, dtype=torch.float8_e4m3fn, device=t.device)
+            sc = torch.empty(t.shape[0], dtype=torch.float32, device=t.device)
+            _lib.check(_lib.lib.rr_op_quantize_fp8_weight(t.data_ptr(), t.shape[0], t.shape[1], t.shape[1], q.data_ptr(),
+                                                          sc.data_ptr(), stream), "rr_op_quantize_fp8_weight")
+            getattr(out, name).append(q)
+            getattr(out, name + "_scale").append(sc)
+    return out
+
+
 def broadcast_weights(w: Weights, src: int = 0, group=None) -> None:
     """Start-up weight broadcast (K12): rank `src` -> every replica of the model group over
     NCCL/NVLink.  The only collective on the path; requests never cross GPUs afterwards.

@@ -158,8 +158,8 @@ def build_backends(cfg: RouterConfig, stub: bool, spec_override: Optional[str] =
                    ctx_max: Optional[int] = None) -> Dict[int, object]:
     """One backend per replica (GPU) named in the config; deployments on the same GPU share it.  Each engine serves the
     deployment's litellm_params.context_window (ctx_max overrides it) with its kv_cache_tokens pool (None: the full
-    max_batch x context window).  A pool outside [context window, max_batch x context window] raises ValueError before
-    any engine is created."""
+    max_batch x context window) and its quantization (fp8: e4m3 layer projections, Engine.synthetic).  A pool outside
+    [context window, max_batch x context window] raises ValueError before any engine is created."""
     backends: Dict[int, object] = {}
     for d in cfg.deployments:
         ctx = ctx_max if ctx_max is not None else d.context_window
@@ -178,7 +178,8 @@ def build_backends(cfg: RouterConfig, stub: bool, spec_override: Optional[str] =
         ctx = ctx_max if ctx_max is not None else d.context_window
         backends[d.gpu] = EngineBackend(Engine.synthetic(spec, seed=0, device=d.gpu, max_batch=max_batch,
                                                          ctx_max=ctx, prefix_cache=d.prefix_cache,
-                                                         kv_cache_tokens=d.kv_cache_tokens))
+                                                         kv_cache_tokens=d.kv_cache_tokens,
+                                                         quantization=d.quantization))
     return backends
 
 
