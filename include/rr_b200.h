@@ -350,6 +350,29 @@ int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const vo
 int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
                                const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies,
                                const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
+/* Decode attention with a sliding window W = window: the arguments of rr_op_decode_attn_qkv_paged plus window.  The row
+ * at position pos attends to positions max(0, pos - W + 1) .. pos of its slot; window 0 is full causal attention, and
+ * rr_op_decode_attn_qkv_paged is this call with window 0.  The kv splits divide the key tiles from the tile of
+ * max(0, pos - W + 1) on, so a row whose every key lies inside the window (pos < W) gets rr_op_decode_attn_qkv_paged's
+ * result bit for bit.  Table entries are read only for the pages of the window's tiles, so a table may map logical page p
+ * to pages[p mod R] (a ring of R pages) when no window spans more than R pages.  Returns RR_INVALID_ARGUMENT before touching the device
+ * for a negative window, and otherwise for whatever rr_op_decode_attn_qkv_paged rejects. */
+int rr_op_decode_attn_qkv_window(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                 void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads,
+                                 int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
+                                 const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream);
+/* Prefill attention with a sliding window W = window: the arguments of rr_op_prefill_attn_cached_paged plus window.  The
+ * query row at absolute position q (seq_pos0 + its row) attends to positions max(0, q - W + 1) .. q of its slot; window 0
+ * is full causal attention, and rr_op_prefill_attn_cached_paged is this call with window 0.  Each 128-row query tile reads
+ * key tiles from the tile of max(0, q0 - W + 1) on, q0 its first row's position; key tiles wholly outside a row's window
+ * leave its softmax state unchanged, so rows whose every key lies inside the window (q < W) get
+ * rr_op_prefill_attn_cached_paged's result bit for bit, and each row is the softmax over exactly its visible keys.
+ * Returns RR_INVALID_ARGUMENT before touching the device for a negative window, and otherwise for whatever
+ * rr_op_prefill_attn_cached_paged rejects. */
+int rr_op_prefill_attn_window(const void* q, const void* k_cache, const void* v_cache, void* out,
+                              const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                              int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
+                              const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream);
 /* Fused decode MLP, one launch exactly as the engine runs it for a batch of `rows` (tile width, K slices, grid and
  * schedule from the engine's rules; env RR_MLP_STATIC / RR_NO_TMA_EPI are read per call):
  *   act[b, n]       = bf16(SiLU(xn[b] . gate[n]) * (xn[b] . up[n]))                        bf16 [rows, inter]
@@ -441,7 +464,9 @@ typedef struct rr_model_weights {
     const void* const* norm_attn; /* n_layers x [hidden] */
     const void* const* norm_mlp;  /* n_layers x [hidden] */
     int32_t flags;                /* RR_WEIGHTS_* */
-    int32_t reserved;
+    /* Sliding-window attention W >= 0 (0: full causal): position q attends to positions max(0, q - W + 1) .. q.  A model
+     * property, not a deployment one; rr_engine_create refuses a negative value.  See rr_engine_submit for the KV ring. */
+    int32_t sliding_window;
     /* RR_WEIGHTS_FP8_E4M3 only (ignored otherwise): n_layers x fp32 [out_features] row scales of wqkv / wo / wgu / wdown */
     const void* const* wqkv_scale;
     const void* const* wo_scale;
@@ -477,7 +502,8 @@ typedef struct rr_engine_opts {
                                      max_batch x ctx_max (every row can hold ctx_max tokens at once, the pool never binds);
                                      otherwise a multiple of 64 in [ctx_max, max_batch x ctx_max], else rr_engine_create
                                      returns RR_INVALID_ARGUMENT before any CUDA call.  Each choice of a request reserves
-                                     ceil((n_prompt + max_new_tokens) / 64) pages when it is admitted; a request that does
+                                     ceil((n_prompt + max_new_tokens) / 64) pages when it is admitted, at most the ring of
+                                     a windowed model (rr_engine_submit); a request that does
                                      not fit waits at the head of the queue (nothing overtakes it).  Memory: 2 x n_layers x
                                      kv_cache_tokens x n_kv_heads x 256 B. */
     int32_t reserved[3];          /* ignored (pass zeros); keeps prefix_cache at offset 44 */
@@ -569,9 +595,16 @@ typedef struct rr_gen_params {
  *   included, and frees its decode row at once; a stop-sequence cut on the same token wins.
  * A choice that reaches max_new_tokens first finishes with reason 0 (length), in JSON mode with a valid prefix.  The
  * request is done when every choice has finished.
+ * Sliding window (rr_model_weights.sliding_window = W > 0): with Tmax = max_prefill_tokens, a choice reserves at most
+ * R = ceil((W + Tmax - 2) / 64) + 1 pages, the most any prefill piece or decode step reads and writes at once.  A request
+ * whose reach (n_prompt + max_new_tokens) needs more is a ring request: each of its slots holds R pages and its page-table
+ * row maps logical page p to the slot's page p mod R, so positions more than W - 1 behind every query still to come are
+ * overwritten.  A ring request takes no prefix-cache hit and its slots retain nothing; every other request pages and
+ * caches as without a window.
  * RR_INVALID_ARGUMENT, before anything is queued and with *ticket untouched, for a NULL engine, prompt or ticket,
  * n_prompt or max_new_tokens below 1, n_prompt + max_new_tokens above ctx_max,
- * n_choices x ceil((n_prompt + max_new_tokens) / 64) x 64 above kv_cache_tokens (the request could never be admitted), a
+ * n_choices x min(ceil((n_prompt + max_new_tokens) / 64), R) x 64 above kv_cache_tokens (the request could never be
+ * admitted; R as above, no limit without a window), a
  * prompt token outside [0, vocab), and for parameters outside these ranges (NaN is outside every range):
  * 1 <= n_choices <= max_batch; -1 <= top_logprobs <= 20; 0 <= temperature <= 2; 0 <= top_p <= 1; -2 <= penalties <= 2;
  * 0 <= n_bias <= 300 with non-null arrays when n_bias > 0, unique bias ids in [0, vocab) and -100 <= bias values <= 100;
@@ -703,8 +736,8 @@ int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
  * RR_NO_GROUP for an unknown group; RR_INVALID_ARGUMENT (HTTP 400) for n_prompt or max_new_tokens below 1, n_choices
  * outside 1..the smallest max_batch of the gateway's engines (a mock replica sets no limit and replies with n_choices
  * copies of its reply), prompt + max_new_tokens beyond a replica's context,
- * n_choices x ceil((prompt + max_new_tokens) / 64) x 64 beyond the smallest KV pool of the gateway's engines (a mock
- * replica sets no KV limit) and a bad token id. */
+ * n_choices x min(ceil((prompt + max_new_tokens) / 64), R) x 64 beyond the KV pool of any of the gateway's engines, R
+ * that engine's ring (rr_engine_submit; no limit without a window; a mock replica sets no KV limit), and a bad token id. */
 int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                       const rr_gen_params* p, uint64_t* ticket);
 /* A closed burst of plain requests (greedy, one choice) as one contiguous block of the admission trace (declare_burst != 0

@@ -77,7 +77,7 @@ class ModelWeights(C.Structure):
     _fields_ = [("embed", vp), ("lm_head", vp), ("final_norm", vp),
                 ("wqkv", C.POINTER(vp)), ("wo", C.POINTER(vp)), ("wgu", C.POINTER(vp)),
                 ("wdown", C.POINTER(vp)), ("norm_attn", C.POINTER(vp)),
-                ("norm_mlp", C.POINTER(vp)), ("flags", C.c_int32), ("reserved", C.c_int32),
+                ("norm_mlp", C.POINTER(vp)), ("flags", C.c_int32), ("sliding_window", C.c_int32),
                 ("wqkv_scale", C.POINTER(vp)), ("wo_scale", C.POINTER(vp)), ("wgu_scale", C.POINTER(vp)),
                 ("wdown_scale", C.POINTER(vp))]
 
@@ -190,6 +190,8 @@ PROTOTYPES = {
     "rr_op_kv_copy_prefix": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int, vp]),
     "rr_op_prefill_attn_cached_paged": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                                   C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]),
+    "rr_op_prefill_attn_window": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                            C.c_int, C.c_float, vp, C.c_int, C.c_int, C.c_int, vp]),
     "rr_op_kv_copy_prefix_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int,
                                              vp, C.c_int, C.c_int, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
@@ -199,6 +201,9 @@ PROTOTYPES = {
     "rr_op_decode_attn_qkv_paged": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
                                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp, C.c_int, C.c_int,
                                               vp]),
+    "rr_op_decode_attn_qkv_window": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,
+                                               C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_i32p, vp, C.c_int, C.c_int,
+                                               C.c_int, vp]),
     "rr_op_add_rmsnorm_pf": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_float, vp, C.c_int, vp]),
     "rr_op_prefill_qkv": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                     C.c_float, vp, vp, vp, vp, vp, c_i32p, vp]),

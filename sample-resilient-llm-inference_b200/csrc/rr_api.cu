@@ -355,8 +355,8 @@ RR_API int rr_op_decode_attn(const void* q,const void* k_cache, const void* v_ca
 static int decode_attn_qkv(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache, void* v_cache,
                            void* out, const int32_t* slot, const int32_t* pos, int rows, int n_heads, int n_kv_heads,
                            int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits, const int32_t* page_table,
-                           int pages_per_slot, int n_pages, void* stream) {
-    if (!qkv || !k_cache || !v_cache || !out || !slot || !pos || !kv_splits) return RR_INVALID_ARGUMENT;
+                           int pages_per_slot, int n_pages, int window, void* stream) {
+    if (!qkv || !k_cache || !v_cache || !out || !slot || !pos || !kv_splits || window < 0) return RR_INVALID_ARGUMENT;
     if (rows < 1 || n_slots < 1 || n_splits < 1) return RR_INVALID_ARGUMENT;
     if (n_kv_heads <= 0 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
     const int G = n_heads / n_kv_heads;
@@ -371,7 +371,7 @@ static int decode_attn_qkv(const float* qkv, int n_splits, long long split_strid
     a.scale = 1.0f / sqrtf((float)head_dim);
     a.kv_splits = pick_kv_splits(rows, n_kv_heads); a.ws = nullptr;
     a.fuse_rope = 1; a.qkv = mk_part(qkv, 0, n_splits, split_stride, ld); a.head_dim = head_dim;
-    a.page_table = page_table; a.pages_per_slot = pages_per_slot;
+    a.page_table = page_table; a.pages_per_slot = pages_per_slot; a.window = window;
     { int rcm = decode_attn_make_maps(&a, page_table ? n_pages : n_slots); if (rcm != RR_OK) return rcm; }
     cudaStream_t st = (cudaStream_t)stream;
     float2* table = nullptr;
@@ -397,7 +397,7 @@ RR_API int rr_op_decode_attn_qkv(const float* qkv, int n_splits, long long split
                                  int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta, int* kv_splits,
                                  void* stream) {
     return decode_attn_qkv(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads, n_kv_heads,
-                           head_dim, ctx_max, n_slots, theta, kv_splits, nullptr, 0, 0, stream);
+                           head_dim, ctx_max, n_slots, theta, kv_splits, nullptr, 0, 0, 0, stream);
 }
 
 // The paged entry points' own checks, made before their counterpart's: a page table, at least one page per slot and in the
@@ -406,14 +406,24 @@ static bool paged_ok(const int32_t* page_table, int pages_per_slot, int n_pages,
     return page_table && pages_per_slot >= 1 && n_pages >= 1 && (long long)ctx_max == (long long)KV_PAGE * pages_per_slot;
 }
 
+RR_API int rr_op_decode_attn_qkv_window(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
+                                        void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows,
+                                        int n_heads, int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta,
+                                        int* kv_splits, const int32_t* page_table, int pages_per_slot, int n_pages,
+                                        int window, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return decode_attn_qkv(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads, n_kv_heads,
+                           head_dim, ctx_max, n_slots, theta, kv_splits, page_table, pages_per_slot, n_pages, window, stream);
+}
+
 RR_API int rr_op_decode_attn_qkv_paged(const float* qkv, int n_splits, long long split_stride, int ld, void* k_cache,
                                        void* v_cache, void* out, const int32_t* slot, const int32_t* pos, int rows,
                                        int n_heads, int n_kv_heads, int head_dim, int ctx_max, int n_slots, float theta,
                                        int* kv_splits, const int32_t* page_table, int pages_per_slot, int n_pages,
                                        void* stream) {
-    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
-    return decode_attn_qkv(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads, n_kv_heads,
-                           head_dim, ctx_max, n_slots, theta, kv_splits, page_table, pages_per_slot, n_pages, stream);
+    return rr_op_decode_attn_qkv_window(qkv, n_splits, split_stride, ld, k_cache, v_cache, out, slot, pos, rows, n_heads,
+                                        n_kv_heads, head_dim, ctx_max, n_slots, theta, kv_splits, page_table, pages_per_slot,
+                                        n_pages, 0, stream);
 }
 
 // Layer 0's RMSNorm of a prefill chunk in the deferred form, the only form run_prefill launches.
@@ -622,8 +632,8 @@ RR_API int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_
 static int prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* seq_start,
                                const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs, int max_len, int n_heads,
                                int n_kv_heads, int ctx_max, float scale, const int32_t* page_table, int pages_per_slot,
-                               int n_pages, void* stream) {
-    if (!q || !k_cache || !v_cache || !out || !seq_start || !seq_slot || !seq_pos0) return RR_INVALID_ARGUMENT;
+                               int n_pages, int window, void* stream) {
+    if (!q || !k_cache || !v_cache || !out || !seq_start || !seq_slot || !seq_pos0 || window < 0) return RR_INVALID_ARGUMENT;
     if (n_seqs < 1 || max_len < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
     if (ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
     cudaStream_t st = (cudaStream_t)stream;
@@ -644,7 +654,7 @@ static int prefill_attn_cached(const void* q, const void* k_cache, const void* v
     a.v_cache = (const __nv_bfloat16*)v_cache; a.out = (__nv_bfloat16*)out; a.seq_start = seq_start;
     a.seq_slot = seq_slot; a.seq_pos0 = seq_pos0; a.n_seqs = n_seqs; a.max_len = max_len; a.n_heads = n_heads;
     a.n_kv_heads = n_kv_heads; a.ctx_max = ctx_max; a.scale = scale; a.head_dim = 128;
-    a.page_table = page_table; a.pages_per_slot = pages_per_slot;
+    a.page_table = page_table; a.pages_per_slot = pages_per_slot; a.window = window;
     (void)prefill_attn_make_maps(&a, h[n_seqs], page_table ? (long long)n_pages * n_kv_heads * KV_PAGE
                                                            : (long long)(max_slot + 1) * n_kv_heads * ctx_max);
     const int rcl = launch_prefill_attn(a, st);
@@ -656,16 +666,24 @@ RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const v
                                      const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
                                      int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream) {
     return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
-                               ctx_max, scale, nullptr, 0, 0, stream);
+                               ctx_max, scale, nullptr, 0, 0, 0, stream);
+}
+
+RR_API int rr_op_prefill_attn_window(const void* q, const void* k_cache, const void* v_cache, void* out,
+                                     const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
+                                     int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
+                                     const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
+                               ctx_max, scale, page_table, pages_per_slot, n_pages, window, stream);
 }
 
 RR_API int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const void* v_cache, void* out,
                                            const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0,
                                            int n_seqs, int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
                                            const int32_t* page_table, int pages_per_slot, int n_pages, void* stream) {
-    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
-    return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
-                               ctx_max, scale, page_table, pages_per_slot, n_pages, stream);
+    return rr_op_prefill_attn_window(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads,
+                                     n_kv_heads, ctx_max, scale, page_table, pages_per_slot, n_pages, 0, stream);
 }
 
 // Prefix copy between KV slots as the engine runs it at the start of a prefill chunk.  The lists are host arrays, checked

@@ -14,6 +14,8 @@
 //    CUDA-core dot-product loop (profiles/r01_*): the kernel is issue-light and stays HBM-bound.
 //  * Each of the 4 consumer warps owns 16 tokens of every tile with a private online-softmax state;
 //    states are merged once at the end (and across kv splits by a small combine kernel).
+//  * Sliding window (DecodeAttnArgs::window): the tiles start at that of the row's first visible key; keys below it are
+//    masked in that tile.
 //
 // Replaces the remote bedrock:InvokeModel call (reference iam/policy.json:8).
 #include <stdlib.h>
@@ -104,13 +106,17 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
         return;
     }
     const int ctx = a.pos[row] + 1;
+    const int pos = ctx - 1;
+    // sliding window: keys lo .. pos.  The splits divide tiles lo / DT .. (ctx - 1) / DT; the first of them holds key lo, so
+    // every split with a tile has a visible key.  Without a window (or pos < W) lo = 0 and the tiles are today's.
+    const int lo = a.window > 0 ? max(0, pos - a.window + 1) : 0;
+    const int tile_lo = lo / DT;
     const int n_tiles_all = (ctx + DT - 1) / DT;
-    const int tiles_per = (n_tiles_all + a.kv_splits - 1) / a.kv_splits;
-    const int tile0 = split * tiles_per;
+    const int tiles_per = (n_tiles_all - tile_lo + a.kv_splits - 1) / a.kv_splits;
+    const int tile0 = tile_lo + split * tiles_per;
     const int tile1 = min(n_tiles_all, tile0 + tiles_per);
     const int n_units = 2 * max(0, tile1 - tile0);
 
-    const int pos = ctx - 1;
     const bool owns_new = a.fuse_rope && tile1 == n_tiles_all && tile1 > tile0;   // this split holds token `pos`
 
     if (warp == 4) {
@@ -308,8 +314,8 @@ decode_attn_mma_kernel(const __grid_constant__ DecodeAttnArgs a) {
             // ---- online softmax over tokens (rows g and g+8 of the fragment), per head column
             const int tok = tile * DT + warp * 16 + g;
             float s00 = c[0] * sc, s01 = c[1] * sc, s10 = c[2] * sc, s11 = c[3] * sc;
-            if (tok >= ctx) { s00 = -INFINITY; s01 = -INFINITY; }
-            if (tok + 8 >= ctx) { s10 = -INFINITY; s11 = -INFINITY; }
+            if (tok >= ctx || tok < lo) { s00 = -INFINITY; s01 = -INFINITY; }
+            if (tok + 8 >= ctx || tok + 8 < lo) { s10 = -INFINITY; s11 = -INFINITY; }
             float mx0 = fmaxf(s00, s10), mx1 = fmaxf(s01, s11);
 #pragma unroll
             for (int of = 4; of < 32; of <<= 1) {

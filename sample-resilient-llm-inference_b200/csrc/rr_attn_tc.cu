@@ -21,6 +21,9 @@
 // mask and the skip test use absolute positions, Q stays at the sequence's rows of q.  A query row visits key tiles
 // 0, 1, ... in order whatever its tile, and a fully masked tile leaves m, l and O bit-unchanged (alpha = 1, P = 0 against
 // finite V), so a row's output does not depend on pos0: it is the row of a cold run over the whole sequence, bit for bit.
+// Sliding window (W > 0): a query tile starts at the key tile of its first row's first visible key, and keys below
+// q - W + 1 are masked too; a tile wholly below a row's window leaves its state unchanged as well (also while the row has
+// seen no key: m = -inf, l = 0, O = 0), so the same holds with a window.
 // Any GQA group size (MHA included): the kv head is head / (n_heads / n_kv_heads).  Head dims below 128 (Phi-3-mini:
 // 96) are zero-padded to 128 in q and the caches; only the true head dim is written.
 //
@@ -59,7 +62,7 @@ __device__ __forceinline__ float ex2(float x) {
 }
 
 struct Work {
-    int qt, seq, head, tok0, len, pos0, n_kt;
+    int qt, seq, head, tok0, len, pos0, kt0, n_kt;   // key tiles kt0 .. n_kt - 1
 };
 // Work item w -> (query tile, sequence, head).  The sequence bounds, its first position (and the slot, for the producer)
 // are loaded one item ahead (WorkFetch) so their latency hides under the current item.
@@ -87,6 +90,8 @@ __device__ __forceinline__ bool decode_work(const PrefillAttnArgs& a, int w, int
     // key tiles up to the tile's last query position (absolute: the cached prefix comes first)
     const int rows = (k.qt + 1) * TQ < k.len ? (k.qt + 1) * TQ : k.len;
     k.n_kt = (k.pos0 + rows + TKV - 1) / TKV;
+    // sliding window: from the tile of the first row's first visible key (0 while that row is below the window)
+    k.kt0 = a.window > 0 ? max(0, k.pos0 + k.qt * TQ - a.window + 1) / TKV : 0;
     return true;
 }
 
@@ -139,8 +144,8 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                     return (int)kv_page_row(paged, kv_page(a.page_table, a.pages_per_slot, f.slot, j * TKV), a.n_kv_heads,
                                             a.ctx_max, kvh, j * TKV);
                 };
-                int kv_next = kv_tile_row(0);
-                for (int j = 0; j < k.n_kt; ++j, ++kv_it) {
+                int kv_next = kv_tile_row(k.kt0);
+                for (int j = k.kt0; j < k.n_kt; ++j, ++kv_it) {
                     const uint32_t s = kv_it % NS;
                     const int kv_r = kv_next;
                     if (j + 1 < k.n_kt) kv_next = kv_tile_row(j + 1);
@@ -173,17 +178,22 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             // causal / ragged bound (inclusive) and the warpgroup's last row, as absolute positions of the slot
             const int last0 = k.pos0 + min(q0, k.len - 1), last1 = k.pos0 + min(q0 + 8, k.len - 1);
             const int wg_last_row = k.pos0 + k.qt * TQ + 64 * g + 63;
+            // sliding window: the first visible key of each row (a lower causal bound), and of the warpgroup's first row.
+            // Without a window the bounds lie below every key.
+            const int W = a.window > 0 ? a.window : (1 << 30);
+            const int first0 = last0 - W + 1, first1 = last1 - W + 1;
+            const int wg_first_key = k.pos0 + k.qt * TQ + 64 * g - W + 1;
             float o[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) o[i] = 0.f;
             float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running max (log2 domain), partial row sums
             mbar_wait(&bars->q_full, q_it & 1);
             ++q_it;
-            for (int j = 0; j < k.n_kt; ++j, ++kv_it) {
+            for (int j = k.kt0; j < k.n_kt; ++j, ++kv_it) {
                 const uint32_t s = kv_it % NS;
                 mbar_wait(&bars->kv_full[s], (kv_it / NS) & 1);
                 const int key0 = j * TKV;
-                if (key0 <= wg_last_row) {
+                if (key0 <= wg_last_row && key0 + TKV > wg_first_key) {
                     const uint32_t k_u = kv_u + s * 2 * KV_BYTES, v_u = k_u + KV_BYTES;
                     float sa[32];
                     wgmma_fence_regs(sa);
@@ -197,14 +207,15 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                     wgmma_fence_regs(sa);
                     // ---- causal mask, online softmax (a row lives in the 4 threads of a quad)
                     const int lim0 = last0 - key0, lim1 = last1 - key0;
+                    const int low0 = first0 - key0, low1 = first1 - key0;
                     float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
                     for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int col = 8 * jj + cq + e;
-                            if (col > lim0) sa[4 * jj + e] = -INFINITY;
-                            if (col > lim1) sa[4 * jj + 2 + e] = -INFINITY;
+                            if (col > lim0 || col < low0) sa[4 * jj + e] = -INFINITY;
+                            if (col > lim1 || col < low1) sa[4 * jj + 2 + e] = -INFINITY;
                             mx0 = fmaxf(mx0, sa[4 * jj + e]);
                             mx1 = fmaxf(mx1, sa[4 * jj + 2 + e]);
                         }
@@ -214,8 +225,11 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
                         mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, x));
                         mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, x));
                     }
+                    // A window can mask a row's whole tile before its first visible key (m = n = -inf): the exponents
+                    // then use 0 instead of -inf - (-inf) = NaN, giving alpha = 0 and P = 0, so the row stays empty.
                     const float n0 = fmaxf(m0, mx0 * sc), n1 = fmaxf(m1, mx1 * sc);
-                    const float al0 = ex2(m0 - n0), al1 = ex2(m1 - n1);   // m = -inf on the first tile: 0
+                    const float e0n = n0 == -INFINITY ? 0.f : n0, e1n = n1 == -INFINITY ? 0.f : n1;
+                    const float al0 = ex2(m0 - e0n), al1 = ex2(m1 - e1n);   // m = -inf on the first tile: 0
                     m0 = n0; m1 = n1;
                     l0 *= al0; l1 *= al1;
 #pragma unroll
@@ -229,8 +243,8 @@ prefill_attn_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
                             const int b = 8 * kk + 4 * h;
-                            const float e0 = ex2(fmaf(sa[b], sc, -n0)), e1 = ex2(fmaf(sa[b + 1], sc, -n0));
-                            const float e2 = ex2(fmaf(sa[b + 2], sc, -n1)), e3 = ex2(fmaf(sa[b + 3], sc, -n1));
+                            const float e0 = ex2(fmaf(sa[b], sc, -e0n)), e1 = ex2(fmaf(sa[b + 1], sc, -e0n));
+                            const float e2 = ex2(fmaf(sa[b + 2], sc, -e1n)), e3 = ex2(fmaf(sa[b + 3], sc, -e1n));
                             l0 += e0 + e1;
                             l1 += e2 + e3;
                             pa[kk][2 * h] = pack_bf16(e0, e1);

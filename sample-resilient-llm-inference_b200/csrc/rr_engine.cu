@@ -282,6 +282,9 @@ struct rr_engine {
     // device table d_table [Bm][pps] has a fixed address (the decode graphs hold it); h_table is its pinned mirror, and
     // table_dirty[b] marks the rows upload_table copies before the next prefill chunk or decode step.
     int n_pages = 0, pps = 0;
+    // Sliding window (rr_model_weights.sliding_window, 0: none) and the ring a windowed request reserves instead of its whole
+    // reach (ring_pages; 0 without a window).  A ring request's table row maps logical page p to slot_pages[b][p % ring].
+    int window = 0, ring = 0;
     int32_t *d_table = nullptr, *h_table = nullptr;
     std::vector<std::vector<int32_t>> slot_pages;
     std::vector<int32_t> free_pages;
@@ -906,6 +909,23 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
 // ---------------------------------------------------------------- KV page pool (caller holds e->mu)
 static int pages_for(int tokens) { return (tokens + KV_PAGE - 1) / KV_PAGE; }
 
+// The ring of a windowed engine: R = ceil((W + Tmax - 2) / 64) + 1 pages.  A prefill piece of len <= Tmax rows at positions
+// pos0 .. pos0 + len - 1 reads keys from pos0 - W + 1 on and writes its own rows in the QKV epilogue before attention reads
+// them, so the positions live at once are the W + len - 1 <= W + Tmax - 1 from pos0 - W + 1 to pos0 + len - 1, and n
+// consecutive positions touch at most ceil((n - 1) / 64) + 1 pages: R pages, which are distinct mod R.  A decode step
+// needs the pages of W positions, fewer.  So mapping logical page p to pages[p mod R] never lets a write land on a page
+// still read, and R - 1 pages fail for the alignment that touches R pages (tests/test_sliding_window_cpu.py).
+static int ring_pages(int window, int tmax) { return window > 0 ? pages_for(window + tmax - 2) + 1 : 0; }
+
+// Pages one choice reaching `reach` positions reserves: ceil(reach / 64), or the ring when that is smaller.
+static int choice_pages(const rr_engine* e, int reach) {
+    const int n = pages_for(reach);
+    return e->ring > 0 && n > e->ring ? e->ring : n;
+}
+static bool ring_request(const rr_engine* e, const Request* r) {
+    return e->ring > 0 && pages_for((int)r->prompt.size() + r->max_new) > e->ring;
+}
+
 // Slot b holds exactly n pages: it keeps its first ones, returns extra ones from the end and takes missing ones from the free
 // stack (the caller made sure there are enough).  Pages go back in the reverse of the order they were taken, so a slot
 // that returns its pages and takes as many again gets the same ones: its table row does not change and is not copied.
@@ -946,17 +966,26 @@ static void reclaim_pages(rr_engine* e, int need) {
     }
 }
 
-// The request just took the slots r->rows: give each ceil((prompt + max_new) / 64) pages, shrinking before growing so the
-// pages a slot returns serve the others first.
+// The request just took the slots r->rows: give each choice_pages pages, shrinking before growing so the pages a slot
+// returns serve the others first.  Entries [0, pages) of a slot's table row always name its pages in order; a ring
+// request's row also maps every later logical page p to pages[p % ring] (rewritten, and so uploaded, only where it changes).
 static void take_pages(rr_engine* e, const Request* r) {
-    const int need = pages_for((int)r->prompt.size() + r->max_new);
+    const int need = choice_pages(e, (int)r->prompt.size() + r->max_new);
     int missing = 0;
     for (int b : r->rows) {
         if ((int)e->slot_pages[b].size() > need) resize_pages(e, b, need);
         missing += need - (int)e->slot_pages[b].size();
     }
     reclaim_pages(e, missing);
-    for (int b : r->rows) resize_pages(e, b, need);
+    const bool ring = ring_request(e, r);
+    for (int b : r->rows) {
+        resize_pages(e, b, need);
+        for (int p = need; ring && p < e->pps; ++p) {
+            int32_t& t = e->h_table[(size_t)b * e->pps + p];
+            const int32_t pg = e->slot_pages[b][p % need];
+            if (t != pg) { t = pg; e->table_dirty[b] = 1; }
+        }
+    }
 }
 
 // Slot b's request is done with it: keep the pages of its retained prefix (none without prefix caching), return the rest.
@@ -1213,7 +1242,10 @@ static void worker_main(rr_engine* e) {
                 Request* r = e->waiting.front();
                 if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all at its admission
                 int m = 0, src = -1;
-                if (e->o.prefix_cache) {
+                const bool ring = ring_request(e, r);       // the ring overwrites its prompt: no prefix hit, nothing kept
+                if (e->o.prefix_cache && ring) {
+                    if ((b = pick_slot_miss(e)) < 0) break;
+                } else if (e->o.prefix_cache) {
                     if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
                 } else {
                     while (b < e->Bm && e->row_req[b] != nullptr) ++b;
@@ -1228,7 +1260,7 @@ static void worker_main(rr_engine* e) {
                     n = room;
                 }
                 // every choice reserves its pages now; a request that does not fit waits at the head of the queue
-                if (r->n_choices * pages_for((int)r->prompt.size() + r->max_new) > pages_available(e)) break;
+                if (r->n_choices * choice_pages(e, (int)r->prompt.size() + r->max_new) > pages_available(e)) break;
                 e->waiting.pop_front();
                 r->n_cached = m;
                 r->n_done = m;
@@ -1302,7 +1334,7 @@ static void worker_main(rr_engine* e) {
                 }
                 r->n_done = pos0[i] + seq_start[i + 1] - seq_start[i];
                 if (!last) continue;                       // the prompt in progress: its next piece leads the next chunk
-                if (e->o.prefix_cache) {                   // every choice's slot holds the prompt's prefill-written KV
+                if (e->o.prefix_cache && !ring_request(e, r)) {   // every choice's slot holds the prompt's prefill-written KV
                     for (int b : r->rows) { e->retained[b] = r->prompt; e->retained_used[b] = ++e->lru_clock; }
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
@@ -1376,6 +1408,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     const long long kv_full = (long long)opts->max_batch * opts->ctx_max;
     const long long kv_tokens = opts->kv_cache_tokens == 0 ? kv_full : opts->kv_cache_tokens;
     if (kv_tokens % KV_PAGE || kv_tokens < opts->ctx_max || kv_tokens > kv_full) return RR_INVALID_ARGUMENT;
+    if (w->sliding_window < 0) return RR_INVALID_ARGUMENT;
     const bool fp8 = (w->flags & RR_WEIGHTS_FP8_E4M3) != 0;
     if (fp8) {      // e4m3 projections the decode GEMMs can stream, and their scales
         if (!w->wqkv_scale || !w->wo_scale || !w->wgu_scale || !w->wdown_scale) return RR_INVALID_ARGUMENT;
@@ -1396,6 +1429,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->nq = d.n_heads * d.head_dim; e->nkv_dim = d.n_kv_heads * d.head_dim; e->nqkv = e->nq + 2 * e->nkv_dim;
     e->Tmax = opts->max_prefill_tokens > 0 ? opts->max_prefill_tokens : 8192;
     if (e->Tmax < 16) e->Tmax = 16;
+    e->window = w->sliding_window;
+    e->ring = ring_pages(e->window, e->Tmax);
     e->embed = w->embed; e->lm_head = w->lm_head; e->final_norm = w->final_norm;
     const int L = d.n_layers;
     for (int l = 0; l < L; ++l) {
@@ -1497,7 +1532,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
             pa.q = e->pq; pa.k_cache = e->kcache + (size_t)l * e->kv_layer_stride;
             pa.v_cache = e->vcache + (size_t)l * e->kv_layer_stride; pa.n_heads = d.n_heads;
             pa.n_kv_heads = d.n_kv_heads; pa.ctx_max = opts->ctx_max; pa.head_dim = d.head_dim;
-            pa.page_table = e->d_table; pa.pages_per_slot = e->pps;
+            pa.page_table = e->d_table; pa.pages_per_slot = e->pps; pa.window = e->window;
             TRY(prefill_attn_make_maps(&pa, T, (long long)e->n_pages * d.n_kv_heads * KV_PAGE));
         }
         DecodeAttnArgs& da = e->attn_args[l];
@@ -1507,7 +1542,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         da.ctx_max = opts->ctx_max; da.scale = 1.0f / sqrtf((float)d.head_dim); da.ws = e->attn_ws;
         da.kv_splits = e->kv_splits;
         da.fuse_rope = 1; da.qkv = part_f32(e->part_qkv, e->s_qkv, B, e->nqkv); da.rope_table = e->rope_table;
-        da.head_dim = d.head_dim; da.page_table = e->d_table; da.pages_per_slot = e->pps;
+        da.head_dim = d.head_dim; da.page_table = e->d_table; da.pages_per_slot = e->pps; da.window = e->window;
         TRY(decode_attn_make_maps(&da, e->n_pages));
         // the decode projections: the same plans on e4m3 weights with FP8 (gemm_plan_init_fp8w)
         auto plan = [&](GemmPlan* p, const void* A, const float* sc, int rowsA, int K, const void* Bop, void* out, int ldo,
@@ -1675,7 +1710,7 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max) return RR_INVALID_ARGUMENT;
-    if ((long long)n_choices * pages_for(n_prompt + max_new_tokens) > e->n_pages) return RR_INVALID_ARGUMENT;
+    if ((long long)n_choices * choice_pages(e, n_prompt + max_new_tokens) > e->n_pages) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
         if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
     Request* r = new (std::nothrow) Request();
@@ -1718,9 +1753,10 @@ void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx) {
     std::lock_guard<std::mutex> lk(e->mu);
     e->hook = fn; e->hook_ctx = ctx;
 }
-int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens) {
+int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens, int* ring) {
     if (!e) return RR_INVALID_ARGUMENT;
     if (kv_tokens) *kv_tokens = e->n_pages * KV_PAGE;
+    if (ring) *ring = e->ring;
     if (max_batch) *max_batch = e->Bm;
     if (ctx_max) *ctx_max = e->o.ctx_max;
     if (vocab) *vocab = e->d.vocab;

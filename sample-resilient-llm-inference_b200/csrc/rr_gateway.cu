@@ -84,7 +84,8 @@ struct rr_gateway {
     int n_deps = 0, n_groups = 0;
     bool latency = false;                   // the router is latency-based: DONE / FAIL events carry samples
     int min_ctx = 0, min_vocab = 0, min_rows = 0;     // min_rows: decode rows, the limit of n_choices
-    int min_kv = 0;                                               // the smallest KV pool in tokens (rr_engine_opts.kv_cache_tokens)
+    // each engine's KV pool in pages and the pages a choice reserves at most (its ring; 0: no window), by engine_limits
+    std::vector<std::pair<int, int>> kv_pools;
     rr_gateway_opts opts;
 
     std::mutex mu;
@@ -379,15 +380,16 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
     memset(&g->st, 0, sizeof(g->st));
     rr::router_shape(router, &g->n_deps, &g->n_groups);
     g->latency = rr::router_strategy(router) == RR_STRATEGY_LATENCY_BASED;
-    g->min_ctx = g->min_vocab = g->min_rows = g->min_kv = 0x7fffffff;
+    g->min_ctx = g->min_vocab = g->min_rows = 0x7fffffff;
     g->stubs.assign((size_t)n_engines, rr_stub_desc{0, 0, 0, 0});
     g->stub_handed.assign((size_t)n_engines, 0);
     for (int i = 0; i < n_engines; ++i) {
         g->engines.push_back(engines[i]);
         g->by_replica[replica_ids[i]] = i;
-        int c = 0x7fffffff, v = 0, rows = 0x7fffffff, kv = 0x7fffffff;   // a mock replica: no KV limit
+        int c = 0x7fffffff, v = 0, rows = 0x7fffffff, kv = 0, ring = 0;   // a mock replica: no KV limit
         if (engines[i]) {
-            rr::engine_limits(engines[i], &c, &v, &rows, &kv);
+            rr::engine_limits(engines[i], &c, &v, &rows, &kv, &ring);
+            g->kv_pools.emplace_back(kv / rr::KV_PAGE, ring);
         } else {
             if (!stubs || stubs[i].reply_tokens < 0 || stubs[i].fail_every < 0 || stubs[i].vocab < 1) {
                 delete g;
@@ -400,7 +402,6 @@ RR_API int rr_gateway_create(rr_router* router, rr_engine* const* engines, const
         if (c < g->min_ctx) g->min_ctx = c;
         if (v < g->min_vocab) g->min_vocab = v;
         if (rows < g->min_rows) g->min_rows = rows;
-        if (kv < g->min_kv) g->min_kv = kv;
     }
     if (g->opts.record_trace > 0) {
         g->tr_ev.resize((size_t)g->opts.record_trace);
@@ -439,8 +440,13 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
     if (!ids || n_prompt < 1 || max_new < 1) return RR_INVALID_ARGUMENT;
     if (n_choices < 1 || n_choices > g->min_rows) return RR_INVALID_ARGUMENT;     // every choice takes a decode row
     if (n_prompt + max_new > g->min_ctx) return RR_INVALID_ARGUMENT;   // -> HTTP 400, before any debit
-    // every choice reserves whole 64-token KV pages of the smallest pool (rr_engine_submit)
-    if ((long long)n_choices * ((n_prompt + max_new + 63) / 64) * 64 > g->min_kv) return RR_INVALID_ARGUMENT;
+    // every choice reserves whole 64-token KV pages, at most a windowed engine's ring, in each engine's pool
+    // (rr_engine_submit): a request some engine could never fit is refused
+    const int pages = (n_prompt + max_new + rr::KV_PAGE - 1) / rr::KV_PAGE;
+    for (const auto& kp : g->kv_pools) {
+        const int per_choice = kp.second > 0 && pages > kp.second ? kp.second : pages;
+        if ((long long)n_choices * per_choice > kp.first) return RR_INVALID_ARGUMENT;
+    }
     for (int i = 0; i < n_prompt; ++i)
         if (ids[i] < 0 || ids[i] >= g->min_vocab) return RR_INVALID_ARGUMENT;
     return RR_OK;

@@ -136,7 +136,9 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
                          uint64_t* ticket, const GenParams& p, int n_choices);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 // kv_tokens: the KV pool (rr_engine_opts.kv_cache_tokens after its default is applied)
-int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens = nullptr);
+// ring: the pages a windowed engine's ring request reserves per choice (0: no window, every choice reserves its reach)
+int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens = nullptr,
+                  int* ring = nullptr);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
 int router_strategy(const rr_router* r);
@@ -373,6 +375,9 @@ struct DecodeAttnArgs {
     // pages of its tiles before the PDL wait.
     const int32_t* page_table = nullptr;
     int pages_per_slot = 0;
+    // sliding window W (0: full causal): the row at pos attends to max(0, pos - W + 1) .. pos, its tiles split from that
+    // key's tile on
+    int window = 0;
 };
 // Fills tmK / tmV (ctx_max % 64 == 0) over n_pages pages: n_slots without a page table.
 int decode_attn_make_maps(DecodeAttnArgs* a, int n_pages);
@@ -394,6 +399,7 @@ struct PrefillAttnArgs {
     CUtensorMap tmQ, tmK, tmV;
     const int32_t* page_table = nullptr;   // KV address rule (kv_row): the producer looks up the page of each key tile
     int pages_per_slot = 0;
+    int window = 0;           // sliding window W (0: full causal): query position q attends to max(0, q - W + 1) .. q
 };
 int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st);   // RR_ERR_ARG when the maps are missing / shape unsupported
 // wgmma kernel (rr_attn_tc.cu): one (sequence, head, 128-row query tile) per work item.

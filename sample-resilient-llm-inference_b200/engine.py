@@ -124,7 +124,7 @@ class Engine:
             scales = self._arrs[6:]
         flags = (_lib.RR_WEIGHTS_WGU_INTERLEAVED64 if interleave else 0) | (_lib.RR_WEIGHTS_FP8_E4M3 if fp8 else 0)
         mw = _lib.ModelWeights(weights.embed.data_ptr(), weights.lm_head.data_ptr(),
-                               weights.final_norm.data_ptr(), *self._arrs[:6], flags, 0, *scales)
+                               weights.final_norm.data_ptr(), *self._arrs[:6], flags, s.sliding_window, *scales)
         opts = _lib.EngineOpts(device, max_batch, ctx_max, max_prefill_tokens,
                                1 if use_cuda_graph else 0, fail_seed, fail_prob,
                                int(kv_cache_tokens or 0), (C.c_int32 * 3)(),

@@ -26,6 +26,8 @@ class ModelSpec:
     head_dim: int = 128
     rope_theta: float = 500000.0
     rms_eps: float = 1e-5
+    # sliding-window attention W (0: full causal): position q attends to positions max(0, q - W + 1) .. q
+    sliding_window: int = 0
 
     @property
     def n_params(self) -> int:
@@ -57,7 +59,8 @@ class ModelSpec:
 
 SPECS: Dict[str, ModelSpec] = {
     "llama-3-8b": ModelSpec("llama-3-8b", 128256, 4096, 14336, 32, 32, 8, 128, 500000.0, 1e-5),
-    "mistral-7b": ModelSpec("mistral-7b", 32000, 4096, 14336, 32, 32, 8, 128, 10000.0, 1e-5),
+    # Mistral-7B-v0.1: MistralConfig().sliding_window = 4096
+    "mistral-7b": ModelSpec("mistral-7b", 32000, 4096, 14336, 32, 32, 8, 128, 10000.0, 1e-5, 4096),
     # Phi-3-mini-4k: fused qkv / gate_up are layout only (our layout is fused anyway); head_dim 96, MHA
     "phi-3-mini": ModelSpec("phi-3-mini", 32064, 3072, 8192, 32, 32, 32, 96, 10000.0, 1e-5),
     # small shapes for parity tests / smoke (same kernels, same code path)
@@ -65,10 +68,22 @@ SPECS: Dict[str, ModelSpec] = {
     "small": ModelSpec("small", 4096, 1024, 2816, 4, 8, 2, 128, 10000.0, 1e-5),
     "llama-3-8b-2l": ModelSpec("llama-3-8b-2l", 128256, 4096, 14336, 2, 32, 8, 128, 500000.0, 1e-5),
     "phi-3-mini-2l": ModelSpec("phi-3-mini-2l", 32064, 3072, 8192, 2, 32, 32, 96, 10000.0, 1e-5),
-    "mistral-7b-2l": ModelSpec("mistral-7b-2l", 32000, 4096, 14336, 2, 32, 8, 128, 10000.0, 1e-5),
+    "mistral-7b-2l": ModelSpec("mistral-7b-2l", 32000, 4096, 14336, 2, 32, 8, 128, 10000.0, 1e-5, 4096),
+    # the tiny shape with a 100-token window (not a multiple of 64), for window tests that run past W in seconds
+    "tiny-sw": ModelSpec("tiny-sw", 1024, 512, 1024, 2, 4, 2, 128, 500000.0, 1e-5, 100),
     "tiny96": ModelSpec("tiny96", 1024, 384, 1024, 2, 4, 4, 96, 10000.0, 1e-5),
     "small96": ModelSpec("small96", 4096, 768, 2048, 3, 8, 2, 96, 10000.0, 1e-5),
 }
+
+
+def ring_pages(sliding_window: int, max_prefill_tokens: int) -> int:
+    """64-token KV pages a windowed engine's ring request reserves per choice: ceil((W + Tmax - 2) / 64) + 1, the most
+    pages the W + Tmax - 1 positions a prefill piece reads or writes can touch, Tmax the engine's prefill chunk
+    (rr_engine.cu ring_pages); 0 without a window.  A choice reserves min(ceil(reach / 64), ring)."""
+    if sliding_window <= 0:
+        return 0
+    tmax = max(16, max_prefill_tokens if max_prefill_tokens > 0 else 8192)
+    return -(-(sliding_window + tmax - 2) // 64) + 1
 
 
 def resolve_spec(model: str) -> ModelSpec:

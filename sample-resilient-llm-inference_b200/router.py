@@ -30,6 +30,7 @@ import numpy as np
 
 from . import _lib
 from .config import RouterConfig, build_config, load_config
+from .models import ring_pages
 
 
 # ---------------------------------------------------------------- errors (OpenAI-SDK names)
@@ -377,6 +378,20 @@ class EngineBackend:
 
 
 # ---------------------------------------------------------------- the router
+def _kv_refusal(backends, n_prompt: int, max_new: int, n: int) -> Optional[int]:
+    """The KV cache (tokens) of an attached engine replica that could never hold `n` choices of n_prompt + max_new tokens,
+    else None.  As in the gateway, a choice reserves its reach in 64-token pages, at most the ring of a replica whose
+    model has a sliding window."""
+    pages = -(-(n_prompt + max_new) // 64)
+    for b in backends.values():
+        if isinstance(b, EngineBackend):
+            e = b.engine
+            ring = ring_pages(getattr(e.spec, "sliding_window", 0), e.max_prefill_tokens)
+            if n * (min(pages, ring) if ring else pages) * 64 > e.kv_cache_tokens:
+                return e.kv_cache_tokens
+    return None
+
+
 class Router:
     def __init__(self, model_list: Optional[List[dict]] = None, *, routing_strategy: str = "simple-shuffle",
                  enable_pre_call_checks: bool = False, allowed_fails: Optional[int] = None,
@@ -515,13 +530,14 @@ class Router:
 
     def _invalid(self, n_prompt: int = 0, max_new: int = 0, n: int = 1) -> BadRequestError:
         """The HTTP 400 of a request the gateway refused with RR_INVALID_ARGUMENT, naming the limit it broke."""
-        ctx, rows, kv = self._limits()
+        ctx, rows, _ = self._limits()
+        kv = _kv_refusal(self.backends, n_prompt, max_new, n)
         if n > rows:
             return BadRequestError(f"`n` = {n} exceeds the {rows} decode rows of the smallest replica")
         if n_prompt + max_new > ctx:
             return BadRequestError(f"prompt ({n_prompt} tokens) + max_tokens ({max_new}) exceed the context window "
                                    f"({ctx} tokens) of the deployment")
-        if n * -(-(n_prompt + max_new) // 64) * 64 > kv:
+        if kv is not None:
             return BadRequestError(f"`n` ({n}) x (prompt ({n_prompt} tokens) + max_tokens ({max_new})), in 64-token pages, "
                                    f"exceed the KV cache ({kv} tokens) of the deployment")
         return BadRequestError("a token id is outside the vocabulary of the deployment, or a generation parameter is out "
