@@ -188,7 +188,8 @@ enum { RR_OUT_ROWMAJOR_BF16 = 0, RR_OUT_TRANSPOSED_F32 = 1,
        RR_OUT_TRANSPOSED_SILU = 2,   /* decode: A = interleaved weight [2*inter, K], out[b*ldo + n], splits = 1 */
        RR_OUT_ROWMAJOR_SILU = 3,     /* prefill: B = interleaved weight, bn >= 128, out[a*ldo + n] */
        RR_OUT_ROWMAJOR_ROPE = 4,     /* engine-internal (prefill QKV epilogue with RoPE + KV scatter) */
-       RR_OUT_ROWMAJOR_RESID = 5 };  /* out = fp32 residual [rowsA, ldo]: out[a*ldo + b] += acc (bn >= 32) */
+       RR_OUT_ROWMAJOR_RESID = 5,    /* out = fp32 residual [rowsA, ldo]: out[a*ldo + b] += acc (bn >= 32) */
+       RR_OUT_ROWMAJOR_F32 = 6 };    /* out fp32 [rowsA, ldo]: out[a*ldo + b] = acc (ldo even, out 8-byte aligned) */
 
 /* D[a,b] = sum_k A[a,k] B[b,k] on wgmma tensor cores (bf16 in, fp32 accumulate).
  * mode RR_OUT_ROWMAJOR_BF16:  out bf16 [rowsA, ldo], out[a*ldo + b]         (splits must be 1)
@@ -429,8 +430,11 @@ int rr_op_prefill_qkv(const void* xhat, const float* rowss, int plan_rows, int T
                       void* stream);
 /* The O, gate/up and down projections of a prefill chunk: rr_gemm_bf16's row-major modes on A [plan_rows][K] (pitch ldA),
  * launched for rows < T.
- *   mode RR_OUT_ROWMAJOR_BF16 / RR_OUT_ROWMAJOR_SILU with n_part > 0: deferred-norm consumer (rowss [plan_rows][n_part],
- *        n_part = ceil(hidden / 128)); n_part = 0: A is used as it is
+ *   mode RR_OUT_ROWMAJOR_BF16 / RR_OUT_ROWMAJOR_SILU / RR_OUT_ROWMAJOR_F32 with n_part > 0: deferred-norm consumer (rowss
+ *        [plan_rows][n_part], n_part = ceil(hidden / 128)); n_part = 0: A is used as it is
+ *   mode RR_OUT_ROWMAJOR_F32: out fp32 [T][ldo], out[t][n] = acc * rinv(t) for n < rowsW (ldo even, out 8-byte aligned);
+ *        rinv(t) = 1 / sqrt(sum(rowss[t][..]) / hidden + eps) with n_part > 0, else 1.  Rows >= T and columns >= rowsW are
+ *        not written.  lm_head over the prompt rows of a scoring prefill chunk (rr_engine_submit_scored).
  *   mode RR_OUT_ROWMAJOR_RESID: out is the fp32 residual [..][ldo], out[t][n] += acc.  With xhat: deferred-norm producer,
  *        xhat[t][n] = bf16(out[t][n] * gamma[n]) (pitch ldo) and rowss_out[t][p] = sum of out[t][n]^2 over n in
  *        [128 p, 128 p + 128), n_part_out = ceil(rowsW / 128)
@@ -615,6 +619,28 @@ typedef struct rr_gen_params {
  * generated_tokens counts every token produced, the ones a stop sequence cut included. */
 int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, const rr_gen_params* p,
                      uint64_t* ticket);
+/* rr_engine_submit that also scores the prompt when prompt_top >= 0 (-1: exactly rr_engine_submit).  Prompt logprobs
+ * (OpenAI /v1/completions `echo` with `logprobs`): for every prompt position t >= 1 the logprob of prompt[t] given
+ * prompt[0..t), and K = max(1, prompt_top) (logprob, id) pairs of the most likely tokens at t, ordered as rr_op_logprobs
+ * orders them.  Position 0 has none.  The prefill chunks that hold the prompt run the last layer and lm_head
+ * (RR_OUT_ROWMAJOR_F32) over its rows in prefill orientation, S = 1024 rows of fp32 logits at a time, then rr_op_logprobs'
+ * kernels with the next prompt token as the target.  A long prompt scores each piece as it runs.  The generated tokens
+ * and their logprobs are bit-identical to the request without scoring; with n_choices > 1 the prompt is scored once.  A
+ * scoring request takes no prefix-cache hit (every row must reach lm_head), so rr_completion.n_cached is 0; it retains
+ * its prompt like any other request.  The engine allocates the scoring buffers (S x vocab x 4 B of logits, about
+ * 525 MB at vocab 128256, and 96 B per max_prefill_tokens row) with its first scoring request; if that fails, the scoring
+ * requests end with RR_INTERNAL and the engine serves on.  Read the scores with rr_engine_prompt_logprobs before
+ * rr_engine_wait.  RR_INVALID_ARGUMENT, before anything is queued, for whatever rr_engine_submit rejects, prompt_top
+ * outside -1..20, and prompt_top >= 0 with a vocabulary that is not a multiple of 4. */
+int rr_engine_submit_scored(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                            const rr_gen_params* p, int prompt_top, uint64_t* ticket);
+/* Blocks like rr_engine_wait until the request is done, then copies its prompt logprobs WITHOUT consuming the ticket
+ * (finish with rr_engine_wait): target_lp_out [n_prompt - 1] (entry t - 1: position t), lp_out / id_out
+ * [n_prompt - 1][K] (each may be NULL).  Returns RR_OK, RR_TIMEOUT while in flight, the request's status when it did not
+ * end RR_OK (a cancel, a failure: nothing is written), and RR_INVALID_ARGUMENT for a NULL engine, an unknown, consumed or
+ * cancelled ticket and a request submitted without scoring. */
+int rr_engine_prompt_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
+                              int32_t* id_out);
 /* Block (release the GIL) until the request is done, or timeout_s (<= 0: no limit) elapses.  RR_TIMEOUT: still in flight
  * (out->status = RR_TIMEOUT), wait again or rr_engine_cancel.  Otherwise the ticket is consumed and the request's status
  * returned (RR_OK / RR_BACKEND_FAILED / ...), with `out` filled and for every choice c of its n_choices:
@@ -740,6 +766,16 @@ int rr_gateway_set_now(rr_gateway* g, int64_t now_ms);
  * that engine's ring (rr_engine_submit; no limit without a window; a mock replica sets no KV limit), and a bad token id. */
 int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                       const rr_gen_params* p, uint64_t* ticket);
+/* rr_gateway_submit with prompt logprobs (rr_engine_submit_scored; prompt_top -1: exactly rr_gateway_submit).  Also
+ * RR_INVALID_ARGUMENT, before anything is debited, for prompt_top outside -1..20, prompt_top >= 0 with a smallest
+ * vocabulary that is not a multiple of 4, and prompt_top >= 0 with a mock replica attached.  A fallback re-admission
+ * scores the prompt again on the new replica. */
+int rr_gateway_submit_scored(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                             const rr_gen_params* p, int prompt_top, uint64_t* ticket);
+/* rr_engine_prompt_logprobs for a gateway ticket: blocks until the request is finished and copies the scores of the
+ * replica that served it without consuming the ticket (finish with rr_gateway_wait).  Same buffers and returns. */
+int rr_gateway_prompt_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
+                               int32_t* id_out);
 /* A closed burst of plain requests (greedy, one choice) as one contiguous block of the admission trace (declare_burst != 0
  * prepends RR_EV_BURST). */
 int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,

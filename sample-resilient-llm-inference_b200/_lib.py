@@ -217,6 +217,9 @@ PROTOTYPES = {
     "rr_engine_prefill": (C.c_int, [vp, c_i32p, c_i32p, c_i32p, C.c_int, c_i32p, c_f32p]),
     "rr_engine_decode_step": (C.c_int, [vp, c_i32p, c_i32p, c_i32p, C.c_int, c_i32p, c_f32p]),
     "rr_engine_submit": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.POINTER(C.c_uint64)]),
+    "rr_engine_submit_scored": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.c_int,
+                                          C.POINTER(C.c_uint64)]),
+    "rr_engine_prompt_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, c_f32p, c_i32p]),
     "rr_engine_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p, c_i32p,
                                  c_i32p]),
     "rr_engine_peek": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
@@ -233,6 +236,9 @@ PROTOTYPES = {
     "rr_gateway_destroy": (None, [vp]),
     "rr_gateway_set_now": (C.c_int, [vp, C.c_int64]),
     "rr_gateway_submit": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.POINTER(C.c_uint64)]),
+    "rr_gateway_submit_scored": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.c_int,
+                                           C.POINTER(C.c_uint64)]),
+    "rr_gateway_prompt_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, c_f32p, c_i32p]),
     "rr_gateway_submit_batch": (C.c_int, [vp, C.c_int, c_i32p, c_i32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
     "rr_gateway_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p, c_i32p,
                                   c_i32p, c_i32p]),

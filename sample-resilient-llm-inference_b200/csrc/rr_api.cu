@@ -518,7 +518,8 @@ RR_API int rr_op_prefill_gemm(const void* A, int plan_rows, int T, int ldA, cons
                               void* xhat, float* rowss_out, int n_part_out, void* stream) {
     if (!A || !W || !out) return RR_INVALID_ARGUMENT;
     if (T < 1 || T > plan_rows || rowsW < 1) return RR_INVALID_ARGUMENT;
-    if (mode != OUT_ROWMAJOR_BF16 && mode != OUT_ROWMAJOR_SILU && mode != OUT_ROWMAJOR_RESID) return RR_INVALID_ARGUMENT;
+    if (mode != OUT_ROWMAJOR_BF16 && mode != OUT_ROWMAJOR_SILU && mode != OUT_ROWMAJOR_RESID && mode != OUT_ROWMAJOR_F32)
+        return RR_INVALID_ARGUMENT;
     if (n_part < 0 || (n_part > 0 && (!rowss || mode == OUT_ROWMAJOR_RESID || hidden < 1 || n_part != pf_norm_parts(hidden))))
         return RR_INVALID_ARGUMENT;
     if (xhat && (mode != OUT_ROWMAJOR_RESID || !gamma || !rowss_out || n_part_out != pf_norm_parts(rowsW)))

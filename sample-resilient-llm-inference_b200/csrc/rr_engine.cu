@@ -92,6 +92,10 @@ struct Request {
     int n_cached = 0;          // prefix caching: prompt tokens taken from the cache (prefill starts at this position)
     int n_done = 0;            // prompt tokens whose KV is in its slot (cached or prefilled), while it is admitted
     uint64_t epoch = 0;        // prefix caching: rr_engine::index_epoch when its first piece was admitted
+    // prompt logprobs (gen.scores()), written as the pieces run: ptgt[t - 1] = the logprob of prompt[t] given prompt[0..t),
+    // plp / plp_id [n_prompt - 1][gen.score_width()] the best pairs at position t
+    std::vector<float> ptgt, plp;
+    std::vector<int32_t> plp_id;
 
     // Tokens of choice c a reader may see: all of a finished choice, else those no stop sequence can take back.
     int visible(int c) const { return (int)out[c].size() - (finish[c] < 0 ? hold[c] : 0); }
@@ -330,6 +334,13 @@ struct rr_engine {
     // copy
     JsonState* d_json = nullptr;
     int32_t *d_json_done = nullptr, *h_json_done = nullptr;
+    // prompt logprobs (ensure_score_buffers, on the first scoring request): the fp32 logits of SCORE_ROWS prompt rows, the
+    // logprobs workspace, and per chunk row targets | prompt_top (d_sc_in / h_sc_in [2][Tmax]), the target's logprob
+    // [Tmax] and the best pairs [Tmax][LP_MAX_TOP], device and pinned
+    float* sc_logits = nullptr;
+    void* sc_ws = nullptr;
+    int32_t *d_sc_in = nullptr, *h_sc_in = nullptr, *d_sc_id = nullptr, *h_sc_id = nullptr;
+    float *d_sc_tlp = nullptr, *h_sc_tlp = nullptr, *d_sc_lp = nullptr, *h_sc_lp = nullptr;
 
     // prefill working set
     int Tmax;
@@ -488,6 +499,38 @@ static int ensure_pen_buffers(rr_engine* e) {
         if (rc == RR_OK) CK(cudaMemsetAsync(e->pen_ws, 0, sizeof(int32_t) * e->Bm * (size_t)e->d.vocab, e->stream));
     }
     return rc != RR_OK ? rc : ensure_block(e, 2);
+}
+
+// Prompt rows per lm_head block of a scoring chunk: the fp32 logits block is SCORE_ROWS x vocab (525 MB at 128256).
+constexpr int SCORE_ROWS = 1024;
+
+// Caller holds gpu_mu.  The prompt-logprob buffers, allocated on the first scoring request: SCORE_ROWS x vocab x 4 B of
+// logits, their logprobs workspace and 96 B x Tmax of inputs and results on the device and pinned.  All or nothing: on a
+// failure nothing stays allocated and the error is cleared, so the engine serves on without them.
+static int ensure_score_buffers(rr_engine* e) {
+    if (e->sc_logits) return RR_OK;
+    const size_t S = (size_t)std::min(SCORE_ROWS, e->Tmax), T = (size_t)e->Tmax, V = (size_t)e->d.vocab;
+    const size_t dev_bytes[5] = {S * V * 4, logprobs_ws_bytes((int)S, (int)V), 2 * T * 4, T * 4, 2 * T * LP_MAX_TOP * 4};
+    const size_t host_bytes[3] = {2 * T * 4, T * 4, 2 * T * LP_MAX_TOP * 4};
+    void* d[5] = {};
+    void* h[3] = {};
+    cudaError_t err = cudaSuccess;
+    for (int i = 0; i < 5 && err == cudaSuccess; ++i) err = cudaMalloc(&d[i], dev_bytes[i]);
+    for (int i = 0; i < 3 && err == cudaSuccess; ++i) err = cudaMallocHost(&h[i], host_bytes[i]);
+    if (err != cudaSuccess) {
+        rr::note_cuda_error(err);
+        for (void* p : d) if (p) cudaFree(p);
+        for (void* p : h) if (p) cudaFreeHost(p);
+        cudaGetLastError();                // an allocation failure is not sticky: later launches must not report it
+        return RR_CUDA_ERROR;
+    }
+    for (void* p : d) e->allocs.push_back(p);
+    e->sc_ws = d[1]; e->d_sc_in = (int32_t*)d[2]; e->d_sc_tlp = (float*)d[3];
+    e->d_sc_lp = (float*)d[4]; e->d_sc_id = (int32_t*)(e->d_sc_lp + T * LP_MAX_TOP);
+    e->h_sc_in = (int32_t*)h[0]; e->h_sc_tlp = (float*)h[1];
+    e->h_sc_lp = (float*)h[2]; e->h_sc_id = (int32_t*)(e->h_sc_lp + T * LP_MAX_TOP);
+    e->sc_logits = (float*)d[0];
+    return RR_OK;
 }
 
 // The rest of layer l after attention on `rows` rows of the decode working set, with the unfused kernels: O GEMM,
@@ -665,13 +708,13 @@ static int run_decode_step(rr_engine* e, int mode) {
 // ---------------------------------------------------------------- prefill chunk
 // FP8 weights: layer l's four projections dequantized into the prefill scratch (the layout init_pf_plans reads), one launch.
 // The last layer needs wqkv only: its O projection and MLP run on the chunk's tail rows through the decode kernels, which
-// read the e4m3 weights themselves.
-static int launch_dequant_layer(rr_engine* e, int l, cudaStream_t s) {
+// read the e4m3 weights themselves -- unless the chunk scores (scoring: the last layer also runs over every row).
+static int launch_dequant_layer(rr_engine* e, int l, bool scoring, cudaStream_t s) {
     const rr_model_desc& d = e->d;
     Fp8DequantJobs J;
     __nv_bfloat16* p = e->deq;
     fp8_dequant_job(&J, e->wqkv[l], e->sqkv[l], e->nqkv, d.hidden, p, d.hidden); p += (size_t)e->nqkv * d.hidden;
-    if (l + 1 == d.n_layers) return launch_dequantize_fp8(J, s);
+    if (l + 1 == d.n_layers && !scoring) return launch_dequantize_fp8(J, s);
     fp8_dequant_job(&J, e->wo[l], e->so[l], d.hidden, e->nq, p, e->nq); p += (size_t)d.hidden * e->nq;
     fp8_dequant_job(&J, e->wgu[l], e->sgu[l], 2 * d.inter, d.hidden, p, d.hidden); p += (size_t)2 * d.inter * d.hidden;
     fp8_dequant_job(&J, e->wdown[l], e->sdown[l], d.hidden, d.inter, p, d.inter);
@@ -738,6 +781,15 @@ struct PrefillTail {
     int mode = 0;
 };
 
+// The prompt rows of a prefill chunk that score (prompt logprobs), one entry per scoring sequence: the first rows[i] rows
+// of sequence seq[i], row j against the next prompt token tgt[o + j] (o = the rows of the entries before), with top[i]
+// pairs (prompt_top).  run_prefill leaves row o + j's results in h_sc_tlp[o + j] and h_sc_lp / h_sc_id [o + j][LP_MAX_TOP].
+struct PrefillScore {
+    std::vector<int> seq, rows, top;
+    std::vector<int32_t> tgt;
+    void clear() { seq.clear(); rows.clear(); top.clear(); tgt.clear(); }
+};
+
 // ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
 // activates the rows. Caller holds gpu_mu.
 // Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
@@ -750,13 +802,22 @@ struct PrefillTail {
 // logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
 // slots, one launch after the last layer copies positions [0, pos0 + its length) of its slot to each of them.
 // A chunk without tail rows (tail->n == 0) stops after the last layer's QKV projection and KV append: nothing after reads
-// its other outputs, and nothing is read back.
+// its other outputs, and nothing is read back -- unless it scores.
+// score (optional, needs ensure_score_buffers): a scoring chunk.  After the tail rows are gathered and have run through the
+// decode kernels, the last layer's O, gate/up and down GEMMs run over all T rows in prefill orientation (its down GEMM
+// leaves bf16(x * final_norm) and the partial sums of squares in pxn / p_rowss), then lm_head (OUT_ROWMAJOR_F32) and
+// launch_logprobs over the scoring rows only, in blocks of SCORE_ROWS rows of one sequence.  The tail rows were copied
+// before the full layer rewrites px, so what they compute does not change.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
-                       const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr) {
+                       const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr,
+                       const PrefillScore* score = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     const int nt = tail ? tail->n : n_seqs;
+    const bool scoring = score && !score->seq.empty();
+    const int n_score = scoring ? (int)score->tgt.size() : 0;
+    if (scoring && (!e->sc_logits || n_score > T)) return RR_INTERNAL;
     // the tail rows' slots and last tokens are listed apart (h_tsl / h_tlast) unless row j is sequence j in its own slot
     bool fan = nt != n_seqs;
     for (int j = 0; tail && !fan && j < nt; ++j) fan = tail->seq[j] != j || tail->slot[j] != slots[j];
@@ -816,6 +877,19 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     CK(cudaMemcpyAsync(e->p_ids, h, n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     e->st.h2d_bytes += n_ints * sizeof(int32_t);
     CK(hp.upload(dp, mode, s, &e->st.h2d_bytes));
+    if (scoring) {              // targets | prompt_top per scoring row
+        for (size_t i = 0, o = 0; i < score->seq.size(); o += (size_t)score->rows[i++]) {
+            const int q = score->seq[i];
+            if (q < 0 || q >= n_seqs || score->rows[i] < 1 || score->rows[i] > seq_start[q + 1] - seq_start[q])
+                return RR_INVALID_ARGUMENT;
+            for (int j = 0; j < score->rows[i]; ++j) e->h_sc_in[e->Tmax + o + j] = score->top[i];
+        }
+        memcpy(e->h_sc_in, score->tgt.data(), sizeof(int32_t) * n_score);
+        for (int half = 0; half < 2; ++half)
+            CK(cudaMemcpyAsync(e->d_sc_in + half * e->Tmax, e->h_sc_in + half * e->Tmax, sizeof(int32_t) * n_score,
+                               cudaMemcpyHostToDevice, s));
+        e->st.h2d_bytes += 2 * sizeof(int32_t) * n_score;
+    }
     int32_t *p_ids = e->p_ids, *p_pos = p_ids + T, *p_slt = p_ids + 2 * T, *p_ss = p_ids + 3 * T,
             *p_sl = p_ss + n_seqs + 1, *p_last = p_sl + n_seqs, *p_p0 = p_last + n_seqs;
     const int32_t* p_tsl = fan ? p_ids + (h_tsl - h) : p_sl;       // the tail rows' slots and last-token indices
@@ -844,7 +918,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         // dequantize starts after the previous layer's GEMMs have finished reading the scratch, and the QKV GEMM (and so
         // every later kernel, whose PDL weight prefetch runs before griddepcontrol.wait) after the scratch is complete.
         if (e->fp8) {
-            if (launch_dequant_layer(e, l, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
+            if (launch_dequant_layer(e, l, scoring, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         }
         if (launch_rows(P.qkv[l], !e->fp8) != RR_OK) return RR_CUDA_ERROR; ++nl;
         RopeArgs ra;
@@ -853,24 +927,50 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ra.n_heads = d.n_heads; ra.n_kv_heads = d.n_kv_heads; ra.ctx_max = e->o.ctx_max; ra.theta = d.rope_theta;
         ra.table = e->rope_table; ra.head_dim = d.head_dim; ra.page_table = e->d_table; ra.pages_per_slot = e->pps;
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
-        if (nt == 0 && l + 1 == d.n_layers) break;    // every layer's KV is written
+        if (nt == 0 && !scoring && l + 1 == d.n_layers) break;    // every layer's KV is written
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer TMA maps made at create
         pa.q = e->pq; pa.k_cache = kc; pa.v_cache = vc; pa.out = e->pattn; pa.seq_start = p_ss; pa.seq_slot = p_sl;
         pa.seq_pos0 = pos0 ? p_p0 : nullptr; pa.n_seqs = n_seqs; pa.max_len = max_len; pa.n_heads = d.n_heads; pa.n_kv_heads = d.n_kv_heads;
         pa.ctx_max = e->o.ctx_max; pa.scale = 1.0f / sqrtf((float)d.head_dim); pa.head_dim = d.head_dim;
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (l + 1 == d.n_layers) {
+        if (l + 1 == d.n_layers && nt > 0) {
             // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers).  The
             // unfused kernels even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
             launch_pdl(gather_last_kernel, dim3(nt), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
                        p_tlast, e->attn_out, e->x, e->nq, d.hidden); ++nl;
             if (enqueue_o_mlp(e, l, nt, s, &nl) != RR_OK) return RR_CUDA_ERROR;
-            break;
         }
+        if (l + 1 == d.n_layers && !scoring) break;    // a scoring chunk runs the whole last layer as well
         if (launch_rows(P.o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (launch_rows(P.gu[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (!e->fuse_silu) { launch_silu_mul(part_bf16(e->pgu, 2 * d.inter), e->pact, T, d.inter, s); ++nl; }
         if (launch_rows(P.down[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
+    }
+    if (scoring) {              // lm_head and log-softmax over the scoring rows, SCORE_ROWS rows of one sequence at a time
+        const int S = std::min(SCORE_ROWS, e->Tmax), V = d.vocab;
+        int o = 0;
+        for (size_t i = 0; i < score->seq.size(); ++i) {
+            const int r0 = seq_start[score->seq[i]];
+            for (int b = 0; b < score->rows[i]; b += S) {
+                const int nb = std::min(S, score->rows[i] - b);
+                GemmPlan hd;
+                if (gemm_plan_init(&hd, e->pxn + (size_t)(r0 + b) * d.hidden, nb, d.hidden, e->lm_head, V, d.hidden, d.hidden,
+                                   e->sc_logits, V, 0, 1, OUT_ROWMAJOR_F32, PF_BN) != RR_OK)
+                    return RR_INVALID_ARGUMENT;
+                pf_norm_consumer(&hd.rope, e->p_rowss + (size_t)(r0 + b) * e->pf_parts, d.hidden, d.rms_eps);
+                if (gemm_launch(hd, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
+                launch_logprobs(e->sc_logits, V, nb, V, e->d_sc_in + e->Tmax + o, LP_MAX_TOP, e->sc_ws,
+                                e->d_sc_lp + (size_t)o * LP_MAX_TOP, e->d_sc_id + (size_t)o * LP_MAX_TOP, s, e->d_sc_in + o,
+                                e->d_sc_tlp + o);
+                nl += LP_LAUNCHES;
+                o += nb;
+            }
+        }
+        const size_t n = (size_t)n_score * LP_MAX_TOP;
+        CK(cudaMemcpyAsync(e->h_sc_tlp, e->d_sc_tlp, sizeof(float) * n_score, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(e->h_sc_lp, e->d_sc_lp, sizeof(float) * n, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(e->h_sc_id, e->d_sc_id, sizeof(int32_t) * n, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += sizeof(float) * n_score + (sizeof(float) + sizeof(int32_t)) * n;
     }
     if (fan_copies.count) {     // every layer's KV of the prompts is written: fan it out before any decode step reads it
         if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, (long long)e->n_pages * d.n_kv_heads * KV_PAGE, d.n_kv_heads,
@@ -1182,12 +1282,52 @@ static void worker_main(rr_engine* e) {
     KvCopyList* copies = new KvCopyList();
     std::vector<int32_t> tail_seq, tail_slot, tail_choice;      // the chunk's tail rows (PrefillTail), one per choice
     std::vector<const GenParams*> tail_gen;
+    PrefillScore score;                                         // the chunk's scoring rows, and for each entry
+    std::vector<Request*> score_req;                            // its request and the position of its first row
+    std::vector<int> score_pos;
+    // sequence `seq` of the chunk is the piece [p0, p0 + n) of r's prompt: its rows that predict a prompt token score
+    auto add_score = [&](Request* r, int seq, int p0, int n) {
+        const int rows = std::min(n, (int)r->prompt.size() - 1 - p0);
+        if (!r->gen.scores() || rows < 1) return;
+        score.seq.push_back(seq); score.rows.push_back(rows); score.top.push_back(r->gen.prompt_top);
+        score.tgt.insert(score.tgt.end(), r->prompt.begin() + p0 + 1, r->prompt.begin() + p0 + 1 + rows);
+        score_req.push_back(r); score_pos.push_back(p0);
+    };
     bool decode_due = false;         // the last chunk left a prompt in progress: one decode step goes before the next chunk
     while (!e->stop.load()) {
         run_hooks(e, notes);
+        if (!e->sc_logits) {
+            // the first scoring request: its buffers before it is admitted.  If they cannot be had, the scoring requests fail
+            // and the engine serves on.
+            bool want = false;
+            {
+                std::lock_guard<std::mutex> lk(e->mu);
+                for (const Request* r : e->waiting) want = want || r->gen.scores();
+            }
+            if (want) {
+                int rc;
+                {
+                    std::lock_guard<std::mutex> gl(e->gpu_mu);
+                    std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
+                    rc = ensure_score_buffers(e);
+                }
+                if (rc != RR_OK) {
+                    std::lock_guard<std::mutex> lk(e->mu);
+                    for (auto it = e->waiting.begin(); it != e->waiting.end();) {
+                        Request* r = *it;
+                        if (!r->gen.scores()) { ++it; continue; }
+                        it = e->waiting.erase(it);
+                        finish_request(e, r, RR_INTERNAL, &notes);
+                    }
+                    e->cv_done.notify_all();
+                    continue;
+                }
+            }
+        }
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
         chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
         tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear();
+        score.clear(); score_req.clear(); score_pos.clear();
         copies->count = 0;
         int active = 0, decoding = 0;                      // rows held / rows decoding (not the prompt in progress's)
         int step = 0, chunk_mode = 0;                      // step_mode bits of the decoding rows / of the chunk's tail rows
@@ -1222,6 +1362,7 @@ static void worker_main(rr_engine* e) {
             decode_due = false;
             if (ip && !decode_first) {                     // its next piece goes first: min(Tmax, remaining) tokens
                 const int n = std::min(e->Tmax, (int)ip->prompt.size() - ip->n_done);
+                add_score(ip, (int)chunk.size(), ip->n_done, n);
                 chunk.push_back(ip);
                 slots.push_back(ip->rows[0]);
                 pos0.push_back(ip->n_done);
@@ -1241,9 +1382,10 @@ static void worker_main(rr_engine* e) {
             while (!decode_first && !e->waiting.empty()) {
                 Request* r = e->waiting.front();
                 if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all at its admission
+                if (r->gen.scores() && !e->sc_logits) break;   // submitted since the check above: the next round allocates
                 int m = 0, src = -1;
                 const bool ring = ring_request(e, r);       // the ring overwrites its prompt: no prefix hit, nothing kept
-                if (e->o.prefix_cache && ring) {
+                if (e->o.prefix_cache && (ring || r->gen.scores())) {     // scoring: every prompt row goes through lm_head
                     if ((b = pick_slot_miss(e)) < 0) break;
                 } else if (e->o.prefix_cache) {
                     if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
@@ -1287,6 +1429,7 @@ static void worker_main(rr_engine* e) {
                     tail_gen.push_back(&r->gen);
                 }
                 take_pages(e, r);
+                add_score(r, (int)chunk.size(), m, n);
                 chunk.push_back(r);
                 slots.push_back(r->rows[0]);
                 if (last) chunk_mode |= step_mode(r->gen);
@@ -1319,9 +1462,19 @@ static void worker_main(rr_engine* e) {
             if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail);
+                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail, &score);
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
+            for (size_t i = 0, o = 0; rc == RR_OK && i < score_req.size(); o += (size_t)score.rows[i++]) {
+                Request* r = score_req[i];
+                const size_t k = (size_t)r->gen.score_width();
+                for (int j = 0; j < score.rows[i]; ++j) {
+                    const size_t p = (size_t)score_pos[i] + j, src = (o + j) * LP_MAX_TOP;
+                    r->ptgt[p] = e->h_sc_tlp[o + j];
+                    memcpy(&r->plp[p * k], e->h_sc_lp + src, sizeof(float) * k);
+                    memcpy(&r->plp_id[p * k], e->h_sc_id + src, sizeof(int32_t) * k);
+                }
+            }
             int j = 0;                                     // the request's first tail row
             for (size_t i = 0; i < chunk.size(); ++i) {
                 Request* r = chunk[i];
@@ -1620,6 +1773,8 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
     if (e->h_stop) cudaFreeHost(e->h_stop);
     if (e->h_json_done) cudaFreeHost(e->h_json_done);
+    for (void* p : {(void*)e->h_sc_in, (void*)e->h_sc_tlp, (void*)e->h_sc_lp})
+        if (p) cudaFreeHost(p);
     for (const ParamBlocks* p : {&e->h_rows, &e->h_pf})
         for (char* b : p->blk)
             if (b) cudaFreeHost(b);
@@ -1707,8 +1862,9 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
     if (n_choices < 1 || n_choices > e->Bm) return RR_INVALID_ARGUMENT;      // the choices decode side by side
     // the vocabularies the logprobs / sampling kernels handle
-    if ((p.logprobs() || p.sampled()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
+    if ((p.logprobs() || p.sampled() || p.scores()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
         return RR_INVALID_ARGUMENT;
+    if (p.prompt_top < -1 || p.prompt_top > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max) return RR_INVALID_ARGUMENT;
     if ((long long)n_choices * choice_pages(e, n_prompt + max_new_tokens) > e->n_pages) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n_prompt; ++i)
@@ -1730,6 +1886,10 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
     }
     r->tag = tag;
     r->gen = p;
+    if (p.scores()) {
+        const size_t n = (size_t)n_prompt - 1, k = (size_t)p.score_width();
+        r->ptgt.assign(n, 0.f); r->plp.assign(n * k, 0.f); r->plp_id.assign(n * k, 0);
+    }
     std::vector<DoneNote> notes;
     {
         std::lock_guard<std::mutex> lk(e->mu);
@@ -1771,6 +1931,40 @@ RR_API int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_promp
     const int rc = p.set(e->d.vocab, params);
     return rc != RR_OK ? rc : rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p,
                                                        params ? params->n_choices : 1);
+}
+
+RR_API int rr_engine_submit_scored(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                   const rr_gen_params* params, int prompt_top, uint64_t* ticket) {
+    if (!e) return RR_INVALID_ARGUMENT;
+    rr::GenParams p;
+    const int rc = p.set(e->d.vocab, params);
+    if (rc != RR_OK) return rc;
+    p.prompt_top = prompt_top;
+    return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, params ? params->n_choices : 1);
+}
+
+RR_API int rr_engine_prompt_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
+                                     int32_t* id_out) {
+    if (!e) return RR_INVALID_ARGUMENT;
+    std::unique_lock<std::mutex> lk(e->mu);
+    const auto deadline = std::chrono::steady_clock::now() +
+                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
+    for (;;) {
+        auto it = e->table.find(ticket);
+        if (it == e->table.end() || !it->second->gen.scores()) return RR_INVALID_ARGUMENT;
+        const Request* r = it->second;
+        if (r->done) {
+            if (r->status != RR_OK) return r->status;
+            if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
+            if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
+            if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
+            return RR_OK;
+        }
+        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
+            it = e->table.find(ticket);
+            if (it == e->table.end() || !it->second->done) return it == e->table.end() ? RR_INVALID_ARGUMENT : RR_TIMEOUT;
+        }
+    }
 }
 
 // Caller holds e->mu.  The first min(n, max_tokens_out) visible tokens of each choice of r (fewer for a shorter choice)

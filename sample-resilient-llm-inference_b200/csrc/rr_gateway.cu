@@ -53,6 +53,10 @@ struct GwReq {
     rr::GenParams gen;                // handed to every engine the request is admitted to
     std::vector<float> lp;            // tokens' pairs, [gen.lp_width()] each
     std::vector<int32_t> lp_id;
+    // prompt logprobs (gen.scores()) of the engine that served it, read before its record was consumed
+    // (rr_engine_prompt_logprobs): [n_prompt - 1] and [n_prompt - 1][gen.score_width()]
+    std::vector<float> ptgt, plp;
+    std::vector<int32_t> plp_id;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;   // t_eng_submit: hand-off to the replica
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
@@ -181,6 +185,7 @@ static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int 
             r->eng = nullptr;
             r->tokens.clear(); r->n_tok.clear(); r->fin.clear();
             r->lp.clear(); r->lp_id.clear();
+            r->ptgt.clear(); r->plp.clear(); r->plp_id.clear();     // the next replica scores the prompt again
             r->n_cached = 0;
             g->st.failed_over++;
             g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
@@ -196,7 +201,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     rr_engine* eng = nullptr;
     int max_new = 0;
     bool logprobs = false;
-    size_t k = 1, n_ch = 1;
+    size_t k = 1, n_ch = 1, n_score = 0, ks = 1;
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -207,6 +212,16 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         logprobs = r->gen.logprobs();
         k = (size_t)r->gen.lp_width();
         n_ch = (size_t)r->n_choices;
+        if (r->gen.scores()) n_score = r->prompt.size() - 1;
+        ks = (size_t)r->gen.score_width();
+    }
+    // the prompt logprobs first: rr_engine_wait consumes the record
+    std::vector<float> ptgt, plp;
+    std::vector<int32_t> plp_id;
+    int prc = RR_INVALID_ARGUMENT;
+    if (eng && status == RR_OK && n_score > 0) {
+        ptgt.resize(n_score); plp.resize(n_score * ks); plp_id.resize(n_score * ks);
+        prc = rr_engine_prompt_logprobs(eng, eng_ticket, 0.001, ptgt.data(), plp.data(), plp_id.data());
     }
     // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
@@ -223,6 +238,9 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
         if (it == g->table.end()) return;
+        if (prc == RR_OK && wrc == RR_OK) {
+            it->second->ptgt.swap(ptgt); it->second->plp.swap(plp); it->second->plp_id.swap(plp_id);
+        }
         gw_settle(g, it->second, status, n_generated, wrc, comp, toks.data(), n_toks.data(), fins.data(), lps.data(),
                   lp_ids.data());
     }
@@ -494,17 +512,53 @@ RR_API int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prom
 
 // The parameters are checked before the group and the prompt: a request with an unknown group and invalid parameters
 // gets RR_INVALID_ARGUMENT.
-RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
-                             const rr_gen_params* params, uint64_t* ticket) {
+static int gw_submit_one(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                         const rr_gen_params* params, int prompt_top, uint64_t* ticket) {
     if (!g) return RR_INVALID_ARGUMENT;
     rr::GenParams p;
     // the format is checked against the smallest vocabulary: a fallback re-admission may take the request to any replica
     const int rc = p.set(g->min_vocab, params);
     if (rc != RR_OK) return rc;
+    if (prompt_top < -1 || prompt_top > rr::LP_MAX_TOP || (prompt_top >= 0 && g->min_vocab % 4)) return RR_INVALID_ARGUMENT;
+    p.prompt_top = prompt_top;
     // a mock replica has no logits to fill the pairs from or to mask, and no decode loop to cut
-    if ((p.logprobs() || p.stops() || p.json()) && g->has_stub) return RR_INVALID_ARGUMENT;
+    if ((p.logprobs() || p.stops() || p.json() || p.scores()) && g->has_stub) return RR_INVALID_ARGUMENT;
     const int32_t start[2] = {0, n_prompt};
     return gw_submit(g, group, prompt_ids, start, 1, max_new_tokens, 0, p, params ? params->n_choices : 1, ticket);
+}
+
+RR_API int rr_gateway_submit(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                             const rr_gen_params* params, uint64_t* ticket) {
+    return gw_submit_one(g, group, prompt_ids, n_prompt, max_new_tokens, params, -1, ticket);
+}
+
+RR_API int rr_gateway_submit_scored(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
+                                    const rr_gen_params* params, int prompt_top, uint64_t* ticket) {
+    return gw_submit_one(g, group, prompt_ids, n_prompt, max_new_tokens, params, prompt_top, ticket);
+}
+
+RR_API int rr_gateway_prompt_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
+                                      int32_t* id_out) {
+    if (!g) return RR_INVALID_ARGUMENT;
+    std::unique_lock<std::mutex> lk(g->mu);
+    const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
+    for (;;) {
+        auto it = g->table.find(ticket);
+        if (it == g->table.end() || !it->second->gen.scores()) return RR_INVALID_ARGUMENT;
+        const GwReq* r = it->second;
+        if (r->state == FINISHED) {
+            if (r->status != RR_OK) return r->status;
+            if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
+            if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
+            if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
+            return RR_OK;
+        }
+        if (g->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
+            it = g->table.find(ticket);
+            if (it == g->table.end()) return RR_INVALID_ARGUMENT;
+            if (it->second->state != FINISHED) return RR_TIMEOUT;
+        }
+    }
 }
 
 // caller holds g->mu.  The first min(n, max_tokens_out) tokens of each choice (fewer for a shorter choice) into tokens_out

@@ -684,6 +684,21 @@ __device__ __forceinline__ void pf_epilogue(const float (&acc)[128], int row0, i
                     }
                 }
             }
+        } else if constexpr (MODE == OUT_ROWMAJOR_F32) {
+            float* c = reinterpret_cast<float*>(out);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = row0 + 8 * h;
+                if (row >= rowsA) continue;
+                float* dst = c + (size_t)row * ldo;
+#pragma unroll
+                for (int j = 0; j < 32; ++j) {
+                    const int col = cb + 8 * j + cq;
+                    const float v0 = acc[4 * j + 2 * h] * rinv[h], v1 = acc[4 * j + 2 * h + 1] * rinv[h];
+                    if (col + 1 < rowsB) *reinterpret_cast<float2*>(dst + col) = make_float2(v0, v1);
+                    else if (col < rowsB) dst[col] = v0;
+                }
+            }
         } else {
             static_assert(MODE == OUT_ROWMAJOR_BF16, "row-major modes");
             __nv_bfloat16* c = reinterpret_cast<__nv_bfloat16*>(out);
@@ -1110,7 +1125,8 @@ int make_tmap_act_store(CUtensorMap* map, const void* base, int rows, int n, int
 }
 
 static bool rowmajor(int mode) {
-    return mode == OUT_ROWMAJOR_BF16 || mode == OUT_ROWMAJOR_SILU || mode == OUT_ROWMAJOR_ROPE || mode == OUT_ROWMAJOR_RESID;
+    return mode == OUT_ROWMAJOR_BF16 || mode == OUT_ROWMAJOR_SILU || mode == OUT_ROWMAJOR_ROPE || mode == OUT_ROWMAJOR_RESID ||
+           mode == OUT_ROWMAJOR_F32;
 }
 
 static std::atomic<int> g_num_sms[64];
@@ -1172,7 +1188,9 @@ int gemm_plan_init(GemmPlan* p, const void* A, int rowsA, int ldA, const void* B
     if (mode == OUT_ROWMAJOR_ROPE && (splits != 1 || bn < 128 || rowsB % 128 != 0)) return RR_ERR_ARG;
     if (bn > MAX_BN) bn = MAX_BN;
     if (mode == OUT_ROWMAJOR_RESID && (splits != 1 || bn < 32 || ldo % 4 != 0)) return RR_ERR_ARG;
-    if (mode < 0 || mode > OUT_ROWMAJOR_RESID) return RR_ERR_ARG;
+    // fp32 pairs are stored 8-byte aligned
+    if (mode == OUT_ROWMAJOR_F32 && (splits != 1 || ldo % 2 != 0 || ((uintptr_t)out & 7) != 0)) return RR_ERR_ARG;
+    if (mode < 0 || mode > OUT_ROWMAJOR_F32) return RR_ERR_ARG;
     memset(&p->rope, 0, sizeof(p->rope));
     p->rowsA = rowsA; p->rowsB = rowsB; p->K = K; p->out = out; p->ldo = ldo; p->ld_rows = ld_rows;
     p->splits = splits; p->mode = mode; p->bn = bn; p->max_ctas = 0; p->scaleA = nullptr;
@@ -1207,6 +1225,7 @@ int gemm_launch(const GemmPlan& p, cudaStream_t st, bool pdl) {
         case OUT_ROWMAJOR_SILU: return launch_pf<OUT_ROWMAJOR_SILU>(p, st, pdl);
         case OUT_ROWMAJOR_ROPE: return launch_pf<OUT_ROWMAJOR_ROPE>(p, st, pdl);
         case OUT_ROWMAJOR_RESID: return launch_pf<OUT_ROWMAJOR_RESID>(p, st, pdl);
+        case OUT_ROWMAJOR_F32: return launch_pf<OUT_ROWMAJOR_F32>(p, st, pdl);
     }
 #define RR_CASE(BN_)                                                                                            \
     case BN_:                                                                                                   \

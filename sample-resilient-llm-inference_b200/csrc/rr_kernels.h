@@ -34,7 +34,9 @@ __host__ __device__ __forceinline__ long long kv_row(const int32_t* table, int p
 }
 
 enum GemmOutMode { OUT_ROWMAJOR_BF16 = 0, OUT_TRANSPOSED_F32 = 1, OUT_TRANSPOSED_SILU = 2, OUT_ROWMAJOR_SILU = 3,
-                   OUT_ROWMAJOR_ROPE = 4, OUT_ROWMAJOR_RESID = 5 };
+                   OUT_ROWMAJOR_ROPE = 4, OUT_ROWMAJOR_RESID = 5, OUT_ROWMAJOR_F32 = 6 };
+// OUT_ROWMAJOR_F32 (lm_head over the prompt rows of a scoring prefill chunk): out[a*ldo + b] = acc * rinv(a) as fp32, the
+// deferred-norm consumer factor included.  fp32 because a logprob needs more than bf16's 8 bits near a logit of 20.
 // OUT_ROWMAJOR_RESID (prefill O / down projections): out is the fp32 residual stream, out[a*ldo + b] += acc —
 // the following norm kernel then only reads x and writes xn (half its bytes).
 
@@ -121,6 +123,11 @@ struct GenParams {
     bool json() const { return fmt == 1; }
     // pairs per token of a logprobs request: max(1, top_lp), plus the sampled token's own pair in the last column
     int lp_width() const { return (top_lp > 1 ? top_lp : 1) + (sampled() ? 1 : 0); }
+    // prompt logprobs (rr_engine_submit_scored): -1 off, else every prompt token t >= 1 gets its own logprob given the
+    // tokens before it and max(1, prompt_top) (logprob, id) pairs.  Not part of rr_gen_params: set() leaves it at -1.
+    int prompt_top = -1;
+    bool scores() const { return prompt_top >= 0; }
+    int score_width() const { return prompt_top > 1 ? prompt_top : 1; }
     // The raw C struct (NULL: the defaults), checked before anything is stored: -1 <= top_logprobs <= LP_MAX_TOP and
     // OpenAI's ranges 0 <= temperature <= 2, 0 <= top_p <= 1, -2 <= penalties <= 2, 0 <= n_bias <= PEN_MAX_BIAS (non-null
     // arrays when n_bias > 0), bias ids unique and in [0, vocab), -100 <= bias values <= 100; NaN fails; 0 <= n_stop <=

@@ -132,6 +132,7 @@ class Engine:
         torch.cuda.synchronize(device)   # weights were produced on torch's stream
         self._lp_k: Dict[int, int] = {}     # ticket -> pairs per token of a request submitted with top_logprobs
         self._n: Dict[int, int] = {}        # ticket -> choices of a request submitted with n > 1
+        self._score: Dict[int, Tuple[int, int]] = {}    # ticket -> (prompt length, pairs per position) of a scoring request
         self._h = C.c_void_p()
         _lib.check(_lib.lib.rr_engine_create(C.byref(desc), C.byref(mw), C.byref(opts),
                                              C.byref(self._h)), "rr_engine_create")
@@ -190,7 +191,8 @@ class Engine:
     def submit(self, prompt_ids: Sequence[int], max_new_tokens: int, top_logprobs: Optional[int] = None,
                temperature: Optional[float] = None, top_p: Optional[float] = None, seed: Optional[int] = None,
                frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
-               logit_bias: Optional[Dict[int, float]] = None, n: int = 1, stop=None, response_format=None) -> int:
+               logit_bias: Optional[Dict[int, float]] = None, n: int = 1, stop=None, response_format=None,
+               prompt_logprobs: Optional[int] = None) -> int:
         """top_logprobs = k in 0..20: also record the max(1, k) most likely tokens and their logprobs at every step
         (the generated tokens do not change).  temperature in (0, 2]: draw every token from the top_p (default 1)
         nucleus of softmax(logits / temperature) with `seed` (taken modulo 2^64; a random one when None), see
@@ -204,15 +206,22 @@ class Engine:
         tokens are a prefix of the same request's without `stop`.
         response_format {"type": "json_object"}: JSON mode: every token is picked from the logits masked to the JSON
         grammar, and a choice ends with finish reason "stop" on the token that closes its top-level object.  None and
-        {"type": "text"} change nothing (check_response_format)."""
+        {"type": "text"} change nothing (check_response_format).
+        prompt_logprobs = k in 0..20: also score the prompt (rr_engine_submit_scored); read the scores with
+        prompt_logprobs() before wait()."""
         ids = _i32(prompt_ids)
         bias = logit_bias or {}
         stops = stop if isinstance(stop, (list, tuple)) and all(isinstance(b, bytes) for b in stop) else check_stop(stop)
         gen = gen_args(top_logprobs, temperature, top_p, seed, frequency_penalty, presence_penalty, list(bias.keys()),
                        list(bias.values()), stop=stops, json_object=check_response_format(response_format), n=n)
         t = C.c_uint64()
-        _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(gen.params), C.byref(t)),
-                   "rr_engine_submit")
+        if prompt_logprobs is None:
+            _lib.check(_lib.lib.rr_engine_submit(self._h, _p(ids), len(ids), max_new_tokens, C.byref(gen.params),
+                                                 C.byref(t)), "rr_engine_submit")
+        else:
+            _lib.check(_lib.lib.rr_engine_submit_scored(self._h, _p(ids), len(ids), max_new_tokens, C.byref(gen.params),
+                                                        int(prompt_logprobs), C.byref(t)), "rr_engine_submit_scored")
+            self._score[t.value] = (len(ids), max(1, int(prompt_logprobs)))
         if n > 1:
             self._n[t.value] = n
         if gen.width:
@@ -226,6 +235,18 @@ class Engine:
         lp, ids = np.zeros((n, max_tokens, k), dtype=np.float32), np.zeros((n, max_tokens, k), dtype=np.int32)
         return lp, ids, lp.ctypes.data_as(C.POINTER(C.c_float)), _p(ids)
 
+    def prompt_logprobs(self, ticket: int, timeout: float = 0.0):
+        """The scores of a request submitted with prompt_logprobs=k, once it is done (the ticket stays for wait()):
+        (target [n_prompt - 1] float32, logprobs [n_prompt - 1][max(1, k)] float32, ids int32 alike); row t - 1 is prompt
+        position t.  Raises RRError when the request did not end RR_OK."""
+        n, k = self._score[ticket]
+        tgt = np.zeros(max(0, n - 1), dtype=np.float32)
+        lp, ids = np.zeros((max(0, n - 1), k), dtype=np.float32), np.zeros((max(0, n - 1), k), dtype=np.int32)
+        f32 = C.POINTER(C.c_float)
+        _lib.check(_lib.lib.rr_engine_prompt_logprobs(self._h, ticket, float(timeout), tgt.ctypes.data_as(f32),
+                                                      lp.ctypes.data_as(f32), _p(ids)), "rr_engine_prompt_logprobs")
+        return tgt, lp, ids
+
     def wait(self, ticket: int, timeout: float = 0.0, max_tokens: int = 4096) -> CompletionRecord:
         c = _lib.Completion()
         nc = self._n.get(ticket, 1)
@@ -237,6 +258,7 @@ class Engine:
         if rc != 6:
             self._lp_k.pop(ticket, None)
             self._n.pop(ticket, None)
+            self._score.pop(ticket, None)
         if rc not in (0, 6, 7):
             _lib.check(rc, "rr_engine_wait")
         ns = [min(k, max_tokens) for k in n_tok]

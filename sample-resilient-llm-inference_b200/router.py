@@ -16,6 +16,7 @@ responses.  There is no Python/CPU implementation of the routing logic or the re
 """
 from __future__ import annotations
 
+import codecs
 import ctypes as C
 import math
 import re
@@ -355,6 +356,136 @@ def logprob_pairs(lp: np.ndarray, ids: np.ndarray, a: int, b: int) -> List[List[
     return [[(int(i), float(v)) for i, v in zip(ids[t], lp[t])] for t in range(a, b)]
 
 
+MAX_COMPLETION_LOGPROBS = 5  # OpenAI's limit for `logprobs` on /v1/completions
+
+
+def check_text_completion(prompt: Any, max_tokens: Any = None, echo: Any = None, logprobs: Any = None,
+                          stream: Any = None, best_of: Any = None, suffix: Any = None):
+    """OpenAI's rules for the fields of a /v1/completions request -> (prompts, logprobs).  `prompt` takes OpenAI's four
+    forms: a string, an array of strings, an array of token ids or an array of arrays of ids; each element of `prompts` is a
+    string or a list of ids (their range is the caller's to check against the vocabulary).  logprobs: None (off) or 0..5.
+    Raises BadRequestError (HTTP 400) naming the field for anything else, and for what this server does not serve: `echo`
+    with `stream`, `best_of` other than 1, `suffix`, and `max_tokens` 0 (a prefill-only request)."""
+    def is_id(v):
+        return isinstance(v, int) and not isinstance(v, bool)
+    if isinstance(prompt, str):
+        prompts: List[Any] = [prompt]
+    elif isinstance(prompt, list) and prompt and all(isinstance(p, str) for p in prompt):
+        prompts = list(prompt)
+    elif isinstance(prompt, list) and prompt and all(is_id(t) for t in prompt):
+        prompts = [list(prompt)]
+    elif isinstance(prompt, list) and prompt and all(isinstance(p, list) and p and all(is_id(t) for t in p) for p in prompt):
+        prompts = [list(p) for p in prompt]
+    else:
+        raise BadRequestError("`prompt` must be a string, an array of strings, an array of token ids or an array of "
+                              "arrays of token ids, none of them empty")
+    if max_tokens is not None and (not isinstance(max_tokens, int) or isinstance(max_tokens, bool) or max_tokens < 1):
+        raise BadRequestError("`max_tokens` must be an integer of at least 1: prefill-only requests are not served")
+    if echo is not None and not isinstance(echo, bool):
+        raise BadRequestError("`echo` must be a boolean")
+    if stream is not None and not isinstance(stream, bool):
+        raise BadRequestError("`stream` must be a boolean")
+    if echo and stream:
+        raise BadRequestError("`echo` is not available with `stream`: send the request without `stream`")
+    if best_of is not None and (isinstance(best_of, bool) or best_of != 1):
+        raise BadRequestError("`best_of` other than 1 is not supported: use `n`")
+    if suffix is not None:
+        raise BadRequestError("`suffix` is not supported")
+    if logprobs is not None and (isinstance(logprobs, bool) or not isinstance(logprobs, int)
+                                 or not 0 <= logprobs <= MAX_COMPLETION_LOGPROBS):
+        raise BadRequestError(f"`logprobs` must be an integer from 0 to {MAX_COMPLETION_LOGPROBS}")
+    return prompts, logprobs
+
+
+_invalid_spans = threading.local()
+
+
+def _note_invalid(exc: UnicodeDecodeError):
+    _invalid_spans.v.append((exc.start, exc.end))
+    return "\ufffd", exc.end
+
+
+codecs.register_error("rr_b200_note_invalid", _note_invalid)
+
+
+def text_offsets(tokens: Sequence[int]) -> Tuple[str, List[int]]:
+    """(detokenize(tokens), each token's `text_offset`): the character offset in that text where the token's first byte
+    starts.  A continuation byte of a multi-byte character gets its character's offset, and every byte of an invalid
+    sequence the offset of the U+FFFD that replaces it; a token without a byte (id < 3) gets the offset of the text after
+    the tokens before it."""
+    raw = bytes(((int(t) - 3) % 256) for t in tokens if int(t) >= 3)
+    _invalid_spans.v = []
+    text = raw.decode("utf-8", errors="rr_b200_note_invalid")
+    spans = dict(_invalid_spans.v)
+    char_of = [0] * (len(raw) + 1)
+    i = c = 0
+    while i < len(raw):
+        b = raw[i]
+        end = spans.get(i, i + (1 if b < 0x80 else 2 if b < 0xE0 else 3 if b < 0xF0 else 4))
+        for j in range(i, end):
+            char_of[j] = c
+        i, c = end, c + 1
+    char_of[len(raw)] = c
+    offs, pos = [], 0
+    for t in tokens:
+        offs.append(char_of[pos])
+        pos += 1 if int(t) >= 3 else 0
+    return text, offs
+
+
+def top_logprobs_dict(tok: int, tok_lp: float, alts: Sequence[Tuple[int, float]]) -> dict:
+    """One entry of /v1/completions `logprobs.top_logprobs`: token string -> logprob over the alternatives and the token
+    itself (up to k + 1 entries).  The byte tokenizer maps many ids to one string (every id >= 259 folds onto a byte, and
+    a lone byte of a multi-byte character is U+FFFD), so a string holds the largest logprob among the listed ids that have
+    it.  -inf (a token JSON mode masked out) is left out: JSON cannot encode it."""
+    out: Dict[str, float] = {}
+    for i, v in list(alts) + [(tok, tok_lp)]:
+        s = detokenize([i])
+        if v != -math.inf and (s not in out or v > out[s]):
+            out[s] = float(v)
+    return out
+
+
+def completion_logprobs(tokens: Sequence[int], token_lps: Sequence[Optional[float]],
+                        alts: Sequence[Optional[Sequence[Tuple[int, float]]]]) -> dict:
+    """`choices[i].logprobs` of /v1/completions over `tokens` (with `echo` the prompt's, then the generated ones):
+    token_lps[t] = the token's logprob and alts[t] its k alternatives as (id, logprob), both None for the first prompt
+    token, which has no context."""
+    _, offs = text_offsets(tokens)
+    return {"tokens": [detokenize([t]) for t in tokens],
+            "token_logprobs": [None if v is None else float(v) for v in token_lps],
+            "top_logprobs": [None if a is None else top_logprobs_dict(t, v, a) for t, v, a in zip(tokens, token_lps, alts)],
+            "text_offset": offs}
+
+
+@dataclass
+class TextChoice:
+    index: int
+    text: str
+    finish_reason: str = "length"
+    logprobs: Optional[dict] = None      # {tokens, token_logprobs, top_logprobs, text_offset}; only when requested
+
+
+@dataclass
+class TextCompletionResponse:
+    """A /v1/completions response (OpenAI `Completion`)."""
+    id: str
+    model: str
+    choices: List[TextChoice]
+    usage: Usage
+    created: int = 0
+    object: str = "text_completion"
+
+    def model_dump(self) -> dict:
+        u = {"prompt_tokens": self.usage.prompt_tokens, "completion_tokens": self.usage.completion_tokens,
+             "total_tokens": self.usage.total_tokens}
+        if self.usage.prompt_tokens_details is not None:
+            u["prompt_tokens_details"] = self.usage.prompt_tokens_details
+        return {"id": self.id, "object": self.object, "created": self.created, "model": self.model,
+                "choices": [{"index": c.index, "text": c.text, "logprobs": c.logprobs, "finish_reason": c.finish_reason}
+                            for c in self.choices], "usage": u}
+
+
 def messages_to_text(messages: Sequence[dict]) -> str:
     return "\n".join(f"{m.get('role', 'user')}: {m.get('content', '')}" for m in messages)
 
@@ -557,13 +688,19 @@ class Router:
             return APIError(f"backend failure on deployment {dep} and no fallback available for model={model}")
         return APIError(f"{_lib.lib.rr_strerror(status).decode()} (model={model})")
 
-    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs) -> int:
+    def _gw_submit(self, gw, g: int, prompt_ids, max_new: int, model: str, gen: GenArgs,
+                   prompt_top: Optional[int] = None) -> int:
+        """prompt_top: also score the prompt (rr_gateway_submit_scored) with that many pairs per position."""
         ids = np.ascontiguousarray(np.asarray(prompt_ids, dtype=np.int32))
         if self._custom_clock:
             _lib.lib.rr_gateway_set_now(gw, self.now_ms())
         t = C.c_uint64()
-        rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
-                                        C.byref(gen.params), C.byref(t))
+        if prompt_top is None:
+            rc = _lib.lib.rr_gateway_submit(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                            C.byref(gen.params), C.byref(t))
+        else:
+            rc = _lib.lib.rr_gateway_submit_scored(gw, g, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(ids), max_new,
+                                                   C.byref(gen.params), int(prompt_top), C.byref(t))
         if rc == 4:
             raise self._invalid(len(ids), max_new, gen.params.n_choices)
         if rc != 0:
@@ -824,6 +961,143 @@ class Router:
             raise BadRequestError(f"Invalid model name passed in model={model}")
         return self._batch_gw(self._gateway(), model, g, prompts, max_tokens, timeout)
 
+    def _completion_prompts(self, prompt) -> List[List[int]]:
+        """Token ids of check_text_completion's prompts: a string is BOS plus its bytes (no role framing), ids are used as
+        they are and must lie in [0, vocab)."""
+        vocab = self._vocab()
+        out = []
+        for p in prompt:
+            if isinstance(p, str):
+                out.append([int(t) for t in tokenize(p, vocab)])
+            elif any(not 0 <= t < vocab for t in p):
+                raise BadRequestError(f"`prompt` holds a token id outside the vocabulary [0, {vocab})")
+            else:
+                out.append(list(p))
+        return out
+
+    def text_completion(self, model: str, prompt: Any, max_tokens: Optional[int] = None, echo: bool = False,
+                        logprobs: Optional[int] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
+                        seed: Optional[int] = None, n: Optional[int] = None, stop: Any = None,
+                        frequency_penalty: Optional[float] = None, presence_penalty: Optional[float] = None,
+                        logit_bias: Optional[Dict[str, float]] = None, timeout: Optional[float] = None,
+                        best_of: Optional[int] = None, suffix: Any = None, **_ignored) -> TextCompletionResponse:
+        """OpenAI's /v1/completions (`client.completions.create`).  prompt: a string, an array of strings, an array of token
+        ids or an array of arrays of ids; each prompt is its own request, all submitted together, and choice i * n + c is
+        choice c of prompt i.  usage sums over the prompts.
+        logprobs = k in 0..5: every generated token's logprob and its k most likely alternatives (the top_logprobs
+        machinery of completion()).  echo: `text` starts with the prompt's text, and with logprobs the prompt is scored
+        on the GPU (rr_gateway_submit_scored): `logprobs` then covers the prompt's tokens, then the generated ones.  The
+        first prompt token has no context: its token_logprobs and top_logprobs entries are None.  top_logprobs[t] maps
+        token strings to logprobs over the k alternatives and the token itself (up to k + 1 entries).  The byte
+        tokenizer maps many ids to one string, so a string holds the largest logprob among the listed ids that have it.
+        text_offset[t] is the character offset in `text` where token t's first byte starts (a continuation byte of a
+        multi-byte character gets its character's offset).  A scoring request takes no prefix-cache hit:
+        cached_tokens is 0.
+        Refused with BadRequestError (check_text_completion): `echo` with streaming, `best_of` other than 1, `suffix`,
+        `max_tokens` 0, and `logprobs` on mock replicas.  Sampling, penalties, logit_bias, stop and n as in completion()."""
+        prompts, lp = check_text_completion(prompt, max_tokens, echo, logprobs, None, best_of, suffix)
+        n = check_n(n)
+        gen = self._params(True if lp is not None else None, lp, temperature, top_p, seed, frequency_penalty,
+                           presence_penalty, logit_bias, stop, None, n)
+        g = self.cfg.group_index(model)
+        if g < 0:
+            raise BadRequestError(f"Invalid model name passed in model={model}")
+        ids = self._completion_prompts(prompts)
+        max_new = max_tokens or self.default_max_tokens
+        if n > self._limits()[1]:
+            raise self._invalid(n=n)
+        gw = self._gateway()
+        t_start = time.perf_counter()
+        score = lp if echo and lp is not None else None
+        tickets: List[int] = []
+        try:
+            for p in ids:
+                tickets.append(self._gw_submit(gw, g, p, max_new, model, gen, prompt_top=score))
+        except APIError:
+            for t in tickets:
+                _lib.lib.rr_gateway_cancel(gw, t, 0)
+            raise
+        choices, usage, label, cached, dep = [], [0, 0], "", 0, 0
+        for i, (p, ticket) in enumerate(zip(ids, tickets)):
+            try:
+                label, plp, waited = self._collect_prompt(gw, model, p, ticket, max_new, timeout, gen, score)
+            except APIError:
+                for t in tickets[i + 1:]:
+                    _lib.lib.rr_gateway_cancel(gw, t, 0)
+                raise
+            res, toks, pairs, n_tok, fin = waited
+            usage[0] += len(p)
+            cached, dep = cached + res.n_cached, res.deployment
+            for c in range(n):
+                gen_toks = toks[c][: n_tok[c]].tolist()
+                shown = (list(p) if echo else []) + gen_toks
+                text = detokenize(shown)
+                lpd = None
+                if lp is not None:
+                    gp = logprob_pairs(pairs[c][0], pairs[c][1], 0, n_tok[c])
+                    g_lps = [next((v for j, v in q if j == t), q[0][1]) for t, q in zip(gen_toks, gp)]
+                    g_alts = [q[:lp] for q in gp]
+                    if echo:
+                        p_lps, p_alts = plp if plp is not None else ([None] * len(p), [None] * len(p))
+                        lpd = completion_logprobs(shown, list(p_lps) + g_lps, list(p_alts) + g_alts)
+                    else:
+                        lpd = completion_logprobs(shown, g_lps, g_alts)
+                choices.append(TextChoice(i * n + c, text, FINISH_REASONS[fin[c]], lpd))
+                usage[1] += len(gen_toks)
+        return TextCompletionResponse("cmpl-" + uuid.uuid4().hex[:24], label, choices, self._usage(dep, *usage, cached),
+                                      int(time.time()))
+
+    def _collect_prompt(self, gw, model, p, ticket, max_new, timeout, gen: GenArgs, score: Optional[int]):
+        """One prompt of text_completion: its prompt logprobs when score is set (read before the wait consumes the ticket)
+        as ([None] + target logprobs, [None] + per position its `score` best (id, logprob) pairs), then its choices
+        (_wait_choices).  -> (model label, prompt logprobs or None, _wait_choices' result)."""
+        plp = None
+        if score is not None:
+            m, k = len(p) - 1, max(1, score)
+            tgt, alt, alt_id = np.zeros(m, np.float32), np.zeros((m, k), np.float32), np.zeros((m, k), np.int32)
+            rc = _lib.lib.rr_gateway_prompt_logprobs(gw, ticket, float(timeout or 0.0),
+                                                     tgt.ctypes.data_as(C.POINTER(C.c_float)),
+                                                     alt.ctypes.data_as(C.POINTER(C.c_float)),
+                                                     alt_id.ctypes.data_as(C.POINTER(C.c_int32)))
+            if rc == 0:
+                plp = ([None] + tgt.tolist(), [None] + [list(zip(r_id.tolist(), r.tolist()))[:score]
+                                                        for r, r_id in zip(alt, alt_id)])
+        waited = self._wait_choices(gw, model, ticket, max_new, timeout, gen)
+        return self.cfg.deployments[waited[0].deployment].response_model, plp, waited
+
+    def _wait_choices(self, gw, model, ticket, max_new, timeout, gen: GenArgs):
+        """rr_gateway_wait for a request of gen.params.n_choices choices -> (result, tokens [n][max_new], per choice
+        (logprobs [max_new][width], ids) or None, tokens per choice, finish codes).  Raises the request's APIError."""
+        n = gen.params.n_choices
+        res = _lib.GatewayResult()
+        toks = np.zeros((n, max_new), dtype=np.int32)
+        lp, ids, lp_p, ids_p = self._lp_bufs(gen, max_new, n)
+        if lp is not None:
+            lp, ids = lp.reshape(n, max_new, gen.width), ids.reshape(n, max_new, gen.width)
+        n_tok, fin = (C.c_int32 * n)(), (C.c_int32 * n)()
+        rc = _lib.lib.rr_gateway_wait(gw, ticket, float(timeout or 0.0), C.byref(res),
+                                      toks.ctypes.data_as(C.POINTER(C.c_int32)), max_new, lp_p, ids_p, n_tok, fin)
+        if rc == 6:
+            _lib.lib.rr_gateway_cancel(gw, ticket, 1)
+        if rc != 0:
+            raise self._gw_error(rc, model, res, timeout)
+        pairs = [(lp[c], ids[c]) for c in range(n)] if lp is not None else None
+        return res, toks, pairs, [min(k, max_new) for k in n_tok], list(fin)
+
+    def text_completion_stream(self, model: str, prompt: Any, max_tokens: Optional[int] = None,
+                               logprobs: Optional[int] = None, timeout: Optional[float] = None, **kw):
+        """/v1/completions with `stream` (no `echo`): one prompt, served by completion_stream on its token ids; yields what
+        completion_stream yields (with logprobs, the chat-shaped content entries of the new tokens)."""
+        prompts, lp = check_text_completion(prompt, max_tokens, None, logprobs, True, kw.pop("best_of", None),
+                                            kw.pop("suffix", None))
+        if len(prompts) != 1:
+            raise BadRequestError("streaming takes one `prompt`: send several prompts without `stream`")
+        if self.cfg.group_index(model) < 0:
+            raise BadRequestError(f"Invalid model name passed in model={model}")
+        ids = self._completion_prompts(prompts)[0]
+        yield from self.completion_stream(model, timeout=timeout, max_tokens=max_tokens, prompt_ids=ids,
+                                          logprobs=True if lp is not None else None, top_logprobs=lp, **kw)
+
 
 # ---------------------------------------------------------------- OpenAI-SDK-shaped facade
 class _Completions:
@@ -840,6 +1114,14 @@ class _Chat:
         self.completions = _Completions(router)
 
 
+class _TextCompletions:
+    def __init__(self, router: Router):
+        self._r = router
+
+    def create(self, model: str, prompt: Any, **kw) -> TextCompletionResponse:
+        return self._r.text_completion(model=model, prompt=prompt, **kw)
+
+
 class OpenAI:
     """In-process stand-in for `openai.OpenAI(api_key=..., base_url=http://0.0.0.0:<port>)`
     (reference src/demo_load_balancing.py:24): same `client.chat.completions.create(...)` call."""
@@ -848,3 +1130,4 @@ class OpenAI:
         self.api_key = api_key
         self.base_url = base_url
         self.chat = _Chat(router)
+        self.completions = _TextCompletions(router)

@@ -17,7 +17,7 @@ from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
                      StubBackend, check_logprobs, check_n, check_penalties, check_response_format, check_sampling,
-                     check_stop)
+                     check_stop, check_text_completion)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -129,6 +129,93 @@ def create_app(router: Router):
     # the SDK appends /chat/completions to base_url; both spellings are served
     app.add_api_route("/chat/completions", chat_completions, methods=["POST"])
     app.add_api_route("/v1/chat/completions", chat_completions, methods=["POST"])
+
+    def _error(e: APIError):
+        if isinstance(e, RateLimitError):
+            return JSONResponse(_error_body(e, "rate_limit_error"), 429, headers={"retry-after": "1"})
+        if isinstance(e, BadRequestError):
+            return JSONResponse(_error_body(e, "invalid_request_error"), 400)
+        if isinstance(e, APITimeoutError):
+            return JSONResponse(_error_body(e, "timeout"), 408)
+        return JSONResponse(_error_body(e, "api_error"), e.status_code)
+
+    async def stream_text_completion(kw):
+        """Server-sent events in the OpenAI `text_completion` chunk format (no `echo`: check_text_completion)."""
+        import json as _json
+        import uuid
+        from fastapi.responses import StreamingResponse
+        from .router import detokenize, text_offsets
+        gen = router.text_completion_stream(**kw)
+        try:
+            first = await run_in_threadpool(next, gen)            # admission errors surface before the 200
+        except APIError as e:
+            return _error(e)
+        cid = "cmpl-" + uuid.uuid4().hex[:24]
+
+        def chunk(item):
+            label, toks, done = item[:3]
+            lp = None
+            if kw.get("logprobs") is not None and not done:
+                # the chunk's tokens from completion_stream's entries; text_offset counts from the chunk's text
+                ents, top = item[4], []
+                for e in ents:
+                    d = {}
+                    for t in e["top_logprobs"] + [e]:
+                        if t["token"] not in d or t["logprob"] > d[t["token"]]:
+                            d[t["token"]] = t["logprob"]
+                    top.append(d)
+                lp = {"tokens": [e["token"] for e in ents], "token_logprobs": [e["logprob"] for e in ents],
+                      "top_logprobs": top, "text_offset": text_offsets(toks)[1]}
+            choice = {"index": 0, "text": "" if done else detokenize(toks), "logprobs": lp,
+                      "finish_reason": (getattr(item, "finish_reason", None) or "length") if done else None}
+            return "data: " + _json.dumps({"id": cid, "object": "text_completion", "created": int(time.time()),
+                                           "model": label, "choices": [choice]}) + "\n\n"
+
+        def events():
+            try:
+                yield chunk(first)
+                if not first[2]:
+                    for item in gen:
+                        yield chunk(item)
+                yield "data: [DONE]\n\n"
+            finally:
+                gen.close()
+
+        return StreamingResponse(events(), media_type="text/event-stream")
+
+    async def text_completions(request: Request):
+        """OpenAI's /v1/completions (Router.text_completion): `prompt` in any of its four forms, `echo` and `logprobs`
+        0..5 (with `echo`, the prompt's tokens scored on the GPU)."""
+        try:
+            body = await request.json()
+        except Exception:
+            return JSONResponse(_error_body(BadRequestError("invalid JSON body"), "invalid_request_error"), 400)
+        model = body.get("model") if isinstance(body, dict) else None
+        if not isinstance(model, str) or "prompt" not in body:
+            return JSONResponse(_error_body(BadRequestError("`model` and `prompt` are required"),
+                                            "invalid_request_error"), 400)
+        try:
+            check_text_completion(body["prompt"], body.get("max_tokens"), body.get("echo"), body.get("logprobs"),
+                                  body.get("stream"), body.get("best_of"), body.get("suffix"))
+            if body.get("stream") and check_n(body.get("n")) > 1:
+                raise BadRequestError("streaming is not available with `n` > 1: send the request without `stream`")
+        except BadRequestError as e:
+            return _error(e)
+        # passed on only when present: absent fields take the router's defaults
+        kw = {k: body[k] for k in ("max_tokens", "logprobs", "temperature", "top_p", "seed", "n", "stop",
+                                   "frequency_penalty", "presence_penalty", "logit_bias", "timeout")
+              if body.get(k) is not None}
+        if body.get("stream"):
+            return await stream_text_completion(dict(kw, model=model, prompt=body["prompt"]))
+        try:
+            resp = await run_in_threadpool(router.text_completion, model=model, prompt=body["prompt"],
+                                           echo=bool(body.get("echo")), **kw)
+            return JSONResponse(resp.model_dump())
+        except APIError as e:
+            return _error(e)
+
+    app.add_api_route("/completions", text_completions, methods=["POST"])
+    app.add_api_route("/v1/completions", text_completions, methods=["POST"])
 
     @app.get("/health")
     async def health():
