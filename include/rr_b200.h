@@ -216,6 +216,22 @@ int rr_op_dequantize_fp8_weight(const void* q, const float* scale, int rows, int
  * D = bf16(A * scale), so the same output bits.  RR_INVALID_ARGUMENT for a row-major mode or a null scale. */
 int rr_gemm_fp8w(const void* A, const float* scale, int rowsA, int ldA, const void* B, int rowsB, int ldB, int K,
                  void* out, int ldo, int ld_rows, int splits, int mode, int bn, void* stream);
+/* One decode projection (QKV, O, gate/up, down or lm_head) exactly as the engine plans and launches it for a decode working
+ * set of `rows` rows (its max_batch): xn bf16 [rows, K], tile width 16 / 32 / 64 / 128 (the narrowest that holds rows;
+ * 129..256 rows run two 128-row batch tiles per weight tile), plane pitch rows, the engine's split-K rule for (rows_w, K)
+ * on this device (lm_head = 1: one plane, as the engine's lm_head), TMA-store epilogue where the engine uses one
+ * (RR_NO_TMA_EPI is read per call).  *n_splits gets the planes used.
+ *   RR_OUT_TRANSPOSED_F32:  w [rows_w, K]; out fp32 [n_splits][rows][rows_w]; plane z = sum over the k-blocks
+ *                           [kb*z/n, kb*(z+1)/n) of xn[b,k] * w[n,k], kb = ceil(K / 64), n = n_splits
+ *   RR_OUT_TRANSPOSED_SILU: w = gate/up rows interleaved in 64-row blocks [2*inter, K], rows_w = 2*inter; out bf16 act
+ *                           [rows][inter] = SiLU(gate) * up; refused where the engine does not fuse it (rows <= 16, or
+ *                           the split rule gives gate/up more than one plane)
+ *   w_scale non-NULL: w is e4m3 with row scales (FP8 weights, rr_op_quantize_fp8_weight): bit for bit the bf16 call on
+ *   the dequantized weight.  Not with lm_head.
+ * RR_INVALID_ARGUMENT, *n_splits unchanged, for a null pointer, rows outside 1..256, another mode and whatever
+ * rr_gemm_bf16 / rr_gemm_fp8w reject; all of these but the SiLU plane count before touching the device. */
+int rr_op_decode_proj(const void* w, const float* w_scale, int rows_w, int K, const void* xn, int rows, void* out,
+                      int mode, int lm_head, int* n_splits, void* stream);
 
 int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows, int hidden,
                 const int32_t* row_active, void* stream);

@@ -165,6 +165,7 @@ PROTOTYPES = {
                                C.c_int, C.c_int, C.c_int, C.c_int, vp]),
     "rr_gemm_fp8w": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, vp, C.c_int,
                                C.c_int, C.c_int, C.c_int, C.c_int, vp]),
+    "rr_op_decode_proj": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, C.c_int, C.c_int, c_i32p, vp]),
     "rr_op_quantize_fp8_weight": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
     "rr_op_dequantize_fp8_weight": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
     "rr_op_embed": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),

@@ -150,6 +150,29 @@ RR_API int rr_gemm_fp8w(const void* A, const float* scale, int rowsA, int ldA, c
     return rc;
 }
 
+// One decode projection as rr_engine_create plans it for max_batch = rows (decode_plan_init) and the decode step launches it.
+RR_API int rr_op_decode_proj(const void* w, const float* w_scale, int rows_w, int K, const void* xn, int rows, void* out,
+                             int mode, int lm_head, int* n_splits, void* stream) {
+    if (!w || !xn || !out || !n_splits) return RR_INVALID_ARGUMENT;
+    if (rows < 1 || rows > MAX_BATCH || rows_w < 1 || K < 8 || K % 8) return RR_INVALID_ARGUMENT;
+    if (mode != OUT_TRANSPOSED_F32 && mode != OUT_TRANSPOSED_SILU) return RR_INVALID_ARGUMENT;
+    if (lm_head && (mode != OUT_TRANSPOSED_F32 || w_scale)) return RR_INVALID_ARGUMENT;
+    if (w_scale && !fp8_weight_ok(w, K)) return RR_INVALID_ARGUMENT;
+    // the engine fuses SiLU * up into the gate/up epilogue only on batch tiles of 32 rows or more and whole 128-row
+    // gate/up tiles (rr_engine_create: fuse_silu) ...
+    if (mode == OUT_TRANSPOSED_SILU && (pick_bn(rows) < 32 || rows_w % 128)) return RR_INVALID_ARGUMENT;
+    const int splits = lm_head ? 1 : pick_splits(rows_w, K);
+    if (mode == OUT_TRANSPOSED_SILU && splits != 1) return RR_INVALID_ARGUMENT;      // ... and one gate/up plane
+    GemmPlan p;
+    int rc = decode_plan_init(&p, w, w_scale, rows_w, K, xn, rows, out, mode == OUT_TRANSPOSED_SILU ? rows_w / 2 : rows_w,
+                              splits, mode);
+    if (rc != RR_OK) return rc;
+    rc = gemm_launch(p, (cudaStream_t)stream);
+    if (rc != RR_OK) { note_cuda_error(cudaPeekAtLastError()); return rc; }
+    *n_splits = p.splits;
+    return check_last();
+}
+
 RR_API int rr_op_quantize_fp8_weight(const void* w, int rows, int K, int ld, void* q_out, float* scale_out, void* stream) {
     if (!w || !scale_out || rows < 1 || ld < K || ld % 8 || ((uintptr_t)w & 15) || !fp8_weight_ok(q_out, K))
         return RR_INVALID_ARGUMENT;

@@ -406,16 +406,6 @@ static int dalloc(rr_engine* e, T** p, size_t n, bool zero = true) {
 // Tile width argument of the prefill plans (row-major modes only validate it; their tiles are 128 x 256).
 constexpr int PF_BN = MAX_BN;
 
-static int pick_splits(int N, int K) {
-    const int tilesA = (N + 127) / 128;
-    int s = num_sms() / tilesA;
-    const int kblocks = (K + 63) / 64;
-    if (s < 1) s = 1;
-    if (s > 8) s = 8;
-    while (s > 1 && kblocks / s < 8) --s;
-    return s;
-}
-
 // One engine at a time per device.  The fused MLP kernel is a persistent grid whose CTAs spin on work of sibling CTAs;
 // two such grids interleaved on one GPU (two engines, two streams) could each hold SMs the other's not-yet-resident CTAs
 // need.  Every path below synchronises its stream before it releases this lock, so engines that share a device alternate
@@ -1555,7 +1545,7 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     const int G = d.n_heads / d.n_kv_heads;
     if (!(G == 1 || G == 2 || G == 4 || G == 8)) return RR_INVALID_ARGUMENT;
     if (d.hidden > 8192) return RR_INVALID_ARGUMENT;      // add_rmsnorm_kernel keeps one row in registers (rr_elementwise.cu)
-    if (opts->max_batch < 1 || opts->max_batch > 256 || opts->ctx_max < 64 || opts->ctx_max % 64)
+    if (opts->max_batch < 1 || opts->max_batch > MAX_BATCH || opts->ctx_max < 64 || opts->ctx_max % 64)
         return RR_INVALID_ARGUMENT;
     // the KV pool: 0 = one ctx_max per decode row, else a multiple of 64 in [ctx_max, max_batch x ctx_max]
     const long long kv_full = (long long)opts->max_batch * opts->ctx_max;
@@ -1698,26 +1688,21 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
         da.head_dim = d.head_dim; da.page_table = e->d_table; da.pages_per_slot = e->pps; da.window = e->window;
         TRY(decode_attn_make_maps(&da, e->n_pages));
         // the decode projections: the same plans on e4m3 weights with FP8 (gemm_plan_init_fp8w)
-        auto plan = [&](GemmPlan* p, const void* A, const float* sc, int rowsA, int K, const void* Bop, void* out, int ldo,
-                        int splits, int mode) {
-            return fp8 ? gemm_plan_init_fp8w(p, A, sc, rowsA, K, Bop, B, K, K, out, ldo, B, splits, mode, e->bn_dec)
-                       : gemm_plan_init(p, A, rowsA, K, Bop, B, K, K, out, ldo, B, splits, mode, e->bn_dec);
-        };
-        TRY(plan(&e->pl_qkv[l], e->wqkv[l], fp8 ? e->sqkv[l] : nullptr, e->nqkv, d.hidden, e->xn, e->part_qkv, e->nqkv,
-                 e->s_qkv, OUT_TRANSPOSED_F32));
-        TRY(plan(&e->pl_o[l], e->wo[l], fp8 ? e->so[l] : nullptr, d.hidden, e->nq, e->attn_out, e->part_o, d.hidden, e->s_o,
-                 OUT_TRANSPOSED_F32));
+        TRY(decode_plan_init(&e->pl_qkv[l], e->wqkv[l], fp8 ? e->sqkv[l] : nullptr, e->nqkv, d.hidden, e->xn, B,
+                             e->part_qkv, e->nqkv, e->s_qkv, OUT_TRANSPOSED_F32));
+        TRY(decode_plan_init(&e->pl_o[l], e->wo[l], fp8 ? e->so[l] : nullptr, d.hidden, e->nq, e->attn_out, B, e->part_o,
+                             d.hidden, e->s_o, OUT_TRANSPOSED_F32));
         if (e->fuse_silu)
-            TRY(plan(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, e->act, d.inter, 1,
-                     OUT_TRANSPOSED_SILU));
+            TRY(decode_plan_init(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, B, e->act,
+                                 d.inter, 1, OUT_TRANSPOSED_SILU));
         else
-            TRY(plan(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, e->part_gu,
-                     2 * d.inter, e->s_gu, OUT_TRANSPOSED_F32));
-        TRY(plan(&e->pl_down[l], e->wdown[l], fp8 ? e->sdown[l] : nullptr, d.hidden, d.inter, e->act, e->part_down, d.hidden,
-                 e->s_down, OUT_TRANSPOSED_F32));
+            TRY(decode_plan_init(&e->pl_gu[l], e->wgu[l], fp8 ? e->sgu[l] : nullptr, 2 * d.inter, d.hidden, e->xn, B,
+                                 e->part_gu, 2 * d.inter, e->s_gu, OUT_TRANSPOSED_F32));
+        TRY(decode_plan_init(&e->pl_down[l], e->wdown[l], fp8 ? e->sdown[l] : nullptr, d.hidden, d.inter, e->act, B,
+                             e->part_down, d.hidden, e->s_down, OUT_TRANSPOSED_F32));
     }
-    TRY(gemm_plan_init(&e->pl_head, e->lm_head, d.vocab, d.hidden, e->xn, B, d.hidden, d.hidden, e->logits, d.vocab,
-                       B, 1, OUT_TRANSPOSED_F32, e->bn_dec));
+    TRY(decode_plan_init(&e->pl_head, e->lm_head, nullptr, d.vocab, d.hidden, e->xn, B, e->logits, d.vocab, 1,
+                         OUT_TRANSPOSED_F32));
     e->fuse_rope_pf = pf_rope_fused(d.head_dim);
     // deferred prefill RMSNorm: hidden % 64 == 0 and hidden <= 8192 (checked above) give the 16-byte rows and the <= 64 partial
     // sums per row that the residual epilogue writes

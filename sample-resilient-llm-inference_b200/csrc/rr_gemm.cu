@@ -1258,6 +1258,23 @@ int pick_bn(int rows) {
     return MAX_BN;
 }
 
+int pick_splits(int rows_w, int K) {
+    const int tilesA = (rows_w + 127) / 128;
+    int s = num_sms() / tilesA;
+    const int kblocks = (K + 63) / 64;
+    if (s < 1) s = 1;
+    if (s > 8) s = 8;
+    while (s > 1 && kblocks / s < 8) --s;
+    return s;
+}
+
+int decode_plan_init(GemmPlan* p, const void* W, const float* scale, int rows_w, int K, const void* X, int rows, void* out,
+                     int ldo, int splits, int mode) {
+    const int bn = pick_bn(rows);
+    return scale ? gemm_plan_init_fp8w(p, W, scale, rows_w, K, X, rows, K, K, out, ldo, rows, splits, mode, bn)
+                 : gemm_plan_init(p, W, rows_w, K, X, rows, K, K, out, ldo, rows, splits, mode, bn);
+}
+
 // ---- fused decode MLP: host side ------------------------------------------------------------------
 int mlp_slices(int inter, int* slice_kb) {
     const int kb1n = inter / BLOCK_K;

@@ -67,9 +67,10 @@ struct RopeEpi {
     int n_part_out;
 };
 
-// Widest GEMM tile along B rows (and so the largest decode batch): a consumer warpgroup holds 128 x MAX_BN fp32
-// accumulators in registers, 2 x 64 per thread at 128.
+// Widest GEMM tile along B rows: a consumer warpgroup holds 128 x MAX_BN fp32 accumulators in registers, 2 x 64 per thread
+// at 128.  Wider decode batches (up to MAX_BATCH rows, rr_engine_opts.max_batch) run several batch tiles per weight tile.
 constexpr int MAX_BN = 128;
+constexpr int MAX_BATCH = 256;
 
 struct GemmPlan {
     CUtensorMap tmA, tmB;
@@ -212,6 +213,14 @@ struct MlpPlan {
 // Decode tile width along the batch rows: the narrowest of 16 / 32 / 64 / MAX_BN that holds `rows`; wider batches run
 // several MAX_BN tiles per weight tile.
 int pick_bn(int rows);
+// Split-K planes of a decode projection W [rows_w, K]: enough (128-row weight tile, plane) items for one per SM, at most 8
+// planes and at least 8 k-blocks of 64 in each (engine.py mirrors this rule to decide the gate/up layout).
+int pick_splits(int rows_w, int K);
+// One decode projection as the engine plans it for a working set of `rows` decode rows (its max_batch): out = W . X^T in
+// `mode` (OUT_TRANSPOSED_F32 / _SILU), X [rows, K] bf16, W [rows_w, K] bf16 or, with scale, e4m3 (gemm_plan_init_fp8w);
+// tile width pick_bn(rows), plane pitch rows, `splits` planes of row pitch ldo.
+int decode_plan_init(GemmPlan* p, const void* W, const float* scale, int rows_w, int K, const void* X, int rows, void* out,
+                     int ldo, int splits, int mode);
 // K slices of the fused MLP's down GEMM: its inter / 64 k-blocks in at most 8 slices of about 16 (one output plane each;
 // 8 x 28 k-blocks for Llama-3-8B balances the per-CTA lists to within 5 %, see mlp_schedule).  Sets *slice_kb and
 // returns the number of slices (0 when inter < 64).

@@ -56,6 +56,16 @@ def _p(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(C.c_int32))
 
 
+def pick_splits(rows_w: int, K: int, n_sm: int) -> int:
+    """Split-K planes of a decode projection of rows_w weight rows over K inputs on a GPU with n_sm SMs; mirrors
+    pick_splits() in csrc/rr_gemm.cu."""
+    tiles, kb = (rows_w + 127) // 128, (K + 63) // 64
+    s = max(1, min(8, n_sm // tiles))
+    while s > 1 and kb // s < 8:
+        s -= 1
+    return s
+
+
 class Engine:
     def __init__(self, weights: Union[Weights, Fp8Weights], device: int = 0, max_batch: int = 64, ctx_max: int = 1024,
                  max_prefill_tokens: int = 8192, use_cuda_graph: bool = True,
@@ -94,10 +104,7 @@ class Engine:
         # epilogue can apply SiLU(gate) * up itself (csrc/rr_gemm.cu, OUT_*_SILU).  Needs one gate/up plane at this
         # batch size (no split-K for gate/up) and batch tiles >= 32 rows; otherwise the [gate; up] layout is kept.
         n_sm = torch.cuda.get_device_properties(device).multi_processor_count
-        tiles, kb = (2 * s.inter + 127) // 128, (s.hidden + 63) // 64
-        gu_splits = max(1, min(8, n_sm // tiles))                 # mirrors pick_splits() in csrc/rr_engine.cu
-        while gu_splits > 1 and kb // gu_splits < 8:
-            gu_splits -= 1
+        gu_splits = pick_splits(2 * s.inter, s.hidden, n_sm)
         interleave = s.inter % 64 == 0 and gu_splits == 1 and max_batch > 16
         fp8 = isinstance(weights, Fp8Weights)
         wgu = weights.wgu

@@ -262,10 +262,13 @@ def _prompts(spec, n, lo, hi, seed):
     return [rs.randint(3, spec.vocab, size=rs.randint(lo, hi)).tolist() for _ in range(n)]
 
 
-@pytest.mark.parametrize("name", ["tiny", "tiny96", "llama-3-8b-2l"])
-def test_engine_fp8_equals_bf16_engine_on_dequantized_weights(name):
+@pytest.mark.parametrize("name,max_batch", [pytest.param("tiny", 64, id="tiny"), pytest.param("tiny96", 64, id="tiny96"),
+                                            pytest.param("llama-3-8b-2l", 64, id="llama-3-8b-2l"),
+                                            # two batch tiles per weight tile, MLP unfused
+                                            pytest.param("tiny", 256, id="tiny-256")])
+def test_engine_fp8_equals_bf16_engine_on_dequantized_weights(name, max_batch):
     from oracle import llama_ref
-    spec, w, q, d, e8, eb = _pair(name, ctx_max=1024, max_prefill_tokens=2048, prefix_cache=True)
+    spec, w, q, d, e8, eb = _pair(name, max_batch, ctx_max=1024, max_prefill_tokens=2048, prefix_cache=True)
     try:
         # low-level prefill / decode logits
         ps = _prompts(spec, 4, 5, 200, 1)
