@@ -233,6 +233,11 @@ int rr_gemm_fp8w(const void* A, const float* scale, int rowsA, int ldA, const vo
 int rr_op_decode_proj(const void* w, const float* w_scale, int rows_w, int K, const void* xn, int rows, void* out,
                       int mode, int lm_head, int* n_splits, void* stream);
 
+/* Embedding gather, as the engine starts a step: x[r][c] = float(table[ids[r]][c]) exactly, for every row r < rows with
+ * row_active NULL or row_active[r] >= 0; other rows of x are not written.  table bf16 [vocab][hidden], x fp32
+ * [rows][hidden], ids / row_active int32 [rows] (device).  Ids are trusted, as slot indices are: each must be in
+ * [0, vocab).  RR_INVALID_ARGUMENT before touching the device for a null ids, table or x, rows < 1, hidden not a positive
+ * multiple of 8, and a table or x that is not 16-byte aligned. */
 int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows, int hidden,
                 const int32_t* row_active, void* stream);
 int rr_op_add_rmsnorm(float* x, const void* part, int part_is_bf16, int n_splits,
@@ -244,6 +249,14 @@ int rr_op_rope_kv(const void* qkv, int is_bf16, int n_splits, long long split_st
                   void* q_out, void* k_cache, void* v_cache, const int32_t* slot,
                   const int32_t* pos, int rows, int n_heads, int n_kv_heads, int ctx_max,
                   float theta, void* stream);
+/* Greedy pick over fp32 logits rows x (row r at logits + r * ld), as the engine picks a token: for every row r < rows with
+ * row_active NULL or row_active[r] >= 0, m = the largest value of x[0 .. vocab) that is not NaN, and
+ *   out_tok[r] = the lowest index i with x_i == m (-0 == +0), or 0 when m is -inf (every value -inf or NaN);
+ *   out_val[r] = x_i of that index (m, or -inf), when out_val is non-NULL;
+ *   pos_inc[r] += 1, when pos_inc is non-NULL.
+ * So NaN never wins and the token is always in [0, vocab).  Inactive rows keep out_tok, out_val and pos_inc; columns
+ * >= vocab are not read.  All arrays are device memory [rows].  RR_INVALID_ARGUMENT before touching the device unless
+ * logits and out_tok are non-null, rows >= 1, 1 <= vocab <= ld, ld % 4 == 0 and logits is 16-byte aligned. */
 int rr_op_argmax(const float* logits, int ld, int rows, int vocab, int32_t* out_tok,
                  float* out_val, const int32_t* row_active, int32_t* pos_inc, void* stream);
 /* Log-probabilities of the best tokens of fp32 logits rows (row r at logits + r * ld), as the engine computes them for
@@ -263,7 +276,9 @@ int rr_op_logprobs(const float* logits, int ld, int rows, int vocab, const int32
  *         (top_p >= 1: every token; tokens tied at tau are all inside),
  *   G_i = -log(-log u_i), u_i = (2 (r_i >> 9) + 1) / 2^24, r_i = word 0 of Philox4x32-10 with key seed[r] (low word first)
  *         and counter (i, position[r], 0, 0).
- * Rows with temperature[r] <= 0 are not touched.  The draw is a pure function of (row, T, top_p, seed, position).
+ * Rows with temperature[r] <= 0 are not touched, nor are rows with no candidate i (every x_i -inf or NaN, or a tau that
+ * is NaN): in the engine, out_tok[r] then keeps the greedy token rr_op_argmax wrote.  The draw is a pure function of (row,
+ * T, top_p, seed, position).
  * RR_INVALID_ARGUMENT before touching the device unless no pointer is null, 1 <= rows <= 65535, 1 <= vocab <= ld,
  * vocab <= 524288 and ld % 4 == 0.  Deterministic: every sum is exact (fixed point) or runs in a fixed order. */
 int rr_op_sample(const float* logits, int ld, int rows, int vocab, const float* temperature, const float* top_p,
@@ -466,6 +481,8 @@ int rr_op_prefill_gemm(const void* A, int plan_rows, int T, int ldA, const void*
  *    Replaces one `litellm_params.model: bedrock/...` deployment (reference config.yaml:39,47,54,
  *    62,69,77,84,91). */
 
+/* vocab: a multiple of 4, >= 4 (each row of the [rows][vocab] fp32 logits is read with 16-byte loads); rr_engine_create
+ * returns RR_INVALID_ARGUMENT before any CUDA call otherwise. */
 typedef struct rr_model_desc {
     int32_t vocab, hidden, inter, n_layers, n_heads, n_kv_heads, head_dim;
     float rope_theta, rms_eps;
@@ -629,8 +646,7 @@ typedef struct rr_gen_params {
  * 1 <= n_choices <= max_batch; -1 <= top_logprobs <= 20; 0 <= temperature <= 2; 0 <= top_p <= 1; -2 <= penalties <= 2;
  * 0 <= n_bias <= 300 with non-null arrays when n_bias > 0, unique bias ids in [0, vocab) and -100 <= bias values <= 100;
  * 0 <= n_stop <= 4 sequences of 1..64 bytes with non-null arrays when n_stop > 0; response_format 0 or 1, and 1 only with
- * vocab >= 259 (some bytes have no token otherwise).  top_logprobs >= 0 and temperature > 0 need a vocabulary that is a
- * multiple of 4.
+ * vocab >= 259 (some bytes have no token otherwise).  top_logprobs >= 0 and temperature > 0 need vocab <= 524288.
  * Stats: prefill_tokens counts the prompt once (over all its pieces), kv_copy_tokens grows by (n_choices - 1) x the prompt length,
  * generated_tokens counts every token produced, the ones a stop sequence cut included. */
 int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, const rr_gen_params* p,
@@ -647,7 +663,7 @@ int rr_engine_submit(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int 
  * 525 MB at vocab 128256, and 96 B per max_prefill_tokens row) with its first scoring request; if that fails, the scoring
  * requests end with RR_INTERNAL and the engine serves on.  Read the scores with rr_engine_prompt_logprobs before
  * rr_engine_wait.  RR_INVALID_ARGUMENT, before anything is queued, for whatever rr_engine_submit rejects, prompt_top
- * outside -1..20, and prompt_top >= 0 with a vocabulary that is not a multiple of 4. */
+ * outside -1..20, and prompt_top >= 0 with vocab above 524288. */
 int rr_engine_submit_scored(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens,
                             const rr_gen_params* p, int prompt_top, uint64_t* ticket);
 /* Blocks like rr_engine_wait until the request is done, then copies its prompt logprobs WITHOUT consuming the ticket

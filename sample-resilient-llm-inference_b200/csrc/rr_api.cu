@@ -209,9 +209,11 @@ static PartIn mk_part(const void* p, int is_bf16, int n_splits, long long split_
     return r;
 }
 
+// The embedding gather as the engine runs it at the start of a step; ids are trusted, as slot indices are.
 RR_API int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows, int hidden,
                        const int32_t* row_active, void* stream) {
-    if (!ids || !table || !x || hidden % 8) return RR_INVALID_ARGUMENT;
+    if (!ids || !table || !x || rows < 1 || hidden < 8 || hidden % 8) return RR_INVALID_ARGUMENT;
+    if (((uintptr_t)table & 15) || ((uintptr_t)x & 15)) return RR_INVALID_ARGUMENT;     // 16-byte loads and stores
     launch_embed(ids, (const __nv_bfloat16*)table, x, rows, hidden, row_active, (cudaStream_t)stream);
     return check_last();
 }
@@ -247,9 +249,11 @@ RR_API int rr_op_rope_kv(const void* qkv, int is_bf16, int n_splits, long long s
     return check_last();
 }
 
+// The greedy pick as the engine runs it first in the logits tail.
 RR_API int rr_op_argmax(const float* logits, int ld, int rows, int vocab, int32_t* out_tok,
                         float* out_val, const int32_t* row_active, int32_t* pos_inc, void* stream) {
-    if (!logits || !out_tok || ld % 4) return RR_INVALID_ARGUMENT;
+    if (!logits || !out_tok || rows < 1 || vocab < 1 || vocab > ld || ld % 4) return RR_INVALID_ARGUMENT;
+    if ((uintptr_t)logits & 15) return RR_INVALID_ARGUMENT;                              // 16-byte loads of each row
     launch_argmax(mk_part(logits, 0, 1, 0, ld), rows, vocab, out_tok, out_val, row_active, pos_inc,
                   (cudaStream_t)stream);
     return check_last();

@@ -385,7 +385,7 @@ void launch_rope_kv(const RopeArgs& a, cudaStream_t st) {
     launch_pdl(rope_kv_kernel, dim3(a.rows), dim3(256), 0, st, a);
 }
 
-// ---- greedy argmax (lowest index wins ties) ------------------------------------------------------
+// ---- greedy argmax (lowest index wins ties; NaN never wins; no value above -inf: token 0) -------------
 __global__ void __launch_bounds__(1024)
 argmax_kernel(PartIn logits, int vocab, int32_t* __restrict__ out_tok, float* __restrict__ out_val,
               const int32_t* __restrict__ row_active, int32_t* __restrict__ pos_inc) {
@@ -444,7 +444,10 @@ argmax_kernel(PartIn logits, int vocab, int32_t* __restrict__ out_tok, float* __
             if (better(ov, oi, best, bi)) { best = ov; bi = oi; }
         }
         if (lane == 0) {
-            out_tok[row] = bi;
+            // only a value above -inf replaces the start (-inf, 0x7fffffff), and NaN never compares above: a row of -inf
+            // and NaN only picks token 0, as torch.argmax does for an all -inf row, so the next step's embedding gather
+            // stays inside the table
+            out_tok[row] = best > -INFINITY ? bi : 0;
             if (out_val) out_val[row] = best;
             if (pos_inc) pos_inc[row] += 1;
         }
@@ -635,7 +638,7 @@ void launch_logprobs(const float* logits, int ld, int rows, int vocab, const int
 // so the shared-memory atomics are order-independent and the result is bit-reproducible; an element lighter than 2^-40 of
 // the row max counts as 0.  top_p >= 1 skips the search (tau = -inf).  (2) One CTA per LP_CHUNK columns draws the chunk's
 // Gumbel-max candidate over {x >= tau}.  (3) One warp per row merges the chunks' candidates in the argmax order, which is
-// a total order, so the result does not depend on the merge order either.
+// a total order, so the result does not depend on the merge order either.  A row without any candidate keeps its token.
 constexpr int SP_THREADS = 1024;
 constexpr int SP_BINS = 2048;
 struct SpPart { float v; int32_t id; };
@@ -837,7 +840,8 @@ sample_merge_kernel(const float* __restrict__ temperature, int n_chunks, const S
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (lp_before(ov, oi, bv, bi)) { bv = ov; bi = oi; }
     }
-    if (threadIdx.x == 0) out_tok[row] = bi;
+    // no chunk had a candidate (every column -inf or NaN, or a NaN tau): the token the argmax wrote stays
+    if (threadIdx.x == 0 && bi != 0x7fffffff) out_tok[row] = bi;
     trace_end(tr_slot);
 }
 

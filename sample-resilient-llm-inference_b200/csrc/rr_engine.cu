@@ -1545,6 +1545,8 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     const int G = d.n_heads / d.n_kv_heads;
     if (!(G == 1 || G == 2 || G == 4 || G == 8)) return RR_INVALID_ARGUMENT;
     if (d.hidden > 8192) return RR_INVALID_ARGUMENT;      // add_rmsnorm_kernel keeps one row in registers (rr_elementwise.cu)
+    // the logits tail reads each row of [rows][vocab] fp32 logits with 16-byte loads: every row must start 16-byte aligned
+    if (d.vocab < 4 || d.vocab % 4) return RR_INVALID_ARGUMENT;
     if (opts->max_batch < 1 || opts->max_batch > MAX_BATCH || opts->ctx_max < 64 || opts->ctx_max % 64)
         return RR_INVALID_ARGUMENT;
     // the KV pool: 0 = one ctx_max per decode row, else a multiple of 64 in [ctx_max, max_batch x ctx_max]
@@ -1846,8 +1848,8 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
                          uint64_t* ticket, const GenParams& p, int n_choices) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
     if (n_choices < 1 || n_choices > e->Bm) return RR_INVALID_ARGUMENT;      // the choices decode side by side
-    // the vocabularies the logprobs / sampling kernels handle
-    if ((p.logprobs() || p.sampled() || p.scores()) && (e->d.vocab % 4 || e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK))
+    // the vocabularies the logprobs / sampling kernels handle (rr_engine_create refused vocab % 4 != 0)
+    if ((p.logprobs() || p.sampled() || p.scores()) && e->d.vocab > LP_MAX_CHUNKS * LP_CHUNK)
         return RR_INVALID_ARGUMENT;
     if (p.prompt_top < -1 || p.prompt_top > LP_MAX_TOP) return RR_INVALID_ARGUMENT;
     if (n_prompt + max_new_tokens > e->o.ctx_max) return RR_INVALID_ARGUMENT;
