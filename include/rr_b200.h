@@ -405,6 +405,20 @@ int rr_op_prefill_attn_window(const void* q, const void* k_cache, const void* v_
                               const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
                               int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale,
                               const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream);
+/* Prefill attention exactly as the engine launches it for one chunk: the arguments of rr_op_prefill_attn_window with the
+ * true head_dim in place of scale, plus q_rows.  The scale is the engine's, 1 / sqrtf(head_dim).  q is [q_rows][n_heads *
+ * 128] bf16 with columns [head_dim, 128) of each head zero, mapped over all q_rows rows as the engine maps its prefill
+ * buffer (q_rows >= T = seq_start[n_seqs]; rows T.. may hold anything and are never written out).  Caches are paged
+ * [n_pages][n_kv_heads][64][128] bf16, columns [head_dim, 128) ignored.  out is [T][n_heads * head_dim] bf16: element
+ * (t, h * head_dim + d) for d < head_dim; nothing else is written.  With head_dim 128 the result equals
+ * rr_op_prefill_attn_window's at scale 1 / sqrtf(128), bit for bit.  Returns RR_INVALID_ARGUMENT before touching the
+ * device for a null pointer, head_dim outside 64..128 or not a multiple of 16, n_heads / n_kv_heads not in {1, 2, 4, 8},
+ * a page table rr_op_prefill_attn_window rejects, max_len below 1, q_rows < max_len or a negative window; and after
+ * reading the index arrays back, for what rr_op_prefill_attn_cached rejects there or q_rows < T. */
+int rr_op_prefill_attn_hd(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* seq_start,
+                          const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs, int max_len, int n_heads,
+                          int n_kv_heads, int head_dim, int ctx_max, const int32_t* page_table, int pages_per_slot,
+                          int n_pages, int window, int q_rows, void* stream);
 /* Fused decode MLP, one launch exactly as the engine runs it for a batch of `rows` (tile width, K slices, grid and
  * schedule from the engine's rules; env RR_MLP_STATIC / RR_NO_TMA_EPI are read per call):
  *   act[b, n]       = bf16(SiLU(xn[b] . gate[n]) * (xn[b] . up[n]))                        bf16 [rows, inter]

@@ -193,6 +193,8 @@ PROTOTYPES = {
                                                   C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]),
     "rr_op_prefill_attn_window": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                             C.c_int, C.c_float, vp, C.c_int, C.c_int, C.c_int, vp]),
+    "rr_op_prefill_attn_hd": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                        C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]),
     "rr_op_kv_copy_prefix_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int,
                                              vp, C.c_int, C.c_int, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),

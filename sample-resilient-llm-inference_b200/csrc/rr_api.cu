@@ -654,16 +654,17 @@ RR_API int rr_op_prefill_attn(const void* q, const void* k_cache, const void* v_
     return check_last();
 }
 
-// Prefill attention with a cached prefix per sequence (seq_pos0): the engine's launch.  Like rr_op_prefill_attn, the TMA
-// maps need the extents of q and of the caches, read back from the caller's index arrays; the positions are checked
-// against ctx_max on the way.
+// Prefill attention with a cached prefix per sequence (seq_pos0): the engine's launch, through the engine's helpers
+// (pf_attn_layer, pf_attn_chunk).  Like rr_op_prefill_attn, the TMA maps need the extents of the caches, and q_rows = 0
+// those of q (T rows), read back from the caller's index arrays; the positions are checked against ctx_max on the way.
+// scale null: the engine's, 1 / sqrt(head_dim).
 static int prefill_attn_cached(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* seq_start,
                                const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs, int max_len, int n_heads,
-                               int n_kv_heads, int ctx_max, float scale, const int32_t* page_table, int pages_per_slot,
-                               int n_pages, int window, void* stream) {
+                               int n_kv_heads, int ctx_max, const float* scale, int head_dim, int q_rows,
+                               const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream) {
     if (!q || !k_cache || !v_cache || !out || !seq_start || !seq_slot || !seq_pos0 || window < 0) return RR_INVALID_ARGUMENT;
     if (n_seqs < 1 || max_len < 1 || n_heads < 1 || n_kv_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
-    if (ctx_max < 64 || ctx_max % 64) return RR_INVALID_ARGUMENT;
+    if (ctx_max < 64 || ctx_max % 64 || q_rows < 0) return RR_INVALID_ARGUMENT;
     cudaStream_t st = (cudaStream_t)stream;
     std::vector<int32_t> h(3 * (size_t)n_seqs + 1);         // seq_start[n + 1] | seq_slot[n] | seq_pos0[n]
     cudaError_t e = cudaMemcpyAsync(h.data(), seq_start, sizeof(int32_t) * (n_seqs + 1), cudaMemcpyDeviceToHost, st);
@@ -677,14 +678,13 @@ static int prefill_attn_cached(const void* q, const void* k_cache, const void* v
         if (len < 0 || len > max_len || slot < 0 || p0 < 0 || p0 + len > ctx_max) return RR_INVALID_ARGUMENT;
         max_slot = slot > max_slot ? slot : max_slot;
     }
+    if (q_rows > 0 && q_rows < h[n_seqs]) return RR_INVALID_ARGUMENT;
     PrefillAttnArgs a;
-    a.q = (const __nv_bfloat16*)q; a.k_cache = (const __nv_bfloat16*)k_cache;
-    a.v_cache = (const __nv_bfloat16*)v_cache; a.out = (__nv_bfloat16*)out; a.seq_start = seq_start;
-    a.seq_slot = seq_slot; a.seq_pos0 = seq_pos0; a.n_seqs = n_seqs; a.max_len = max_len; a.n_heads = n_heads;
-    a.n_kv_heads = n_kv_heads; a.ctx_max = ctx_max; a.scale = scale; a.head_dim = 128;
-    a.page_table = page_table; a.pages_per_slot = pages_per_slot; a.window = window;
-    (void)prefill_attn_make_maps(&a, h[n_seqs], page_table ? (long long)n_pages * n_kv_heads * KV_PAGE
-                                                           : (long long)(max_slot + 1) * n_kv_heads * ctx_max);
+    (void)pf_attn_layer(&a, (const __nv_bfloat16*)q, (const __nv_bfloat16*)k_cache, (const __nv_bfloat16*)v_cache, n_heads,
+                        n_kv_heads, head_dim, ctx_max, page_table, pages_per_slot, page_table ? n_pages : max_slot + 1,
+                        window, q_rows > 0 ? q_rows : h[n_seqs]);
+    if (scale) a.scale = *scale;
+    pf_attn_chunk(&a, (__nv_bfloat16*)out, seq_start, seq_slot, seq_pos0, n_seqs, max_len);
     const int rcl = launch_prefill_attn(a, st);
     if (rcl != RR_OK) return rcl;
     return check_last();
@@ -694,7 +694,7 @@ RR_API int rr_op_prefill_attn_cached(const void* q, const void* k_cache, const v
                                      const int32_t* seq_start, const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs,
                                      int max_len, int n_heads, int n_kv_heads, int ctx_max, float scale, void* stream) {
     return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
-                               ctx_max, scale, nullptr, 0, 0, 0, stream);
+                               ctx_max, &scale, 128, 0, nullptr, 0, 0, 0, stream);
 }
 
 RR_API int rr_op_prefill_attn_window(const void* q, const void* k_cache, const void* v_cache, void* out,
@@ -703,7 +703,23 @@ RR_API int rr_op_prefill_attn_window(const void* q, const void* k_cache, const v
                                      const int32_t* page_table, int pages_per_slot, int n_pages, int window, void* stream) {
     if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
     return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
-                               ctx_max, scale, page_table, pages_per_slot, n_pages, window, stream);
+                               ctx_max, &scale, 128, 0, page_table, pages_per_slot, n_pages, window, stream);
+}
+
+// Prefill attention exactly as run_prefill launches it: the true head dim, its compact output and the engine's scale, the
+// page table and window, q mapped over q_rows rows.  Refuses whatever rr_engine_create would not build.
+RR_API int rr_op_prefill_attn_hd(const void* q, const void* k_cache, const void* v_cache, void* out, const int32_t* seq_start,
+                                 const int32_t* seq_slot, const int32_t* seq_pos0, int n_seqs, int max_len, int n_heads,
+                                 int n_kv_heads, int head_dim, int ctx_max, const int32_t* page_table, int pages_per_slot,
+                                 int n_pages, int window, int q_rows, void* stream) {
+    if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
+    if (head_dim < 64 || head_dim > 128 || head_dim % 16) return RR_INVALID_ARGUMENT;
+    if (n_kv_heads < 1 || n_heads < 1 || n_heads % n_kv_heads) return RR_INVALID_ARGUMENT;
+    const int G = n_heads / n_kv_heads;
+    if (!(G == 1 || G == 2 || G == 4 || G == 8)) return RR_INVALID_ARGUMENT;
+    if (max_len < 1 || q_rows < max_len) return RR_INVALID_ARGUMENT;     // q_rows >= T >= max_len; T is checked on read-back
+    return prefill_attn_cached(q, k_cache, v_cache, out, seq_start, seq_slot, seq_pos0, n_seqs, max_len, n_heads, n_kv_heads,
+                               ctx_max, nullptr, head_dim, q_rows, page_table, pages_per_slot, n_pages, window, stream);
 }
 
 RR_API int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const void* v_cache, void* out,

@@ -918,10 +918,8 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ra.table = e->rope_table; ra.head_dim = d.head_dim; ra.page_table = e->d_table; ra.pages_per_slot = e->pps;
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
         if (nt == 0 && !scoring && l + 1 == d.n_layers) break;    // every layer's KV is written
-        PrefillAttnArgs pa = e->pf_attn[l];          // per-layer TMA maps made at create
-        pa.q = e->pq; pa.k_cache = kc; pa.v_cache = vc; pa.out = e->pattn; pa.seq_start = p_ss; pa.seq_slot = p_sl;
-        pa.seq_pos0 = pos0 ? p_p0 : nullptr; pa.n_seqs = n_seqs; pa.max_len = max_len; pa.n_heads = d.n_heads; pa.n_kv_heads = d.n_kv_heads;
-        pa.ctx_max = e->o.ctx_max; pa.scale = 1.0f / sqrtf((float)d.head_dim); pa.head_dim = d.head_dim;
+        PrefillAttnArgs pa = e->pf_attn[l];          // per-layer operands, scale and TMA maps made at create (pf_attn_layer)
+        pf_attn_chunk(&pa, e->pattn, p_ss, p_sl, pos0 ? p_p0 : nullptr, n_seqs, max_len);
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (l + 1 == d.n_layers && nt > 0) {
             // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers).  The
@@ -1672,14 +1670,9 @@ RR_API int rr_engine_create(const rr_model_desc* desc, const rr_model_weights* w
     e->attn_args.resize(L);
     e->pf_attn.resize(L);
     for (int l = 0; l < L; ++l) {
-        {
-            PrefillAttnArgs& pa = e->pf_attn[l];
-            pa.q = e->pq; pa.k_cache = e->kcache + (size_t)l * e->kv_layer_stride;
-            pa.v_cache = e->vcache + (size_t)l * e->kv_layer_stride; pa.n_heads = d.n_heads;
-            pa.n_kv_heads = d.n_kv_heads; pa.ctx_max = opts->ctx_max; pa.head_dim = d.head_dim;
-            pa.page_table = e->d_table; pa.pages_per_slot = e->pps; pa.window = e->window;
-            TRY(prefill_attn_make_maps(&pa, T, (long long)e->n_pages * d.n_kv_heads * KV_PAGE));
-        }
+        TRY(pf_attn_layer(&e->pf_attn[l], e->pq, e->kcache + (size_t)l * e->kv_layer_stride,
+                          e->vcache + (size_t)l * e->kv_layer_stride, d.n_heads, d.n_kv_heads, d.head_dim, opts->ctx_max,
+                          e->d_table, e->pps, e->n_pages, e->window, T));
         DecodeAttnArgs& da = e->attn_args[l];
         da.q = e->qbuf; da.k_cache = e->kcache + (size_t)l * e->kv_layer_stride;
         da.v_cache = e->vcache + (size_t)l * e->kv_layer_stride; da.out = e->attn_out; da.slot = e->d_slot;

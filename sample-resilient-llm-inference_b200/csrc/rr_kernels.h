@@ -404,7 +404,7 @@ struct PrefillAttnArgs {
     const __nv_bfloat16* q;   // [T, n_heads*128] (RoPE applied)
     const __nv_bfloat16* k_cache;
     const __nv_bfloat16* v_cache;
-    __nv_bfloat16* out;       // [T, n_heads*128]
+    __nv_bfloat16* out;       // [T, n_heads*head_dim]
     const int32_t* seq_start; // [n_seqs+1] token offsets into T
     const int32_t* seq_slot;  // [n_seqs]
     const int32_t* seq_pos0 = nullptr;   // [n_seqs] position of each sequence's first query row (cached prefix); null: all 0
@@ -422,6 +422,25 @@ int launch_prefill_attn(const PrefillAttnArgs& a, cudaStream_t st);   // RR_ERR_
 int prefill_attn_make_maps(PrefillAttnArgs* a, long long q_rows, long long kv_rows);
 bool prefill_attn_tc_eligible(const PrefillAttnArgs& a);
 int launch_prefill_attn_tc(const PrefillAttnArgs& a, cudaStream_t st);
+// Prefill attention as the engine launches it, in two parts.  Per layer (rr_engine_create): the operands, the true head
+// dim and its scale 1 / sqrt(head_dim), the page table, the window, and the TMA maps: q over q_rows rows (the engine's Tmax,
+// so a chunk of T < q_rows rows loads stale q rows into its last query tile; their outputs are never written) and each
+// cache over n_pages pages (slots without a page table).  Per chunk (run_prefill): `out` [T][n_heads * head_dim] and the
+// chunk's sequences.
+inline int pf_attn_layer(PrefillAttnArgs* a, const __nv_bfloat16* q, const __nv_bfloat16* k_cache, const __nv_bfloat16* v_cache,
+                         int n_heads, int n_kv_heads, int head_dim, int ctx_max, const int32_t* page_table, int pages_per_slot,
+                         int n_pages, int window, long long q_rows) {
+    a->q = q; a->k_cache = k_cache; a->v_cache = v_cache;
+    a->n_heads = n_heads; a->n_kv_heads = n_kv_heads; a->ctx_max = ctx_max;
+    a->head_dim = head_dim; a->scale = 1.0f / sqrtf((float)head_dim);
+    a->page_table = page_table; a->pages_per_slot = pages_per_slot; a->window = window;
+    return prefill_attn_make_maps(a, q_rows, (long long)n_pages * n_kv_heads * (page_table ? KV_PAGE : ctx_max));
+}
+inline void pf_attn_chunk(PrefillAttnArgs* a, __nv_bfloat16* out, const int32_t* seq_start, const int32_t* seq_slot,
+                          const int32_t* seq_pos0, int n_seqs, int max_len) {
+    a->out = out; a->seq_start = seq_start; a->seq_slot = seq_slot; a->seq_pos0 = seq_pos0;
+    a->n_seqs = n_seqs; a->max_len = max_len;
+}
 
 // ---- prompt prefix caching (rr_kv_copy.cu): positions [0, n[i]) of slot src[i] -> slot dst[i], every layer and kv head,
 // K and V, one launch for the whole list (passed by value as a kernel parameter).  Each layer's cache is layer_rows rows of
