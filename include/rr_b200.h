@@ -240,6 +240,14 @@ int rr_op_decode_proj(const void* w, const float* w_scale, int rows_w, int K, co
  * multiple of 8, and a table or x that is not 16-byte aligned. */
 int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows, int hidden,
                 const int32_t* row_active, void* stream);
+/* Embedding pool, as the engine pools a prefill chunk's embedding rows: for i < n, v = float(xn[rows ? rows[i] : i][0..hidden))
+ * (bf16, row pitch ld elements), S = sum_c v_c^2 accumulated in fp64 in a fixed order (each square is exact),
+ * out[i * out_ld + c] = fp32(v_c / sqrt(S)) computed in fp64 and rounded once, for c < hidden; S == 0 gives zeros.
+ * Columns >= hidden of out and rows not listed are not written.  Deterministic: two calls agree bit for bit.  Row indices
+ * are trusted, as ids are.  RR_INVALID_ARGUMENT before touching the device for a null xn or out, n outside 1..65535,
+ * hidden not a positive multiple of 8 up to 16384, ld < hidden, out_ld < hidden, or a misaligned xn (16 B: xn itself and
+ * ld % 8, every row). */
+int rr_op_embed_pool(const void* xn, int ld, const int32_t* rows, int n, int hidden, float* out, int out_ld, void* stream);
 int rr_op_add_rmsnorm(float* x, const void* part, int part_is_bf16, int n_splits,
                       long long split_stride, int part_ld, const void* w, void* xn, int rows,
                       int hidden, float eps, void* stream);
@@ -687,6 +695,31 @@ int rr_engine_submit_scored(rr_engine* e, const int32_t* prompt_ids, int n_promp
  * cancelled ticket and a request submitted without scoring. */
 int rr_engine_prompt_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
                               int32_t* id_out);
+/* Queue an embedding request (OpenAI /v1/embeddings): prefill the prompt, pool its last position's final-norm row
+ * (rr_op_embed_pool: L2-normalised, fp32 [hidden]) and finish.  No decode row, no token.
+ * - Admission: as a prompt.  It waits at the head of the queue for a free row and ceil(n_prompt / 64) pages (or the ring
+ *   R of a windowed model, as in rr_engine_submit), goes into the chunk as one sequence, and a long prompt is prefilled in
+ *   pieces with the usual decode step between them.  It takes prefix-cache hits and, on success, leaves its prompt
+ *   retained, exactly as a generation request does.
+ * - The chunk that holds its last piece gives it one embedding row after the chunk's tail rows: the trimmed last layer
+ *   runs over both, lm_head and the logits tail over the tail rows only (a chunk of embedding rows only launches neither).
+ *   Every kernel of the trimmed layer is row-independent, so generation requests in the same chunk get bit-identical
+ *   tokens, logprobs and stop / JSON results, and the embedding does not depend on the chunk, the pieces, the prefix
+ *   cache or the slot.
+ * - After that chunk the request is done and its row free: it never enters the decode working set or changes the decode
+ *   graph.  generated_tokens does not grow; prefill_tokens counts its prompt.  Cancellation, fail_prob and internal errors
+ *   behave as for any request; the done hook reports 0 tokens.
+ * - The engine allocates the embedding buffers (4 B x max_batch x hidden, device and pinned) with its first embedding row:
+ *   an engine that never embeds allocates nothing for them.
+ * Read the embedding with rr_engine_embedding, then finish with rr_engine_wait (0 tokens) or rr_engine_cancel.
+ * RR_INVALID_ARGUMENT, before anything is queued, for a NULL engine / prompt / ticket, n_prompt below 1 or above ctx_max,
+ * min(ceil(n_prompt / 64), R) x 64 above kv_cache_tokens and a prompt token outside [0, vocab). */
+int rr_engine_submit_embed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, uint64_t* ticket);
+/* Blocks like rr_engine_prompt_logprobs until the request is done, then copies its embedding (fp32 [hidden]) into out
+ * WITHOUT consuming the ticket (finish with rr_engine_wait, which reports 0 tokens); *dim_out = hidden (dim_out may be
+ * NULL).  Same returns as rr_engine_prompt_logprobs; RR_INVALID_ARGUMENT also for a NULL out, capacity < hidden and a
+ * request that is not an embedding. */
+int rr_engine_embedding(rr_engine* e, uint64_t ticket, double timeout_s, float* out, int capacity, int* dim_out);
 /* Block (release the GIL) until the request is done, or timeout_s (<= 0: no limit) elapses.  RR_TIMEOUT: still in flight
  * (out->status = RR_TIMEOUT), wait again or rr_engine_cancel.  Otherwise the ticket is consumed and the request's status
  * returned (RR_OK / RR_BACKEND_FAILED / ...), with `out` filled and for every choice c of its n_choices:
@@ -822,6 +855,17 @@ int rr_gateway_submit_scored(rr_gateway* g, int group, const int32_t* prompt_ids
  * replica that served it without consuming the ticket (finish with rr_gateway_wait).  Same buffers and returns. */
 int rr_gateway_prompt_logprobs(rr_gateway* g, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
                                int32_t* id_out);
+/* An embedding request (rr_engine_submit_embed) through the gateway: one ADMIT event carrying its n_prompt tokens (the tpm
+ * debit), and on success one DONE event with 0 completion tokens and the usual latency sample.  A backend failure walks
+ * the fallback chain and the new replica prefills the prompt again.  Refusals in rr_gateway_submit's order and codes (a
+ * prompt of up to the smallest context window, ceil(n_prompt / 64) pages per engine pool); RR_INVALID_ARGUMENT also with a
+ * mock replica attached, which has no hidden state. */
+int rr_gateway_submit_embed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, uint64_t* ticket);
+/* rr_engine_embedding for a gateway ticket: blocks until the request is finished and copies the embedding of the replica
+ * that served it without consuming the ticket (finish with rr_gateway_wait); *dim_out = that replica's hidden size.  Same
+ * returns as rr_gateway_prompt_logprobs; RR_INVALID_ARGUMENT also for a NULL out, capacity below the served embedding's
+ * size and a request that is not an embedding. */
+int rr_gateway_embedding(rr_gateway* g, uint64_t ticket, double timeout_s, float* out, int capacity, int* dim_out);
 /* A closed burst of plain requests (greedy, one choice) as one contiguous block of the admission trace (declare_burst != 0
  * prepends RR_EV_BURST). */
 int rr_gateway_submit_batch(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,

@@ -169,6 +169,7 @@ PROTOTYPES = {
     "rr_op_quantize_fp8_weight": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
     "rr_op_dequantize_fp8_weight": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
     "rr_op_embed": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
+    "rr_op_embed_pool": (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
     "rr_op_add_rmsnorm": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp, vp,
                                     C.c_int, C.c_int, C.c_float, vp]),
     "rr_op_silu_mul": (C.c_int, [vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp, C.c_int,
@@ -223,6 +224,8 @@ PROTOTYPES = {
     "rr_engine_submit_scored": (C.c_int, [vp, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.c_int,
                                           C.POINTER(C.c_uint64)]),
     "rr_engine_prompt_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, c_f32p, c_i32p]),
+    "rr_engine_submit_embed": (C.c_int, [vp, c_i32p, C.c_int, C.POINTER(C.c_uint64)]),
+    "rr_engine_embedding": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, C.c_int, c_i32p]),
     "rr_engine_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(Completion), c_i32p, C.c_int, c_f32p, c_i32p, c_i32p,
                                  c_i32p]),
     "rr_engine_peek": (C.c_int, [vp, C.c_uint64, C.c_int, C.c_double, c_i32p, C.c_int, c_i32p, c_i32p,
@@ -242,6 +245,8 @@ PROTOTYPES = {
     "rr_gateway_submit_scored": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.c_int, C.POINTER(GenParams), C.c_int,
                                            C.POINTER(C.c_uint64)]),
     "rr_gateway_prompt_logprobs": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, c_f32p, c_i32p]),
+    "rr_gateway_submit_embed": (C.c_int, [vp, C.c_int, c_i32p, C.c_int, C.POINTER(C.c_uint64)]),
+    "rr_gateway_embedding": (C.c_int, [vp, C.c_uint64, C.c_double, c_f32p, C.c_int, c_i32p]),
     "rr_gateway_submit_batch": (C.c_int, [vp, C.c_int, c_i32p, c_i32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint64)]),
     "rr_gateway_wait": (C.c_int, [vp, C.c_uint64, C.c_double, C.POINTER(GatewayResult), c_i32p, C.c_int, c_f32p, c_i32p,
                                   c_i32p, c_i32p]),

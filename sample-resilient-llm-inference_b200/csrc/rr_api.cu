@@ -218,6 +218,16 @@ RR_API int rr_op_embed(const int32_t* ids, const void* table, float* x, int rows
     return check_last();
 }
 
+// The embedding pool as the engine runs it over a prefill chunk's embedding rows; row indices are trusted, as ids are.
+RR_API int rr_op_embed_pool(const void* xn, int ld, const int32_t* rows, int n, int hidden, float* out, int out_ld,
+                            void* stream) {
+    if (!xn || !out || n < 1 || n > 65535 || hidden < 8 || hidden > 16384 || hidden % 8 || ld < hidden || out_ld < hidden)
+        return RR_INVALID_ARGUMENT;
+    if (((uintptr_t)xn & 15) || ld % 8) return RR_INVALID_ARGUMENT;         // 16-byte loads of every row
+    launch_embed_pool((const __nv_bfloat16*)xn, ld, rows, n, hidden, out, out_ld, (cudaStream_t)stream);
+    return check_last();
+}
+
 RR_API int rr_op_add_rmsnorm(float* x, const void* part, int part_is_bf16, int n_splits,
                              long long split_stride, int part_ld, const void* w, void* xn, int rows,
                              int hidden, float eps, void* stream) {

@@ -1219,6 +1219,56 @@ void launch_json_advance(int rows, const int32_t* fmt, const int32_t* row_active
                state_out, out_row, done);
 }
 
+// ---- embedding pool (rr_op_embed_pool) ------------------------------------------------------------
+// One CTA of EMBED_POOL_THREADS per row.  Thread t owns the 8-column groups t, t + 256, ...; it squares its bf16 values in
+// fp64 (exact: 8-bit mantissas) and sums them in column order, then a fixed xor tree per warp and warp 0..7 in order:
+// the same shape every call, so the same bits.  The normalise pass reads the row again (it is in L1 / L2).
+constexpr int EMBED_POOL_THREADS = 256;
+
+__global__ void __launch_bounds__(EMBED_POOL_THREADS)
+embed_pool_kernel(const __nv_bfloat16* __restrict__ xn, int ld, const int32_t* __restrict__ rows, int hidden,
+                  float* __restrict__ out, int out_ld) {
+    __shared__ double red[EMBED_POOL_THREADS / 32];
+    griddep_launch();
+    griddep_wait();
+    const int i = blockIdx.x;
+    const __nv_bfloat16* src = xn + (size_t)(rows ? rows[i] : i) * ld;
+    double s = 0.0;
+    for (int c = threadIdx.x * 8; c < hidden; c += EMBED_POOL_THREADS * 8) {
+        const uint4 v = *reinterpret_cast<const uint4*>(src + c);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const double a = (double)bf16_lo(w[j]), b = (double)bf16_hi(w[j]);
+            s += a * a;
+            s += b * b;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    double S = 0.0;
+#pragma unroll
+    for (int w = 0; w < EMBED_POOL_THREADS / 32; ++w) S += red[w];
+    const double norm = sqrt(S);
+    float* dst = out + (size_t)i * out_ld;
+    for (int c = threadIdx.x * 8; c < hidden; c += EMBED_POOL_THREADS * 8) {
+        const uint4 v = *reinterpret_cast<const uint4*>(src + c);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            dst[c + 2 * j] = S > 0.0 ? (float)((double)bf16_lo(w[j]) / norm) : 0.f;
+            dst[c + 2 * j + 1] = S > 0.0 ? (float)((double)bf16_hi(w[j]) / norm) : 0.f;
+        }
+    }
+}
+
+void launch_embed_pool(const __nv_bfloat16* xn, int ld, const int32_t* rows, int n, int hidden, float* out, int out_ld,
+                       cudaStream_t st) {
+    if (n <= 0) return;
+    launch_pdl(embed_pool_kernel, dim3(n), dim3(EMBED_POOL_THREADS), 0, st, xn, ld, rows, hidden, out, out_ld);
+}
+
 void rr_trace_set_elementwise(unsigned long long* p) { rr_trace_set_local(p); }
 
 }  // namespace rr

@@ -96,6 +96,10 @@ struct Request {
     // plp / plp_id [n_prompt - 1][gen.score_width()] the best pairs at position t
     std::vector<float> ptgt, plp;
     std::vector<int32_t> plp_id;
+    // an embedding request (rr_engine_submit_embed): max_new 0, one choice that never decodes; emb = the pooled,
+    // L2-normalised final-norm row of its last prompt position [hidden], written when its last piece has run
+    bool embed = false;
+    std::vector<float> emb;
 
     // Tokens of choice c a reader may see: all of a finished choice, else those no stop sequence can take back.
     int visible(int c) const { return (int)out[c].size() - (finish[c] < 0 ? hold[c] : 0); }
@@ -341,6 +345,9 @@ struct rr_engine {
     void* sc_ws = nullptr;
     int32_t *d_sc_in = nullptr, *h_sc_in = nullptr, *d_sc_id = nullptr, *h_sc_id = nullptr;
     float *d_sc_tlp = nullptr, *h_sc_tlp = nullptr, *d_sc_lp = nullptr, *h_sc_lp = nullptr;
+    // embeddings (ensure_embed_buffers, on the first chunk with an embedding row): the pooled rows [Bm][hidden] fp32,
+    // device and pinned
+    float *d_emb = nullptr, *h_emb = nullptr;
 
     // prefill working set
     int Tmax;
@@ -520,6 +527,18 @@ static int ensure_score_buffers(rr_engine* e) {
     e->h_sc_in = (int32_t*)h[0]; e->h_sc_tlp = (float*)h[1];
     e->h_sc_lp = (float*)h[2]; e->h_sc_id = (int32_t*)(e->h_sc_lp + T * LP_MAX_TOP);
     e->sc_logits = (float*)d[0];
+    return RR_OK;
+}
+
+// Caller holds gpu_mu.  The embedding buffers, allocated on the first chunk with an embedding row: 4 B x Bm x hidden on the
+// device and pinned.  An engine that never embeds allocates nothing.
+static int ensure_embed_buffers(rr_engine* e) {
+    if (e->h_emb) return RR_OK;
+    if (!e->d_emb) {
+        const int rc = dalloc(e, &e->d_emb, (size_t)e->Bm * e->d.hidden, false);
+        if (rc != RR_OK) return rc;
+    }
+    CK(cudaMallocHost(&e->h_emb, sizeof(float) * e->Bm * e->d.hidden));
     return RR_OK;
 }
 
@@ -798,39 +817,54 @@ struct PrefillScore {
 // leaves bf16(x * final_norm) and the partial sums of squares in pxn / p_rowss), then lm_head (OUT_ROWMAJOR_F32) and
 // launch_logprobs over the scoring rows only, in blocks of SCORE_ROWS rows of one sequence.  The tail rows were copied
 // before the full layer rewrites px, so what they compute does not change.
+// emb_seq[n_emb] (optional, needs ensure_embed_buffers): the sequences whose last token is an embedding row.  These rows
+// follow the tail rows through the trimmed last layer (rows nt .. nt + n_emb - 1 of the decode working set, each in its
+// sequence's slot), and rr_op_embed_pool turns their final-norm rows in e->xn into e->h_emb row k; lm_head, the logits tail,
+// activate_rows_kernel and the readback see the tail rows only.  Such a sequence needs no position after its prompt, so
+// its prompt may reach ctx_max.
 static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
                        int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
                        const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr,
-                       const PrefillScore* score = nullptr) {
+                       const PrefillScore* score = nullptr, int n_emb = 0, const int32_t* emb_seq = nullptr) {
     const rr_model_desc& d = e->d;
     const int T = seq_start[n_seqs];
     const int nt = tail ? tail->n : n_seqs;
+    const int ne = emb_seq ? n_emb : 0;
+    const int nr = nt + ne;                            // rows through the trimmed last layer
     const bool scoring = score && !score->seq.empty();
     const int n_score = scoring ? (int)score->tgt.size() : 0;
     if (scoring && (!e->sc_logits || n_score > T)) return RR_INTERNAL;
+    if (ne > 0 && !e->h_emb) return RR_INTERNAL;
     // the tail rows' slots and last tokens are listed apart (h_tsl / h_tlast) unless row j is sequence j in its own slot
-    bool fan = nt != n_seqs;
+    bool fan = nr != n_seqs;
     for (int j = 0; tail && !fan && j < nt; ++j) fan = tail->seq[j] != j || tail->slot[j] != slots[j];
+    for (int k = 0; !fan && k < ne; ++k) fan = emb_seq[k] != nt + k;
     int mode = tail ? tail->mode : 0;
-    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < 0 || nt > e->Bm) return RR_INVALID_ARGUMENT;
+    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < 0 || ne < 0 || nr > e->Bm) return RR_INVALID_ARGUMENT;
+    std::vector<char> is_emb(ne > 0 ? n_seqs : 0, 0);
+    for (int k = 0; k < ne; ++k) {
+        if (emb_seq[k] < 0 || emb_seq[k] >= n_seqs) return RR_INVALID_ARGUMENT;
+        is_emb[emb_seq[k]] = 1;
+    }
     cudaStream_t s = e->stream;
     // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n] (| pos0[n])
-    //                 (| tail_slot[nt] | tail_last[nt] with fan-out)
+    //                 (| tail_slot[nr] | tail_last[nr] with fan-out: the tail rows, then the embedding rows)
     int32_t* h = e->h_stage;
     int32_t *h_ids = h, *h_pos = h + T, *h_slt = h + 2 * T, *h_ss = h + 3 * T, *h_sl = h_ss + n_seqs + 1,
-            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs, *h_tsl = h_p0 + (pos0 ? n_seqs : 0), *h_tlast = h_tsl + nt;
+            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs, *h_tsl = h_p0 + (pos0 ? n_seqs : 0), *h_tlast = h_tsl + nr;
     int max_len = 0;
     memcpy(h_ids, ids, sizeof(int32_t) * T);
     for (int i = 0; i < n_seqs; ++i) {
         const int a = seq_start[i], b = seq_start[i + 1], p0 = pos0 ? pos0[i] : 0;
-        if (b <= a || p0 < 0 || p0 + b - a + 1 > e->o.ctx_max || slots[i] < 0 || slots[i] >= e->Bm) return RR_INVALID_ARGUMENT;
+        const int reach = p0 + b - a + (ne > 0 && is_emb[i] ? 0 : 1);       // + the first generated token's position
+        if (b <= a || p0 < 0 || reach > e->o.ctx_max || slots[i] < 0 || slots[i] >= e->Bm) return RR_INVALID_ARGUMENT;
         for (int t = a; t < b; ++t) { h_pos[t] = p0 + t - a; h_slt[t] = slots[i]; }
         h_ss[i] = a; h_sl[i] = slots[i]; h_last[i] = b - 1;
         if (pos0) h_p0[i] = p0;
         if (b - a > max_len) max_len = b - a;
     }
     h_ss[n_seqs] = T;
-    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1 + (fan ? 2 * nt : 0);
+    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1 + (fan ? 2 * nr : 0);
     uint64_t copy_tokens = 0;
     if (copies && copies->count > 0) {
         if (kv_copy_check(*copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
@@ -849,6 +883,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         fan_copies.n[c] = (pos0 ? pos0[q] : 0) + seq_start[q + 1] - seq_start[q];
         copy_tokens += fan_copies.n[c];
     }
+    for (int k = 0; fan && k < ne; ++k) { h_tsl[nt + k] = slots[emb_seq[k]]; h_tlast[nt + k] = h_last[emb_seq[k]]; }
     if (fan_copies.count && kv_copy_check(fan_copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
     // the chunk's parameter blocks, at the stride of its tail rows and of its largest bias count
     int max_bias = 0;
@@ -917,16 +952,17 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         ra.n_heads = d.n_heads; ra.n_kv_heads = d.n_kv_heads; ra.ctx_max = e->o.ctx_max; ra.theta = d.rope_theta;
         ra.table = e->rope_table; ra.head_dim = d.head_dim; ra.page_table = e->d_table; ra.pages_per_slot = e->pps;
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
-        if (nt == 0 && !scoring && l + 1 == d.n_layers) break;    // every layer's KV is written
+        if (nr == 0 && !scoring && l + 1 == d.n_layers) break;    // every layer's KV is written
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer operands, scale and TMA maps made at create (pf_attn_layer)
         pf_attn_chunk(&pa, e->pattn, p_ss, p_sl, pos0 ? p_p0 : nullptr, n_seqs, max_len);
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
-        if (l + 1 == d.n_layers && nt > 0) {
-            // ---- trimmed tail: n_seqs rows through O, MLP, final norm (decode-orientation kernels, decode buffers).  The
-            // unfused kernels even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
-            launch_pdl(gather_last_kernel, dim3(nt), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
+        if (l + 1 == d.n_layers && nr > 0) {
+            // ---- trimmed tail: the tail and embedding rows through O, MLP, final norm (decode-orientation kernels, decode
+            // buffers; every kernel is row-independent, so a row's bits do not depend on the others).  The unfused kernels
+            // even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
+            launch_pdl(gather_last_kernel, dim3(nr), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
                        p_tlast, e->attn_out, e->x, e->nq, d.hidden); ++nl;
-            if (enqueue_o_mlp(e, l, nt, s, &nl) != RR_OK) return RR_CUDA_ERROR;
+            if (enqueue_o_mlp(e, l, nr, s, &nl) != RR_OK) return RR_CUDA_ERROR;
         }
         if (l + 1 == d.n_layers && !scoring) break;    // a scoring chunk runs the whole last layer as well
         if (launch_rows(P.o[l]) != RR_OK) return RR_CUDA_ERROR; ++nl;
@@ -973,6 +1009,11 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
                    (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
         const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
         if (rc != RR_OK) return rc;
+    }
+    if (ne > 0) {               // the embedding rows' final-norm rows, pooled and read back
+        launch_embed_pool(e->xn + (size_t)nt * d.hidden, d.hidden, nullptr, ne, d.hidden, e->d_emb, d.hidden, s); ++nl;
+        CK(cudaMemcpyAsync(e->h_emb, e->d_emb, sizeof(float) * (size_t)ne * d.hidden, cudaMemcpyDeviceToHost, s));
+        e->st.d2h_bytes += sizeof(float) * (size_t)ne * d.hidden;
     }
     if (logits_host) {
         CK(cudaMemcpyAsync(logits_host, e->logits, sizeof(float) * (size_t)n_seqs * d.vocab, cudaMemcpyDeviceToHost, s));
@@ -1270,6 +1311,7 @@ static void worker_main(rr_engine* e) {
     KvCopyList* copies = new KvCopyList();
     std::vector<int32_t> tail_seq, tail_slot, tail_choice;      // the chunk's tail rows (PrefillTail), one per choice
     std::vector<const GenParams*> tail_gen;
+    std::vector<int32_t> emb_seq;                               // the chunk's embedding rows, after the tail rows
     PrefillScore score;                                         // the chunk's scoring rows, and for each entry
     std::vector<Request*> score_req;                            // its request and the position of its first row
     std::vector<int> score_pos;
@@ -1314,7 +1356,7 @@ static void worker_main(rr_engine* e) {
         }
         // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
         chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
-        tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear();
+        tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear(); emb_seq.clear();
         score.clear(); score_req.clear(); score_pos.clear();
         copies->count = 0;
         int active = 0, decoding = 0;                      // rows held / rows decoding (not the prompt in progress's)
@@ -1358,7 +1400,8 @@ static void worker_main(rr_engine* e) {
                 seq_start.push_back((int)ids.size());
                 resumed = true;
                 if (ip->n_done + n == (int)ip->prompt.size()) {     // its last piece: the tail rows of its choices
-                    for (int c = 0; c < ip->n_choices; ++c) {
+                    if (ip->embed) emb_seq.push_back(0);
+                    for (int c = 0; !ip->embed && c < ip->n_choices; ++c) {
                         tail_seq.push_back(0); tail_slot.push_back(ip->rows[c]); tail_choice.push_back(c);
                         tail_gen.push_back(&ip->gen);
                     }
@@ -1413,6 +1456,7 @@ static void worker_main(rr_engine* e) {
                     r->rows.push_back(b);
                     if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this prompt; set again once it succeeds
                     if (!last) continue;
+                    if (r->embed) { emb_seq.push_back((int)chunk.size()); continue; }
                     tail_seq.push_back((int)chunk.size()); tail_slot.push_back(b); tail_choice.push_back(c);
                     tail_gen.push_back(&r->gen);
                 }
@@ -1448,9 +1492,11 @@ static void worker_main(rr_engine* e) {
             if (rc == RR_OK && (chunk_mode & 4)) rc = ensure_pen_buffers(e);
             if (rc == RR_OK && (chunk_mode & 8)) rc = ensure_stop_buffers(e);
             if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
+            if (rc == RR_OK && !emb_seq.empty()) rc = ensure_embed_buffers(e);
             if (rc == RR_OK)
                 rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail, &score);
+                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail, &score,
+                                 (int)emb_seq.size(), emb_seq.data());
             const double t = now_s(e);
             std::lock_guard<std::mutex> lk(e->mu);
             for (size_t i = 0, o = 0; rc == RR_OK && i < score_req.size(); o += (size_t)score.rows[i++]) {
@@ -1463,12 +1509,13 @@ static void worker_main(rr_engine* e) {
                     memcpy(&r->plp_id[p * k], e->h_sc_id + src, sizeof(int32_t) * k);
                 }
             }
-            int j = 0;                                     // the request's first tail row
+            int j = 0, k = 0;                              // the request's first tail row / its embedding row
             for (size_t i = 0; i < chunk.size(); ++i) {
                 Request* r = chunk[i];
-                const int row0 = j;
+                const int row0 = j, emb_row = k;
                 const bool last = pos0[i] + seq_start[i + 1] - seq_start[i] == (int)r->prompt.size();
-                if (last) j += r->n_choices;
+                if (last && r->embed) ++k;
+                else if (last) j += r->n_choices;
                 if (rc != RR_OK) {
                     release_request(e, r, RR_INTERNAL, &notes);
                     continue;
@@ -1480,6 +1527,13 @@ static void worker_main(rr_engine* e) {
                     if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
                 }
                 r->t_first = t;
+                if (r->embed) {                            // done: its row is free at once, it never decodes
+                    const float* v = e->h_emb + (size_t)emb_row * e->d.hidden;
+                    r->emb.assign(v, v + e->d.hidden);
+                    r->finish[0] = 0;
+                    release_request(e, r, RR_OK, &notes);
+                    continue;
+                }
                 for (int c = 0; c < r->n_choices; ++c) {
                     if (take_token(e, r, c, row0 + c)) release_row(e, r, c);
                     else set_row_params(e, r->rows[c], r, c);
@@ -1753,7 +1807,7 @@ RR_API void rr_engine_destroy(rr_engine* e) {
     if (e->h_tok_lp) cudaFreeHost(e->h_tok_lp);
     if (e->h_stop) cudaFreeHost(e->h_stop);
     if (e->h_json_done) cudaFreeHost(e->h_json_done);
-    for (void* p : {(void*)e->h_sc_in, (void*)e->h_sc_tlp, (void*)e->h_sc_lp})
+    for (void* p : {(void*)e->h_sc_in, (void*)e->h_sc_tlp, (void*)e->h_sc_lp, (void*)e->h_emb})
         if (p) cudaFreeHost(p);
     for (const ParamBlocks* p : {&e->h_rows, &e->h_pf})
         for (char* b : p->blk)
@@ -1836,7 +1890,44 @@ static bool injected_failure(const rr_engine* e, uint64_t ticket) {
     return (double)(z >> 11) * (1.0 / 9007199254740992.0) < (double)e->o.fail_prob;
 }
 
+// Gives r its ticket and queues it (or fails it at once: fail_prob), then wakes the worker and runs the done hook.
+static void enqueue_request(rr_engine* e, Request* r, uint64_t* ticket) {
+    std::vector<DoneNote> notes;
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        r->ticket = e->next_ticket++;
+        r->t_submit = now_s(e);
+        e->table[r->ticket] = r;
+        *ticket = r->ticket;
+        if (injected_failure(e, r->ticket)) {
+            r->t_first = r->t_submit;
+            finish_request(e, r, RR_BACKEND_FAILED, &notes);
+        } else {
+            e->waiting.push_back(r);
+        }
+    }
+    e->cv_work.notify_one();
+    e->cv_done.notify_all();
+    run_hooks(e, notes);
+}
+
 namespace rr {
+int engine_submit_embed_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, uint64_t tag, uint64_t* ticket) {
+    if (!e || !prompt_ids || !ticket || n_prompt < 1 || n_prompt > e->o.ctx_max) return RR_INVALID_ARGUMENT;
+    if (choice_pages(e, n_prompt) > e->n_pages) return RR_INVALID_ARGUMENT;
+    for (int i = 0; i < n_prompt; ++i)
+        if (prompt_ids[i] < 0 || prompt_ids[i] >= e->d.vocab) return RR_INVALID_ARGUMENT;
+    Request* r = new (std::nothrow) Request();
+    if (!r) return RR_INTERNAL;
+    r->prompt.assign(prompt_ids, prompt_ids + n_prompt);
+    r->max_new = 0;
+    r->embed = true;
+    r->out.resize(1); r->finish.assign(1, -1); r->hold.assign(1, 0); r->lp.resize(1); r->lp_id.resize(1);
+    r->tag = tag;
+    enqueue_request(e, r, ticket);
+    return RR_OK;
+}
+
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, const GenParams& p, int n_choices) {
     if (!e || !prompt_ids || !ticket || n_prompt < 1 || max_new_tokens < 1) return RR_INVALID_ARGUMENT;
@@ -1870,31 +1961,16 @@ int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, 
         const size_t n = (size_t)n_prompt - 1, k = (size_t)p.score_width();
         r->ptgt.assign(n, 0.f); r->plp.assign(n * k, 0.f); r->plp_id.assign(n * k, 0);
     }
-    std::vector<DoneNote> notes;
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        r->ticket = e->next_ticket++;
-        r->t_submit = now_s(e);
-        e->table[r->ticket] = r;
-        *ticket = r->ticket;
-        if (injected_failure(e, r->ticket)) {
-            r->t_first = r->t_submit;
-            finish_request(e, r, RR_BACKEND_FAILED, &notes);
-        } else {
-            e->waiting.push_back(r);
-        }
-    }
-    e->cv_work.notify_one();
-    e->cv_done.notify_all();
-    run_hooks(e, notes);
+    enqueue_request(e, r, ticket);
     return RR_OK;
 }
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx) {
     std::lock_guard<std::mutex> lk(e->mu);
     e->hook = fn; e->hook_ctx = ctx;
 }
-int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens, int* ring) {
+int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens, int* ring, int* hidden) {
     if (!e) return RR_INVALID_ARGUMENT;
+    if (hidden) *hidden = e->d.hidden;
     if (kv_tokens) *kv_tokens = e->n_pages * KV_PAGE;
     if (ring) *ring = e->ring;
     if (max_batch) *max_batch = e->Bm;
@@ -1938,6 +2014,32 @@ RR_API int rr_engine_prompt_logprobs(rr_engine* e, uint64_t ticket, double timeo
             if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
             if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
             if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
+            return RR_OK;
+        }
+        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
+            it = e->table.find(ticket);
+            if (it == e->table.end() || !it->second->done) return it == e->table.end() ? RR_INVALID_ARGUMENT : RR_TIMEOUT;
+        }
+    }
+}
+
+RR_API int rr_engine_submit_embed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, uint64_t* ticket) {
+    return rr::engine_submit_embed_tagged(e, prompt_ids, n_prompt, 0, ticket);
+}
+
+RR_API int rr_engine_embedding(rr_engine* e, uint64_t ticket, double timeout_s, float* out, int capacity, int* dim_out) {
+    if (!e || !out || capacity < e->d.hidden) return RR_INVALID_ARGUMENT;
+    std::unique_lock<std::mutex> lk(e->mu);
+    const auto deadline = std::chrono::steady_clock::now() +
+                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
+    for (;;) {
+        auto it = e->table.find(ticket);
+        if (it == e->table.end() || !it->second->embed) return RR_INVALID_ARGUMENT;
+        const Request* r = it->second;
+        if (r->done) {
+            if (r->status != RR_OK) return r->status;
+            memcpy(out, r->emb.data(), sizeof(float) * r->emb.size());
+            if (dim_out) *dim_out = (int)r->emb.size();
             return RR_OK;
         }
         if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {

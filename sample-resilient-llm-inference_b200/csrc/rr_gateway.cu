@@ -57,6 +57,10 @@ struct GwReq {
     // (rr_engine_prompt_logprobs): [n_prompt - 1] and [n_prompt - 1][gen.score_width()]
     std::vector<float> ptgt, plp;
     std::vector<int32_t> plp_id;
+    // an embedding request (rr_gateway_submit_embed, max_new 0): the embedding of the engine that served it, read before
+    // its record was consumed (rr_engine_embedding), [that engine's hidden size]
+    bool embed = false;
+    std::vector<float> emb;
     int n_cached = 0;                 // rr_completion.n_cached of the engine that served it
     double t_submit = 0, t_admit = 0, t_first = 0, t_done = 0, t_eng_submit = 0;   // t_eng_submit: hand-off to the replica
     bool cancelled = false, cancel_as_failure = false, abandoned = false;
@@ -186,6 +190,7 @@ static void gw_settle(rr_gateway* g, GwReq* r, int status, int n_generated, int 
             r->tokens.clear(); r->n_tok.clear(); r->fin.clear();
             r->lp.clear(); r->lp_id.clear();
             r->ptgt.clear(); r->plp.clear(); r->plp_id.clear();     // the next replica scores the prompt again
+            r->emb.clear();                                          // and embeds it again
             r->n_cached = 0;
             g->st.failed_over++;
             g->pending.push_back(Pending{RR_EV_ADMIT, r, 0, 0});
@@ -202,6 +207,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     int max_new = 0;
     bool logprobs = false;
     size_t k = 1, n_ch = 1, n_score = 0, ks = 1;
+    bool embed = false;
     {
         std::lock_guard<std::mutex> lk(g->mu);
         auto it = g->table.find(tag);
@@ -214,6 +220,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         n_ch = (size_t)r->n_choices;
         if (r->gen.scores()) n_score = r->prompt.size() - 1;
         ks = (size_t)r->gen.score_width();
+        embed = r->embed;
     }
     // the prompt logprobs first: rr_engine_wait consumes the record
     std::vector<float> ptgt, plp;
@@ -222,6 +229,14 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
     if (eng && status == RR_OK && n_score > 0) {
         ptgt.resize(n_score); plp.resize(n_score * ks); plp_id.resize(n_score * ks);
         prc = rr_engine_prompt_logprobs(eng, eng_ticket, 0.001, ptgt.data(), plp.data(), plp_id.data());
+    }
+    std::vector<float> emb;
+    int erc = RR_INVALID_ARGUMENT;
+    if (eng && status == RR_OK && embed) {
+        int hidden = 0, dim = 0;
+        rr::engine_limits(eng, nullptr, nullptr, nullptr, nullptr, nullptr, &hidden);
+        emb.resize((size_t)hidden);
+        erc = rr_engine_embedding(eng, eng_ticket, 0.001, emb.data(), hidden, &dim);
     }
     // consume the engine's record (tokens, logprobs, timestamps); a cancelled request has none left
     rr_completion comp;
@@ -241,6 +256,7 @@ static void gw_on_done(void* ctx, uint64_t tag, uint64_t eng_ticket, int status,
         if (prc == RR_OK && wrc == RR_OK) {
             it->second->ptgt.swap(ptgt); it->second->plp.swap(plp); it->second->plp_id.swap(plp_id);
         }
+        if (erc == RR_OK && wrc == RR_OK) it->second->emb.swap(emb);
         gw_settle(g, it->second, status, n_generated, wrc, comp, toks.data(), n_toks.data(), fins.data(), lps.data(),
                   lp_ids.data());
     }
@@ -355,7 +371,9 @@ static void gw_dispatch(rr_gateway* g) {
             }
             uint64_t tk = 0;
             int src = RR_INTERNAL;
-            if (!cancelled && eng)
+            if (!cancelled && eng && r->embed)
+                src = rr::engine_submit_embed_tagged(eng, r->prompt.data(), (int)r->prompt.size(), id, &tk);
+            else if (!cancelled && eng)
                 src = rr::engine_submit_tagged(eng, r->prompt.data(), (int)r->prompt.size(), r->max_new, id, &tk, r->gen,
                                                r->n_choices);
             bool cancel_now = false;
@@ -453,9 +471,10 @@ RR_API int rr_gateway_set_now(rr_gateway* g, int64_t now_ms) {
     return RR_OK;
 }
 
-static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, int max_new, int n_choices) {
+// embed: an embedding request, max_new 0 (its prompt may fill the context window)
+static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, int max_new, int n_choices, bool embed) {
     if (group < 0 || group >= g->n_groups) return RR_NO_GROUP;
-    if (!ids || n_prompt < 1 || max_new < 1) return RR_INVALID_ARGUMENT;
+    if (!ids || n_prompt < 1 || max_new < (embed ? 0 : 1)) return RR_INVALID_ARGUMENT;
     if (n_choices < 1 || n_choices > g->min_rows) return RR_INVALID_ARGUMENT;     // every choice takes a decode row
     if (n_prompt + max_new > g->min_ctx) return RR_INVALID_ARGUMENT;   // -> HTTP 400, before any debit
     // every choice reserves whole 64-token KV pages, at most a windowed engine's ring, in each engine's pool
@@ -472,18 +491,19 @@ static int gw_check(rr_gateway* g, int group, const int32_t* ids, int n_prompt, 
 
 // p is checked (GenParams::set) against the smallest vocabulary, as prompt ids are: any engine of a fallback accepts it.
 static int gw_submit(rr_gateway* g, int group, const int32_t* prompt_ids, const int32_t* prompt_start, int n,
-                     int max_new_tokens, int declare_burst, const rr::GenParams& p, int n_choices, uint64_t* tickets) {
+                     int max_new_tokens, int declare_burst, const rr::GenParams& p, int n_choices, uint64_t* tickets,
+                     bool embed = false) {
     if (!g || !prompt_ids || !prompt_start || n < 1 || !tickets) return RR_INVALID_ARGUMENT;
     for (int i = 0; i < n; ++i) {
         const int rc = gw_check(g, group, prompt_ids + prompt_start[i], prompt_start[i + 1] - prompt_start[i], max_new_tokens,
-                                n_choices);
+                                n_choices, embed);
         if (rc != RR_OK) return rc;
     }
     std::vector<GwReq*> reqs((size_t)n);
     for (int i = 0; i < n; ++i) {
         GwReq* r = new (std::nothrow) GwReq();
         if (!r) { for (int j = 0; j < i; ++j) delete reqs[j]; return RR_INTERNAL; }
-        r->group = group; r->max_new = max_new_tokens; r->gen = p; r->n_choices = n_choices;
+        r->group = group; r->max_new = max_new_tokens; r->gen = p; r->n_choices = n_choices; r->embed = embed;
         r->prompt.assign(prompt_ids + prompt_start[i], prompt_ids + prompt_start[i + 1]);
         reqs[i] = r;
     }
@@ -551,6 +571,36 @@ RR_API int rr_gateway_prompt_logprobs(rr_gateway* g, uint64_t ticket, double tim
             if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
             if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
             if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
+            return RR_OK;
+        }
+        if (g->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
+            it = g->table.find(ticket);
+            if (it == g->table.end()) return RR_INVALID_ARGUMENT;
+            if (it->second->state != FINISHED) return RR_TIMEOUT;
+        }
+    }
+}
+
+RR_API int rr_gateway_submit_embed(rr_gateway* g, int group, const int32_t* prompt_ids, int n_prompt, uint64_t* ticket) {
+    if (!g) return RR_INVALID_ARGUMENT;
+    if (g->has_stub) return RR_INVALID_ARGUMENT;       // a mock replica has no hidden state to pool
+    const int32_t start[2] = {0, n_prompt};
+    return gw_submit(g, group, prompt_ids, start, 1, 0, 0, rr::GenParams(), 1, ticket, true);
+}
+
+RR_API int rr_gateway_embedding(rr_gateway* g, uint64_t ticket, double timeout_s, float* out, int capacity, int* dim_out) {
+    if (!g || !out) return RR_INVALID_ARGUMENT;
+    std::unique_lock<std::mutex> lk(g->mu);
+    const auto deadline = std::chrono::steady_clock::now() + std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
+    for (;;) {
+        auto it = g->table.find(ticket);
+        if (it == g->table.end() || !it->second->embed) return RR_INVALID_ARGUMENT;
+        const GwReq* r = it->second;
+        if (r->state == FINISHED) {
+            if (r->status != RR_OK) return r->status;
+            if ((size_t)capacity < r->emb.size()) return RR_INVALID_ARGUMENT;
+            memcpy(out, r->emb.data(), sizeof(float) * r->emb.size());
+            if (dim_out) *dim_out = (int)r->emb.size();
             return RR_OK;
         }
         if (g->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {

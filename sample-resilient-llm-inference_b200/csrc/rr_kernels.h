@@ -142,11 +142,14 @@ struct GenParams {
 // the tokens the choices return (a choice cut by a stop sequence counts what is left of it).
 int engine_submit_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, int max_new_tokens, uint64_t tag,
                          uint64_t* ticket, const GenParams& p, int n_choices);
+// An embedding request (rr_engine_submit_embed) with the done hook's `tag`; the hook reports 0 tokens.
+int engine_submit_embed_tagged(rr_engine* e, const int32_t* prompt_ids, int n_prompt, uint64_t tag, uint64_t* ticket);
 void engine_set_done_hook(rr_engine* e, EngineDoneHook fn, void* ctx);
 // kv_tokens: the KV pool (rr_engine_opts.kv_cache_tokens after its default is applied)
 // ring: the pages a windowed engine's ring request reserves per choice (0: no window, every choice reserves its reach)
+// hidden: the model's hidden size, the length of its embeddings
 int engine_limits(const rr_engine* e, int* ctx_max, int* vocab, int* max_batch, int* kv_tokens = nullptr,
-                  int* ring = nullptr);
+                  int* ring = nullptr, int* hidden = nullptr);
 int router_shape(const rr_router* r, int* n_deployments, int* n_groups);
 int router_dep_replica(const rr_router* r, int deployment);
 int router_strategy(const rr_router* r);
@@ -248,6 +251,11 @@ struct PartIn {
 
 void launch_embed(const int32_t* ids, const __nv_bfloat16* table, float* x, int rows, int hidden,
                   const int32_t* row_active, cudaStream_t st);
+// Embedding pool (rr_op_embed_pool): for i < n, out[i][0..hidden) = v / ||v||_2 with v = float(xn[rows ? rows[i] : i]),
+// the sum of squares in fp64 in a fixed order, each quotient in fp64 rounded once to fp32; a zero row gives zeros.  One CTA
+// per row, 16-byte loads (xn 16-byte aligned, ld % 8 == 0, hidden % 8 == 0).
+void launch_embed_pool(const __nv_bfloat16* xn, int ld, const int32_t* rows, int n, int hidden, float* out, int out_ld,
+                       cudaStream_t st);
 // x[row] (+)= sum_z part[z][row]; xn[row] = rmsnorm(x[row]) * w   (part.ptr may be null: norm only)
 // `zero` (optional): zero_n dependency counters reset by the kernel (the fused MLP kernel that follows it).
 void launch_add_rmsnorm(float* x, PartIn part, const __nv_bfloat16* w, __nv_bfloat16* xn, int rows,

@@ -254,6 +254,23 @@ class Engine:
                                                       lp.ctypes.data_as(f32), _p(ids)), "rr_engine_prompt_logprobs")
         return tgt, lp, ids
 
+    def submit_embedding(self, prompt_ids: Sequence[int]) -> int:
+        """An embedding request (rr_engine_submit_embed): the prompt is prefilled and its last position's final-norm row
+        pooled and L2-normalised; no token is generated.  Read it with embedding(), then finish with wait()."""
+        ids = _i32(prompt_ids)
+        t = C.c_uint64()
+        _lib.check(_lib.lib.rr_engine_submit_embed(self._h, _p(ids), len(ids), C.byref(t)), "rr_engine_submit_embed")
+        return t.value
+
+    def embedding(self, ticket: int, timeout: float = 0.0) -> np.ndarray:
+        """The embedding of a request from submit_embedding(), once it is done (the ticket stays for wait()): float32
+        [hidden].  Raises RRError when the request did not end RR_OK."""
+        out = np.zeros(self.spec.hidden, dtype=np.float32)
+        dim = C.c_int32()
+        _lib.check(_lib.lib.rr_engine_embedding(self._h, ticket, float(timeout), out.ctypes.data_as(C.POINTER(C.c_float)),
+                                                len(out), C.byref(dim)), "rr_engine_embedding")
+        return out[: dim.value]
+
     def wait(self, ticket: int, timeout: float = 0.0, max_tokens: int = 4096) -> CompletionRecord:
         c = _lib.Completion()
         nc = self._n.get(ticket, 1)

@@ -16,6 +16,7 @@ responses.  There is no Python/CPU implementation of the routing logic or the re
 """
 from __future__ import annotations
 
+import base64
 import codecs
 import ctypes as C
 import math
@@ -395,6 +396,64 @@ def check_text_completion(prompt: Any, max_tokens: Any = None, echo: Any = None,
                                  or not 0 <= logprobs <= MAX_COMPLETION_LOGPROBS):
         raise BadRequestError(f"`logprobs` must be an integer from 0 to {MAX_COMPLETION_LOGPROBS}")
     return prompts, logprobs
+
+
+MAX_EMBEDDING_INPUTS = 2048  # OpenAI's limit on the inputs of one /v1/embeddings request
+ENCODING_FORMATS = ("float", "base64")
+
+
+def check_embedding(input: Any, encoding_format: Any = None, dimensions: Any = None) -> Tuple[List[Any], str]:
+    """OpenAI's rules for the fields of a /v1/embeddings request -> (inputs, encoding format).  `input` takes OpenAI's
+    four forms: a string, an array of strings, an array of token ids or an array of arrays of ids; each element of
+    `inputs` is a non-empty string or a non-empty list of ids (their range is the caller's to check against the
+    vocabulary), at most 2048 of them.  encoding_format: "float" (None) or "base64".  dimensions: None or a positive
+    integer (the caller checks it against the model's hidden size).  Raises BadRequestError (HTTP 400) naming the field for
+    anything else."""
+    def is_id(v):
+        return isinstance(v, int) and not isinstance(v, bool)
+    if isinstance(input, str) and input:
+        inputs: List[Any] = [input]
+    elif isinstance(input, list) and input and all(isinstance(p, str) and p for p in input):
+        inputs = list(input)
+    elif isinstance(input, list) and input and all(is_id(t) for t in input):
+        inputs = [list(input)]
+    elif isinstance(input, list) and input and all(isinstance(p, list) and p and all(is_id(t) for t in p) for p in input):
+        inputs = [list(p) for p in input]
+    else:
+        raise BadRequestError("`input` must be a string, an array of strings, an array of token ids or an array of "
+                              "arrays of token ids, none of them empty")
+    if len(inputs) > MAX_EMBEDDING_INPUTS:
+        raise BadRequestError(f"`input` holds {len(inputs)} inputs: at most {MAX_EMBEDDING_INPUTS} are allowed")
+    fmt = "float" if encoding_format is None else encoding_format
+    if fmt not in ENCODING_FORMATS:
+        raise BadRequestError("`encoding_format` must be \"float\" or \"base64\"")
+    if dimensions is not None and (not is_id(dimensions) or dimensions < 1):
+        raise BadRequestError("`dimensions` must be a positive integer")
+    return inputs, fmt
+
+
+def encode_embedding(v: np.ndarray, encoding_format: str):
+    """One `data[i].embedding` of /v1/embeddings: a list of floats (each the exact value of its fp32 component), or with
+    "base64" the little-endian fp32 bytes, base64-encoded (what the OpenAI SDK asks for by default and decodes itself)."""
+    v = np.asarray(v, dtype=np.float32)
+    if encoding_format == "base64":
+        return base64.b64encode(v.astype("<f4").tobytes()).decode("ascii")
+    return [float(x) for x in v]
+
+
+@dataclass
+class EmbeddingResponse:
+    """A /v1/embeddings response (OpenAI `CreateEmbeddingResponse`)."""
+    model: str
+    data: List[Any]                      # per input, in order: its embedding (list of floats or a base64 string)
+    prompt_tokens: int
+    object: str = "list"
+
+    def model_dump(self) -> dict:
+        return {"object": self.object,
+                "data": [{"object": "embedding", "index": i, "embedding": e} for i, e in enumerate(self.data)],
+                "model": self.model,
+                "usage": {"prompt_tokens": self.prompt_tokens, "total_tokens": self.prompt_tokens}}
 
 
 _invalid_spans = threading.local()
@@ -1098,6 +1157,91 @@ class Router:
         yield from self.completion_stream(model, timeout=timeout, max_tokens=max_tokens, prompt_ids=ids,
                                           logprobs=True if lp is not None else None, top_logprobs=lp, **kw)
 
+    def embedding(self, model: str, input: Any, encoding_format: Optional[str] = None, dimensions: Optional[int] = None,
+                  timeout: Optional[float] = None, user: Optional[str] = None, **_ignored) -> EmbeddingResponse:
+        """OpenAI's /v1/embeddings (`client.embeddings.create`, litellm's `Router.embedding`): per input the last prompt
+        position's final-norm hidden state, L2-normalised, computed on the GPU (rr_gateway_submit_embed), as decoder
+        embedding models such as e5-mistral-7b-instruct pool.  input: a string, an array of strings, an array of token
+        ids or an array of arrays of ids (check_embedding); a string is BOS plus its bytes (no chat template).  Each input
+        is its own gateway request (rpm and tpm count it like a prompt), all submitted together; on the first error the
+        rest are cancelled and that error is raised.  encoding_format "float" (default) or "base64" (little-endian fp32).
+        dimensions: absent or the model's hidden size (no truncation).  usage counts the inputs' tokens.
+        Refused with BadRequestError: anything check_embedding refuses, a token id outside the vocabulary, an input beyond
+        the context window or the KV cache, `dimensions` other than the hidden size, and mock replicas (no hidden state)."""
+        inputs, fmt = check_embedding(input, encoding_format, dimensions)
+        g = self.cfg.group_index(model)
+        if g < 0:
+            raise BadRequestError(f"Invalid model name passed in model={model}")
+        if any(isinstance(b, StubBackend) for b in self.backends.values()):
+            raise BadRequestError("embeddings are not available: the backends of this router are not model replicas")
+        hidden = {b.engine.spec.hidden for b in self.backends.values() if isinstance(b, EngineBackend)}
+        if dimensions is not None and hidden != {dimensions}:
+            raise BadRequestError(f"`dimensions` must be the model's hidden size {sorted(hidden)}: embeddings are not "
+                                  f"truncated")
+        vocab = self._vocab()
+        ids = []
+        for p in inputs:
+            if isinstance(p, str):
+                ids.append([int(t) for t in tokenize(p, vocab)])
+            elif any(not 0 <= t < vocab for t in p):
+                raise BadRequestError(f"`input` holds a token id outside the vocabulary [0, {vocab})")
+            else:
+                ids.append(list(p))
+        ctx = self._limits()[0]
+        for i, p in enumerate(ids):
+            kv = _kv_refusal(self.backends, len(p), 0, 1)
+            if len(p) > ctx or kv is not None:
+                raise BadRequestError(f"`input` {i} ({len(p)} tokens) exceeds the context window ({ctx} tokens) or the "
+                                      f"KV cache of the deployment")
+        gw = self._gateway()
+        tickets: List[int] = []
+        try:
+            for p in ids:
+                a = np.ascontiguousarray(np.asarray(p, dtype=np.int32))
+                if self._custom_clock:
+                    _lib.lib.rr_gateway_set_now(gw, self.now_ms())
+                t = C.c_uint64()
+                rc = _lib.lib.rr_gateway_submit_embed(gw, g, a.ctypes.data_as(C.POINTER(C.c_int32)), len(a), C.byref(t))
+                if rc != 0:
+                    raise self._invalid(len(a)) if rc == 4 else self._gw_error(rc, model)
+                tickets.append(t.value)
+        except APIError:
+            for t in tickets:
+                _lib.lib.rr_gateway_cancel(gw, t, 0)
+            raise
+        data, label = [], ""
+        for i, t in enumerate(tickets):
+            try:
+                v, label = self._collect_embedding(gw, model, t, max(hidden, default=1), timeout)
+            except APIError:
+                for u in tickets[i + 1:]:
+                    _lib.lib.rr_gateway_cancel(gw, u, 0)
+                raise
+            data.append(encode_embedding(v, fmt))
+        return EmbeddingResponse(label, data, sum(len(p) for p in ids))
+
+    def _collect_embedding(self, gw, model, ticket, capacity, timeout) -> Tuple[np.ndarray, str]:
+        """One input of embedding(): its vector (read before the wait consumes the ticket) and the served model's label.
+        Raises the request's APIError; a client-side timeout cancels it as a failure."""
+        v = np.zeros(capacity, dtype=np.float32)
+        dim = C.c_int32()
+        rc = _lib.lib.rr_gateway_embedding(gw, ticket, float(timeout or 0.0), v.ctypes.data_as(C.POINTER(C.c_float)),
+                                           capacity, C.byref(dim))
+        res = _lib.GatewayResult()
+        if rc == 6:
+            _lib.lib.rr_gateway_cancel(gw, ticket, 1)
+            raise self._gw_error(6, model, res, timeout)
+        wrc = _lib.lib.rr_gateway_wait(gw, ticket, 1.0, C.byref(res), None, 0, None, None, None, None)
+        if wrc == 6:
+            _lib.lib.rr_gateway_cancel(gw, ticket, 1)
+        for code in (wrc, rc):
+            if code != 0:
+                raise self._gw_error(code, model, res, timeout)
+        v = v[: dim.value]
+        if not np.isfinite(v).all():
+            raise APIError(f"the embedding of deployment {res.deployment} holds a non-finite value (model={model})")
+        return v, self.cfg.deployments[res.deployment].response_model
+
 
 # ---------------------------------------------------------------- OpenAI-SDK-shaped facade
 class _Completions:
@@ -1122,6 +1266,14 @@ class _TextCompletions:
         return self._r.text_completion(model=model, prompt=prompt, **kw)
 
 
+class _Embeddings:
+    def __init__(self, router: Router):
+        self._r = router
+
+    def create(self, model: str, input: Any, **kw) -> EmbeddingResponse:
+        return self._r.embedding(model=model, input=input, **kw)
+
+
 class OpenAI:
     """In-process stand-in for `openai.OpenAI(api_key=..., base_url=http://0.0.0.0:<port>)`
     (reference src/demo_load_balancing.py:24): same `client.chat.completions.create(...)` call."""
@@ -1131,3 +1283,4 @@ class OpenAI:
         self.base_url = base_url
         self.chat = _Chat(router)
         self.completions = _TextCompletions(router)
+        self.embeddings = _Embeddings(router)

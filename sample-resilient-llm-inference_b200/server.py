@@ -16,8 +16,8 @@ from typing import Dict, Optional
 from .config import RouterConfig, load_config
 from .models import resolve_spec
 from .router import (APIError, APITimeoutError, BadRequestError, EngineBackend, RateLimitError, Router,
-                     StubBackend, check_logprobs, check_n, check_penalties, check_response_format, check_sampling,
-                     check_stop, check_text_completion)
+                     StubBackend, check_embedding, check_logprobs, check_n, check_penalties, check_response_format,
+                     check_sampling, check_stop, check_text_completion)
 
 
 def _error_body(e: APIError, typ: str) -> dict:
@@ -216,6 +216,31 @@ def create_app(router: Router):
 
     app.add_api_route("/completions", text_completions, methods=["POST"])
     app.add_api_route("/v1/completions", text_completions, methods=["POST"])
+
+    async def embeddings(request: Request):
+        """OpenAI's /v1/embeddings (Router.embedding): `input` in any of its four forms, `encoding_format` "float" or
+        "base64" (the OpenAI SDK's default), `dimensions` absent or the hidden size."""
+        try:
+            body = await request.json()
+        except Exception:
+            return JSONResponse(_error_body(BadRequestError("invalid JSON body"), "invalid_request_error"), 400)
+        model = body.get("model") if isinstance(body, dict) else None
+        if not isinstance(model, str) or "input" not in body:
+            return JSONResponse(_error_body(BadRequestError("`model` and `input` are required"),
+                                            "invalid_request_error"), 400)
+        try:
+            check_embedding(body["input"], body.get("encoding_format"), body.get("dimensions"))
+        except BadRequestError as e:
+            return _error(e)
+        kw = {k: body[k] for k in ("encoding_format", "dimensions", "timeout", "user") if body.get(k) is not None}
+        try:
+            resp = await run_in_threadpool(router.embedding, model=model, input=body["input"], **kw)
+            return JSONResponse(resp.model_dump())
+        except APIError as e:
+            return _error(e)
+
+    app.add_api_route("/embeddings", embeddings, methods=["POST"])
+    app.add_api_route("/v1/embeddings", embeddings, methods=["POST"])
 
     @app.get("/health")
     async def health():
