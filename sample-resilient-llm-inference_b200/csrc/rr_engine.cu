@@ -778,138 +778,145 @@ static int init_pf_plans(rr_engine* e) {
     return RR_OK;
 }
 
-// The tail rows of a prefill chunk: the rows the trimmed last layer, lm_head and the logits tail run on, one per choice of
-// each request.  Row j reads the last token of sequence seq[j], decodes in slot[j] and is choice choice[j] of the request
-// whose parameters are gen[j]; mode = the step_mode bits over gen.  Rows of the same sequence in other slots than the
-// sequence's get its prompt KV copied there.  A sequence may have no tail row (a piece of a long prompt that is not its
-// last).  Without a tail, row i is sequence i in slots[i], plain greedy.
-struct PrefillTail {
-    int n = 0;
-    const int32_t *seq = nullptr, *slot = nullptr, *choice = nullptr;
-    const GenParams* const* gen = nullptr;
-    int mode = 0;
+// One prefill chunk: the tokens of its sequences back to back, one record per sequence, the cached prefixes to copy
+// between slots before its first layer (prefix caching) and the index epoch it was admitted under.  A sequence is the
+// piece [pos0, pos0 + len) of a prompt, prefilled into its slot, which holds positions [0, pos0) already.  The rows after
+// attention follow from the records; add() numbers them in sequence order:
+//   tail rows: one per choice of a last piece, row `row` + c for choice c, decoding in r->rows[c] (a sequence without a
+//              request: one plain greedy row in its own slot);
+//   embedding rows: one per last piece of an embedding request (it has no tail rows), after every tail row: n_tail + `row`;
+//   scoring rows (prompt logprobs): the rows of a scoring request's piece that predict a prompt token, from `score_row` on.
+struct Chunk {
+    struct Seq {
+        Request* r;                    // null: a sequence of rr_engine_prefill
+        int slot, pos0, start, len;    // its tokens are ids[start, start + len)
+        bool last;                     // the prompt's last piece
+        int row, score_row;
+        bool embeds() const { return last && r && r->embed; }
+        int n_tail() const { return !last || embeds() ? 0 : r ? r->n_choices : 1; }
+        int score_rows() const {
+            return r && r->gen.scores() ? std::max(0, std::min(len, (int)r->prompt.size() - 1 - pos0)) : 0;
+        }
+        const GenParams& gen() const { static const GenParams plain; return r ? r->gen : plain; }
+    };
+    std::vector<int32_t> ids;
+    std::vector<Seq> seqs;
+    KvCopyList copies;
+    uint64_t epoch = 0;
+    bool has_pos0 = false;             // attention reads seq_pos0: prefix caching is on or the chunk continues a prompt
+    int n_tail = 0, n_emb = 0, n_score = 0;
+    int mode = 0;                      // the step_mode bits of the last pieces' requests
+
+    void reset(uint64_t ep, bool pos0) {
+        ids.clear(); seqs.clear(); copies.count = 0;
+        epoch = ep; has_pos0 = pos0;
+        n_tail = n_emb = n_score = mode = 0;
+    }
+    void add(Request* r, int slot, int pos0, const int32_t* tok, int n, bool last) {
+        Seq q{r, slot, pos0, (int)ids.size(), n, last, 0, n_score};
+        ids.insert(ids.end(), tok, tok + std::max(n, 0));      // n < 1: run_prefill refuses the chunk
+        if (q.embeds()) q.row = n_emb++;
+        else if (last) { q.row = n_tail; n_tail += q.n_tail(); }
+        n_score += q.score_rows();
+        if (last && r) mode |= step_mode(r->gen);
+        seqs.push_back(q);
+    }
 };
 
-// The prompt rows of a prefill chunk that score (prompt logprobs), one entry per scoring sequence: the first rows[i] rows
-// of sequence seq[i], row j against the next prompt token tgt[o + j] (o = the rows of the entries before), with top[i]
-// pairs (prompt_top).  run_prefill leaves row o + j's results in h_sc_tlp[o + j] and h_sc_lp / h_sc_id [o + j][LP_MAX_TOP].
-struct PrefillScore {
-    std::vector<int> seq, rows, top;
-    std::vector<int32_t> tgt;
-    void clear() { seq.clear(); rows.clear(); top.clear(); tgt.clear(); }
-};
-
-// ids: T tokens of n_seqs prompts; slots[n_seqs]. Leaves first tokens in e->p_first (device) and
-// activates the rows. Caller holds gpu_mu.
-// Prefix caching: pos0[n_seqs] (optional) = positions already in the slot, so sequence i's tokens are the prompt from
-// position pos0[i] on; copies (optional) = the prefixes to copy between slots first, in one launch.
-// tail (optional): the tail rows and their request parameters.  Stop sequences are matched over the first token (needs
-// ensure_stop_buffers; results in e->h_stop row j).  A JSON-mode row picks its first token from the initial state's mask
-// and leaves its state in its slot (needs ensure_json_buffers; done in e->h_json_done row j).  Only a logit bias applies (penalties count generated
-// tokens only, so the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position
-// pos0 + the sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's
-// logprobs in e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other
-// slots, one launch after the last layer copies positions [0, pos0 + its length) of its slot to each of them.
-// A chunk without tail rows (tail->n == 0) stops after the last layer's QKV projection and KV append: nothing after reads
+// Runs chunk c.  Caller holds gpu_mu.  Leaves first tokens in e->p_first (device) and activates the tail rows.
+// Prefix caching: sequence i's tokens are the prompt from position pos0 on; c.copies run first, in one launch.
+// Tail rows: stop sequences are matched over the first token (needs ensure_stop_buffers; results in e->h_stop row j).  A
+// JSON-mode row picks its first token from the initial state's mask and leaves its state in its slot (needs
+// ensure_json_buffers; done in e->h_json_done row j).  Only a logit bias applies (penalties count generated tokens only, so
+// the first token has none; needs ensure_pen_buffers).  A sampled row draws its first token at position pos0 + the
+// sequence's length (the prompt length) with its choice's seed.  A logprobs row j also gets its first token's logprobs in
+// e->h_lp / e->h_lp_id row j, and if sampled its own logprob in h_tok_lp.  When a sequence has rows in other slots, one
+// launch after the last layer copies positions [0, pos0 + its length) of its slot to each of them.
+// A chunk without tail or embedding rows stops after the last layer's QKV projection and KV append: nothing after reads
 // its other outputs, and nothing is read back -- unless it scores.
-// score (optional, needs ensure_score_buffers): a scoring chunk.  After the tail rows are gathered and have run through the
-// decode kernels, the last layer's O, gate/up and down GEMMs run over all T rows in prefill orientation (its down GEMM
-// leaves bf16(x * final_norm) and the partial sums of squares in pxn / p_rowss), then lm_head (OUT_ROWMAJOR_F32) and
+// Scoring rows (needs ensure_score_buffers): after the tail rows are gathered and have run through the decode kernels, the
+// last layer's O, gate/up and down GEMMs run over all T rows in prefill orientation (its down GEMM leaves
+// bf16(x * final_norm) and the partial sums of squares in pxn / p_rowss), then lm_head (OUT_ROWMAJOR_F32) and
 // launch_logprobs over the scoring rows only, in blocks of SCORE_ROWS rows of one sequence.  The tail rows were copied
-// before the full layer rewrites px, so what they compute does not change.
-// emb_seq[n_emb] (optional, needs ensure_embed_buffers): the sequences whose last token is an embedding row.  These rows
-// follow the tail rows through the trimmed last layer (rows nt .. nt + n_emb - 1 of the decode working set, each in its
-// sequence's slot), and rr_op_embed_pool turns their final-norm rows in e->xn into e->h_emb row k; lm_head, the logits tail,
+// before the full layer rewrites px, so what they compute does not change.  Scoring row o's results are left in
+// h_sc_tlp[o] and h_sc_lp / h_sc_id [o][LP_MAX_TOP].
+// Embedding rows (needs ensure_embed_buffers) follow the tail rows through the trimmed last layer, each in its sequence's
+// slot, and rr_op_embed_pool turns their final-norm rows in e->xn into e->h_emb row `row`; lm_head, the logits tail,
 // activate_rows_kernel and the readback see the tail rows only.  Such a sequence needs no position after its prompt, so
 // its prompt may reach ctx_max.
-static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_start, const int32_t* slots,
-                       int n_seqs, int32_t* first_tok_host, float* logits_host, const int32_t* pos0 = nullptr,
-                       const KvCopyList* copies = nullptr, const PrefillTail* tail = nullptr,
-                       const PrefillScore* score = nullptr, int n_emb = 0, const int32_t* emb_seq = nullptr) {
+static int run_prefill(rr_engine* e, const Chunk& c, int32_t* first_tok_host, float* logits_host) {
     const rr_model_desc& d = e->d;
-    const int T = seq_start[n_seqs];
-    const int nt = tail ? tail->n : n_seqs;
-    const int ne = emb_seq ? n_emb : 0;
-    const int nr = nt + ne;                            // rows through the trimmed last layer
-    const bool scoring = score && !score->seq.empty();
-    const int n_score = scoring ? (int)score->tgt.size() : 0;
-    if (scoring && (!e->sc_logits || n_score > T)) return RR_INTERNAL;
+    const int T = (int)c.ids.size(), n_seqs = (int)c.seqs.size();
+    const int nt = c.n_tail, ne = c.n_emb, nr = nt + ne;       // rows through the trimmed last layer
+    const int n_score = c.n_score;
+    const bool scoring = n_score > 0;
+    if (scoring && !e->sc_logits) return RR_INTERNAL;
     if (ne > 0 && !e->h_emb) return RR_INTERNAL;
-    // the tail rows' slots and last tokens are listed apart (h_tsl / h_tlast) unless row j is sequence j in its own slot
-    bool fan = nr != n_seqs;
-    for (int j = 0; tail && !fan && j < nt; ++j) fan = tail->seq[j] != j || tail->slot[j] != slots[j];
-    for (int k = 0; !fan && k < ne; ++k) fan = emb_seq[k] != nt + k;
-    int mode = tail ? tail->mode : 0;
-    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nt < 0 || ne < 0 || nr > e->Bm) return RR_INVALID_ARGUMENT;
-    std::vector<char> is_emb(ne > 0 ? n_seqs : 0, 0);
-    for (int k = 0; k < ne; ++k) {
-        if (emb_seq[k] < 0 || emb_seq[k] >= n_seqs) return RR_INVALID_ARGUMENT;
-        is_emb[emb_seq[k]] = 1;
-    }
+    if (T <= 0 || T > e->Tmax || n_seqs > e->Bm || nr > e->Bm) return RR_INVALID_ARGUMENT;
     cudaStream_t s = e->stream;
     // pinned staging: ids[T] | pos[T] | slot_tok[T] | seq_start[n+1] | seq_slot[n] | last[n] (| pos0[n])
-    //                 (| tail_slot[nr] | tail_last[nr] with fan-out: the tail rows, then the embedding rows)
+    //                 | tail_slot[nr] | tail_last[nr] (the tail rows, then the embedding rows)
+    // The last two are uploaded only with fan-out: unless row i is sequence i in its own slot.
     int32_t* h = e->h_stage;
     int32_t *h_ids = h, *h_pos = h + T, *h_slt = h + 2 * T, *h_ss = h + 3 * T, *h_sl = h_ss + n_seqs + 1,
-            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs, *h_tsl = h_p0 + (pos0 ? n_seqs : 0), *h_tlast = h_tsl + nr;
-    int max_len = 0;
-    memcpy(h_ids, ids, sizeof(int32_t) * T);
-    for (int i = 0; i < n_seqs; ++i) {
-        const int a = seq_start[i], b = seq_start[i + 1], p0 = pos0 ? pos0[i] : 0;
-        const int reach = p0 + b - a + (ne > 0 && is_emb[i] ? 0 : 1);       // + the first generated token's position
-        if (b <= a || p0 < 0 || reach > e->o.ctx_max || slots[i] < 0 || slots[i] >= e->Bm) return RR_INVALID_ARGUMENT;
-        for (int t = a; t < b; ++t) { h_pos[t] = p0 + t - a; h_slt[t] = slots[i]; }
-        h_ss[i] = a; h_sl[i] = slots[i]; h_last[i] = b - 1;
-        if (pos0) h_p0[i] = p0;
-        if (b - a > max_len) max_len = b - a;
-    }
-    h_ss[n_seqs] = T;
-    const size_t n_ints = (size_t)3 * T + (pos0 ? 4 : 3) * n_seqs + 1 + (fan ? 2 * nr : 0);
+            *h_last = h_sl + n_seqs, *h_p0 = h_last + n_seqs, *h_tsl = h_p0 + (c.has_pos0 ? n_seqs : 0),
+            *h_tlast = h_tsl + nr;
+    bool fan = nr != n_seqs;
+    int max_len = 0, max_bias = 0;
     uint64_t copy_tokens = 0;
-    if (copies && copies->count > 0) {
-        if (kv_copy_check(*copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
-        for (int i = 0; i < copies->count; ++i) copy_tokens += copies->n[i];
-    }
     KvCopyList fan_copies;                             // the fan-out: source slot -> the slot of each further tail row
     fan_copies.count = 0;
-    for (int j = 0; tail && j < nt; ++j) {
-        const int q = tail->seq[j], sl = tail->slot[j];
-        if (q < 0 || q >= n_seqs || sl < 0 || sl >= e->Bm) return RR_INVALID_ARGUMENT;
-        if (!fan) continue;
-        h_tsl[j] = sl; h_tlast[j] = h_last[q];
-        if (sl == slots[q]) continue;
-        const int c = fan_copies.count++;              // < nt <= Bm <= KV_COPY_MAX
-        fan_copies.src[c] = slots[q]; fan_copies.dst[c] = sl;
-        fan_copies.n[c] = (pos0 ? pos0[q] : 0) + seq_start[q + 1] - seq_start[q];
-        copy_tokens += fan_copies.n[c];
+    memcpy(h_ids, c.ids.data(), sizeof(int32_t) * T);
+    for (int i = 0; i < n_seqs; ++i) {
+        const Chunk::Seq& q = c.seqs[i];
+        const int a = q.start, b = q.start + q.len;
+        const int reach = q.pos0 + q.len + (q.embeds() ? 0 : 1);       // + the first generated token's position
+        if (q.len < 1 || q.pos0 < 0 || reach > e->o.ctx_max || q.slot < 0 || q.slot >= e->Bm) return RR_INVALID_ARGUMENT;
+        for (int t = a; t < b; ++t) { h_pos[t] = q.pos0 + t - a; h_slt[t] = q.slot; }
+        h_ss[i] = a; h_sl[i] = q.slot; h_last[i] = b - 1;
+        if (c.has_pos0) h_p0[i] = q.pos0;
+        max_len = std::max(max_len, q.len);
+        if (q.embeds()) {
+            h_tsl[nt + q.row] = q.slot; h_tlast[nt + q.row] = b - 1;
+            fan = fan || nt + q.row != i;
+        }
+        for (int ch = 0; ch < q.n_tail(); ++ch) {
+            const int j = q.row + ch, sl = q.r ? q.r->rows[ch] : q.slot;
+            h_tsl[j] = sl; h_tlast[j] = b - 1;
+            fan = fan || j != i || sl != q.slot;
+            max_bias = std::max(max_bias, (int)q.gen().bias_id.size());
+            if (sl == q.slot) continue;
+            const int k = fan_copies.count++;          // < nt <= Bm <= KV_COPY_MAX
+            fan_copies.src[k] = q.slot; fan_copies.dst[k] = sl; fan_copies.n[k] = q.pos0 + q.len;
+            copy_tokens += fan_copies.n[k];
+        }
     }
-    for (int k = 0; fan && k < ne; ++k) { h_tsl[nt + k] = slots[emb_seq[k]]; h_tlast[nt + k] = h_last[emb_seq[k]]; }
+    h_ss[n_seqs] = T;
+    const size_t n_ints = (size_t)3 * T + (c.has_pos0 ? 4 : 3) * n_seqs + 1 + (fan ? 2 * nr : 0);
+    if (c.copies.count > 0) {
+        if (kv_copy_check(c.copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
+        for (int i = 0; i < c.copies.count; ++i) copy_tokens += c.copies.n[i];
+    }
     if (fan_copies.count && kv_copy_check(fan_copies, e->Bm, e->o.ctx_max) != RR_OK) return RR_INVALID_ARGUMENT;
     // the chunk's parameter blocks, at the stride of its tail rows and of its largest bias count
-    int max_bias = 0;
-    for (int j = 0; (mode & 4) && j < nt; ++j) max_bias = std::max(max_bias, (int)tail->gen[j]->bias_id.size());
+    int mode = c.mode;
     if (max_bias == 0) mode &= ~4;
     else if (!e->d_pf.blk[2]) return RR_INTERNAL;
     if ((mode & 8) && !e->d_pf.blk[3]) return RR_INTERNAL;
     if ((mode & 16) && !e->d_pf.blk[4]) return RR_INTERNAL;
     const ParamBlocks hp = e->h_pf.at(nt, max_bias), dp = e->d_pf.at(nt, max_bias);
-    for (int j = 0; mode && j < nt; ++j) {
-        const int q = tail->seq[j];
-        hp.put_row(j, *tail->gen[j], tail->choice[j], (pos0 ? pos0[q] : 0) + seq_start[q + 1] - seq_start[q], 0.f, 0.f,
-                   0);
-    }
+    for (const Chunk::Seq& q : c.seqs)
+        for (int ch = 0; mode && ch < q.n_tail(); ++ch) hp.put_row(q.row + ch, q.gen(), ch, q.pos0 + q.len, 0.f, 0.f, 0);
     CK(cudaEventRecord(e->ev0, s));
     CK(cudaMemcpyAsync(e->p_ids, h, n_ints * sizeof(int32_t), cudaMemcpyHostToDevice, s));
     e->st.h2d_bytes += n_ints * sizeof(int32_t);
     CK(hp.upload(dp, mode, s, &e->st.h2d_bytes));
     if (scoring) {              // targets | prompt_top per scoring row
-        for (size_t i = 0, o = 0; i < score->seq.size(); o += (size_t)score->rows[i++]) {
-            const int q = score->seq[i];
-            if (q < 0 || q >= n_seqs || score->rows[i] < 1 || score->rows[i] > seq_start[q + 1] - seq_start[q])
-                return RR_INVALID_ARGUMENT;
-            for (int j = 0; j < score->rows[i]; ++j) e->h_sc_in[e->Tmax + o + j] = score->top[i];
-        }
-        memcpy(e->h_sc_in, score->tgt.data(), sizeof(int32_t) * n_score);
+        for (const Chunk::Seq& q : c.seqs)
+            for (int j = 0; j < q.score_rows(); ++j) {
+                e->h_sc_in[q.score_row + j] = q.r->prompt[q.pos0 + 1 + j];
+                e->h_sc_in[e->Tmax + q.score_row + j] = q.r->gen.prompt_top;
+            }
         for (int half = 0; half < 2; ++half)
             CK(cudaMemcpyAsync(e->d_sc_in + half * e->Tmax, e->h_sc_in + half * e->Tmax, sizeof(int32_t) * n_score,
                                cudaMemcpyHostToDevice, s));
@@ -923,9 +930,9 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     rr_engine::PfPlans& P = e->pf;
     auto launch_rows = [&](const GemmPlan& pl, bool pdl = true) { GemmPlan q = pl; q.rowsA = T; return gemm_launch(q, s, pdl); };
     uint64_t nl = 0;
-    if (copies && copies->count > 0) {   // cached prefixes of busy slots into this chunk's slots, before any layer reads them
+    if (c.copies.count > 0) {   // cached prefixes of busy slots into this chunk's slots, before any layer reads them
         if (launch_kv_copy(e->kcache, e->vcache, d.n_layers, (long long)e->n_pages * d.n_kv_heads * KV_PAGE, d.n_kv_heads,
-                           e->o.ctx_max, e->d_table, e->pps, *copies, s) != RR_OK)
+                           e->o.ctx_max, e->d_table, e->pps, c.copies, s) != RR_OK)
             return RR_CUDA_ERROR;
         ++nl;
     }
@@ -954,7 +961,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
         if (!e->fuse_rope_pf) { launch_rope_kv(ra, s); ++nl; }
         if (nr == 0 && !scoring && l + 1 == d.n_layers) break;    // every layer's KV is written
         PrefillAttnArgs pa = e->pf_attn[l];          // per-layer operands, scale and TMA maps made at create (pf_attn_layer)
-        pf_attn_chunk(&pa, e->pattn, p_ss, p_sl, pos0 ? p_p0 : nullptr, n_seqs, max_len);
+        pf_attn_chunk(&pa, e->pattn, p_ss, p_sl, c.has_pos0 ? p_p0 : nullptr, n_seqs, max_len);
         if (launch_prefill_attn(pa, s) != RR_OK) return RR_CUDA_ERROR; ++nl;
         if (l + 1 == d.n_layers && nr > 0) {
             // ---- trimmed tail: the tail and embedding rows through O, MLP, final norm (decode-orientation kernels, decode
@@ -972,11 +979,10 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     }
     if (scoring) {              // lm_head and log-softmax over the scoring rows, SCORE_ROWS rows of one sequence at a time
         const int S = std::min(SCORE_ROWS, e->Tmax), V = d.vocab;
-        int o = 0;
-        for (size_t i = 0; i < score->seq.size(); ++i) {
-            const int r0 = seq_start[score->seq[i]];
-            for (int b = 0; b < score->rows[i]; b += S) {
-                const int nb = std::min(S, score->rows[i] - b);
+        for (const Chunk::Seq& q : c.seqs) {
+            const int r0 = q.start;
+            for (int b = 0; b < q.score_rows(); b += S) {
+                const int nb = std::min(S, q.score_rows() - b), o = q.score_row + b;
                 GemmPlan hd;
                 if (gemm_plan_init(&hd, e->pxn + (size_t)(r0 + b) * d.hidden, nb, d.hidden, e->lm_head, V, d.hidden, d.hidden,
                                    e->sc_logits, V, 0, 1, OUT_ROWMAJOR_F32, PF_BN) != RR_OK)
@@ -987,7 +993,6 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
                                 e->d_sc_lp + (size_t)o * LP_MAX_TOP, e->d_sc_id + (size_t)o * LP_MAX_TOP, s, e->d_sc_in + o,
                                 e->d_sc_tlp + o);
                 nl += LP_LAUNCHES;
-                o += nb;
             }
         }
         const size_t n = (size_t)n_score * LP_MAX_TOP;
@@ -1029,8 +1034,7 @@ static int run_prefill(rr_engine* e, const int32_t* ids, const int32_t* seq_star
     e->st.kernel_launches += nl;
     for (int j = 0; j < nt; ++j) {
         if (first_tok_host) first_tok_host[j] = e->h_tok[j];
-        const int sl = fan ? h_tsl[j] : slots[j];
-        e->h_slot_mirror[sl] = sl;
+        e->h_slot_mirror[h_tsl[j]] = h_tsl[j];
     }
     return RR_OK;
 }
@@ -1303,286 +1307,256 @@ static void forget_prefixes(rr_engine* e) {
     ++e->index_epoch;
 }
 
+// Caller holds no lock.  The first scoring request gets its buffers before it is admitted.  If they cannot be had, the
+// waiting scoring requests fail, the engine serves on, and this returns false.
+static bool alloc_scoring(rr_engine* e, std::vector<DoneNote>* notes) {
+    if (e->sc_logits) return true;
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        if (std::none_of(e->waiting.begin(), e->waiting.end(), [](const Request* r) { return r->gen.scores(); })) return true;
+    }
+    int rc;
+    {
+        std::lock_guard<std::mutex> gl(e->gpu_mu);
+        std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
+        rc = ensure_score_buffers(e);
+    }
+    if (rc == RR_OK) return true;
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (auto it = e->waiting.begin(); it != e->waiting.end();) {
+        Request* r = *it;
+        if (!r->gen.scores()) { ++it; continue; }
+        it = e->waiting.erase(it);
+        finish_request(e, r, RR_INTERNAL, notes);
+    }
+    e->cv_done.notify_all();
+    return false;
+}
+
+// The rows at the start of a round: held, decoding (not the prompt in progress's), and the step_mode bits of the decoding.
+struct RowCount { int active = 0, decoding = 0, step = 0; };
+
+// Caller holds e->mu.  Sends the prompt in progress back to the queue if a low-level call cleared the index since its
+// admission, frees the rows of cancelled requests and counts the rest.
+static RowCount sweep_rows(rr_engine* e, std::vector<DoneNote>* notes) {
+    Request* ip = e->in_progress;
+    if (ip && !ip->cancel && e->o.prefix_cache && ip->epoch != e->index_epoch) requeue(e, ip);
+    RowCount n;
+    for (int b = 0; b < e->Bm; ++b) {
+        Request* r = e->row_req[b];
+        if (!r) continue;
+        if (r->cancel) {                               // rr_engine_cancel: free the rows, keep what was generated
+            release_request(e, r, RR_CANCELLED, notes);
+            continue;
+        }
+        ++n.active;
+        if (r == e->in_progress) continue;             // held for its next piece: no token yet
+        ++n.decoding;
+        n.step |= step_mode(r->gen);
+    }
+    return n;
+}
+
+// Caller holds e->mu.  Fills chunk c: the next piece of the prompt in progress first, then waiting requests in FIFO
+// order while the head fits; nothing overtakes it.  Returns the rows held after admission (`active` before).
+static int admit(rr_engine* e, Chunk* c, int active) {
+    if (Request* ip = e->in_progress) {               // its next piece goes first: min(Tmax, remaining) tokens
+        const int n = std::min(e->Tmax, (int)ip->prompt.size() - ip->n_done);
+        const bool last = ip->n_done + n == (int)ip->prompt.size();
+        c->add(ip, ip->rows[0], ip->n_done, ip->prompt.data() + ip->n_done, n, last);
+        c->has_pos0 = true;
+        if (last) e->in_progress = nullptr;
+    }
+    int b = 0;
+    while (!e->waiting.empty()) {
+        Request* r = e->waiting.front();
+        if (r->n_choices > e->Bm - active) break;      // its choices take that many free rows, all at its admission
+        if (r->gen.scores() && !e->sc_logits) break;   // submitted since alloc_scoring: the next round allocates
+        int m = 0, src = -1;
+        const bool ring = ring_request(e, r);           // the ring overwrites its prompt: no prefix hit, nothing kept
+        if (e->o.prefix_cache && (ring || r->gen.scores())) {     // scoring: every prompt row goes through lm_head
+            if ((b = pick_slot_miss(e)) < 0) break;
+        } else if (e->o.prefix_cache) {
+            if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
+        } else {
+            while (b < e->Bm && e->row_req[b] != nullptr) ++b;
+            if (b >= e->Bm) break;
+        }
+        // a chunk holds Tmax uncached tokens; with no prompt in progress, one that does not fit the room left starts with a
+        // piece that fills it
+        int n = (int)r->prompt.size() - m;
+        const int room = e->Tmax - (int)c->ids.size();
+        if (n > room) {
+            if (e->in_progress || room == 0) break;
+            n = room;
+        }
+        // every choice reserves its pages now; a request that does not fit waits at the head of the queue
+        if (r->n_choices * choice_pages(e, (int)r->prompt.size() + r->max_new) > pages_available(e)) break;
+        e->waiting.pop_front();
+        r->n_cached = m;
+        r->n_done = m;
+        if (e->o.prefix_cache) {
+            if (m > 0) e->retained_used[src >= 0 ? src : b] = ++e->lru_clock;
+            if (src >= 0) {
+                const int k = c->copies.count++;
+                c->copies.src[k] = src; c->copies.dst[k] = b; c->copies.n[k] = m;
+            }
+        }
+        for (int ch = 0; ch < r->n_choices; ++ch) {    // choice 0 in the prompt's slot, the others in free ones
+            if (ch > 0) {
+                if (e->o.prefix_cache) b = pick_slot_miss(e);
+                else while (e->row_req[b] != nullptr) ++b;
+            }
+            e->row_req[b] = r;
+            e->row_choice[b] = ch;
+            r->rows.push_back(b);
+            if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this prompt; set again once it succeeds
+        }
+        take_pages(e, r);
+        const bool last = m + n == (int)r->prompt.size();
+        c->add(r, r->rows[0], m, r->prompt.data() + m, n, last);
+        if (!last) { e->in_progress = r; r->epoch = c->epoch; }
+        active += r->n_choices;
+    }
+    return active;
+}
+
+// Caller holds gpu_mu.  The lazily allocated buffers that the tail rows of step_mode bits `mode` read, and the embedding
+// rows' if there are any.
+static int ensure_chunk_buffers(rr_engine* e, int mode, bool embeds) {
+    int rc = (mode & 4) ? ensure_pen_buffers(e) : RR_OK;
+    if (rc == RR_OK && (mode & 8)) rc = ensure_stop_buffers(e);
+    if (rc == RR_OK && (mode & 16)) rc = ensure_json_buffers(e);
+    return rc == RR_OK && embeds ? ensure_embed_buffers(e) : rc;
+}
+
+// Caller holds gpu_mu and the device lock.  Runs chunk c and hands its results to its requests: scores, embeddings,
+// first tokens, retained prefixes; a request whose prompt is done and has nothing left to decode is released, and every
+// request of a failed chunk ends with RR_INTERNAL.  Returns whether a prompt is still in progress.
+static bool run_chunk(rr_engine* e, const Chunk& c, std::vector<DoneNote>* notes) {
+    if (e->o.prefix_cache) {
+        // a low-level call took the GPU between admission and here and cleared the index: its matches may be stale, so
+        // the chunk goes back to the head of the queue and is admitted again (a prompt in progress from position 0)
+        std::lock_guard<std::mutex> lk(e->mu);
+        if (e->index_epoch != c.epoch) {
+            for (size_t i = c.seqs.size(); i-- > 0;) requeue(e, c.seqs[i].r);
+            return false;
+        }
+    }
+    int rc = upload_table(e);
+    if (rc == RR_OK) rc = ensure_chunk_buffers(e, c.mode, c.n_emb > 0);
+    if (rc == RR_OK) rc = run_prefill(e, c, nullptr, nullptr);
+    const double t = now_s(e);
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (const Chunk::Seq& q : c.seqs) {
+        Request* r = q.r;
+        if (rc != RR_OK) {
+            release_request(e, r, RR_INTERNAL, notes);
+            continue;
+        }
+        const size_t k = (size_t)r->gen.score_width();
+        for (int j = 0; j < q.score_rows(); ++j) {
+            const size_t p = (size_t)q.pos0 + j, o = (size_t)q.score_row + j;
+            r->ptgt[p] = e->h_sc_tlp[o];
+            memcpy(&r->plp[p * k], e->h_sc_lp + o * LP_MAX_TOP, sizeof(float) * k);
+            memcpy(&r->plp_id[p * k], e->h_sc_id + o * LP_MAX_TOP, sizeof(int32_t) * k);
+        }
+        r->n_done = q.pos0 + q.len;
+        if (!q.last) continue;                         // the prompt in progress: its next piece leads the next chunk
+        if (e->o.prefix_cache && !ring_request(e, r)) {   // every choice's slot holds the prompt's prefill-written KV
+            for (int b : r->rows) { e->retained[b] = r->prompt; e->retained_used[b] = ++e->lru_clock; }
+            if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
+        }
+        r->t_first = t;
+        if (r->embed) {                                // done: its row is free at once, it never decodes
+            const float* v = e->h_emb + (size_t)q.row * e->d.hidden;
+            r->emb.assign(v, v + e->d.hidden);
+            r->finish[0] = 0;
+            release_request(e, r, RR_OK, notes);
+            continue;
+        }
+        for (int ch = 0; ch < r->n_choices; ++ch) {
+            if (take_token(e, r, ch, q.row + ch)) release_row(e, r, ch);
+            else set_row_params(e, r->rows[ch], r, ch);
+        }
+        if (r->all_finished()) release_request(e, r, RR_OK, notes);
+    }
+    e->cv_done.notify_all();
+    return e->in_progress != nullptr;
+}
+
+// Caller holds gpu_mu and the device lock.  One decode step for every active row, of step_mode bits `step`, and its
+// tokens taken; a row whose choice finished is free for the next waiting prompt at once.
+static void run_step(rr_engine* e, int step, std::vector<DoneNote>* notes) {
+    cudaStream_t s = e->stream;
+    if (e->slots_dirty) {
+        memcpy(e->h_stage, e->h_slot_mirror.data(), sizeof(int32_t) * e->Bm);
+        cudaMemcpyAsync(e->d_slot, e->h_stage, sizeof(int32_t) * e->Bm, cudaMemcpyHostToDevice, s);
+        e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
+        e->slots_dirty = false;
+    }
+    upload_row_params(e, step);
+    int rc = upload_table(e);
+    cudaEventRecord(e->ev0, s);
+    if (rc == RR_OK) rc = run_decode_step(e, step);
+    cudaEventRecord(e->ev1, s);
+    const int rb = enqueue_readback(e, e->d_tok, e->Bm, step, s);     // outside ev0 .. ev1: decode_ms_total excludes it
+    if (rc == RR_OK) rc = rb;
+    cudaError_t se = cudaStreamSynchronize(s);
+    if (se != cudaSuccess) { rr::note_cuda_error(se); rc = RR_CUDA_ERROR; }
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+    e->st.decode_ms_total += ms;
+    e->st.decode_steps += 1;
+    {
+        std::lock_guard<std::mutex> lk(e->mu);
+        for (int b = 0; b < e->Bm; ++b) {              // a released request's later rows are already free
+            Request* r = e->row_req[b];
+            if (!r) continue;
+            if (rc != RR_OK) { release_request(e, r, RR_INTERNAL, notes); continue; }
+            if (r == e->in_progress) continue;         // its rows are inactive on the device
+            const int c = e->row_choice[b];
+            if (!take_token(e, r, c, b)) continue;
+            release_row(e, r, c);
+            if (r->all_finished()) release_request(e, r, RR_OK, notes);
+        }
+    }
+    e->cv_done.notify_all();
+}
+
+// Prefill first (best TTFT): a round that admits a chunk runs it and looks for more waiting prompts before decoding.  But
+// a running reply waits at most one chunk between tokens, however many pieces a long prompt takes.  Done hooks run outside
+// e->mu, before the worker idles.
 static void worker_main(rr_engine* e) {
     cudaSetDevice(e->o.device);
-    std::vector<int32_t> ids, seq_start, slots, pos0;
-    std::vector<Request*> chunk;
     std::vector<DoneNote> notes;
-    KvCopyList* copies = new KvCopyList();
-    std::vector<int32_t> tail_seq, tail_slot, tail_choice;      // the chunk's tail rows (PrefillTail), one per choice
-    std::vector<const GenParams*> tail_gen;
-    std::vector<int32_t> emb_seq;                               // the chunk's embedding rows, after the tail rows
-    PrefillScore score;                                         // the chunk's scoring rows, and for each entry
-    std::vector<Request*> score_req;                            // its request and the position of its first row
-    std::vector<int> score_pos;
-    // sequence `seq` of the chunk is the piece [p0, p0 + n) of r's prompt: its rows that predict a prompt token score
-    auto add_score = [&](Request* r, int seq, int p0, int n) {
-        const int rows = std::min(n, (int)r->prompt.size() - 1 - p0);
-        if (!r->gen.scores() || rows < 1) return;
-        score.seq.push_back(seq); score.rows.push_back(rows); score.top.push_back(r->gen.prompt_top);
-        score.tgt.insert(score.tgt.end(), r->prompt.begin() + p0 + 1, r->prompt.begin() + p0 + 1 + rows);
-        score_req.push_back(r); score_pos.push_back(p0);
-    };
+    Chunk chunk;
     bool decode_due = false;         // the last chunk left a prompt in progress: one decode step goes before the next chunk
     while (!e->stop.load()) {
         run_hooks(e, notes);
-        if (!e->sc_logits) {
-            // the first scoring request: its buffers before it is admitted.  If they cannot be had, the scoring requests fail
-            // and the engine serves on.
-            bool want = false;
-            {
-                std::lock_guard<std::mutex> lk(e->mu);
-                for (const Request* r : e->waiting) want = want || r->gen.scores();
-            }
-            if (want) {
-                int rc;
-                {
-                    std::lock_guard<std::mutex> gl(e->gpu_mu);
-                    std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
-                    rc = ensure_score_buffers(e);
-                }
-                if (rc != RR_OK) {
-                    std::lock_guard<std::mutex> lk(e->mu);
-                    for (auto it = e->waiting.begin(); it != e->waiting.end();) {
-                        Request* r = *it;
-                        if (!r->gen.scores()) { ++it; continue; }
-                        it = e->waiting.erase(it);
-                        finish_request(e, r, RR_INTERNAL, &notes);
-                    }
-                    e->cv_done.notify_all();
-                    continue;
-                }
-            }
-        }
-        // ---- admit waiting requests into free rows (prefill has priority: best TTFT)
-        chunk.clear(); ids.clear(); seq_start.assign(1, 0); slots.clear(); pos0.clear();
-        tail_seq.clear(); tail_slot.clear(); tail_choice.clear(); tail_gen.clear(); emb_seq.clear();
-        score.clear(); score_req.clear(); score_pos.clear();
-        copies->count = 0;
-        int active = 0, decoding = 0;                      // rows held / rows decoding (not the prompt in progress's)
-        int step = 0, chunk_mode = 0;                      // step_mode bits of the decoding rows / of the chunk's tail rows
-        bool resumed = false;                              // the chunk continues a prompt in progress
-        uint64_t epoch = 0;
+        if (!alloc_scoring(e, &notes)) continue;
+        RowCount rows;
         {
             std::unique_lock<std::mutex> lk(e->mu);
-            epoch = e->index_epoch;
-            Request* ip = e->in_progress;
-            if (ip && !ip->cancel && e->o.prefix_cache && ip->epoch != epoch) { requeue(e, ip); ip = nullptr; }
-            for (int b = 0; b < e->Bm; ++b) {
-                Request* r = e->row_req[b];
-                if (!r) continue;
-                if (r->cancel) {                           // rr_engine_cancel: free the rows, keep what was generated
-                    release_request(e, r, RR_CANCELLED, &notes);
-                    continue;
-                }
-                ++active;
-                if (r == e->in_progress) continue;         // held for its next piece: no token yet
-                ++decoding;
-                step |= step_mode(r->gen);
-            }
-            ip = e->in_progress;
-            if (e->waiting.empty() && active == 0) {
+            rows = sweep_rows(e, &notes);
+            if (e->waiting.empty() && rows.active == 0) {
                 if (!notes.empty()) continue;              // report the requests a cancel just ended before idling
                 e->st.queued = 0; e->st.active_rows = 0;   // idle: every row is free and every done hook has run
                 e->cv_work.wait_for(lk, std::chrono::milliseconds(50));
                 continue;
             }
-            // a running reply waits at most one chunk between tokens, however many pieces a long prompt takes
-            const bool decode_first = decode_due && decoding > 0;
+            const bool decode_first = decode_due && rows.decoding > 0;
             decode_due = false;
-            if (ip && !decode_first) {                     // its next piece goes first: min(Tmax, remaining) tokens
-                const int n = std::min(e->Tmax, (int)ip->prompt.size() - ip->n_done);
-                add_score(ip, (int)chunk.size(), ip->n_done, n);
-                chunk.push_back(ip);
-                slots.push_back(ip->rows[0]);
-                pos0.push_back(ip->n_done);
-                ids.insert(ids.end(), ip->prompt.begin() + ip->n_done, ip->prompt.begin() + ip->n_done + n);
-                seq_start.push_back((int)ids.size());
-                resumed = true;
-                if (ip->n_done + n == (int)ip->prompt.size()) {     // its last piece: the tail rows of its choices
-                    if (ip->embed) emb_seq.push_back(0);
-                    for (int c = 0; !ip->embed && c < ip->n_choices; ++c) {
-                        tail_seq.push_back(0); tail_slot.push_back(ip->rows[c]); tail_choice.push_back(c);
-                        tail_gen.push_back(&ip->gen);
-                    }
-                    chunk_mode |= step_mode(ip->gen);
-                    e->in_progress = nullptr;
-                }
-            }
-            int b = 0;
-            while (!decode_first && !e->waiting.empty()) {
-                Request* r = e->waiting.front();
-                if (r->n_choices > e->Bm - active) break;  // its choices take that many free rows, all at its admission
-                if (r->gen.scores() && !e->sc_logits) break;   // submitted since the check above: the next round allocates
-                int m = 0, src = -1;
-                const bool ring = ring_request(e, r);       // the ring overwrites its prompt: no prefix hit, nothing kept
-                if (e->o.prefix_cache && (ring || r->gen.scores())) {     // scoring: every prompt row goes through lm_head
-                    if ((b = pick_slot_miss(e)) < 0) break;
-                } else if (e->o.prefix_cache) {
-                    if (!pick_slot_cached(e, r->prompt, &b, &m, &src)) break;
-                } else {
-                    while (b < e->Bm && e->row_req[b] != nullptr) ++b;
-                    if (b >= e->Bm) break;
-                }
-                // a chunk holds Tmax uncached tokens; with no prompt in progress, one that does not fit the room left
-                // starts with a piece that fills it
-                int n = (int)r->prompt.size() - m;
-                const int room = e->Tmax - (int)ids.size();
-                if (n > room) {
-                    if (e->in_progress || room == 0) break;
-                    n = room;
-                }
-                // every choice reserves its pages now; a request that does not fit waits at the head of the queue
-                if (r->n_choices * choice_pages(e, (int)r->prompt.size() + r->max_new) > pages_available(e)) break;
-                e->waiting.pop_front();
-                r->n_cached = m;
-                r->n_done = m;
-                if (e->o.prefix_cache) {
-                    if (m > 0) e->retained_used[src >= 0 ? src : b] = ++e->lru_clock;
-                    if (src >= 0) {
-                        const int c = copies->count++;
-                        copies->src[c] = src; copies->dst[c] = b; copies->n[c] = m;
-                    }
-                }
-                pos0.push_back(m);
-                const bool last = m + n == (int)r->prompt.size();
-                for (int c = 0; c < r->n_choices; ++c) {   // choice 0 in the prompt's slot, the others in free ones
-                    if (c > 0) {
-                        if (e->o.prefix_cache) b = pick_slot_miss(e);
-                        else while (e->row_req[b] != nullptr) ++b;
-                    }
-                    e->row_req[b] = r;
-                    e->row_choice[b] = c;
-                    r->rows.push_back(b);
-                    if (e->o.prefix_cache) e->retained[b].clear();   // rewritten by this prompt; set again once it succeeds
-                    if (!last) continue;
-                    if (r->embed) { emb_seq.push_back((int)chunk.size()); continue; }
-                    tail_seq.push_back((int)chunk.size()); tail_slot.push_back(b); tail_choice.push_back(c);
-                    tail_gen.push_back(&r->gen);
-                }
-                take_pages(e, r);
-                add_score(r, (int)chunk.size(), m, n);
-                chunk.push_back(r);
-                slots.push_back(r->rows[0]);
-                if (last) chunk_mode |= step_mode(r->gen);
-                else { e->in_progress = r; r->epoch = epoch; }
-                ids.insert(ids.end(), r->prompt.begin() + m, r->prompt.begin() + m + n);
-                seq_start.push_back((int)ids.size());
-                active += r->n_choices;
-            }
+            chunk.reset(e->index_epoch, e->o.prefix_cache);
+            e->st.active_rows = decode_first ? rows.active : admit(e, &chunk, rows.active);
             e->st.queued = (int)e->waiting.size();
-            e->st.active_rows = active;
         }
         std::lock_guard<std::mutex> gl(e->gpu_mu);
         std::lock_guard<std::mutex> dl(device_mutex(e->o.device));
-        if (!chunk.empty() && e->o.prefix_cache) {
-            // a low-level call took the GPU between admission and here and cleared the index: its matches may be stale,
-            // so the chunk goes back to the head of the queue and is admitted again (a prompt in progress from position 0)
-            std::lock_guard<std::mutex> lk(e->mu);
-            if (e->index_epoch != epoch) {
-                for (size_t i = chunk.size(); i-- > 0;) requeue(e, chunk[i]);
-                continue;
-            }
-        }
-        if (!chunk.empty()) {
-            PrefillTail tail;
-            tail.n = (int)tail_seq.size(); tail.seq = tail_seq.data(); tail.slot = tail_slot.data();
-            tail.choice = tail_choice.data(); tail.gen = tail_gen.data(); tail.mode = chunk_mode;
-            int rc = upload_table(e);
-            if (rc == RR_OK && (chunk_mode & 4)) rc = ensure_pen_buffers(e);
-            if (rc == RR_OK && (chunk_mode & 8)) rc = ensure_stop_buffers(e);
-            if (rc == RR_OK && (chunk_mode & 16)) rc = ensure_json_buffers(e);
-            if (rc == RR_OK && !emb_seq.empty()) rc = ensure_embed_buffers(e);
-            if (rc == RR_OK)
-                rc = run_prefill(e, ids.data(), seq_start.data(), slots.data(), (int)chunk.size(), nullptr, nullptr,
-                                 e->o.prefix_cache || resumed ? pos0.data() : nullptr, copies, &tail, &score,
-                                 (int)emb_seq.size(), emb_seq.data());
-            const double t = now_s(e);
-            std::lock_guard<std::mutex> lk(e->mu);
-            for (size_t i = 0, o = 0; rc == RR_OK && i < score_req.size(); o += (size_t)score.rows[i++]) {
-                Request* r = score_req[i];
-                const size_t k = (size_t)r->gen.score_width();
-                for (int j = 0; j < score.rows[i]; ++j) {
-                    const size_t p = (size_t)score_pos[i] + j, src = (o + j) * LP_MAX_TOP;
-                    r->ptgt[p] = e->h_sc_tlp[o + j];
-                    memcpy(&r->plp[p * k], e->h_sc_lp + src, sizeof(float) * k);
-                    memcpy(&r->plp_id[p * k], e->h_sc_id + src, sizeof(int32_t) * k);
-                }
-            }
-            int j = 0, k = 0;                              // the request's first tail row / its embedding row
-            for (size_t i = 0; i < chunk.size(); ++i) {
-                Request* r = chunk[i];
-                const int row0 = j, emb_row = k;
-                const bool last = pos0[i] + seq_start[i + 1] - seq_start[i] == (int)r->prompt.size();
-                if (last && r->embed) ++k;
-                else if (last) j += r->n_choices;
-                if (rc != RR_OK) {
-                    release_request(e, r, RR_INTERNAL, &notes);
-                    continue;
-                }
-                r->n_done = pos0[i] + seq_start[i + 1] - seq_start[i];
-                if (!last) continue;                       // the prompt in progress: its next piece leads the next chunk
-                if (e->o.prefix_cache && !ring_request(e, r)) {   // every choice's slot holds the prompt's prefill-written KV
-                    for (int b : r->rows) { e->retained[b] = r->prompt; e->retained_used[b] = ++e->lru_clock; }
-                    if (r->n_cached > 0) { e->st.prefix_hits += 1; e->st.prefix_cached_tokens += r->n_cached; }
-                }
-                r->t_first = t;
-                if (r->embed) {                            // done: its row is free at once, it never decodes
-                    const float* v = e->h_emb + (size_t)emb_row * e->d.hidden;
-                    r->emb.assign(v, v + e->d.hidden);
-                    r->finish[0] = 0;
-                    release_request(e, r, RR_OK, &notes);
-                    continue;
-                }
-                for (int c = 0; c < r->n_choices; ++c) {
-                    if (take_token(e, r, c, row0 + c)) release_row(e, r, c);
-                    else set_row_params(e, r->rows[c], r, c);
-                }
-                if (r->all_finished()) release_request(e, r, RR_OK, &notes);
-            }
-            decode_due = e->in_progress != nullptr;
-            e->cv_done.notify_all();
-            continue;   // look for more waiting prompts before decoding
-        }
-        if (decoding == 0) continue;
-        // ---- one decode step for all active rows
-        cudaStream_t s = e->stream;
-        if (e->slots_dirty) {
-            memcpy(e->h_stage, e->h_slot_mirror.data(), sizeof(int32_t) * e->Bm);
-            cudaMemcpyAsync(e->d_slot, e->h_stage, sizeof(int32_t) * e->Bm, cudaMemcpyHostToDevice, s);
-            e->st.h2d_bytes += sizeof(int32_t) * e->Bm;
-            e->slots_dirty = false;
-        }
-        upload_row_params(e, step);
-        int rc = upload_table(e);
-        cudaEventRecord(e->ev0, s);
-        if (rc == RR_OK) rc = run_decode_step(e, step);
-        cudaEventRecord(e->ev1, s);
-        const int rb = enqueue_readback(e, e->d_tok, e->Bm, step, s);     // outside ev0 .. ev1: decode_ms_total excludes it
-        if (rc == RR_OK) rc = rb;
-        cudaError_t se = cudaStreamSynchronize(s);
-        if (se != cudaSuccess) { rr::note_cuda_error(se); rc = RR_CUDA_ERROR; }
-        float ms = 0;
-        cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-        e->st.decode_ms_total += ms;
-        e->st.decode_steps += 1;
-        {
-            std::lock_guard<std::mutex> lk(e->mu);
-            for (int b = 0; b < e->Bm; ++b) {              // a released request's later rows are already free
-                Request* r = e->row_req[b];
-                if (!r) continue;
-                if (rc != RR_OK) { release_request(e, r, RR_INTERNAL, &notes); continue; }
-                if (r == e->in_progress) continue;         // its rows are inactive on the device
-                const int c = e->row_choice[b];
-                if (!take_token(e, r, c, b)) continue;
-                release_row(e, r, c);                      // the row is free for the next waiting prompt at once
-                if (r->all_finished()) release_request(e, r, RR_OK, &notes);
-            }
-        }
-        e->cv_done.notify_all();
+        if (!chunk.seqs.empty()) decode_due = run_chunk(e, chunk, &notes);
+        else if (rows.decoding > 0) run_step(e, rows.step, &notes);
     }
     run_hooks(e, notes);
-    delete copies;
 }
 
 // ---------------------------------------------------------------- C-ABI
@@ -1833,7 +1807,11 @@ RR_API int rr_engine_prefill(rr_engine* e, const int32_t* ids, const int32_t* se
     }
     int rc = grow_pages(e, slots, n_pos.data(), n_seqs);
     if (rc == RR_OK) rc = upload_table(e);
-    return rc != RR_OK ? rc : run_prefill(e, ids, seq_start, slots, n_seqs, first_tok, logits_out);
+    if (rc != RR_OK) return rc;
+    Chunk c;                                           // plain last pieces: one greedy tail row per sequence, in its slot
+    c.reset(0, false);
+    for (int i = 0; i < n_seqs; ++i) c.add(nullptr, slots[i], 0, ids + seq_start[i], seq_start[i + 1] - seq_start[i], true);
+    return run_prefill(e, c, first_tok, logits_out);
 }
 
 RR_API int rr_engine_decode_step(rr_engine* e, const int32_t* slots, const int32_t* tok, const int32_t* pos, int n,
@@ -1999,28 +1977,34 @@ RR_API int rr_engine_submit_scored(rr_engine* e, const int32_t* prompt_ids, int 
     return rr::engine_submit_tagged(e, prompt_ids, n_prompt, max_new_tokens, 0, ticket, p, params ? params->n_choices : 1);
 }
 
+// Caller holds lk on e->mu.  The request of `ticket` once ready(r) holds, else as it is at the deadline (timeout_s <= 0:
+// none); null when the ticket is unknown or consumed.  It is looked up again after every wake-up: another thread may have
+// consumed (wait) or cancelled the ticket meanwhile.  A caller that reads one kind of request makes ready() true for the
+// other kinds, and refuses them.
+template <typename Ready>
+static Request* await_request(rr_engine* e, std::unique_lock<std::mutex>& lk, uint64_t ticket, double timeout_s,
+                              Ready ready) {
+    const auto deadline = std::chrono::steady_clock::now() +
+                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
+    for (bool late = false;; late = e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
+        auto it = e->table.find(ticket);
+        if (it == e->table.end()) return nullptr;
+        if (late || ready(it->second)) return it->second;
+    }
+}
+
 RR_API int rr_engine_prompt_logprobs(rr_engine* e, uint64_t ticket, double timeout_s, float* target_lp_out, float* lp_out,
                                      int32_t* id_out) {
     if (!e) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
-    const auto deadline = std::chrono::steady_clock::now() +
-                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
-    for (;;) {
-        auto it = e->table.find(ticket);
-        if (it == e->table.end() || !it->second->gen.scores()) return RR_INVALID_ARGUMENT;
-        const Request* r = it->second;
-        if (r->done) {
-            if (r->status != RR_OK) return r->status;
-            if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
-            if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
-            if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
-            return RR_OK;
-        }
-        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
-            it = e->table.find(ticket);
-            if (it == e->table.end() || !it->second->done) return it == e->table.end() ? RR_INVALID_ARGUMENT : RR_TIMEOUT;
-        }
-    }
+    const Request* r = await_request(e, lk, ticket, timeout_s, [](const Request* q) { return !q->gen.scores() || q->done; });
+    if (!r || !r->gen.scores()) return RR_INVALID_ARGUMENT;
+    if (!r->done) return RR_TIMEOUT;
+    if (r->status != RR_OK) return r->status;
+    if (target_lp_out) memcpy(target_lp_out, r->ptgt.data(), sizeof(float) * r->ptgt.size());
+    if (lp_out) memcpy(lp_out, r->plp.data(), sizeof(float) * r->plp.size());
+    if (id_out) memcpy(id_out, r->plp_id.data(), sizeof(int32_t) * r->plp_id.size());
+    return RR_OK;
 }
 
 RR_API int rr_engine_submit_embed(rr_engine* e, const int32_t* prompt_ids, int n_prompt, uint64_t* ticket) {
@@ -2030,23 +2014,13 @@ RR_API int rr_engine_submit_embed(rr_engine* e, const int32_t* prompt_ids, int n
 RR_API int rr_engine_embedding(rr_engine* e, uint64_t ticket, double timeout_s, float* out, int capacity, int* dim_out) {
     if (!e || !out || capacity < e->d.hidden) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
-    const auto deadline = std::chrono::steady_clock::now() +
-                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
-    for (;;) {
-        auto it = e->table.find(ticket);
-        if (it == e->table.end() || !it->second->embed) return RR_INVALID_ARGUMENT;
-        const Request* r = it->second;
-        if (r->done) {
-            if (r->status != RR_OK) return r->status;
-            memcpy(out, r->emb.data(), sizeof(float) * r->emb.size());
-            if (dim_out) *dim_out = (int)r->emb.size();
-            return RR_OK;
-        }
-        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
-            it = e->table.find(ticket);
-            if (it == e->table.end() || !it->second->done) return it == e->table.end() ? RR_INVALID_ARGUMENT : RR_TIMEOUT;
-        }
-    }
+    const Request* r = await_request(e, lk, ticket, timeout_s, [](const Request* q) { return !q->embed || q->done; });
+    if (!r || !r->embed) return RR_INVALID_ARGUMENT;
+    if (!r->done) return RR_TIMEOUT;
+    if (r->status != RR_OK) return r->status;
+    memcpy(out, r->emb.data(), sizeof(float) * r->emb.size());
+    if (dim_out) *dim_out = (int)r->emb.size();
+    return RR_OK;
 }
 
 // Caller holds e->mu.  The first min(n, max_tokens_out) visible tokens of each choice of r (fewer for a shorter choice)
@@ -2101,23 +2075,10 @@ RR_API int rr_engine_peek(rr_engine* e, uint64_t ticket, int have, double timeou
                           int32_t* id_out) {
     if (!e || !n_generated || !done) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
-    const auto deadline = std::chrono::steady_clock::now() +
-                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
-    Request* r = nullptr;
-    for (;;) {
-        // looked up again after every wake-up: another thread may have consumed (wait) or cancelled the ticket meanwhile
-        auto it = e->table.find(ticket);
-        if (it == e->table.end()) return RR_INVALID_ARGUMENT;
-        r = it->second;
-        if (r->n_choices > 1) return RR_INVALID_ARGUMENT;
-        if (r->done || r->n_generated() > have) break;
-        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
-            it = e->table.find(ticket);
-            if (it == e->table.end()) return RR_INVALID_ARGUMENT;
-            r = it->second;
-            break;
-        }
-    }
+    const Request* r = await_request(e, lk, ticket, timeout_s, [have](const Request* q) {
+        return q->n_choices > 1 || q->done || q->n_generated() > have;
+    });
+    if (!r || r->n_choices > 1) return RR_INVALID_ARGUMENT;
     const int n = r->n_generated();
     *n_generated = n;
     *done = r->done ? 1 : 0;
@@ -2130,21 +2091,11 @@ RR_API int rr_engine_wait(rr_engine* e, uint64_t ticket, double timeout_s, rr_co
                           int max_tokens_out, float* lp_out, int32_t* id_out, int32_t* n_tokens_out, int32_t* finish_out) {
     if (!e || !out) return RR_INVALID_ARGUMENT;
     std::unique_lock<std::mutex> lk(e->mu);
-    const auto deadline = std::chrono::steady_clock::now() +
-                          std::chrono::duration<double>(timeout_s > 0 ? timeout_s : 1e9);
-    Request* r = nullptr;
-    for (;;) {
-        auto it = e->table.find(ticket);
-        if (it == e->table.end()) return RR_INVALID_ARGUMENT;      // unknown, already consumed, or cancelled
-        r = it->second;
-        if (r->done) break;
-        if (e->cv_done.wait_until(lk, deadline) == std::cv_status::timeout) {
-            it = e->table.find(ticket);
-            if (it == e->table.end()) return RR_INVALID_ARGUMENT;
-            if (it->second->done) { r = it->second; break; }
-            out->ticket = ticket; out->status = RR_TIMEOUT;
-            return RR_TIMEOUT;   // the request stays in flight: wait again, or rr_engine_cancel
-        }
+    Request* r = await_request(e, lk, ticket, timeout_s, [](const Request* q) { return q->done; });
+    if (!r) return RR_INVALID_ARGUMENT;                // unknown, already consumed, or cancelled
+    if (!r->done) {
+        out->ticket = ticket; out->status = RR_TIMEOUT;
+        return RR_TIMEOUT;   // the request stays in flight: wait again, or rr_engine_cancel
     }
     out->ticket = ticket; out->status = r->status; out->n_prompt = (int)r->prompt.size();
     out->n_generated = r->n_generated(); out->n_cached = r->n_cached;
