@@ -211,6 +211,13 @@ int rr_gemm_bf16(const void* A, int rowsA, int ldA, const void* B, int rowsB, in
  * dequantize: out bf16 [rows, ld_out] = bf16(Q * scale) exactly (16-byte aligned, ld_out % 8 == 0, ld_out >= K). */
 int rr_op_quantize_fp8_weight(const void* w, int rows, int K, int ld, void* q_out, float* scale_out, void* stream);
 int rr_op_dequantize_fp8_weight(const void* q, const float* scale, int rows, int K, void* out, int ld_out, void* stream);
+/* The dequantize of n_jobs (1..4) weights in one launch, as the engine runs it before each prefill layer of an FP8 model
+ * (QKV, O, gate/up and down; the last layer QKV only): job i is rr_op_dequantize_fp8_weight(q[i], scale[i], rows[i], K[i],
+ * out[i], ld_out[i]), with the same result bit for bit.  The arguments are host arrays of n_jobs entries.  Nothing outside
+ * the jobs' rows [0, rows[i]) x columns [0, K[i]) of out[i] is written.  RR_INVALID_ARGUMENT before touching the device
+ * for a null array, n_jobs outside 1..4, or a job rr_op_dequantize_fp8_weight would refuse. */
+int rr_op_dequantize_fp8_jobs(const void* const* q, const float* const* scale, const int32_t* rows, const int32_t* K,
+                              void* const* out, const int32_t* ld_out, int n_jobs, void* stream);
 /* rr_gemm_bf16's decode modes (RR_OUT_TRANSPOSED_F32 / _SILU) with A an e4m3 weight [rowsA, K] (pitch ldA bytes, a
  * multiple of 16) and its row scales: the same tiles, splits, summation order and epilogues as rr_gemm_bf16 on
  * D = bf16(A * scale), so the same output bits.  RR_INVALID_ARGUMENT for a row-major mode or a null scale. */
@@ -390,6 +397,21 @@ int rr_op_prefill_attn_cached_paged(const void* q, const void* k_cache, const vo
 int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers, int n_slots, int n_kv_heads, int ctx_max,
                                const int32_t* src, const int32_t* dst, const int32_t* n_tok, int n_copies,
                                const int32_t* page_table, int pages_per_slot, int n_pages, void* stream);
+/* The hand-off of a prefill chunk to decode, as the engine runs it after the chunk's last layer (device arrays).
+ * gather_last: for r < n_rows, attn_out[r][0..nq) = attn[last[r]][0..nq) (bf16) and x_out[r][0..hidden) =
+ *   x[last[r]][0..hidden) (fp32), bit for bit; the rows of the tail and embedding rows of a chunk, several of them may name
+ *   the same last[r].  Rows >= n_rows of the outputs are not written.  RR_INVALID_ARGUMENT before touching the device for a
+ *   null pointer, n_rows < 1, nq not a positive multiple of 8, hidden not a positive multiple of 4, or a buffer that is not
+ *   16-byte aligned.
+ * activate_rows: for i < n, slot s = seq_slot[i] becomes a live decode row: d_tok[s] = first_tok[i],
+ *   d_pos[s] = tok_pos[last[i]] + 1 (the position after the prompt's last token, a cached prefix included), d_slot[s] = s.
+ *   No other entry is written; the slots must be distinct.  RR_INVALID_ARGUMENT before touching the device for a null
+ *   pointer or n < 1.
+ * Indices are trusted, as slot indices are. */
+int rr_op_gather_last(const void* attn, const float* x, const int32_t* last, int n_rows, int nq, int hidden, void* attn_out,
+                      float* x_out, void* stream);
+int rr_op_activate_rows(const int32_t* seq_slot, const int32_t* first_tok, const int32_t* tok_pos, const int32_t* last, int n,
+                        int32_t* d_tok, int32_t* d_pos, int32_t* d_slot, void* stream);
 /* Decode attention with a sliding window W = window: the arguments of rr_op_decode_attn_qkv_paged plus window.  The row
  * at position pos attends to positions max(0, pos - W + 1) .. pos of its slot; window 0 is full causal attention, and
  * rr_op_decode_attn_qkv_paged is this call with window 0.  The kv splits divide the key tiles from the tile of

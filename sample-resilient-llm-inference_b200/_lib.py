@@ -168,6 +168,7 @@ PROTOTYPES = {
     "rr_op_decode_proj": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp, C.c_int, C.c_int, c_i32p, vp]),
     "rr_op_quantize_fp8_weight": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
     "rr_op_dequantize_fp8_weight": (C.c_int, [vp, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
+    "rr_op_dequantize_fp8_jobs": (C.c_int, [vp, vp, c_i32p, c_i32p, vp, c_i32p, C.c_int, vp]),
     "rr_op_embed": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp]),
     "rr_op_embed_pool": (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp]),
     "rr_op_add_rmsnorm": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_longlong, C.c_int, vp, vp,
@@ -198,6 +199,8 @@ PROTOTYPES = {
                                         C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]),
     "rr_op_kv_copy_prefix_paged": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, c_i32p, c_i32p, c_i32p, C.c_int,
                                              vp, C.c_int, C.c_int, vp]),
+    "rr_op_gather_last": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
+    "rr_op_activate_rows": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]),
     "rr_op_decode_mlp": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_mlp_fp8": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, c_i32p, c_i32p, vp]),
     "rr_op_decode_attn_qkv": (C.c_int, [vp, C.c_int, C.c_longlong, C.c_int, vp, vp, vp, vp, vp, C.c_int, C.c_int,

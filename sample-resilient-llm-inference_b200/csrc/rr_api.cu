@@ -202,6 +202,22 @@ RR_API int rr_op_dequantize_fp8_weight(const void* q, const float* scale, int ro
     return check_last();
 }
 
+// A layer's dequantize as the engine runs it before each prefill layer: up to four jobs in one launch (launch_dequant_layer).
+RR_API int rr_op_dequantize_fp8_jobs(const void* const* q, const float* const* scale, const int32_t* rows, const int32_t* K,
+                                     void* const* out, const int32_t* ld_out, int n_jobs, void* stream) {
+    if (!q || !scale || !rows || !K || !out || !ld_out || n_jobs < 1 || n_jobs > 4) return RR_INVALID_ARGUMENT;
+    Fp8DequantJobs J;
+    for (int i = 0; i < n_jobs; ++i) {
+        if (!scale[i] || !out[i] || rows[i] < 1 || !fp8_weight_ok(q[i], K[i]) || ld_out[i] < K[i] || ld_out[i] % 8 ||
+            ((uintptr_t)out[i] & 15))
+            return RR_INVALID_ARGUMENT;
+        fp8_dequant_job(&J, q[i], scale[i], rows[i], K[i], (__nv_bfloat16*)out[i], ld_out[i]);
+    }
+    const int rc = launch_dequantize_fp8(J, (cudaStream_t)stream);
+    if (rc != RR_OK) { note_cuda_error(cudaPeekAtLastError()); return rc; }
+    return check_last();
+}
+
 static PartIn mk_part(const void* p, int is_bf16, int n_splits, long long split_stride, int ld) {
     PartIn r;
     r.ptr = p; r.is_bf16 = is_bf16; r.n_splits = n_splits < 1 ? 1 : n_splits;
@@ -771,4 +787,23 @@ RR_API int rr_op_kv_copy_prefix_paged(void* k_cache, void* v_cache, int n_layers
     if (!paged_ok(page_table, pages_per_slot, n_pages, ctx_max)) return RR_INVALID_ARGUMENT;
     return kv_copy_prefix(k_cache, v_cache, n_layers, n_slots, n_kv_heads, ctx_max, src, dst, n_tok, n_copies, page_table,
                           pages_per_slot, n_pages, stream);
+}
+
+// The hand-off of a prefill chunk to decode, as run_prefill launches it; row, slot and index arrays are trusted, as slot
+// indices are.
+RR_API int rr_op_gather_last(const void* attn, const float* x, const int32_t* last, int n_rows, int nq, int hidden,
+                             void* attn_out, float* x_out, void* stream) {
+    if (!attn || !x || !last || !attn_out || !x_out) return RR_INVALID_ARGUMENT;
+    if (n_rows < 1 || nq < 8 || nq % 8 || hidden < 4 || hidden % 4) return RR_INVALID_ARGUMENT;
+    if ((((uintptr_t)attn | (uintptr_t)x | (uintptr_t)attn_out | (uintptr_t)x_out) & 15)) return RR_INVALID_ARGUMENT;
+    launch_gather_last((const __nv_bfloat16*)attn, x, last, n_rows, nq, hidden, (__nv_bfloat16*)attn_out, x_out,
+                       (cudaStream_t)stream);
+    return check_last();
+}
+
+RR_API int rr_op_activate_rows(const int32_t* seq_slot, const int32_t* first_tok, const int32_t* tok_pos, const int32_t* last,
+                               int n, int32_t* d_tok, int32_t* d_pos, int32_t* d_slot, void* stream) {
+    if (!seq_slot || !first_tok || !tok_pos || !last || !d_tok || !d_pos || !d_slot || n < 1) return RR_INVALID_ARGUMENT;
+    launch_activate_rows(seq_slot, first_tok, tok_pos, last, n, d_tok, d_pos, d_slot, (cudaStream_t)stream);
+    return check_last();
 }

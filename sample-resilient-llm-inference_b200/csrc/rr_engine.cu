@@ -65,6 +65,19 @@ __global__ void activate_rows_kernel(const int32_t* __restrict__ seq_slot, const
     d_slot[s] = s;
 }
 
+void launch_gather_last(const __nv_bfloat16* attn, const float* x, const int32_t* last, int n_rows, int nq, int hidden,
+                        __nv_bfloat16* attn_out, float* x_out, cudaStream_t st) {
+    if (n_rows <= 0) return;
+    launch_pdl(gather_last_kernel, dim3(n_rows), dim3(256), 0, st, attn, x, last, attn_out, x_out, nq, hidden);
+}
+
+void launch_activate_rows(const int32_t* seq_slot, const int32_t* first_tok, const int32_t* tok_pos, const int32_t* last,
+                          int n, int32_t* d_tok, int32_t* d_pos, int32_t* d_slot, cudaStream_t st) {
+    if (n <= 0) return;
+    launch_pdl(activate_rows_kernel, dim3((n + 127) / 128), dim3(128), 0, st, seq_slot, first_tok, tok_pos, last, n, d_tok,
+               d_pos, d_slot);
+}
+
 // One request of n_choices choices.  Choice c decodes in row rows[c] (== its KV slot); the prompt is prefilled once, into
 // rows[0], and its KV copied to the other rows.  The choices are admitted together and get one token each per step.  A
 // choice finishes when it holds max_new tokens, a stop sequence cuts it or (JSON mode) its top-level object closes, and
@@ -967,8 +980,7 @@ static int run_prefill(rr_engine* e, const Chunk& c, int32_t* first_tok_host, fl
             // ---- trimmed tail: the tail and embedding rows through O, MLP, final norm (decode-orientation kernels, decode
             // buffers; every kernel is row-independent, so a row's bits do not depend on the others).  The unfused kernels
             // even with fuse_mlp: the fused kernel's down GEMM sums in a different order.
-            launch_pdl(gather_last_kernel, dim3(nr), dim3(256), 0, s, (const __nv_bfloat16*)e->pattn, (const float*)e->px,
-                       p_tlast, e->attn_out, e->x, e->nq, d.hidden); ++nl;
+            launch_gather_last(e->pattn, e->px, p_tlast, nr, e->nq, d.hidden, e->attn_out, e->x, s); ++nl;
             if (enqueue_o_mlp(e, l, nr, s, &nl) != RR_OK) return RR_CUDA_ERROR;
         }
         if (l + 1 == d.n_layers && !scoring) break;    // a scoring chunk runs the whole last layer as well
@@ -1010,8 +1022,7 @@ static int run_prefill(rr_engine* e, const Chunk& c, int32_t* first_tok_host, fl
     if (nt > 0) {
         if (gemm_launch(e->pl_head, s) != RR_OK) return RR_CUDA_ERROR; ++nl;      // B = e->xn (rows 0..nt-1)
         nl += enqueue_tail(e, dp, nt, mode, e->p_first, nullptr, nullptr, dp.pos(), nullptr, s, p_tsl);
-        launch_pdl(activate_rows_kernel, dim3((nt + 127) / 128), dim3(128), 0, s, p_tsl, (const int32_t*)e->p_first,
-                   (const int32_t*)p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot); ++nl;
+        launch_activate_rows(p_tsl, e->p_first, p_pos, p_tlast, nt, e->d_tok, e->d_pos, e->d_slot, s); ++nl;
         const int rc = enqueue_readback(e, e->p_first, nt, mode, s);
         if (rc != RR_OK) return rc;
     }

@@ -450,6 +450,16 @@ inline void pf_attn_chunk(PrefillAttnArgs* a, __nv_bfloat16* out, const int32_t*
     a->n_seqs = n_seqs; a->max_len = max_len;
 }
 
+// ---- the prefill chunk's hand-off to decode (rr_engine.cu, run_prefill; rr_op_gather_last / rr_op_activate_rows)
+// Rows of the trimmed last layer: attn_out[r][0..nq) = attn[last[r]][..] and x_out[r][0..hidden) = x[last[r]][..] for
+// r < n_rows, one CTA per row, 16-byte loads and stores (nq % 8 == 0, hidden % 4 == 0, 16-byte aligned buffers).
+void launch_gather_last(const __nv_bfloat16* attn, const float* x, const int32_t* last, int n_rows, int nq, int hidden,
+                        __nv_bfloat16* attn_out, float* x_out, cudaStream_t st);
+// Tail row i < n becomes a live decode row in slot s = seq_slot[i]: d_tok[s] = first_tok[i], d_pos[s] = tok_pos[last[i]] + 1,
+// d_slot[s] = s.  Nothing else of d_tok / d_pos / d_slot is written.
+void launch_activate_rows(const int32_t* seq_slot, const int32_t* first_tok, const int32_t* tok_pos, const int32_t* last,
+                          int n, int32_t* d_tok, int32_t* d_pos, int32_t* d_slot, cudaStream_t st);
+
 // ---- prompt prefix caching (rr_kv_copy.cu): positions [0, n[i]) of slot src[i] -> slot dst[i], every layer and kv head,
 // K and V, one launch for the whole list (passed by value as a kernel parameter).  Each layer's cache is layer_rows rows of
 // 128 (n_pages * n_kv_heads * P); positions are addressed by kv_row through page_table (null: slot-contiguous).

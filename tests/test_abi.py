@@ -165,3 +165,70 @@ def test_fused_mlp_schedule_is_a_partition_and_deadlock_free(grid, inter, hidden
     assert sum(loads) == total
     if grid >= 64 and total // grid >= 100:                    # the production shapes: within 15 % of the mean
         assert max(loads) <= 1.15 * total / grid + slice_kb
+
+
+def _prototype_arity():
+    """{name: parameter count} of every function declared in include/rr_b200.h"""
+    text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "rr_b200.h").read_text(), flags=re.S)
+    out = {}
+    for m in re.finditer(r"\b(rr_[a-z0-9_]+)\s*\(([^;{]*?)\)\s*;", text):
+        params = m.group(2).strip()
+        out[m.group(1)] = 0 if params in ("", "void") else params.count(",") + 1
+    return out
+
+
+def test_ctypes_argument_counts_match_the_header():
+    """Every _lib.py prototype takes as many arguments as the header declares (a missing or extra argument would shift
+    every later one)."""
+    from rr_b200 import _lib
+    arity = _prototype_arity()
+    assert sorted(arity) == sorted(_lib.PROTOTYPES)
+    wrong = {n: (arity[n], len(a)) for n, (_, a) in _lib.PROTOTYPES.items() if arity[n] != len(a)}
+    assert not wrong, wrong
+
+
+def test_handoff_entry_points_validate_before_touching_the_device():
+    """rr_op_gather_last, rr_op_activate_rows and rr_op_dequantize_fp8_jobs reject null pointers and bad shapes with
+    RR_INVALID_ARGUMENT before they touch the device (so this passes without one).  The non-null addresses below are never
+    dereferenced: every call is refused by its host-side checks."""
+    from rr_b200 import _lib
+    L = _lib.lib
+    a = 1 << 20                                                          # a 16-byte aligned address, never read
+    # gather_last(attn, x, last, n_rows, nq, hidden, attn_out, x_out, stream)
+    assert L.rr_op_gather_last(None, a, a, 4, 4096, 4096, a, a, None) == 4
+    assert L.rr_op_gather_last(a, None, a, 4, 4096, 4096, a, a, None) == 4
+    assert L.rr_op_gather_last(a, a, None, 4, 4096, 4096, a, a, None) == 4
+    assert L.rr_op_gather_last(a, a, a, 4, 4096, 4096, None, a, None) == 4
+    assert L.rr_op_gather_last(a, a, a, 4, 4096, 4096, a, None, None) == 4
+    assert L.rr_op_gather_last(a, a, a, 0, 4096, 4096, a, a, None) == 4          # n_rows < 1
+    assert L.rr_op_gather_last(a, a, a, 4, 4092, 4096, a, a, None) == 4          # nq % 8
+    assert L.rr_op_gather_last(a, a, a, 4, 4096, 4094, a, a, None) == 4          # hidden % 4
+    assert L.rr_op_gather_last(a + 8, a, a, 4, 4096, 4096, a, a, None) == 4      # misaligned attn
+    assert L.rr_op_gather_last(a, a, a, 4, 4096, 4096, a, a + 4, None) == 4      # misaligned x_out
+    # activate_rows(seq_slot, first_tok, tok_pos, last, n, d_tok, d_pos, d_slot, stream)
+    for k in range(7):
+        args = [a] * 7
+        args[k] = None
+        assert L.rr_op_activate_rows(*args[:4], 8, *args[4:], None) == 4, k
+    assert L.rr_op_activate_rows(a, a, a, a, 0, a, a, a, None) == 4              # n < 1
+    # dequantize_fp8_jobs(q[], scale[], rows[], K[], out[], ld_out[], n_jobs, stream): four valid jobs of a Llama-3-8B
+    # layer's shapes, the last one changed by `last`
+
+    def jobs(n, **last):
+        cols = {"q": [a] * n, "scale": [a] * n, "rows": [6144, 4096, 28672, 4096][:n], "K": [4096, 4096, 4096, 14336][:n],
+                "out": [a] * n, "ld_out": [4096, 4096, 4096, 14336][:n]}
+        for c, v in last.items():
+            cols[c][-1] = v
+        P = lambda v: (C.c_void_p * n)(*v)
+        I = lambda v: (C.c_int32 * n)(*v)
+        return [P(cols["q"]), P(cols["scale"]), I(cols["rows"]), I(cols["K"]), P(cols["out"]), I(cols["ld_out"])]
+
+    for k in range(6):
+        args = jobs(4)
+        args[k] = None
+        assert L.rr_op_dequantize_fp8_jobs(*args, 4, None) == 4, k
+    assert L.rr_op_dequantize_fp8_jobs(*jobs(4), 0, None) == 4                    # job count outside 1..4
+    assert L.rr_op_dequantize_fp8_jobs(*jobs(4), 5, None) == 4
+    for bad in [{"q": None}, {"scale": None}, {"out": None}, {"q": a + 8}, {"out": a + 8}, {"rows": 0}, {"K": 14328},
+                {"K": 0}, {"ld_out": 14320}, {"ld_out": 14340}]:
+        assert L.rr_op_dequantize_fp8_jobs(*jobs(4, **bad), 4, None) == 4, bad
